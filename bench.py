@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- rendered faces/sec of the FENeRF volumetric render hot path on B200.
+"""bench.py -- rendered faces/sec of the FENeRF volumetric render hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model A|B]
-                    [--precision guard|fast|exact] [--no-graph] [--quick]
+                    [--precision guard|fast|exact] [--no-graph] [--extras] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic latents: BASELINE.json configs[1]
 -- 128x128 image, 24 (+24 hierarchical) samples per ray, batch 4 per GPU, forward-only -- through
@@ -11,7 +11,9 @@ all-gather when N > 1.  Weights are the reference's random init under manual_see
 N(0,1); camera poses gaussian (h_stddev 0.3, v_stddev 0.155); nerf_noise 0.  Every timed arm (resident,
 end to end, per model and precision mode) starts from the same device state: queue drained, SETTLE_S
 of idle, W warm-up steps, then exactly K timed steps (StepRunner.settle says why).  One JSON line on
-stdout (rank 0).  Nothing here reads /root/reference.
+stdout (rank 0).  --extras adds the sustained run, the other model, the other precision modes and a training
+step, each with its own step count.  --dump-outputs DIR writes what the last timed step of the headline arm
+returned (frames and camera poses, rank 0) as DIR/<name>.npy; the inputs depend only on the arguments.
 """
 import argparse
 import json
@@ -183,8 +185,7 @@ def cpu_faces_per_sec(model, steps, warmup, budget_s=200.0):
     dt = (time.perf_counter() - t0) / steps
     frac = (r / IMG) ** 2
     sample = ("%d step(s) of %dx%d rays (%.3g of one cfg2 face, B=1, %d+%d samples/ray), oracle port, fp32, %d threads (best of a "
-              "thread-count probe on %d host cores); the port takes 0.93-1.16x the live reference's time on the build container "
-              "(profiles/r02_port_vs_reference.txt)" % (steps, r, r, frac, STEPS_PER_RAY, STEPS_PER_RAY, cores, avail))
+              "thread-count probe on %d host cores)" % (steps, r, r, frac, STEPS_PER_RAY, STEPS_PER_RAY, cores, avail))
     return frac / dt, sample, cores
 
 
@@ -211,7 +212,7 @@ def workload_config(args, world):
             "global_batch": BATCH_PER_GPU * world, "parallelism": "dp%d (images sharded, one frame all-gather)" % world,
             "precision_mode": args.precision,
             "l2_policy": "inputs_larger_than_l2 (per-step working set ~140 MB of RNG draws, sample points and raw outputs vs "
-                         "126 MB L2; fresh latents and RNG draws every step, also under graph replay)"}
+                         "50 MB L2; fresh latents and RNG draws every step, also under graph replay)"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -246,14 +247,22 @@ class StepRunner:
             with torch.no_grad():
                 self.graph = GraphedRender(self.gen, self.lat_dev[0], self.md)
 
-    def render(self, latents):
-        if self.graph is not None:
-            return self.graph(*latents)[0]
-        with torch.no_grad():
-            return self.gen(*latents, **self.md)[0]
-
     def step_resident(self, i):
-        return self.gatherer.gather(self.render(self.lat_dev[i % len(self.lat_dev)]))
+        lat = self.lat_dev[i % len(self.lat_dev)]
+        if self.graph is not None:
+            pixels, poses = self.graph(*lat)
+        else:
+            with torch.no_grad():
+                pixels, poses = self.gen(*lat, **self.md)
+        self.last = (self.gatherer.gather(pixels), poses)
+        return self.last[0]
+
+    def dump_outputs(self, out_dir):
+        """The frames (all ranks' images) and this rank's camera poses of the last step, as float32 .npy files."""
+        import numpy as np
+        os.makedirs(out_dir, exist_ok=True)
+        for name, t in zip(("frames", "poses"), self.last):
+            np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
     def step_e2e(self, i):
         k = i % len(self.lat_host)
@@ -284,10 +293,9 @@ class StepRunner:
         self.host_sink += float(self.out_host[i & 1][0, 0, 0, 0]) + float(self.out_host[i & 1][-1, -1, -1, -1])
 
     def settle(self):
-        """Both arms start from the same device state: queue drained, then SETTLE_S of idle, then their warm-up steps.  On
-        this part the power limiter pulls the SM clock down within ~0.1-0.2 s of full load (profiles/r02_diag_e2e.txt:
-        the same graph replay takes 3.13-3.18 ms per step in a 20-step burst from idle and 3.48-3.56 ms once capped, with or
-        without the host copies), so an arm timed right behind another one measured the limiter, not its pipeline."""
+        """Both arms start from the same device state: queue drained, then SETTLE_S of idle, then their warm-up steps.  A
+        power-limited GPU lowers its SM clock within a fraction of a second of full load, so an arm timed right behind
+        another one would measure the limiter, not its pipeline."""
         torch.cuda.synchronize()
         time.sleep(SETTLE_S)
 
@@ -340,11 +348,13 @@ class StepRunner:
         return sum(z.numel() * 4 for z in self.lat_host[0]), self.out_host[0].numel() * 4
 
 
-def measure_model(args, model, world, rank, local, steps, warmup, precision=None, sustained_s=0.0, roofline=True):
+def measure_model(args, model, world, rank, local, steps, warmup, precision=None, sustained_s=0.0, roofline=True, dump_dir=None):
     device = torch.device("cuda", local)
     n_batches = min(steps + warmup, 64)
     r = StepRunner(args, model, world, rank, device, n_batches, precision=precision, use_graph=not args.no_graph)
     ms_step, _ = r.time_resident(steps, warmup)
+    if dump_dir and rank == 0:
+        r.dump_outputs(dump_dir)
     ms_e2e = r.time_e2e(steps, warmup)
     B = BATCH_PER_GPU
     h2d, d2h = r.bytes_per_step()
@@ -416,7 +426,7 @@ def measure_train_step(args, world, rank, local):
                         "1 differentiable render + backward per split, Adam step; synthetic loss (fixed projection of the frames)"
                         % (MODEL_NAME["B"], R, R, S, S, BATCH, SPLIT, BATCH // SPLIT),
             "ms_per_iteration": ms, "faces_rendered_per_iteration": 3 * BATCH, "rendered_faces_per_s": 3 * BATCH / (ms / 1e3),
-            "iterations_per_s": 1e3 / ms, "backward": "fenerf_b200/backward.py (CUDA kernels + the library's tcgen05 GEMMs, csrc/gemm5.cu), fp16 streams"}
+            "iterations_per_s": 1e3 / ms, "backward": "fenerf_b200/backward.py (CUDA kernels + the library's wgmma GEMMs, csrc/gemm.cu), fp16 streams"}
 
 
 def run_ours(args, world, rank, local):
@@ -427,10 +437,10 @@ def run_ours(args, world, rank, local):
     ops.set_default_precision(args.precision)
     torch.manual_seed(4242 + rank)
     sampler = ClockSampler(local) if rank == 0 else None
-    main = measure_model(args, args.model, world, rank, local, args.steps, args.warmup, sustained_s=0.0)
+    main = measure_model(args, args.model, world, rank, local, args.steps, args.warmup, sustained_s=0.0, dump_dir=args.dump_outputs)
     clocks = sampler.stop() if sampler else None
     extras = {}
-    if not args.quick:
+    if args.extras:
         other = "B" if args.model == "A" else "A"
         short = max(5, min(args.steps, 10))
         # the >= 3 s run of the headline workload, the other field (the curriculum BASELINE configs[2..4] name), the
@@ -457,7 +467,7 @@ def run_ours(args, world, rank, local):
         "metric": "rendered faces/sec at 128px x 24 samples/ray", "value": main["value"], "unit": "faces/s",
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": main["ms_per_step"],
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f16 operands / f32 accumulate (tcgen05) + f32 refinement" if args.precision != "exact" else "f32",
+        "dtype": "f16 operands / f32 accumulate (wgmma) + f32 refinement" if args.precision != "exact" else "f32",
         "data": "synthetic", "config": workload_config(args, world), "clocks": clocks,
         "e2e": main["e2e"], "gpu_launches": main["gpu_launches"], "gpu_launches_per_step": main["gpu_launches_per_step"],
         "cuda_graph": main["cuda_graph"], "roofline": main.get("roofline"),
@@ -472,17 +482,12 @@ def run_ours(args, world, rank, local):
 def field_roofline(gen, args, model, precision, latents, md, device):
     """Times the point-network launches of one step with CUDA events on the launching stream
     (same sizes and inputs as inside the step: ray_setup -> field -> resample -> field).  The launches are
-    timed alone behind a GPU-side spin, i.e. in the burst-clock regime: `frac` is against the BURST bf16 peak of
-    MEASURED_PEAKS.json (`frac_of_sustained_peak` is given beside it)."""
+    timed alone behind a GPU-side spin, i.e. in the burst-clock regime: `frac` is against the dense fp16 rate of NVIDIA's
+    H100 SXM data sheet (989 TFLOP/s at 700 W), which a power-limited card does not reach."""
     from fenerf_b200 import ops
     from fenerf_b200.generators import volumetric_rendering as vr
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = peaks.get("bf16_tflops") or 1700.0
-    peak_src = "MEASURED_PEAKS.json bf16_tflops (burst: the kernel is timed alone, ~1.5 ms launches)" if peaks else "fallback (B200_PROFILING.md ~1.7 PF burst)"
+    peak = 989.0
+    peak_src = "H100 SXM data sheet, dense fp16 / bf16 (700 W)"
     B, S, R = latents[0].shape[0], md["num_steps"], md["img_size"]
     N = R * R
     with torch.no_grad():
@@ -516,15 +521,9 @@ def field_roofline(gen, args, model, precision, latents, md, device):
     ms = durations[len(durations) // 2] if len(durations) % 2 else 0.5 * (durations[len(durations) // 2 - 1] + durations[len(durations) // 2])
     flops = B * N * S * FLOP_PER_POINT[model]
     achieved = flops / (ms * 1e-3) / 1e12
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get("%s_%s" % (model, precision))
-    except Exception:
-        pass
     return {"bound": "tensor", "kernel": "siren point network (%s, model %s)" % (precision, model), "achieved": achieved, "peak": peak,
-            "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic, "ms_per_launch": ms,
-            "flop_per_launch": flops, "peak_source": peak_src,
-            "frac_of_sustained_peak": achieved / peaks["bf16_tflops_sustained"] if peaks.get("bf16_tflops_sustained") else None}
+            "unit": "TFLOP/s", "frac": achieved / peak, "ms_per_launch": ms,
+            "flop_per_launch": flops, "peak_source": peak_src}
 
 
 _RESULT_FD = None
@@ -559,8 +558,13 @@ def main():
     ap.add_argument("--precision", default=os.environ.get("FENERF_B200_PRECISION", "guard"), choices=["guard", "fast", "exact"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="run the step eagerly instead of as a captured CUDA graph")
-    ap.add_argument("--quick", action="store_true", help="headline numbers only (no sustained run / other model / modes / train step)")
+    ap.add_argument("--quick", action="store_true", help="headline numbers only (the default; kept for old command lines)")
+    ap.add_argument("--extras", action="store_true", help="also the sustained run, the other model, the other modes and a train step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's frames and poses as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of the GPU path (--impl ours)")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
         world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))

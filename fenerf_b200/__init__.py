@@ -1,7 +1,7 @@
-"""fenerf_b200 -- B200-native volumetric face renderer behind FENeRF's generator API.
+"""fenerf_b200 -- H100-native volumetric face renderer behind FENeRF's generator API.
 
 Layout (only what the hot path needs, SURVEY.md section 8):
-  csrc/                 sm_100a CUDA kernels + the C-ABI (include/fenerf_b200.h)
+  csrc/                 sm_90a CUDA kernels + the C-ABI (include/fenerf_b200.h)
   _lib.py, ops.py       ctypes binding and thin operators (plumbing)
   packing.py            raw nn.Parameter pointers -> fenerf_pack_field
   generators/, siren/   host-side mirror of the reference's class API (drop-in boundary)

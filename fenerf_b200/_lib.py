@@ -12,7 +12,7 @@ LIB_PATH = os.environ.get("FENERF_B200_LIB") or os.path.join(_HERE, "libfenerf_b
 
 MAX_TRUNK, MAX_COLOR, MAX_LABEL, HIDDEN = 8, 8, 32, 256
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 PRECISION = {"exact": 0, "fast": 1, "guard": 2}
 CLAMP = {"relu": 0, "softplus": 1}
 FILL_MODE = {None: 0, "debug": 1, "weight": 2, "weight_debug": 3, "seg_padding_background": 4,
@@ -24,7 +24,7 @@ CAMERA_MODE = {"uniform": 1, "normal": 2, "gaussian": 2, "truncated_gaussian": 3
 EXPORTS = (
     "fenerf_packed_bytes", "fenerf_pack_field", "fenerf_siren_points", "fenerf_ray_setup", "fenerf_resample",
     "fenerf_composite", "fenerf_workspace_bytes", "fenerf_render_forward", "fenerf_last_error",
-    "fenerf_abi_version", "fenerf_launch_count", "fenerf_debug_trace", "fenerf_camera_poses",
+    "fenerf_abi_version", "fenerf_launch_count", "fenerf_camera_poses",
     "fenerf_field_fingerprint", "fenerf_composite_backward", "fenerf_film_forward_stash", "fenerf_gate_backward",
     "fenerf_head_grads", "fenerf_extras_gather", "fenerf_grid_scatter_add", "fenerf_grid_unpack_grad",
     "fenerf_workspace_layout", "fenerf_mask2color", "fenerf_frames_to_u8", "fenerf_mapping_film",
@@ -133,8 +133,6 @@ def _declare(lib):
     lib.fenerf_abi_version.argtypes = []
     lib.fenerf_launch_count.restype = i64
     lib.fenerf_launch_count.argtypes = []
-    lib.fenerf_debug_trace.restype = None
-    lib.fenerf_debug_trace.argtypes = [vp]
 
 
 def lib():

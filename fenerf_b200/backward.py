@@ -11,7 +11,7 @@ forward   ONE ``fenerf_render_forward`` call into a private workspace -- the sam
 backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per ray), then the point
           network layer by layer, recomputing activations chunk by chunk (nothing but the workspace
           survives from the forward):
-            recompute   ``fenerf_gemm_nt_film``: z = a W^T on tcgen05 with the epilogue fused -- a = sin(f z + p) and
+            recompute   ``fenerf_gemm_nt_film``: z = a W^T on wgmma with the epilogue fused -- a = sin(f z + p) and
                         the gate f cos(f z + p) leave as fp16, z never does
             backward    ``fenerf_gate_backward`` dZ = dA * gate (+ per-image column sums), dA' = dZ W
                         (``fenerf_gemm_nt_f16``) and the per-image dW_b = dZ^T a (``fenerf_gemm_tn_f16``, split-K)
@@ -22,7 +22,7 @@ Gradients flow to the FiLM table (and through torch's autograd into the mapping 
 frequency offsets) and to every field parameter.  The fp16 gradient stream is scaled by a power of two
 taken from max|d raw| on the device (no host sync) and unscaled at the end.
 
-The three 256-wide products per layer run on tcgen05 (csrc/gemm5.cu: ``fenerf_gemm_nt_film`` -- the recompute with its FiLM
+The three 256-wide products per layer run on wgmma (csrc/gemm.cu: ``fenerf_gemm_nt_film`` -- the recompute with its FiLM
 epilogue fused, ``fenerf_gemm_nt_f16`` for dA' = dZ W, ``fenerf_gemm_tn_f16`` split-K for the per-image dW); only the narrow
 products (heads, the 3 / 35-wide inputs) go to the library.  ``FENERF_B200_BWD_GEMM=cublas`` switches the wide ones back
 (A/B timing); ``precision='exact'`` always uses fp32 library GEMMs.  (The kernels can also fold the next layer's gate multiply
@@ -38,9 +38,9 @@ from . import _lib, ops, packing
 import os
 
 CHUNK_POINTS = 1 << 19
-#: the 256-wide products: 'tcgen05' = csrc/gemm5.cu (default), 'cublas' = torch.mm / bmm (kept for A/B timing and as the
+#: the 256-wide products: 'wgmma' = csrc/gemm.cu (default), 'cublas' = torch.mm / bmm (kept for A/B timing and as the
 #: fp32 path of precision='exact')
-BWD_GEMM = os.environ.get("FENERF_B200_BWD_GEMM", "tcgen05")
+BWD_GEMM = os.environ.get("FENERF_B200_BWD_GEMM", "wgmma")
 
 
 def _ptr(t):
@@ -159,13 +159,13 @@ class _FieldBackward:
         # fp16 / fp32 weight views for the GEMMs
         fw = self.fw
         self.W0 = fw.trunk[0][0].detach().float().contiguous()                    # (256, 3)
-        self.own_gemm = (not exact) and BWD_GEMM == "tcgen05"
+        self.own_gemm = (not exact) and BWD_GEMM == "wgmma"
         self.Wh16 = [None] + [w.detach().to(self.dt).contiguous() for w, _ in fw.trunk[1:]]
         wc0 = fw.color[0][0].detach().float()
         self.Wc0x_narrow = wc0[:, :self.kx].contiguous()                          # (256, 3 + G) fp32
         self.Wc16 = [wc0[:, self.kx:].to(self.dt).contiguous()] + [w.detach().to(self.dt).contiguous() for w, _ in fw.color[1:]]
         self.Wfeat16 = wc0[:, 3:self.kx].to(self.dt).contiguous() if G else None       # (256, G)
-        # dA' = dZ W on the tcgen05 NT kernel wants the transposed weights as its (N, K) operand
+        # dA' = dZ W on the wgmma NT kernel wants the transposed weights as its (N, K) operand
         self.WhT16 = [None] + [w.t().contiguous() for w in self.Wh16[1:]] if self.own_gemm else None
         self.WcT16 = [w.t().contiguous() for w in self.Wc16] if self.own_gemm else None
         if self.own_gemm:

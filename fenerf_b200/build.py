@@ -1,4 +1,4 @@
-"""Builds libfenerf_b200.so (the C-ABI library of include/fenerf_b200.h) in-tree with nvcc for sm_100a.
+"""Builds libfenerf_b200.so (the C-ABI library of include/fenerf_b200.h) in-tree with nvcc for sm_90a.
 
 One object per translation unit under build/ (so edits rebuild only what changed), linked into
 fenerf_b200/libfenerf_b200.so.  No torch involvement: the library has a plain C ABI.
@@ -17,11 +17,11 @@ LIB_PATH = os.path.join(HERE, "libfenerf_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
     "-DFENERF_BUILDING_LIB",
 ]
-# experiment builds (tools/ab_field.py): FENERF_NVCC_DEFINES="-DFOO=1 ..." + FENERF_B200_LIB=<output .so>
+# experiment builds: FENERF_NVCC_DEFINES="-DFOO=1 ..." + FENERF_B200_LIB=<output .so>
 NVCC_FLAGS += os.environ.get("FENERF_NVCC_DEFINES", "").split()
 if os.environ.get("FENERF_B200_LIB"):
     LIB_PATH = os.path.abspath(os.environ["FENERF_B200_LIB"])
@@ -65,7 +65,7 @@ def _compile_one(src, verbose):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA translation unit for sm_100a and link the shared library. Returns its path."""
+    """Compile every CUDA translation unit for sm_90a and link the shared library. Returns its path."""
     os.makedirs(OBJ_DIR, exist_ok=True)
     if force:
         for f in os.listdir(OBJ_DIR):
@@ -75,7 +75,7 @@ def build(force=False, verbose=False):
         results = list(ex.map(lambda s: _compile_one(s, verbose), srcs))
     objs = [o for o, _ in results]
     if any(changed for _, changed in results) or not os.path.exists(LIB_PATH):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

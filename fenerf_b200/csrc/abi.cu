@@ -52,7 +52,7 @@ int check_render_desc(const fenerf_render_desc* rd) {
     return 0;
 }
 
-// ---- diagnostics: per-stage CUDA-event timing of fenerf_render_forward (warm, in-step numbers; ncu's are cold) ----
+// ---- diagnostics: per-stage CUDA-event timing of fenerf_render_forward (warm, in-step numbers) ----
 constexpr int kStages = 6;       // ray_setup, field(coarse), guard, resample, field(fine), composite
 bool g_stage_timing = false;
 cudaEvent_t g_stage_ev[kStages + 1];
@@ -70,10 +70,8 @@ int run_field(const FnLayout& L, const void* packed, const float* points, const 
     const unsigned char* pk = static_cast<const unsigned char*>(packed);
     if (precision == FENERF_PRECISION_EXACT)
         return siren_points_exact(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, nullptr, 0, out, st, sigma_only);
-    // the tcgen05 kernel (siren_fast3.cu: third generation; its predecessors are described in DESIGN.md
-    // section 5 and live in the history only)
-    return siren_points_fast3(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, get_fast_trace(), sigma_only, st,
-                              sigma_out);
+    // the wgmma kernel (siren_fast.cu)
+    return siren_points_fast(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
 }
 
 }  // namespace
@@ -83,7 +81,6 @@ extern "C" {
 
 const char* fenerf_last_error(void) { return g_err; }
 int32_t fenerf_abi_version(void) { return FENERF_ABI_VERSION; }
-void fenerf_debug_trace(void* device_buffer) { set_fast_trace(static_cast<long long*>(device_buffer)); }
 int64_t fenerf_launch_count(void) { return (int64_t)g_launches.load(); }
 
 size_t fenerf_packed_bytes(const fenerf_field_desc* field) {
@@ -256,7 +253,7 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
     stage_mark(0, st);
     if (int e = ray_setup(rd, x_lin, y_lin, z_lin, cam2world, rng_perturb, points_c, z_c, dirs, origins, st)) return e;
     stage_mark(1, st);
-    // the tcgen05 pass also leaves the densities as one float per point for the resampler (which never reads the far
+    // the wgmma pass also leaves the densities as one float per point for the resampler (which never reads the far
     // sample, so the GUARD refinement of raw_c below does not concern that copy)
     float* sigma_c = (rd->hierarchical && rd->precision != FENERF_PRECISION_EXACT) ? (float*)(ws + w.sigma_c) : nullptr;
     if (int e = run_field(L, packed, points_c, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,

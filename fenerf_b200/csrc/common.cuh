@@ -61,7 +61,7 @@ inline int num_sms() {
     int n = cached[dev].load(std::memory_order_relaxed);
     if (n <= 0) {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
         cached[dev].store(n, std::memory_order_relaxed);
     }
     return n;
@@ -85,11 +85,9 @@ int siren_points_exact(const FnLayout& L, const unsigned char* packed, const flo
                        const float* film, int batch, long long ppb, int dir_group, int lock_dirs,
                        const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only = 0);
 int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st);
-void set_fast_trace(long long* buf);
-long long* get_fast_trace();
-int siren_points_fast3(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
-                       const float* film, int batch, long long ppb, int dir_group, int lock_dirs, float* out,
-                       long long* trace, int sigma_only, cudaStream_t st, float* sigma_out = nullptr);
+int siren_points_fast(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
+                      const float* film, int batch, long long ppb, int dir_group, int lock_dirs, float* out,
+                      int sigma_only, cudaStream_t st, float* sigma_out = nullptr);
 int guard_refine(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
                  const float* film, int batch, long long rays_per_batch, int num_steps, int lock_dirs, float tau,
                  const float* noise_far, long long noise_stride, float noise_std,
@@ -109,7 +107,7 @@ int composite(const fenerf_render_desc* rd, int C, const float* raw_c, const flo
               const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
               int32_t* sort_idx, cudaStream_t st);
 
-// gemm5.cu
+// gemm.cu
 int gemm_nt(const void* A, const void* B, long long M, float* c32, void* c16, void* a_out, void* gate_out, const float* bias,
             const float* film, long long film_stride, long long ppb, cudaStream_t st, const void* gate_mul = nullptr,
             const void* A2 = nullptr, const void* B2 = nullptr);

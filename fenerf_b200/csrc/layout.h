@@ -1,14 +1,14 @@
 // Packed (kernel-layout) parameter block of a FiLM-SIREN field.  Internal to the library.
 //
-// One contiguous device buffer; every section is 1024-byte aligned (the UMMA images need it, the
+// One contiguous device buffer; every section is 1024-byte aligned (the swizzled wgmma images need it, the
 // rest does not care).  Host and device share this header: the host computes the offsets once per
 // call and passes the struct by value to the kernels.
 //
 //   first layer      Wt0 [3][256] f32 (k-major)          b0 [256]
 //   hidden layer l   Wt  [K_l][256] f32 (k-major)        b  [256]        (exact kernel)
-//                    img [2 halves][K_l/64][128 rows][64 k] f16, 128B-swizzled (tcgen05 kernel):
+//                    img [2 halves][K_l/64][128 rows][64 k] f16, 128B-swizzled (wgmma kernel):
 //                        feature half h, k-chunk kc at byte h*64 KB + kc*16 KB, so one bulk copy can
-//                        bring several k-chunks of a half (32 KB = 8 MMAs of work per ring stage)
+//                        bring several k-chunks of a half (32 KB per ring slot)
 //     l in [0, n_hidden): trunk layers 1.., then colour layers 0..;  K_l = 256 except the first
 //     colour layer, whose extra inputs are appended after the 256 x-rows:
 //        f32:  rows 256.. = dir(3), feat(G), zero pad to KX_PAD
@@ -19,10 +19,10 @@
 //                    (power-of-two scaled) label map, row L the sigma weights, rest zero
 //                    rgb-head image   [4 chunks][ 8 rows][64 k] f16 swizzled: rows 0..2
 //   grid             channels-last [R][R][R][G] f32 (exact path, backward)
-//   grid16           the same in f16 (tcgen05 path: 64 B per voxel -- the features become fp16 MMA operands anyway;
-//                    57 MB for 32 x 96^3, which the 126 MB L2 can hold next to the weights, and half the gather stream)
+//   grid16           the same in f16 (wgmma path: 64 B per voxel -- the features become fp16 MMA operands anyway;
+//                    57 MB for 32 x 96^3: half the gather stream of the fp32 copy)
 //
-// "Input chunk" slot order (the 64-wide A chunk the tcgen05 kernel builds per point):
+// "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
 // matched on the B side by (W_hi, W_hi, W_lo) so that hi*hi + lo*hi + hi*lo reproduces an
 // fp32-accurate product from fp16 operands.
@@ -102,7 +102,7 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     return 0;
 }
 
-// Byte offset of element (row, k) inside one [rows][64] f16 image with the UMMA/TMA 128-byte
+// Byte offset of element (row, k) inside one [rows][64] f16 image with the wgmma/TMA 128-byte
 // swizzle (K-major): 8-row groups of 1024 B, 128 B per row, the 16-byte chunk index XORed with
 // row % 8.
 #if defined(__CUDACC__)

@@ -139,7 +139,7 @@ __global__ void label_step3_kernel(float* __restrict__ lw, int L) {
     if (threadIdx.x == 0) lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] = 1.f / scale;
 }
 
-// head images for the tcgen05 kernel (one block):
+// head images for the wgmma kernel (one block):
 //   trunk head  [4][32 rows][64 k]: rows 0..L-1 = Weff * scale, row L = sigma weights
 //   rgb head    [4][ 8 rows][64 k]: rows 0..2
 __global__ void pack_head_imgs_kernel(const float* __restrict__ lw, int L, const float* __restrict__ sigma_w,

@@ -5,10 +5,10 @@
 // :1509-1530 for the texture-embedding field) -- in the reference one addmm + three elementwise
 // passes per FiLM layer, each materialising a (P, 256) fp32 tensor in memory.
 //
-// Role on B200: this is the fp32-faithful engine.  It serves FENERF_PRECISION_EXACT, and in the
+// Role: this is the fp32-faithful engine.  It serves FENERF_PRECISION_EXACT, and in the
 // default GUARD mode it re-evaluates the handful of far samples whose sigma sits next to the
 // reference's relu(sigma) * 1e10 step (volumetric_rendering.py:24,32); the bulk of the points go
-// through the tcgen05 kernel in siren_fast.cu.  FP32-pipe bound: 2 * 256 * 256 FLOP per layer per
+// through the wgmma kernel in siren_fast.cu.  FP32-pipe bound: 2 * 256 * 256 FLOP per layer per
 // point on 128 FMA lanes / SM.
 //
 // Tile structure (256 threads, 2 CTAs / SM):
@@ -282,7 +282,7 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                     long long flat = s.flat[pt];
                     if (flat >= 0) {
                         if (kGather && a.guard_stats && o == 0) {
-                            // how far the tcgen05 density was from this fp32 one, and whether its sign was wrong: the
+                            // how far the wgmma density was from this fp32 one, and whether its sign was wrong: the
                             // margin of the GUARD threshold, measured on the very weights / points being rendered
                             const float old = a.out[flat * C + C - 1];
                             atomicMax(a.guard_stats + 1, __float_as_int(fabsf(r - old)));
@@ -414,7 +414,7 @@ int guard_refine(const FnLayout& L, const unsigned char* packed, const float* po
     a.L = L; a.packed = packed; a.points = points; a.dirs = dirs; a.film = film; a.out = raw;
     a.only_idx = scratch_idx + 1; a.n_only_dev = scratch_idx; a.n_only = 0; a.n_items = 0;
     a.ppb = rays_per_batch * num_steps; a.tiles_per_batch = 1; a.dir_group = num_steps; a.lock_dirs = lock_dirs;
-    a.sigma_only = 1;      // only the sign of the far sample's density matters; its colour stays the tcgen05 one
+    a.sigma_only = 1;      // only the sign of the far sample's density matters; its colour stays the wgmma one
     a.guard_stats = stats;
     // (stats[0..2] were zeroed and stats[3] = tau written by guard_scan_kernel's launch above: no host memory is
     // touched here, so the whole refinement can sit inside a captured CUDA graph)

@@ -3,7 +3,7 @@
 Every image is independent (SURVEY.md section 8e): weights, grid and curriculum are replicated, the
 per-image inputs are a latent (1-2 KB) and its RNG draws.  Rank r renders images
 [r*B/W, (r+1)*B/W) straight into its slice of one (B, C, R, R) frame buffer and a single
-``all_gather_into_tensor`` (NCCL over NVLink/NVSwitch on the B200 box; gloo in the CPU tests) fills
+``all_gather_into_tensor`` (NCCL over NVLink/NVSwitch within one box; gloo in the CPU tests) fills
 the other slices -- no staging copy precedes the collective because the render kernel's NCHW
 output *is* the gather operand.  The reference has no such step (each DDP rank feeds its own
 discriminator, train_double_latent_semantic.py:148-150); this is the north-star's "frames back to

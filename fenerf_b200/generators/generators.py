@@ -1,4 +1,4 @@
-"""Drop-in generator wrappers: the reference's class API over the B200 render library.
+"""Drop-in generator wrappers: the reference's class API over the H100 render library.
 
 Mirrors the interface of generators/generators.py -- ``ImplicitGenerator3d`` (:13-431) and
 ``DoubleImplicitGenerator3d`` (:434-910): constructor arguments, attributes, method signatures,
@@ -30,7 +30,7 @@ class _RenderSkeleton:
                 v_mean, hierarchical_sample, sample_dist, lock_view_dependence, kwargs, staged, grad_points=None):
         device = torch.device(self.device)
         if device.type != 'cuda':
-            raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to a B200 (got %s)" % device)
+            raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to an H100 (got %s)" % device)
         rng = kwargs.get('_rng') or vr.DeviceRng(device)
         with_grad = (not staged) and ops.needs_grad(self.siren, film)
         if staged:
@@ -90,7 +90,7 @@ class _RenderSkeleton:
                     want_weights_sum=staged or debug is not None, want_weights=wants_per_sample_weights,
                     want_inds=debug is not None)
                 if staged and rd.precision == _lib.PRECISION['guard'] and clamp_mode == 'relu':
-                    # GUARD self-check (the staged methods synchronise anyway): the refinement measured how far the tcgen05
+                    # GUARD self-check (the staged methods synchronise anyway): the refinement measured how far the wgmma
                     # far-sample densities were from fp32 ON THESE WEIGHTS.  The default threshold was calibrated on the
                     # reference's random initialisation; if the measured error eats more than a third of it, widen it (it
                     # sticks to this field for later calls) and render this call again.

@@ -263,7 +263,7 @@ DEFAULT_GUARD_TAU = 1.5e-3
 
 
 def guard_stats(device):
-    """The GUARD self-check of the last render_forward on the current stream (fenerf_guard_stats): how far the tcgen05
+    """The GUARD self-check of the last render_forward on the current stream (fenerf_guard_stats): how far the wgmma
     far-sample densities were from their fp32 re-evaluation.  Synchronises the stream."""
     device = torch.device(device)
     ws = _WORKSPACES.get((device, torch.cuda.current_stream(device).cuda_stream))
@@ -376,7 +376,7 @@ def mapping_film(net, z, film, first_layer, n_layers, avg=None, psi=1.0):
 
 
 # --------------------------------------------------------------------------------------------
-# tcgen05 GEMMs of the backward (csrc/gemm5.cu)
+# wgmma GEMMs of the backward (csrc/gemm.cu)
 # --------------------------------------------------------------------------------------------
 def gemm_nt(a16, b16, out_dtype=torch.float32, gate=None):
     """(M, 256) fp16 . (256, 256)^T fp16 -> (M, 256) fp32 or fp16 (fenerf_gemm_nt_f16); `gate` (M, 256) fp16 multiplies

@@ -51,7 +51,7 @@ def collect_params(module, device):
     """-> (FieldParams, keepalive list). Parameter order / names per SURVEY.md section 8b."""
     spec = module.field_spec()
     if getattr(module, "hidden_dim", 256) != _lib.HIDDEN:
-        raise ValueError("the sm_100a kernels are specialised for hidden_dim=256 (got %s)" % module.hidden_dim)
+        raise ValueError("the sm_90a kernels are specialised for hidden_dim=256 (got %s)" % module.hidden_dim)
     keep = []
 
     def ptr(t):
@@ -92,7 +92,7 @@ def pack_field(module) -> PackedField:
     lib = _lib.lib()
     device = next(module.parameters()).device
     if device.type != "cuda":
-        raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to a B200 (got %s)" % device)
+        raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to an H100 (got %s)" % device)
     spec = module.field_spec()
     desc = field_desc(spec)
     nbytes = lib.fenerf_packed_bytes(C.byref(desc))

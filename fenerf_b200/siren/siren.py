@@ -3,12 +3,12 @@
 Only the module *interface* is kept from the reference -- class names, constructor arguments,
 attribute names, parameter registration order (EMA ``copy_to`` is positional), state-dict keys and
 the init RNG consumption -- so that checkpoints pickled as ``siren.siren.<Class>`` load and the
-reference's callers run unchanged.  The per-point arithmetic is not here: it is the sm_100a CUDA
+reference's callers run unchanged.  The per-point arithmetic is not here: it is the sm_90a CUDA
 kernel behind ``fenerf_siren_points`` (include/fenerf_b200.h).  Each network describes itself to
 the kernel through a small layer table (:class:`FieldSpec`), which is how further reference variants
 can be added without new kernels (SURVEY.md section 8f-4).
 
-Reference interfaces mirrored (file:line under /root/reference):
+Reference interfaces mirrored (file:line in the reference tree):
   FiLMLayer                                   siren/siren.py:113-123
   CustomMappingNetwork                        siren/siren.py:82-102
   frequency_init / first-layer inits          siren/siren.py:45-49, 104-110, 333-338

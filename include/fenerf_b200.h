@@ -1,5 +1,5 @@
 /*
- * fenerf_b200 -- C-ABI of the B200-native volumetric face renderer.
+ * fenerf_b200 -- C-ABI of the H100-native (sm_90a) volumetric face renderer.
  *
  * This is the drop-in boundary for the one hot path of MrTornado24/FENeRF: the per-image
  * volumetric render inside generators.*Generator3d.forward / staged_forward.  The reference has
@@ -28,7 +28,8 @@
 extern "C" {
 #endif
 
-#define FENERF_ABI_VERSION 2   /* 2: FENERF_MAX_COLOR 4 -> 8 (fenerf_field_params grew), backward entry points */
+#define FENERF_ABI_VERSION 3   /* 2: FENERF_MAX_COLOR 4 -> 8 (fenerf_field_params grew), backward entry points;
+                                  3: fenerf_debug_trace removed */
 
 /* error codes */
 #define FENERF_OK            0
@@ -88,8 +89,8 @@ typedef struct fenerf_field_params {
 /* Bytes of the packed, kernel-layout copy of a field's parameters. */
 size_t fenerf_packed_bytes(const fenerf_field_desc* field);
 
-/* Re-lays the raw parameters out for the kernels (k-major fp32 for the exact path, UMMA
- * 128B-swizzled fp16 images for the tcgen05 path, pre-multiplied label chain, channels-last
+/* Re-lays the raw parameters out for the kernels (k-major fp32 for the exact path, 128B-swizzled
+ * fp16 images for the wgmma path, pre-multiplied label chain, channels-last
  * grid).  Call again whenever the parameters change (optimizer step, EMA copy_to).
  * `packed` must be 1024-byte aligned. */
 int fenerf_pack_field(const fenerf_field_desc* field, const fenerf_field_params* params,
@@ -105,7 +106,7 @@ int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_
 
 /* precision modes of the point network */
 #define FENERF_PRECISION_EXACT 0  /* fp32 FFMA + precise sinf everywhere (CUDA cores)            */
-#define FENERF_PRECISION_FAST  1  /* fp16 operands / fp32 accumulate on tcgen05, sin.approx      */
+#define FENERF_PRECISION_FAST  1  /* fp16 operands / fp32 accumulate on wgmma, sin.approx        */
 #define FENERF_PRECISION_GUARD 2  /* FAST, then EXACT re-evaluation of the far sample of every ray
                                      whose |sigma| < guard_tau (the reference's delta=1e10 step,
                                      volumetric_rendering.py:24,32) -- the default                */
@@ -121,7 +122,7 @@ int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_
  *             others are left untouched in `out` (used by the GUARD refinement)               */
 /* OR-ed into `precision`: only the density channel out[..., C-1] is required (a 256^3 density grid for
  * marching cubes, extract_double_semantic_shapes.py:59-62 keeps `[:, :, -1:]`); the colour / label
- * branches are skipped on the tcgen05 path and the other channels of `out` are then left unspecified. */
+ * branches are skipped on the wgmma path and the other channels of `out` are then left unspecified. */
 #define FENERF_POINTS_SIGMA_ONLY 0x100
 
 int fenerf_siren_points(const fenerf_field_desc* field, const void* packed,
@@ -161,7 +162,7 @@ typedef struct fenerf_render_desc {
     float   noise_std;          /* nerf_noise */
     float   tan_half_fov;       /* (float) tan(2*pi*fov/360 / 2), volumetric_rendering.py:119 */
     float   guard_tau;          /* GUARD threshold on |sigma_far| (default 1.5e-3 if <= 0: 5x the fp16 path's
-                                   measured 3e-4 max sigma error, profiles/r01_field_fast_vs_exact*.log) */
+                                   3e-4 max sigma error on the reference's initialisation) */
 } fenerf_render_desc;
 
 /* Camera pose sampling after the random draws, and the look-at camera-to-world matrix.
@@ -224,7 +225,7 @@ int fenerf_composite(const fenerf_render_desc* rd, int32_t out_dim, const float*
 /* Scratch bytes fenerf_render_forward needs for this (render, field) pair. */
 size_t fenerf_workspace_bytes(const fenerf_render_desc* rd, const fenerf_field_desc* field);
 
-/* GUARD self-check.  The refinement pass knows, for every far sample it re-evaluates in fp32, what the tcgen05
+/* GUARD self-check.  The refinement pass knows, for every far sample it re-evaluates in fp32, what the wgmma
  * density was: the largest |difference| and the number of wrong signs are the measured margin of `guard_tau` on
  * the weights and points actually rendered (the default tau was calibrated on the reference's random
  * initialisation; trained weights can have larger activations).  A refinement is only trustworthy while
@@ -233,8 +234,8 @@ size_t fenerf_workspace_bytes(const fenerf_render_desc* rd, const fenerf_field_d
  * and synchronises that stream. */
 typedef struct fenerf_guard_report {
     int32_t refined;        /* far samples re-evaluated (|sigma + noise| < tau) */
-    float   max_abs_delta;  /* max |sigma_fp32 - sigma_tcgen05| over them */
-    int32_t sign_flips;     /* of which the tcgen05 sign was wrong (these are what the GUARD fixes) */
+    float   max_abs_delta;  /* max |sigma_fp32 - sigma_wgmma| over them */
+    int32_t sign_flips;     /* of which the wgmma sign was wrong (these are what the GUARD fixes) */
     float   tau;            /* the threshold that was used */
 } fenerf_guard_report;
 int fenerf_guard_stats(const void* workspace, fenerf_guard_report* out, void* stream);
@@ -313,7 +314,7 @@ int fenerf_frames_to_u8(const float* frames, int32_t batch, int32_t channels, in
 #define FENERF_DTYPE_F16 0
 #define FENERF_DTYPE_F32 1
 
-/* The 256-wide products of a FiLM layer's backward on tcgen05 (csrc/gemm5.cu); fp16 row-major operands, fp32 accumulate.
+/* The 256-wide products of a FiLM layer's backward on wgmma (csrc/gemm.cu); fp16 row-major operands, fp32 accumulate.
  *   fenerf_gemm_nt_f16   C (M, 256) = A (M, 256) . B (256, 256)^T  -> c_f32 or c_f16 (exactly one non-NULL)
  *                        (dA' = dZ W: pass B = W^T); optional gate_mul (M, 256) fp16 multiplies the fp16 output in the
  *                        epilogue: dZ of the layer below = (dZ W) * its gate, without a pass of its own
@@ -386,12 +387,6 @@ int64_t fenerf_launch_count(void);
  * enable = 1 with ms_out reads the six durations (ms) of the LAST call (synchronises on it).  Process-wide, not
  * thread-safe, inactive during CUDA-graph capture. */
 int fenerf_debug_stage_times(int32_t enable, float* ms_out /* host, 6 floats */);
-
-/* Diagnostics: install a device buffer of 4 * 4096 int64 that CTA 0 of the tcgen05 point-network
- * kernel fills with (tag, clock64) pairs for its first two tile pairs, one 4096-entry lane per warp
- * role (producer, MMA issuer, epilogue X, epilogue Y); NULL (the default) disables.  Process-wide,
- * not thread-safe. */
-void fenerf_debug_trace(void* device_buffer);
 
 #ifdef __cplusplus
 }

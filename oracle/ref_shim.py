@@ -1,8 +1,7 @@
-"""Import shim for the UNMODIFIED reference at /root/reference (test infrastructure only).
+"""Import shim for a checkout of the UNMODIFIED reference named by $FENERF_REFERENCE_ROOT (test infrastructure only).
 
-Used only by ``tests/golden/make_goldens.py`` and ``tests/test_oracle_vs_reference.py`` in the
-build container; ``/root/reference`` does not exist on the GPU box, so nothing on the product path
-and nothing under ``-m gpu`` imports this module.
+Used by ``tests/golden/make_goldens.py`` (which needs it) and ``tests/test_oracle_vs_reference.py`` (which
+compares against the stored reference outputs without it); nothing on the product path imports this module.
 
 The reference has four dead imports that are not installable here (SURVEY.md section 8c):
 ``matplotlib.pyplot`` (generators/volumetric_rendering.py:12), ``numpy.lib.type_check.imag``
@@ -13,11 +12,11 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("FENERF_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("FENERF_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "generators"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "generators"))
 
 
 def _stub(name, **attrs):
@@ -33,7 +32,7 @@ def _stub(name, **attrs):
 def load():
     """Returns (generators.generators, siren.siren, curriculums) of the reference."""
     if not available():
-        raise RuntimeError("reference tree not present at %s" % REFERENCE_ROOT)
+        raise RuntimeError("reference tree not found: set FENERF_REFERENCE_ROOT to a checkout of the reference")
     os.environ.setdefault("PYTHONDONTWRITEBYTECODE", "1")
     sys.dont_write_bytecode = True
     mpl = _stub("matplotlib")

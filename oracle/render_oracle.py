@@ -14,7 +14,7 @@ section 4), so the pin is the unmodified reference itself, imported in the build
 ``tests/golden/make_goldens.py`` (committed) runs it on fixed seeds and stores its outputs under
 ``tests/golden/``; ``tests/test_oracle.py`` checks this oracle against those files everywhere, and
 ``tests/test_oracle_vs_reference.py`` checks bit-equality against the live reference where
-``/root/reference`` exists.
+``$FENERF_REFERENCE_ROOT`` names a checkout of it (and against the stored outputs otherwise).
 
 RNG: every random draw goes through a ``Draws`` object so that a run can be recorded on the CPU
 and replayed, tensor for tensor, into the CUDA path (CPU and CUDA generators differ).

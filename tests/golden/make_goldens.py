@@ -1,10 +1,10 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (needs /root/reference).
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (a checkout of it named by $FENERF_REFERENCE_ROOT).
 
-    python tests/golden/make_goldens.py
+    python tests/golden/make_goldens.py [--grads | --part | --dropin]
 
 The reference holds no golden vectors for the render path (SURVEY.md section 4), so the pin of the
-oracle is the reference's own forward on fixed seeds, captured here.  Run in the build container
-only; the .npz files travel with the repo, /root/reference does not.
+oracle is the reference's own forward on fixed seeds, captured here.  The .npz files travel with
+the repository; the reference does not.
 
 Seed protocol (shared with tests/_cases.py):
   torch.manual_seed(0)            -> construct the generator (reference init order)
@@ -210,8 +210,54 @@ def part_forward_goldens():
                                                         os.path.getsize(path) / 1024))
 
 
+def dropin_goldens():
+    """What tests/test_dropin.py needs from the reference, so that it runs without it:
+      dropin_ref_<model>.pth.gz (+ .meta.gz)  whole-module checkpoints written by the reference's classes
+          (torch.save(generator), train_double_latent_semantic.py:523 style) and the parameter names / state_dict beside
+          them; every state_dict tensor is filled with its own constant (i + 1) / 64 so that the files compress to a few KB
+          and a key mix-up still shows
+      dropin_ref_layout.json  the module names of the reference's generators / siren packages and the model / generator
+          names of three curriculums"""
+    import gzip
+    import io
+    import json
+    ref_generators, ref_siren, ref_curriculums = ref_shim.load()
+    out_dir = os.path.dirname(os.path.abspath(__file__))
+    for model in ("A", "D"):
+        torch.manual_seed(0)
+        if model == "A":
+            gen = ref_generators.ImplicitGenerator3d(ref_siren.TALLSIREN, 256, 4)
+        else:
+            gen = ref_generators.DoubleImplicitGenerator3d(ref_siren.SIRENBASELINESEMANTICDISENTANGLE, 256, 256, 22)
+        gen.set_device("cpu")
+        gen.step, gen.epoch = 1234, 7
+        with torch.no_grad():
+            for i, t in enumerate(gen.state_dict().values()):
+                t.fill_((i + 1) / 64.0)
+        for suffix, obj in (("", gen), (".meta", {"names": [n for n, _ in gen.named_parameters()], "state": gen.state_dict()})):
+            buf = io.BytesIO()
+            torch.save(obj, buf)
+            with gzip.open(os.path.join(out_dir, "dropin_ref_%s.pth%s.gz" % (model, suffix)), "wb", compresslevel=9) as f:
+                f.write(buf.getvalue())
+    root = ref_shim.REFERENCE_ROOT
+
+    def modules(pkg):
+        d = os.path.join(root, pkg)
+        return sorted(n[:-3] if n.endswith(".py") else n for n in os.listdir(d)
+                      if (n.endswith(".py") and n != "__init__.py") or os.path.isfile(os.path.join(d, n, "__init__.py")))
+    layout = {"generators": modules("generators"), "siren": modules("siren"), "curriculums": {}}
+    for name in ("CelebA_double_semantic_texture_embedding_256_dim_96", "CelebA", "CelebA_double_semantic"):
+        md = ref_curriculums.extract_metadata(getattr(ref_curriculums, name), 0)
+        layout["curriculums"][name] = {"model": md["model"], "generator": md["generator"]}
+    with open(os.path.join(out_dir, "dropin_ref_layout.json"), "w") as f:
+        json.dump(layout, f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
 if __name__ == "__main__":
-    if sys.argv[1:2] == ["--part"]:
+    if sys.argv[1:2] == ["--dropin"]:
+        dropin_goldens()
+    elif sys.argv[1:2] == ["--part"]:
         part_forward_goldens()
     elif sys.argv[1:2] == ["--grads"]:
         grad_goldens()

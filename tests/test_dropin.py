@@ -3,52 +3,49 @@
 CPU part (this file, ``-m "not gpu"``): every test runs in a fresh interpreter, because ``install()``
 edits ``sys.modules``.
   * stand-alone install (no reference on sys.path): the two submodule names resolve to the mirror;
-  * with the reference tree importable (build container only; skipped elsewhere): after ``install()``
-    the reference's ``curriculums`` imports (curriculums.py:1 needs the reference's own
-    ``generators.neural_rendering``), ``extract_metadata`` works, the train script's class lookups
-    (train_double_latent_semantic.py:20-22, 116, 142) find the mirror classes;
+  * next to a tree with the reference's package layout (its module names, recorded in
+    tests/golden/dropin_ref_layout.json): after ``install()`` the reference's sibling modules stay importable
+    (curriculums.py:1 needs the reference's own ``generators.neural_rendering``) and the train script's class
+    lookups by curriculum name (train_double_latent_semantic.py:20-22, 116, 142) find the mirror classes;
   * a generator built from the REFERENCE classes and saved with ``torch.save(generator)``
-    (train_double_latent_semantic.py:128-150 / render_multiview_images_double_semantic.py:58) loads
-    under the mirror with an identical state_dict and the same parameter order, so torch_ema's
-    positional ``copy_to`` / ``restore`` (``param.data.copy_``) lands on the right tensors.
+    (train_double_latent_semantic.py:128-150 / render_multiview_images_double_semantic.py:58; stored as
+    tests/golden/dropin_ref_*.pth.gz) loads under the mirror with an identical state_dict and the same parameter
+    order, so torch_ema's positional ``copy_to`` / ``restore`` (``param.data.copy_``) lands on the right tensors;
+  * a checkpoint written under the mirror references the same classes and carries the same attributes and
+    state_dict layout as the reference's own.
+tests/golden/make_goldens.py --dropin records those files from the unmodified reference.
 GPU part: tests/test_gpu_parity.py::test_render_script_call_sequence replays
 render_multiview_images_double_semantic.py:43-65 against a golden.
 """
+import gzip
+import json
 import os
+import shutil
 import subprocess
 import sys
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("FENERF_REFERENCE_ROOT", "/root/reference")
-HAVE_REF = os.path.isdir(os.path.join(REF, "generators"))
-needs_ref = pytest.mark.skipif(not HAVE_REF, reason="reference tree not present (build container only)")
+GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
-def _run(code, *args, timeout=600):
+def _run(code, *args, ref="", timeout=600):
     env = dict(os.environ, PYTHONDONTWRITEBYTECODE="1")
-    r = subprocess.run([sys.executable, "-c", code, ROOT, REF] + list(args), capture_output=True, text=True,
+    r = subprocess.run([sys.executable, "-c", code, ROOT, ref] + list(args), capture_output=True, text=True,
                        timeout=timeout, env=env)
     assert r.returncode == 0, "child failed:\n%s\n%s" % (r.stdout[-3000:], r.stderr[-3000:])
     return r.stdout
 
 
-# the four dead imports of the reference that this image cannot satisfy (SURVEY.md section 8c); a user's
-# environment has the real packages
-_STUBS = r'''
-import sys, types
-def _stub(name, **attrs):
-    m = types.ModuleType(name)
-    for k, v in attrs.items(): setattr(m, k, v)
-    sys.modules[name] = m
-    return m
-mpl = _stub("matplotlib"); mpl.pyplot = _stub("matplotlib.pyplot")
-import numpy.lib
-sys.modules["numpy.lib"].type_check = _stub("numpy.lib.type_check", imag=None)
-_stub("fid_evaluation", output_images=None)
-k = _stub("kornia"); k.filters = _stub("kornia.filters", filter2D=None)
-'''
+def _reference_checkpoint(tmp_path, model):
+    """The reference-written checkpoint of `model` and its metadata, unpacked under tmp_path."""
+    path = str(tmp_path / "generator.pth")
+    for suffix in ("", ".meta"):
+        with gzip.open(os.path.join(GOLDEN, "dropin_ref_%s.pth%s.gz" % (model, suffix)), "rb") as src, \
+                open(path + suffix, "wb") as dst:
+            shutil.copyfileobj(src, dst)
+    return path
 
 
 def test_standalone_install_resolves_the_two_submodules():
@@ -71,13 +68,22 @@ print("ok")
     assert "ok" in out
 
 
-@needs_ref
-def test_install_keeps_the_reference_packages_importable():
-    out = _run(_STUBS + r'''
+def test_install_keeps_the_reference_packages_importable(tmp_path):
+    layout = json.load(open(os.path.join(GOLDEN, "dropin_ref_layout.json")))
+    ref = tmp_path / "reference"
+    for pkg in ("generators", "siren"):
+        (ref / pkg).mkdir(parents=True)
+        (ref / pkg / "__init__.py").write_text("")
+        for name in layout[pkg]:
+            (ref / pkg / (name + ".py")).write_text("")
+    # curriculums.py:1 imports the reference's own generators.neural_rendering
+    (ref / "curriculums.py").write_text("import generators.neural_rendering\nLAYOUT = %r\n" % (layout["curriculums"],))
+    out = _run(r'''
+import sys
 sys.path.insert(0, sys.argv[2]); sys.path.insert(0, sys.argv[1])
 import fenerf_b200
 fenerf_b200.install()
-import curriculums                                    # curriculums.py:1 -> generators.neural_rendering (reference's)
+import curriculums
 import generators.neural_rendering as nr
 assert nr.__file__.startswith(sys.argv[2]), nr.__file__
 from generators import generators                     # train_double_latent_semantic.py:20
@@ -86,38 +92,14 @@ assert generators.__name__ == "fenerf_b200.generators.generators", generators.__
 assert siren.__name__ == "fenerf_b200.siren.siren"
 import importlib.util                                 # reference-only subpackages still reachable (networks.py:18)
 assert importlib.util.find_spec("siren.op") is not None and importlib.util.find_spec("generators.BiSeNet") is not None
-md = curriculums.extract_metadata(curriculums.CelebA_double_semantic_texture_embedding_256_dim_96, 0)
-SIREN = getattr(siren, md['model'])                   # :116
-gen_cls = getattr(generators, md['generator'])        # :142
-assert gen_cls.__module__ == "generators.generators" and SIREN.__module__ == "siren.siren"
-md2 = curriculums.extract_metadata(curriculums.CelebA, 0)
-assert hasattr(siren, md2['model']) and hasattr(generators, md2['generator'])
-md3 = curriculums.extract_metadata(curriculums.CelebA_double_semantic, 0)
-assert hasattr(siren, md3['model']) and hasattr(generators, md3['generator'])
-print("ok", md['model'], md['generator'])
-''')
-    assert "ok TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_DIM_96 DoubleImplicitGenerator3d" in out
+for name, md in curriculums.LAYOUT.items():
+    SIREN = getattr(siren, md['model'])               # :116
+    gen_cls = getattr(generators, md['generator'])    # :142
+    assert gen_cls.__module__ == "generators.generators" and SIREN.__module__ == "siren.siren", name
+print("ok", len(curriculums.LAYOUT))
+''', ref=str(ref))
+    assert "ok 3" in out
 
-
-_SAVE_WITH_REFERENCE = _STUBS + r'''
-sys.path.insert(0, sys.argv[2])
-import warnings; warnings.simplefilter("ignore")
-import torch
-from generators import generators
-from siren import siren
-assert generators.__file__.startswith(sys.argv[2])
-torch.manual_seed(0)
-model = sys.argv[4]
-if model == "A":
-    gen = generators.ImplicitGenerator3d(siren.TALLSIREN, 256, 4)
-else:
-    gen = generators.DoubleImplicitGenerator3d(siren.SIRENBASELINESEMANTICDISENTANGLE, 256, 256, 22)
-gen.set_device("cpu")
-gen.step, gen.epoch = 1234, 7
-torch.save(gen, sys.argv[3])                                        # train_double_latent_semantic.py:523 style
-names = [n for n, _ in gen.named_parameters()]
-torch.save({"names": names, "state": gen.state_dict()}, sys.argv[3] + ".meta")
-'''
 
 _LOAD_WITH_MIRROR = r'''
 import sys
@@ -156,46 +138,48 @@ print("ok")
 '''
 
 
-@needs_ref
 @pytest.mark.parametrize("model", ["A", "D"])
 def test_reference_pickle_loads_under_the_mirror(tmp_path, model):
-    path = str(tmp_path / "generator.pth")
-    _run(_SAVE_WITH_REFERENCE, path, model)
-    out = _run(_LOAD_WITH_MIRROR, path)
+    out = _run(_LOAD_WITH_MIRROR, _reference_checkpoint(tmp_path, model))
     assert "ok" in out
 
 
-@needs_ref
 def test_mirror_pickle_loads_under_the_reference(tmp_path):
-    """The other direction: a whole-module checkpoint written under this library is a valid
-    reference checkpoint (same module paths, attribute names and state_dict)."""
-    path = str(tmp_path / "generator.pth")
-    _run(r'''
-import sys
+    """The other direction: a whole-module checkpoint written under this library is a valid reference checkpoint --
+    it references the same classes as the reference's own checkpoint of the same generator and carries, module by
+    module, the same attribute names and the same state_dict keys and shapes."""
+    ref_path = _reference_checkpoint(tmp_path, "A")
+    out = _run(r'''
+import sys, zipfile, pickletools
 sys.path.insert(0, sys.argv[1])
 import torch, fenerf_b200
 g, s = fenerf_b200.install()
 torch.manual_seed(0)
 gen = g.ImplicitGenerator3d(s.TALLSIREN, 256, 4)
 gen.set_device("cpu")
-torch.save(gen, sys.argv[3])
-torch.save(gen.state_dict(), sys.argv[3] + ".sd")
-''', path)
-    out = _run(_STUBS + r'''
-sys.path.insert(0, sys.argv[2])
-import warnings; warnings.simplefilter("ignore")
-import torch
-gen = torch.load(sys.argv[3], map_location="cpu", weights_only=False)
-import generators.generators as gg
-assert gg.__file__.startswith(sys.argv[2]) and type(gen) is gg.ImplicitGenerator3d
-sd = torch.load(sys.argv[3] + ".sd", map_location="cpu")
+gen.step, gen.epoch = 1234, 7
+path = sys.argv[3] + ".mirror"
+torch.save(gen, path)
+
+def globals_of(p):
+    with zipfile.ZipFile(p) as z:
+        data = z.read(next(n for n in z.namelist() if n.endswith("/data.pkl")))
+    return sorted({arg for op, arg, _ in pickletools.genops(data) if op.name == "GLOBAL"})
+want, got = globals_of(sys.argv[3]), globals_of(path)
+assert got == want, (sorted(set(got) ^ set(want)))
+assert all(not x.startswith("fenerf_b200") for x in got)
+ref = torch.load(sys.argv[3], map_location="cpu", weights_only=False)
+mine = torch.load(path, map_location="cpu", weights_only=False)
+mods_ref, mods_mine = dict(ref.named_modules()), dict(mine.named_modules())
+assert list(mods_ref) == list(mods_mine)
+for name, m in mods_ref.items():
+    assert type(m).__name__ == type(mods_mine[name]).__name__, name
+    assert sorted(vars(m)) == sorted(vars(mods_mine[name])), (name, sorted(set(vars(m)) ^ set(vars(mods_mine[name]))))
+sd_ref, sd_mine = ref.state_dict(), mine.state_dict()
+assert list(sd_ref) == list(sd_mine)
+assert all(sd_ref[k].shape == sd_mine[k].shape for k in sd_ref)
 for k, v in gen.state_dict().items():
-    assert torch.equal(v, sd[k]), k
-torch.manual_seed(3)
-with torch.no_grad():
-    px, poses = gen(torch.randn(1, 256), img_size=8, fov=12, ray_start=0.88, ray_end=1.12, num_steps=4, h_stddev=0.,
-                    v_stddev=0., h_mean=1.57, v_mean=1.57, hierarchical_sample=True, clamp_mode='relu', nerf_noise=0.)
-assert px.shape == (1, 3, 8, 8)
+    assert torch.equal(v, sd_mine[k]), k
 print("ok")
-''', path)
+''', ref_path)
     assert "ok" in out

@@ -3,7 +3,7 @@
 At BASELINE.json's sizes (cfg2: 4 x 128 x 128 rays x 24+24 samples; cfg5: 256 x 256 x 48+48) the CPU
 oracle would need minutes per case, so these tests use what the domain offers instead:
 
-  * mode agreement: the tcgen05 path (default GUARD precision) against the fp32 CUDA-core path (EXACT),
+  * mode agreement: the wgmma path (default GUARD precision) against the fp32 CUDA-core path (EXACT),
     which tests/test_gpu_parity.py pins to the oracle at small sizes, on the same replayed RNG draws --
     the north-star bound (1e-3 max-abs on pixels) must hold at full size;
   * image independence: every ray is independent (SURVEY.md section 8e), so rendering four faces in one

@@ -95,7 +95,7 @@ def test_field_exact_stage(runs, name):
 
 @pytest.mark.parametrize("name", ["a_small", "b_small", "b_small_opaque", "c_small", "d_small"])
 def test_field_fast_stage(runs, name):
-    """tcgen05 path vs oracle on the raw field outputs: fp16 operand rounding through 9-11 FiLM
+    """wgmma path vs oracle on the raw field outputs: fp16 operand rounding through 9-11 FiLM
     layers (gain ~1 per layer) stays at the few-1e-4 level (SURVEY.md section 7, hard part 1)."""
     case, run = runs(name)
     st = run["out"]["stages"]
@@ -111,7 +111,7 @@ def test_field_fast_stage(runs, name):
 @pytest.mark.parametrize("model", ["a_small", "b_small"])
 @pytest.mark.parametrize("n_points", [1, 127, 128, 129, 256, 389, 148 * 256 + 128, 148 * 512 + 37])
 def test_field_fast_tile_counts_against_the_fp32_path(model, n_points):
-    """One tile, a lone odd tile, a ragged last tile, one / two tile pairs per CTA plus a remainder: the persistent tcgen05
+    """One tile, a lone odd tile, a ragged last tile, one / two tile pairs per CTA plus a remainder: the persistent wgmma
     kernel against the fp32 path of the same library on the same points.  (Round 2 found that results depended on how
     the issuer warps' lanes left their barrier waits once the issue instructions became warp-level: a single tile was
     enough to show it.)"""
@@ -140,9 +140,6 @@ def _oracle_cdf(st, s):
     return torch.cat([torch.zeros_like(cdf[:, :1]), cdf], -1)
 
 
-_INDS_REPORT = {}
-
-
 @pytest.mark.parametrize("name,z_tol,inds_frac,tie_tol", [
     ("a_small_opaque", 2e-5, 0.999, 2e-6), ("b_small_opaque", 2e-5, 0.999, 2e-6), ("a_small", 5e-4, 0.99, 2e-4),
     ("a_small_noise", 5e-4, 0.99, 2e-4), ("b_small", 5e-4, 0.99, 2e-4), ("a_hier_softplus", 5e-4, 0.99, 2e-4),
@@ -156,7 +153,6 @@ def test_resample_stage(runs, name, z_tol, inds_frac, tie_tol):
     sigma ~ 0.03 of a random-init field (alpha ~ 4e-4: one ulp of exp() is 1.4e-4 relative -- torch's
     vectorised CPU exp and CUDA's expf both stay within their 1-2 ulp but are not the same function), the
     opaque fixtures (alpha ~ 1e-2) pin it 100x tighter.  z_fine is continuous across such a flip."""
-    import json, os
     case, run = runs(name)
     st = run["out"]["stages"]
     rd = _desc(case)
@@ -179,12 +175,6 @@ def test_resample_stage(runs, name, z_tol, inds_frac, tie_tol):
         adjacent = bool(((got - want).abs()[mism] == 1).all())
         worst_tie = float((u[mism] - cdf[rows, edge]).abs().max())
     rate = float(same.float().mean())
-    _INDS_REPORT[name] = dict(rays=int(got.shape[0]), draws=int(got.numel()), exact_match_rate=rate, mismatches=n_mis,
-                              all_mismatches_adjacent=adjacent, max_abs_u_minus_cdf_edge=worst_tie, tie_tol=tie_tol,
-                              max_abs_dz=zerr)
-    os.makedirs(os.path.join(_cases.ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(_cases.ROOT, "gpurun_out", "resample_inds_report.json"), "w") as f:
-        json.dump(_INDS_REPORT, f, indent=1)
     msg = "inds identical %.4f %% (%d of %d differ), worst |u - cdf_edge| %.3g, max|dz| %.3g, max|dp| %.3g" % (
         100 * rate, n_mis, got.numel(), worst_tie, zerr, perr)
     assert adjacent, msg
@@ -269,7 +259,7 @@ def test_end_to_end_exact(runs, case):
 
 @pytest.mark.parametrize("case", _cases.CASES, ids=lambda c: c.name)
 def test_end_to_end_default_precision(runs, case):
-    """The default (tcgen05 + guard refinement) mode against the north-star bound."""
+    """The default (wgmma + guard refinement) mode against the north-star bound."""
     case, run = runs(case.name)
     gen, pixels, poses, depth_map = _end_to_end(case, run, "guard")
     _check_pixels(case, run, pixels, 1e-3)
@@ -412,7 +402,7 @@ def test_inversion_gradients_through_forward_with_frequencies(runs, name):
     assert all(p.grad is None for p in gen.parameters())
 
 
-def test_part_forward_ray_subset_training():
+def test_part_forward_ray_subset_training(monkeypatch):
     """generators.py:858-910 (`grad_points`): every ray rendered, a random 3/8 of them carry the gradient.  Frames,
     poses and gradients against the reference's own part_forward, its draws (per ray subset) replayed."""
     import os
@@ -438,12 +428,30 @@ def test_part_forward_ray_subset_training():
         worst[key] = ((got[key].detach().cpu() - want).abs().max() / want.abs().max()).item()
     bad = {k: "%.2e" % v for k, v in worst.items() if v > (0.3 if k[2:] in KINK_KEYS else 2e-2)}
     assert not bad, "part_forward gradients: %s (all %s)" % (bad, {k: "%.1e" % v for k, v in worst.items()})
-    # and the no_grad flavour of the same call renders the same frames
+    # and the no_grad flavour of the same call renders the same frames.  Both flavours run the same fenerf_render_forward
+    # on the same draws; only the FiLM table differs: under no_grad it comes from the fused mapping kernels, with
+    # autograd from the torch modules.  From the modules' table the no_grad render is bit-identical to the grad one ...
+    from fenerf_b200.siren import siren as siren_mod
+    zs = [z.detach() for z in latents]
+    kw = dict(case.cfg, grad_points=int(gold["grad_points"]))
     with torch.no_grad():
-        px2, _ = gen(*[z.detach() for z in latents], **dict(case.cfg, grad_points=int(gold["grad_points"]), _rng=ReplayRng(draws, DEV)))
-    # (not bit-equal: under no_grad the FiLM table comes from the fused mapping kernels, with autograd from the modules)
+        px2, _ = gen(*zs, **kw, _rng=ReplayRng(draws, DEV))
+        film_fused = gen.siren.film_from_latents(*zs)
+        with monkeypatch.context() as m:
+            m.setattr(siren_mod, "_fused_mapping_ok", lambda *a: False)
+            film_mod = gen.siren.film_from_latents(*zs)
+            px3, _ = gen(*zs, **kw, _rng=ReplayRng(draws, DEV))
+    assert torch.equal(px3, pixels.detach()), float((px3 - pixels.detach()).abs().max())
+    # ... and the two tables agree to fp32 rounding (different summation orders of the same fp32 products) ...
+    ferr = float(((film_fused - film_mod).abs() / film_mod.abs().clamp_min(1.0)).max())
+    assert ferr <= 1e-5, "fused vs module FiLM table: %g" % ferr
+    # ... which the fp16 operands of the default point network turn into one-ulp flips of a few fp16 activations.  Those
+    # move a handful of pixels by ~1e-4 (on H100: 3 pixels beyond 1e-4, the largest 2.1e-4); none may reach the parity bound.
     d = (px2 - pixels.detach()).abs().amax(1)
-    assert int((d > 1e-4).sum()) <= 2, "no_grad vs grad frames differ: %d pixels beyond 1e-4 (max %g)" % (int((d > 1e-4).sum()), float(d.max()))
+    msg = "no_grad vs grad frames differ: %d pixels beyond 1e-4 (max %g; FiLM tables %g apart)" % (
+        int((d > 1e-4).sum()), float(d.max()), ferr)
+    assert int((d > 1e-4).sum()) <= 4, msg
+    assert float(d.max()) <= 1e-3, msg
 
 
 def test_backward_under_autocast_and_gradscaler():
@@ -658,7 +666,7 @@ def test_frame_consumers_match_the_reference_loops():
 
 def test_guard_self_check_widens_the_threshold_on_large_weights():
     """The GUARD threshold was calibrated on the reference's initialisation (VERDICT r1, weak #4).  The refinement
-    reports max |sigma_fp32 - sigma_tcgen05| over the samples it re-evaluates; staged_* widens tau when that error
+    reports max |sigma_fp32 - sigma_wgmma| over the samples it re-evaluates; staged_* widens tau when that error
     comes within 3x of it.  Scaling the density head by 30 scales the fp16 error with it."""
     import warnings
     case = _cases.CASE_BY_NAME["a_small"]

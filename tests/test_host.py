@@ -32,7 +32,7 @@ def test_library_exports_every_symbol_the_header_declares():
     assert sorted(_lib.EXPORTS) == declared
     # no compute calls without a GPU: only the pure-host queries
     lib.fenerf_abi_version.restype = ctypes.c_int32
-    assert lib.fenerf_abi_version() == 2
+    assert lib.fenerf_abi_version() == 3
 
 
 def test_packed_and_workspace_sizes_are_computed_on_the_host():

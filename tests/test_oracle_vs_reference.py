@@ -1,5 +1,9 @@
-"""Bit-equality of the oracle with the live, unmodified reference.  Runs only where /root/reference
-exists (the build container); the GPU box relies on the committed goldens instead."""
+"""The oracle against the unmodified reference on the same inputs.  With a reference checkout
+($FENERF_REFERENCE_ROOT) the reference runs live and the match must be bit-exact; without one the
+reference's stored outputs (tests/golden/*.npz, made by tests/golden/make_goldens.py) stand in for it, at
+the cross-host tolerance of test_oracle.py (the goldens' host may round sgemm / vectorised sums differently).
+That fallback overlaps test_oracle.py::test_oracle_matches_reference_golden on these cases; the bit-exact
+comparison needs the live reference."""
 import numpy as np
 import pytest
 import torch
@@ -8,7 +12,7 @@ import _cases
 import _harness
 from oracle import ref_shim
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present")
+TOL = 2e-5
 
 
 @pytest.mark.parametrize("name", ["a_small", "a_small_noise", "a_nohier_softplus", "a_lockview_uniform", "b_small", "c_small", "d_small",
@@ -19,6 +23,12 @@ def test_oracle_is_bit_exact_with_reference(name):
     sys.path.insert(0, _cases.GOLDEN_DIR)
     import make_goldens
     case = _cases.CASE_BY_NAME[name]
+    run = _harness.oracle_run(case, keep_stages=False)
+    if not ref_shim.available():
+        gold = np.load(_cases.golden_path(case))
+        assert np.abs(run["out"]["pixels"].numpy() - gold["pixels"]).max() <= TOL
+        assert np.abs(run["out"]["poses"].numpy() - gold["poses"]).max() <= 1e-6
+        return
     ref_generators, ref_siren, _ = ref_shim.load()
     gen_ref, _ = make_goldens.build_reference(case, ref_generators, ref_siren)
     latents = _cases.make_latents(case)
@@ -27,6 +37,5 @@ def test_oracle_is_bit_exact_with_reference(name):
     random.seed(case.seed)
     with torch.no_grad():
         px_ref, poses_ref = gen_ref(*latents, **_cases.reference_kwargs(case))
-    run = _harness.oracle_run(case, keep_stages=False)
     assert torch.equal(run["out"]["pixels"], px_ref), float((run["out"]["pixels"] - px_ref).abs().max())
     assert torch.equal(run["out"]["poses"], poses_ref)
