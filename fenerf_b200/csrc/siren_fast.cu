@@ -4,13 +4,22 @@
 //   warps 0..3, 4..7   two consumer warpgroups; each evaluates the whole network for its own tile of 64 points
 //   warp 8             weight producer (its warpgroup gives its registers to the consumers): bulk copies of the packed weight images (layout.h) into a ring of six
 //                      32 KB slots, in the order the consumers read them; both warpgroups read every slot
+//   warps 9, 10        FiLM producers, one per consumer warpgroup: bulk copies of each layer's FiLM frequencies, phases
+//                      and bias (3 KB) into a two-entry ring of that warpgroup, so that the epilogue reads them from
+//                      shared memory
 //
 // A layer is D[64 points x 256] = A[64 x 256] . W^T with A in registers (wgmma m64n128k16, one feature half at a
 // time) and W from the ring.  The accumulator fragment of wgmma is the register A fragment of the next layer
 // (sm90.cuh), so the FiLM epilogue sin(f z + (f b + p)) turns half h of the accumulator into k-slices 8h .. 8h+7
-// of the next layer's A operand without touching shared memory.  While one warpgroup runs its epilogue the other
-// keeps the tensor cores busy.  Registers per consumer thread: 64 (A) + 64 (accumulator) + 32 (half of the next
-// A) + the input slots of the first colour layer, within the 232 that setmaxnreg grants.
+// of the next layer's A operand without touching shared memory.  Registers per consumer thread: 64 (A) + 64
+// (accumulator) + 32 (half of the next A) + the input slots of the first colour layer, within the 232 that setmaxnreg
+// grants.
+//
+// The two consumer warpgroups take turns at the tensor cores (ping-pong): a warpgroup waits for its turn, issues one
+// MMA group (a half layer with the colour-layer input slices, a first-layer half, or a head), commits it and hands the
+// turn to the other warpgroup; only then does it wait for its own MMAs and run their epilogue.  The tensor cores
+// execute the MMA groups in issue order, so one warpgroup's sin epilogue runs under the other's MMAs instead of both
+// warpgroups computing sines at once while the tensor cores idle.  The turns are a pair of mbarriers (bounded waits).
 //
 // The input slots of a point (layout.h: positions, view direction and grid features, hi / lo split in fp16) are
 // built once per tile by one thread per point into a small staging buffer and read from there as A fragments.
@@ -31,8 +40,12 @@ constexpr int RING = 6;
 constexpr uint32_t SLOT_BYTES = 32768;
 constexpr int XSTRIDE = 72;                         // f16 per point row of the input-slot staging buffer (144 B)
 constexpr uint32_t SMEM_X = RING * SLOT_BYTES;      // [2 warpgroups][64 points][XSTRIDE] f16
-constexpr uint32_t SMEM_BAR = SMEM_X + 2 * TILE * XSTRIDE * 2;
-constexpr uint32_t SMEM_TOTAL = SMEM_BAR + 16 * RING;
+constexpr int FRING = 2;                            // FiLM entries per consumer warpgroup
+constexpr uint32_t FILM_BYTES = 3 * FN_H * 4;       // one layer: [frequency 256][phase 256][bias 256] f32
+constexpr uint32_t SMEM_FILM = SMEM_X + 2 * TILE * XSTRIDE * 2;   // [2 warpgroups][FRING] entries
+constexpr uint32_t SMEM_BAR = SMEM_FILM + 2 * FRING * FILM_BYTES;
+// full[RING], empty[RING], turn[2], film_full[2 * FRING], film_empty[2 * FRING]
+constexpr uint32_t SMEM_TOTAL = SMEM_BAR + 16 * RING + 16 + 16 * 2 * FRING;
 constexpr int MAX_LOADS = 72;
 constexpr uint32_t CHUNK = 16384;                   // one [128 rows][64 k] f16 image chunk
 constexpr uint32_t HEAD_CHUNK = 32 * 128;           // one [32 rows][64 k] chunk of the trunk-head image
@@ -64,11 +77,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * RING;
+    const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * RING, bar_turn = bar_empty + 8 * RING;
+    const uint32_t bar_ffull = bar_turn + 16, bar_fempty = bar_ffull + 8 * 2 * FRING;
     if (threadIdx.x == 0) {
         for (int i = 0; i < RING; ++i) {
             mbar_init(bar_full + 8 * i, 1);
             mbar_init(bar_empty + 8 * i, 8);        // one arrival per consumer warp
+        }
+        for (int g = 0; g < 2; ++g) mbar_init(bar_turn + 8 * g, 4);     // warpgroup g's turn: one arrival per warp of the other
+        for (int e = 0; e < 2 * FRING; ++e) {
+            mbar_init(bar_ffull + 8 * e, 1);
+            mbar_init(bar_fempty + 8 * e, 4);       // one arrival per warp of the entry's warpgroup
         }
         fence_barrier_init();
     }
@@ -87,6 +106,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                     mbar_arrive_expect_tx(bar_full + 8 * slot, a.loads[i].bytes);
                     bulk_g2s(sbase + slot * SLOT_BYTES, a.packed + a.loads[i].src, a.loads[i].bytes, bar_full + 8 * slot);
                 }
+        } else if ((warp == PROD_WARP + 1 || warp == PROD_WARP + 2) && lane == 0) {
+            // the FiLM layers of consumer warpgroup g's tiles, in the order its epilogues use them: the first layer, then
+            // hidden layers 0 .. n - 1 (n = trunk_hidden when the network stops after the trunk head)
+            const int g = warp - PROD_WARP - 1;
+            const int n_film = 1 + (a.sigma_only ? a.L.trunk_hidden : a.L.n_hidden);
+            uint32_t it = 0;
+            for (long long pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
+                const long long tile = pair * 2 + g;
+                const long long b = tile < a.n_tiles ? tile / a.tiles_per_batch : 0;
+                const float* film_b = a.film + (size_t)b * a.L.n_film * 2 * FN_H;
+                for (int i = 0; i < n_film; ++i, ++it) {
+                    const uint32_t e = g * FRING + it % FRING;
+                    const uint32_t dst = sbase + SMEM_FILM + e * FILM_BYTES;
+                    mbar_wait(bar_fempty + 8 * e, ((it / FRING) & 1u) ^ 1u);
+                    mbar_arrive_expect_tx(bar_ffull + 8 * e, FILM_BYTES);
+                    bulk_g2s(dst, film_b + (size_t)i * 2 * FN_H, 2 * FN_H * 4, bar_ffull + 8 * e);
+                    bulk_g2s(dst + 2 * FN_H * 4, a.packed + (i == 0 ? a.L.first_b : a.L.hid_b[i - 1]), FN_H * 4, bar_ffull + 8 * e);
+                }
+            }
         }
         return;
     }
@@ -114,6 +152,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_empty + 8 * slot);
     };
+    // MMA turns, strictly alternating and warpgroup 0 first: turn n of warpgroup 1 waits for phase n of its barrier, turn
+    // n of warpgroup 0 for phase n - 1 of its own (its first turn passes at once).  Invariant: both warpgroups take the
+    // same number of turns for every tile pair -- they run the same sequence of layers, the warpgroup without a tile in a
+    // CTA's last pair included, and the sigma_only stop comes after the same trunk-head turn in both.  A warpgroup that
+    // took one turn more would wait for a handover that never comes (and trap).
+    uint32_t turns = 0;
+    // this warpgroup's FiLM entries (filled by its FiLM producer), one per layer, in layer order
+    uint32_t fit = 0;
+    auto film_acquire = [&]() -> const float* {
+        const uint32_t e = wg * FRING + fit % FRING;
+        mbar_wait(bar_ffull + 8 * e, (fit / FRING) & 1u);
+        return reinterpret_cast<const float*>(smem + SMEM_FILM + e * FILM_BYTES);
+    };
+    auto film_release = [&]() {
+        const uint32_t e = wg * FRING + fit % FRING;
+        ++fit;
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_fempty + 8 * e);
+    };
+    auto turn_begin = [&]() { mbar_wait(bar_turn + 8 * wg, (turns & 1u) ^ (wg == 0 ? 1u : 0u)); };
+    auto turn_end = [&]() {                          // after wg_commit: this warp's share of the MMA group is issued
+        ++turns;
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_turn + 8 * (wg ^ 1));
+    };
     // A fragment of k-slice s of the staged input slots
     auto xfrag = [&](int s, uint32_t (&f)[4]) {
         const __half* p = xs + r0 * XSTRIDE + 16 * s + 2 * q;
@@ -130,7 +193,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         const bool tile_ok = tile < a.n_tiles;
         const long long b = tile_ok ? tile / a.tiles_per_batch : 0;
         const long long p0 = tile_ok ? (tile % a.tiles_per_batch) * TILE : a.ppb;
-        const float* film_b = a.film + (size_t)b * L.n_film * 2 * FN_H;
 
         // ---- input slots of the tile's points (layout.h), one thread per point ----
         wg_bar(wg);                                  // the previous tile's fragment reads are done
@@ -175,16 +237,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         uint32_t act[16][4];                         // A operand: k-slice s = features 16 s .. 16 s + 15
         uint32_t nxt[8][4];                          // the next layer's slices 0..7 while half 1 is still being computed
         float d[64];
-        // FiLM epilogue of accumulator half h: sin(f z + (f b + p)) -> dst[0..7] = k-slices 8h .. 8h+7 of the next layer
-        auto film_epi = [&](int film_idx, size_t bias_off, int h, uint32_t (&dst)[8][4]) {
-            const float* fl = film_b + (size_t)film_idx * 2 * FN_H + h * 128;
-            const float* bias = reinterpret_cast<const float*>(a.packed + bias_off) + h * 128;
+        // FiLM epilogue of accumulator half h: sin(f z + (f b + p)) -> dst[0..7] = k-slices 8h .. 8h+7 of the next layer;
+        // fs is the layer's FiLM entry in shared memory
+        auto film_epi = [&](const float* fs, int h, uint32_t (&dst)[8][4]) {
+            const float* fl = fs + h * 128;
+            const float* bias = fs + 2 * FN_H + h * 128;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
                 const int c = 8 * j + 2 * q;
-                const float2 fr = __ldg(reinterpret_cast<const float2*>(fl + c));
-                const float2 ph = __ldg(reinterpret_cast<const float2*>(fl + FN_H + c));
-                const float2 bi = __ldg(reinterpret_cast<const float2*>(bias + c));
+                const float2 fr = *reinterpret_cast<const float2*>(fl + c);
+                const float2 ph = *reinterpret_cast<const float2*>(fl + FN_H + c);
+                const float2 bi = *reinterpret_cast<const float2*>(bias + c);
                 const float px = fmaf(fr.x, bi.x, ph.x), py = fmaf(fr.y, bi.y, ph.y);
                 dst[j >> 1][(j & 1) * 2] = pack_half2(__sinf(fmaf(fr.x, d[4 * j], px)), __sinf(fmaf(fr.y, d[4 * j + 1], py)));
                 dst[j >> 1][(j & 1) * 2 + 1] = pack_half2(__sinf(fmaf(fr.x, d[4 * j + 2], px)), __sinf(fmaf(fr.y, d[4 * j + 3], py)));
@@ -195,20 +258,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         // ---- first layer: input slots (k-slice 0) against the [256][64] input image ----
         {
             uint32_t xf[4], slot;
+            const float* fs = nullptr;
             xfrag(0, xf);
             const uint32_t w = acquire(slot);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
+                turn_begin();
                 wg_fence();
                 mma_rs_n128(d, xf, desc_kmajor(w + h * CHUNK), 0u);
                 wg_commit();
+                turn_end();
                 wg_wait<0>();
                 fence_regs(d);
                 fence_regs(xf);
-                if (h == 0) film_epi(0, L.first_b, 0, nxt);
-                else film_epi(0, L.first_b, 1, act_hi());
+                if (h == 0) fs = film_acquire();
+                if (h == 0) film_epi(fs, 0, nxt);
+                else film_epi(fs, 1, act_hi());
             }
             release(slot);
+            film_release();
 #pragma unroll
             for (int s = 0; s < 8; ++s)
 #pragma unroll
@@ -222,12 +290,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 float dh[16];
                 uint32_t slot;
                 const uint32_t w = acquire(slot);
+                turn_begin();                        // after acquire: the other order makes ptxas serialize the wgmmas
                 wg_fence();
 #pragma unroll
                 for (int c = 0; c < 4; ++c)
 #pragma unroll
                     for (int k = 0; k < 4; ++k) mma_rs_n32(dh, act[4 * c + k], desc_kmajor(w + c * HEAD_CHUNK + 32 * k), (c | k) ? 1u : 0u);
                 wg_commit();
+                turn_end();
                 wg_wait<0>();
                 fence_regs(dh);
                 fence_regs(act);
@@ -264,9 +334,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                 for (int s = 0; s < 3; ++s) xfrag(1 + s, xf[s]);
             uint32_t slot_x = 0, w_x = 0;
+            const float* fs = nullptr;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 uint32_t sl[2];
+                turn_begin();
                 wg_fence();
 #pragma unroll
                 for (int sb = 0; sb < 2; ++sb) {
@@ -284,6 +356,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                         if (s < nx) mma_rs_n128(d, xf[s], desc_kmajor(w_x + h * CHUNK + 32 * (1 + s)), 1u);
                 }
                 wg_commit();
+                turn_end();
                 wg_wait<0>();
                 fence_regs(d);
                 fence_regs(act);
@@ -291,9 +364,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 release(sl[0]);
                 release(sl[1]);
                 if (c0 && h == 1) release(slot_x);
-                if (h == 0) film_epi(l + 1, L.hid_b[l], 0, nxt);
-                else film_epi(l + 1, L.hid_b[l], 1, act_hi());
+                if (h == 0) fs = film_acquire();
+                if (h == 0) film_epi(fs, 0, nxt);
+                else film_epi(fs, 1, act_hi());
             }
+            film_release();
 #pragma unroll
             for (int s = 0; s < 8; ++s)
 #pragma unroll
@@ -306,12 +381,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             float dr[4];
             uint32_t slot;
             const uint32_t w = acquire(slot);
+            turn_begin();
             wg_fence();
 #pragma unroll
             for (int c = 0; c < 4; ++c)
 #pragma unroll
                 for (int k = 0; k < 4; ++k) mma_rs_n8(dr, act[4 * c + k], desc_kmajor(w + c * RGB_CHUNK + 32 * k), (c | k) ? 1u : 0u);
             wg_commit();
+            turn_end();
             wg_wait<0>();
             fence_regs(dr);
             fence_regs(act);
@@ -367,6 +444,7 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     FN_REQUIRE(L.trunk_hidden >= 1 && L.n_hidden - L.trunk_hidden >= 1, "field needs >= 2 trunk and >= 1 colour layers");
     FN_REQUIRE(L.label_dim < 32, "the fast path packs labels and sigma into one 32-column head (label_dim <= 31)");
     FN_REQUIRE(L.rgb_img < 0xFFFFFFFFull, "packed weight images beyond 4 GB");
+    FN_REQUIRE(((uintptr_t)film & 15) == 0, "the FiLM table must be 16-byte aligned");
     FastArgs a;
     memset(&a, 0, sizeof(a));
     FN_REQUIRE(build_loads(L, a, sigma_only != 0), "field too deep for the weight stream");
