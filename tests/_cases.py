@@ -200,6 +200,22 @@ def loss_weights(shape):
     return torch.randn(shape, generator=g)
 
 
+#: point-network launch shapes named after what they do to the fast kernel's persistent schedule (csrc/siren_fast.cu):
+#: 64-point tiles, never shared between images; two tiles (one per consumer warpgroup) form a pair; CTAs = min(pairs, SMs),
+#: each striding over the pairs.  The last tile of every image is ragged.
+TILE_LAYOUTS = ("one_pair_per_cta", "lone_tile_in_second_pair", "4sms_minus_1", "b3_pairs_straddle_images")
+
+
+def tile_layout(name, sms, dir_group=1):
+    """-> (batch, points per image) of a TILE_LAYOUTS entry on a GPU with `sms` SMs (points a multiple of dir_group)."""
+    batch, tiles = {"one_pair_per_cta": (2, sms),                    # 2 SMs tiles: every CTA runs exactly one pair
+                    "lone_tile_in_second_pair": (1, 2 * sms + 1),    # CTA 0 comes back for a pair holding one tile
+                    "4sms_minus_1": (1, 4 * sms - 1),                # two pairs per CTA, the very last one half empty
+                    "b3_pairs_straddle_images": (3, sms | 1)}[name]  # odd tiles per image: pairs cross image borders
+    ppb = tiles * 64 - 37
+    return batch, ppb - ppb % dir_group
+
+
 def grid_probe_index(numel, n):
     """Fixed pseudo-random flat indices into the feature grid (the gradient goldens store only these entries)."""
     g = torch.Generator().manual_seed(7)

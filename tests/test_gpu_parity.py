@@ -108,27 +108,56 @@ def test_field_fast_stage(runs, name):
     assert err.max() <= 3e-3, "max|fast field - oracle| = %g (per channel %s)" % (err.max(), err.amax((0, 1, 2)))
 
 
-@pytest.mark.parametrize("model", ["a_small", "b_small"])
-@pytest.mark.parametrize("n_points", [1, 127, 128, 129, 256, 389, 148 * 256 + 128, 148 * 512 + 37])
+#: one parity case per field class A-H (E: e_staged_debug's 23-channel D)
+FIELD_CASES = ["a_small", "b_small", "c_small", "d_small", "e_staged_debug", "f_small", "g_small", "h_small"]
+
+
+def _tile_test_inputs(n_points, seed):
+    """(batch, points per image, how directions are passed) of a point count or of a named _cases.TILE_LAYOUTS schedule.
+    The named schedules pass one direction per 24-sample ray, or one locked (0, 0, -1) per image, in turn."""
+    if isinstance(n_points, int):
+        return 2, n_points, "per_point"
+    sms = torch.cuda.get_device_properties(DEV).multi_processor_count
+    mode = ("per_point", "dir_group24", "lock_dirs")[seed % 3]
+    batch, ppb = _cases.tile_layout(n_points, sms, 24 if mode == "dir_group24" else 1)
+    return batch, ppb, mode
+
+
+def _tile_test_dirs(batch, ppb, mode, g):
+    n = {"per_point": ppb, "dir_group24": ppb // 24, "lock_dirs": 1}[mode]
+    dirs = torch.nn.functional.normalize(torch.randn(batch, n, 3, device=DEV, generator=g), dim=-1)
+    if mode == "lock_dirs":
+        dirs = torch.zeros_like(dirs)
+        dirs[..., 2] = -1
+    return dirs
+
+
+@pytest.mark.parametrize("model", FIELD_CASES)
+@pytest.mark.parametrize("n_points", [1, 127, 128, 129, 256, 389] + list(_cases.TILE_LAYOUTS))
 def test_field_fast_tile_counts_against_the_fp32_path(model, n_points):
-    """One tile, a lone odd tile, a ragged last tile, one / two tile pairs per CTA plus a remainder: the persistent wgmma
-    kernel against the fp32 path of the same library on the same points.  (Round 2 found that results depended on how
-    the issuer warps' lanes left their barrier waits once the issue instructions became warp-level: a single tile was
-    enough to show it.)"""
+    """One tile, a lone odd tile, a ragged last tile, and the persistent schedules of the device's own SM count (one pair
+    per CTA, a lone tile in a second pair, two pairs per CTA, pairs across image borders): the wgmma kernel against the
+    fp32 path of the same library on the same points, and the density-only entry against the full evaluation.  (Round 2
+    found that results depended on how the issuer warps' lanes left their barrier waits once the issue instructions
+    became warp-level: a single tile was enough to show it.)"""
     case = _cases.CASE_BY_NAME[model]
     gen = _cases.build_mirror(case, DEV)
-    g = torch.Generator(device=DEV).manual_seed(n_points)
-    pts = (torch.rand(2, n_points, 3, device=DEV, generator=g) - 0.5) * 0.3
-    dirs = torch.nn.functional.normalize(torch.randn(2, n_points, 3, device=DEV, generator=g), dim=-1)
-    zs = [torch.randn(2, 256, device=DEV, generator=g) for _ in range(_cases.n_latents(model[0].upper()))]
+    seed = n_points if isinstance(n_points, int) else _cases.TILE_LAYOUTS.index(n_points) + FIELD_CASES.index(model)
+    batch, ppb, mode = _tile_test_inputs(n_points, seed)
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    pts = (torch.rand(batch, ppb, 3, device=DEV, generator=g) - 0.5) * 0.3
+    dirs = _tile_test_dirs(batch, ppb, mode, g)
+    zs = [torch.randn(batch, 256, device=DEV, generator=g) for _ in range(_cases.n_latents(case.model))]
     with torch.no_grad():
         film = gen.siren.film_from_latents(*zs)
         fast = ops.siren_points(gen.siren, pts, film, dirs, precision="fast")
         again = ops.siren_points(gen.siren, pts, film, dirs, precision="fast")
         exact = ops.siren_points(gen.siren, pts, film, dirs, precision="exact")
+        sigma = ops.siren_sigma(gen.siren, pts, film, precision="fast")
     assert torch.equal(fast, again), "two launches on the same inputs differ"
+    assert torch.equal(sigma, fast[..., -1:]), "the density-only entry differs from the full evaluation"
     err = (fast - exact).abs().amax((0, 1))
-    assert torch.isfinite(fast).all() and err.max() <= 5e-3, "max|fast - exact| per channel %s" % err
+    assert torch.isfinite(fast).all() and err.max() <= 5e-3, "max|fast - exact| per channel %s (%s)" % (err, mode)
 
 
 def _oracle_cdf(st, s):
