@@ -26,6 +26,7 @@ import torch
 import torch.nn.functional as F
 
 import _cases
+from _fp64 import _ZeroDraws, _film, _grid_lookup_keep_dtype, _opt, _rel, _siren, composite_ref, field_ref, noise_offset
 from fenerf_b200 import _lib, backward, ops
 from oracle import render_oracle as oracle
 
@@ -55,48 +56,6 @@ FWD_BOUND = {"exact": 1e-5, "fast": 5e-3}
 FIELD_MODELS = ("A", "B", "C", "D", "E", "F", "G", "H", "D32")   # S shares A's field; D32: the widest renderable head
 
 
-@functools.lru_cache(maxsize=None)
-def _generator_cpu(model):
-    if model != "D32":
-        return _cases._mirror_generator_cached(model, False)
-    from fenerf_b200.generators import generators as g
-    from fenerf_b200.siren import siren as s
-    torch.manual_seed(0)
-    gen = g.DoubleImplicitGenerator3d(s.SIRENBASELINESEMANTICDISENTANGLE, 256, 256, 32)   # 28 labels
-    gen.eval()
-    return gen
-
-
-def _siren(model, device, sigma_bias_shift=0.0):
-    gen = copy.deepcopy(_generator_cpu(model))
-    if sigma_bias_shift:
-        with torch.no_grad():
-            gen.siren.final_layer.bias += sigma_bias_shift
-    gen.to(device)
-    gen.device = device
-    gen.siren.device = device
-    return gen.siren
-
-
-def _film(siren, batch, seed, edges=False):
-    """FiLM table (B, L, 2, 256) from random latents.  edges: 10 % of the frequencies negated and 5 % set to
-    0.25 <= |f| <= 1, so that finish()'s dp = db_b / f is exercised away from f ~ 30."""
-    g = torch.Generator().manual_seed(seed)
-    n_lat = 2 if hasattr(siren, "geo_mapping_network") else 1
-    zs = [torch.randn(batch, 256, generator=g) for _ in range(n_lat)]
-    dev = next(siren.parameters()).device
-    with torch.no_grad():
-        film = siren.film_from_latents(*[z.to(dev) for z in zs]).clone()
-    if edges:
-        f = film[:, :, 0]
-        u = torch.rand(f.shape, generator=g).to(dev)
-        mag = (0.25 + 0.75 * torch.rand(f.shape, generator=g)).to(dev) * torch.sign(f)
-        f[u < 0.1] = -f[u < 0.1]
-        small = (u >= 0.1) & (u < 0.15)
-        f[small] = mag[small]
-    return film.contiguous()
-
-
 def _render_points(batch, img, steps, seed):
     """Jittered sample points of a render (the oracle's ray set-up, gaussian poses): points (B, R², S, 3),
     depths (B, R², S), directions (B, R², 3), origins (B, R², 3); CPU fp32."""
@@ -124,61 +83,9 @@ def _per_point(dirs, ppb, lock):
     return dirs.repeat_interleave(ppb // dirs.shape[1], dim=1)
 
 
-def _rel(got, want):
-    s = want.abs().max().item()
-    return (got.double() - want.double()).abs().max().item() / (s if s > 0 else 1.0)
-
-
 # --------------------------------------------------------------------------------------------
 # 0. float64 references
 # --------------------------------------------------------------------------------------------
-class _ZeroDraws:
-    """alpha_composite's noise draw: zero (the noise is added to sigma beforehand, in fp32)."""
-
-    def __init__(self, like):
-        self.like = like
-
-    def randn(self, *shape):
-        return torch.zeros(shape, dtype=self.like.dtype, device=self.like.device)
-
-
-def _merge(raw_c, z_c, raw_f, z_f):
-    """Stable sort on depth, fine samples first (composite.cu's tie rule)."""
-    if raw_f is None:
-        return raw_c, z_c
-    raw, z = torch.cat([raw_f, raw_c], 2), torch.cat([z_f, z_c], 2)
-    z, order = torch.sort(z, dim=2, stable=True)
-    return torch.gather(raw, 2, order.to(raw.device).unsqueeze(-1).expand(-1, -1, -1, raw.shape[-1])), z
-
-
-def noise_offset(raw_c, z_c, raw_f, z_f, noise, std):
-    """(sigma + noise * std) - sigma per merged sample, with the sum formed in fp32 as the reference and the kernel form it."""
-    sig = _merge(raw_c, z_c, raw_f, z_f)[0][..., -1].detach().float()
-    return (sig + noise.to(sig.device) * std).double() - sig.double()
-
-
-def composite_ref(raw_c, z_c, raw_f, z_f, noise, opt, offset=None):
-    """float64 pixels (B, C-1, R, R) of the final compositing.  raw_* float64 (B, N, S, C), possibly requiring grad;
-    z_* (B, N, S) and noise (B, N, n) are the kernel's own fp32 inputs (noise is in merged-sample order).
-
-    Merge fine-first; sigma + noise * std formed in fp32 and then upcast (noise_offset; fixed by `offset` where the
-    function must stay smooth under perturbation), so the relu sees the same sign as in the kernel.  Then
-    oracle.alpha_composite in float64, the label softmax and `* 2 - 1` to NCHW."""
-    raw, z = _merge(raw_c, z_c, raw_f, z_f)
-    sig = raw[..., -1]
-    if noise is not None:
-        sig = sig + (offset if offset is not None else noise_offset(raw_c, z_c, raw_f, z_f, noise, opt["noise"]))
-    raw = torch.cat([raw[..., :-1], sig.unsqueeze(-1)], -1)
-    z = z.to(raw.device).double().unsqueeze(-1)
-    px = oracle.alpha_composite(raw, z, _ZeroDraws(raw), 0.0, opt["clamp"], last_back=opt["last_back"], white_back=opt["white_back"],
-                                black_back=opt["black_back"])[0]
-    if opt["softmax"]:
-        px = torch.cat([torch.softmax(px[..., :-3], -1), px[..., -3:]], -1)
-    b, n = px.shape[:2]
-    r = math.isqrt(n)
-    return px.reshape(b, r, r, -1).permute(0, 3, 1, 2) * 2 - 1
-
-
 def composite_vjp(raw_c, z_c, raw_f, z_f, noise, opt, d_pixels):
     """(d raw_c, d raw_f) in float64 for the upstream gradient d_pixels."""
     leaves = [raw_c.double().requires_grad_(True)] + ([raw_f.double().requires_grad_(True)] if raw_f is not None else [])
@@ -187,47 +94,9 @@ def composite_vjp(raw_c, z_c, raw_f, z_f, noise, opt, d_pixels):
     return grads[0], (grads[1] if raw_f is not None else None)
 
 
-def _grid_lookup_keep_dtype(coords, grid):
-    """oracle.grid_lookup without its .float() casts (the oracle itself stays pinned bit for bit to the reference)."""
-    b, n, d = coords.shape
-    s = F.grid_sample(grid.expand(b, -1, -1, -1, -1), coords.reshape(b, 1, 1, -1, d), mode='bilinear',
-                      padding_mode='zeros', align_corners=True)
-    nn_, c, h, w, dd = s.shape
-    return s.permute(0, 4, 3, 2, 1).reshape(nn_, h * w * dd, c)
-
-
-def field_ref(siren, monkeypatch, points, dirs_pp, film, d_raw=None, film_rows=None, chunk=1 << 15):
-    """oracle.field_eval on a float64 copy of `siren`, on the tensors' device, in point chunks.
-    -> (out (B, P, C) float64, d_film, {parameter name: float64 gradient}); the gradients (the VJP with d_raw, accumulated
-    over the chunks) only when d_raw is given.  film_rows: image index whose FiLM rows each image uses (fault checks)."""
-    monkeypatch.setattr(oracle, "grid_lookup", _grid_lookup_keep_dtype)
-    ref = copy.deepcopy(siren).double()
-    want_grad = d_raw is not None
-    film64 = film.double().requires_grad_(want_grad)
-    for p in ref.parameters():
-        p.requires_grad_(want_grad)
-    outs = []
-    with torch.set_grad_enabled(want_grad):
-        for p0 in range(0, points.shape[1], chunk):
-            p1 = min(points.shape[1], p0 + chunk)
-            fl = film64 if film_rows is None else film64[film_rows]
-            out = oracle.field_eval(ref, points[:, p0:p1].double(), fl, dirs_pp[:, p0:p1].double())
-            if want_grad:
-                (out * d_raw[:, p0:p1].double()).sum().backward()
-            outs.append(out.detach())
-    out = torch.cat(outs, 1)
-    if not want_grad:
-        return out, None, None
-    return out, film64.grad, {n: p.grad for n, p in ref.named_parameters() if p.grad is not None}
-
-
 # --------------------------------------------------------------------------------------------
 # the references' own checks (CPU)
 # --------------------------------------------------------------------------------------------
-def _opt(clamp="relu", noise=0.0, last_back=False, white_back=False, black_back=False, softmax=False):
-    return dict(clamp=clamp, noise=noise, last_back=last_back, white_back=white_back, black_back=black_back, softmax=softmax)
-
-
 @pytest.mark.parametrize("opt", [
     _opt("relu"), _opt("softplus"), _opt("relu", noise=0.5), _opt("softplus", last_back=True), _opt("relu", white_back=True),
     _opt("softplus", black_back=True), _opt("relu", softmax=True), _opt("softplus", noise=0.3, softmax=True, last_back=True)],
