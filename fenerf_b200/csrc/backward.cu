@@ -2,10 +2,9 @@
 //
 // What differentiates through the render in the reference (train_double_latent_semantic.py:405-446,
 // inverse_render_double_semantic.py:385-407): the final fancy_integration over the merged samples and the
-// two point-network passes; ray set-up and resampling are no_grad there too (generators.py:41, 59).
+// two point-network passes; ray set-up and resampling are no_grad there too (generators.py:41, 59).  The
+// compositing backward (composite_backward_kernel) lives beside the forward in composite.cu; the point network's are:
 //
-//   composite_backward_kernel   d pixels -> d raw outputs (coarse and fine), one warp per ray: re-does the
-//                               merge sort and the transmittance scan of composite.cu, then the reverse scan
 //   film_forward_stash_kernel   z (fp32 GEMM output) -> a = sin(f (z + b) + p) and the gate f cos(.) as fp16:
 //                               everything the backward of a FiLM layer needs besides the GEMMs
 //   gate_backward_kernel        dZ = dA * gate in place (fp16) + per-image column sums (bias / phase grads)
@@ -23,172 +22,6 @@
 namespace fn {
 
 namespace {
-
-constexpr unsigned kFull = 0xffffffffu;
-constexpr int kMaxN = 128;
-constexpr int kRaysPerBlock = 8;
-
-__device__ __forceinline__ float softplus_torch(float x) { return x > 20.f ? x : log1pf(expf(x)); }
-
-struct CompositeBwdArgs {
-    long long n_rays, rays_per_batch;
-    int S, n, C, C_img;
-    int clamp_mode, last_back, white_back, black_back, softmax_label;
-    float noise_std;
-    const float *raw_c, *z_c, *raw_f, *z_f, *noise, *d_pixels;
-    float *d_raw_c, *d_raw_f;
-    int n_pad, warp_floats;
-};
-
-// Per-warp shared memory: z[n_pad] zs[n_pad] w[n_pad] ord[n_pad] al[n_pad] tt[n_pad] r[n_pad] raw[n*C] g[32] o[32]
-__global__ void __launch_bounds__(kRaysPerBlock * 32) composite_backward_kernel(CompositeBwdArgs A) {
-    extern __shared__ __align__(16) float dyn[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n = A.n, S = A.S, C = A.C, np = A.n_pad;
-    const bool hier = (n != S);
-    float* z = dyn + (size_t)warp * A.warp_floats;
-    float* zs = z + np;
-    float* w = zs + np;
-    int* ord = reinterpret_cast<int*>(w + np);
-    float* al = w + 2 * np;
-    float* tt = al + np;
-    float* rr = tt + np;
-    float* g = rr + np;          // [32] upstream gradient per composited channel
-    float* o = g + 32;           // [32] composited value per channel (softmax backward)
-    float* raw = o + 32;
-    for (long long ray = (long long)blockIdx.x * kRaysPerBlock + warp; ray < A.n_rays;
-         ray += (long long)gridDim.x * kRaysPerBlock) {
-        const long long base = ray * S;
-        for (int i = lane; i < np; i += 32)
-            z[i] = i < n ? (hier ? (i < S ? A.z_f[base + i] : A.z_c[base + i - S]) : A.z_c[base + i]) : INFINITY;
-        {
-            const int run = S * C;
-            const float* g0 = (hier ? A.raw_f : A.raw_c) + base * C;
-            const float* g1 = A.raw_c + base * C;
-            for (int i = lane; i < run; i += 32) raw[i] = g0[i];
-            if (hier) for (int i = lane; i < run; i += 32) raw[run + i] = g1[i];
-        }
-        __syncwarp();
-        // stable rank sort (ties keep concatenation order), as composite.cu
-        for (int i = lane; i < n; i += 32) {
-            const float zi = z[i];
-            int r = 0;
-            for (int j = 0; j < n; ++j) {
-                const float zj = z[j];
-                r += (zj < zi) || (zj == zi && j < i);
-            }
-            zs[r] = zi;
-            ord[r] = i;
-        }
-        __syncwarp();
-        // alpha, t, transmittance, weights (same scan as the forward)
-        float carry = 1.f, wpart = 0.f;
-        for (int j0 = 0; j0 < n; j0 += 32) {
-            const int j = j0 + lane;
-            float alpha = 0.f, t = 1.f;
-            if (j < n) {
-                const int oi = ord[j];
-                float sig = raw[oi * C + (C - 1)];
-                if (A.noise) sig = __fadd_rn(sig, __fmul_rn(A.noise[ray * n + j], A.noise_std));
-                const float delta = (j < n - 1) ? __fsub_rn(zs[j + 1], zs[j]) : 1e10f;
-                const float act = A.clamp_mode == FENERF_CLAMP_RELU ? fmaxf(sig, 0.f) : softplus_torch(sig);
-                const float e = expf(__fmul_rn(-delta, act));
-                alpha = __fsub_rn(1.f, e);
-                t = __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f);
-                // d alpha / d sigma = delta * exp(-delta act) * act'(pre)
-                const float dact = A.clamp_mode == FENERF_CLAMP_RELU ? (sig > 0.f ? 1.f : 0.f) : 1.f / (1.f + expf(-sig));
-                rr[j] = delta * e * dact;          // reused below as d alpha / d sigma
-                al[j] = alpha;
-                tt[j] = t;
-            }
-            float p = t;
-#pragma unroll
-            for (int off = 1; off < 32; off <<= 1) {
-                const float q = __shfl_up_sync(kFull, p, off);
-                if (lane >= off) p = __fmul_rn(p, q);
-            }
-            float excl = __shfl_up_sync(kFull, p, 1);
-            if (lane == 0) excl = 1.f;
-            const float T = __fmul_rn(carry, excl);
-            if (j < n) { z[j] = T; const float wj = __fmul_rn(alpha, T); w[j] = wj; wpart += wj; }   // z[] now holds T_j
-            carry = __fmul_rn(carry, __shfl_sync(kFull, p, 31));
-        }
-        float wsum = wpart;
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) wsum += __shfl_xor_sync(kFull, wsum, off);
-        __syncwarp();
-        // upstream gradient per channel: pixels = out * 2 - 1, NCHW
-        {
-            const unsigned rpb = (unsigned)A.rays_per_batch;
-            const long long b = (unsigned)ray / rpb, p = (unsigned)ray % rpb;
-            float gv = 0.f;
-            if (lane < C - 1) gv = 2.f * A.d_pixels[(b * A.C_img + lane) * A.rays_per_batch + p];
-            if (A.softmax_label) {
-                // forward value of the composited channel (before white/black back: they do not combine with
-                // softmax in the reference's callers, but keep the order of generators.py:97-100 anyway)
-                float ov = 0.f;
-                if (lane < C - 1) {
-                    for (int j = 0; j < n; ++j) {
-                        float wj = w[j];
-                        if (A.last_back && j == n - 1) wj += 1.f - wsum;
-                        ov = fmaf(wj, raw[ord[j] * C + lane], ov);
-                    }
-                    if (A.white_back) ov = ov + 1.f - wsum;
-                    if (A.black_back) ov = ov + (1.f - wsum) * -1.f;
-                }
-                const int n_seg = C - 1 - 3;
-                float x = lane < n_seg ? ov : -INFINITY, m = x;
-                for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, off));
-                float e = lane < n_seg ? expf(x - m) : 0.f, sum = e;
-                for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(kFull, sum, off);
-                const float pr = e / sum;
-                float dot = lane < n_seg ? pr * gv : 0.f;
-                for (int off = 16; off > 0; off >>= 1) dot += __shfl_xor_sync(kFull, dot, off);
-                if (lane < n_seg) gv = pr * (gv - dot);
-            }
-            g[lane] = lane < C - 1 ? gv : 0.f;
-        }
-        __syncwarp();
-        float gsum = 0.f;
-        for (int c = 0; c < C - 1; ++c) gsum += g[c];
-        const float d_wsum = (A.white_back ? -gsum : 0.f) + (A.black_back ? gsum : 0.f);
-        // q_j = sum_c g_c v_jc ; r_j = dL/dw_j
-        float q_last = 0.f;
-        {
-            const int ol = ord[n - 1];
-            for (int c = 0; c < C - 1; ++c) q_last = fmaf(g[c], raw[ol * C + c], q_last);
-        }
-        for (int j = lane; j < n; j += 32) {
-            const int oi = ord[j];
-            float q = 0.f;
-            for (int c = 0; c < C - 1; ++c) q = fmaf(g[c], raw[oi * C + c], q);
-            float r = q + d_wsum;
-            if (A.last_back) r = (j == n - 1) ? d_wsum : (q - q_last + d_wsum);
-            zs[j] = r;                              // zs[] now holds r_j = dL/dw_j
-        }
-        __syncwarp();
-        // reverse scan U_j = r_{j+1} alpha_{j+1} + t_{j+1} U_{j+1}; dL/dalpha_j = T_j (r_j - U_j)
-        if (lane == 0) {
-            float U = 0.f;
-            for (int j = n - 1; j >= 0; --j) {
-                const float d_alpha = z[j] * (zs[j] - U);
-                U = fmaf(tt[j], U, zs[j] * al[j]);
-                rr[j] = d_alpha * rr[j];            // dL/dsigma_j
-            }
-        }
-        __syncwarp();
-        // scatter: d raw[ord[j]][c] = w'_j g_c (c < C-1), [C-1] = d sigma
-        for (int j = 0; j < n; ++j) {
-            const int oi = ord[j];
-            float wj = w[j];
-            if (A.last_back && j == n - 1) wj += 1.f - wsum;
-            float* dst = (hier ? (oi < S ? A.d_raw_f + (base + oi) * C : A.d_raw_c + (base + oi - S) * C) : A.d_raw_c + (base + oi) * C);
-            if (lane < C - 1) dst[lane] = wj * g[lane];
-            else if (lane == C - 1) dst[lane] = rr[j];
-        }
-        __syncwarp();
-    }
-}
 
 // ---- FiLM layer: forward values the backward needs --------------------------------------------------
 // thread = (point, 8 consecutive features).  z may be NULL (first layer: only the narrow inputs), xin may be
@@ -362,14 +195,8 @@ template <typename T>
 __global__ void grid_scatter_add_kernel(const float* __restrict__ points, const T* __restrict__ d_feat, int ld,
                                         long long P, float input_scale, int R, float* __restrict__ grad_cl) {
     for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < P; p += (long long)gridDim.x * blockDim.x) {
-        const float x = __fmul_rn(points[p * 3], input_scale), y = __fmul_rn(points[p * 3 + 1], input_scale),
-                    zc = __fmul_rn(points[p * 3 + 2], input_scale);
-        const float half = (float)(R - 1);
-        const float ix = (x + 1.f) * 0.5f * half, iy = (y + 1.f) * 0.5f * half, iz = (zc + 1.f) * 0.5f * half;
-        const float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
-        const float wx1 = ix - x0f, wx0 = 1.f - wx1, wy1 = iy - y0f, wy0 = 1.f - wy1, wz1 = iz - z0f, wz0 = 1.f - wz1;
-        auto clampi = [](float f) { return (int)fminf(fmaxf(f, -2.f), 1.0e6f); };
-        const int x0 = clampi(x0f), y0 = clampi(y0f), z0 = clampi(z0f);
+        const Trilinear t = trilinear(R, __fmul_rn(points[p * 3], input_scale), __fmul_rn(points[p * 3 + 1], input_scale),
+                                      __fmul_rn(points[p * 3 + 2], input_scale));
         float d[32];
 #pragma unroll
         for (int c8 = 0; c8 < 4; ++c8) {
@@ -379,12 +206,10 @@ __global__ void grid_scatter_add_kernel(const float* __restrict__ points, const 
             for (int i = 0; i < 8; ++i) d[c8 * 8 + i] = v.get(i);
         }
 #pragma unroll
-        for (int corner = 0; corner < 8; ++corner) {
-            const int dx = corner & 1, dy = (corner >> 1) & 1, dz = corner >> 2;
-            const int xx = x0 + dx, yy = y0 + dy, zz = z0 + dz;
-            if ((unsigned)xx < (unsigned)R && (unsigned)yy < (unsigned)R && (unsigned)zz < (unsigned)R) {
-                const float wgt = (dx ? wx1 : wx0) * (dy ? wy1 : wy0) * (dz ? wz1 : wz0);
-                float4* dst = reinterpret_cast<float4*>(grad_cl + (((size_t)zz * R + yy) * R + xx) * 32);
+        for (int k = 0; k < 8; ++k) {
+            if (t.inside(k)) {
+                const float wgt = t.weight(k);
+                float4* dst = reinterpret_cast<float4*>(grad_cl + t.voxel(k) * 32);
 #pragma unroll
                 for (int c4 = 0; c4 < 8; ++c4)
                     atomicAdd(dst + c4, make_float4(d[c4 * 4] * wgt, d[c4 * 4 + 1] * wgt, d[c4 * 4 + 2] * wgt, d[c4 * 4 + 3] * wgt));
@@ -418,38 +243,6 @@ int grid_blocks(long long items, int threads) {
 }
 
 }  // namespace
-
-int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
-                       const float* z_f, const float* noise, const float* d_pixels, float* d_raw_c, float* d_raw_f,
-                       cudaStream_t st) {
-    CompositeBwdArgs A;
-    A.rays_per_batch = (long long)rd->img_h * rd->img_w;
-    A.n_rays = A.rays_per_batch * rd->batch;
-    FN_REQUIRE(A.n_rays < (1ll << 31), "too many rays for one launch: %lld", A.n_rays);
-    A.S = rd->num_steps;
-    A.n = rd->hierarchical ? 2 * rd->num_steps : rd->num_steps;
-    FN_REQUIRE(A.n <= kMaxN && A.S >= 2, "num_steps %d unsupported", rd->num_steps);
-    FN_REQUIRE(C >= 2 && C <= 32, "out_dim %d unsupported", C);
-    FN_REQUIRE(rd->fill_mode == FENERF_FILL_NONE, "fill modes belong to staged_forward (no_grad)");
-    A.C = C; A.C_img = C - 1;
-    A.clamp_mode = rd->clamp_mode; A.last_back = rd->last_back; A.white_back = rd->white_back;
-    A.black_back = rd->black_back; A.softmax_label = rd->softmax_label; A.noise_std = rd->noise_std;
-    A.raw_c = raw_c; A.z_c = z_c; A.raw_f = raw_f; A.z_f = z_f; A.noise = noise; A.d_pixels = d_pixels;
-    A.d_raw_c = d_raw_c; A.d_raw_f = d_raw_f;
-    if (rd->hierarchical) FN_REQUIRE(raw_f && z_f && d_raw_f, "hierarchical render needs the fine tensors");
-    A.n_pad = (A.n + 3) & ~3;
-    A.warp_floats = (7 * A.n_pad + 64 + A.n * C + 3) & ~3;
-    const size_t smem = (size_t)kRaysPerBlock * A.warp_floats * sizeof(float);
-    static std::atomic<int> smem_set[kMaxDevices];
-    if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(composite_backward_kernel, smem_set, (int)smem));
-    long long groups = (A.n_rays + kRaysPerBlock - 1) / kRaysPerBlock;
-    int per_sm = (int)(200 * 1024 / (smem + 1024));
-    per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
-    int blocks = (int)(groups < (long long)num_sms() * per_sm ? groups : (long long)num_sms() * per_sm);
-    composite_backward_kernel<<<blocks < 1 ? 1 : blocks, kRaysPerBlock * 32, smem, st>>>(A);
-    FN_LAUNCH_OK("composite_backward_kernel");
-    return 0;
-}
 
 int film_forward_stash(const float* z, const float* bias, const float* film_layer, long long film_batch_stride, long long P,
                        long long ppb, const float* xin, int kx, const float* wx, void* a_out, void* gate_out, int f32,

@@ -78,6 +78,28 @@ inline cudaError_t ensure_dynamic_smem(F kernel, std::atomic<int>* state /*[kMax
     return e;
 }
 
+// ---- the per-sample terms of fancy_integration (volumetric_rendering.py:18-38): compositors and resampler ----
+// Rounded op by op as the reference: the build contracts a * b + c into an FMA, so these spell out every rounding.
+constexpr float kFarDelta = 1e10f;      // the interval behind the far sample (volumetric_rendering.py:24)
+
+// F.softplus(beta=1, threshold=20)
+__device__ __forceinline__ float softplus_torch(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+
+// the density activation: relu or softplus of sigma (+ noise)
+__device__ __forceinline__ float density_act(float sigma, int clamp_mode) {
+    return clamp_mode == FENERF_CLAMP_RELU ? fmaxf(sigma, 0.f) : softplus_torch(sigma);
+}
+
+// alpha = 1 - exp(-delta act); `decay` (if given) receives exp(-delta act)
+__device__ __forceinline__ float sample_alpha(float delta, float act, float* decay = nullptr) {
+    const float e = expf(__fmul_rn(-delta, act));
+    if (decay) *decay = e;
+    return __fsub_rn(1.f, e);
+}
+
+// the factor 1 - alpha + 1e-10 of the transmittance product (torch.cumprod)
+__device__ __forceinline__ float transmittance_term(float alpha) { return __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f); }
+
 // ---- entry points of the individual translation units (called by abi.cu) ----
 int pack_field(const fenerf_field_desc* f, const FnLayout& L, const fenerf_field_params* p, void* packed,
                cudaStream_t st);
@@ -106,6 +128,9 @@ int composite_sorted(const fenerf_render_desc* rd, int C, const float* raw_c, co
 int composite(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
               const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
               int32_t* sort_idx, cudaStream_t st);
+int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
+                       const float* z_f, const float* noise, const float* d_pixels, float* d_raw_c, float* d_raw_f,
+                       cudaStream_t st);
 
 // gemm.cu
 int gemm_nt(const void* A, const void* B, long long M, float* c32, void* c16, void* a_out, void* gate_out, const float* bias,
@@ -121,9 +146,6 @@ int mapping_film(const float* const* w, const float* const* b, const float* z, i
 int mask2color(const float* masks, int B, int K, long long HW, float* out, cudaStream_t st);
 int frames_to_u8(const float* frames, int B, int C, int c0, int nc, long long HW, unsigned char* out, cudaStream_t st);
 // backward.cu
-int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
-                       const float* z_f, const float* noise, const float* d_pixels, float* d_raw_c, float* d_raw_f,
-                       cudaStream_t st);
 int film_forward_stash(const float* z, const float* bias, const float* film_layer, long long film_batch_stride, long long P,
                        long long ppb, const float* xin, int kx, const float* wx, void* a_out, void* gate_out, int f32,
                        cudaStream_t st);

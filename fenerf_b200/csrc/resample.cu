@@ -20,11 +20,6 @@ namespace {
 
 constexpr int kMaxS = 64;
 
-__device__ __forceinline__ float softplus_torch(float x) {
-    // F.softplus(beta=1, threshold=20)
-    return x > 20.f ? x : log1pf(expf(x));
-}
-
 // ONE THREAD PER RAY: every product and sum runs in the reference's left-to-right order (torch.cumprod, torch.cumsum;
 // the pdf normaliser is a sequential sum -- torch.sum's vectorised order is host-ISA dependent and is not
 // reproduced), the running transmittance / CDF live in registers and three small local arrays.  (Round 1 ran the same
@@ -71,14 +66,13 @@ resample_ray_kernel(long long n_rays, long long rays_per_batch, int S, int C, in
                 float sig = sigma_compact ? cdf(s) : raw[(base + s) * C + (C - 1)];      // (slot s is overwritten only by s-1)
                 if (noise) sig = __fadd_rn(sig, __fmul_rn(noise[base + s], noise_std));
                 const float delta = __fsub_rn(z(s + 1), z(s));
-                const float act = clamp_mode == FENERF_CLAMP_RELU ? fmaxf(sig, 0.f) : softplus_torch(sig);
-                const float alpha = __fsub_rn(1.f, expf(__fmul_rn(-delta, act)));
+                const float alpha = sample_alpha(delta, density_act(sig, clamp_mode));
                 if (s >= 1) {
                     const float wj = __fadd_rn(__fadd_rn(__fmul_rn(alpha, T), 1e-5f), 1e-5f);
                     cdf(s - 1) = wj;                       // weights for now
                     total = __fadd_rn(total, wj);
                 }
-                T = __fmul_rn(T, __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f));
+                T = __fmul_rn(T, transmittance_term(alpha));
             }
             // pdf -> cdf in place: cdf(0) = 0, cdf(i) = cdf(i-1) + pdf(i-1)   (S-1 entries)
             {

@@ -17,7 +17,8 @@
 //   Wbuf [2][16][256]   double-buffered 16-row slabs of the k-major weights via cp.async
 //   each thread owns a 4-point x 16-column micro tile; 5 LDS.128 feed 64 FFMA per k
 //   (the 16-point gather variant maps lanes point-major so a warp's weight reads broadcast)
-#include "common.cuh"
+#include "siren_common.cuh"
+#include "sm90.cuh"
 
 namespace fn {
 
@@ -61,20 +62,12 @@ struct Smem {
     int bidx[TM];
 };
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-    unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-
 __device__ __forceinline__ void load_slab(float (*dst)[FN_H], const float* src, int tid) {
     // 16 rows x 256 floats = 1024 float4, 4 per thread, fully coalesced
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         int q = tid + i * NTHREADS;
-        cp_async16(&dst[0][0] + q * 4, src + q * 4);
+        sm90::cp_async16(sm90::smem_u32(&dst[0][0] + q * 4), src + q * 4);
     }
 }
 
@@ -87,13 +80,13 @@ __device__ __forceinline__ void gemm_tile(Smem<P>& s, const float* __restrict__ 
 #pragma unroll
     for (int st = 0; st < NS - 1; ++st) {
         if (st < nslab) load_slab(s.W[st], wt + (size_t)st * KC * FN_H, tid);
-        cp_async_commit();
+        sm90::cp_async_commit();
     }
     for (int c = 0; c < nslab; ++c) {
-        cp_async_wait<NS - 2>();       // slab c has landed (one group per slab, NS-1 in flight)
-        __syncthreads();               // ... for every thread, and slab c-1's buffer is free again
+        sm90::cp_async_wait<NS - 2>();       // slab c has landed (one group per slab, NS-1 in flight)
+        __syncthreads();                     // ... for every thread, and slab c-1's buffer is free again
         if (c + NS - 1 < nslab) load_slab(s.W[(c + NS - 1) % NS], wt + (size_t)(c + NS - 1) * KC * FN_H, tid);
-        cp_async_commit();
+        sm90::cp_async_commit();
         const float(*W)[FN_H] = s.W[c % NS];
 #pragma unroll
         for (int kk = 0; kk < KC; ++kk) {
@@ -116,7 +109,7 @@ __device__ __forceinline__ void gemm_tile(Smem<P>& s, const float* __restrict__ 
             }
         }
     }
-    cp_async_wait<0>();
+    sm90::cp_async_wait<0>();
     __syncthreads();                   // all reads of A and W done before the caller overwrites A
 }
 
@@ -156,35 +149,13 @@ __device__ __forceinline__ void init_bias(const float* __restrict__ bias, float 
         }
 }
 
-// trilinear lookup, align_corners=True, zero padding; x -> W (innermost), y -> H, z -> D
-// (siren/siren.py:314-330; corner order and weight products as ATen's grid_sampler_3d)
+// channel ch of the channels-last feature grid at one position
 __device__ __forceinline__ float grid_feature(const float* __restrict__ grid, int R, int G, float x, float y, float z, int ch) {
-    const float half = (float)(R - 1);
-    float ix = __fmul_rn(__fdiv_rn(__fadd_rn(x, 1.f), 2.f), half);
-    float iy = __fmul_rn(__fdiv_rn(__fadd_rn(y, 1.f), 2.f), half);
-    float iz = __fmul_rn(__fdiv_rn(__fadd_rn(z, 1.f), 2.f), half);
-    float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
-    float x1f = x0f + 1.f, y1f = y0f + 1.f, z1f = z0f + 1.f;
-    float wx0 = __fsub_rn(x1f, ix), wx1 = __fsub_rn(ix, x0f);
-    float wy0 = __fsub_rn(y1f, iy), wy1 = __fsub_rn(iy, y0f);
-    float wz0 = __fsub_rn(z1f, iz), wz1 = __fsub_rn(iz, z0f);
-    // guard the float->int conversion against wild coordinates
-    auto clampi = [](float f) { return (int)fminf(fmaxf(f, -2.f), 1.0e6f); };
-    int x0 = clampi(x0f), y0 = clampi(y0f), z0 = clampi(z0f);
-    int x1 = x0 + 1, y1 = y0 + 1, z1 = z0 + 1;
+    const Trilinear t = trilinear(R, x, y, z);
     float out = 0.f;
-    auto tap = [&](int zz, int yy, int xx, float w) {
-        if ((unsigned)xx < (unsigned)R && (unsigned)yy < (unsigned)R && (unsigned)zz < (unsigned)R)
-            out = __fadd_rn(out, __fmul_rn(__ldg(grid + (((size_t)zz * R + yy) * R + xx) * G + ch), w));
-    };
-    tap(z0, y0, x0, __fmul_rn(__fmul_rn(wx0, wy0), wz0));
-    tap(z0, y0, x1, __fmul_rn(__fmul_rn(wx1, wy0), wz0));
-    tap(z0, y1, x0, __fmul_rn(__fmul_rn(wx0, wy1), wz0));
-    tap(z0, y1, x1, __fmul_rn(__fmul_rn(wx1, wy1), wz0));
-    tap(z1, y0, x0, __fmul_rn(__fmul_rn(wx0, wy0), wz1));
-    tap(z1, y0, x1, __fmul_rn(__fmul_rn(wx1, wy0), wz1));
-    tap(z1, y1, x0, __fmul_rn(__fmul_rn(wx0, wy1), wz1));
-    tap(z1, y1, x1, __fmul_rn(__fmul_rn(wx1, wy1), wz1));
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+        if (t.inside(k)) out = __fadd_rn(out, __fmul_rn(__ldg(grid + t.voxel(k) * G + ch), t.weight(k)));
     return out;
 }
 

@@ -224,15 +224,20 @@ def resample(rd, raw_coarse, z_vals, dirs, origins, rng_noise, rng_u, want_inds=
     return z_fine, pts, inds
 
 
+def _image_channels(rd, c):
+    """Channels of the rendered image for a field of c outputs: the c - 1 colour / label channels, plus the
+    background channel the seg-padding fill modes add."""
+    pad = rd.fill_mode in (_lib.FILL_MODE["seg_padding_background"], _lib.FILL_MODE["eval_seg_padding_background"])
+    return c - 1 + (1 if pad else 0)
+
+
 def composite(rd, raw_coarse, z_coarse, raw_fine=None, z_fine=None, rng_noise=None, want_weights=False,
               want_sort_idx=False):
     device = raw_coarse.device
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
     c = raw_coarse.shape[-1]
     ns = 2 * s if rd.hierarchical else s
-    pad = rd.fill_mode in (_lib.FILL_MODE["seg_padding_background"], _lib.FILL_MODE["eval_seg_padding_background"])
-    c_img = c - 1 + (1 if pad else 0)
-    pixels = torch.empty((b, c_img, rd.img_h, rd.img_w), dtype=torch.float32, device=device)
+    pixels = torch.empty((b, _image_channels(rd, c), rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     depth = torch.empty((b, n, 1), dtype=torch.float32, device=device)
     wsum = torch.empty((b, n, 1), dtype=torch.float32, device=device)
     weights = torch.empty((b, n, ns, 1), dtype=torch.float32, device=device) if want_weights else None
@@ -284,12 +289,10 @@ def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
     ns = 2 * s if rd.hierarchical else s
     c = packed.desc.out_dim
-    pad = rd.fill_mode in (_lib.FILL_MODE["seg_padding_background"], _lib.FILL_MODE["eval_seg_padding_background"])
-    c_img = c - 1 + (1 if pad else 0)
     film = _prep(film, device)
     if film.shape != (b, packed.desc.trunk_layers + packed.desc.color_layers, 2, _lib.HIDDEN):
         raise ValueError("film table has shape %s" % (tuple(film.shape),))
-    pixels = torch.empty((b, c_img, rd.img_h, rd.img_w), dtype=torch.float32, device=device)
+    pixels = torch.empty((b, _image_channels(rd, c), rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     depth = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_depth else None
     wsum = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_weights_sum else None
     weights = torch.empty((b, n, ns, 1), dtype=torch.float32, device=device) if want_weights else None

@@ -11,7 +11,8 @@ restatement computed from the kernel's OWN fp32 inputs, read from that workspace
   (c) the GUARD refinement: which far samples are re-evaluated, their values, and fenerf_guard_stats, with 16-point
       tiles (probes only) and 32-point tiles (every ray);
   (d) composite_ray_kernel<CMAX, TPR>: pixels, depth, weights_sum and per-sample weights, every compositing and fill
-      option; and the stand-alone warp-per-ray composite_kernel on inputs with exact depth ties.
+      option; the stand-alone fenerf_composite on the render's own inputs (bit for bit: one computation), and on
+      unsorted inputs with exact depth ties.
 
 The 'loop' render holds more rays than one pass of the resampler, the compositor and the guard scan covers on the
 device it runs on, so every grid-stride loop takes a second pass.  The 'straddle' render has 200² rays per image, not a
@@ -47,7 +48,7 @@ RAY_BOUND = 1e-6
 #: within 0.15 of the first term of cdf64's edge.  The faults exceed the bound >= 3.8e4-fold.
 CDF_A, CDF_B = 1.0, 1.0
 #: compositor, max |kernel - fp64| over pixels, depth, weights_sum and weights.  Measured: 3.2e-6 (flat63-A's pixels),
-#: 2.5e-6 for the stand-alone kernel (n = 128, C = 4).  The faults move it by >= 7.8e-2.
+#: 2.8e-6 for the stand-alone entry on unsorted inputs (n = 128, C = 4).  The faults move it by >= 7.8e-2.
 COMPOSITE_FWD_BOUND = 1e-5
 #: fill modes switch at weights_sum = 0.9: rays with |weights_sum fp64 - 0.9| < FILL_TIE are not compared, and at most
 #: FILL_TIE_FRACTION of the rays may be such rays
@@ -338,6 +339,12 @@ def check_composite(x):
     print("%s composite: %s, %d rays skipped" % (x["name"], errs, skipped))
     assert skipped <= FILL_TIE_FRACTION * x["b"] * x["n"], "%d rays within %g of weights_sum = 0.9" % (skipped, FILL_TIE)
     assert max(errs.values()) <= COMPOSITE_FWD_BOUND, errs
+    # the public entry on the render's own inputs (raw_c after GUARD, draw #6) is the render's computation, bit for bit
+    px, depth, wsum, w, _ = ops.composite(x["rd"], x["raw_c"], x["z_c"], x["raw_f"], x["z_f"],
+                                          x["noise_f"] if o["noise"] else None, want_weights=True)
+    for name, got, want in (("pixels", px, x["pixels"]), ("depth", depth[..., 0], x["depth"]),
+                            ("weights_sum", wsum[..., 0], x["wsum"]), ("weights", w[..., 0], x["weights"])):
+        assert torch.equal(got, want), "fenerf_composite's %s differ from fenerf_render_forward's" % name
     return dict(errs, skipped=skipped)
 
 
@@ -386,8 +393,9 @@ _STANDALONE_FILLS = {"seg_padding_grey_softmax": _opt(fill_mode="seg_padding_bac
 @pytest.mark.parametrize("c", [4, 22, 32])
 @pytest.mark.parametrize("n", [33, 64, 96, 128])
 def test_standalone_composite_vs_fp64(n, c, fill):
-    """fenerf_composite (warp-per-ray, the public entry) on the backward test's inputs (exact depth ties between fine
-    and coarse samples): the merge order is the stable fine-first one, the outputs are within the compositor's bound."""
+    """fenerf_composite (the public entry: samples in any order) on the backward test's inputs (exact depth ties between
+    fine and coarse samples): the merge order is the stable fine-first one, the outputs are within the compositor's
+    bound."""
     hier = n > 64
     steps = n // 2 if hier else n
     xi = _composite_inputs(c, steps, hier, False)
