@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("FENERF_B200_LIB") or os.path.join(_HERE, "libfenerf_b
 MAX_TRUNK, MAX_COLOR, MAX_LABEL, HIDDEN = 8, 8, 32, 256
 
 ABI_VERSION = 3
+FIELD_LABEL_FILM = 0x1        # fenerf_field_desc.reserved (the flags word): FENERF_FIELD_LABEL_FILM
 PRECISION = {"exact": 0, "fast": 1, "guard": 2}
 CLAMP = {"relu": 0, "softplus": 1}
 FILL_MODE = {None: 0, "debug": 1, "weight": 2, "weight_debug": 3, "seg_padding_background": 4,

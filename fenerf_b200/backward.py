@@ -17,7 +17,9 @@ backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per
                         (``fenerf_gemm_nt_f16``) and the per-image dW_b = dZ^T a (``fenerf_gemm_tn_f16``, split-K)
           FiLM gradients need no further pass over the points:  dp = db_b / f,
           df = (sum_k W[f,k] dW_b[f,k]) / f + b dp   (u = f z + p, z = W a + b).
-          Heads, the pre-multiplied label chain and the grid (``fenerf_grid_scatter_add``) close the chain.
+          Heads, the pre-multiplied label chain and the grid (``fenerf_grid_scatter_add``) close the chain.  A label FiLM
+          field (SPATIALSIRENSEMANTIC) recomputes its label layer from the trunk output at FiLM row T and runs it
+          backward like a colour layer, its dZ W joining the trunk's dA.
 Gradients flow to the FiLM table (and through torch's autograd into the mapping network / latents /
 frequency offsets) and to every field parameter.  The fp16 gradient stream is scaled by a power of two
 taken from max|d raw| on the device (no host sync) and unscaled at the end.
@@ -80,11 +82,17 @@ class FieldWeights:
         self.labels = []
         if spec.label_dim:
             self.labels = [(m.weight, m.bias) for m in module.label_layer_linear if isinstance(m, torch.nn.Linear)]
+        # the label FiLM layer (FiLM row len(trunk)); self.labels is then its one-Linear head
+        self.label_film = [(module.label_layer_sine.layer.weight, module.label_layer_sine.layer.bias)] if spec.label_film else []
         self.grid = module.spatial_embeddings if spec.grid_channels else None
+
+    def film_layers(self):
+        """(weight, bias) of every FiLM layer in FiLM-table row order: trunk, label FiLM layer, colour."""
+        return self.trunk + self.label_film + self.color
 
     def parameters(self):
         ps = []
-        for w, b in self.trunk + self.color + [self.sigma, self.rgb] + self.labels:
+        for w, b in self.film_layers() + [self.sigma, self.rgb] + self.labels:
             ps += [w, b]
         if self.grid is not None:
             ps.append(self.grid)
@@ -137,7 +145,8 @@ class _FieldBackward:
         self.dev = dev
         B = self.film.shape[0]
         T, Cn = len(self.fw.trunk), len(self.fw.color)
-        self.T, self.Cn, self.n_film = T, Cn, T + Cn
+        self.lf = len(self.fw.label_film)                          # 1: a label FiLM layer at row T, colour from T + 1
+        self.T, self.Cn, self.c0, self.n_film = T, Cn, T + self.lf, T + self.lf + Cn
         G = self.spec.grid_channels
         self.kx = 3 + G
         self.kx_pad = (self.kx + 7) // 8 * 8
@@ -168,13 +177,17 @@ class _FieldBackward:
         # dA' = dZ W on the wgmma NT kernel wants the transposed weights as its (N, K) operand
         self.WhT16 = [None] + [w.t().contiguous() for w in self.Wh16[1:]] if self.own_gemm else None
         self.WcT16 = [w.t().contiguous() for w in self.Wc16] if self.own_gemm else None
+        if self.lf:
+            self.Wl16 = fw.label_film[0][0].detach().to(self.dt).contiguous()
+            self.WlT16 = self.Wl16.t().contiguous() if self.own_gemm else None
+            self.Wlhead32 = fw.labels[0][0].detach().float().contiguous()                 # (L, 256)
         if self.own_gemm:
             self.Wn64 = torch.zeros((256, 64), dtype=torch.float16, device=dev)
             self.Wn64[:, :self.kx] = self.Wc0x_narrow
         L = self.spec.label_dim
         self.L = L
         heads = torch.zeros((32, 256), dtype=torch.float32, device=dev)
-        if L:
+        if L and not self.lf:      # (a label FiLM field's head acts on the label layer: its rows stay zero here)
             weff, _ = _label_eff(fw.labels)
             heads[:L] = weff
         heads[L] = fw.sigma[0].detach().float().reshape(-1)
@@ -182,7 +195,7 @@ class _FieldBackward:
         rgbw = torch.zeros((8, 256), dtype=self.dt, device=dev)
         rgbw[:3] = fw.rgb[0].detach().to(self.dt)
         self.Wrgb16 = rgbw
-        self.bias = [b.detach().float().contiguous() for _, b in fw.trunk + fw.color]
+        self.bias = [b.detach().float().contiguous() for _, b in fw.film_layers()]
 
     # ---- one point set: points (B, ppb, 3), dirs (B, ppb/dir_group, 3), raw / d_raw (B, ppb, C) ----
     def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
@@ -221,7 +234,7 @@ class _FieldBackward:
         dev, spec = self.dev, self.spec
         k, ppb = points.shape[0], points.shape[1]
         P = k * ppb
-        T, Cn = self.T, self.Cn
+        T, Cn, c0 = self.T, self.Cn, self.c0
         points = points.contiguous()
         dirs = dirs.contiguous()
         raw = raw.contiguous()
@@ -241,19 +254,25 @@ class _FieldBackward:
                     A[l], Gt[l] = ops.gemm_nt_film(A[l - 1], self.Wh16[l], self.bias[l], self.film, b0, l, ppb)
                 else:
                     A[l], Gt[l] = self._stash(_mm32(A[l - 1], self.Wh16[l].t()), l, b0, P, ppb)
+            if self.lf:     # the label FiLM layer, on the trunk output
+                if own:
+                    A[T], Gt[T] = ops.gemm_nt_film(A[T - 1], self.Wl16, self.bias[T], self.film, b0, T, ppb)
+                else:
+                    A[T], Gt[T] = self._stash(_mm32(A[T - 1], self.Wl16.t()), T, b0, P, ppb)
             if own:     # the narrow inputs [dir, grid features] ride as a fifth 64-wide k-chunk of the same kernel
                 e64 = torch.zeros((P, 64), dtype=torch.float16, device=dev)
                 e64[:, :self.kx] = extras
-                A[T], Gt[T] = ops.gemm_nt_film(A[T - 1], self.Wc16[0], self.bias[T], self.film, b0, T, ppb, narrow_in=e64,
-                                               narrow_w=self.Wn64)
+                A[c0], Gt[c0] = ops.gemm_nt_film(A[T - 1], self.Wc16[0], self.bias[c0], self.film, b0, c0, ppb, narrow_in=e64,
+                                                 narrow_w=self.Wn64)
                 del e64
             else:
-                A[T], Gt[T] = self._stash(_mm32(A[T - 1], self.Wc16[0].t()), T, b0, P, ppb, xin=extras, wx=self.Wc0x_narrow)
+                A[c0], Gt[c0] = self._stash(_mm32(A[T - 1], self.Wc16[0].t()), c0, b0, P, ppb, xin=extras, wx=self.Wc0x_narrow)
             for j in range(1, Cn):
                 if own:
-                    A[T + j], Gt[T + j] = ops.gemm_nt_film(A[T + j - 1], self.Wc16[j], self.bias[T + j], self.film, b0, T + j, ppb)
+                    A[c0 + j], Gt[c0 + j] = ops.gemm_nt_film(A[c0 + j - 1], self.Wc16[j], self.bias[c0 + j], self.film, b0, c0 + j,
+                                                             ppb)
                 else:
-                    A[T + j], Gt[T + j] = self._stash(_mm32(A[T + j - 1], self.Wc16[j].t()), T + j, b0, P, ppb)
+                    A[c0 + j], Gt[c0 + j] = self._stash(_mm32(A[c0 + j - 1], self.Wc16[j].t()), c0 + j, b0, P, ppb)
             # ---- head gradients ----
             dH = torch.empty((P, 32), dtype=self.dt, device=dev)
             dRGB = torch.empty((P, 8), dtype=self.dt, device=dev)
@@ -262,14 +281,19 @@ class _FieldBackward:
             a_last = A[self.n_film - 1]
             self.d_rgb_w += _mm32(dRGB.t(), a_last)
             self.d_rgb_b += dRGB.float().sum(0)
-            self.d_heads_w += _mm32(dH.t(), A[T - 1])
+            if self.lf:     # label rows on the label layer's activations, the sigma row on the trunk's
+                L = self.L
+                self.d_heads_w[:L] += _mm32(dH[:, :L].t(), A[T])
+                self.d_heads_w[L:] += _mm32(dH[:, L:].t(), A[T - 1])
+            else:
+                self.d_heads_w += _mm32(dH.t(), A[T - 1])
             self.d_heads_b += dH.float().sum(0)
             # ---- colour branch, top down ----
             dA = torch.mm(dRGB, self.Wrgb16)                                   # (P, 256) fp16
             for j in range(Cn - 1, -1, -1):
-                idx = T + j
+                idx = c0 + j
                 self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dZ now
-                a_in = A[idx - 1]
+                a_in = A[idx - 1] if j else A[T - 1]
                 dz3 = dA.view(k, ppb, 256).transpose(1, 2)
                 self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(dz3, a_in.view(k, ppb, 256))
                 if j == 0:
@@ -284,6 +308,17 @@ class _FieldBackward:
                 A[idx], Gt[idx] = None, None
             # ---- trunk: colour-branch gradient + sigma / label heads ----
             dA += torch.mm(dH.float(), self.Wheads32)
+            if self.lf:     # label branch: d logits W_head -> gate -> dW, colsum of row T; dZ W_label joins the trunk's dA
+                # (P, 256), formed in fp32: an fp16 product's reduction order depends on the chunk's row count
+                dAl = torch.mm(dH[:, :self.L].float(), self.Wlhead32).to(self.dt)
+                self._gate(dAl, Gt[T], T, b0, b1, P, ppb)
+                if own:
+                    self.dW_b[T][b0:b1] += ops.gemm_tn(dAl, A[T - 1], k, ppb)
+                    dA += ops.gemm_nt(dAl, self.WlT16, torch.float16)
+                else:
+                    self.dW_b[T][b0:b1] += _bmm32(dAl.view(k, ppb, 256).transpose(1, 2), A[T - 1].view(k, ppb, 256))
+                    dA += torch.mm(dAl, self.Wl16)
+                A[T], Gt[T] = None, None
             for l in range(T - 1, 0, -1):
                 self._gate(dA, Gt[l], l, b0, b1, P, ppb)
                 if own:
@@ -304,7 +339,7 @@ class _FieldBackward:
         film = self.film
         d_film = torch.zeros_like(film)
         grads = {}
-        layers = fw.trunk + fw.color
+        layers = fw.film_layers()
         for idx, (w, b) in enumerate(layers):
             f = film[:, idx, 0]                                             # (B, 256)
             db_b = self.colsum[:, idx]
@@ -313,7 +348,7 @@ class _FieldBackward:
             if idx == 0:
                 dwb = self.dW_b[0][:, :, :3]
                 full = dwb
-            elif idx == self.T:
+            elif idx == self.c0:
                 full = torch.cat([self.dWx_b[:, :, :self.kx], self.dW_b[idx]], dim=2)   # column order of the reference: [dir, feat, x]
             else:
                 full = self.dW_b[idx]
@@ -327,7 +362,11 @@ class _FieldBackward:
         grads[id(fw.sigma[1])] = (self.d_heads_b[L] * inv).reshape(fw.sigma[1].shape)
         grads[id(fw.rgb[0])] = self.d_rgb_w[:3] * inv
         grads[id(fw.rgb[1])] = self.d_rgb_b[:3] * inv
-        if L:
+        if self.lf:
+            (hw, hb), = fw.labels
+            grads[id(hw)] = self.d_heads_w[:L] * inv
+            grads[id(hb)] = self.d_heads_b[:L] * inv
+        elif L:
             chain = _label_chain_grads(fw.labels, self.d_heads_w[:L] * inv, self.d_heads_b[:L] * inv)
             for (w, b), (gw, gb) in zip(fw.labels, chain):
                 grads[id(w)] = gw.float()

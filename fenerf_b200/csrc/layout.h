@@ -22,6 +22,15 @@
 //   grid16           the same in f16 (wgmma path: 64 B per voxel -- the features become fp16 MMA operands anyway;
 //                    57 MB for 32 x 96^3: half the gather stream of the fp32 copy)
 //
+// Label FiLM fields (FENERF_FIELD_LABEL_FILM): hidden layer trunk_hidden is the label FiLM layer, packed like any
+// hidden layer, and the colour layers follow it -- so hidden layer l still takes FiLM row l + 1, and the rows are the
+// reference's (trunk, label, colour).  The label head needs no pre-multiplication: `label_w` holds its fp32 copy in the
+// Weff / beff format (1/scale = 1), the trunk-head image carries sigma only (row label_dim, rows below zero), and the
+// label head gets an image of its own, appended after grid16 so that every other section keeps its offset:
+//   label_img        [4 chunks][32 rows][64 k] f16 swizzled: rows 0..L-1 the label head, rest zero
+// These fields live in FnLabelFilm, not in FnLayout, so that the kernels' argument blocks of the other fields keep
+// their layout.
+//
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
 // matched on the B side by (W_hi, W_hi, W_lo) so that hi*hi + lo*hi + hi*lo reproduces an
@@ -32,7 +41,7 @@
 #include "../../include/fenerf_b200.h"
 
 #define FN_H 256            // hidden width
-#define FN_MAX_HIDDEN 15    // (8-1) trunk + 8 colour
+#define FN_MAX_HIDDEN 15    // (8-1) trunk + 8 colour; a label FiLM field: (8-1) trunk + 1 label + at most 7 colour
 #define FN_KCHUNK 64        // k elements per 128-byte swizzle row
 #define FN_IMG_BYTES (256 * FN_KCHUNK * 2)   // one [256][64] f16 image = 32 KB
 #define FN_SLOT_POS 0
@@ -55,11 +64,22 @@ struct FnLayout {
     size_t total;
 };
 
+// The label FiLM branch of a FENERF_FIELD_LABEL_FILM field (all zero for other fields).
+struct FnLabelFilm {
+    int32_t on;             // 1: hidden layer `layer` is the label FiLM layer, the colour layers start at layer + 1
+    int32_t layer;          // = trunk_hidden
+    size_t img;             // label-head image (see above)
+};
+
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Returns 0 and fills `L`, or -1 if the description is outside what the kernels support.
-static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
+// Returns 0 and fills `L` (and `lf` if given), -2 if the flags hold an unknown bit, or -1 if the description is
+// outside what the kernels support.
+static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabelFilm* lf = nullptr) {
     if (!f || !L) return -1;
+    if (f->reserved & ~FENERF_FIELD_LABEL_FILM) return -2;
+    const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
+    if (label_film && (f->label_dim < 1 || f->color_layers + 1 > FN_MAX_HIDDEN - (FENERF_MAX_TRUNK - 1))) return -1;
     if (f->trunk_layers < 2 || f->trunk_layers > FENERF_MAX_TRUNK) return -1;
     if (f->color_layers < 1 || f->color_layers > FENERF_MAX_COLOR) return -1;
     if (f->label_dim < 0 || f->label_dim > FENERF_MAX_LABEL) return -1;
@@ -67,8 +87,8 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     if (f->grid_channels && (f->grid_res < 2 || f->grid_res > 512)) return -1;
     if (f->out_dim != f->label_dim + 4) return -1;
     L->trunk_hidden = f->trunk_layers - 1;
-    L->n_hidden = L->trunk_hidden + f->color_layers;
-    L->n_film = f->trunk_layers + f->color_layers;
+    L->n_hidden = L->trunk_hidden + label_film + f->color_layers;
+    L->n_film = f->trunk_layers + label_film + f->color_layers;
     L->kx = 3 + f->grid_channels;
     L->kx_pad = (L->kx + 15) / 16 * 16;
     L->label_dim = f->label_dim;
@@ -83,7 +103,7 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     L->first_img = take(FN_IMG_BYTES);
     for (int l = 0; l < FN_MAX_HIDDEN; ++l) { L->hid_w32[l] = L->hid_b[l] = L->hid_img[l] = 0; }
     for (int l = 0; l < L->n_hidden; ++l) {
-        int k = FN_H + (l == L->trunk_hidden ? L->kx_pad : 0);
+        int k = FN_H + (l == L->trunk_hidden + label_film ? L->kx_pad : 0);   // the first colour layer's extra rows
         L->hid_w32[l] = take((size_t)k * FN_H * 4);
         L->hid_b[l] = take(FN_H * 4);
         L->hid_img[l] = take((size_t)(FN_H / FN_KCHUNK) * FN_IMG_BYTES);
@@ -98,6 +118,9 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     size_t r = (size_t)f->grid_res;
     L->grid = take(f->grid_channels ? r * r * r * (size_t)f->grid_channels * 4 : 4);
     L->grid16 = take(f->grid_channels ? r * r * r * (size_t)f->grid_channels * 2 : 4);
+    FnLabelFilm lab = {label_film, label_film ? L->trunk_hidden : 0, 0};
+    if (label_film) lab.img = take((size_t)(FN_H / FN_KCHUNK) * 32 * FN_KCHUNK * 2);
+    if (lf) *lf = lab;
     L->total = off;
     return 0;
 }

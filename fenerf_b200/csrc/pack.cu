@@ -139,17 +139,33 @@ __global__ void label_step3_kernel(float* __restrict__ lw, int L) {
     if (threadIdx.x == 0) lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] = 1.f / scale;
 }
 
+// label head of a label FiLM field (one block): the fp32 copy in the Weff / beff format (1/scale = 1) and the
+// label-head image [4][32 rows][64 k], rows 0..L-1
+__global__ void pack_label_film_head_kernel(const float* __restrict__ w, const float* __restrict__ b, int L,
+                                            float* __restrict__ lw, unsigned char* __restrict__ img) {
+    for (int i = threadIdx.x; i < 32 * FN_H; i += blockDim.x) {
+        int row = i / FN_H, k = i % FN_H;
+        const float v = row < L ? w[row * FN_H + k] : 0.f;
+        lw[row * FN_H + k] = v;
+        unsigned char* chunk = img + (size_t)(k / FN_KCHUNK) * (32 * FN_KCHUNK * 2);
+        *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
+    }
+    if (threadIdx.x < FENERF_MAX_LABEL) lw[FENERF_MAX_LABEL * FN_H + threadIdx.x] = (int)threadIdx.x < L ? b[threadIdx.x] : 0.f;
+    if (threadIdx.x == 0) lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] = 1.f;
+}
+
 // head images for the wgmma kernel (one block):
-//   trunk head  [4][32 rows][64 k]: rows 0..L-1 = Weff * scale, row L = sigma weights
+//   trunk head  [4][32 rows][64 k]: rows 0..label_rows-1 = Weff * scale, row L = sigma weights
+//               (label_rows = L, or 0 for a label FiLM field, whose label head has an image of its own)
 //   rgb head    [4][ 8 rows][64 k]: rows 0..2
-__global__ void pack_head_imgs_kernel(const float* __restrict__ lw, int L, const float* __restrict__ sigma_w,
+__global__ void pack_head_imgs_kernel(const float* __restrict__ lw, int L, int label_rows, const float* __restrict__ sigma_w,
                                       const float* __restrict__ rgb_w, unsigned char* __restrict__ head_img,
                                       unsigned char* __restrict__ rgb_img) {
     const float scale = L > 0 ? 1.f / lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] : 1.f;
     for (int i = threadIdx.x; i < 32 * FN_H; i += blockDim.x) {
         int row = i / FN_H, k = i % FN_H;
         float v = 0.f;
-        if (row < L) v = lw[row * FN_H + k] * scale;
+        if (row < label_rows) v = lw[row * FN_H + k] * scale;
         else if (row == L) v = sigma_w[k];
         unsigned char* chunk = head_img + (size_t)(k / FN_KCHUNK) * (32 * FN_KCHUNK * 2);
         *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
@@ -220,13 +236,15 @@ __global__ void fingerprint_kernel(FpSegments seg, unsigned long long* __restric
 
 }  // namespace
 
-int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st) {
+int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const fenerf_field_params* p, unsigned long long* out,
+                      cudaStream_t st) {
     FpSegments seg;
     seg.n = 0;
     auto add = [&](const float* ptr, unsigned long long count) {
         if (ptr && count) { seg.ptr[seg.n] = ptr; seg.count[seg.n] = count; ++seg.n; }
     };
-    const int n_trunk = L.trunk_hidden + 1, n_color = L.n_hidden - L.trunk_hidden;
+    // (a label FiLM layer takes a hidden slot: it is hashed with the label parameters below, label_w[0])
+    const int n_trunk = L.trunk_hidden + 1, n_color = L.n_hidden - L.trunk_hidden - lf.on;
     for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? 3 : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
     add(p->sigma_w, FN_H); add(p->sigma_b, 1);
     for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (unsigned long long)(i == 0 ? L.kx + FN_H : FN_H) * FN_H); add(p->color_b[i], FN_H); }
@@ -243,17 +261,22 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
     return 0;
 }
 
-int pack_field(const fenerf_field_desc* f, const FnLayout& L, const fenerf_field_params* p, void* packed_v,
-               cudaStream_t st) {
+int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const fenerf_field_params* p,
+               void* packed_v, cudaStream_t st) {
     unsigned char* packed = static_cast<unsigned char*>(packed_v);
     FN_REQUIRE(p->trunk_w[0] && p->trunk_b[0], "trunk_w[0]/trunk_b[0] missing");
     pack_first_kernel<<<1, 256, 0, st>>>(p->trunk_w[0], p->trunk_b[0], (float*)(packed + L.first_w),
                                          (float*)(packed + L.first_b), packed + L.first_img);
     FN_LAUNCH_OK("pack_first_kernel");
+    if (lf.on)
+        FN_REQUIRE(p->label_w[0] && p->label_b[0] && p->label_w[2] && p->label_b[2] && !p->label_w[1] && !p->label_b[1],
+                   "label FiLM field: label_w/b[0] (FiLM layer) and [2] (head) required, [1] must be NULL");
+    const int c0 = L.trunk_hidden + lf.on;    // hidden slot of the first colour layer
     for (int l = 0; l < L.n_hidden; ++l) {
-        bool is_c0 = (l == L.trunk_hidden);
-        const float* w = l < L.trunk_hidden ? p->trunk_w[l + 1] : p->color_w[l - L.trunk_hidden];
-        const float* b = l < L.trunk_hidden ? p->trunk_b[l + 1] : p->color_b[l - L.trunk_hidden];
+        bool is_c0 = (l == c0);
+        const bool is_label = lf.on && l == lf.layer;
+        const float* w = l < L.trunk_hidden ? p->trunk_w[l + 1] : is_label ? p->label_w[0] : p->color_w[l - c0];
+        const float* b = l < L.trunk_hidden ? p->trunk_b[l + 1] : is_label ? p->label_b[0] : p->color_b[l - c0];
         FN_REQUIRE(w && b, "weight/bias of hidden layer %d missing", l);
         int in_dim = is_c0 ? L.kx + FN_H : FN_H;
         int x_off = is_c0 ? L.kx : 0;
@@ -271,7 +294,11 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const fenerf_field
     pack_heads_kernel<<<3, 256, 0, st>>>(p->sigma_w, p->sigma_b, p->rgb_w, p->rgb_b, (float*)(packed + L.sigma_w),
                                          (float*)(packed + L.rgb_w));
     FN_LAUNCH_OK("pack_heads_kernel");
-    if (L.label_dim > 0) {
+    if (lf.on) {             // no chain to pre-multiply: the head is one Linear
+        pack_label_film_head_kernel<<<1, 256, 0, st>>>(p->label_w[2], p->label_b[2], L.label_dim, (float*)(packed + L.label_w),
+                                                       packed + lf.img);
+        FN_LAUNCH_OK("pack_label_film_head_kernel");
+    } else if (L.label_dim > 0) {
         for (int i = 0; i < 3; i += 2) FN_REQUIRE(p->label_w[i] && p->label_b[i], "label layer %d missing", i);
         FN_REQUIRE((p->label_w[1] == nullptr) == (p->label_b[1] == nullptr), "label layer 1: weight and bias must both be given or both be NULL");
         double* u = reinterpret_cast<double*>(packed + L.label_scratch);
@@ -283,7 +310,8 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const fenerf_field
         label_step3_kernel<<<1, 256, 0, st>>>((float*)(packed + L.label_w), L.label_dim);
         FN_LAUNCH_OK("label_step3_kernel");
     }
-    pack_head_imgs_kernel<<<1, 256, 0, st>>>((const float*)(packed + L.label_w), L.label_dim, p->sigma_w, p->rgb_w,
+    pack_head_imgs_kernel<<<1, 256, 0, st>>>((const float*)(packed + L.label_w), L.label_dim, lf.on ? 0 : L.label_dim,
+                                             p->sigma_w, p->rgb_w,
                                              packed + L.head_img, packed + L.rgb_img);
     FN_LAUNCH_OK("pack_head_imgs_kernel");
     if (L.grid_channels > 0) {

@@ -17,6 +17,11 @@
 //   Wbuf [2][16][256]   double-buffered 16-row slabs of the k-major weights via cp.async
 //   each thread owns a 4-point x 16-column micro tile; 5 LDS.128 feed 64 FFMA per k
 //   (the 16-point gather variant maps lanes point-major so a warp's weight reads broadcast)
+//
+// Label FiLM fields (kLabelFilm): A keeps the trunk output for the first colour layer, so the label FiLM layer's output
+// goes through the weight-slab buffer instead, which is free between layers: one 64-feature quarter at a time, each
+// followed by its share of the label head's k-sum (the running sums sit in the same buffer), so shared memory and
+// occupancy stay those of the other fields.
 #include "siren_common.cuh"
 #include "sm90.cuh"
 
@@ -159,7 +164,7 @@ __device__ __forceinline__ float grid_feature(const float* __restrict__ grid, in
     return out;
 }
 
-template <bool kGather, int P>
+template <bool kGather, int P, bool kLabelFilm = false>
 __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned char* smem_raw) {
     constexpr int TM = 16 * P;
     Smem<P>& s = *reinterpret_cast<Smem<P>*>(smem_raw);
@@ -245,7 +250,8 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                 // heads on the trunk output: sigma, then the pre-multiplied label map
                 const float* sw = reinterpret_cast<const float*>(pk + L.sigma_w);
                 const float* lw = reinterpret_cast<const float*>(pk + L.label_w);
-                for (int it = tid; it < TM * (1 + (a.sigma_only ? 0 : L.label_dim)); it += NTHREADS) {
+                // (a label FiLM field's labels come from its label branch below)
+                for (int it = tid; it < TM * (1 + ((kLabelFilm || a.sigma_only) ? 0 : L.label_dim)); it += NTHREADS) {
                     int pt = it % TM, o = it / TM;
                     const float* w = o == 0 ? sw : lw + (size_t)(o - 1) * FN_H;
                     float r = o == 0 ? __ldg(sw + FN_H) : __ldg(lw + FENERF_MAX_LABEL * FN_H + (o - 1));
@@ -265,8 +271,52 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                 if (kGather && a.guard_stats && tile == 0 && tid == 0) a.guard_stats[0] = n_only;
                 __syncthreads();
                 if (a.sigma_only) break;          // the colour branch does not feed the density
+                if constexpr (kLabelFilm) {
+                    // ---- label FiLM layer (hidden layer l) on the trunk output, then the label head ----
+                    static_assert(sizeof(s.W) >= (64 + FENERF_MAX_LABEL) * TM * sizeof(float), "label scratch fits the slab buffer");
+                    init_bias(reinterpret_cast<const float*>(pk + L.hid_b[l]), acc, tid);
+                    gemm_tile(s, reinterpret_cast<const float*>(pk + L.hid_w32[l]), FN_H, acc, tid);   // ends in a barrier
+                    // the slab buffer: [64 features][TM points] of label activations, then the running sums [label][TM]
+                    float* lab = &s.W[0][0][0];
+                    float* sums = lab + 64 * TM;
+                    const float* lw = reinterpret_cast<const float*>(pk + L.label_w);
+                    const int n_items = TM * L.label_dim;
+                    // one 64-feature quarter at a time (this thread's column group j): the FiLM epilogue, rounded as
+                    // film_store (FiLM row l + 1), then its share of the head's k-sum -- the sums run over k = 0 .. 255 in
+                    // order, as the trunk heads' do
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                        for (int m = 0; m < P; ++m) {
+                            const float* fl = a.film + ((size_t)s.bidx[tm * P + m] * L.n_film + l + 1) * 2 * FN_H;
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                const int col = tn * 4 + j * 64 + i;
+                                const float fr = __ldg(fl + col), ph = __ldg(fl + FN_H + col);
+                                lab[(tn * 4 + i) * TM + tm * P + m] = sinf(__fadd_rn(__fmul_rn(fr, acc[m][j * 4 + i]), ph));
+                            }
+                        }
+                        __syncthreads();
+#pragma unroll 1
+                        for (int it = tid; it < n_items; it += NTHREADS) {
+                            const int pt = it % TM, o = it / TM;
+                            const float* w = lw + (size_t)o * FN_H + 64 * j;
+                            float r = j == 0 ? __ldg(lw + FENERF_MAX_LABEL * FN_H + o) : sums[it];   // bias first
+#pragma unroll 8
+                            for (int k = 0; k < 64; ++k) r = fmaf(lab[k * TM + pt], __ldg(w + k), r);
+                            sums[it] = r;
+                        }
+                        __syncthreads();
+                    }
+                    for (int it = tid; it < n_items; it += NTHREADS) {
+                        const long long flat = s.flat[it % TM];
+                        if (flat >= 0) a.out[flat * C + it / TM] = sums[it];
+                    }
+                    __syncthreads();                                           // the sums are read before the next slab lands
+                    continue;                                                  // s.A still holds the trunk output
+                }
             }
-            const int K = FN_H + (l == L.trunk_hidden ? L.kx_pad : 0);
+            const int K = FN_H + (l == L.trunk_hidden + (kLabelFilm ? 1 : 0) ? L.kx_pad : 0);
             init_bias(reinterpret_cast<const float*>(pk + L.hid_b[l]), acc, tid);
             gemm_tile(s, reinterpret_cast<const float*>(pk + L.hid_w32[l]), K, acc, tid);
             film_store(s, a.film, L.n_film, l + 1, acc, tid);
@@ -288,10 +338,10 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
     }
 }
 
-template <bool kGather, int P>
+template <bool kGather, int P, bool kLabelFilm>
 __global__ void __launch_bounds__(NTHREADS, 2) siren_exact_kernel(ExactArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    siren_exact_body<kGather, P>(a, smem_raw);
+    siren_exact_body<kGather, P, kLabelFilm>(a, smem_raw);
 }
 
 // GUARD refinement: the list length is only known on the device.  Short lists (small renders; fields whose densities
@@ -307,8 +357,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_exact_guard_kernel(ExactArg
 
 }  // namespace
 
-int siren_points_exact(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
-                       const float* film, int batch, long long ppb, int dir_group, int lock_dirs,
+int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const unsigned char* packed, const float* points,
+                       const float* dirs, const float* film, int batch, long long ppb, int dir_group, int lock_dirs,
                        const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only) {
     static_assert(sizeof(Smem<4>) <= 113 * 1024, "two CTAs per SM must fit");
     constexpr int TM = 64;
@@ -325,13 +375,17 @@ int siren_points_exact(const FnLayout& L, const unsigned char* packed, const flo
     FN_REQUIRE(ppb % a.dir_group == 0, "points_per_batch %lld not a multiple of dir_group %d", ppb, a.dir_group);
     size_t smem = sizeof(Smem<4>);
     int blocks = (int)(a.n_items < (long long)num_sms() * 2 ? a.n_items : (long long)num_sms() * 2);
-    if (gather) {
-        FN_CUDA_OK(cudaFuncSetAttribute(siren_exact_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        siren_exact_kernel<true, 4><<<blocks, NTHREADS, smem, st>>>(a);
-    } else {
-        FN_CUDA_OK(cudaFuncSetAttribute(siren_exact_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        siren_exact_kernel<false, 4><<<blocks, NTHREADS, smem, st>>>(a);
-    }
+    // (the density alone never reaches the label branch: sigma_only runs the plain instantiation)
+    auto launch = [&](auto kernel) -> int {
+        FN_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<blocks, NTHREADS, smem, st>>>(a);
+        return 0;
+    };
+    const bool label_film = lf.on && !sigma_only;
+    int e;
+    if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true>) : launch(siren_exact_kernel<true, 4, false>);
+    else e = label_film ? launch(siren_exact_kernel<false, 4, true>) : launch(siren_exact_kernel<false, 4, false>);
+    if (e) return e;
     FN_LAUNCH_OK("siren_exact_kernel");
     return 0;
 }

@@ -290,7 +290,8 @@ def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb
     ns = 2 * s if rd.hierarchical else s
     c = packed.desc.out_dim
     film = _prep(film, device)
-    if film.shape != (b, packed.desc.trunk_layers + packed.desc.color_layers, 2, _lib.HIDDEN):
+    n_film = packed.desc.trunk_layers + packed.desc.color_layers + (1 if packed.desc.reserved & _lib.FIELD_LABEL_FILM else 0)
+    if film.shape != (b, n_film, 2, _lib.HIDDEN):
         raise ValueError("film table has shape %s" % (tuple(film.shape),))
     pixels = torch.empty((b, _image_channels(rd, c), rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     depth = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_depth else None

@@ -37,7 +37,7 @@ class PackedField:
 def field_desc(spec) -> "_lib.FieldDesc":
     return _lib.FieldDesc(trunk_layers=spec.trunk_layers, color_layers=spec.color_layers, label_dim=spec.label_dim,
                           grid_channels=spec.grid_channels, grid_res=spec.grid_res, out_dim=spec.out_dim,
-                          input_scale=spec.input_scale, reserved=0)
+                          input_scale=spec.input_scale, reserved=_lib.FIELD_LABEL_FILM if spec.label_film else 0)
 
 
 def _f32(t, device):
@@ -72,7 +72,15 @@ def collect_params(module, device):
         p.color_b[i] = ptr(layer.layer.bias)
     p.rgb_w = ptr(module.color_layer_linear[0].weight)
     p.rgb_b = ptr(module.color_layer_linear[0].bias)
-    if spec.label_dim:
+    if spec.label_film:
+        # slots: [label FiLM layer, NULL, head 256->label_dim] (include/fenerf_b200.h, FENERF_FIELD_LABEL_FILM)
+        head = [m for m in module.label_layer_linear if isinstance(m, torch.nn.Linear)]
+        if len(head) != 1:
+            raise ValueError("label FiLM head: expected one Linear layer, got %d" % len(head))
+        for i, lin in ((0, module.label_layer_sine.layer), (2, head[0])):
+            p.label_w[i] = ptr(lin.weight)
+            p.label_b[i] = ptr(lin.bias)
+    elif spec.label_dim:
         chain = [m for m in module.label_layer_linear if isinstance(m, torch.nn.Linear)]
         if len(chain) not in (2, 3):
             raise ValueError("label head: expected a chain of 2 or 3 Linear layers, got %d" % len(chain))

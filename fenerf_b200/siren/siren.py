@@ -16,6 +16,7 @@ Reference interfaces mirrored (file:line in the reference tree):
   UniformBoxWarp                              siren/siren.py:181-187
   sample_from_3dgrid                          siren/siren.py:314-330
   SPATIALSIRENBASELINE                        siren/siren.py:189-244
+  SPATIALSIRENSEMANTIC                        siren/siren.py:597-671
   SPATIALSIRENBASELINESEMANTIC                siren/siren.py:674-744
   SPATIALSIRENDISENTANGLE                     siren/siren.py:747-813
   SPATIALSIRENSEMANTICDISENTANGLE             siren/siren.py:1085-1161
@@ -144,6 +145,8 @@ class FieldSpec:
                    cat[ray_dir(3), grid_feat(grid_channels), trunk_out(256)]
     label_dim      semantic logits (0 = none); the reference's activation-free Linear chain
                    (siren/siren.py:1486-1490) is pre-multiplied into one 256 -> label_dim map
+    label_film     the label head is a FiLM layer on the trunk output followed by one Linear
+                   (siren/siren.py:663-665); its FiLM row sits between the trunk's and the colour branch's
     grid_channels  feature-grid channels (0 = no grid)
     input_scale    UniformBoxWarp factor applied to the position before the trunk and the grid
     out_dim        label_dim + 3 (rgb) + 1 (sigma); channel order [labels, rgb, sigma]
@@ -156,6 +159,7 @@ class FieldSpec:
     input_scale: float
     out_dim: int
     double_latent: bool
+    label_film: bool = False
 
 
 def _fused_mapping_ok(net, z):
@@ -264,6 +268,10 @@ class TALLSIREN(_FieldBase):
         return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=0, grid_channels=0,
                          grid_res=0, input_scale=1.0, out_dim=4, double_latent=False)
 
+    def film_rows(self):
+        """FiLM layers of the table: the trunk's and the colour layer's."""
+        return len(self.network) + 1
+
     def film_table(self, frequencies, phase_shifts):
         """(B, L*256) raw mapping outputs -> (B, L, 2, 256) [15 f + 30, phase] (siren.py:165)."""
         b = frequencies.shape[0]
@@ -276,7 +284,7 @@ class TALLSIREN(_FieldBase):
         launches); otherwise the PyTorch modules, so that autograd reaches the mapping network and the latent.
         `avg` = (avg_frequencies, avg_phase_shifts) enables the psi truncation of staged_forward."""
         from .. import ops
-        n = len(self.network) + 1
+        n = self.film_rows()
         if _fused_mapping_ok(self.mapping_network, z):
             film = torch.empty((z.shape[0], n, 2, self.hidden_dim), dtype=torch.float32, device=z.device)
             return ops.mapping_film(self.mapping_network, z, film, 0, n, avg=avg, psi=psi)
@@ -352,6 +360,45 @@ class SPATIALSIRENBASELINESEMANTIC(TALLSIREN):
     def field_spec(self):
         return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=19, grid_channels=0, grid_res=0,
                          input_scale=float(self.gridwarper.scale_factor), out_dim=23, double_latent=False)
+
+
+class SPATIALSIRENSEMANTIC(TALLSIREN):
+    """SPATIALSIRENBASELINE plus a label branch beside the colour branch (siren/siren.py:597-671): a FiLM layer on the
+    trunk output, then Linear(256 -> 19).  FiLM rows: trunk 0..7, label 8, colour 9; output channels [labels (19),
+    rgb (3), sigma (1)] whatever `output_dim` says."""
+
+    def __init__(self, input_dim=2, z_dim=100, hidden_dim=256, output_dim=1, device=None):
+        nn.Module.__init__(self)
+        self.device = device
+        self.input_dim = input_dim
+        self.z_dim = z_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+        self.max_batch_size = 2500
+
+        widths = [3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        self.final_layer = nn.Linear(hidden_dim, 1)
+        self.label_layer_sine = FiLMLayer(hidden_dim, hidden_dim)
+        self.label_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 19))
+        self.color_layer_sine = FiLMLayer(hidden_dim + 3, hidden_dim)
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 3))
+        self.mapping_network = CustomMappingNetwork(z_dim, 256, (len(self.network) + 2) * hidden_dim * 2)
+
+        for part in (self.network, self.final_layer, self.label_layer_sine, self.label_layer_linear,
+                     self.color_layer_sine, self.color_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(first_layer_film_sine_init)
+        self.activation = nn.Softmax(dim=-1)     # unused, as in the reference (its forward returns raw logits)
+        self.gridwarper = UniformBoxWarp(0.24)
+
+    def field_spec(self):
+        return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=19, grid_channels=0, grid_res=0,
+                         input_scale=float(self.gridwarper.scale_factor), out_dim=23, double_latent=False,
+                         label_film=True)
+
+    def film_rows(self):
+        return len(self.network) + 2             # trunk, label, colour (siren.py:656-668)
 
 
 class _DoubleLatentField(_FieldBase):

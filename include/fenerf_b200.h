@@ -46,17 +46,26 @@ extern "C" {
  *   x = FiLM_0(3->256)(x); x = FiLM_i(256->256)(x), i < trunk_layers      (siren.py:113-123)
  *   sigma  = Linear(256->1)(x)
  *   labels = Linear chain 256->256->256->label_dim (no activation; pre-multiplied)   [optional]
+ *     or, with FENERF_FIELD_LABEL_FILM, a FiLM branch beside the colour branch:
+ *   labels = Linear(256->label_dim)(FiLM(256->256)(x))                                 (siren.py:663-665)
  *   c = FiLM(cat[dir(3), grid_feat(G), x(256)] -> 256); c = FiLM(256->256)(c) ...  color_layers
  *   rgb = sigmoid(Linear(256->3)(c))
  *   out = [labels, rgb, sigma]
  * TALLSIREN (siren.py:126-178):  trunk 8, color 1, label 0, grid 0, scale 1, out 4.
  * TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_DIM_96 (siren.py:1451-1546):
  *                                trunk 8, color 3, label 18, grid 32 x 96^3, scale 2/0.24, out 22.
+ * SPATIALSIRENSEMANTIC (siren.py:597-671):
+ *                                trunk 8, color 1, label 19 (FENERF_FIELD_LABEL_FILM), grid 0, scale 2/0.24, out 23.
  * The hidden width is fixed at 256.                                                            */
 #define FENERF_MAX_TRUNK 8
 #define FENERF_MAX_COLOR 8
 #define FENERF_MAX_LABEL 32
 #define FENERF_HIDDEN 256
+
+/* fenerf_field_desc.flags.  Unknown bits are rejected with FENERF_E_UNSUPPORTED. */
+#define FENERF_FIELD_LABEL_FILM 0x1   /* the label head is FiLM(256->256) then Linear(256->label_dim) on the trunk
+                                         output; label_dim >= 1 and color_layers <= 7 (the packed layout holds 15
+                                         256-wide layers after the first: 7 trunk + 1 label + the colour layers) */
 
 typedef struct fenerf_field_desc {
     int32_t trunk_layers;   /* 2..8 */
@@ -66,7 +75,7 @@ typedef struct fenerf_field_desc {
     int32_t grid_res;       /* cubic grid side (D = H = W), 0 if no grid */
     int32_t out_dim;        /* label_dim + 4 */
     float   input_scale;
-    int32_t reserved;
+    int32_t reserved;       /* flags: FENERF_FIELD_* bits, 0 = a plain field */
 } fenerf_field_desc;
 
 /* Raw parameters exactly as torch stores them: nn.Linear.weight is [out][in] row-major fp32,
@@ -81,7 +90,9 @@ typedef struct fenerf_field_params {
     const float* rgb_w;                      /* [3][256] */
     const float* rgb_b;                      /* [3] */
     const float* label_w[3];                 /* [256][256], [256][256], [label_dim][256]; NULL if label_dim == 0;
-                                                label_w[1] / label_b[1] NULL for a two-layer chain (siren.py:1189-1191) */
+                                                label_w[1] / label_b[1] NULL for a two-layer chain (siren.py:1189-1191);
+                                                FENERF_FIELD_LABEL_FILM: [0] the label FiLM layer [256][256], [1] NULL,
+                                                [2] the label head [label_dim][256] */
     const float* label_b[3];
     const float* grid;                       /* (1, G, R, R, R) or NULL */
 } fenerf_field_params;
@@ -116,13 +127,15 @@ int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_
  * also the entry extract_*shapes.py needs (extract_double_semantic_shapes.py:59,80).
  *   points  (B, P, 3)      positions, not yet box-warped
  *   dirs    (B, P/dir_group, 3)  one direction per `dir_group` consecutive points (1 = per point)
- *   film    (B, trunk+color, 2, 256)  [15*freq+30, phase] per FiLM layer
+ *   film    (B, trunk+color, 2, 256)  [15*freq+30, phase] per FiLM layer; FENERF_FIELD_LABEL_FILM:
+ *           (B, trunk+1+color, 2, 256), rows trunk.., label, colour.. (the reference's order, siren.py:656-668)
  *   out     (B, P, C)
  *   only_idx  optional int32 list (n_only entries) of flat point indices b*P+p to evaluate;
  *             others are left untouched in `out` (used by the GUARD refinement)               */
 /* OR-ed into `precision`: only the density channel out[..., C-1] is required (a 256^3 density grid for
  * marching cubes, extract_double_semantic_shapes.py:59-62 keeps `[:, :, -1:]`); the colour / label
- * branches are skipped on the wgmma path and the other channels of `out` are then left unspecified. */
+ * branches (the label FiLM branch included) are skipped on the wgmma path and the other channels of `out` are then left
+ * unspecified. */
 #define FENERF_POINTS_SIGMA_ONLY 0x100
 
 int fenerf_siren_points(const fenerf_field_desc* field, const void* packed,
