@@ -157,10 +157,14 @@ class _FieldBackward:
         for i in range(1, self.n_film):
             self.dW_b[i] = torch.zeros((B, 256, 256), dtype=torch.float32, device=dev)
         self.dWx_b = torch.zeros((B, 256, self.kx_pad), dtype=torch.float32, device=dev)   # colour 0's narrow inputs
-        self.d_heads_w = torch.zeros((32, 256), dtype=torch.float32, device=dev)
-        self.d_heads_b = torch.zeros((32,), dtype=torch.float32, device=dev)
-        self.d_rgb_w = torch.zeros((8, 256), dtype=torch.float32, device=dev)
-        self.d_rgb_b = torch.zeros((8,), dtype=torch.float32, device=dev)
+        # head-gradient widths of fenerf_head_grads: [labels, sigma, pad] and the colour head's (include/fenerf_b200.h)
+        L = self.spec.label_dim
+        self.n_heads = L + 8 if self.spec.feature_head else 32
+        self.n_rgb = 64 if self.spec.feature_head else 8
+        self.d_heads_w = torch.zeros((self.n_heads, 256), dtype=torch.float32, device=dev)
+        self.d_heads_b = torch.zeros((self.n_heads,), dtype=torch.float32, device=dev)
+        self.d_rgb_w = torch.zeros((self.n_rgb, 256), dtype=torch.float32, device=dev)
+        self.d_rgb_b = torch.zeros((self.n_rgb,), dtype=torch.float32, device=dev)
         self.grid_grad_cl = None
         if G:
             r = self.spec.grid_res
@@ -184,16 +188,15 @@ class _FieldBackward:
         if self.own_gemm:
             self.Wn64 = torch.zeros((256, 64), dtype=torch.float16, device=dev)
             self.Wn64[:, :self.kx] = self.Wc0x_narrow
-        L = self.spec.label_dim
         self.L = L
-        heads = torch.zeros((32, 256), dtype=torch.float32, device=dev)
+        heads = torch.zeros((self.n_heads, 256), dtype=torch.float32, device=dev)
         if L and not self.lf:      # (a label FiLM field's head acts on the label layer: its rows stay zero here)
             weff, _ = _label_eff(fw.labels)
             heads[:L] = weff
         heads[L] = fw.sigma[0].detach().float().reshape(-1)
         self.Wheads32 = heads
-        rgbw = torch.zeros((8, 256), dtype=self.dt, device=dev)
-        rgbw[:3] = fw.rgb[0].detach().to(self.dt)
+        rgbw = torch.zeros((self.n_rgb, 256), dtype=self.dt, device=dev)
+        rgbw[:self.spec.rgb_dim] = fw.rgb[0].detach().to(self.dt)
         self.Wrgb16 = rgbw
         self.bias = [b.detach().float().contiguous() for _, b in fw.film_layers()]
 
@@ -274,8 +277,8 @@ class _FieldBackward:
                 else:
                     A[c0 + j], Gt[c0 + j] = self._stash(_mm32(A[c0 + j - 1], self.Wc16[j].t()), c0 + j, b0, P, ppb)
             # ---- head gradients ----
-            dH = torch.empty((P, 32), dtype=self.dt, device=dev)
-            dRGB = torch.empty((P, 8), dtype=self.dt, device=dev)
+            dH = torch.empty((P, self.n_heads), dtype=self.dt, device=dev)
+            dRGB = torch.empty((P, self.n_rgb), dtype=self.dt, device=dev)
             _lib.check(lib.fenerf_head_grads(d_raw.data_ptr(), raw.data_ptr(), P, spec.out_dim, self.L, self.scale.data_ptr(),
                                              dH.data_ptr(), dRGB.data_ptr(), self.dtc, st))
             a_last = A[self.n_film - 1]
@@ -360,8 +363,9 @@ class _FieldBackward:
         L = self.L
         grads[id(fw.sigma[0])] = (self.d_heads_w[L] * inv).reshape(fw.sigma[0].shape)
         grads[id(fw.sigma[1])] = (self.d_heads_b[L] * inv).reshape(fw.sigma[1].shape)
-        grads[id(fw.rgb[0])] = self.d_rgb_w[:3] * inv
-        grads[id(fw.rgb[1])] = self.d_rgb_b[:3] * inv
+        n_rgb = self.spec.rgb_dim
+        grads[id(fw.rgb[0])] = self.d_rgb_w[:n_rgb] * inv
+        grads[id(fw.rgb[1])] = self.d_rgb_b[:n_rgb] * inv
         if self.lf:
             (hw, hb), = fw.labels
             grads[id(hw)] = self.d_heads_w[:L] * inv

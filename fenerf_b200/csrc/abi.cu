@@ -65,21 +65,25 @@ void stage_mark(int i, cudaStream_t st) {
 }
 
 // fn_make_layout with the library's error codes: unknown flag bits are FENERF_E_UNSUPPORTED
-int make_layout(const fenerf_field_desc* field, FnLayout* L, FnLabelFilm* lf = nullptr) {
-    const int r = fn_make_layout(field, L, lf);
+int make_layout(const fenerf_field_desc* field, FnLayout* L, FnLabelFilm* lf = nullptr, FnFeatureHead* fh = nullptr) {
+    const int r = fn_make_layout(field, L, lf, fh);
     if (r == -2) return fail(FENERF_E_UNSUPPORTED, "unknown field flag bits 0x%x", (unsigned)field->reserved);
+    if (r == -3)
+        return fail(FENERF_E_UNSUPPORTED, "FENERF_FIELD_FEATURE_HEAD: only label_dim 0 (no other flag) or label_dim 64 with "
+                    "FENERF_FIELD_LABEL_FILM, without a grid (flags 0x%x, label_dim %d, grid %d)", (unsigned)field->reserved,
+                    field->label_dim, field->grid_channels);
     FN_REQUIRE(r == 0, "unsupported field description");
     return 0;
 }
 
-int run_field(const FnLayout& L, const FnLabelFilm& lf, const void* packed, const float* points, const float* dirs, const float* film,
+int run_field(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const void* packed, const float* points, const float* dirs, const float* film,
               int batch, long long ppb, int dir_group, int lock_dirs, int precision, float* out, cudaStream_t st,
               int sigma_only = 0, float* sigma_out = nullptr) {
     const unsigned char* pk = static_cast<const unsigned char*>(packed);
     if (precision == FENERF_PRECISION_EXACT)
-        return siren_points_exact(L, lf, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, nullptr, 0, out, st, sigma_only);
+        return siren_points_exact(L, lf, fh, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, nullptr, 0, out, st, sigma_only);
     // the wgmma kernel (siren_fast.cu)
-    return siren_points_fast(L, lf, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
+    return siren_points_fast(L, lf, fh, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
 }
 
 }  // namespace
@@ -101,21 +105,23 @@ int fenerf_pack_field(const fenerf_field_desc* field, const fenerf_field_params*
                       size_t packed_bytes, void* stream) {
     FnLayout L;
     FnLabelFilm lf;
-    if (int e = make_layout(field, &L, &lf)) return e;
+    FnFeatureHead fh;
+    if (int e = make_layout(field, &L, &lf, &fh)) return e;
     FN_REQUIRE(params && packed, "params/packed is NULL");
     FN_REQUIRE(((uintptr_t)packed & 1023) == 0, "packed buffer must be 1024-byte aligned");
     if (packed_bytes < L.total) return fail(FENERF_E_WORKSPACE, "packed buffer too small: %zu < %zu", packed_bytes, L.total);
-    return pack_field(field, L, lf, params, packed, (cudaStream_t)stream);
+    return pack_field(field, L, lf, fh, params, packed, (cudaStream_t)stream);
 }
 
 int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_params* params, uint64_t* out,
                              void* stream) {
     FnLayout L;
     FnLabelFilm lf;
-    if (int e = make_layout(field, &L, &lf)) return e;
+    FnFeatureHead fh;
+    if (int e = make_layout(field, &L, &lf, &fh)) return e;
     FN_REQUIRE(params && out, "params/out is NULL");
     FN_REQUIRE(((uintptr_t)out & 7) == 0, "out must be 8-byte aligned");
-    return field_fingerprint(L, lf, params, reinterpret_cast<unsigned long long*>(out), (cudaStream_t)stream);
+    return field_fingerprint(L, lf, fh, params, reinterpret_cast<unsigned long long*>(out), (cudaStream_t)stream);
 }
 
 int fenerf_siren_points(const fenerf_field_desc* field, const void* packed, const float* points, const float* dirs,
@@ -123,10 +129,11 @@ int fenerf_siren_points(const fenerf_field_desc* field, const void* packed, cons
                         int32_t precision, const int32_t* only_idx, int32_t n_only, float* out, void* stream) {
     FnLayout L;
     FnLabelFilm lf;
+    FnFeatureHead fh;
     const int sigma_only = (precision & FENERF_POINTS_SIGMA_ONLY) ? 1 : 0;
     precision &= 0xff;
     FN_REQUIRE(precision >= FENERF_PRECISION_EXACT && precision <= FENERF_PRECISION_GUARD, "unknown precision %d", precision);
-    if (int e = make_layout(field, &L, &lf)) return e;
+    if (int e = make_layout(field, &L, &lf, &fh)) return e;
     FN_REQUIRE(packed && points && film && out, "NULL argument");
     FN_REQUIRE(dirs, "dirs is NULL (pass any (B,P/dir_group,3) tensor; the colour branch consumes it)");
     FN_REQUIRE(batch >= 1 && points_per_batch >= 1 && dir_group >= 1, "bad sizes");
@@ -134,11 +141,11 @@ int fenerf_siren_points(const fenerf_field_desc* field, const void* packed, cons
     cudaStream_t st = (cudaStream_t)stream;
     if (only_idx) {
         if (n_only <= 0) return 0;
-        return siren_points_exact(L, lf, (const unsigned char*)packed, points, dirs, film, batch, points_per_batch, dir_group,
+        return siren_points_exact(L, lf, fh, (const unsigned char*)packed, points, dirs, film, batch, points_per_batch, dir_group,
                                   0, only_idx, n_only, out, st);
     }
     FN_REQUIRE(precision >= FENERF_PRECISION_EXACT && precision <= FENERF_PRECISION_GUARD, "unknown precision %d", precision);
-    return run_field(L, lf, packed, points, dirs, film, batch, points_per_batch, dir_group, 0, precision, out, st, sigma_only);
+    return run_field(L, lf, fh, packed, points, dirs, film, batch, points_per_batch, dir_group, 0, precision, out, st, sigma_only);
 }
 
 int fenerf_camera_poses(int32_t n, int32_t mode, float h_stddev, float v_stddev, float h_mean, float v_mean,
@@ -164,7 +171,7 @@ int fenerf_resample(const fenerf_render_desc* rd, int32_t out_dim, const float* 
                     float* points_fine, int64_t* inds, void* stream) {
     if (int e = check_render_desc(rd)) return e;
     FN_REQUIRE(raw_coarse && z_vals && dirs && origins && rng_u && z_fine && points_fine, "NULL argument");
-    FN_REQUIRE(out_dim >= 2 && out_dim <= 36, "out_dim %d unsupported", out_dim);
+    FN_REQUIRE(out_dim >= 2 && out_dim <= 129, "out_dim %d unsupported", out_dim);
     FN_REQUIRE(rd->noise_std == 0.f || rng_noise, "noise_std != 0 needs rng_noise");
     return resample(rd, out_dim, raw_coarse, z_vals, dirs, origins, rd->noise_std != 0.f ? rng_noise : nullptr, rng_u,
                     z_fine, points_fine, (long long*)inds, (cudaStream_t)stream);
@@ -234,7 +241,8 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
     if (int e = check_render_desc(rd)) return e;
     FnLayout L;
     FnLabelFilm lf;
-    if (int e = make_layout(field, &L, &lf)) return e;
+    FnFeatureHead fh;
+    if (int e = make_layout(field, &L, &lf, &fh)) return e;
     FN_REQUIRE(packed && film && x_lin && y_lin && z_lin && cam2world && rng_perturb && pixels && workspace, "NULL argument");
     FN_REQUIRE(!rd->hierarchical || rng_u, "hierarchical render needs rng_u");
     FN_REQUIRE(!rd->hierarchical || rd->num_steps >= 3, "hierarchical render needs num_steps >= 3");
@@ -265,13 +273,13 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
     // the wgmma pass also leaves the densities as one float per point for the resampler (which never reads the far
     // sample, so the GUARD refinement of raw_c below does not concern that copy)
     float* sigma_c = (rd->hierarchical && rd->precision != FENERF_PRECISION_EXACT) ? (float*)(ws + w.sigma_c) : nullptr;
-    if (int e = run_field(L, lf, packed, points_c, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
+    if (int e = run_field(L, lf, fh, packed, points_c, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
                           rd->precision, raw_c, st, 0, sigma_c)) return e;
     stage_mark(2, st);
     if (rd->precision == FENERF_PRECISION_GUARD) {
         float tau = rd->guard_tau > 0.f ? rd->guard_tau : 1.5e-3f;
         const int n_samples = rd->hierarchical ? 2 * rd->num_steps : rd->num_steps;
-        if (int e = guard_refine(L, (const unsigned char*)packed, points_c, dirs, film, rd->batch, rays, rd->num_steps,
+        if (int e = guard_refine(fn_trunk_view(L, fh), (const unsigned char*)packed, points_c, dirs, film, rd->batch, rays, rd->num_steps,
                                  rd->lock_view_dependence, tau, noise_f ? noise_f + (n_samples - 1) : nullptr, n_samples,
                                  rd->noise_std, raw_c, guard, (int32_t*)(ws + w.stats), st)) return e;
     }
@@ -280,7 +288,7 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
         if (int e = resample(rd, C, raw_c, z_c, dirs, origins, noise_c, rng_u, z_f, points_f, (long long*)inds_dbg, st,
                              /*sort_fine=*/1, sigma_c)) return e;
         stage_mark(4, st);
-        if (int e = run_field(L, lf, packed, points_f, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
+        if (int e = run_field(L, lf, fh, packed, points_f, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
                               rd->precision, raw_f, st)) return e;
     } else {
         stage_mark(4, st);

@@ -9,6 +9,7 @@
 //                               everything the backward of a FiLM layer needs besides the GEMMs
 //   gate_backward_kernel        dZ = dA * gate in place (fp16) + per-image column sums (bias / phase grads)
 //   head_grads_kernel           d raw -> scaled fp16 head gradients (sigmoid', label / sigma columns)
+//   head_grads_feature_kernel   the same for the feature-head fields: 64 linear feature columns, 0 / 64 label columns
 //   extras_gather_kernel        [dir, trilinear grid features] per point (the first colour layer's extra inputs)
 //   grid_scatter_add_kernel     d features -> channels-last grid gradient (vector atomics)
 //   grid_unpack_grad_kernel     channels-last -> torch's channel-major (1, G, R, R, R) layout
@@ -167,6 +168,35 @@ __global__ void head_grads_kernel(const float* __restrict__ d_raw, const float* 
     }
 }
 
+// feature-head layout (C = L + 65): d raw (P, C) -> dH (P, L + 8) = [d labels (L), d sigma, 0...] * scale,
+// dF (P, 64) = d feat * scale (a linear head: no sigmoid factor).  Thread = (point, 8 consecutive columns of dH | dF).
+template <typename T>
+__global__ void head_grads_feature_kernel(const float* __restrict__ d_raw, long long P, int C, int L,
+                                          const float* __restrict__ scale_ptr, T* __restrict__ dH, T* __restrict__ dF) {
+    const float scale = *scale_ptr;
+    const int groups = (L + 8) / 8 + FN_FEAT / 8;
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < P * groups;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const long long p = idx / groups;
+        const int gi = (int)(idx % groups);
+        const float* d = d_raw + p * C;
+        Vec8<T> v;
+        if (gi < (L + 8) / 8) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int col = 8 * gi + i;
+                v.set(i, col < L ? d[col] * scale : (col == L ? d[C - 1] * scale : 0.f));
+            }
+            v.store(dH + p * (L + 8) + 8 * gi);
+        } else {
+            const int c0 = 8 * (gi - (L + 8) / 8);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v.set(i, d[L + c0 + i] * scale);
+            v.store(dF + p * FN_FEAT + c0);
+        }
+    }
+}
+
 // ---- first colour layer's narrow inputs: [dir(3), grid features(G)] per point ----------------------------
 __global__ void extras_gather_kernel(const float* __restrict__ points, const float* __restrict__ dirs, long long P,
                                      long long ppb, int dir_group, int lock_dirs, float input_scale,
@@ -274,6 +304,13 @@ int gate_backward(void* dA, const void* gate, long long P, long long ppb, float*
 
 int head_grads(const float* d_raw, const float* raw, long long P, int C, int L, const float* scale, void* dH, void* dRGB,
                int f32, cudaStream_t st) {
+    if (C == L + FN_FEAT + 1 && (L == 0 || L == FN_FEAT)) {      // feature-head fields
+        const long long items = P * ((L + 8) / 8 + FN_FEAT / 8);
+        if (f32) head_grads_feature_kernel<float><<<grid_blocks(items, 256), 256, 0, st>>>(d_raw, P, C, L, scale, (float*)dH, (float*)dRGB);
+        else head_grads_feature_kernel<__half><<<grid_blocks(items, 256), 256, 0, st>>>(d_raw, P, C, L, scale, (__half*)dH, (__half*)dRGB);
+        FN_LAUNCH_OK("head_grads_feature_kernel");
+        return 0;
+    }
     FN_REQUIRE(L >= 0 && L < 32 && C == L + 4, "head layout");
     if (f32) head_grads_kernel<float><<<grid_blocks(P, 256), 256, 0, st>>>(d_raw, raw, P, C, L, scale, (float*)dH, (float*)dRGB);
     else head_grads_kernel<__half><<<grid_blocks(P, 256), 256, 0, st>>>(d_raw, raw, P, C, L, scale, (__half*)dH, (__half*)dRGB);

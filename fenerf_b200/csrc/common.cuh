@@ -101,16 +101,16 @@ __device__ __forceinline__ float sample_alpha(float delta, float act, float* dec
 __device__ __forceinline__ float transmittance_term(float alpha) { return __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f); }
 
 // ---- entry points of the individual translation units (called by abi.cu) ----
-int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const fenerf_field_params* p,
-               void* packed, cudaStream_t st);
-int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const unsigned char* packed, const float* points,
-                       const float* dirs, const float* film, int batch, long long ppb, int dir_group, int lock_dirs,
-                       const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only = 0);
-int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const fenerf_field_params* p, unsigned long long* out,
-                      cudaStream_t st);
-int siren_points_fast(const FnLayout& L, const FnLabelFilm& lf, const unsigned char* packed, const float* points,
-                      const float* dirs, const float* film, int batch, long long ppb, int dir_group, int lock_dirs,
-                      float* out, int sigma_only, cudaStream_t st, float* sigma_out = nullptr);
+int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh,
+               const fenerf_field_params* p, void* packed, cudaStream_t st);
+int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
+                       const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
+                       int lock_dirs, const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only = 0);
+int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const fenerf_field_params* p,
+                      unsigned long long* out, cudaStream_t st);
+int siren_points_fast(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
+                      const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
+                      int lock_dirs, float* out, int sigma_only, cudaStream_t st, float* sigma_out = nullptr);
 int guard_refine(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
                  const float* film, int batch, long long rays_per_batch, int num_steps, int lock_dirs, float tau,
                  const float* noise_far, long long noise_stride, float noise_std,
@@ -152,7 +152,7 @@ int film_forward_stash(const float* z, const float* bias, const float* film_laye
                        cudaStream_t st);
 int gate_backward(void* dA, const void* gate, long long P, long long ppb, float* colsum, int f32, cudaStream_t st);
 int head_grads(const float* d_raw, const float* raw, long long P, int C, int L, const float* scale, void* dH, void* dRGB,
-               int f32, cudaStream_t st);
+               int f32, cudaStream_t st);   // (both layouts of fenerf_head_grads)
 int extras_gather(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, long long P,
                   long long ppb, int dir_group, int lock_dirs, float* out, cudaStream_t st);
 int grid_scatter_add(const FnLayout& L, const float* points, const void* d_feat, int ld, long long P, float* grad_cl,

@@ -31,6 +31,17 @@
 // These fields live in FnLabelFilm, not in FnLayout, so that the kernels' argument blocks of the other fields keep
 // their layout.
 //
+// Feature-head fields (FENERF_FIELD_FEATURE_HEAD): the 64-wide heads get sections of their own, appended after
+// everything else (FnFeatureHead):
+//   rgb_w            [64][256] f32 + bias [64]           the colour head (linear, no sigmoid)
+//   label_w          [64][256] f32 + bias [64]           the label FiLM field's head (label_dim 64), else absent
+//   rgb_img          [4 chunks][64 rows][64 k] f16 swizzled, 32 KB = one ring slot of the wgmma kernel
+//   label_img        the same for the label head
+// The trunk-head image carries sigma in ROW 0 (no label rows), so that the trunk-only launches (density, GUARD
+// refinement) run the plain kernels on fn_trunk_view(L) -- label_dim 0, sigma at row / column 0.  The label FiLM
+// field's 32-row label image (FnLabelFilm::img) is not allocated.  fn_head_view(L, fh) is the FnLayout the
+// feature-head instantiations get: rgb_w / label_w point at the 64-row copies.
+//
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
 // matched on the B side by (W_hi, W_hi, W_lo) so that hi*hi + lo*hi + hi*lo reproduces an
@@ -71,21 +82,36 @@ struct FnLabelFilm {
     size_t img;             // label-head image (see above)
 };
 
+// The 64-wide heads of a FENERF_FIELD_FEATURE_HEAD field (all zero for other fields).
+constexpr int FN_FEAT = 64;             // feature-head width (and the label head's of the label FiLM variant)
+constexpr size_t FN_FEAT_IMG_BYTES = (size_t)(FN_H / FN_KCHUNK) * FN_FEAT * FN_KCHUNK * 2;   // 32 KB
+struct FnFeatureHead {
+    int32_t on;
+    size_t rgb_w, label_w;     // [64][256] f32 + [64] bias; label_w 0 without the label FiLM branch
+    size_t rgb_img, label_img; // [4][64 rows][64 k] f16 swizzled; label_img 0 without the label FiLM branch
+};
+
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Returns 0 and fills `L` (and `lf` if given), -2 if the flags hold an unknown bit, or -1 if the description is
-// outside what the kernels support.
-static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabelFilm* lf = nullptr) {
+// Returns 0 and fills `L` (and `lf` / `fh` if given), -2 if the flags hold an unknown bit, -3 if they ask for a
+// feature head on a field shape no reference class has, or -1 if the description is outside what the kernels support.
+static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabelFilm* lf = nullptr, FnFeatureHead* fh = nullptr) {
     if (!f || !L) return -1;
-    if (f->reserved & ~FENERF_FIELD_LABEL_FILM) return -2;
+    if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD)) return -2;
     const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
+    const int feature_head = (f->reserved & FENERF_FIELD_FEATURE_HEAD) ? 1 : 0;
+    if (feature_head) {
+        // SPATIALSIRENBASELINEHD (label_dim 0) and SPATIALSIRENSEMANTICHD (label FiLM, label_dim 64), no grid
+        if (f->grid_channels != 0 || f->label_dim != (label_film ? FN_FEAT : 0)) return -3;
+        if (f->out_dim != f->label_dim + FN_FEAT + 1) return -1;
+    }
     if (label_film && (f->label_dim < 1 || f->color_layers + 1 > FN_MAX_HIDDEN - (FENERF_MAX_TRUNK - 1))) return -1;
     if (f->trunk_layers < 2 || f->trunk_layers > FENERF_MAX_TRUNK) return -1;
     if (f->color_layers < 1 || f->color_layers > FENERF_MAX_COLOR) return -1;
-    if (f->label_dim < 0 || f->label_dim > FENERF_MAX_LABEL) return -1;
+    if (f->label_dim < 0 || f->label_dim > (feature_head ? FN_FEAT : FENERF_MAX_LABEL)) return -1;
     if (!(f->grid_channels == 0 || f->grid_channels == 32)) return -1;
     if (f->grid_channels && (f->grid_res < 2 || f->grid_res > 512)) return -1;
-    if (f->out_dim != f->label_dim + 4) return -1;
+    if (!feature_head && f->out_dim != f->label_dim + 4) return -1;
     L->trunk_hidden = f->trunk_layers - 1;
     L->n_hidden = L->trunk_hidden + label_film + f->color_layers;
     L->n_film = f->trunk_layers + label_film + f->color_layers;
@@ -119,10 +145,36 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabe
     L->grid = take(f->grid_channels ? r * r * r * (size_t)f->grid_channels * 4 : 4);
     L->grid16 = take(f->grid_channels ? r * r * r * (size_t)f->grid_channels * 2 : 4);
     FnLabelFilm lab = {label_film, label_film ? L->trunk_hidden : 0, 0};
-    if (label_film) lab.img = take((size_t)(FN_H / FN_KCHUNK) * 32 * FN_KCHUNK * 2);
+    if (label_film && !feature_head) lab.img = take((size_t)(FN_H / FN_KCHUNK) * 32 * FN_KCHUNK * 2);
     if (lf) *lf = lab;
+    FnFeatureHead hd = {feature_head, 0, 0, 0, 0};
+    if (feature_head) {
+        hd.rgb_w = take((size_t)(FN_FEAT * FN_H + FN_FEAT) * 4);
+        if (label_film) hd.label_w = take((size_t)(FN_FEAT * FN_H + FN_FEAT) * 4);
+        hd.rgb_img = take(FN_FEAT_IMG_BYTES);
+        if (label_film) hd.label_img = take(FN_FEAT_IMG_BYTES);
+    }
+    if (fh) *fh = hd;
     L->total = off;
     return 0;
+}
+
+// What the trunk-only launches (density, GUARD refinement) of a feature-head field see: no label rows, so the
+// density sits at row / column 0 of the trunk head, as packed.  Any other field passes through unchanged.
+static inline FnLayout fn_trunk_view(const FnLayout& L, const FnFeatureHead& fh) {
+    FnLayout t = L;
+    if (fh.on) t.label_dim = 0;
+    return t;
+}
+
+// The layout the feature-head kernel instantiations get: the fp32 head copies are the 64-row ones.
+static inline FnLayout fn_head_view(const FnLayout& L, const FnFeatureHead& fh) {
+    FnLayout t = L;
+    if (fh.on) {
+        t.rgb_w = fh.rgb_w;
+        if (fh.label_w) t.label_w = fh.label_w;
+    }
+    return t;
 }
 
 // Byte offset of element (row, k) inside one [rows][64] f16 image with the wgmma/TMA 128-byte

@@ -154,6 +154,20 @@ __global__ void pack_label_film_head_kernel(const float* __restrict__ w, const f
     if (threadIdx.x == 0) lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] = 1.f;
 }
 
+// a 64-wide head of a feature-head field (one block): fp32 copy [64][256] + bias [64], and its image
+// [4 chunks][64 rows][64 k] f16 swizzled
+__global__ void pack_feature_head_kernel(const float* __restrict__ w, const float* __restrict__ b, float* __restrict__ lw,
+                                         unsigned char* __restrict__ img) {
+    for (int i = threadIdx.x; i < FN_FEAT * FN_H; i += blockDim.x) {
+        const int row = i / FN_H, k = i % FN_H;
+        const float v = w[i];
+        lw[i] = v;
+        unsigned char* chunk = img + (size_t)(k / FN_KCHUNK) * (FN_FEAT * FN_KCHUNK * 2);
+        *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
+    }
+    if (threadIdx.x < FN_FEAT) lw[FN_FEAT * FN_H + threadIdx.x] = b[threadIdx.x];
+}
+
 // head images for the wgmma kernel (one block):
 //   trunk head  [4][32 rows][64 k]: rows 0..label_rows-1 = Weff * scale, row L = sigma weights
 //               (label_rows = L, or 0 for a label FiLM field, whose label head has an image of its own)
@@ -236,8 +250,9 @@ __global__ void fingerprint_kernel(FpSegments seg, unsigned long long* __restric
 
 }  // namespace
 
-int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const fenerf_field_params* p, unsigned long long* out,
-                      cudaStream_t st) {
+int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const fenerf_field_params* p,
+                      unsigned long long* out, cudaStream_t st) {
+    const int rgb_rows = fh.on ? FN_FEAT : 3;
     FpSegments seg;
     seg.n = 0;
     auto add = [&](const float* ptr, unsigned long long count) {
@@ -248,7 +263,7 @@ int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const fenerf_fie
     for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? 3 : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
     add(p->sigma_w, FN_H); add(p->sigma_b, 1);
     for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (unsigned long long)(i == 0 ? L.kx + FN_H : FN_H) * FN_H); add(p->color_b[i], FN_H); }
-    add(p->rgb_w, 3 * FN_H); add(p->rgb_b, 3);
+    add(p->rgb_w, (unsigned long long)rgb_rows * FN_H); add(p->rgb_b, rgb_rows);
     if (L.label_dim > 0) {
         add(p->label_w[0], FN_H * FN_H); add(p->label_b[0], FN_H);
         add(p->label_w[1], FN_H * FN_H); add(p->label_b[1], FN_H);
@@ -261,8 +276,8 @@ int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const fenerf_fie
     return 0;
 }
 
-int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const fenerf_field_params* p,
-               void* packed_v, cudaStream_t st) {
+int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh,
+               const fenerf_field_params* p, void* packed_v, cudaStream_t st) {
     unsigned char* packed = static_cast<unsigned char*>(packed_v);
     FN_REQUIRE(p->trunk_w[0] && p->trunk_b[0], "trunk_w[0]/trunk_b[0] missing");
     pack_first_kernel<<<1, 256, 0, st>>>(p->trunk_w[0], p->trunk_b[0], (float*)(packed + L.first_w),
@@ -294,7 +309,15 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm&
     pack_heads_kernel<<<3, 256, 0, st>>>(p->sigma_w, p->sigma_b, p->rgb_w, p->rgb_b, (float*)(packed + L.sigma_w),
                                          (float*)(packed + L.rgb_w));
     FN_LAUNCH_OK("pack_heads_kernel");
-    if (lf.on) {             // no chain to pre-multiply: the head is one Linear
+    if (fh.on) {             // the 64-wide heads, in sections of their own (layout.h)
+        pack_feature_head_kernel<<<1, 256, 0, st>>>(p->rgb_w, p->rgb_b, (float*)(packed + fh.rgb_w), packed + fh.rgb_img);
+        FN_LAUNCH_OK("pack_feature_head_kernel");
+        if (lf.on) {
+            pack_feature_head_kernel<<<1, 256, 0, st>>>(p->label_w[2], p->label_b[2], (float*)(packed + fh.label_w),
+                                                        packed + fh.label_img);
+            FN_LAUNCH_OK("pack_feature_head_kernel");
+        }
+    } else if (lf.on) {      // no chain to pre-multiply: the head is one Linear
         pack_label_film_head_kernel<<<1, 256, 0, st>>>(p->label_w[2], p->label_b[2], L.label_dim, (float*)(packed + L.label_w),
                                                        packed + lf.img);
         FN_LAUNCH_OK("pack_label_film_head_kernel");
@@ -310,7 +333,8 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm&
         label_step3_kernel<<<1, 256, 0, st>>>((float*)(packed + L.label_w), L.label_dim);
         FN_LAUNCH_OK("label_step3_kernel");
     }
-    pack_head_imgs_kernel<<<1, 256, 0, st>>>((const float*)(packed + L.label_w), L.label_dim, lf.on ? 0 : L.label_dim,
+    // (a feature-head field: no label rows, sigma in row 0 -- layout.h)
+    pack_head_imgs_kernel<<<1, 256, 0, st>>>((const float*)(packed + L.label_w), fh.on ? 0 : L.label_dim, lf.on ? 0 : L.label_dim,
                                              p->sigma_w, p->rgb_w,
                                              packed + L.head_img, packed + L.rgb_img);
     FN_LAUNCH_OK("pack_head_imgs_kernel");

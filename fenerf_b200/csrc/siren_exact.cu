@@ -22,6 +22,11 @@
 // goes through the weight-slab buffer instead, which is free between layers: one 64-feature quarter at a time, each
 // followed by its share of the label head's k-sum (the running sums sit in the same buffer), so shared memory and
 // occupancy stay those of the other fields.
+//
+// Feature-head fields (kFeatureHead, FENERF_FIELD_FEATURE_HEAD): the colour head is 64 linear outputs (no sigmoid) and
+// the label FiLM branch's head 64 rows; both are ordered fp32 k-sums like the 3- / label_dim-row heads.  The label
+// activations (64 x TM) and the 64 running sums fill the weight-slab buffer exactly.  The kernel gets
+// fn_head_view(L): rgb_w / label_w are the 64-row copies.
 #include "siren_common.cuh"
 #include "sm90.cuh"
 
@@ -164,7 +169,7 @@ __device__ __forceinline__ float grid_feature(const float* __restrict__ grid, in
     return out;
 }
 
-template <bool kGather, int P, bool kLabelFilm = false>
+template <bool kGather, int P, bool kLabelFilm = false, bool kFeatureHead = false>
 __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned char* smem_raw) {
     constexpr int TM = 16 * P;
     Smem<P>& s = *reinterpret_cast<Smem<P>*>(smem_raw);
@@ -273,7 +278,8 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                 if (a.sigma_only) break;          // the colour branch does not feed the density
                 if constexpr (kLabelFilm) {
                     // ---- label FiLM layer (hidden layer l) on the trunk output, then the label head ----
-                    static_assert(sizeof(s.W) >= (64 + FENERF_MAX_LABEL) * TM * sizeof(float), "label scratch fits the slab buffer");
+                    constexpr int kLabelRows = kFeatureHead ? FN_FEAT : FENERF_MAX_LABEL;   // bias offset of the head copy
+                    static_assert(sizeof(s.W) >= (64 + kLabelRows) * TM * sizeof(float), "label scratch fits the slab buffer");
                     init_bias(reinterpret_cast<const float*>(pk + L.hid_b[l]), acc, tid);
                     gemm_tile(s, reinterpret_cast<const float*>(pk + L.hid_w32[l]), FN_H, acc, tid);   // ends in a barrier
                     // the slab buffer: [64 features][TM points] of label activations, then the running sums [label][TM]
@@ -301,7 +307,7 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                         for (int it = tid; it < n_items; it += NTHREADS) {
                             const int pt = it % TM, o = it / TM;
                             const float* w = lw + (size_t)o * FN_H + 64 * j;
-                            float r = j == 0 ? __ldg(lw + FENERF_MAX_LABEL * FN_H + o) : sums[it];   // bias first
+                            float r = j == 0 ? __ldg(lw + kLabelRows * FN_H + o) : sums[it];   // bias first
 #pragma unroll 8
                             for (int k = 0; k < 64; ++k) r = fmaf(lab[k * TM + pt], __ldg(w + k), r);
                             sums[it] = r;
@@ -322,14 +328,15 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
             film_store(s, a.film, L.n_film, l + 1, acc, tid);
             __syncthreads();
         }
-        // ---- rgb head: sigmoid(Linear(256 -> 3)) ----
+        // ---- rgb head: sigmoid(Linear(256 -> 3)); a feature head: Linear(256 -> 64) ----
         if (!a.sigma_only) {
+            constexpr int kRgb = kFeatureHead ? FN_FEAT : 3;
             const float* rw = reinterpret_cast<const float*>(pk + L.rgb_w);
-            for (int it = tid; it < TM * 3; it += NTHREADS) {
+            for (int it = tid; it < TM * kRgb; it += NTHREADS) {
                 int pt = it % TM, o = it / TM;
-                float r = __ldg(rw + 3 * FN_H + o);
+                float r = __ldg(rw + kRgb * FN_H + o);
                 for (int k = 0; k < FN_H; ++k) r = fmaf(s.A[k][pt], __ldg(rw + o * FN_H + k), r);
-                r = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-r)));
+                if (!kFeatureHead) r = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-r)));
                 long long flat = s.flat[pt];
                 if (flat >= 0) a.out[flat * C + L.label_dim + o] = r;
             }
@@ -338,10 +345,10 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
     }
 }
 
-template <bool kGather, int P, bool kLabelFilm>
+template <bool kGather, int P, bool kLabelFilm, bool kFeatureHead = false>
 __global__ void __launch_bounds__(NTHREADS, 2) siren_exact_kernel(ExactArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    siren_exact_body<kGather, P, kLabelFilm>(a, smem_raw);
+    siren_exact_body<kGather, P, kLabelFilm, kFeatureHead>(a, smem_raw);
 }
 
 // GUARD refinement: the list length is only known on the device.  Short lists (small renders; fields whose densities
@@ -357,13 +364,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_exact_guard_kernel(ExactArg
 
 }  // namespace
 
-int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const unsigned char* packed, const float* points,
-                       const float* dirs, const float* film, int batch, long long ppb, int dir_group, int lock_dirs,
-                       const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only) {
+int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
+                       const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
+                       int lock_dirs, const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only) {
     static_assert(sizeof(Smem<4>) <= 113 * 1024, "two CTAs per SM must fit");
     constexpr int TM = 64;
     ExactArgs a;
-    a.L = L; a.packed = packed; a.points = points; a.dirs = dirs; a.film = film; a.only_idx = only_idx; a.out = out;
+    // (a feature-head field: the 64-row head copies for its own instantiations, no label rows for the density alone)
+    const bool feature_head = fh.on && !sigma_only;
+    a.L = feature_head ? fn_head_view(L, fh) : fn_trunk_view(L, fh);
+    a.packed = packed; a.points = points; a.dirs = dirs; a.film = film; a.only_idx = only_idx; a.out = out;
     a.n_only_dev = nullptr; a.guard_stats = nullptr;
     a.ppb = ppb; a.n_only = n_only; a.dir_group = dir_group < 1 ? 1 : dir_group; a.lock_dirs = lock_dirs;
     a.sigma_only = sigma_only ? 1 : 0;
@@ -383,7 +393,10 @@ int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const unsigned 
     };
     const bool label_film = lf.on && !sigma_only;
     int e;
-    if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true>) : launch(siren_exact_kernel<true, 4, false>);
+    if (feature_head) {
+        if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true, true>) : launch(siren_exact_kernel<true, 4, false, true>);
+        else e = label_film ? launch(siren_exact_kernel<false, 4, true, true>) : launch(siren_exact_kernel<false, 4, false, true>);
+    } else if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true>) : launch(siren_exact_kernel<true, 4, false>);
     else e = label_film ? launch(siren_exact_kernel<false, 4, true>) : launch(siren_exact_kernel<false, 4, false>);
     if (e) return e;
     FN_LAUNCH_OK("siren_exact_kernel");

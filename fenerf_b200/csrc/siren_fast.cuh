@@ -29,8 +29,14 @@
 // through the FiLM epilogue into `nxt` and straight into the m64n32 label head (k-slices 8h .. 8h+7), so the label
 // activations never need more than those 32 registers: four turns, [layer half 0] [head on it] [layer half 1] [head].
 //
-// The kernel is a template over the label FiLM branch; its two instantiations live in two translation units
-// (siren_fast.cu, siren_fast_label.cu), so that the plain one compiles exactly as it does on its own.
+// Feature-head fields (FENERF_FIELD_FEATURE_HEAD, the kFeatureHead instantiations): the colour head is m64n64 on the
+// colour activations, 64 linear outputs with their bias and no sigmoid; the label FiLM variant's head is m64n64 too, with
+// the same turn sequence.  Each head image is [4 chunks][64 rows][64 k], one 32 KB ring slot.  The trunk head carries
+// sigma only, in column 0.  The kernel gets fn_head_view(L): rgb_w / label_w are the 64-row fp32 copies (for the biases).
+//
+// The kernel is a template over the label FiLM branch and the feature head; the plain and the label FiLM
+// instantiations live in translation units of their own (siren_fast.cu, siren_fast_label.cu), the two feature-head
+// ones in a third (siren_fast_hd.cu), so that the plain one compiles exactly as it does on its own.
 #pragma once
 #include "common.cuh"
 #include "siren_common.cuh"
@@ -59,6 +65,7 @@ constexpr int MAX_LOADS = 72;
 constexpr uint32_t CHUNK = 16384;                   // one [128 rows][64 k] f16 image chunk
 constexpr uint32_t HEAD_CHUNK = 32 * 128;           // one [32 rows][64 k] chunk of the trunk-head image
 constexpr uint32_t RGB_CHUNK = 8 * 128;             // one [8 rows][64 k] chunk of the rgb-head image
+constexpr uint32_t FEAT_CHUNK = FN_FEAT * 128;      // one [64 rows][64 k] chunk of a feature-head field's head image
 
 struct Load {
     uint32_t src;      // byte offset in the packed buffer
@@ -82,7 +89,7 @@ struct FastArgs {
 
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-template <bool kLabelFilm>
+template <bool kLabelFilm, bool kFeatureHead = false>
 __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_constant__ FastArgs a) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
@@ -325,9 +332,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                         for (int e = 0; e < 2; ++e) {
                             const int o = 8 * i + 2 * q + e;
                             const float v = dh[4 * i + 2 * rr + e];
-                            if (o < L.label_dim) {         // (zero rows for a label FiLM field: its labels come below)
+                            if (!kFeatureHead && o < L.label_dim) {   // (zero rows for a label FiLM field: its labels come below)
                                 if (!kLabelFilm && !a.sigma_only) a.out[flat * C + o] = fmaf(v, inv_scale, __ldg(lb + o));
-                            } else if (o == L.label_dim) {
+                            } else if (o == (kFeatureHead ? 0 : L.label_dim)) {   // a feature-head field: sigma in row 0
                                 const float sig = v + __ldg(sigma_w + FN_H);
                                 a.out[flat * C + (C - 1)] = sig;
                                 if (a.sigma_out) a.sigma_out[flat] = sig;
@@ -337,7 +344,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 if (a.sigma_only) { stop = true; break; }
                 if constexpr (kLabelFilm) {
                     // ---- label FiLM layer (hidden layer l) on the trunk activations, and the label head ----
-                    float dl[16];
+                    constexpr int kLabN = kFeatureHead ? FN_FEAT : 32;              // head columns (m64n64 / m64n32)
+                    constexpr uint32_t kLabChunk = kFeatureHead ? FEAT_CHUNK : HEAD_CHUNK;
+                    float dl[kLabN / 2];
                     uint32_t slot_h = 0, w_h = 0;
                     const float* fs = nullptr;
 #pragma unroll
@@ -369,7 +378,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                         for (int s = 0; s < 8; ++s) {
                             const int g = 8 * h + s;
-                            mma_rs_n32(dl, nxt[s], desc_kmajor(w_h + (g >> 2) * HEAD_CHUNK + 32 * (g & 3)), (h | s) ? 1u : 0u);
+                            const uint64_t desc = desc_kmajor(w_h + (g >> 2) * kLabChunk + 32 * (g & 3));
+                            if constexpr (kFeatureHead) mma_rs_n64(dl, nxt[s], desc, (h | s) ? 1u : 0u);
+                            else mma_rs_n32(dl, nxt[s], desc, (h | s) ? 1u : 0u);
                         }
                         wg_commit();
                         turn_end();
@@ -384,12 +395,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                         const long long pnt = p0 + r0 + 8 * rr;
                         if (pnt >= a.ppb) continue;
                         const long long flat = b * a.ppb + pnt;
+                        const float* lbias = kFeatureHead ? label_w + FN_FEAT * FN_H : lb;
 #pragma unroll
-                        for (int i = 0; i < 4; ++i)
+                        for (int i = 0; i < kLabN / 8; ++i)
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int o = 8 * i + 2 * q + e;
-                                if (o < L.label_dim) a.out[flat * C + o] = dl[4 * i + 2 * rr + e] + __ldg(lb + o);
+                                if (o < L.label_dim) a.out[flat * C + o] = dl[4 * i + 2 * rr + e] + __ldg(lbias + o);
                             }
                     }
                     continue;                        // act still holds the trunk output: the colour layers follow
@@ -445,6 +457,38 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         }
         if (stop) continue;
 
+        // ---- feature head: A . rgb^T + b, 64 columns, no sigmoid ----
+        if constexpr (kFeatureHead) {
+            float dr[32];
+            uint32_t slot;
+            const uint32_t w = acquire(slot);
+            turn_begin();
+            wg_fence();
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+#pragma unroll
+                for (int k = 0; k < 4; ++k) mma_rs_n64(dr, act[4 * c + k], desc_kmajor(w + c * FEAT_CHUNK + 32 * k), (c | k) ? 1u : 0u);
+            wg_commit();
+            turn_end();
+            wg_wait<0>();
+            fence_regs(dr);
+            fence_regs(act);
+            release(slot);
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const long long pnt = p0 + r0 + 8 * rr;
+                if (pnt >= a.ppb) continue;
+                const long long flat = b * a.ppb + pnt;
+#pragma unroll
+                for (int i = 0; i < 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int o = 8 * i + 2 * q + e;
+                        a.out[flat * C + L.label_dim + o] = dr[4 * i + 2 * rr + e] + __ldg(rgb_w + FN_FEAT * FN_H + o);
+                    }
+            }
+            continue;
+        }
         // ---- rgb head: sigmoid(A . rgb^T + b), 8 columns of which 3 are used ----
         {
             float dr[4];

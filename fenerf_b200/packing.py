@@ -37,7 +37,9 @@ class PackedField:
 def field_desc(spec) -> "_lib.FieldDesc":
     return _lib.FieldDesc(trunk_layers=spec.trunk_layers, color_layers=spec.color_layers, label_dim=spec.label_dim,
                           grid_channels=spec.grid_channels, grid_res=spec.grid_res, out_dim=spec.out_dim,
-                          input_scale=spec.input_scale, reserved=_lib.FIELD_LABEL_FILM if spec.label_film else 0)
+                          input_scale=spec.input_scale,
+                          reserved=(_lib.FIELD_LABEL_FILM if spec.label_film else 0)
+                          | (_lib.FIELD_FEATURE_HEAD if spec.feature_head else 0))
 
 
 def _f32(t, device):

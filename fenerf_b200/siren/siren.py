@@ -149,7 +149,9 @@ class FieldSpec:
                    (siren/siren.py:663-665); its FiLM row sits between the trunk's and the colour branch's
     grid_channels  feature-grid channels (0 = no grid)
     input_scale    UniformBoxWarp factor applied to the position before the trunk and the grid
-    out_dim        label_dim + 3 (rgb) + 1 (sigma); channel order [labels, rgb, sigma]
+    feature_head   the colour head is Linear(256 -> 64) without the sigmoid: 64 features for a neural renderer
+                   (siren/siren.py:300-301, 1365-1366)
+    out_dim        label_dim + 3 (rgb; 64 features with feature_head) + 1 (sigma); channel order [labels, rgb, sigma]
     """
     trunk_layers: int
     color_layers: int
@@ -160,6 +162,11 @@ class FieldSpec:
     out_dim: int
     double_latent: bool
     label_film: bool = False
+    feature_head: bool = False
+
+    @property
+    def rgb_dim(self):
+        return 64 if self.feature_head else 3
 
 
 def _fused_mapping_ok(net, z):
@@ -399,6 +406,72 @@ class SPATIALSIRENSEMANTIC(TALLSIREN):
 
     def film_rows(self):
         return len(self.network) + 2             # trunk, label, colour (siren.py:656-668)
+
+
+class SPATIALSIRENBASELINEHD(TALLSIREN):
+    """SPATIALSIRENBASELINE with a 64-feature colour head and no sigmoid (siren/siren.py:247-302), the field of a
+    neural-renderer generator: output channels [features (64), sigma (1)] whatever `output_dim` says."""
+
+    def __init__(self, input_dim=2, z_dim=100, hidden_dim=256, output_dim=1, device=None):
+        nn.Module.__init__(self)
+        self.device = device
+        self.input_dim = input_dim
+        self.z_dim = z_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+
+        widths = [3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        self.final_layer = nn.Linear(hidden_dim, 1)
+        self.color_layer_sine = FiLMLayer(hidden_dim + 3, hidden_dim)
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 64))
+        self.mapping_network = CustomMappingNetwork(z_dim, 256, (len(self.network) + 1) * hidden_dim * 2)
+
+        for part in (self.network, self.final_layer, self.color_layer_sine, self.color_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(first_layer_film_sine_init)
+        self.gridwarper = UniformBoxWarp(0.24)
+
+    def field_spec(self):
+        return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=0, grid_channels=0, grid_res=0,
+                         input_scale=float(self.gridwarper.scale_factor), out_dim=65, double_latent=False,
+                         feature_head=True)
+
+
+class SPATIALSIRENSEMANTICHD(SPATIALSIRENSEMANTIC):
+    """SPATIALSIRENSEMANTIC with 64-wide heads (siren/siren.py:1301-1367): Linear(256 -> 64) label head and a 64-feature
+    colour head without the sigmoid.  FiLM rows: trunk 0..7, label 8, colour 9; output channels [labels (64),
+    features (64), sigma (1)] whatever `output_dim` says."""
+
+    def __init__(self, input_dim=2, z_dim=100, hidden_dim=256, output_dim=1, device=None):
+        nn.Module.__init__(self)
+        self.device = device
+        self.input_dim = input_dim
+        self.z_dim = z_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+        self.max_batch_size = 2500
+
+        widths = [3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        self.final_layer = nn.Linear(hidden_dim, 1)
+        self.label_layer_sine = FiLMLayer(hidden_dim, hidden_dim)
+        self.label_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 64))
+        self.color_layer_sine = FiLMLayer(hidden_dim + 3, hidden_dim)
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 64))
+        self.mapping_network = CustomMappingNetwork(z_dim, 256, (len(self.network) + 2) * hidden_dim * 2)
+
+        for part in (self.network, self.final_layer, self.label_layer_sine, self.label_layer_linear,
+                     self.color_layer_sine, self.color_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(first_layer_film_sine_init)
+        self.activation = nn.Softmax(dim=-1)     # unused, as in the reference
+        self.gridwarper = UniformBoxWarp(0.24)
+
+    def field_spec(self):
+        return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=64, grid_channels=0, grid_res=0,
+                         input_scale=float(self.gridwarper.scale_factor), out_dim=129, double_latent=False,
+                         label_film=True, feature_head=True)
 
 
 class _DoubleLatentField(_FieldBase):

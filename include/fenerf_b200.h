@@ -56,6 +56,11 @@ extern "C" {
  *                                trunk 8, color 3, label 18, grid 32 x 96^3, scale 2/0.24, out 22.
  * SPATIALSIRENSEMANTIC (siren.py:597-671):
  *                                trunk 8, color 1, label 19 (FENERF_FIELD_LABEL_FILM), grid 0, scale 2/0.24, out 23.
+ * With FENERF_FIELD_FEATURE_HEAD the colour head is Linear(256->64) without the sigmoid: 64 features for a
+ * neural renderer, out = [labels, feat(64), sigma]:
+ * SPATIALSIRENBASELINEHD (siren.py:247-302):  trunk 8, color 1, label 0, grid 0, scale 2/0.24, out 65.
+ * SPATIALSIRENSEMANTICHD (siren.py:1301-1367): trunk 8, color 1, label 64 (FENERF_FIELD_LABEL_FILM), grid 0,
+ *                                scale 2/0.24, out 129.
  * The hidden width is fixed at 256.                                                            */
 #define FENERF_MAX_TRUNK 8
 #define FENERF_MAX_COLOR 8
@@ -66,14 +71,19 @@ extern "C" {
 #define FENERF_FIELD_LABEL_FILM 0x1   /* the label head is FiLM(256->256) then Linear(256->label_dim) on the trunk
                                          output; label_dim >= 1 and color_layers <= 7 (the packed layout holds 15
                                          256-wide layers after the first: 7 trunk + 1 label + the colour layers) */
+#define FENERF_FIELD_FEATURE_HEAD 0x8 /* the colour head is Linear(256->64) with no sigmoid (rgb_w [64][256], rgb_b [64]);
+                                         out_dim = label_dim + 64 + 1.  Only the reference's two shapes are accepted:
+                                         label_dim 0 without other flags (SPATIALSIRENBASELINEHD), or label_dim 64 with
+                                         FENERF_FIELD_LABEL_FILM (SPATIALSIRENSEMANTICHD; label_w[2] [64][256]); no grid.
+                                         Anything else with this bit is FENERF_E_UNSUPPORTED. */
 
 typedef struct fenerf_field_desc {
     int32_t trunk_layers;   /* 2..8 */
     int32_t color_layers;   /* 1..8 */
-    int32_t label_dim;      /* 0..32 */
+    int32_t label_dim;      /* 0..32; 64 with FENERF_FIELD_FEATURE_HEAD */
     int32_t grid_channels;  /* 0 or 32 */
     int32_t grid_res;       /* cubic grid side (D = H = W), 0 if no grid */
-    int32_t out_dim;        /* label_dim + 4 */
+    int32_t out_dim;        /* label_dim + 4; label_dim + 65 with FENERF_FIELD_FEATURE_HEAD (at most 129) */
     float   input_scale;
     int32_t reserved;       /* flags: FENERF_FIELD_* bits, 0 = a plain field */
 } fenerf_field_desc;
@@ -87,8 +97,8 @@ typedef struct fenerf_field_params {
     const float* sigma_b;                    /* [1] */
     const float* color_w[FENERF_MAX_COLOR];  /* first [256][3+G+256] (cat order dir, feat, x), rest [256][256] */
     const float* color_b[FENERF_MAX_COLOR];
-    const float* rgb_w;                      /* [3][256] */
-    const float* rgb_b;                      /* [3] */
+    const float* rgb_w;                      /* [3][256]; FENERF_FIELD_FEATURE_HEAD: [64][256] */
+    const float* rgb_b;                      /* [3]; FENERF_FIELD_FEATURE_HEAD: [64] */
     const float* label_w[3];                 /* [256][256], [256][256], [label_dim][256]; NULL if label_dim == 0;
                                                 label_w[1] / label_b[1] NULL for a two-layer chain (siren.py:1189-1191);
                                                 FENERF_FIELD_LABEL_FILM: [0] the label FiLM layer [256][256], [1] NULL,
@@ -213,7 +223,7 @@ int fenerf_ray_setup(const fenerf_render_desc* rd, const float* x_lin, const flo
 /* Coarse weights + inverse-CDF resampling + fine points.
  * Replaces fancy_integration(coarse) -> weights, the resample prep and sample_pdf
  * (generators/generators.py:59-74; volumetric_rendering.py:18-38, 259-300).
- *   raw_coarse (B,N,S,C) (sigma = last channel); z_vals (B,N,S)
+ *   raw_coarse (B,N,S,C) (sigma = last channel, 2 <= C <= 129); z_vals (B,N,S)
  *   rng_noise (B,N,S) normal draw #4 or NULL (treated as 0; required if noise_std != 0)
  *   rng_u (B*N,S) uniform draw #5
  * out: z_fine (B,N,S); points_fine (B,N,S,3); inds (B*N,S) int64 searchsorted result or NULL */
@@ -225,6 +235,8 @@ int fenerf_resample(const fenerf_render_desc* rd, int32_t out_dim, const float* 
 /* Merge-sort of coarse + fine samples, alpha compositing, fill modes, NCHW epilogue.
  * Replaces cat/sort/gather (generators/generators.py:85-89), the final fancy_integration
  * (volumetric_rendering.py:18-106) and the softmax / permute / *2-1 epilogue (:97-104).
+ *   out_dim C: 2..129 (up to 32 one thread or four per ray; wider fields -- the feature-head fields' 65 / 129 --
+ *              one warp per ray, each lane owning every 32nd channel)
  *   raw_fine / z_fine may be NULL when !hierarchical
  *   rng_noise (B,N,S') normal draw #6 (S' = 2S if hierarchical) or NULL
  * out: pixels (B, C_img, H, W) already *2-1, C_img = C-1 (+1 for the seg_padding fill modes)
@@ -349,7 +361,8 @@ int fenerf_gemm_tn_f16(const void* X, const void* Y, int32_t batch, int64_t poin
 
 /* d pixels (B, C-1, H, W) -> d raw outputs.  Backward of the merge + fancy_integration + softmax / *2-1
  * epilogue (generators.py:85-104, volumetric_rendering.py:18-50); same arguments as fenerf_composite.
- * d_raw_fine / raw_fine / z_fine NULL when !hierarchical.  fill modes are staged_forward-only (no_grad). */
+ * d_raw_fine / raw_fine / z_fine NULL when !hierarchical.  fill modes are staged_forward-only (no_grad).
+ * out_dim 2..129 as fenerf_composite. */
 int fenerf_composite_backward(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse,
                               const float* z_coarse, const float* raw_fine, const float* z_fine,
                               const float* rng_noise, const float* d_pixels,
@@ -370,7 +383,10 @@ int fenerf_gate_backward(void* dA, const void* gate, int64_t n_points, int64_t p
                          int32_t dtype, void* stream);
 
 /* d raw (n_points, C) -> scaled head gradients of `dtype`: d_heads (n_points, 32) = [d labels.., d sigma, 0..],
- * d_rgb (n_points, 8) = [d rgb * rgb (1 - rgb), 0..]; `scale` is a DEVICE scalar (power of two). */
+ * d_rgb (n_points, 8) = [d rgb * rgb (1 - rgb), 0..]; `scale` is a DEVICE scalar (power of two).
+ * Feature-head layout (out_dim == label_dim + 65, label_dim 0 or 64; FENERF_FIELD_FEATURE_HEAD): d_heads
+ * (n_points, label_dim + 8) = [d labels.., d sigma, 0..], d_rgb (n_points, 64) = d feat (linear head: no sigmoid
+ * factor), both scaled. */
 int fenerf_head_grads(const float* d_raw, const float* raw, int64_t n_points, int32_t out_dim, int32_t label_dim,
                       const float* scale, void* d_heads, void* d_rgb, int32_t dtype, void* stream);
 
