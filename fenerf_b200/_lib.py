@@ -30,7 +30,8 @@ EXPORTS = (
     "fenerf_field_fingerprint", "fenerf_composite_backward", "fenerf_film_forward_stash", "fenerf_gate_backward",
     "fenerf_head_grads", "fenerf_extras_gather", "fenerf_grid_scatter_add", "fenerf_grid_unpack_grad",
     "fenerf_workspace_layout", "fenerf_mask2color", "fenerf_frames_to_u8", "fenerf_mapping_film",
-    "fenerf_guard_stats", "fenerf_debug_stage_times", "fenerf_gemm_nt_f16", "fenerf_gemm_nt_film", "fenerf_gemm_tn_f16",
+    "fenerf_guard_stats", "fenerf_debug_stage_times", "fenerf_debug_fast_variant", "fenerf_debug_soft_sine",
+    "fenerf_gemm_nt_f16", "fenerf_gemm_nt_film", "fenerf_gemm_tn_f16",
 )
 
 
@@ -121,6 +122,10 @@ def _declare(lib):
     lib.fenerf_gemm_tn_f16.argtypes = [vp, vp, i32, i64, i32, vp, vp, vp]
     lib.fenerf_debug_stage_times.restype = C.c_int
     lib.fenerf_debug_stage_times.argtypes = [i32, vp]
+    lib.fenerf_debug_fast_variant.restype = C.c_int
+    lib.fenerf_debug_fast_variant.argtypes = [i32, vp, i32]
+    lib.fenerf_debug_soft_sine.restype = C.c_int
+    lib.fenerf_debug_soft_sine.argtypes = [vp, vp, i64, vp]
     lib.fenerf_guard_stats.restype = C.c_int
     lib.fenerf_guard_stats.argtypes = [vp, P(GuardReport), vp]
     lib.fenerf_mapping_film.restype = C.c_int

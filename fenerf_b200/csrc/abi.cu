@@ -210,6 +210,15 @@ int fenerf_debug_stage_times(int32_t enable, float* ms_out) {
     return 0;
 }
 
+int fenerf_debug_fast_variant(int32_t variant, void* trace, int32_t trace_ctas) {
+    return siren_fast_debug_variant(variant, static_cast<unsigned long long*>(trace), trace_ctas);
+}
+
+int fenerf_debug_soft_sine(const float* a, float* out, int64_t n, void* stream) {
+    FN_REQUIRE(a && out && n >= 0, "bad argument");
+    return soft_sine_eval(a, out, n, (cudaStream_t)stream);
+}
+
 int fenerf_guard_stats(const void* workspace, fenerf_guard_report* out, void* stream) {
     FN_REQUIRE(workspace && out, "NULL argument");
     int32_t raw[4];

@@ -111,6 +111,9 @@ int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureH
 int siren_points_fast(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
                       const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
                       int lock_dirs, float* out, int sigma_only, cudaStream_t st, float* sigma_out = nullptr);
+// debug: which instantiation siren_points_fast launches (0 production; siren_fast_debug.cu) and the device software sine
+int siren_fast_debug_variant(int variant, unsigned long long* trace, int trace_ctas);
+int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st);
 int guard_refine(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
                  const float* film, int batch, long long rays_per_batch, int num_steps, int lock_dirs, float tau,
                  const float* noise_far, long long noise_stride, float noise_std,

@@ -7,8 +7,15 @@ namespace fn {
 // FastArgs
 int siren_fast_label_launch(const void* args, int blocks, cudaStream_t st);
 int siren_fast_hd_launch(const void* args, int blocks, bool label_film, cudaStream_t st);
+// the debug instantiations (siren_fast_debug.cu): variant 1 = one column pair in four on the software sine, 2 / 3 = the
+// timeline of the production / the variant-1 kernel
+int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st);
 
 namespace {
+
+std::atomic<int> g_variant{0};
+unsigned long long* g_trace = nullptr;
+int g_trace_ctas = 0;
 
 // one tile's weight stream, in the order the consumers read it
 bool build_loads(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, FastArgs& A, bool sigma_only) {
@@ -45,6 +52,15 @@ bool build_loads(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& 
 
 }  // namespace
 
+int siren_fast_debug_variant(int variant, unsigned long long* trace, int trace_ctas) {
+    FN_REQUIRE(variant >= 0 && variant <= 3, "unknown point-network variant %d", variant);
+    FN_REQUIRE(variant < 2 || (trace && trace_ctas >= 1), "a timeline variant needs its trace buffer");
+    g_trace = trace;
+    g_trace_ctas = trace_ctas;
+    g_variant.store(variant);
+    return 0;
+}
+
 int siren_points_fast(const FnLayout& L_in, const FnLabelFilm& lf_in, const FnFeatureHead& fh_in, const unsigned char* packed,
                       const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
                       int lock_dirs, float* out, int sigma_only, cudaStream_t st, float* sigma_out) {
@@ -77,6 +93,11 @@ int siren_points_fast(const FnLayout& L_in, const FnLabelFilm& lf_in, const FnFe
     const long long n_pairs = (a.n_tiles + 1) / 2;
     static std::atomic<int> attr_set[kMaxDevices];
     const int blocks = (int)(n_pairs < (long long)num_sms() ? n_pairs : (long long)num_sms());
+    if (const int variant = g_variant.load()) {
+        a.trace = g_trace;
+        a.trace_ctas = g_trace_ctas;
+        return siren_fast_debug_launch(&a, blocks, lf.on != 0, fh.on != 0, variant, st);
+    }
     if (fh.on) return siren_fast_hd_launch(&a, blocks, lf.on != 0, st);
     if (lf.on) return siren_fast_label_launch(&a, blocks, st);
     FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<false>, attr_set, (int)SMEM_TOTAL));

@@ -4,9 +4,9 @@
 //   warps 0..3, 4..7   two consumer warpgroups; each evaluates the whole network for its own tile of 64 points
 //   warp 8             weight producer (its warpgroup gives its registers to the consumers): bulk copies of the packed weight images (layout.h) into a ring of six
 //                      32 KB slots, in the order the consumers read them; both warpgroups read every slot
-//   warps 9, 10        FiLM producers, one per consumer warpgroup: bulk copies of each layer's FiLM frequencies, phases
-//                      and bias (3 KB) into a two-entry ring of that warpgroup, so that the epilogue reads them from
-//                      shared memory
+//   warps 9, 10        FiLM producers, one per consumer warpgroup: each fills a two-entry ring of that warpgroup with
+//                      every layer's FiLM constants already folded, per column pair {f_c, f_c+1, f_c b_c + p_c, ...}
+//                      (2 KB, one LDS.128 per four epilogue elements), so that the epilogue does no f b + p
 //
 // A layer is D[64 points x 256] = A[64 x 256] . W^T with A in registers (wgmma m64n128k16, one feature half at a
 // time) and W from the ring.  The accumulator fragment of wgmma is the register A fragment of the next layer
@@ -36,7 +36,9 @@
 //
 // The kernel is a template over the label FiLM branch and the feature head; the plain and the label FiLM
 // instantiations live in translation units of their own (siren_fast.cu, siren_fast_label.cu), the two feature-head
-// ones in a third (siren_fast_hd.cu), so that the plain one compiles exactly as it does on its own.
+// ones in a third (siren_fast_hd.cu), so that the plain one compiles exactly as it does on its own.  The debug
+// instantiations -- a share of the sines on the FMA pipe (kSoftSin, soft_sinf) and the clock64 timeline (kTrace) -- live
+// in siren_fast_debug.cu.
 #pragma once
 #include "common.cuh"
 #include "siren_common.cuh"
@@ -56,7 +58,7 @@ constexpr uint32_t SLOT_BYTES = 32768;
 constexpr int XSTRIDE = 72;                         // f16 per point row of the input-slot staging buffer (144 B)
 constexpr uint32_t SMEM_X = RING * SLOT_BYTES;      // [2 warpgroups][64 points][XSTRIDE] f16
 constexpr int FRING = 2;                            // FiLM entries per consumer warpgroup
-constexpr uint32_t FILM_BYTES = 3 * FN_H * 4;       // one layer: [frequency 256][phase 256][bias 256] f32
+constexpr uint32_t FILM_BYTES = 2 * FN_H * 4;       // one layer: [128 column pairs] {f_c, f_c+1, f_c b_c + p_c, f_c+1 b_c+1 + p_c+1} f32
 constexpr uint32_t SMEM_FILM = SMEM_X + 2 * TILE * XSTRIDE * 2;   // [2 warpgroups][FRING] entries
 constexpr uint32_t SMEM_BAR = SMEM_FILM + 2 * FRING * FILM_BYTES;
 // full[RING], empty[RING], turn[2], film_full[2 * FRING], film_empty[2 * FRING]
@@ -66,6 +68,44 @@ constexpr uint32_t CHUNK = 16384;                   // one [128 rows][64 k] f16 
 constexpr uint32_t HEAD_CHUNK = 32 * 128;           // one [32 rows][64 k] chunk of the trunk-head image
 constexpr uint32_t RGB_CHUNK = 8 * 128;             // one [8 rows][64 k] chunk of the rgb-head image
 constexpr uint32_t FEAT_CHUNK = FN_FEAT * 128;      // one [64 rows][64 k] chunk of a feature-head field's head image
+// split of the epilogue's sines: column pairs j = kSoftSin - 1, 2 kSoftSin - 1, ... of the 16 per thread and half (one in
+// kSoftSin) take soft_sinf, the rest __sinf.  Production keeps every sine on the SFU (0): with one pair in four on the
+// FMA pipe the epilogue did not get shorter and the other warpgroup's MMA groups got longer (DESIGN section 5); the
+// split kernel is the debug variant kSoftSinSplit
+#ifndef FENERF_SOFT_SIN_EVERY
+#define FENERF_SOFT_SIN_EVERY 0
+#endif
+constexpr int kSoftSinEvery = FENERF_SOFT_SIN_EVERY;
+constexpr int kSoftSinSplit = 4;
+// timeline (kTrace): 64-bit events per traced warp, {kind 8 bits, group 8 bits, clock64 48 bits}
+constexpr int TRACE_CAP = 1024;
+constexpr int TRACE_WARPS = 11;
+enum TraceEvent {
+    TR_PAIR = 1, TR_TURN_WAIT, TR_TURN_DONE, TR_ACQ_WAIT, TR_ACQ_DONE, TR_COMMIT, TR_MMA_DONE, TR_EPI_DONE,
+    TR_FILM_WAIT, TR_FILM_DONE, TR_EMPTY_WAIT, TR_EMPTY_DONE,
+};
+// MMA group kinds (the group byte of TR_COMMIT)
+enum TraceGroup { TG_FIRST = 0, TG_HIDDEN, TG_COLOR0, TG_TRUNK_HEAD, TG_LABEL_LAYER, TG_LABEL_HEAD, TG_OUT_HEAD };
+
+// sin(a) on the FMA pipe.  a - n 2pi with n = rint(a / 2pi) (the 1.5 2^23 add rounds; Cody-Waite in two fused steps, so
+// the reduction costs one float32 rounding of r for |a| up to a few thousand), then r P(r^2), the odd degree-11
+// minimax fit of sin on [-pi (1 + 5e-4), pi (1 + 5e-4)] (tools/fit_soft_sine.py).  |soft_sinf(a) - sin(a)| <= 2^-20
+// (the polynomial 8.2e-8, its float32 evaluation 3.8e-7); sin.approx is 2^-20.9 on [-pi, pi] and loses the bits of
+// its own a / 2pi product beyond.  12 FMA-pipe instructions.
+__device__ __forceinline__ float soft_sinf(float a) {
+    const float k = fmaf(a, 0.159154943f, 12582912.f);
+    const float n = k - 12582912.f;
+    float r = fmaf(-n, 6.28318548f, a);
+    r = fmaf(-n, -1.74845553e-7f, r);
+    const float r2 = r * r;
+    float p = -2.041572245e-08f;
+    p = fmaf(p, r2, 2.701100129e-06f);
+    p = fmaf(p, r2, -1.980991656e-04f);
+    p = fmaf(p, r2, 8.332454599e-03f);
+    p = fmaf(p, r2, -1.666656137e-01f);
+    p = fmaf(p, r2, 9.999996424e-01f);
+    return r * p;
+}
 
 struct Load {
     uint32_t src;      // byte offset in the packed buffer
@@ -85,17 +125,30 @@ struct FastArgs {
     long long ppb, tiles_per_batch, n_tiles;
     int dir_group, lock_dirs;
     int sigma_only;             // the network stops after the trunk head; only out[..., C-1] is written
+    unsigned long long* trace;  // kTrace: [trace_ctas][TRACE_WARPS][TRACE_CAP] events of CTAs 0 .. trace_ctas - 1
+    int trace_ctas;
 };
 
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-template <bool kLabelFilm, bool kFeatureHead = false>
+template <bool kLabelFilm, bool kFeatureHead = false, int kSoftSin = kSoftSinEvery, bool kTrace = false>
 __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_constant__ FastArgs a) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * RING, bar_turn = bar_empty + 8 * RING;
     const uint32_t bar_ffull = bar_turn + 16, bar_fempty = bar_ffull + 8 * 2 * FRING;
+    // timeline: lane 0 of every warp of the first trace_ctas CTAs appends {kind, group, clock64} until its buffer is full
+    unsigned long long* tbuf = nullptr;
+    uint32_t tn = 0;
+    if constexpr (kTrace)
+        if (lane == 0 && (int)blockIdx.x < a.trace_ctas) tbuf = a.trace + ((size_t)blockIdx.x * TRACE_WARPS + warp) * TRACE_CAP;
+    auto trace = [&](int kind, int group = 0) {
+        if constexpr (kTrace)
+            if (tbuf && tn < TRACE_CAP)
+                tbuf[tn++] = ((unsigned long long)kind << 56) | ((unsigned long long)group << 48) |
+                             ((unsigned long long)clock64() & ((1ull << 48) - 1));
+    };
     if (threadIdx.x == 0) {
         for (int i = 0; i < RING; ++i) {
             mbar_init(bar_full + 8 * i, 1);
@@ -103,7 +156,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         }
         for (int g = 0; g < 2; ++g) mbar_init(bar_turn + 8 * g, 4);     // warpgroup g's turn: one arrival per warp of the other
         for (int e = 0; e < 2 * FRING; ++e) {
-            mbar_init(bar_ffull + 8 * e, 1);
+            mbar_init(bar_ffull + 8 * e, 32);       // one arrival per lane of the entry's FiLM producer
             mbar_init(bar_fempty + 8 * e, 4);       // one arrival per warp of the entry's warpgroup
         }
         fence_barrier_init();
@@ -119,13 +172,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             for (long long pair = blockIdx.x; pair < n_pairs; pair += gridDim.x)
                 for (int i = 0; i < a.n_loads; ++i, ++it) {
                     const uint32_t slot = it % RING;
+                    trace(TR_EMPTY_WAIT);
                     mbar_wait(bar_empty + 8 * slot, ((it / RING) & 1u) ^ 1u);
+                    trace(TR_EMPTY_DONE);
                     mbar_arrive_expect_tx(bar_full + 8 * slot, a.loads[i].bytes);
                     bulk_g2s(sbase + slot * SLOT_BYTES, a.packed + a.loads[i].src, a.loads[i].bytes, bar_full + 8 * slot);
                 }
-        } else if ((warp == PROD_WARP + 1 || warp == PROD_WARP + 2) && lane == 0) {
+        } else if (warp == PROD_WARP + 1 || warp == PROD_WARP + 2) {
             // the FiLM layers of consumer warpgroup g's tiles, in the order its epilogues use them: the first layer, then
-            // hidden layers 0 .. n - 1 (n = trunk_hidden when the network stops after the trunk head)
+            // hidden layers 0 .. n - 1 (n = trunk_hidden when the network stops after the trunk head).  Each lane folds
+            // four column pairs, c = f b + p with the expression the epilogue used to evaluate (the same bits), and
+            // arrives on the entry's barrier (release: its own stores).
             const int g = warp - PROD_WARP - 1;
             const int n_film = 1 + (a.sigma_only ? a.L.trunk_hidden : a.L.n_hidden);
             uint32_t it = 0;
@@ -135,11 +192,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 const float* film_b = a.film + (size_t)b * a.L.n_film * 2 * FN_H;
                 for (int i = 0; i < n_film; ++i, ++it) {
                     const uint32_t e = g * FRING + it % FRING;
-                    const uint32_t dst = sbase + SMEM_FILM + e * FILM_BYTES;
+                    const float2* row = reinterpret_cast<const float2*>(film_b + (size_t)i * 2 * FN_H);
+                    const float2* bias = reinterpret_cast<const float2*>(a.packed + (i == 0 ? a.L.first_b : a.L.hid_b[i - 1]));
+                    float4* dst = reinterpret_cast<float4*>(smem + SMEM_FILM + e * FILM_BYTES);
+                    trace(TR_EMPTY_WAIT);
                     mbar_wait(bar_fempty + 8 * e, ((it / FRING) & 1u) ^ 1u);
-                    mbar_arrive_expect_tx(bar_ffull + 8 * e, FILM_BYTES);
-                    bulk_g2s(dst, film_b + (size_t)i * 2 * FN_H, 2 * FN_H * 4, bar_ffull + 8 * e);
-                    bulk_g2s(dst + 2 * FN_H * 4, a.packed + (i == 0 ? a.L.first_b : a.L.hid_b[i - 1]), FN_H * 4, bar_ffull + 8 * e);
+                    trace(TR_EMPTY_DONE);
+#pragma unroll 1
+                    for (int k = 0; k < FN_H / 64; ++k) {    // (not unrolled: the producers live on 40 registers)
+                        const int cp = lane + 32 * k;        // column pair: columns 2 cp, 2 cp + 1
+                        const float2 f = __ldg(row + cp), p = __ldg(row + FN_H / 2 + cp), bb = __ldg(bias + cp);
+                        dst[cp] = make_float4(f.x, f.y, fmaf(f.x, bb.x, p.x), fmaf(f.y, bb.y, p.y));
+                    }
+                    mbar_arrive(bar_ffull + 8 * e);
                 }
             }
         }
@@ -161,7 +226,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
     // the next load of the stream: wait until it has landed, return its slot's shared-memory address
     auto acquire = [&](uint32_t& slot) -> uint32_t {
         slot = it % RING;
+        trace(TR_ACQ_WAIT);
         mbar_wait(bar_full + 8 * slot, (it / RING) & 1u);
+        trace(TR_ACQ_DONE);
         ++it;
         return sbase + slot * SLOT_BYTES;
     };
@@ -177,10 +244,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
     uint32_t turns = 0;
     // this warpgroup's FiLM entries (filled by its FiLM producer), one per layer, in layer order
     uint32_t fit = 0;
-    auto film_acquire = [&]() -> const float* {
+    auto film_acquire = [&]() -> const float4* {
         const uint32_t e = wg * FRING + fit % FRING;
+        trace(TR_FILM_WAIT);
         mbar_wait(bar_ffull + 8 * e, (fit / FRING) & 1u);
-        return reinterpret_cast<const float*>(smem + SMEM_FILM + e * FILM_BYTES);
+        trace(TR_FILM_DONE);
+        return reinterpret_cast<const float4*>(smem + SMEM_FILM + e * FILM_BYTES);
     };
     auto film_release = [&]() {
         const uint32_t e = wg * FRING + fit % FRING;
@@ -188,8 +257,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_fempty + 8 * e);
     };
-    auto turn_begin = [&]() { mbar_wait(bar_turn + 8 * wg, (turns & 1u) ^ (wg == 0 ? 1u : 0u)); };
-    auto turn_end = [&]() {                          // after wg_commit: this warp's share of the MMA group is issued
+    auto turn_begin = [&]() {
+        trace(TR_TURN_WAIT);
+        mbar_wait(bar_turn + 8 * wg, (turns & 1u) ^ (wg == 0 ? 1u : 0u));
+        trace(TR_TURN_DONE);
+    };
+    auto turn_end = [&](int group) {                 // after wg_commit: this warp's share of the MMA group is issued
+        trace(TR_COMMIT, group);
         ++turns;
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_turn + 8 * (wg ^ 1));
@@ -210,6 +284,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         const bool tile_ok = tile < a.n_tiles;
         const long long b = tile_ok ? tile / a.tiles_per_batch : 0;
         const long long p0 = tile_ok ? (tile % a.tiles_per_batch) * TILE : a.ppb;
+        trace(TR_PAIR);
 
         // ---- input slots of the tile's points (layout.h), one thread per point ----
         wg_bar(wg);                                  // the previous tile's fragment reads are done
@@ -255,27 +330,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         uint32_t nxt[8][4];                          // the next layer's slices 0..7 while half 1 is still being computed
         float d[64];
         // FiLM epilogue of accumulator half h: sin(f z + (f b + p)) -> dst[0..7] = k-slices 8h .. 8h+7 of the next layer;
-        // fs is the layer's FiLM entry in shared memory
-        auto film_epi = [&](const float* fs, int h, uint32_t (&dst)[8][4]) {
-            const float* fl = fs + h * 128;
-            const float* bias = fs + 2 * FN_H + h * 128;
+        // fs is the layer's folded FiLM entry in shared memory.  Column pair j = 8 j + 2 q of the half: one LDS.128; every
+        // kSoftSin-th pair takes soft_sinf (both columns, so each pack still holds two results of one kind)
+        auto film_epi = [&](const float4* fs, int h, uint32_t (&dst)[8][4]) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
-                const int c = 8 * j + 2 * q;
-                const float2 fr = *reinterpret_cast<const float2*>(fl + c);
-                const float2 ph = *reinterpret_cast<const float2*>(fl + FN_H + c);
-                const float2 bi = *reinterpret_cast<const float2*>(bias + c);
-                const float px = fmaf(fr.x, bi.x, ph.x), py = fmaf(fr.y, bi.y, ph.y);
-                dst[j >> 1][(j & 1) * 2] = pack_half2(__sinf(fmaf(fr.x, d[4 * j], px)), __sinf(fmaf(fr.y, d[4 * j + 1], py)));
-                dst[j >> 1][(j & 1) * 2 + 1] = pack_half2(__sinf(fmaf(fr.x, d[4 * j + 2], px)), __sinf(fmaf(fr.y, d[4 * j + 3], py)));
+                const float4 e = fs[64 * h + 4 * j + q];
+                const bool soft = kSoftSin > 0 && j % (kSoftSin > 0 ? kSoftSin : 1) == kSoftSin - 1;
+                auto sn = [soft](float x) { return soft ? soft_sinf(x) : __sinf(x); };
+                dst[j >> 1][(j & 1) * 2] = pack_half2(sn(fmaf(e.x, d[4 * j], e.z)), sn(fmaf(e.y, d[4 * j + 1], e.w)));
+                dst[j >> 1][(j & 1) * 2 + 1] = pack_half2(sn(fmaf(e.x, d[4 * j + 2], e.z)), sn(fmaf(e.y, d[4 * j + 3], e.w)));
             }
+            trace(TR_EPI_DONE);
         };
         auto act_hi = [&]() -> uint32_t (&)[8][4] { return *reinterpret_cast<uint32_t (*)[8][4]>(&act[8]); };
 
         // ---- first layer: input slots (k-slice 0) against the [256][64] input image ----
         {
             uint32_t xf[4], slot;
-            const float* fs = nullptr;
+            const float4* fs = nullptr;
             xfrag(0, xf);
             const uint32_t w = acquire(slot);
 #pragma unroll
@@ -284,8 +357,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 wg_fence();
                 mma_rs_n128(d, xf, desc_kmajor(w + h * CHUNK), 0u);
                 wg_commit();
-                turn_end();
+                turn_end(TG_FIRST);
                 wg_wait<0>();
+                trace(TR_MMA_DONE);
                 fence_regs(d);
                 fence_regs(xf);
                 if (h == 0) fs = film_acquire();
@@ -314,8 +388,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                     for (int k = 0; k < 4; ++k) mma_rs_n32(dh, act[4 * c + k], desc_kmajor(w + c * HEAD_CHUNK + 32 * k), (c | k) ? 1u : 0u);
                 wg_commit();
-                turn_end();
+                turn_end(TG_TRUNK_HEAD);
                 wg_wait<0>();
+                trace(TR_MMA_DONE);
                 fence_regs(dh);
                 fence_regs(act);
                 release(slot);
@@ -348,7 +423,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                     constexpr uint32_t kLabChunk = kFeatureHead ? FEAT_CHUNK : HEAD_CHUNK;
                     float dl[kLabN / 2];
                     uint32_t slot_h = 0, w_h = 0;
-                    const float* fs = nullptr;
+                    const float4* fs = nullptr;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         uint32_t sl[2];
@@ -364,8 +439,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                                     mma_rs_n128(d, act[8 * sb + 4 * c + k], desc_kmajor(w + c * CHUNK + 32 * k), (sb | c | k) ? 1u : 0u);
                         }
                         wg_commit();
-                        turn_end();
+                        turn_end(TG_LABEL_LAYER);
                         wg_wait<0>();
+                        trace(TR_MMA_DONE);
                         fence_regs(d);
                         fence_regs(act);
                         release(sl[0]);
@@ -383,8 +459,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                             else mma_rs_n32(dl, nxt[s], desc, (h | s) ? 1u : 0u);
                         }
                         wg_commit();
-                        turn_end();
+                        turn_end(TG_LABEL_HEAD);
                         wg_wait<0>();
+                        trace(TR_MMA_DONE);
                         fence_regs(dl);
                         fence_regs(nxt);
                     }
@@ -415,7 +492,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                 for (int s = 0; s < 3; ++s) xfrag(1 + s, xf[s]);
             uint32_t slot_x = 0, w_x = 0;
-            const float* fs = nullptr;
+            const float4* fs = nullptr;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 uint32_t sl[2];
@@ -437,8 +514,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                         if (s < nx) mma_rs_n128(d, xf[s], desc_kmajor(w_x + h * CHUNK + 32 * (1 + s)), 1u);
                 }
                 wg_commit();
-                turn_end();
+                turn_end(c0 ? TG_COLOR0 : TG_HIDDEN);
                 wg_wait<0>();
+                trace(TR_MMA_DONE);
                 fence_regs(d);
                 fence_regs(act);
                 fence_regs(xf);
@@ -469,8 +547,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                 for (int k = 0; k < 4; ++k) mma_rs_n64(dr, act[4 * c + k], desc_kmajor(w + c * FEAT_CHUNK + 32 * k), (c | k) ? 1u : 0u);
             wg_commit();
-            turn_end();
+            turn_end(TG_OUT_HEAD);
             wg_wait<0>();
+            trace(TR_MMA_DONE);
             fence_regs(dr);
             fence_regs(act);
             release(slot);
@@ -501,8 +580,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                 for (int k = 0; k < 4; ++k) mma_rs_n8(dr, act[4 * c + k], desc_kmajor(w + c * RGB_CHUNK + 32 * k), (c | k) ? 1u : 0u);
             wg_commit();
-            turn_end();
+            turn_end(TG_OUT_HEAD);
             wg_wait<0>();
+            trace(TR_MMA_DONE);
             fence_regs(dr);
             fence_regs(act);
             release(slot);

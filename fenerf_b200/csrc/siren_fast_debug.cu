@@ -1,0 +1,47 @@
+// Point network, FAST mode, debug instantiations of the wgmma kernel (siren_fast.cuh), in a translation unit of their
+// own so that the production instantiations compile exactly as they do without them:
+//   variant 1   one column pair in kSoftSinSplit of the epilogue on soft_sinf, for all four field kinds
+//   variant 2   the clock64 timeline of the production kernel (plain fields)
+//   variant 3   the clock64 timeline of the variant-1 kernel (plain fields)
+// and the device software sine on its own (soft_sine_eval).
+#include "siren_fast.cuh"
+
+namespace fn {
+
+namespace {
+
+template <bool kLabelFilm, bool kFeatureHead, int kSoftSin, bool kTrace>
+int launch(const FastArgs& a, int blocks, cudaStream_t st) {
+    static std::atomic<int> attr_set[kMaxDevices];
+    FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace>, attr_set, (int)SMEM_TOTAL));
+    siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace><<<blocks, NTHREADS, SMEM_TOTAL, st>>>(a);
+    FN_LAUNCH_OK("siren_fast_kernel<debug>");
+    return 0;
+}
+
+__global__ void soft_sine_kernel(const float* a, float* out, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = soft_sinf(a[i]);
+}
+
+}  // namespace
+
+int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st) {
+    const FastArgs& a = *static_cast<const FastArgs*>(args);
+    if (variant == 1) {
+        if (feature_head) return label_film ? launch<true, true, kSoftSinSplit, false>(a, blocks, st) : launch<false, true, kSoftSinSplit, false>(a, blocks, st);
+        return label_film ? launch<true, false, kSoftSinSplit, false>(a, blocks, st) : launch<false, false, kSoftSinSplit, false>(a, blocks, st);
+    }
+    FN_REQUIRE(!label_film && !feature_head, "the point-network timeline covers plain fields only");
+    if (variant == 2) return launch<false, false, kSoftSinEvery, true>(a, blocks, st);
+    return launch<false, false, kSoftSinSplit, true>(a, blocks, st);
+}
+
+int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st) {
+    if (n <= 0) return 0;
+    soft_sine_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, out, n);
+    FN_LAUNCH_OK("soft_sine_kernel");
+    return 0;
+}
+
+}  // namespace fn
