@@ -12,20 +12,22 @@ backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per
           network layer by layer, recomputing activations chunk by chunk (nothing but the workspace
           survives from the forward):
             recompute   ``fenerf_gemm_nt_film``: z = a W^T on wgmma with the epilogue fused -- a = sin(f z + p) and
-                        the gate f cos(f z + p) leave as fp16, z never does
-            backward    ``fenerf_gate_backward`` dZ = dA * gate (+ per-image column sums), dA' = dZ W
-                        (``fenerf_gemm_nt_f16``) and the per-image dW_b = dZ^T a (``fenerf_gemm_tn_f16``, split-K)
-          FiLM gradients need no further pass over the points:  dp = db_b / f,
-          df = (sum_k W[f,k] dW_b[f,k]) / f + b dp   (u = f z + p, z = W a + b).
+                        the gate cos(f z + p) leave as fp16, z never does
+            backward    ``fenerf_gate_backward`` dU = dA * gate = dL/du (+ per-image column sums dp_b),
+                        dA' = dU diag(f_b) W (``fenerf_gemm_nt_f16`` with a per-image scaled weight, one launch per
+                        image of the chunk) and the per-image M_b = dU_b^T a (``fenerf_gemm_tn_f16``, split-K)
+          Every gradient of the layer follows from M_b and dp_b without another pass over the points, and none divides
+          by f (a frequency of exactly 0 is reachable from the mapping network's 15 x + 30):
+          dW = sum_b diag(f_b) M_b,  db = sum_b f_b dp_b,  df_b = rowsum(W * M_b) + b dp_b   (u = f z + p, z = W a + b).
           Heads, the pre-multiplied label chain and the grid (``fenerf_grid_scatter_add``) close the chain.  A label FiLM
           field (SPATIALSIRENSEMANTIC) recomputes its label layer from the trunk output at FiLM row T and runs it
-          backward like a colour layer, its dZ W joining the trunk's dA.
+          backward like a colour layer, its dU diag(f) W joining the trunk's dA.
 Gradients flow to the FiLM table (and through torch's autograd into the mapping network / latents /
 frequency offsets) and to every field parameter.  The fp16 gradient stream is scaled by a power of two
 taken from max|d raw| on the device (no host sync) and unscaled at the end.
 
 The three 256-wide products per layer run on wgmma (csrc/gemm.cu: ``fenerf_gemm_nt_film`` -- the recompute with its FiLM
-epilogue fused, ``fenerf_gemm_nt_f16`` for dA' = dZ W, ``fenerf_gemm_tn_f16`` split-K for the per-image dW); only the narrow
+epilogue fused, ``fenerf_gemm_nt_f16`` for dA' = dU diag(f_b) W, ``fenerf_gemm_tn_f16`` split-K for the per-image M_b); only the narrow
 products (heads, the 3 / 35-wide inputs) go to the library.  ``FENERF_B200_BWD_GEMM=cublas`` switches the wide ones back
 (A/B timing); ``precision='exact'`` always uses fp32 library GEMMs.  (The kernels can also fold the next layer's gate multiply
 into the dA product's epilogue and produce the bias column sums from the dW kernel's staged tiles -- measured: the gate kernel's
@@ -177,14 +179,19 @@ class _FieldBackward:
         wc0 = fw.color[0][0].detach().float()
         self.Wc0x_narrow = wc0[:, :self.kx].contiguous()                          # (256, 3 + G) fp32
         self.Wc16 = [wc0[:, self.kx:].to(self.dt).contiguous()] + [w.detach().to(self.dt).contiguous() for w, _ in fw.color[1:]]
-        self.Wfeat16 = wc0[:, 3:self.kx].to(self.dt).contiguous() if G else None       # (256, G)
-        # dA' = dZ W on the wgmma NT kernel wants the transposed weights as its (N, K) operand
-        self.WhT16 = [None] + [w.t().contiguous() for w in self.Wh16[1:]] if self.own_gemm else None
-        self.WcT16 = [w.t().contiguous() for w in self.Wc16] if self.own_gemm else None
+        self.Wfeat32 = wc0[:, 3:self.kx].contiguous() if G else None                  # (256, G)
+        # fp32 weights of the chain products dA' = dU diag(f_b) W, by FiLM row (row 0 has none: its inputs are the points)
+        self.Wchain32 = [None] + [w.detach().float() for w, _ in fw.trunk[1:]]
         if self.lf:
             self.Wl16 = fw.label_film[0][0].detach().to(self.dt).contiguous()
-            self.WlT16 = self.Wl16.t().contiguous() if self.own_gemm else None
+            self.Wchain32.append(fw.label_film[0][0].detach().float())
             self.Wlhead32 = fw.labels[0][0].detach().float().contiguous()                 # (L, 256)
+        self.Wchain32 += [wc0[:, self.kx:]] + [w.detach().float() for w, _ in fw.color[1:]]
+        # ... scaled per image once for every chunk: diag(f_b) W, (B, n_film - 1, 256, 256); the NT kernel wants it transposed
+        fW = self.film[:, 1:, 0].unsqueeze(3) * torch.stack(self.Wchain32[1:])
+        self.fW = fW.transpose(2, 3).to(torch.float16).contiguous() if self.own_gemm else fW.to(self.dt)
+        del fW
+        self.fWfeat = (self.film[:, self.c0, 0].unsqueeze(2) * self.Wfeat32).to(self.dt) if G else None    # (B, 256, G)
         if self.own_gemm:
             self.Wn64 = torch.zeros((256, 64), dtype=torch.float16, device=dev)
             self.Wn64[:, :self.kx] = self.Wc0x_narrow
@@ -231,6 +238,17 @@ class _FieldBackward:
         tmp = torch.zeros((b1 - b0, 256), dtype=torch.float32, device=self.dev)
         _lib.check(_lib.lib().fenerf_gate_backward(dA.data_ptr(), gate.data_ptr(), P, ppb, tmp.data_ptr(), self.dtc, _stream(self.dev)))
         cs += tmp
+
+    def _chain(self, dU, idx, b0, b1, ppb):
+        """dU diag(f_b) W of FiLM row idx for each image b of the chunk: the gradient of the layer's input (P, 256)."""
+        k = b1 - b0
+        if not self.own_gemm:
+            return torch.bmm(dU.view(k, ppb, 256), self.fW[b0:b1, idx - 1]).view(k * ppb, 256)
+        out = torch.empty_like(dU)
+        for i in range(k):
+            rows = slice(i * ppb, (i + 1) * ppb)
+            ops.gemm_nt(dU[rows], self.fW[b0 + i, idx - 1], torch.float16, out=out[rows])
+        return out
 
     def _chunk(self, points, dirs, dir_group, lock_dirs, raw, d_raw, b0, b1):
         lib = _lib.lib()
@@ -295,41 +313,39 @@ class _FieldBackward:
             dA = torch.mm(dRGB, self.Wrgb16)                                   # (P, 256) fp16
             for j in range(Cn - 1, -1, -1):
                 idx = c0 + j
-                self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dZ now
+                self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dU now
                 a_in = A[idx - 1] if j else A[T - 1]
-                dz3 = dA.view(k, ppb, 256).transpose(1, 2)
-                self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(dz3, a_in.view(k, ppb, 256))
+                du3 = dA.view(k, ppb, 256).transpose(1, 2)
+                self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(du3, a_in.view(k, ppb, 256))
                 if j == 0:
                     e16 = torch.zeros((P, self.kx_pad), dtype=self.dt, device=dev)
                     e16[:, :self.kx] = extras
-                    self.dWx_b[b0:b1] += _bmm32(dz3, e16.view(k, ppb, self.kx_pad))
-                    if spec.grid_channels:
-                        d_feat = torch.mm(dA, self.Wfeat16).contiguous()       # (P, G) fp16
+                    self.dWx_b[b0:b1] += _bmm32(du3, e16.view(k, ppb, self.kx_pad))
+                    if spec.grid_channels:                                     # d features = dU diag(f_b) W_feat, (P, G)
+                        d_feat = torch.bmm(dA.view(k, ppb, 256), self.fWfeat[b0:b1]).view(P, -1).contiguous()
                         _lib.check(lib.fenerf_grid_scatter_add(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
                                                                d_feat.shape[1], P, self.grid_grad_cl.data_ptr(), self.dtc, st))
-                dA = ops.gemm_nt(dA, self.WcT16[j], torch.float16) if own else torch.mm(dA, self.Wc16[j])
+                dA = self._chain(dA, idx, b0, b1, ppb)
                 A[idx], Gt[idx] = None, None
             # ---- trunk: colour-branch gradient + sigma / label heads ----
             dA += torch.mm(dH.float(), self.Wheads32)
-            if self.lf:     # label branch: d logits W_head -> gate -> dW, colsum of row T; dZ W_label joins the trunk's dA
+            if self.lf:     # label branch: d logits W_head -> gate -> M_b, colsum of row T; dU diag(f) W_label joins the trunk's dA
                 # (P, 256), formed in fp32: an fp16 product's reduction order depends on the chunk's row count
                 dAl = torch.mm(dH[:, :self.L].float(), self.Wlhead32).to(self.dt)
                 self._gate(dAl, Gt[T], T, b0, b1, P, ppb)
                 if own:
                     self.dW_b[T][b0:b1] += ops.gemm_tn(dAl, A[T - 1], k, ppb)
-                    dA += ops.gemm_nt(dAl, self.WlT16, torch.float16)
                 else:
                     self.dW_b[T][b0:b1] += _bmm32(dAl.view(k, ppb, 256).transpose(1, 2), A[T - 1].view(k, ppb, 256))
-                    dA += torch.mm(dAl, self.Wl16)
+                dA += self._chain(dAl, T, b0, b1, ppb)
                 A[T], Gt[T] = None, None
             for l in range(T - 1, 0, -1):
                 self._gate(dA, Gt[l], l, b0, b1, P, ppb)
                 if own:
                     self.dW_b[l][b0:b1] += ops.gemm_tn(dA, A[l - 1], k, ppb)
-                    dA = ops.gemm_nt(dA, self.WhT16[l], torch.float16)
                 else:
                     self.dW_b[l][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), A[l - 1].view(k, ppb, 256))
-                    dA = torch.mm(dA, self.Wh16[l])
+                dA = self._chain(dA, l, b0, b1, ppb)
                 A[l], Gt[l] = None, None
             self._gate(dA, Gt[0], 0, b0, b1, P, ppb)
             x16 = torch.zeros((P, 8), dtype=self.dt, device=dev)
@@ -345,21 +361,19 @@ class _FieldBackward:
         layers = fw.film_layers()
         for idx, (w, b) in enumerate(layers):
             f = film[:, idx, 0]                                             # (B, 256)
-            db_b = self.colsum[:, idx]
-            dp = db_b / f
+            dp = self.colsum[:, idx]                                        # sum of dU per image
             w32 = w.detach().float()
             if idx == 0:
-                dwb = self.dW_b[0][:, :, :3]
-                full = dwb
+                m = self.dW_b[0][:, :, :3]
             elif idx == self.c0:
-                full = torch.cat([self.dWx_b[:, :, :self.kx], self.dW_b[idx]], dim=2)   # column order of the reference: [dir, feat, x]
+                m = torch.cat([self.dWx_b[:, :, :self.kx], self.dW_b[idx]], dim=2)   # column order of the reference: [dir, feat, x]
             else:
-                full = self.dW_b[idx]
-            df = torch.einsum('fk,bfk->bf', w32, full) / f + b.detach().float().unsqueeze(0) * dp
+                m = self.dW_b[idx]                                          # M_b = dU_b^T a
+            df = torch.einsum('fk,bfk->bf', w32, m) + b.detach().float().unsqueeze(0) * dp
             d_film[:, idx, 0] = df * inv
             d_film[:, idx, 1] = dp * inv
-            grads[id(w)] = full.sum(0) * inv
-            grads[id(b)] = db_b.sum(0) * inv
+            grads[id(w)] = torch.einsum('bf,bfk->fk', f, m) * inv
+            grads[id(b)] = (f * dp).sum(0) * inv
         L = self.L
         grads[id(fw.sigma[0])] = (self.d_heads_w[L] * inv).reshape(fw.sigma[0].shape)
         grads[id(fw.sigma[1])] = (self.d_heads_b[L] * inv).reshape(fw.sigma[1].shape)

@@ -5,18 +5,20 @@
 // two point-network passes; ray set-up and resampling are no_grad there too (generators.py:41, 59).  The
 // compositing backward (composite_backward_kernel) lives beside the forward in composite.cu; the point network's are:
 //
-//   film_forward_stash_kernel   z (fp32 GEMM output) -> a = sin(f (z + b) + p) and the gate f cos(.) as fp16:
+//   film_forward_stash_kernel   z (fp32 GEMM output) -> a = sin(f (z + b) + p) and the gate cos(.) as fp16:
 //                               everything the backward of a FiLM layer needs besides the GEMMs
-//   gate_backward_kernel        dZ = dA * gate in place (fp16) + per-image column sums (bias / phase grads)
+//   gate_backward_kernel        dU = dA * gate in place (fp16) + per-image column sums (the phase grads)
 //   head_grads_kernel           d raw -> scaled fp16 head gradients (sigmoid', label / sigma columns)
 //   head_grads_feature_kernel   the same for the feature-head fields: 64 linear feature columns, 0 / 64 label columns
 //   extras_gather_kernel        [dir, trilinear grid features] per point (the first colour layer's extra inputs)
 //   grid_scatter_add_kernel     d features -> channels-last grid gradient (vector atomics)
 //   grid_unpack_grad_kernel     channels-last -> torch's channel-major (1, G, R, R, R) layout
 //
-// The 256-wide GEMMs between them (recompute z, dA = dZ W, dW = dZ^T a) are plain library GEMMs issued by
-// the host (fenerf_b200/backward.py); FiLM gradients follow from the per-image dW without another pass:
-//   d f = (sum_k W[f,k] dW_b[f,k]) / f + b dp,   dp = db_b / f        (u = f z + p, z = W a + b).
+// The 256-wide GEMMs between them (recompute z, dA = dU diag(f_b) W, M_b = dU_b^T a) are issued by the host
+// (fenerf_b200/backward.py); every gradient of the layer follows from the per-image M_b and column sums dp_b
+// without another pass, and without dividing by f (f = 0 is a valid frequency):
+//   dp_b = sum dU_b,  df_b = sum_k W[f,k] M_b[f,k] + b dp_b,  dW = sum_b diag(f_b) M_b,  db = sum_b f_b dp_b
+//   (u = f z + p, z = W a + b, dU = dL/du = dA cos(u)).
 #include "common.cuh"
 #include "siren_common.cuh"
 
@@ -26,7 +28,7 @@ namespace {
 
 // ---- FiLM layer: forward values the backward needs --------------------------------------------------
 // thread = (point, 8 consecutive features).  z may be NULL (first layer: only the narrow inputs), xin may be
-// NULL (plain hidden layer).  out: a (fp16, the next GEMM's input) and gate = f cos(f z + p) (fp16).
+// NULL (plain hidden layer).  out: a (fp16, the next GEMM's input) and gate = cos(f z + p) (fp16).
 template <typename T> struct Vec8;
 template <> struct Vec8<__half> {
     __align__(16) __half v[8];
@@ -91,14 +93,14 @@ __global__ void __launch_bounds__(256) film_forward_stash_kernel(
             if (sizeof(T) == 2) __sincosf(u, &sn, &cs);     // fp16 streams: the MUFU pair is far inside their rounding
             else sincosf(u, &sn, &cs);
             av.set(i, sn);
-            gv.set(i, fr * cs);
+            gv.set(i, cs);
         }
         av.store(a_out + p * FN_H + f0);
         gv.store(gate_out + p * FN_H + f0);
     }
 }
 
-// ---- dZ = dA * gate (in place), column sums per image -------------------------------------------------
+// ---- dU = dA * gate (in place), column sums per image -------------------------------------------------
 // block = 32 feature groups (8 features) x 8 point lanes, one slab of `slab` points of ONE image
 template <typename T>
 __global__ void __launch_bounds__(256) gate_backward_kernel(T* __restrict__ dA, const T* __restrict__ gate,

@@ -2,10 +2,11 @@
 //
 //   gemm_nt_kernel     C[M, 256] = A[M, 256] . B[256, 256]^T        A, B fp16 row-major (K contiguous)
 //                        recompute   z = a W^T   -> fp32, or with the FiLM epilogue fused: a' = sin(f (z + b) + p) and
-//                                                   the gate f cos(.) written as fp16, z never leaves the SM
-//                        backward    dA' = dZ W  -> fp16 (B = W^T, transposed once per call by the host)
+//                                                   the gate cos(.) written as fp16, z never leaves the SM
+//                        backward    dA' = dU diag(f_b) W  -> fp16 (B = (diag(f_b) W)^T, built per image by the host;
+//                                    a chunk of several images runs one launch per image on its rows)
 //   gemm_tn_kernel     C_b[256, 256] = sum over the points of image b of  X[p, :]^T  Y[p, :]   (split-K over CTAs)
-//                        dW_b = dZ^T a: both operands are MN-major views of the row-major (P, 256) streams
+//                        M_b = dU^T a: both operands are MN-major views of the row-major (P, 256) streams
 //
 // 256 threads = two warpgroups, each owning 64 rows of a 128-row output tile with a 64 x 256 fp32 accumulator in
 // registers (wgmma m64n256k16, both operands in shared memory).  Operands are plain row-major tensors, so every thread
@@ -32,8 +33,8 @@ struct NtArgs {
     float* C32;           // (M, 256) fp32 out, or
     __half* C16;          // (M, 256) fp16 out, or (FiLM epilogue) both of:
     __half* a_out;        // (M, 256) sin(f (c + bias) + p)
-    __half* gate_out;     // (M, 256) f cos(f (c + bias) + p)
-    const __half* gate_mul;  // optional (M, 256): the fp16 output is multiplied by it (dZ' = (dZ W) * gate of the layer below)
+    __half* gate_out;     // (M, 256) cos(f (c + bias) + p)
+    const __half* gate_mul;  // optional (M, 256): the fp16 output is multiplied by it (dU' = (dU W') * gate of the layer below)
     const __half* A2;     // optional fifth k-chunk: narrow inputs (M, 64) fp16 (zero padded) ...
     const __half* B2;     // ... against (256, 64) fp16: C += A2 B2^T  (the first colour layer's [dir, grid features])
     const float* bias;    // (256)
@@ -132,16 +133,16 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_nt_kernel(const __grid_const
 #pragma unroll
                 for (int i = 0; i < 32; ++i) {
                     const int c = 8 * i + 2 * q;
-                    float sn[2], cs[2], fr[2];
+                    float sn[2], cs[2];
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        fr[e] = fl ? __ldg(fl + c + e) : s_film[c + e];
+                        const float fr = fl ? __ldg(fl + c + e) : s_film[c + e];
                         const float ph = fl ? __ldg(fl + 256 + c + e) : s_film[256 + c + e];
-                        const float u = fmaf(fr[e], d[4 * i + 2 * rr + e] + s_film[512 + c + e], ph);
+                        const float u = fmaf(fr, d[4 * i + 2 * rr + e] + s_film[512 + c + e], ph);
                         __sincosf(u, &sn[e], &cs[e]);        // MUFU: ~|u| * 2^-24 absolute, far inside the fp16 streams' rounding
                     }
                     *reinterpret_cast<uint32_t*>(a.a_out + m * 256 + c) = pack_half2(sn[0], sn[1]);
-                    *reinterpret_cast<uint32_t*>(a.gate_out + m * 256 + c) = pack_half2(fr[0] * cs[0], fr[1] * cs[1]);
+                    *reinterpret_cast<uint32_t*>(a.gate_out + m * 256 + c) = pack_half2(cs[0], cs[1]);
                 }
             } else if (a.C32) {
 #pragma unroll

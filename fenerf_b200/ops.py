@@ -382,12 +382,15 @@ def mapping_film(net, z, film, first_layer, n_layers, avg=None, psi=1.0):
 # --------------------------------------------------------------------------------------------
 # wgmma GEMMs of the backward (csrc/gemm.cu)
 # --------------------------------------------------------------------------------------------
-def gemm_nt(a16, b16, out_dtype=torch.float32, gate=None):
+def gemm_nt(a16, b16, out_dtype=torch.float32, gate=None, out=None):
     """(M, 256) fp16 . (256, 256)^T fp16 -> (M, 256) fp32 or fp16 (fenerf_gemm_nt_f16); `gate` (M, 256) fp16 multiplies
-    the fp16 output in the epilogue."""
+    the fp16 output in the epilogue.  `out`: a contiguous (M, 256) tensor of out_dtype to write into."""
     dev = a16.device
     m = a16.shape[0]
-    out = torch.empty((m, 256), dtype=out_dtype, device=dev)
+    if out is None:
+        out = torch.empty((m, 256), dtype=out_dtype, device=dev)
+    elif out.shape != (m, 256) or out.dtype != out_dtype or not out.is_contiguous():
+        raise ValueError("out must be a contiguous (%d, 256) %s tensor" % (m, out_dtype))
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().fenerf_gemm_nt_f16(
             _chk(a16, "A", dev, torch.float16), _chk(b16, "B", dev, torch.float16), m,

@@ -341,16 +341,16 @@ int fenerf_frames_to_u8(const float* frames, int32_t batch, int32_t channels, in
 
 /* The 256-wide products of a FiLM layer's backward on wgmma (csrc/gemm.cu); fp16 row-major operands, fp32 accumulate.
  *   fenerf_gemm_nt_f16   C (M, 256) = A (M, 256) . B (256, 256)^T  -> c_f32 or c_f16 (exactly one non-NULL)
- *                        (dA' = dZ W: pass B = W^T); optional gate_mul (M, 256) fp16 multiplies the fp16 output in the
- *                        epilogue: dZ of the layer below = (dZ W) * its gate, without a pass of its own
+ *                        (dA' = dU diag(f) W: pass B = (diag(f) W)^T of one image); optional gate_mul (M, 256) fp16
+ *                        multiplies the fp16 output in the epilogue: dU of the layer below = (dU W') * its gate
  *   fenerf_gemm_nt_film  the recompute of a layer with its epilogue fused: z = A W^T never leaves the SM,
- *                        a_out = sin(f (z + bias) + p), gate_out = f cos(f (z + bias) + p), both (M, 256) fp16;
+ *                        a_out = sin(f (z + bias) + p), gate_out = cos(f (z + bias) + p), both (M, 256) fp16;
  *                        film_layer / film_batch_stride / points_per_batch as in fenerf_film_forward_stash; optional
  *                        narrow_in (M, 64) fp16 / narrow_w (256, 64) fp16, zero padded: a fifth k-chunk, z += narrow_in
  *                        narrow_w^T (the first colour layer's [dir, grid features] inputs, siren.py:1519-1522)
  *   fenerf_gemm_tn_f16   partial (batch, slices, 256, 256) fp32: for image b, slice s the sum over its 64-point stages
- *                        s, s + slices, ... of X[p, :]^T Y[p, :]  (dW_b = dZ^T a = the sum over the slices); optional
- *                        colsum (batch, slices, 256): column sums of X over the same stages (= d bias), computed by the
+ *                        s, s + slices, ... of X[p, :]^T Y[p, :]  (M_b = dU^T a = the sum over the slices); optional
+ *                        colsum (batch, slices, 256): column sums of X over the same stages (= d phase), computed by the
  *                        epilogue warps from the staged tiles while the tensor core runs                              */
 int fenerf_gemm_nt_f16(const void* A, const void* B, int64_t M, float* c_f32, void* c_f16, const void* gate_mul, void* stream);
 int fenerf_gemm_nt_film(const void* A, const void* W, int64_t M, const float* bias, const float* film_layer,
@@ -371,14 +371,15 @@ int fenerf_composite_backward(const fenerf_render_desc* rd, int32_t out_dim, con
 /* One FiLM layer's forward values for the backward (siren/siren.py:113-123): from the GEMM output
  * z (n_points, 256) fp32 (NULL for the first layer) plus optional narrow inputs narrow_in (n_points, w) fp32
  * against narrow_w (256, w) fp32 (positions; [dir, grid features] of the first colour layer):
- *   a = sin(f (z + bias) + p)  -> a_out (n_points, 256);   gate = f cos(f (z + bias) + p) -> gate_out   (both of `dtype`)
+ *   a = sin(f (z + bias) + p)  -> a_out (n_points, 256);   gate = cos(f (z + bias) + p) -> gate_out   (both of `dtype`)
  * film_layer points at image 0's [2][256] block of the layer, film_batch_stride floats between images. */
 int fenerf_film_forward_stash(const float* z, const float* bias, const float* film_layer, int64_t film_batch_stride,
                               int64_t n_points, int64_t points_per_batch, const float* narrow_in, int32_t narrow_width,
                               const float* narrow_w, void* a_out, void* gate_out, int32_t dtype, void* stream);
 
-/* dZ = dA * gate in place ((n_points, 256) of `dtype`); colsum (B, 256) fp32 += per-image column sums of dZ
- * (= d bias; d phase = colsum / f; d freq follows from the per-image dW, see csrc/backward.cu). */
+/* dU = dA * gate in place ((n_points, 256) of `dtype`): the gradient with respect to the pre-activation u = f z + p;
+ * colsum (B, 256) fp32 += per-image column sums of dU (= d phase; d bias = sum_b f_b colsum_b; d freq follows from the
+ * per-image M_b = dU_b^T a, see csrc/backward.cu -- no gradient divides by f). */
 int fenerf_gate_backward(void* dA, const void* gate, int64_t n_points, int64_t points_per_batch, float* colsum,
                          int32_t dtype, void* stream);
 

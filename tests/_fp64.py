@@ -36,7 +36,8 @@ def _siren(model, device, sigma_bias_shift=0.0):
 
 def _film(siren, batch, seed, edges=False):
     """FiLM table (B, L, 2, 256) from random latents.  edges: 10 % of the frequencies negated and 5 % set to
-    0.25 <= |f| <= 1, so that finish()'s dp = db_b / f is exercised away from f ~ 30."""
+    0.25 <= |f| <= 1, so that the backward sees frequencies away from f ~ 30 (plant_frequencies() adds f = 0, tiny and
+    large |f| in chosen columns)."""
     g = torch.Generator().manual_seed(seed)
     n_lat = 2 if hasattr(siren, "geo_mapping_network") else 1
     zs = [torch.randn(batch, 256, generator=g) for _ in range(n_lat)]
@@ -51,6 +52,36 @@ def _film(siren, batch, seed, edges=False):
         small = (u >= 0.1) & (u < 0.15)
         f[small] = mag[small]
     return film.contiguous()
+
+
+#: frequencies at the edges of the FiLM gradient algebra: zero of either sign (the table's 15 x + 30 is exactly 0 at
+#: x = -2), one ulp of 30 (2^-19, the smallest non-zero |f| the table can hold near 0), values where the fp16 gate and
+#: gradient streams would go subnormal if they carried f, and a large |f| where |u| reaches the hundreds
+EDGE_FREQS = (0.0, -0.0, 2.0 ** -19, -2.0 ** -19, 1e-5, -1e-5, 1e-3, -1e-3, 0.05, -0.05, 150.0, -150.0)
+
+
+def film_rows(siren):
+    """FiLM rows by role: first / middle / last trunk layer, the label FiLM layer (or None), first / last colour layer."""
+    t = len(siren.network)
+    lf = int(hasattr(siren, "label_layer_sine"))
+    color = siren.color_layer_sine
+    n_color = len(color) if isinstance(color, torch.nn.ModuleList) else 1
+    return dict(trunk_first=0, trunk_mid=t // 2, trunk_last=t - 1, label=t if lf else None, color_first=t + lf,
+                color_last=t + lf + n_color - 1)
+
+
+def plant_frequencies(film, rows, freqs=EDGE_FREQS):
+    """Writes each frequency of `freqs` into every row of `rows` twice: in column 17 i + 5 of every image, and in
+    column 17 i + 13 of the last image only (image b0 > 0 of a multi-image chunk).  -> (film, [(row, col, image or None)])"""
+    film = film.clone()
+    planted = []
+    last = film.shape[0] - 1
+    for row in sorted(set(rows)):
+        for i, v in enumerate(freqs):
+            film[:, row, 0, 17 * i + 5] = v
+            film[last, row, 0, 17 * i + 13] = v
+            planted += [(row, 17 * i + 5, None), (row, 17 * i + 13, last)]
+    return film.contiguous(), planted
 
 
 def _rel(got, want):

@@ -1,6 +1,6 @@
 """Generates tests/golden/*.npz by running the UNMODIFIED reference (a checkout of it named by $FENERF_REFERENCE_ROOT).
 
-    python tests/golden/make_goldens.py [--grads | --part | --dropin]
+    python tests/golden/make_goldens.py [--grads | --zero-freq | --part | --dropin]
 
 The reference holds no golden vectors for the render path (SURVEY.md section 4), so the pin of the
 oracle is the reference's own forward on fixed seeds, captured here.  The .npz files travel with
@@ -159,6 +159,53 @@ def frequency_grad_goldens():
         print("%-28s loss %.6f -> %s (%.1f KB)" % (name, loss.item(), os.path.basename(path), os.path.getsize(path) / 1024))
 
 
+#: FiLM-table columns (layer * 256 + feature) whose raw frequency becomes exactly -2.0 (table frequency 15 x + 30 = 0) or
+#: -2.0 moved by a few ulps (table frequencies of a few 2^-19), in image 0 only or in every image
+ZERO_FREQ_COLUMNS = {"all": [0 * 256 + 7, 4 * 256 + 100, 7 * 256 + 255, 8 * 256 + 3],
+                     "image0": [0 * 256 + 50, 4 * 256 + 9, 7 * 256 + 128, 8 * 256 + 200]}
+ZERO_FREQ_ULPS = [1, -1, 3, -3, 8, -8]
+
+
+def zero_frequency_grad_golden():
+    """tests/golden/gradfreq_a_small_zero_f.npz: as gradfreq_a_small.npz, with raw frequencies set to exactly -2.0 and to
+    -2.0 +- a few ulps in ZERO_FREQ_COLUMNS.  Stores the edited inputs ("freq_in", "phase_in") and the gradients.  The
+    run's draws are those of the unedited case (they depend on shapes only; checked against the recorded draws when the
+    golden is made), so the GPU test replays the oracle's draws of a_small."""
+    ref_generators, ref_siren, _ = ref_shim.load()
+    out_dir = os.path.dirname(os.path.abspath(__file__))
+    case = _cases.CASE_BY_NAME["a_small"]
+    gen, _ = build_reference(case, ref_generators, ref_siren)
+    latents = _cases.make_latents(case)
+    with torch.no_grad():
+        freq, phase = (t.clone() for t in gen.siren.mapping_network(latents[0]))
+        m2 = torch.tensor(-2.0)
+        for i, col in enumerate(ZERO_FREQ_COLUMNS["all"] + ZERO_FREQ_COLUMNS["image0"]):
+            rows = slice(None) if i < len(ZERO_FREQ_COLUMNS["all"]) else slice(0, 1)
+            freq[rows, col] = -2.0
+            for j, k in enumerate(ZERO_FREQ_ULPS):        # the next columns: -2 moved by k ulps
+                v = m2
+                for _ in range(abs(k)):
+                    v = torch.nextafter(v, torch.tensor(0.0 if k > 0 else -4.0))
+                freq[rows, col + 1 + j if col + 1 + j < (col // 256 + 1) * 256 else col - 1 - j] = v
+    fp = [freq.requires_grad_(True), phase.requires_grad_(True)]
+    freq_in = freq.detach().clone()
+    torch.manual_seed(case.seed)
+    with _RecordDraws() as rec:
+        pixels, _ = gen.forward_with_frequencies(*fp, **case.cfg)
+    loss = (pixels * _cases.loss_weights(pixels.shape)).sum()
+    loss.backward()
+    out = {"loss": np.array(loss.item()), "freq_in": freq_in.numpy(), "phase_in": phase.detach().numpy(),
+           "arg0": fp[0].grad.numpy(), "arg1": fp[1].grad.numpy()}
+    import _harness
+    draws = _harness.oracle_run(case)["draws"]
+    assert len(draws) == len(rec.log) and all(k == kr and torch.equal(t, tr) for (k, t), (kr, tr) in zip(draws, rec.log))
+    path = os.path.join(out_dir, "gradfreq_a_small_zero_f.npz")
+    np.savez_compressed(path, **out)
+    print("%-28s loss %.6f  %d draws, %d zero table frequencies -> %s (%.1f KB)" % (
+        "a_small_zero_f", loss.item(), len(rec.log), int(((freq_in * 15 + 30) == 0).sum()), os.path.basename(path),
+        os.path.getsize(path) / 1024))
+
+
 class _RecordDraws:
     """Records every torch.rand / randn / randperm made while the reference runs (part_forward draws per ray subset,
     which the oracle does not restate): the GPU test replays them through ReplayRng."""
@@ -262,5 +309,8 @@ if __name__ == "__main__":
     elif sys.argv[1:2] == ["--grads"]:
         grad_goldens()
         frequency_grad_goldens()
+        zero_frequency_grad_golden()
+    elif sys.argv[1:2] == ["--zero-freq"]:
+        zero_frequency_grad_golden()
     else:
         main()

@@ -12,9 +12,10 @@ checked on its own against a float64 restatement of the same operation, at the s
 D. The bounds are shown to catch faults: each fault is applied to the float64 reference (not to a kernel) and must move
 the result past the committed bound.  Those checks and the references' own gradchecks run on the CPU.
 
-Bounds: measured on an H100 80GB HBM3 (132 SMs); each constant below states the measured maximum.
+E. The FiLM-gradient algebra of finish() restated in float64 from autograd pieces, at f = 0, tiny and large |f| (CPU);
+   the kernels at those frequencies are in test_gpu_fp64_film_edges.py.
 
-Not covered: f = 0 in the FiLM table (finish() divides by f: dp = db_b / f); the frequencies here stay at |f| >= 0.25.
+Bounds: measured on an H100 80GB HBM3 (132 SMs); each constant below states the measured maximum.
 """
 import copy
 import ctypes
@@ -26,7 +27,8 @@ import torch
 import torch.nn.functional as F
 
 import _cases
-from _fp64 import _ZeroDraws, _film, _grid_lookup_keep_dtype, _opt, _rel, _siren, composite_ref, field_ref, noise_offset
+from _fp64 import (EDGE_FREQS, _ZeroDraws, _film, _grid_lookup_keep_dtype, _opt, _rel, _siren, composite_ref, field_ref,
+                   noise_offset, plant_frequencies)
 from fenerf_b200 import _lib, backward, ops
 from oracle import render_oracle as oracle
 
@@ -38,7 +40,7 @@ gpu = pytest.mark.gpu
 COMPOSITE_BOUND = 1e-5
 #: field backward, max |grad - fp64| / max |grad fp64| per parameter tensor, the whole grid and each FiLM layer's
 #: frequency and phase gradients.  Measured: exact 3.1e-5 (model H, L1: d film of colour layer 5), 1.0e-5 at L4;
-#: default 1.21e-2 (model H, L1), 5.5e-3 at L4 -- the fp16 streams (gate = f cos(f z + p), f ~ 30) set it.
+#: default 1.21e-2 (model H, L1), 5.5e-3 at L4 -- the fp16 streams (u = f z + p recomputed from them, f ~ 30) set it.
 FIELD_BOUND = {"exact": 1e-4, "default": 2e-2}
 #: the same gradients from a chunked run (L2 / L3) and a one-chunk run of the same kernels, relative to the tensor's
 #: maximum.  Measured: exact 1.7e-5 (model H: the fp32 library GEMMs pick other algorithms for other row counts, and 16
@@ -150,12 +152,15 @@ def test_grid_lookup_swap_is_the_oracles_lookup():
                                                             grid.double().requires_grad_(True)))
 
 
-@pytest.mark.parametrize("model", ["A", "D"])
-def test_field_reference_gradcheck(model, monkeypatch):
+@pytest.mark.parametrize("model,edges", [("A", False), ("D", False), ("A", True), ("D", True)],
+                         ids=["A", "D", "A-zero_tiny_f", "D-zero_tiny_f"])
+def test_field_reference_gradcheck(model, edges, monkeypatch):
     """The float64 field VJP (every parameter and the FiLM table) on 2 points, checked in gradcheck's fast mode
-    (random projections of the full Jacobian)."""
+    (random projections of the full Jacobian); with `edges`, every FiLM row also holds f = 0, -0, tiny and large |f|."""
     siren = _siren(model, "cpu")
     film = _film(siren, 1, 6).double()
+    if edges:
+        film = plant_frequencies(film, range(film.shape[1]))[0]
     pts, dirs = _field_points(1, 2, 2, 7)
     monkeypatch.setattr(oracle, "grid_lookup", _grid_lookup_keep_dtype)
     ref = copy.deepcopy(siren).double()
@@ -486,3 +491,68 @@ def test_forward_faults_exceed_the_bounds(monkeypatch, model):
     moved = {k: float((v - good).abs().amax((0, 1)).max()) for k, v in (("film_rows", swapped), ("bias_half1", dropped))}
     print("forward faults %s: %s" % (model, moved))
     assert min(moved.values()) > 10 * FWD_BOUND["fast"], moved
+
+
+# --------------------------------------------------------------------------------------------
+# E. the FiLM-gradient algebra of finish() at the frequency edges (CPU, float64)
+# --------------------------------------------------------------------------------------------
+def _record_film_layers(monkeypatch):
+    log = []
+
+    def film_layer(linear, x, freq, phase):
+        u = freq.unsqueeze(1) * linear(x) + phase.unsqueeze(1)
+        u.retain_grad()
+        log.append((linear, x.detach(), u))
+        return torch.sin(u)
+    monkeypatch.setattr(oracle, "_film", film_layer)
+    return log
+
+
+def _film_grads_new(f, w, b, a, du):
+    """finish()'s algebra: M_b = dU_b^T a, dp_b = sum dU_b -> (d freq, d phase, dW, db), no division by f."""
+    m = torch.einsum("bpf,bpk->bfk", du, a)
+    dp = du.sum(1)
+    return torch.einsum("fk,bfk->bf", w, m) + b * dp, dp, torch.einsum("bf,bfk->fk", f, m), (f * dp).sum(0)
+
+
+def _film_grads_divided(f, w, b, a, du):
+    """The earlier algebra: from dZ = dU f, dp = db_b / f and df = rowsum(W dW_b) / f + b dp."""
+    dz = du * f.unsqueeze(1)
+    dw_b = torch.einsum("bpf,bpk->bfk", dz, a)
+    db_b = dz.sum(1)
+    dp = db_b / f
+    return torch.einsum("fk,bfk->bf", w, dw_b) / f + b * dp, dp, dw_b.sum(0), db_b.sum(0)
+
+
+@pytest.mark.parametrize("model", ["A", "D", "I", "K"])
+def test_film_gradient_algebra_at_edge_frequencies(monkeypatch, model):
+    """finish()'s FiLM-gradient algebra, restated from float64 autograd pieces (each layer's input and dL/du), equals
+    the autograd gradients of the FiLM table and of every FiLM layer's weight and bias, with f in EDGE_FREQS planted in
+    every FiLM row (in all images and in image 1 only).  The algebra that divided by f gives NaN at f = 0 and -0."""
+    import _hd_fields as HD             # registers models J / K; its field_eval covers the label FiLM and plain fields
+    siren = copy.deepcopy(_siren(model, "cpu")).double()
+    n = 300
+    pts, dirs = _field_points(2, n, 3, 21)
+    pts, dirs = pts.double(), _per_point(dirs, n, False).double()
+    film0 = _film(_siren(model, "cpu"), 2, 21, edges=True).double()
+    film, planted = plant_frequencies(film0, range(film0.shape[1]))
+    film.requires_grad_(True)
+    monkeypatch.setattr(oracle, "grid_lookup", _grid_lookup_keep_dtype)
+    log = _record_film_layers(monkeypatch)
+    out = HD.field_eval(siren, pts, film, dirs)
+    d_out = torch.randn(out.shape, generator=torch.Generator().manual_seed(22), dtype=torch.float64)
+    (out * d_out).sum().backward()
+    assert len(log) == film.shape[1]
+    zero_cols = [(r, c) for r, c, img in planted if img is None and EDGE_FREQS[(c - 5) // 17] == 0.0]
+    for row, (linear, a, u) in enumerate(log):
+        f = film.detach()[:, row, 0]
+        w, b = linear.weight.detach(), linear.bias.detach()
+        want = (film.grad[:, row, 0], film.grad[:, row, 1], linear.weight.grad, linear.bias.grad)
+        got = _film_grads_new(f, w, b, a, u.grad)
+        for name, g, wv in zip(("freq", "phase", "weight", "bias"), got, want):
+            assert torch.isfinite(wv).all() and torch.isfinite(g).all(), (row, name)
+            assert _rel(g, wv) <= 1e-12, (row, name, _rel(g, wv))
+        old = _film_grads_divided(f, w, b, a, u.grad)
+        cols = [c for r, c in zero_cols if r == row]
+        assert torch.isnan(old[0][:, cols]).all() and torch.isnan(old[1][:, cols]).all(), row
+        assert torch.isfinite(want[0][:, cols]).all() and torch.isfinite(want[1][:, cols]).all()

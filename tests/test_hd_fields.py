@@ -27,8 +27,8 @@ from _fp64 import _film, _opt, _rel, _siren, composite_ref, field_ref
 from fenerf_b200 import _lib, ops, packing
 from oracle import render_oracle as oracle
 from test_dropin import _LOAD_WITH_MIRROR, _reference_checkpoint, _run
-from test_gpu_fp64_reference import (COMPOSITE_BOUND, FIELD_BOUND, FWD_BOUND, _forward_inputs, _per_point, _render_points,
-                                     composite_vjp)
+from test_gpu_fp64_reference import (COMPOSITE_BOUND, FIELD_BOUND, FWD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward,
+                                     _field_points, _forward_inputs, _grad_errors, _per_point, _render_points, composite_vjp)
 
 DEV = "cuda:0"
 gpu = pytest.mark.gpu
@@ -330,6 +330,47 @@ def test_point_network_vs_fp64(monkeypatch, model, layout):
     assert torch.equal(fast, fast2)
     assert torch.equal(sigma, fast[..., -1:])
     assert torch.equal(sigma_x, exact[..., -1:])
+
+
+_FIELD = [(lay, m, p) for lay in ("L1", "L2", "L3") for m in ("J", "K") for p in ("exact", "default")] + \
+    [("L4", "K", p) for p in ("exact", "default")]
+
+
+@gpu
+@pytest.mark.parametrize("layout,model,precision", _FIELD, ids=["%s-%s-%s" % c for c in _FIELD])
+def test_field_backward_vs_fp64(monkeypatch, layout, model, precision):
+    """_FieldBackward against the float64 VJP under the chunk layouts of test_gpu_fp64_reference.py: the 64-wide colour
+    head, K's (64 + 8)-row head block, head_grads_feature_kernel, and FiLM rows 8 / 9 from image b0 > 0 of a chunk (L2)
+    and from images split into point chunks (L3, L4 = cfg2's pass); L2 / L3 also within LAYOUT_BOUND of a one-chunk run."""
+    from fenerf_b200 import backward
+    batch, ppb, dir_group, chunk = _LAYOUTS[layout]
+    exact = precision == "exact"
+    if exact:
+        monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
+    siren = _siren(model, DEV)
+    seed = 3200 + 10 * (model == "K") + int(layout[1])
+    pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
+    film = _film(siren, batch, seed, edges=True)
+    out_dim = siren.field_spec().out_dim
+    d_raw = torch.randn(batch, ppb, out_dim, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
+    monkeypatch.setattr(oracle, "field_eval", HD.field_eval)
+    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    raw = out64.float().contiguous()
+    if chunk:
+        monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
+    d_film, grads = _field_backward(siren, film, pts, dirs, dir_group, False, raw, d_raw, exact)
+    errs = _grad_errors(d_film, grads, want_film, want)
+    worst = max(errs, key=errs.get)
+    print("field %s %s %s: worst %s %.3g (colour head %.3g)" % (layout, model, precision, worst, errs[worst],
+                                                              errs["color_layer_linear.0.weight"]))
+    assert errs[worst] <= FIELD_BOUND[precision], {k: "%.2e" % v for k, v in errs.items() if v > FIELD_BOUND[precision]}
+    if chunk:
+        monkeypatch.setattr(backward, "CHUNK_POINTS", 1 << 30)
+        d_film1, grads1 = _field_backward(siren, film, pts, dirs, dir_group, False, raw, d_raw, exact)
+        inv = _grad_errors(d_film, grads, d_film1, grads1)
+        worst = max(inv, key=inv.get)
+        print("layout %s %s %s: worst %s %.3g" % (layout, model, precision, worst, inv[worst]))
+        assert inv[worst] <= LAYOUT_BOUND, {k: "%.2e" % v for k, v in inv.items() if v > LAYOUT_BOUND}
 
 
 @gpu
