@@ -101,16 +101,14 @@ __device__ __forceinline__ float sample_alpha(float delta, float act, float* dec
 __device__ __forceinline__ float transmittance_term(float alpha) { return __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f); }
 
 // ---- entry points of the individual translation units (called by abi.cu) ----
-int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh,
-               const fenerf_field_params* p, void* packed, cudaStream_t st);
-int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
-                       const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
-                       int lock_dirs, const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only = 0);
-int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const fenerf_field_params* p,
-                      unsigned long long* out, cudaStream_t st);
-int siren_points_fast(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
-                      const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
-                      int lock_dirs, float* out, int sigma_only, cudaStream_t st, float* sigma_out = nullptr);
+int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed, cudaStream_t st);
+int siren_points_exact(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
+                       int batch, long long ppb, int dir_group, int lock_dirs, const int32_t* only_idx, int n_only, float* out,
+                       cudaStream_t st, int sigma_only = 0);
+int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st);
+int siren_points_fast(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
+                      int batch, long long ppb, int dir_group, int lock_dirs, float* out, int sigma_only, cudaStream_t st,
+                      float* sigma_out = nullptr);
 // debug: which instantiation siren_points_fast launches (0 production; siren_fast_debug.cu) and the device software sine
 int siren_fast_debug_variant(int variant, unsigned long long* trace, int trace_ctas);
 int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st);

@@ -14,33 +14,32 @@
 //        f32:  rows 256.. = dir(3), feat(G), zero pad to KX_PAD
 //        f16:  one more 64-wide chunk in the "input chunk" slot order (see below)
 //   input-chunk image of the first layer: [256 rows][64 k] f16 (only slots 0..8 non-zero)
-//   heads            sigma: w[256], b[1]   rgb: w[3][256], b[3]   label: Weff[L][256], beff[L] (f32)
-//                    trunk-head image [4 chunks][32 rows][64 k] f16 swizzled: rows 0..L-1 the
-//                    (power-of-two scaled) label map, row L the sigma weights, rest zero
-//                    rgb-head image   [4 chunks][ 8 rows][64 k] f16 swizzled: rows 0..2
+//   heads            sigma_w   w[256], b[1] (f32)
+//                    rgb.w     [3][256] + b[3] (f32): the sigmoid colour head
+//                    label_w   [32][256] + b[32] (f32): the pre-multiplied label chain Weff, beff (then its 1/scale), or
+//                              the label FiLM branch's head
+//                    head_img  [4 chunks][32 rows][64 k] f16 swizzled: the trunk head (below)
+//                    rgb.img   [4 chunks][ 8 rows][64 k] f16 swizzled: rows 0..2 the colour head
+//                    label_scratch (doubles, pack-time only)
 //   grid             channels-last [R][R][R][G] f32 (exact path, backward)
 //   grid16           the same in f16 (wgmma path: 64 B per voxel -- the features become fp16 MMA operands anyway;
 //                    57 MB for 32 x 96^3: half the gather stream of the fp32 copy)
+//   label_img        [4 chunks][32 rows][64 k] f16 swizzled: the label FiLM branch's head (label FiLM fields only)
+//   feature heads    (FENERF_FIELD_FEATURE_HEAD fields only) the colour head and, with the label FiLM branch, its label
+//                    head: [64][256] + b[64] f32 each, then [4 chunks][64 rows][64 k] f16 each (32 KB, one ring slot of
+//                    the wgmma kernel).  These fields leave the 3-row colour sections and label_w allocated but unused.
 //
-// Label FiLM fields (FENERF_FIELD_LABEL_FILM): hidden layer trunk_hidden is the label FiLM layer, packed like any
-// hidden layer, and the colour layers follow it -- so hidden layer l still takes FiLM row l + 1, and the rows are the
-// reference's (trunk, label, colour).  The label head needs no pre-multiplication: `label_w` holds its fp32 copy in the
-// Weff / beff format (1/scale = 1), the trunk-head image carries sigma only (row label_dim, rows below zero), and the
-// label head gets an image of its own, appended after grid16 so that every other section keeps its offset:
-//   label_img        [4 chunks][32 rows][64 k] f16 swizzled: rows 0..L-1 the label head, rest zero
-// These fields live in FnLabelFilm, not in FnLayout, so that the kernels' argument blocks of the other fields keep
-// their layout.
-//
-// Feature-head fields (FENERF_FIELD_FEATURE_HEAD): the 64-wide heads get sections of their own, appended after
-// everything else (FnFeatureHead):
-//   rgb_w            [64][256] f32 + bias [64]           the colour head (linear, no sigmoid)
-//   label_w          [64][256] f32 + bias [64]           the label FiLM field's head (label_dim 64), else absent
-//   rgb_img          [4 chunks][64 rows][64 k] f16 swizzled, 32 KB = one ring slot of the wgmma kernel
-//   label_img        the same for the label head
-// The trunk-head image carries sigma in ROW 0 (no label rows), so that the trunk-only launches (density, GUARD
-// refinement) run the plain kernels on fn_trunk_view(L) -- label_dim 0, sigma at row / column 0.  The label FiLM
-// field's 32-row label image (FnLabelFilm::img) is not allocated.  fn_head_view(L, fh) is the FnLayout the
-// feature-head instantiations get: rgb_w / label_w point at the 64-row copies.
+// fn_make_layout turns the field's flags into FnLayout fields once; packers, launchers and kernels read them as they are.
+//   trunk head       rows 0..trunk_labels-1 the (power-of-two scaled) label chain, row sigma_row the sigma weights, rest
+//                    zero.  A plain field: trunk_labels = sigma_row = label_dim.  A label FiLM field: no label rows, sigma
+//                    in row label_dim.  A feature-head field: no label rows, sigma in row 0, so that its density alone runs
+//                    the plain kernels on the same layout.
+//   label FiLM       (FENERF_FIELD_LABEL_FILM) hidden slot label_layer = trunk_hidden is the label FiLM layer, packed like
+//                    any hidden layer, and the colour layers follow it (color0 = trunk_hidden + 1) -- so hidden layer l
+//                    still takes FiLM row l + 1, and the rows are the reference's (trunk, label, colour).
+//   linear heads     FnHead `rgb`, and `label` for the label FiLM branch (no chain to pre-multiply): an fp32 copy of
+//                    w_rows rows with the bias after them, at w + w_rows * 256 floats, and an image of img_rows rows;
+//                    rows from n_out on are zero.
 //
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
@@ -59,10 +58,27 @@
 #define FN_SLOT_DIR 16
 #define FN_SLOT_FEAT 32
 
+// The f16 image of a head with `rows` rows: [4 chunks][rows][64 k]
+#define FN_HEAD_IMG_BYTES(rows) ((size_t)(FN_H / FN_KCHUNK) * (rows) * FN_KCHUNK * 2)
+constexpr int FN_FEAT = 64;             // feature-head width (and the label head's of the label FiLM variant)
+constexpr int FN_FEAT_SIGMA_ROW = 0;    // a feature-head field's trunk head: sigma alone, in row 0
+
+// A linear head on the last activations: an fp32 copy and an f16 image (see above)
+struct FnHead {
+    size_t w;               // [w_rows][256] f32, then the bias [w_rows]
+    size_t img;             // [4 chunks][img_rows][64 k] f16 swizzled
+    int32_t n_out, w_rows, img_rows;
+};
+
 struct FnLayout {
+    int32_t label_film, feature_head;   // the variant flags (FENERF_FIELD_LABEL_FILM, FENERF_FIELD_FEATURE_HEAD)
     int32_t n_hidden;       // number of 256-wide FiLM layers after the first
     int32_t trunk_hidden;   // of which belong to the trunk (= trunk_layers - 1)
-    int32_t n_film;         // trunk_layers + color_layers
+    int32_t label_layer;    // hidden slot of the label FiLM layer, -1 without one
+    int32_t color0;         // hidden slot of the first colour layer
+    int32_t trunk_labels;   // label rows of the trunk head (the pre-multiplied chain's)
+    int32_t sigma_row;      // trunk-head row of sigma
+    int32_t n_film;         // FiLM rows: trunk_layers + the label FiLM layer + color_layers
     int32_t kx;             // 3 + G extra inputs of the first colour layer
     int32_t kx_pad;         // padded to a multiple of 16
     int32_t label_dim, grid_channels, grid_res, out_dim;
@@ -70,32 +86,18 @@ struct FnLayout {
     size_t first_w, first_b, first_img;
     size_t hid_w32[FN_MAX_HIDDEN], hid_b[FN_MAX_HIDDEN], hid_img[FN_MAX_HIDDEN];
     size_t color0_ximg;     // input-chunk image of the first colour layer
-    size_t sigma_w, rgb_w, label_w, head_img, rgb_img, label_scratch;
+    size_t sigma_w, label_w, head_img, label_scratch;
     size_t grid, grid16;
+    FnHead rgb;             // the colour head
+    FnHead label;           // the label FiLM branch's head (all zero without one)
     size_t total;
-};
-
-// The label FiLM branch of a FENERF_FIELD_LABEL_FILM field (all zero for other fields).
-struct FnLabelFilm {
-    int32_t on;             // 1: hidden layer `layer` is the label FiLM layer, the colour layers start at layer + 1
-    int32_t layer;          // = trunk_hidden
-    size_t img;             // label-head image (see above)
-};
-
-// The 64-wide heads of a FENERF_FIELD_FEATURE_HEAD field (all zero for other fields).
-constexpr int FN_FEAT = 64;             // feature-head width (and the label head's of the label FiLM variant)
-constexpr size_t FN_FEAT_IMG_BYTES = (size_t)(FN_H / FN_KCHUNK) * FN_FEAT * FN_KCHUNK * 2;   // 32 KB
-struct FnFeatureHead {
-    int32_t on;
-    size_t rgb_w, label_w;     // [64][256] f32 + [64] bias; label_w 0 without the label FiLM branch
-    size_t rgb_img, label_img; // [4][64 rows][64 k] f16 swizzled; label_img 0 without the label FiLM branch
 };
 
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Returns 0 and fills `L` (and `lf` / `fh` if given), -2 if the flags hold an unknown bit, -3 if they ask for a
-// feature head on a field shape no reference class has, or -1 if the description is outside what the kernels support.
-static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabelFilm* lf = nullptr, FnFeatureHead* fh = nullptr) {
+// Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head on a field shape no
+// reference class has, or -1 if the description is outside what the kernels support.
+static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     if (!f || !L) return -1;
     if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD)) return -2;
     const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
@@ -112,9 +114,15 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabe
     if (!(f->grid_channels == 0 || f->grid_channels == 32)) return -1;
     if (f->grid_channels && (f->grid_res < 2 || f->grid_res > 512)) return -1;
     if (!feature_head && f->out_dim != f->label_dim + 4) return -1;
+    L->label_film = label_film;
+    L->feature_head = feature_head;
     L->trunk_hidden = f->trunk_layers - 1;
-    L->n_hidden = L->trunk_hidden + label_film + f->color_layers;
-    L->n_film = f->trunk_layers + label_film + f->color_layers;
+    L->label_layer = label_film ? L->trunk_hidden : -1;
+    L->color0 = L->trunk_hidden + label_film;
+    L->n_hidden = L->color0 + f->color_layers;
+    L->n_film = 1 + L->n_hidden;
+    L->trunk_labels = (label_film || feature_head) ? 0 : f->label_dim;
+    L->sigma_row = feature_head ? FN_FEAT_SIGMA_ROW : f->label_dim;
     L->kx = 3 + f->grid_channels;
     L->kx_pad = (L->kx + 15) / 16 * 16;
     L->label_dim = f->label_dim;
@@ -129,52 +137,31 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L, FnLabe
     L->first_img = take(FN_IMG_BYTES);
     for (int l = 0; l < FN_MAX_HIDDEN; ++l) { L->hid_w32[l] = L->hid_b[l] = L->hid_img[l] = 0; }
     for (int l = 0; l < L->n_hidden; ++l) {
-        int k = FN_H + (l == L->trunk_hidden + label_film ? L->kx_pad : 0);   // the first colour layer's extra rows
+        int k = FN_H + (l == L->color0 ? L->kx_pad : 0);   // the first colour layer's extra rows
         L->hid_w32[l] = take((size_t)k * FN_H * 4);
         L->hid_b[l] = take(FN_H * 4);
         L->hid_img[l] = take((size_t)(FN_H / FN_KCHUNK) * FN_IMG_BYTES);
     }
     L->color0_ximg = take(FN_IMG_BYTES);
     L->sigma_w = take((FN_H + 1) * 4);
-    L->rgb_w = take((3 * FN_H + 3) * 4);
+    L->rgb = FnHead{take((3 * FN_H + 3) * 4), 0, 3, 3, 8};
     L->label_w = take((size_t)(FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL + 1) * 4);  // Weff, beff, 1/scale
-    L->head_img = take((size_t)(FN_H / FN_KCHUNK) * 32 * FN_KCHUNK * 2);
-    L->rgb_img = take((size_t)(FN_H / FN_KCHUNK) * 8 * FN_KCHUNK * 2);
+    L->head_img = take(FN_HEAD_IMG_BYTES(32));
+    L->rgb.img = take(FN_HEAD_IMG_BYTES(8));
     L->label_scratch = take((size_t)FENERF_MAX_LABEL * (FN_H + 1) * 8);  // doubles, pack-time only
     size_t r = (size_t)f->grid_res;
     L->grid = take(f->grid_channels ? r * r * r * (size_t)f->grid_channels * 4 : 4);
     L->grid16 = take(f->grid_channels ? r * r * r * (size_t)f->grid_channels * 2 : 4);
-    FnLabelFilm lab = {label_film, label_film ? L->trunk_hidden : 0, 0};
-    if (label_film && !feature_head) lab.img = take((size_t)(FN_H / FN_KCHUNK) * 32 * FN_KCHUNK * 2);
-    if (lf) *lf = lab;
-    FnFeatureHead hd = {feature_head, 0, 0, 0, 0};
+    L->label = FnHead{0, 0, 0, 0, 0};
+    if (label_film && !feature_head) L->label = FnHead{L->label_w, take(FN_HEAD_IMG_BYTES(32)), f->label_dim, FENERF_MAX_LABEL, 32};
     if (feature_head) {
-        hd.rgb_w = take((size_t)(FN_FEAT * FN_H + FN_FEAT) * 4);
-        if (label_film) hd.label_w = take((size_t)(FN_FEAT * FN_H + FN_FEAT) * 4);
-        hd.rgb_img = take(FN_FEAT_IMG_BYTES);
-        if (label_film) hd.label_img = take(FN_FEAT_IMG_BYTES);
+        L->rgb = FnHead{take((size_t)(FN_FEAT * FN_H + FN_FEAT) * 4), 0, FN_FEAT, FN_FEAT, FN_FEAT};
+        if (label_film) L->label = FnHead{take((size_t)(FN_FEAT * FN_H + FN_FEAT) * 4), 0, FN_FEAT, FN_FEAT, FN_FEAT};
+        L->rgb.img = take(FN_HEAD_IMG_BYTES(FN_FEAT));
+        if (label_film) L->label.img = take(FN_HEAD_IMG_BYTES(FN_FEAT));
     }
-    if (fh) *fh = hd;
     L->total = off;
     return 0;
-}
-
-// What the trunk-only launches (density, GUARD refinement) of a feature-head field see: no label rows, so the
-// density sits at row / column 0 of the trunk head, as packed.  Any other field passes through unchanged.
-static inline FnLayout fn_trunk_view(const FnLayout& L, const FnFeatureHead& fh) {
-    FnLayout t = L;
-    if (fh.on) t.label_dim = 0;
-    return t;
-}
-
-// The layout the feature-head kernel instantiations get: the fp32 head copies are the 64-row ones.
-static inline FnLayout fn_head_view(const FnLayout& L, const FnFeatureHead& fh) {
-    FnLayout t = L;
-    if (fh.on) {
-        t.rgb_w = fh.rgb_w;
-        if (fh.label_w) t.label_w = fh.label_w;
-    }
-    return t;
 }
 
 // Byte offset of element (row, k) inside one [rows][64] f16 image with the wgmma/TMA 128-byte

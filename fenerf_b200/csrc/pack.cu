@@ -75,16 +75,6 @@ __global__ void pack_color0_ximg_kernel(const float* __restrict__ w, int in_dim,
         *reinterpret_cast<__half*>(img + fn_sw128_offset(n, FN_SLOT_FEAT + c)) = __float2half_rn(w[(size_t)n * in_dim + 3 + c]);
 }
 
-__global__ void pack_heads_kernel(const float* __restrict__ sw, const float* __restrict__ sb,
-                                  const float* __restrict__ rw, const float* __restrict__ rb,
-                                  float* __restrict__ so, float* __restrict__ ro) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < FN_H) so[i] = sw[i];
-    if (i == 0) so[FN_H] = sb[0];
-    if (i < 3 * FN_H) ro[i] = rw[i];
-    if (i < 3) ro[3 * FN_H + i] = rb[i];
-}
-
 // ---- label chain: Weff = W3 W2 W1, beff = W3 (W2 b1 + b2) + b3, in double ---------------------
 // step 1: U = W3 W2 (L x 256), ub = W3 b2 + b3          grid L blocks x 256 threads
 __global__ void label_step1_kernel(const float* __restrict__ w3, const float* __restrict__ b3,
@@ -139,55 +129,39 @@ __global__ void label_step3_kernel(float* __restrict__ lw, int L) {
     if (threadIdx.x == 0) lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] = 1.f / scale;
 }
 
-// label head of a label FiLM field (one block): the fp32 copy in the Weff / beff format (1/scale = 1) and the
-// label-head image [4][32 rows][64 k], rows 0..L-1
-__global__ void pack_label_film_head_kernel(const float* __restrict__ w, const float* __restrict__ b, int L,
-                                            float* __restrict__ lw, unsigned char* __restrict__ img) {
-    for (int i = threadIdx.x; i < 32 * FN_H; i += blockDim.x) {
-        int row = i / FN_H, k = i % FN_H;
-        const float v = row < L ? w[row * FN_H + k] : 0.f;
-        lw[row * FN_H + k] = v;
-        unsigned char* chunk = img + (size_t)(k / FN_KCHUNK) * (32 * FN_KCHUNK * 2);
-        *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
-    }
-    if (threadIdx.x < FENERF_MAX_LABEL) lw[FENERF_MAX_LABEL * FN_H + threadIdx.x] = (int)threadIdx.x < L ? b[threadIdx.x] : 0.f;
-    if (threadIdx.x == 0) lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] = 1.f;
-}
-
-// a 64-wide head of a feature-head field (one block): fp32 copy [64][256] + bias [64], and its image
-// [4 chunks][64 rows][64 k] f16 swizzled
-__global__ void pack_feature_head_kernel(const float* __restrict__ w, const float* __restrict__ b, float* __restrict__ lw,
-                                         unsigned char* __restrict__ img) {
-    for (int i = threadIdx.x; i < FN_FEAT * FN_H; i += blockDim.x) {
+// a linear head (layout.h, FnHead; one block): the fp32 copy [w_rows][256] + bias [w_rows] and the image
+// [4 chunks][img_rows][64 k], rows from n_out on zero
+__global__ void pack_linear_head_kernel(const float* __restrict__ w, const float* __restrict__ b, FnHead h,
+                                        unsigned char* __restrict__ packed) {
+    float* lw = reinterpret_cast<float*>(packed + h.w);
+    const int rows = h.w_rows > h.img_rows ? h.w_rows : h.img_rows;
+    for (int i = threadIdx.x; i < rows * FN_H; i += blockDim.x) {
         const int row = i / FN_H, k = i % FN_H;
-        const float v = w[i];
-        lw[i] = v;
-        unsigned char* chunk = img + (size_t)(k / FN_KCHUNK) * (FN_FEAT * FN_KCHUNK * 2);
-        *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
+        const float v = row < h.n_out ? w[i] : 0.f;
+        if (row < h.w_rows) lw[i] = v;
+        if (row < h.img_rows) {
+            unsigned char* chunk = packed + h.img + (size_t)(k / FN_KCHUNK) * (h.img_rows * FN_KCHUNK * 2);
+            *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
+        }
     }
-    if (threadIdx.x < FN_FEAT) lw[FN_FEAT * FN_H + threadIdx.x] = b[threadIdx.x];
+    for (int i = threadIdx.x; i < h.w_rows; i += blockDim.x) lw[h.w_rows * FN_H + i] = i < h.n_out ? b[i] : 0.f;
 }
 
-// head images for the wgmma kernel (one block):
-//   trunk head  [4][32 rows][64 k]: rows 0..label_rows-1 = Weff * scale, row L = sigma weights
-//               (label_rows = L, or 0 for a label FiLM field, whose label head has an image of its own)
-//   rgb head    [4][ 8 rows][64 k]: rows 0..2
-__global__ void pack_head_imgs_kernel(const float* __restrict__ lw, int L, int label_rows, const float* __restrict__ sigma_w,
-                                      const float* __restrict__ rgb_w, unsigned char* __restrict__ head_img,
-                                      unsigned char* __restrict__ rgb_img) {
-    const float scale = L > 0 ? 1.f / lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] : 1.f;
+// the trunk head (one block): the fp32 sigma copy, and the image [4][32 rows][64 k]: rows 0..trunk_labels-1 = Weff *
+// scale, row sigma_row = the sigma weights (layout.h)
+__global__ void pack_trunk_head_kernel(const float* __restrict__ sw, const float* __restrict__ sb, FnLayout L,
+                                       unsigned char* __restrict__ packed) {
+    const float* lw = reinterpret_cast<const float*>(packed + L.label_w);
+    float* so = reinterpret_cast<float*>(packed + L.sigma_w);
+    const float scale = L.trunk_labels > 0 ? 1.f / lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL] : 1.f;
+    for (int i = threadIdx.x; i < FN_H; i += blockDim.x) so[i] = sw[i];
+    if (threadIdx.x == 0) so[FN_H] = sb[0];
     for (int i = threadIdx.x; i < 32 * FN_H; i += blockDim.x) {
         int row = i / FN_H, k = i % FN_H;
         float v = 0.f;
-        if (row < label_rows) v = lw[row * FN_H + k] * scale;
-        else if (row == L) v = sigma_w[k];
-        unsigned char* chunk = head_img + (size_t)(k / FN_KCHUNK) * (32 * FN_KCHUNK * 2);
-        *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
-    }
-    for (int i = threadIdx.x; i < 8 * FN_H; i += blockDim.x) {
-        int row = i / FN_H, k = i % FN_H;
-        float v = row < 3 ? rgb_w[row * FN_H + k] : 0.f;
-        unsigned char* chunk = rgb_img + (size_t)(k / FN_KCHUNK) * (8 * FN_KCHUNK * 2);
+        if (row < L.trunk_labels) v = lw[row * FN_H + k] * scale;
+        else if (row == L.sigma_row) v = sw[k];
+        unsigned char* chunk = packed + L.head_img + (size_t)(k / FN_KCHUNK) * (32 * FN_KCHUNK * 2);
         *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
     }
 }
@@ -250,20 +224,18 @@ __global__ void fingerprint_kernel(FpSegments seg, unsigned long long* __restric
 
 }  // namespace
 
-int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const fenerf_field_params* p,
-                      unsigned long long* out, cudaStream_t st) {
-    const int rgb_rows = fh.on ? FN_FEAT : 3;
+int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st) {
     FpSegments seg;
     seg.n = 0;
     auto add = [&](const float* ptr, unsigned long long count) {
         if (ptr && count) { seg.ptr[seg.n] = ptr; seg.count[seg.n] = count; ++seg.n; }
     };
     // (a label FiLM layer takes a hidden slot: it is hashed with the label parameters below, label_w[0])
-    const int n_trunk = L.trunk_hidden + 1, n_color = L.n_hidden - L.trunk_hidden - lf.on;
+    const int n_trunk = L.trunk_hidden + 1, n_color = L.n_hidden - L.color0;
     for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? 3 : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
     add(p->sigma_w, FN_H); add(p->sigma_b, 1);
     for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (unsigned long long)(i == 0 ? L.kx + FN_H : FN_H) * FN_H); add(p->color_b[i], FN_H); }
-    add(p->rgb_w, (unsigned long long)rgb_rows * FN_H); add(p->rgb_b, rgb_rows);
+    add(p->rgb_w, (unsigned long long)L.rgb.n_out * FN_H); add(p->rgb_b, L.rgb.n_out);
     if (L.label_dim > 0) {
         add(p->label_w[0], FN_H * FN_H); add(p->label_b[0], FN_H);
         add(p->label_w[1], FN_H * FN_H); add(p->label_b[1], FN_H);
@@ -276,22 +248,20 @@ int field_fingerprint(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureH
     return 0;
 }
 
-int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh,
-               const fenerf_field_params* p, void* packed_v, cudaStream_t st) {
+int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, cudaStream_t st) {
     unsigned char* packed = static_cast<unsigned char*>(packed_v);
     FN_REQUIRE(p->trunk_w[0] && p->trunk_b[0], "trunk_w[0]/trunk_b[0] missing");
     pack_first_kernel<<<1, 256, 0, st>>>(p->trunk_w[0], p->trunk_b[0], (float*)(packed + L.first_w),
                                          (float*)(packed + L.first_b), packed + L.first_img);
     FN_LAUNCH_OK("pack_first_kernel");
-    if (lf.on)
+    if (L.label_film)
         FN_REQUIRE(p->label_w[0] && p->label_b[0] && p->label_w[2] && p->label_b[2] && !p->label_w[1] && !p->label_b[1],
                    "label FiLM field: label_w/b[0] (FiLM layer) and [2] (head) required, [1] must be NULL");
-    const int c0 = L.trunk_hidden + lf.on;    // hidden slot of the first colour layer
     for (int l = 0; l < L.n_hidden; ++l) {
-        bool is_c0 = (l == c0);
-        const bool is_label = lf.on && l == lf.layer;
-        const float* w = l < L.trunk_hidden ? p->trunk_w[l + 1] : is_label ? p->label_w[0] : p->color_w[l - c0];
-        const float* b = l < L.trunk_hidden ? p->trunk_b[l + 1] : is_label ? p->label_b[0] : p->color_b[l - c0];
+        bool is_c0 = (l == L.color0);
+        const bool is_label = l == L.label_layer;
+        const float* w = l < L.trunk_hidden ? p->trunk_w[l + 1] : is_label ? p->label_w[0] : p->color_w[l - L.color0];
+        const float* b = l < L.trunk_hidden ? p->trunk_b[l + 1] : is_label ? p->label_b[0] : p->color_b[l - L.color0];
         FN_REQUIRE(w && b, "weight/bias of hidden layer %d missing", l);
         int in_dim = is_c0 ? L.kx + FN_H : FN_H;
         int x_off = is_c0 ? L.kx : 0;
@@ -306,22 +276,12 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm&
         }
     }
     FN_REQUIRE(p->sigma_w && p->sigma_b && p->rgb_w && p->rgb_b, "sigma/rgb head parameters missing");
-    pack_heads_kernel<<<3, 256, 0, st>>>(p->sigma_w, p->sigma_b, p->rgb_w, p->rgb_b, (float*)(packed + L.sigma_w),
-                                         (float*)(packed + L.rgb_w));
-    FN_LAUNCH_OK("pack_heads_kernel");
-    if (fh.on) {             // the 64-wide heads, in sections of their own (layout.h)
-        pack_feature_head_kernel<<<1, 256, 0, st>>>(p->rgb_w, p->rgb_b, (float*)(packed + fh.rgb_w), packed + fh.rgb_img);
-        FN_LAUNCH_OK("pack_feature_head_kernel");
-        if (lf.on) {
-            pack_feature_head_kernel<<<1, 256, 0, st>>>(p->label_w[2], p->label_b[2], (float*)(packed + fh.label_w),
-                                                        packed + fh.label_img);
-            FN_LAUNCH_OK("pack_feature_head_kernel");
-        }
-    } else if (lf.on) {      // no chain to pre-multiply: the head is one Linear
-        pack_label_film_head_kernel<<<1, 256, 0, st>>>(p->label_w[2], p->label_b[2], L.label_dim, (float*)(packed + L.label_w),
-                                                       packed + lf.img);
-        FN_LAUNCH_OK("pack_label_film_head_kernel");
-    } else if (L.label_dim > 0) {
+    pack_linear_head_kernel<<<1, 256, 0, st>>>(p->rgb_w, p->rgb_b, L.rgb, packed);
+    FN_LAUNCH_OK("pack_linear_head_kernel");
+    if (L.label_film) {      // no chain to pre-multiply: the head is one Linear
+        pack_linear_head_kernel<<<1, 256, 0, st>>>(p->label_w[2], p->label_b[2], L.label, packed);
+        FN_LAUNCH_OK("pack_linear_head_kernel");
+    } else if (L.trunk_labels > 0) {
         for (int i = 0; i < 3; i += 2) FN_REQUIRE(p->label_w[i] && p->label_b[i], "label layer %d missing", i);
         FN_REQUIRE((p->label_w[1] == nullptr) == (p->label_b[1] == nullptr), "label layer 1: weight and bias must both be given or both be NULL");
         double* u = reinterpret_cast<double*>(packed + L.label_scratch);
@@ -333,11 +293,8 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm&
         label_step3_kernel<<<1, 256, 0, st>>>((float*)(packed + L.label_w), L.label_dim);
         FN_LAUNCH_OK("label_step3_kernel");
     }
-    // (a feature-head field: no label rows, sigma in row 0 -- layout.h)
-    pack_head_imgs_kernel<<<1, 256, 0, st>>>((const float*)(packed + L.label_w), fh.on ? 0 : L.label_dim, lf.on ? 0 : L.label_dim,
-                                             p->sigma_w, p->rgb_w,
-                                             packed + L.head_img, packed + L.rgb_img);
-    FN_LAUNCH_OK("pack_head_imgs_kernel");
+    pack_trunk_head_kernel<<<1, 256, 0, st>>>(p->sigma_w, p->sigma_b, L, packed);
+    FN_LAUNCH_OK("pack_trunk_head_kernel");
     if (L.grid_channels > 0) {
         FN_REQUIRE(p->grid, "grid missing");
         int R = L.grid_res, G = L.grid_channels;
@@ -348,7 +305,6 @@ int pack_field(const fenerf_field_desc* f, const FnLayout& L, const FnLabelFilm&
         pack_grid_kernel<<<R * R, 256, smem, st>>>(p->grid, (float*)(packed + L.grid), (__half*)(packed + L.grid16), R, G);
         FN_LAUNCH_OK("pack_grid_kernel");
     }
-    (void)f;
     return 0;
 }
 

@@ -18,15 +18,14 @@
 //   each thread owns a 4-point x 16-column micro tile; 5 LDS.128 feed 64 FFMA per k
 //   (the 16-point gather variant maps lanes point-major so a warp's weight reads broadcast)
 //
+// The heads are ordered fp32 k-sums over the fp32 copies that the layout describes (layout.h): the trunk head (sigma and
+// the pre-multiplied label chain), the colour head (L.rgb) and the label FiLM branch's head (L.label).
+//
 // Label FiLM fields (kLabelFilm): A keeps the trunk output for the first colour layer, so the label FiLM layer's output
 // goes through the weight-slab buffer instead, which is free between layers: one 64-feature quarter at a time, each
 // followed by its share of the label head's k-sum (the running sums sit in the same buffer), so shared memory and
-// occupancy stay those of the other fields.
-//
-// Feature-head fields (kFeatureHead, FENERF_FIELD_FEATURE_HEAD): the colour head is 64 linear outputs (no sigmoid) and
-// the label FiLM branch's head 64 rows; both are ordered fp32 k-sums like the 3- / label_dim-row heads.  The label
-// activations (64 x TM) and the 64 running sums fill the weight-slab buffer exactly.  The kernel gets
-// fn_head_view(L): rgb_w / label_w are the 64-row copies.
+// occupancy stay those of the other fields.  With the 64-row label head of a feature-head field (kFeatureHead) the label
+// activations (64 x TM) and the 64 running sums fill the buffer exactly; its colour head has no sigmoid.
 #include "siren_common.cuh"
 #include "sm90.cuh"
 
@@ -255,8 +254,8 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                 // heads on the trunk output: sigma, then the pre-multiplied label map
                 const float* sw = reinterpret_cast<const float*>(pk + L.sigma_w);
                 const float* lw = reinterpret_cast<const float*>(pk + L.label_w);
-                // (a label FiLM field's labels come from its label branch below)
-                for (int it = tid; it < TM * (1 + ((kLabelFilm || a.sigma_only) ? 0 : L.label_dim)); it += NTHREADS) {
+                // (a label FiLM field's labels come from its label branch below: no trunk label rows)
+                for (int it = tid; it < TM * (1 + (a.sigma_only ? 0 : L.trunk_labels)); it += NTHREADS) {
                     int pt = it % TM, o = it / TM;
                     const float* w = o == 0 ? sw : lw + (size_t)(o - 1) * FN_H;
                     float r = o == 0 ? __ldg(sw + FN_H) : __ldg(lw + FENERF_MAX_LABEL * FN_H + (o - 1));
@@ -278,15 +277,16 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                 if (a.sigma_only) break;          // the colour branch does not feed the density
                 if constexpr (kLabelFilm) {
                     // ---- label FiLM layer (hidden layer l) on the trunk output, then the label head ----
-                    constexpr int kLabelRows = kFeatureHead ? FN_FEAT : FENERF_MAX_LABEL;   // bias offset of the head copy
-                    static_assert(sizeof(s.W) >= (64 + kLabelRows) * TM * sizeof(float), "label scratch fits the slab buffer");
+                    constexpr int kMaxLabels = kFeatureHead ? FN_FEAT : FENERF_MAX_LABEL;
+                    static_assert(sizeof(s.W) >= (64 + kMaxLabels) * TM * sizeof(float), "label scratch fits the slab buffer");
                     init_bias(reinterpret_cast<const float*>(pk + L.hid_b[l]), acc, tid);
                     gemm_tile(s, reinterpret_cast<const float*>(pk + L.hid_w32[l]), FN_H, acc, tid);   // ends in a barrier
                     // the slab buffer: [64 features][TM points] of label activations, then the running sums [label][TM]
                     float* lab = &s.W[0][0][0];
                     float* sums = lab + 64 * TM;
-                    const float* lw = reinterpret_cast<const float*>(pk + L.label_w);
-                    const int n_items = TM * L.label_dim;
+                    const float* lw = reinterpret_cast<const float*>(pk + L.label.w);
+                    const float* lb = lw + (size_t)L.label.w_rows * FN_H;
+                    const int n_items = TM * L.label.n_out;
                     // one 64-feature quarter at a time (this thread's column group j): the FiLM epilogue, rounded as
                     // film_store (FiLM row l + 1), then its share of the head's k-sum -- the sums run over k = 0 .. 255 in
                     // order, as the trunk heads' do
@@ -307,7 +307,7 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                         for (int it = tid; it < n_items; it += NTHREADS) {
                             const int pt = it % TM, o = it / TM;
                             const float* w = lw + (size_t)o * FN_H + 64 * j;
-                            float r = j == 0 ? __ldg(lw + kLabelRows * FN_H + o) : sums[it];   // bias first
+                            float r = j == 0 ? __ldg(lb + o) : sums[it];   // bias first
 #pragma unroll 8
                             for (int k = 0; k < 64; ++k) r = fmaf(lab[k * TM + pt], __ldg(w + k), r);
                             sums[it] = r;
@@ -322,7 +322,7 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                     continue;                                                  // s.A still holds the trunk output
                 }
             }
-            const int K = FN_H + (l == L.trunk_hidden + (kLabelFilm ? 1 : 0) ? L.kx_pad : 0);
+            const int K = FN_H + (l == L.color0 ? L.kx_pad : 0);
             init_bias(reinterpret_cast<const float*>(pk + L.hid_b[l]), acc, tid);
             gemm_tile(s, reinterpret_cast<const float*>(pk + L.hid_w32[l]), K, acc, tid);
             film_store(s, a.film, L.n_film, l + 1, acc, tid);
@@ -330,11 +330,11 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
         }
         // ---- rgb head: sigmoid(Linear(256 -> 3)); a feature head: Linear(256 -> 64) ----
         if (!a.sigma_only) {
-            constexpr int kRgb = kFeatureHead ? FN_FEAT : 3;
-            const float* rw = reinterpret_cast<const float*>(pk + L.rgb_w);
-            for (int it = tid; it < TM * kRgb; it += NTHREADS) {
+            const float* rw = reinterpret_cast<const float*>(pk + L.rgb.w);
+            const float* rb = rw + (size_t)L.rgb.w_rows * FN_H;
+            for (int it = tid; it < TM * L.rgb.n_out; it += NTHREADS) {
                 int pt = it % TM, o = it / TM;
-                float r = __ldg(rw + kRgb * FN_H + o);
+                float r = __ldg(rb + o);
                 for (int k = 0; k < FN_H; ++k) r = fmaf(s.A[k][pt], __ldg(rw + o * FN_H + k), r);
                 if (!kFeatureHead) r = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-r)));
                 long long flat = s.flat[pt];
@@ -364,15 +364,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_exact_guard_kernel(ExactArg
 
 }  // namespace
 
-int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const FnFeatureHead& fh, const unsigned char* packed,
-                       const float* points, const float* dirs, const float* film, int batch, long long ppb, int dir_group,
-                       int lock_dirs, const int32_t* only_idx, int n_only, float* out, cudaStream_t st, int sigma_only) {
+int siren_points_exact(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
+                       int batch, long long ppb, int dir_group, int lock_dirs, const int32_t* only_idx, int n_only, float* out,
+                       cudaStream_t st, int sigma_only) {
     static_assert(sizeof(Smem<4>) <= 113 * 1024, "two CTAs per SM must fit");
     constexpr int TM = 64;
     ExactArgs a;
-    // (a feature-head field: the 64-row head copies for its own instantiations, no label rows for the density alone)
-    const bool feature_head = fh.on && !sigma_only;
-    a.L = feature_head ? fn_head_view(L, fh) : fn_trunk_view(L, fh);
+    a.L = L;
     a.packed = packed; a.points = points; a.dirs = dirs; a.film = film; a.only_idx = only_idx; a.out = out;
     a.n_only_dev = nullptr; a.guard_stats = nullptr;
     a.ppb = ppb; a.n_only = n_only; a.dir_group = dir_group < 1 ? 1 : dir_group; a.lock_dirs = lock_dirs;
@@ -385,13 +383,13 @@ int siren_points_exact(const FnLayout& L, const FnLabelFilm& lf, const FnFeature
     FN_REQUIRE(ppb % a.dir_group == 0, "points_per_batch %lld not a multiple of dir_group %d", ppb, a.dir_group);
     size_t smem = sizeof(Smem<4>);
     int blocks = (int)(a.n_items < (long long)num_sms() * 2 ? a.n_items : (long long)num_sms() * 2);
-    // (the density alone never reaches the label branch: sigma_only runs the plain instantiation)
+    // (the density alone never reaches the heads after the trunk: sigma_only runs the plain instantiation)
     auto launch = [&](auto kernel) -> int {
         FN_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kernel<<<blocks, NTHREADS, smem, st>>>(a);
         return 0;
     };
-    const bool label_film = lf.on && !sigma_only;
+    const bool label_film = L.label_film && !sigma_only, feature_head = L.feature_head && !sigma_only;
     int e;
     if (feature_head) {
         if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true, true>) : launch(siren_exact_kernel<true, 4, false, true>);

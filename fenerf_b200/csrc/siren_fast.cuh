@@ -24,19 +24,19 @@
 // The input slots of a point (layout.h: positions, view direction and grid features, hi / lo split in fp16) are
 // built once per tile by one thread per point into a small staging buffer and read from there as A fragments.
 //
-// Label FiLM fields (FENERF_FIELD_LABEL_FILM, the kLabelFilm instantiation): after the trunk head (sigma only), the label
-// FiLM layer runs on the trunk activations, which stay in `act` for the first colour layer.  Each half of its output goes
-// through the FiLM epilogue into `nxt` and straight into the m64n32 label head (k-slices 8h .. 8h+7), so the label
-// activations never need more than those 32 registers: four turns, [layer half 0] [head on it] [layer half 1] [head].
+// The kernel reads where sigma and the labels sit, and where each head's bias is, from the layout (layout.h); the
+// feature-head instantiations take these as the constants fn_make_layout writes for their fields (see the trunk head).
+// The template flags choose the MMA shapes and the turn sequence:
+//   kLabelFilm     (FENERF_FIELD_LABEL_FILM) after the trunk head, the label FiLM layer runs on the trunk activations,
+//                  which stay in `act` for the first colour layer.  Each half of its output goes through the FiLM epilogue
+//                  into `nxt` and straight into the label head (k-slices 8h .. 8h+7), so the label activations never need
+//                  more than those 32 registers: four turns, [layer half 0] [head on it] [layer half 1] [head].
+//   kFeatureHead   (FENERF_FIELD_FEATURE_HEAD) the colour head is m64n64, 64 linear outputs with no sigmoid, and so is
+//                  the label head (m64n32 otherwise).  Each of their images is one 32 KB ring slot.
 //
-// Feature-head fields (FENERF_FIELD_FEATURE_HEAD, the kFeatureHead instantiations): the colour head is m64n64 on the
-// colour activations, 64 linear outputs with their bias and no sigmoid; the label FiLM variant's head is m64n64 too, with
-// the same turn sequence.  Each head image is [4 chunks][64 rows][64 k], one 32 KB ring slot.  The trunk head carries
-// sigma only, in column 0.  The kernel gets fn_head_view(L): rgb_w / label_w are the 64-row fp32 copies (for the biases).
-//
-// The kernel is a template over the label FiLM branch and the feature head; the plain and the label FiLM
-// instantiations live in translation units of their own (siren_fast.cu, siren_fast_label.cu), the two feature-head
-// ones in a third (siren_fast_hd.cu), so that the plain one compiles exactly as it does on its own.  The debug
+// The plain and the label FiLM instantiations live in translation units of their own (siren_fast.cu,
+// siren_fast_label.cu), the two feature-head ones in a third (siren_fast_hd.cu), so that the plain one compiles exactly as
+// it does on its own.  The debug
 // instantiations -- a share of the sines on the FMA pipe (kSoftSin, soft_sinf) and the clock64 timeline (kTrace) -- live
 // in siren_fast_debug.cu.
 #pragma once
@@ -219,8 +219,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
     const FnLayout& L = a.L;
     const int C = L.out_dim;
     const float* sigma_w = reinterpret_cast<const float*>(a.packed + L.sigma_w);
-    const float* rgb_w = reinterpret_cast<const float*>(a.packed + L.rgb_w);
     const float* label_w = reinterpret_cast<const float*>(a.packed + L.label_w);
+    // The heads' rows as the layout states them.  The feature-head instantiations use the values fn_make_layout writes
+    // for their fields as constants: read at run time, the row compares changed the schedule of their FiLM epilogue
+    // (BASELINEHD about 3 % slower on an H100).  Only the plain instantiation meets trunk label rows.
+    const int trunk_labels = (kLabelFilm || kFeatureHead) ? 0 : L.trunk_labels;
+    const int sigma_row = kFeatureHead ? FN_FEAT_SIGMA_ROW : L.sigma_row;
+    const int rgb_rows = kFeatureHead ? FN_FEAT : L.rgb.w_rows;
+    const int label_rows = kFeatureHead ? FN_FEAT : L.label.w_rows;
     __half* xs = reinterpret_cast<__half*>(smem + SMEM_X) + wg * TILE * XSTRIDE;
     uint32_t it = 0;
     // the next load of the stream: wait until it has landed, return its slot's shared-memory address
@@ -394,7 +400,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 fence_regs(dh);
                 fence_regs(act);
                 release(slot);
-                const float inv_scale = L.label_dim > 0 ? __ldg(label_w + FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL) : 1.f;
+                // the chain's beff, then its 1/scale, read where a label is written (hoisted out of the layer loop
+                // beside trunk_labels and sigma_row, it cost the hidden layers' MMA issue a uniform register)
                 const float* lb = label_w + FENERF_MAX_LABEL * FN_H;
 #pragma unroll
                 for (int rr = 0; rr < 2; ++rr) {
@@ -407,9 +414,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                         for (int e = 0; e < 2; ++e) {
                             const int o = 8 * i + 2 * q + e;
                             const float v = dh[4 * i + 2 * rr + e];
-                            if (!kFeatureHead && o < L.label_dim) {   // (zero rows for a label FiLM field: its labels come below)
-                                if (!kLabelFilm && !a.sigma_only) a.out[flat * C + o] = fmaf(v, inv_scale, __ldg(lb + o));
-                            } else if (o == (kFeatureHead ? 0 : L.label_dim)) {   // a feature-head field: sigma in row 0
+                            if (o < trunk_labels) {
+                                if (!a.sigma_only) a.out[flat * C + o] = fmaf(v, __ldg(lb + FENERF_MAX_LABEL), __ldg(lb + o));
+                            } else if (o == sigma_row) {
                                 const float sig = v + __ldg(sigma_w + FN_H);
                                 a.out[flat * C + (C - 1)] = sig;
                                 if (a.sigma_out) a.sigma_out[flat] = sig;
@@ -472,20 +479,20 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                         const long long pnt = p0 + r0 + 8 * rr;
                         if (pnt >= a.ppb) continue;
                         const long long flat = b * a.ppb + pnt;
-                        const float* lbias = kFeatureHead ? label_w + FN_FEAT * FN_H : lb;
+                        const float* lbias = reinterpret_cast<const float*>(a.packed + L.label.w) + label_rows * FN_H;
 #pragma unroll
                         for (int i = 0; i < kLabN / 8; ++i)
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int o = 8 * i + 2 * q + e;
-                                if (o < L.label_dim) a.out[flat * C + o] = dl[4 * i + 2 * rr + e] + __ldg(lbias + o);
+                                if (o < L.label.n_out) a.out[flat * C + o] = dl[4 * i + 2 * rr + e] + __ldg(lbias + o);
                             }
                     }
                     continue;                        // act still holds the trunk output: the colour layers follow
                 }
             }
             // ---- FiLM layer l + 1: weight image halves 64 KB apart, two 32 KB slabs per half ----
-            const bool c0 = (l == L.trunk_hidden + (kLabelFilm ? 1 : 0));   // first colour layer: + direction / grid-feature slots
+            const bool c0 = (l == L.color0);     // first colour layer: + direction / grid-feature slots
             const int nx = L.grid_channels > 0 ? 3 : 1;
             uint32_t xf[3][4];
             if (c0)
@@ -553,6 +560,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             fence_regs(dr);
             fence_regs(act);
             release(slot);
+            const float* rgb_b = reinterpret_cast<const float*>(a.packed + L.rgb.w) + rgb_rows * FN_H;
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const long long pnt = p0 + r0 + 8 * rr;
@@ -563,7 +571,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const int o = 8 * i + 2 * q + e;
-                        a.out[flat * C + L.label_dim + o] = dr[4 * i + 2 * rr + e] + __ldg(rgb_w + FN_FEAT * FN_H + o);
+                        a.out[flat * C + L.label_dim + o] = dr[4 * i + 2 * rr + e] + __ldg(rgb_b + o);
                     }
             }
             continue;
@@ -586,6 +594,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             fence_regs(dr);
             fence_regs(act);
             release(slot);
+            const float* rgb_b = reinterpret_cast<const float*>(a.packed + L.rgb.w) + rgb_rows * FN_H;
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const long long pnt = p0 + r0 + 8 * rr;
@@ -595,7 +604,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 for (int e = 0; e < 2; ++e) {
                     const int o = 2 * q + e;
                     if (o < 3) {
-                        const float x = dr[2 * rr + e] + __ldg(rgb_w + 3 * FN_H + o);
+                        const float x = dr[2 * rr + e] + __ldg(rgb_b + o);
                         a.out[flat * C + L.label_dim + o] = __fdividef(1.f, 1.f + __expf(-x));
                     }
                 }
