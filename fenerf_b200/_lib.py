@@ -14,6 +14,7 @@ MAX_TRUNK, MAX_COLOR, MAX_LABEL, HIDDEN = 8, 8, 32, 256
 
 ABI_VERSION = 3
 FIELD_LABEL_FILM = 0x1        # fenerf_field_desc.reserved (the flags word): FENERF_FIELD_LABEL_FILM
+FIELD_GRID_TRUNK = 0x2        # FENERF_FIELD_GRID_TRUNK: the grid features feed the first trunk layer
 FIELD_FEATURE_HEAD = 0x8      # FENERF_FIELD_FEATURE_HEAD: Linear(256 -> 64) colour head without the sigmoid
 PRECISION = {"exact": 0, "fast": 1, "guard": 2}
 CLAMP = {"relu": 0, "softplus": 1}

@@ -19,7 +19,8 @@ backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per
           Every gradient of the layer follows from M_b and dp_b without another pass over the points, and none divides
           by f (a frequency of exactly 0 is reachable from the mapping network's 15 x + 30):
           dW = sum_b diag(f_b) M_b,  db = sum_b f_b dp_b,  df_b = rowsum(W * M_b) + b dp_b   (u = f z + p, z = W a + b).
-          Heads, the pre-multiplied label chain and the grid (``fenerf_grid_scatter_add``) close the chain.  A label FiLM
+          Heads, the pre-multiplied label chain and the grid (``fenerf_grid_scatter_add``, from the first colour layer's
+          dU, or from the first layer's where the grid feeds the trunk, EmbeddingPiGAN256) close the chain.  A label FiLM
           field (SPATIALSIRENSEMANTIC) recomputes its label layer from the trunk output at FiLM row T and runs it
           backward like a colour layer, its dU diag(f) W joining the trunk's dA.
 Gradients flow to the FiLM table (and through torch's autograd into the mapping network / latents /
@@ -150,12 +151,17 @@ class _FieldBackward:
         self.lf = len(self.fw.label_film)                          # 1: a label FiLM layer at row T, colour from T + 1
         self.T, self.Cn, self.c0, self.n_film = T, Cn, T + self.lf, T + self.lf + Cn
         G = self.spec.grid_channels
-        self.kx = 3 + G
+        # narrow inputs: the first layer's [pos] -- [feat, pos] with the grid in the trunk (EmbeddingPiGAN256) -- and the
+        # first colour layer's [dir, feat] -- [dir] with the grid in the trunk
+        self.gt = self.spec.grid_trunk
+        self.k0 = 3 + G if self.gt else 3
+        self.k0_pad = (self.k0 + 7) // 8 * 8
+        self.kx = 3 if self.gt else 3 + G
         self.kx_pad = (self.kx + 7) // 8 * 8
         # per-image accumulators (scaled by `scale`)
         self.colsum = torch.zeros((B, self.n_film, 256), dtype=torch.float32, device=dev)
         self.dW_b = [None] * self.n_film
-        self.dW_b[0] = torch.zeros((B, 256, 8), dtype=torch.float32, device=dev)
+        self.dW_b[0] = torch.zeros((B, 256, self.k0_pad), dtype=torch.float32, device=dev)
         for i in range(1, self.n_film):
             self.dW_b[i] = torch.zeros((B, 256, 256), dtype=torch.float32, device=dev)
         self.dWx_b = torch.zeros((B, 256, self.kx_pad), dtype=torch.float32, device=dev)   # colour 0's narrow inputs
@@ -173,13 +179,16 @@ class _FieldBackward:
             self.grid_grad_cl = torch.zeros((r, r, r, G), dtype=torch.float32, device=dev)
         # fp16 / fp32 weight views for the GEMMs
         fw = self.fw
-        self.W0 = fw.trunk[0][0].detach().float().contiguous()                    # (256, 3)
+        self.W0 = fw.trunk[0][0].detach().float().contiguous()                    # (256, 3); grid trunk (256, G + 3)
         self.own_gemm = (not exact) and BWD_GEMM == "wgmma"
         self.Wh16 = [None] + [w.detach().to(self.dt).contiguous() for w, _ in fw.trunk[1:]]
         wc0 = fw.color[0][0].detach().float()
         self.Wc0x_narrow = wc0[:, :self.kx].contiguous()                          # (256, 3 + G) fp32
         self.Wc16 = [wc0[:, self.kx:].to(self.dt).contiguous()] + [w.detach().to(self.dt).contiguous() for w, _ in fw.color[1:]]
-        self.Wfeat32 = wc0[:, 3:self.kx].contiguous() if G else None                  # (256, G)
+        # the weights the grid features meet, (256, G): the first colour layer's, or the first layer's with the grid in
+        # the trunk, whose FiLM row is then 0
+        self.feat_row = 0 if self.gt else self.c0
+        self.Wfeat32 = (self.W0[:, :G] if self.gt else wc0[:, 3:self.kx].contiguous()) if G else None
         # fp32 weights of the chain products dA' = dU diag(f_b) W, by FiLM row (row 0 has none: its inputs are the points)
         self.Wchain32 = [None] + [w.detach().float() for w, _ in fw.trunk[1:]]
         if self.lf:
@@ -191,7 +200,7 @@ class _FieldBackward:
         fW = self.film[:, 1:, 0].unsqueeze(3) * torch.stack(self.Wchain32[1:])
         self.fW = fW.transpose(2, 3).to(torch.float16).contiguous() if self.own_gemm else fW.to(self.dt)
         del fW
-        self.fWfeat = (self.film[:, self.c0, 0].unsqueeze(2) * self.Wfeat32).to(self.dt) if G else None    # (B, 256, G)
+        self.fWfeat = (self.film[:, self.feat_row, 0].unsqueeze(2) * self.Wfeat32).to(self.dt) if G else None    # (B, 256, G)
         if self.own_gemm:
             self.Wn64 = torch.zeros((256, 64), dtype=torch.float16, device=dev)
             self.Wn64[:, :self.kx] = self.Wc0x_narrow
@@ -264,9 +273,13 @@ class _FieldBackward:
             st = _stream(dev)
             # ---- recompute the forward, stashing activations and gates (fp16) ----
             x = (points.reshape(P, 3) * spec.input_scale).contiguous() if spec.input_scale != 1.0 else points.reshape(P, 3)
-            extras = torch.empty((P, self.kx), dtype=torch.float32, device=dev)
+            G = spec.grid_channels
+            extras = torch.empty((P, 3 + G), dtype=torch.float32, device=dev)     # [dir, feat]
             _lib.check(lib.fenerf_extras_gather(C.byref(self.packed.desc), self.packed.ptr, points.data_ptr(), dirs.data_ptr(),
                                                 P, ppb, dir_group, int(bool(lock_dirs)), extras.data_ptr(), st))
+            if self.gt:     # the first layer takes [feat, pos] (the reference's column order), the colour layer [dir]
+                x = torch.cat([extras[:, 3:], x], dim=1).contiguous()
+                extras = extras[:, :3].contiguous()
             A, Gt = [None] * self.n_film, [None] * self.n_film
             own = self.own_gemm
             A[0], Gt[0] = self._stash(None, 0, b0, P, ppb, xin=x, wx=self.W0)
@@ -321,10 +334,8 @@ class _FieldBackward:
                     e16 = torch.zeros((P, self.kx_pad), dtype=self.dt, device=dev)
                     e16[:, :self.kx] = extras
                     self.dWx_b[b0:b1] += _bmm32(du3, e16.view(k, ppb, self.kx_pad))
-                    if spec.grid_channels:                                     # d features = dU diag(f_b) W_feat, (P, G)
-                        d_feat = torch.bmm(dA.view(k, ppb, 256), self.fWfeat[b0:b1]).view(P, -1).contiguous()
-                        _lib.check(lib.fenerf_grid_scatter_add(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
-                                                               d_feat.shape[1], P, self.grid_grad_cl.data_ptr(), self.dtc, st))
+                    if G and not self.gt:
+                        self._grid_grad(dA, points, k, ppb, b0, b1)
                 dA = self._chain(dA, idx, b0, b1, ppb)
                 A[idx], Gt[idx] = None, None
             # ---- trunk: colour-branch gradient + sigma / label heads ----
@@ -348,9 +359,19 @@ class _FieldBackward:
                 dA = self._chain(dA, l, b0, b1, ppb)
                 A[l], Gt[l] = None, None
             self._gate(dA, Gt[0], 0, b0, b1, P, ppb)
-            x16 = torch.zeros((P, 8), dtype=self.dt, device=dev)
-            x16[:, :3] = x
-            self.dW_b[0][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), x16.view(k, ppb, 8))
+            if self.gt:
+                self._grid_grad(dA, points, k, ppb, b0, b1)
+            x16 = torch.zeros((P, self.k0_pad), dtype=self.dt, device=dev)
+            x16[:, :self.k0] = x
+            self.dW_b[0][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), x16.view(k, ppb, self.k0_pad))
+
+    def _grid_grad(self, dU, points, k, ppb, b0, b1):
+        """d features = dU diag(f_b) W_feat, (P, G), of the layer the grid feeds, scattered into the grid accumulator."""
+        P = k * ppb
+        d_feat = torch.bmm(dU.view(k, ppb, 256), self.fWfeat[b0:b1]).view(P, -1).contiguous()
+        _lib.check(_lib.lib().fenerf_grid_scatter_add(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
+                                                      d_feat.shape[1], P, self.grid_grad_cl.data_ptr(), self.dtc,
+                                                      _stream(self.dev)))
 
     # ---- after every point set: fold the per-image accumulators into parameter / FiLM gradients ----
     def finish(self):
@@ -364,7 +385,7 @@ class _FieldBackward:
             dp = self.colsum[:, idx]                                        # sum of dU per image
             w32 = w.detach().float()
             if idx == 0:
-                m = self.dW_b[0][:, :, :3]
+                m = self.dW_b[0][:, :, :self.k0]                                # columns [pos], or [feat, pos]
             elif idx == self.c0:
                 m = torch.cat([self.dWx_b[:, :, :self.kx], self.dW_b[idx]], dim=2)   # column order of the reference: [dir, feat, x]
             else:

@@ -72,6 +72,10 @@ int make_layout(const fenerf_field_desc* field, FnLayout* L) {
         return fail(FENERF_E_UNSUPPORTED, "FENERF_FIELD_FEATURE_HEAD: only label_dim 0 (no other flag) or label_dim 64 with "
                     "FENERF_FIELD_LABEL_FILM, without a grid (flags 0x%x, label_dim %d, grid %d)", (unsigned)field->reserved,
                     field->label_dim, field->grid_channels);
+    if (r == -4)
+        return fail(FENERF_E_UNSUPPORTED, "unknown field flag combination 0x%x for this field: FENERF_FIELD_GRID_TRUNK only "
+                    "with grid_channels 32, label_dim 0 and no other flag (label_dim %d, grid %d)", (unsigned)field->reserved,
+                    field->label_dim, field->grid_channels);
     FN_REQUIRE(r == 0, "unsupported field description");
     return 0;
 }

@@ -4,7 +4,9 @@
 // rest does not care).  Host and device share this header: the host computes the offsets once per
 // call and passes the struct by value to the kernels.
 //
-//   first layer      Wt0 [3][256] f32 (k-major)          b0 [256]
+//   first layer      Wt0 [first_k][256] f32 (k-major)    b0 [256]
+//                        rows 0..2 the position; with the grid in the trunk (FENERF_FIELD_GRID_TRUNK) rows 3.. the G
+//                        grid features (the reference's column order [feat, pos] is re-laid out here)
 //   hidden layer l   Wt  [K_l][256] f32 (k-major)        b  [256]        (exact kernel)
 //                    img [2 halves][K_l/64][128 rows][64 k] f16, 128B-swizzled (wgmma kernel):
 //                        feature half h, k-chunk kc at byte h*64 KB + kc*16 KB, so one bulk copy can
@@ -13,7 +15,8 @@
 //     colour layer, whose extra inputs are appended after the 256 x-rows:
 //        f32:  rows 256.. = dir(3), feat(G), zero pad to KX_PAD
 //        f16:  one more 64-wide chunk in the "input chunk" slot order (see below)
-//   input-chunk image of the first layer: [256 rows][64 k] f16 (only slots 0..8 non-zero)
+//   input-chunk image of the first layer: [256 rows][64 k] f16 (slots 0..8 non-zero, and 32.. the feature columns of a
+//                    grid-trunk field, whose low parts (w - f16(w)) get an image of their own, first_img_lo, at the end)
 //   heads            sigma_w   w[256], b[1] (f32)
 //                    rgb.w     [3][256] + b[3] (f32): the sigmoid colour head
 //                    label_w   [32][256] + b[32] (f32): the pre-multiplied label chain Weff, beff (then its 1/scale), or
@@ -40,6 +43,8 @@
 //   linear heads     FnHead `rgb`, and `label` for the label FiLM branch (no chain to pre-multiply): an fp32 copy of
 //                    w_rows rows with the bias after them, at w + w_rows * 256 floats, and an image of img_rows rows;
 //                    rows from n_out on are zero.
+//   grid trunk       (FENERF_FIELD_GRID_TRUNK) the grid features feed the first layer (first_k = 3 + G) instead of the
+//                    first colour layer (kx = 3: the direction alone), so the density needs them too.
 //
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
@@ -91,17 +96,23 @@ struct FnLayout {
     FnHead rgb;             // the colour head
     FnHead label;           // the label FiLM branch's head (all zero without one)
     size_t total;
+    int32_t grid_trunk;     // the variant flag FENERF_FIELD_GRID_TRUNK
+    int32_t first_k;        // inputs of the first layer: 3, or 3 + G with the grid in the trunk
+    size_t first_img_lo;    // grid trunk: the feature columns' fp16 low parts, image as first_img (0 otherwise)
 };
 
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head on a field shape no
-// reference class has, or -1 if the description is outside what the kernels support.
+// Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head or -4 for the grid in
+// the trunk on a field shape no reference class has, or -1 if the description is outside what the kernels support.
 static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     if (!f || !L) return -1;
-    if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD)) return -2;
+    if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD | FENERF_FIELD_GRID_TRUNK)) return -2;
     const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
     const int feature_head = (f->reserved & FENERF_FIELD_FEATURE_HEAD) ? 1 : 0;
+    const int grid_trunk = (f->reserved & FENERF_FIELD_GRID_TRUNK) ? 1 : 0;
+    // EmbeddingPiGAN256: a 32-channel grid, no labels, no other flag
+    if (grid_trunk && (f->reserved != FENERF_FIELD_GRID_TRUNK || f->grid_channels != 32 || f->label_dim != 0)) return -4;
     if (feature_head) {
         // SPATIALSIRENBASELINEHD (label_dim 0) and SPATIALSIRENSEMANTICHD (label FiLM, label_dim 64), no grid
         if (f->grid_channels != 0 || f->label_dim != (label_film ? FN_FEAT : 0)) return -3;
@@ -123,7 +134,9 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     L->n_film = 1 + L->n_hidden;
     L->trunk_labels = (label_film || feature_head) ? 0 : f->label_dim;
     L->sigma_row = feature_head ? FN_FEAT_SIGMA_ROW : f->label_dim;
-    L->kx = 3 + f->grid_channels;
+    L->grid_trunk = grid_trunk;
+    L->first_k = grid_trunk ? 3 + f->grid_channels : 3;
+    L->kx = grid_trunk ? 3 : 3 + f->grid_channels;
     L->kx_pad = (L->kx + 15) / 16 * 16;
     L->label_dim = f->label_dim;
     L->grid_channels = f->grid_channels;
@@ -132,7 +145,7 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     L->input_scale = f->input_scale;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = fn_align_up(off + bytes, 1024); return o; };
-    L->first_w = take(3 * FN_H * 4);
+    L->first_w = take((size_t)L->first_k * FN_H * 4);
     L->first_b = take(FN_H * 4);
     L->first_img = take(FN_IMG_BYTES);
     for (int l = 0; l < FN_MAX_HIDDEN; ++l) { L->hid_w32[l] = L->hid_b[l] = L->hid_img[l] = 0; }
@@ -160,6 +173,7 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
         L->rgb.img = take(FN_HEAD_IMG_BYTES(FN_FEAT));
         if (label_film) L->label.img = take(FN_HEAD_IMG_BYTES(FN_FEAT));
     }
+    L->first_img_lo = grid_trunk ? take(FN_IMG_BYTES) : 0;
     L->total = off;
     return 0;
 }

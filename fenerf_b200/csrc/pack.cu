@@ -14,18 +14,31 @@ __device__ __forceinline__ __half f16_hi(float w) { return __float2half_rn(w); }
 __device__ __forceinline__ __half f16_lo(float w) { return __float2half_rn(w - __half2float(__float2half_rn(w))); }
 
 // ---- first layer: Wt0, b0 and the input-chunk image (hi, hi, lo) -------------------------------
-__global__ void pack_first_kernel(const float* __restrict__ w /*[256][3]*/, const float* __restrict__ b,
-                                  float* __restrict__ wt, float* __restrict__ bo, unsigned char* __restrict__ img) {
+// w is [256][g + 3] in the reference's column order [feat(g), pos(3)] (g = 0 unless the grid feeds the trunk); Wt0 rows
+// 0..2 are the position, rows 3.. the features, which the image takes in the feature slots -- their fp16 high parts, and
+// the low parts in img_lo
+__global__ void pack_first_kernel(const float* __restrict__ w, int g, const float* __restrict__ b,
+                                  float* __restrict__ wt, float* __restrict__ bo, unsigned char* __restrict__ img,
+                                  unsigned char* __restrict__ img_lo) {
     int n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= FN_H) return;
+    const int in_dim = g + 3;
     bo[n] = b[n];
     for (int k = 0; k < FN_KCHUNK; ++k) *reinterpret_cast<__half*>(img + fn_sw128_offset(n, k)) = __float2half_rn(0.f);
     for (int k = 0; k < 3; ++k) {
-        float v = w[n * 3 + k];
+        float v = w[n * in_dim + g + k];
         wt[k * FN_H + n] = v;
         *reinterpret_cast<__half*>(img + fn_sw128_offset(n, FN_SLOT_POS + k)) = f16_hi(v);
         *reinterpret_cast<__half*>(img + fn_sw128_offset(n, FN_SLOT_POS + 3 + k)) = f16_hi(v);
         *reinterpret_cast<__half*>(img + fn_sw128_offset(n, FN_SLOT_POS + 6 + k)) = f16_lo(v);
+    }
+    if (img_lo)
+        for (int k = 0; k < FN_KCHUNK; ++k) *reinterpret_cast<__half*>(img_lo + fn_sw128_offset(n, k)) = __float2half_rn(0.f);
+    for (int c = 0; c < g; ++c) {
+        const float v = w[n * in_dim + c];
+        wt[(3 + c) * FN_H + n] = v;
+        *reinterpret_cast<__half*>(img + fn_sw128_offset(n, FN_SLOT_FEAT + c)) = f16_hi(v);
+        *reinterpret_cast<__half*>(img_lo + fn_sw128_offset(n, FN_SLOT_FEAT + c)) = f16_lo(v);
     }
 }
 
@@ -232,7 +245,7 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
     };
     // (a label FiLM layer takes a hidden slot: it is hashed with the label parameters below, label_w[0])
     const int n_trunk = L.trunk_hidden + 1, n_color = L.n_hidden - L.color0;
-    for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? 3 : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
+    for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? L.first_k : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
     add(p->sigma_w, FN_H); add(p->sigma_b, 1);
     for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (unsigned long long)(i == 0 ? L.kx + FN_H : FN_H) * FN_H); add(p->color_b[i], FN_H); }
     add(p->rgb_w, (unsigned long long)L.rgb.n_out * FN_H); add(p->rgb_b, L.rgb.n_out);
@@ -251,8 +264,9 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
 int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, cudaStream_t st) {
     unsigned char* packed = static_cast<unsigned char*>(packed_v);
     FN_REQUIRE(p->trunk_w[0] && p->trunk_b[0], "trunk_w[0]/trunk_b[0] missing");
-    pack_first_kernel<<<1, 256, 0, st>>>(p->trunk_w[0], p->trunk_b[0], (float*)(packed + L.first_w),
-                                         (float*)(packed + L.first_b), packed + L.first_img);
+    pack_first_kernel<<<1, 256, 0, st>>>(p->trunk_w[0], L.first_k - 3, p->trunk_b[0], (float*)(packed + L.first_w),
+                                         (float*)(packed + L.first_b), packed + L.first_img,
+                                         L.grid_trunk ? packed + L.first_img_lo : nullptr);
     FN_LAUNCH_OK("pack_first_kernel");
     if (L.label_film)
         FN_REQUIRE(p->label_w[0] && p->label_b[0] && p->label_w[2] && p->label_b[2] && !p->label_w[1] && !p->label_b[1],
@@ -271,7 +285,7 @@ int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, 
                                                    (float*)(packed + L.hid_b[l]), packed + L.hid_img[l]);
         FN_LAUNCH_OK("pack_hidden_kernel");
         if (is_c0) {
-            pack_color0_ximg_kernel<<<1, 256, 0, st>>>(w, in_dim, L.grid_channels, packed + L.color0_ximg);
+            pack_color0_ximg_kernel<<<1, 256, 0, st>>>(w, in_dim, L.kx - 3, packed + L.color0_ximg);
             FN_LAUNCH_OK("pack_color0_ximg_kernel");
         }
     }

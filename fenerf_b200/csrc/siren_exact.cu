@@ -26,6 +26,9 @@
 // followed by its share of the label head's k-sum (the running sums sit in the same buffer), so shared memory and
 // occupancy stay those of the other fields.  With the 64-row label head of a feature-head field (kFeatureHead) the label
 // activations (64 x TM) and the 64 running sums fill the buffer exactly; its colour head has no sigmoid.
+//
+// Grid-trunk fields (kGridTrunk, FENERF_FIELD_GRID_TRUNK): the first layer sums over the position and the 32 grid features
+// the tile gathered into A rows 259..290, for the density alone as well (GUARD refinement, density grids).
 #include "siren_common.cuh"
 #include "sm90.cuh"
 
@@ -168,7 +171,7 @@ __device__ __forceinline__ float grid_feature(const float* __restrict__ grid, in
     return out;
 }
 
-template <bool kGather, int P, bool kLabelFilm = false, bool kFeatureHead = false>
+template <bool kGather, int P, bool kLabelFilm = false, bool kFeatureHead = false, bool kGridTrunk = false>
 __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned char* smem_raw) {
     constexpr int TM = 16 * P;
     Smem<P>& s = *reinterpret_cast<Smem<P>*>(smem_raw);
@@ -216,25 +219,27 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
         }
         for (int i = tid; i < (KA - FN_H - 3) * TM; i += NTHREADS) s.A[FN_H + 3 + i / TM][i % TM] = 0.f;
         __syncthreads();
-        if (L.grid_channels > 0 && !a.sigma_only) {
+        if (L.grid_channels > 0 && (kGridTrunk || !a.sigma_only)) {   // the density needs them where they feed the trunk
             const float* grid = reinterpret_cast<const float*>(pk + L.grid);
             const int G = L.grid_channels;
             for (int it = tid; it < TM * G; it += NTHREADS) {
                 int pt = it / G, ch = it % G;
                 s.A[FN_H + 3 + ch][pt] = grid_feature(grid, L.grid_res, G, s.pos[0][pt], s.pos[1][pt], s.pos[2][pt], ch);
             }
+            if constexpr (kGridTrunk) __syncthreads();            // the first layer reads them
         }
         float acc[P][16];
         const int tn = P == 4 ? (tid & 15) : (tid >> 4), tm = P == 4 ? (tid >> 4) : (tid & 15);
-        // ---- first layer: 3 -> 256 ----
+        // ---- first layer: 3 -> 256; with the grid in the trunk 3 + 32 -> 256 (Wt0 rows 3.. = the features) ----
         {
             const float* wt = reinterpret_cast<const float*>(pk + L.first_w);
             init_bias(reinterpret_cast<const float*>(pk + L.first_b), acc, tid);
+            constexpr int K0 = kGridTrunk ? 3 + 32 : 3;
 #pragma unroll
-            for (int k = 0; k < 3; ++k) {
+            for (int k = 0; k < K0; ++k) {
                 float av[P];
 #pragma unroll
-                for (int m = 0; m < P; ++m) av[m] = s.pos[k][tm * P + m];
+                for (int m = 0; m < P; ++m) av[m] = k < 3 ? s.pos[k][tm * P + m] : s.A[FN_H + k][tm * P + m];
 #pragma unroll
                 for (int j = 0; j < 4; ++j)
 #pragma unroll
@@ -345,21 +350,22 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
     }
 }
 
-template <bool kGather, int P, bool kLabelFilm, bool kFeatureHead = false>
+template <bool kGather, int P, bool kLabelFilm, bool kFeatureHead = false, bool kGridTrunk = false>
 __global__ void __launch_bounds__(NTHREADS, 2) siren_exact_kernel(ExactArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    siren_exact_body<kGather, P, kLabelFilm, kFeatureHead>(a, smem_raw);
+    siren_exact_body<kGather, P, kLabelFilm, kFeatureHead, kGridTrunk>(a, smem_raw);
 }
 
 // GUARD refinement: the list length is only known on the device.  Short lists (small renders; fields whose densities
 // rarely come near zero) take 16-point tiles -- lowest latency per tile, one wave as long as the list fits
 // 16 x gridDim points -- longer ones 32-point tiles, which keep it to one wave up to twice that and do twice the FFMA
 // per weight slab fetched from L2.
+template <bool kGridTrunk>
 __global__ void __launch_bounds__(NTHREADS, 1) siren_exact_guard_kernel(ExactArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int n_only = *a.n_only_dev;
-    if (n_only <= 16 * (int)gridDim.x) siren_exact_body<true, 1>(a, smem_raw);
-    else siren_exact_body<true, 2>(a, smem_raw);
+    if (n_only <= 16 * (int)gridDim.x) siren_exact_body<true, 1, false, false, kGridTrunk>(a, smem_raw);
+    else siren_exact_body<true, 2, false, false, kGridTrunk>(a, smem_raw);
 }
 
 }  // namespace
@@ -391,7 +397,9 @@ int siren_points_exact(const FnLayout& L, const unsigned char* packed, const flo
     };
     const bool label_film = L.label_film && !sigma_only, feature_head = L.feature_head && !sigma_only;
     int e;
-    if (feature_head) {
+    if (L.grid_trunk)     // (the density alone too: the trunk needs the grid features)
+        e = gather ? launch(siren_exact_kernel<true, 4, false, false, true>) : launch(siren_exact_kernel<false, 4, false, false, true>);
+    else if (feature_head) {
         if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true, true>) : launch(siren_exact_kernel<true, 4, false, true>);
         else e = label_film ? launch(siren_exact_kernel<false, 4, true, true>) : launch(siren_exact_kernel<false, 4, false, true>);
     } else if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true>) : launch(siren_exact_kernel<true, 4, false>);
@@ -456,8 +464,13 @@ int guard_refine(const FnLayout& L, const unsigned char* packed, const float* po
     // touched here, so the whole refinement can sit inside a captured CUDA graph)
     // one CTA per SM (118 / 140 KB of shared memory); tile size chosen on the device from the list length
     size_t smem = sizeof(Smem<2>) > sizeof(Smem<1>) ? sizeof(Smem<2>) : sizeof(Smem<1>);
-    FN_CUDA_OK(cudaFuncSetAttribute(siren_exact_guard_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    siren_exact_guard_kernel<<<num_sms(), NTHREADS, smem, st>>>(a);
+    auto launch = [&](auto kernel) -> int {
+        FN_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<num_sms(), NTHREADS, smem, st>>>(a);
+        return 0;
+    };
+    // (the density of a grid-trunk field needs the grid features: its own instantiation)
+    if (int e = L.grid_trunk ? launch(siren_exact_guard_kernel<true>) : launch(siren_exact_guard_kernel<false>)) return e;
     FN_LAUNCH_OK("siren_exact_kernel(guard)");
     return 0;
 }

@@ -7,6 +7,8 @@ namespace fn {
 // FastArgs
 int siren_fast_label_launch(const void* args, int blocks, cudaStream_t st);
 int siren_fast_hd_launch(const void* args, int blocks, bool label_film, cudaStream_t st);
+// the grid-trunk instantiation (siren_fast_grid.cu), the density alone included
+int siren_fast_grid_launch(const void* args, int blocks, cudaStream_t st);
 // the debug instantiations (siren_fast_debug.cu): variant 1 = one column pair in four on the software sine, 2 / 3 = the
 // timeline of the production / the variant-1 kernel
 int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st);
@@ -25,6 +27,7 @@ bool build_loads(const FnLayout& L, FastArgs& A, bool sigma_only) {
         ++A.n_loads;
     };
     push(L.first_img, 2 * CHUNK);
+    if (L.grid_trunk) push(L.first_img_lo, 2 * CHUNK);      // the feature columns' low parts
     for (int l = 0; l < L.n_hidden; ++l) {
         if (l == L.trunk_hidden) {
             push(L.head_img, 4 * HEAD_CHUNK);
@@ -65,7 +68,8 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     FN_REQUIRE(L.trunk_hidden >= 1 && L.n_hidden - L.color0 >= 1, "field needs >= 2 trunk and >= 1 colour layers");
     FN_REQUIRE(L.sigma_row < 32, "the fast path packs labels and sigma into one 32-column head (label_dim <= 31)");
     // (the offsets the weight stream carries in 32 bits; the grid sections are indexed in 64 bits)
-    FN_REQUIRE(L.rgb.img < 0xFFFFFFFFull && L.label.img < 0xFFFFFFFFull, "packed weight images beyond 4 GB");
+    FN_REQUIRE(L.rgb.img < 0xFFFFFFFFull && L.label.img < 0xFFFFFFFFull && L.first_img_lo < 0xFFFFFFFFull,
+               "packed weight images beyond 4 GB");
     FN_REQUIRE(((uintptr_t)film & 15) == 0, "the FiLM table must be 16-byte aligned");
     FastArgs a;
     memset(&a, 0, sizeof(a));
@@ -80,10 +84,12 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     static std::atomic<int> attr_set[kMaxDevices];
     const int blocks = (int)(n_pairs < (long long)num_sms() ? n_pairs : (long long)num_sms());
     if (const int variant = g_variant.load()) {
+        FN_REQUIRE(!L.grid_trunk, "the debug point-network variants do not cover fields with the grid in the trunk");
         a.trace = g_trace;
         a.trace_ctas = g_trace_ctas;
         return siren_fast_debug_launch(&a, blocks, label_film, feature_head, variant, st);
     }
+    if (L.grid_trunk) return siren_fast_grid_launch(&a, blocks, st);
     if (feature_head) return siren_fast_hd_launch(&a, blocks, label_film, st);
     if (label_film) return siren_fast_label_launch(&a, blocks, st);
     FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<false>, attr_set, (int)SMEM_TOTAL));

@@ -33,10 +33,16 @@
 //                  more than those 32 registers: four turns, [layer half 0] [head on it] [layer half 1] [head].
 //   kFeatureHead   (FENERF_FIELD_FEATURE_HEAD) the colour head is m64n64, 64 linear outputs with no sigmoid, and so is
 //                  the label head (m64n32 otherwise).  Each of their images is one 32 KB ring slot.
+//   kGridTrunk     (FENERF_FIELD_GRID_TRUNK) the grid features feed the first layer, so they are gathered for the
+//                  density alone too, from the fp32 grid, and split hi / lo like the position: hi in the feature slots of
+//                  the staging row, lo in a region of their own (SMEM_XLO).  The first layer issues the feature slices 2, 3
+//                  three times, hi * W_hi + lo * W_hi + hi * W_lo, the low parts of W coming from a second image in the
+//                  weight stream (DESIGN section 5 has the error budget).  The first colour layer takes the direction
+//                  slice only.
 //
 // The plain and the label FiLM instantiations live in translation units of their own (siren_fast.cu,
-// siren_fast_label.cu), the two feature-head ones in a third (siren_fast_hd.cu), so that the plain one compiles exactly as
-// it does on its own.  The debug
+// siren_fast_label.cu), the two feature-head ones in a third (siren_fast_hd.cu) and the grid-trunk one in a fourth
+// (siren_fast_grid.cu), so that the plain one compiles exactly as it does on its own.  The debug
 // instantiations -- a share of the sines on the FMA pipe (kSoftSin, soft_sinf) and the clock64 timeline (kTrace) -- live
 // in siren_fast_debug.cu.
 #pragma once
@@ -63,6 +69,11 @@ constexpr uint32_t SMEM_FILM = SMEM_X + 2 * TILE * XSTRIDE * 2;   // [2 warpgrou
 constexpr uint32_t SMEM_BAR = SMEM_FILM + 2 * FRING * FILM_BYTES;
 // full[RING], empty[RING], turn[2], film_full[2 * FRING], film_empty[2 * FRING]
 constexpr uint32_t SMEM_TOTAL = SMEM_BAR + 16 * RING + 16 + 16 * 2 * FRING;
+// kGridTrunk only: the grid features' fp16 low parts, [2 warpgroups][64 points][32] f16 after everything else (8 KB of
+// the 9 KB the other variants leave free; read once per tile, so the 64-byte rows' bank conflicts do not matter)
+constexpr uint32_t SMEM_XLO = SMEM_TOTAL;
+constexpr int XLO_STRIDE = 32;
+constexpr uint32_t SMEM_TOTAL_GRID = SMEM_XLO + 2 * TILE * XLO_STRIDE * 2;
 constexpr int MAX_LOADS = 72;
 constexpr uint32_t CHUNK = 16384;                   // one [128 rows][64 k] f16 image chunk
 constexpr uint32_t HEAD_CHUNK = 32 * 128;           // one [32 rows][64 k] chunk of the trunk-head image
@@ -131,7 +142,8 @@ struct FastArgs {
 
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-template <bool kLabelFilm, bool kFeatureHead = false, int kSoftSin = kSoftSinEvery, bool kTrace = false>
+template <bool kLabelFilm, bool kFeatureHead = false, int kSoftSin = kSoftSinEvery, bool kTrace = false,
+          bool kGridTrunk = false>
 __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_constant__ FastArgs a) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
@@ -320,7 +332,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 split_f16(dir[i], hi, lo);
                 slots[FN_SLOT_DIR + i] = hi; slots[FN_SLOT_DIR + 3 + i] = lo; slots[FN_SLOT_DIR + 6 + i] = hi;
             }
-            if (L.grid_channels > 0 && valid && !a.sigma_only) {      // density needs no grid features
+            if constexpr (kGridTrunk) {
+                // the features feed the trunk, the density included: fp32 lookup, split hi / lo like the position
+                __align__(16) __half lo[32];
+#pragma unroll
+                for (int i = 0; i < 32; ++i) lo[i] = __float2half_rn(0.f);
+                if (valid) {
+                    float feat[32];
+                    grid_features32(reinterpret_cast<const float*>(a.packed + L.grid), L.grid_res, pos[0], pos[1], pos[2], feat);
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) split_f16(feat[i], slots[FN_SLOT_FEAT + i], lo[i]);
+                }
+                __half* xlo = reinterpret_cast<__half*>(smem + SMEM_XLO) + (wg * TILE + tid) * XLO_STRIDE;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) reinterpret_cast<uint4*>(xlo)[i] = reinterpret_cast<const uint4*>(lo)[i];
+            } else if (L.grid_channels > 0 && valid && !a.sigma_only) {      // density needs no grid features
                 float feat[32];
                 grid_features32_h(reinterpret_cast<const __half*>(a.packed + L.grid16), L.grid_res, pos[0], pos[1], pos[2], feat);
 #pragma unroll
@@ -351,28 +377,52 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         };
         auto act_hi = [&]() -> uint32_t (&)[8][4] { return *reinterpret_cast<uint32_t (*)[8][4]>(&act[8]); };
 
-        // ---- first layer: input slots (k-slice 0) against the [256][64] input image ----
+        // ---- first layer: input slots (k-slice 0) against the [256][64] input image; with the grid in the trunk also the
+        // feature slices 2, 3 as hi * W_hi + lo * W_hi + hi * W_lo (the low parts of W: the image after it) ----
         {
-            uint32_t xf[4], slot;
+            uint32_t xf[4], slot, slot_lo = 0, w_lo = 0;
+            uint32_t xg[2][4], xl[2][4];             // kGridTrunk: feature slots 32..63, hi and lo
             const float4* fs = nullptr;
             xfrag(0, xf);
+            if constexpr (kGridTrunk) {
+                const __half* xlo = reinterpret_cast<const __half*>(smem + SMEM_XLO) + wg * TILE * XLO_STRIDE;
+#pragma unroll
+                for (int s = 0; s < 2; ++s) {
+                    xfrag(2 + s, xg[s]);
+                    const __half* p = xlo + r0 * XLO_STRIDE + 16 * s + 2 * q;
+                    xl[s][0] = *reinterpret_cast<const uint32_t*>(p);
+                    xl[s][1] = *reinterpret_cast<const uint32_t*>(p + 8 * XLO_STRIDE);
+                    xl[s][2] = *reinterpret_cast<const uint32_t*>(p + 8);
+                    xl[s][3] = *reinterpret_cast<const uint32_t*>(p + 8 * XLO_STRIDE + 8);
+                }
+            }
             const uint32_t w = acquire(slot);
+            if constexpr (kGridTrunk) w_lo = acquire(slot_lo);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 turn_begin();
                 wg_fence();
                 mma_rs_n128(d, xf, desc_kmajor(w + h * CHUNK), 0u);
+                if constexpr (kGridTrunk)
+#pragma unroll
+                    for (int s = 0; s < 2; ++s) {
+                        mma_rs_n128(d, xg[s], desc_kmajor(w + h * CHUNK + 32 * (2 + s)), 1u);
+                        mma_rs_n128(d, xl[s], desc_kmajor(w + h * CHUNK + 32 * (2 + s)), 1u);
+                        mma_rs_n128(d, xg[s], desc_kmajor(w_lo + h * CHUNK + 32 * (2 + s)), 1u);
+                    }
                 wg_commit();
                 turn_end(TG_FIRST);
                 wg_wait<0>();
                 trace(TR_MMA_DONE);
                 fence_regs(d);
                 fence_regs(xf);
+                if constexpr (kGridTrunk) { fence_regs(xg); fence_regs(xl); }
                 if (h == 0) fs = film_acquire();
                 if (h == 0) film_epi(fs, 0, nxt);
                 else film_epi(fs, 1, act_hi());
             }
             release(slot);
+            if constexpr (kGridTrunk) release(slot_lo);
             film_release();
 #pragma unroll
             for (int s = 0; s < 8; ++s)
@@ -493,7 +543,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             }
             // ---- FiLM layer l + 1: weight image halves 64 KB apart, two 32 KB slabs per half ----
             const bool c0 = (l == L.color0);     // first colour layer: + direction / grid-feature slots
-            const int nx = L.grid_channels > 0 ? 3 : 1;
+            const int nx = !kGridTrunk && L.grid_channels > 0 ? 3 : 1;     // (a grid-trunk field: the direction alone)
             uint32_t xf[3][4];
             if (c0)
 #pragma unroll

@@ -39,7 +39,8 @@ def field_desc(spec) -> "_lib.FieldDesc":
                           grid_channels=spec.grid_channels, grid_res=spec.grid_res, out_dim=spec.out_dim,
                           input_scale=spec.input_scale,
                           reserved=(_lib.FIELD_LABEL_FILM if spec.label_film else 0)
-                          | (_lib.FIELD_FEATURE_HEAD if spec.feature_head else 0))
+                          | (_lib.FIELD_FEATURE_HEAD if spec.feature_head else 0)
+                          | (_lib.FIELD_GRID_TRUNK if spec.grid_trunk else 0))
 
 
 def _f32(t, device):

@@ -16,6 +16,7 @@ Reference interfaces mirrored (file:line in the reference tree):
   UniformBoxWarp                              siren/siren.py:181-187
   sample_from_3dgrid                          siren/siren.py:314-330
   SPATIALSIRENBASELINE                        siren/siren.py:189-244
+  EmbeddingPiGAN256                           siren/siren.py:341-410
   SPATIALSIRENSEMANTIC                        siren/siren.py:597-671
   SPATIALSIRENBASELINESEMANTIC                siren/siren.py:674-744
   SPATIALSIRENDISENTANGLE                     siren/siren.py:747-813
@@ -151,6 +152,8 @@ class FieldSpec:
     input_scale    UniformBoxWarp factor applied to the position before the trunk and the grid
     feature_head   the colour head is Linear(256 -> 64) without the sigmoid: 64 features for a neural renderer
                    (siren/siren.py:300-301, 1365-1366)
+    grid_trunk     the grid features feed the first trunk layer, cat[feat, pos] -> 256, and not the colour branch
+                   (siren/siren.py:396-398)
     out_dim        label_dim + 3 (rgb; 64 features with feature_head) + 1 (sigma); channel order [labels, rgb, sigma]
     """
     trunk_layers: int
@@ -163,6 +166,7 @@ class FieldSpec:
     double_latent: bool
     label_film: bool = False
     feature_head: bool = False
+    grid_trunk: bool = False
 
     @property
     def rgb_dim(self):
@@ -472,6 +476,45 @@ class SPATIALSIRENSEMANTICHD(SPATIALSIRENSEMANTIC):
         return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=64, grid_channels=0, grid_res=0,
                          input_scale=float(self.gridwarper.scale_factor), out_dim=129, double_latent=False,
                          label_film=True, feature_head=True)
+
+
+class EmbeddingPiGAN256(TALLSIREN):
+    """pi-GAN's embedding field at width 256 (siren/siren.py:341-410): a 32 x 64^3 feature grid feeds the first trunk
+    layer, FiLM(cat[feat(32), pos(3)] -> 256), and not the colour branch, FiLM(cat[dir(3), x] -> 256).  FiLM rows: trunk
+    0..7, colour 8; output channels [rgb (3), sigma (1)] whatever `output_dim` says.
+
+    The reference builds it as EmbeddingPiGAN128.__init__(hidden_dim=256): that init draws a 32 x 96^3 grid (scaled by
+    0.01) before this class replaces it with a 32 x 64^3 one (scaled by 0.1); both draws move the RNG, as here."""
+
+    def __init__(self, input_dim=2, z_dim=100, hidden_dim=256, output_dim=1, device=None):
+        nn.Module.__init__(self)
+        self.device = device
+        self.input_dim = input_dim
+        self.z_dim = z_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+
+        widths = [32 + 3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        print(self.network)
+        self.final_layer = nn.Linear(hidden_dim, 1)
+        self.color_layer_sine = FiLMLayer(hidden_dim + 3, hidden_dim)
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 3))
+        self.mapping_network = CustomMappingNetwork(z_dim, 256, (len(self.network) + 1) * hidden_dim * 2)
+
+        for part in (self.network, self.final_layer, self.color_layer_sine, self.color_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(modified_first_sine_init)     # U(+-1/3) over all 35 columns
+        torch.randn(1, 32, 96, 96, 96)                      # the 128-wide class's grid draw, replaced below
+        self.gridwarper = UniformBoxWarp(0.24)
+        self.spatial_embeddings = nn.Parameter(torch.randn(1, 32, 64, 64, 64) * 0.1)
+
+    def field_spec(self):
+        g = self.spatial_embeddings
+        assert g.shape[2] == g.shape[3] == g.shape[4], "cubic feature grid expected"
+        return FieldSpec(trunk_layers=len(self.network), color_layers=1, label_dim=0, grid_channels=g.shape[1],
+                         grid_res=g.shape[2], input_scale=float(self.gridwarper.scale_factor), out_dim=4,
+                         double_latent=False, grid_trunk=True)
 
 
 class _DoubleLatentField(_FieldBase):

@@ -61,6 +61,10 @@ extern "C" {
  * SPATIALSIRENBASELINEHD (siren.py:247-302):  trunk 8, color 1, label 0, grid 0, scale 2/0.24, out 65.
  * SPATIALSIRENSEMANTICHD (siren.py:1301-1367): trunk 8, color 1, label 64 (FENERF_FIELD_LABEL_FILM), grid 0,
  *                                scale 2/0.24, out 129.
+ * With FENERF_FIELD_GRID_TRUNK the grid features feed the first trunk layer instead of the colour branch:
+ *   x = FiLM_0(cat[grid_feat(G), x(3)] -> 256)(x); ...;  c = FiLM(cat[dir(3), x(256)] -> 256)
+ * EmbeddingPiGAN256 (siren.py:341-410):     trunk 8, color 1, label 0, grid 32 x 64^3 (FENERF_FIELD_GRID_TRUNK),
+ *                                scale 2/0.24, out 4.
  * The hidden width is fixed at 256.                                                            */
 #define FENERF_MAX_TRUNK 8
 #define FENERF_MAX_COLOR 8
@@ -76,6 +80,10 @@ extern "C" {
                                          label_dim 0 without other flags (SPATIALSIRENBASELINEHD), or label_dim 64 with
                                          FENERF_FIELD_LABEL_FILM (SPATIALSIRENSEMANTICHD; label_w[2] [64][256]); no grid.
                                          Anything else with this bit is FENERF_E_UNSUPPORTED. */
+#define FENERF_FIELD_GRID_TRUNK 0x2   /* the grid features feed the first trunk layer, not the colour branch: trunk_w[0] is
+                                         [256][G+3] in the column order [feat, pos], color_w[0] is [256][3+256] (dir, x).
+                                         Only the reference's shape is accepted (EmbeddingPiGAN256): grid_channels 32,
+                                         label_dim 0, no other flag.  Anything else with this bit is FENERF_E_UNSUPPORTED. */
 
 typedef struct fenerf_field_desc {
     int32_t trunk_layers;   /* 2..8 */
@@ -91,11 +99,12 @@ typedef struct fenerf_field_desc {
 /* Raw parameters exactly as torch stores them: nn.Linear.weight is [out][in] row-major fp32,
  * bias [out]; grid is the reference's channel-major (1, G, D, H, W) tensor (siren.py:1546). */
 typedef struct fenerf_field_params {
-    const float* trunk_w[FENERF_MAX_TRUNK];  /* [256][3] then [256][256] */
+    const float* trunk_w[FENERF_MAX_TRUNK];  /* [256][3] then [256][256]; FENERF_FIELD_GRID_TRUNK: [256][G+3] first */
     const float* trunk_b[FENERF_MAX_TRUNK];
     const float* sigma_w;                    /* [1][256] */
     const float* sigma_b;                    /* [1] */
-    const float* color_w[FENERF_MAX_COLOR];  /* first [256][3+G+256] (cat order dir, feat, x), rest [256][256] */
+    const float* color_w[FENERF_MAX_COLOR];  /* first [256][3+G+256] (cat order dir, feat, x), rest [256][256];
+                                                FENERF_FIELD_GRID_TRUNK: first [256][3+256] */
     const float* color_b[FENERF_MAX_COLOR];
     const float* rgb_w;                      /* [3][256]; FENERF_FIELD_FEATURE_HEAD: [64][256] */
     const float* rgb_b;                      /* [3]; FENERF_FIELD_FEATURE_HEAD: [64] */

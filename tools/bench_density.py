@@ -1,22 +1,35 @@
 """256^3 density grid through the point network (extract_double_semantic_shapes.py:59-62 workload):
-density-only entry vs the full evaluation, both models.  Prints one line per run."""
+density-only entry vs the full evaluation, for both benchmarked models, SPATIALSIRENBASELINE (C) and the grid-trunk
+EmbeddingPiGAN256 (L), whose density needs the grid.  Prints one line per run.
+
+    python tools/bench_density.py [res] [--models C,L] [--rounds N]     (--rounds: the models N times, alternating)"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
 import _cases
+import _grid_trunk  # (registers model L)
 from fenerf_b200 import ops
 
+CASE = {"A": "a_small", "B": "b_small", "C": "c_small", "L": "l_small"}
+
 def main():
-    res = int(sys.argv[1]) if len(sys.argv) > 1 else 256
-    for model in ("A", "B"):
-        case = _cases.CASE_BY_NAME["a_small" if model == "A" else "b_small"]
+    import argparse
+    ap = argparse.ArgumentParser()
+    ap.add_argument("res", type=int, nargs="?", default=256)
+    ap.add_argument("--models", default="A,B,C,L")
+    ap.add_argument("--rounds", type=int, default=1)
+    args = ap.parse_args()
+    res = args.res
+    print("device: %s" % torch.cuda.get_device_name("cuda:0"))
+    for model in args.models.split(",") * args.rounds:
+        case = _cases.CASE_BY_NAME.get(CASE[model]) or _grid_trunk.CASE_BY_NAME[CASE[model]]
         gen = _cases.build_mirror(case, "cuda:0")
         lin = torch.linspace(-0.15, 0.15, res, device="cuda")
         pts = torch.stack(torch.meshgrid(lin, lin, lin, indexing="ij"), -1).reshape(1, -1, 3).contiguous()
         dirs = torch.zeros(1, 1, 3, device="cuda"); dirs[..., -1] = -1
         with torch.no_grad():
-            if model == "A":
+            if model != "B":
                 film = gen.siren.film_table(*gen.siren.mapping_network(torch.randn(1, 256, device="cuda")))
             else:
                 fg, pg = gen.siren.geo_mapping_network(torch.randn(1, 256, device="cuda"))
