@@ -15,7 +15,9 @@ MAX_TRUNK, MAX_COLOR, MAX_LABEL, HIDDEN = 8, 8, 32, 256
 ABI_VERSION = 3
 FIELD_LABEL_FILM = 0x1        # fenerf_field_desc.reserved (the flags word): FENERF_FIELD_LABEL_FILM
 FIELD_GRID_TRUNK = 0x2        # FENERF_FIELD_GRID_TRUNK: the grid features feed the first trunk layer
+FIELD_BRIDGE = 0x4            # FENERF_FIELD_BRIDGE: the colour branch starts from v = Linear(256 -> 3)(trunk output)
 FIELD_FEATURE_HEAD = 0x8      # FENERF_FIELD_FEATURE_HEAD: Linear(256 -> 64) colour head without the sigmoid
+FIELD_BRIDGE_RES = 0x10       # FENERF_FIELD_BRIDGE_RES: v adds the position, the density is a Linear chain on v
 PRECISION = {"exact": 0, "fast": 1, "guard": 2}
 CLAMP = {"relu": 0, "softplus": 1}
 FILL_MODE = {None: 0, "debug": 1, "weight": 2, "weight_debug": 3, "seg_padding_background": 4,
@@ -33,6 +35,7 @@ EXPORTS = (
     "fenerf_workspace_layout", "fenerf_mask2color", "fenerf_frames_to_u8", "fenerf_mapping_film",
     "fenerf_guard_stats", "fenerf_debug_stage_times", "fenerf_debug_fast_variant", "fenerf_debug_soft_sine",
     "fenerf_gemm_nt_f16", "fenerf_gemm_nt_film", "fenerf_gemm_tn_f16",
+    "fenerf_pack_field_bridge", "fenerf_field_fingerprint_bridge",
 )
 
 
@@ -49,6 +52,10 @@ class FieldParams(C.Structure):
                 ("rgb_w", C.c_void_p), ("rgb_b", C.c_void_p),
                 ("label_w", C.c_void_p * 3), ("label_b", C.c_void_p * 3),
                 ("grid", C.c_void_p)]
+
+
+class BridgeParams(C.Structure):
+    _fields_ = [("density_w", C.c_void_p * 4), ("density_b", C.c_void_p * 4), ("pre_w", C.c_void_p), ("pre_b", C.c_void_p)]
 
 
 class RenderDesc(C.Structure):
@@ -85,6 +92,10 @@ def _declare(lib):
     lib.fenerf_pack_field.argtypes = [P(FieldDesc), P(FieldParams), vp, sz, vp]
     lib.fenerf_field_fingerprint.restype = C.c_int
     lib.fenerf_field_fingerprint.argtypes = [P(FieldDesc), P(FieldParams), vp, vp]
+    lib.fenerf_pack_field_bridge.restype = C.c_int
+    lib.fenerf_pack_field_bridge.argtypes = [P(FieldDesc), P(FieldParams), P(BridgeParams), vp, sz, vp]
+    lib.fenerf_field_fingerprint_bridge.restype = C.c_int
+    lib.fenerf_field_fingerprint_bridge.argtypes = [P(FieldDesc), P(FieldParams), P(BridgeParams), vp, vp]
     lib.fenerf_siren_points.restype = C.c_int
     lib.fenerf_siren_points.argtypes = [P(FieldDesc), vp, vp, vp, vp, i32, i64, i32, i32, vp, i32, vp, vp]
     lib.fenerf_camera_poses.restype = C.c_int

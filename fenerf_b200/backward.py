@@ -22,7 +22,9 @@ backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per
           Heads, the pre-multiplied label chain and the grid (``fenerf_grid_scatter_add``, from the first colour layer's
           dU, or from the first layer's where the grid feeds the trunk, EmbeddingPiGAN256) close the chain.  A label FiLM
           field (SPATIALSIRENSEMANTIC) recomputes its label layer from the trunk output at FiLM row T and runs it
-          backward like a colour layer, its dU diag(f) W joining the trunk's dA.
+          backward like a colour layer, its dU diag(f) W joining the trunk's dA.  A bridge field (SPATIALSIRENAUGDISENTANGLE,
+          RESSIRENDISENTANGLE) recomputes v = W_v a + b_v (+ the position) off the trunk output and its first colour layer
+          from [dir, v] like a first layer; dv = dU diag(f) W_c0[:, v] (+ dsigma a for RES) joins the trunk as dv W_v.
 Gradients flow to the FiLM table (and through torch's autograd into the mapping network / latents /
 frequency offsets) and to every field parameter.  The fp16 gradient stream is scaled by a power of two
 taken from max|d raw| on the device (no host sync) and unscaled at the end.
@@ -80,7 +82,15 @@ class FieldWeights:
         color = list(color) if isinstance(color, torch.nn.ModuleList) else [color]
         self.trunk = [(l.layer.weight, l.layer.bias) for l in net]
         self.color = [(l.layer.weight, l.layer.bias) for l in color]
-        self.sigma = (module.final_layer.weight, module.final_layer.bias)
+        # (RESSIRENDISENTANGLE has no final_layer: its density is the chain on v)
+        self.sigma = None if spec.bridge_res else (module.final_layer.weight, module.final_layer.bias)
+        # a bridge field's v = Linear(256 -> 3) of the trunk output, its density chain and color_layer_pre (RES)
+        self.bridge = None
+        if spec.bridge:
+            lin = module.res_coord_layer if spec.bridge_res else module.color_layer_pre[0]
+            self.bridge = (lin.weight, lin.bias)
+        self.density = [(m.weight, m.bias) for m in module.density_layer_linear] if spec.bridge_res else []
+        self.pre = (module.color_layer_pre[0].weight, module.color_layer_pre[0].bias) if spec.bridge_res else None
         self.rgb = (module.color_layer_linear[0].weight, module.color_layer_linear[0].bias)
         self.labels = []
         if spec.label_dim:
@@ -95,7 +105,9 @@ class FieldWeights:
 
     def parameters(self):
         ps = []
-        for w, b in self.film_layers() + [self.sigma, self.rgb] + self.labels:
+        extra = [self.sigma] if self.sigma is not None else []
+        extra += ([self.bridge] if self.bridge is not None else []) + self.density + ([self.pre] if self.pre else [])
+        for w, b in self.film_layers() + extra + [self.rgb] + self.labels:
             ps += [w, b]
         if self.grid is not None:
             ps.append(self.grid)
@@ -131,6 +143,35 @@ def _label_chain_grads(labels, d_weff, d_beff):
     return [(w3.t() @ dw, w3.t() @ db), (dw @ w1.t() + torch.outer(db, b1), db)]
 
 
+def _linear_chain_eff(chain):
+    """Weff, beff of an activation-free chain of Linears (first applied first), in fp64."""
+    weff, beff = None, None
+    for w, b in chain:
+        w, b = w.detach().double(), b.detach().double()
+        weff, beff = (w, b) if weff is None else (w @ weff, w @ beff + b)
+    return weff, beff
+
+
+def _linear_chain_grads(chain, d_weff, d_beff):
+    """Gradients of every Linear of an activation-free chain from those of its product map (fp64; RESSIRENDISENTANGLE's
+    density_layer_linear): layer i sees dW_i = U_i^T (dWeff R_i^T + dbeff s_i^T), db_i = U_i^T dbeff, with U_i the
+    product of the layers after it, R_i the one before it and s_i the bias that reaches its input."""
+    ws = [w.detach().double() for w, _ in chain]
+    bs = [b.detach().double() for _, b in chain]
+    dw, db = d_weff.double(), d_beff.double()
+    out = []
+    for i in range(len(chain)):
+        u = torch.eye(ws[i].shape[0], dtype=torch.float64, device=dw.device)
+        for w in ws[i + 1:]:
+            u = w @ u
+        r = torch.eye(ws[0].shape[1], dtype=torch.float64, device=dw.device)
+        s_in = torch.zeros(ws[0].shape[1], dtype=torch.float64, device=dw.device)
+        for w, b in zip(ws[:i], bs[:i]):
+            r, s_in = w @ r, w @ s_in + b
+        out.append((u.t() @ (dw @ r.t() + torch.outer(db, s_in)), u.t() @ db))
+    return out
+
+
 class _FieldBackward:
     """Accumulates the gradients of one field over any number of point sets."""
 
@@ -156,7 +197,8 @@ class _FieldBackward:
         self.gt = self.spec.grid_trunk
         self.k0 = 3 + G if self.gt else 3
         self.k0_pad = (self.k0 + 7) // 8 * 8
-        self.kx = 3 if self.gt else 3 + G
+        self.br, self.res = self.spec.bridge, self.spec.bridge_res
+        self.kx = 3 if self.gt else 6 if self.br else 3 + G
         self.kx_pad = (self.kx + 7) // 8 * 8
         # per-image accumulators (scaled by `scale`)
         self.colsum = torch.zeros((B, self.n_film, 256), dtype=torch.float32, device=dev)
@@ -183,6 +225,25 @@ class _FieldBackward:
         self.own_gemm = (not exact) and BWD_GEMM == "wgmma"
         self.Wh16 = [None] + [w.detach().to(self.dt).contiguous() for w, _ in fw.trunk[1:]]
         wc0 = fw.color[0][0].detach().float()
+        self.bias = [b.detach().float().contiguous() for _, b in fw.film_layers()]
+        if self.br:
+            # the first colour layer on [dir, v]; RES: color_layer_pre folded into its v columns and bias (fp64)
+            wc0d = fw.color[0][0].detach().double()
+            if self.res:
+                pw, pb = (t.detach().double() for t in fw.pre)
+                self.Wc0eff = torch.cat([wc0d[:, :3], wc0d[:, 3:] @ pw], dim=1).float().contiguous()
+                self.bias[self.c0] = (fw.color[0][1].detach().double() + wc0d[:, 3:] @ pb).float().contiguous()
+                a, c = _linear_chain_eff(fw.density)
+                self.dens_a, self.dens_c = a.float().reshape(3), c.float().reshape(())
+                self.d_a = torch.zeros(3, dtype=torch.float32, device=dev)
+                self.d_c = torch.zeros((), dtype=torch.float32, device=dev)
+            else:
+                self.Wc0eff = wc0.contiguous()
+            self.Wv32 = fw.bridge[0].detach().float().contiguous()                  # (3, 256)
+            self.bv32 = fw.bridge[1].detach().float().contiguous()
+            self.d_wv = torch.zeros((3, 256), dtype=torch.float32, device=dev)
+            self.d_bv = torch.zeros(3, dtype=torch.float32, device=dev)
+            wc0 = torch.cat([self.Wc0eff, torch.zeros((256, 256), dtype=torch.float32, device=dev)], dim=1)
         self.Wc0x_narrow = wc0[:, :self.kx].contiguous()                          # (256, 3 + G) fp32
         self.Wc16 = [wc0[:, self.kx:].to(self.dt).contiguous()] + [w.detach().to(self.dt).contiguous() for w, _ in fw.color[1:]]
         # the weights the grid features meet, (256, G): the first colour layer's, or the first layer's with the grid in
@@ -209,12 +270,12 @@ class _FieldBackward:
         if L and not self.lf:      # (a label FiLM field's head acts on the label layer: its rows stay zero here)
             weff, _ = _label_eff(fw.labels)
             heads[:L] = weff
-        heads[L] = fw.sigma[0].detach().float().reshape(-1)
+        if fw.sigma is not None:       # (RES: the density comes from v; its gradient goes there)
+            heads[L] = fw.sigma[0].detach().float().reshape(-1)
         self.Wheads32 = heads
         rgbw = torch.zeros((self.n_rgb, 256), dtype=self.dt, device=dev)
         rgbw[:self.spec.rgb_dim] = fw.rgb[0].detach().to(self.dt)
         self.Wrgb16 = rgbw
-        self.bias = [b.detach().float().contiguous() for _, b in fw.film_layers()]
 
     # ---- one point set: points (B, ppb, 3), dirs (B, ppb/dir_group, 3), raw / d_raw (B, ppb, C) ----
     def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
@@ -293,7 +354,14 @@ class _FieldBackward:
                     A[T], Gt[T] = ops.gemm_nt_film(A[T - 1], self.Wl16, self.bias[T], self.film, b0, T, ppb)
                 else:
                     A[T], Gt[T] = self._stash(_mm32(A[T - 1], self.Wl16.t()), T, b0, P, ppb)
-            if own:     # the narrow inputs [dir, grid features] ride as a fifth 64-wide k-chunk of the same kernel
+            v = None
+            if self.br:     # v off the trunk output (fp32), then the first colour layer on [dir, v] like a first layer
+                v = _mm32(A[T - 1], self.Wv32.t().to(self.dt)) + self.bv32
+                if self.res:
+                    v = v + x
+                extras = torch.cat([extras, v], dim=1).contiguous()
+                A[c0], Gt[c0] = self._stash(None, c0, b0, P, ppb, xin=extras, wx=self.Wc0eff)
+            elif own:     # the narrow inputs [dir, grid features] ride as a fifth 64-wide k-chunk of the same kernel
                 e64 = torch.zeros((P, 64), dtype=torch.float16, device=dev)
                 e64[:, :self.kx] = extras
                 A[c0], Gt[c0] = ops.gemm_nt_film(A[T - 1], self.Wc16[0], self.bias[c0], self.film, b0, c0, ppb, narrow_in=e64,
@@ -313,6 +381,7 @@ class _FieldBackward:
             _lib.check(lib.fenerf_head_grads(d_raw.data_ptr(), raw.data_ptr(), P, spec.out_dim, self.L, self.scale.data_ptr(),
                                              dH.data_ptr(), dRGB.data_ptr(), self.dtc, st))
             a_last = A[self.n_film - 1]
+            d_sigma = dH[:, self.L].float()
             self.d_rgb_w += _mm32(dRGB.t(), a_last)
             self.d_rgb_b += dRGB.float().sum(0)
             if self.lf:     # label rows on the label layer's activations, the sigma row on the trunk's
@@ -327,6 +396,10 @@ class _FieldBackward:
             for j in range(Cn - 1, -1, -1):
                 idx = c0 + j
                 self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dU now
+                if self.br and j == 0:
+                    dA = self._bridge_back(dA, extras, v, A[T - 1], d_sigma, k, ppb, b0, b1)
+                    A[idx], Gt[idx] = None, None
+                    break
                 a_in = A[idx - 1] if j else A[T - 1]
                 du3 = dA.view(k, ppb, 256).transpose(1, 2)
                 self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(du3, a_in.view(k, ppb, 256))
@@ -365,6 +438,24 @@ class _FieldBackward:
             x16[:, :self.k0] = x
             self.dW_b[0][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), x16.view(k, ppb, self.k0_pad))
 
+    def _bridge_back(self, dU, extras, v, a_trunk, d_sigma, k, ppb, b0, b1):
+        """First colour layer of a bridge field on [dir, v]: its narrow weight gradient, dv = dU diag(f) W_c0[:, v]
+        (+ dsigma a for RES), v's own gradients, and the trunk's dA = dv W_v.  In fp32 (3 columns)."""
+        P = k * ppb
+        du = dU.float().view(k, ppb, 256)
+        e = torch.zeros((P, self.kx_pad), dtype=torch.float32, device=self.dev)
+        e[:, :self.kx] = extras
+        self.dWx_b[b0:b1] += torch.bmm(du.transpose(1, 2), e.view(k, ppb, self.kx_pad))
+        fwv = self.film[b0:b1, self.c0, 0].unsqueeze(2) * self.Wc0eff[:, 3:6]      # (k, 256, 3), no division by f
+        dv = torch.bmm(du, fwv).view(P, 3)
+        if self.res:
+            dv = dv + d_sigma.unsqueeze(1) * self.dens_a
+            self.d_a += (d_sigma.unsqueeze(1) * v).sum(0)
+            self.d_c += d_sigma.sum()
+        self.d_wv += dv.t() @ a_trunk.float()
+        self.d_bv += dv.sum(0)
+        return (dv @ self.Wv32).to(self.dt)
+
     def _grid_grad(self, dU, points, k, ppb, b0, b1):
         """d features = dU diag(f_b) W_feat, (P, G), of the layer the grid feeds, scattered into the grid accumulator."""
         P = k * ppb
@@ -386,18 +477,39 @@ class _FieldBackward:
             w32 = w.detach().float()
             if idx == 0:
                 m = self.dW_b[0][:, :, :self.k0]                                # columns [pos], or [feat, pos]
+            elif idx == self.c0 and self.br:
+                m = self.dWx_b[:, :, :self.kx]                                  # [dir, v]
+                w32 = self.Wc0eff                                               # (RES: color_layer_pre folded in)
             elif idx == self.c0:
                 m = torch.cat([self.dWx_b[:, :, :self.kx], self.dW_b[idx]], dim=2)   # column order of the reference: [dir, feat, x]
             else:
                 m = self.dW_b[idx]                                          # M_b = dU_b^T a
-            df = torch.einsum('fk,bfk->bf', w32, m) + b.detach().float().unsqueeze(0) * dp
+            df = torch.einsum('fk,bfk->bf', w32, m) + self.bias[idx].unsqueeze(0) * dp
             d_film[:, idx, 0] = df * inv
             d_film[:, idx, 1] = dp * inv
             grads[id(w)] = torch.einsum('bf,bfk->fk', f, m) * inv
             grads[id(b)] = (f * dp).sum(0) * inv
         L = self.L
-        grads[id(fw.sigma[0])] = (self.d_heads_w[L] * inv).reshape(fw.sigma[0].shape)
-        grads[id(fw.sigma[1])] = (self.d_heads_b[L] * inv).reshape(fw.sigma[1].shape)
+        if fw.sigma is not None:
+            grads[id(fw.sigma[0])] = (self.d_heads_w[L] * inv).reshape(fw.sigma[0].shape)
+            grads[id(fw.sigma[1])] = (self.d_heads_b[L] * inv).reshape(fw.sigma[1].shape)
+        if self.br:
+            grads[id(fw.bridge[0])] = self.d_wv * inv
+            grads[id(fw.bridge[1])] = self.d_bv * inv
+        if self.res:
+            # the folded maps back to their Linears, in fp64: color_layer_pre and the first colour layer's x columns from
+            # the gradient of the folded [dir, v] weight g and bias gb; the density chain from d a, d c
+            w, b = fw.color[0]
+            g, gb = grads[id(w)].double(), grads[id(b)].double()
+            wx = w.detach().double()[:, 3:]
+            pw, pb = (t.detach().double() for t in fw.pre)
+            grads[id(w)] = torch.cat([g[:, :3], g[:, 3:] @ pw.t() + torch.outer(gb, pb)], dim=1).float()
+            grads[id(fw.pre[0])] = (wx.t() @ g[:, 3:]).float()
+            grads[id(fw.pre[1])] = (wx.t() @ gb).float()
+            chain = _linear_chain_grads(fw.density, (self.d_a * inv).reshape(1, 3), (self.d_c * inv).reshape(1))
+            for (dw_, db_), (gw, gbb) in zip(fw.density, chain):
+                grads[id(dw_)] = gw.float()
+                grads[id(db_)] = gbb.float()
         n_rgb = self.spec.rgb_dim
         grads[id(fw.rgb[0])] = self.d_rgb_w[:n_rgb] * inv
         grads[id(fw.rgb[1])] = self.d_rgb_b[:n_rgb] * inv

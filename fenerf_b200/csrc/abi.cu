@@ -76,6 +76,10 @@ int make_layout(const fenerf_field_desc* field, FnLayout* L) {
         return fail(FENERF_E_UNSUPPORTED, "unknown field flag combination 0x%x for this field: FENERF_FIELD_GRID_TRUNK only "
                     "with grid_channels 32, label_dim 0 and no other flag (label_dim %d, grid %d)", (unsigned)field->reserved,
                     field->label_dim, field->grid_channels);
+    if (r == -5)
+        return fail(FENERF_E_UNSUPPORTED, "unknown field flag combination 0x%x for this field: FENERF_FIELD_BRIDGE only with "
+                    "label_dim 0, no grid and no other flag than FENERF_FIELD_BRIDGE_RES, which needs it (label_dim %d, "
+                    "grid %d)", (unsigned)field->reserved, field->label_dim, field->grid_channels);
     FN_REQUIRE(r == 0, "unsupported field description");
     return 0;
 }
@@ -105,23 +109,37 @@ size_t fenerf_packed_bytes(const fenerf_field_desc* field) {
     return L.total;
 }
 
-int fenerf_pack_field(const fenerf_field_desc* field, const fenerf_field_params* params, void* packed,
-                      size_t packed_bytes, void* stream) {
+int fenerf_pack_field_bridge(const fenerf_field_desc* field, const fenerf_field_params* params,
+                             const fenerf_bridge_params* bridge, void* packed, size_t packed_bytes, void* stream) {
     FnLayout L;
     if (int e = make_layout(field, &L)) return e;
     FN_REQUIRE(params && packed, "params/packed is NULL");
     FN_REQUIRE(((uintptr_t)packed & 1023) == 0, "packed buffer must be 1024-byte aligned");
+    FN_REQUIRE(!L.bridge_res || bridge, "FENERF_FIELD_BRIDGE_RES: the density chain and color_layer_pre come in "
+               "fenerf_bridge_params (fenerf_pack_field_bridge)");
     if (packed_bytes < L.total) return fail(FENERF_E_WORKSPACE, "packed buffer too small: %zu < %zu", packed_bytes, L.total);
-    return pack_field(L, params, packed, (cudaStream_t)stream);
+    return pack_field(L, params, packed, (cudaStream_t)stream, bridge);
 }
 
-int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_params* params, uint64_t* out,
-                             void* stream) {
+int fenerf_pack_field(const fenerf_field_desc* field, const fenerf_field_params* params, void* packed,
+                      size_t packed_bytes, void* stream) {
+    return fenerf_pack_field_bridge(field, params, nullptr, packed, packed_bytes, stream);
+}
+
+int fenerf_field_fingerprint_bridge(const fenerf_field_desc* field, const fenerf_field_params* params,
+                                    const fenerf_bridge_params* bridge, uint64_t* out, void* stream) {
     FnLayout L;
     if (int e = make_layout(field, &L)) return e;
     FN_REQUIRE(params && out, "params/out is NULL");
     FN_REQUIRE(((uintptr_t)out & 7) == 0, "out must be 8-byte aligned");
-    return field_fingerprint(L, params, reinterpret_cast<unsigned long long*>(out), (cudaStream_t)stream);
+    FN_REQUIRE(!L.bridge_res || bridge, "FENERF_FIELD_BRIDGE_RES: the density chain and color_layer_pre come in "
+               "fenerf_bridge_params (fenerf_field_fingerprint_bridge)");
+    return field_fingerprint(L, params, reinterpret_cast<unsigned long long*>(out), (cudaStream_t)stream, bridge);
+}
+
+int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_params* params, uint64_t* out,
+                             void* stream) {
+    return fenerf_field_fingerprint_bridge(field, params, nullptr, out, stream);
 }
 
 int fenerf_siren_points(const fenerf_field_desc* field, const void* packed, const float* points, const float* dirs,

@@ -101,11 +101,13 @@ __device__ __forceinline__ float sample_alpha(float delta, float act, float* dec
 __device__ __forceinline__ float transmittance_term(float alpha) { return __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f); }
 
 // ---- entry points of the individual translation units (called by abi.cu) ----
-int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed, cudaStream_t st);
+int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed, cudaStream_t st,
+               const fenerf_bridge_params* bridge = nullptr);
 int siren_points_exact(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
                        int batch, long long ppb, int dir_group, int lock_dirs, const int32_t* only_idx, int n_only, float* out,
                        cudaStream_t st, int sigma_only = 0);
-int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st);
+int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st,
+                      const fenerf_bridge_params* bridge = nullptr);
 int siren_points_fast(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
                       int batch, long long ppb, int dir_group, int lock_dirs, float* out, int sigma_only, cudaStream_t st,
                       float* sigma_out = nullptr);

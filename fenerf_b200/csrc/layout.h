@@ -45,6 +45,13 @@
 //                    rows from n_out on are zero.
 //   grid trunk       (FENERF_FIELD_GRID_TRUNK) the grid features feed the first layer (first_k = 3 + G) instead of the
 //                    first colour layer (kx = 3: the direction alone), so the density needs them too.
+//   bridge           (FENERF_FIELD_BRIDGE) the first colour layer reads [dir, v] alone (kx = 6): its fp32 copy is
+//                    [kx_pad = 16][256] (rows dir, v, zero pad), it has no 256-wide image, and its input-chunk image holds v
+//                    in slots 32..40 (hi, hi, lo) beside the direction.  The trunk head carries v's weights in rows 1..3
+//                    (sigma_row 0), their fp32 copy and bias sit at bridge_w.  With FENERF_FIELD_BRIDGE_RES v adds the
+//                    position, sigma = a . v + c (a, c: the density chain folded in double, after the bias at bridge_w;
+//                    the trunk head's sigma row is zero), and the first colour layer's v columns and bias are
+//                    W_c0[:, 3:] W_pre and b_c0 + W_c0[:, 3:] b_pre, folded in double as well.
 //
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
@@ -99,20 +106,32 @@ struct FnLayout {
     int32_t grid_trunk;     // the variant flag FENERF_FIELD_GRID_TRUNK
     int32_t first_k;        // inputs of the first layer: 3, or 3 + G with the grid in the trunk
     size_t first_img_lo;    // grid trunk: the feature columns' fp16 low parts, image as first_img (0 otherwise)
+    int32_t bridge;         // the variant flag FENERF_FIELD_BRIDGE: the colour branch reads [dir, v], v off the trunk
+    int32_t bridge_res;     // FENERF_FIELD_BRIDGE_RES: v adds the position, the density is a . v + c
+    size_t bridge_w;        // bridge: [3][256] f32 weights of v, b[3], then a[3], c (RES; 0 otherwise)
 };
 
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head or -4 for the grid in
-// the trunk on a field shape no reference class has, or -1 if the description is outside what the kernels support.
+// Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head, -4 for the grid in
+// the trunk or -5 for a bridge on a field shape no reference class has, or -1 if the description is outside what the
+// kernels support.
 static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     if (!f || !L) return -1;
-    if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD | FENERF_FIELD_GRID_TRUNK)) return -2;
+    if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD | FENERF_FIELD_GRID_TRUNK | FENERF_FIELD_BRIDGE |
+                        FENERF_FIELD_BRIDGE_RES))
+        return -2;
     const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
     const int feature_head = (f->reserved & FENERF_FIELD_FEATURE_HEAD) ? 1 : 0;
     const int grid_trunk = (f->reserved & FENERF_FIELD_GRID_TRUNK) ? 1 : 0;
+    const int bridge = (f->reserved & FENERF_FIELD_BRIDGE) ? 1 : 0;
+    const int bridge_res = (f->reserved & FENERF_FIELD_BRIDGE_RES) ? 1 : 0;
     // EmbeddingPiGAN256: a 32-channel grid, no labels, no other flag
     if (grid_trunk && (f->reserved != FENERF_FIELD_GRID_TRUNK || f->grid_channels != 32 || f->label_dim != 0)) return -4;
+    // SPATIALSIRENAUGDISENTANGLE (bridge) and RESSIRENDISENTANGLE (bridge + res): no labels, no grid, no other flag
+    if ((bridge || bridge_res) &&
+        ((f->reserved & ~(FENERF_FIELD_BRIDGE | FENERF_FIELD_BRIDGE_RES)) || !bridge || f->label_dim != 0 || f->grid_channels != 0))
+        return -5;
     if (feature_head) {
         // SPATIALSIRENBASELINEHD (label_dim 0) and SPATIALSIRENSEMANTICHD (label FiLM, label_dim 64), no grid
         if (f->grid_channels != 0 || f->label_dim != (label_film ? FN_FEAT : 0)) return -3;
@@ -136,8 +155,10 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     L->sigma_row = feature_head ? FN_FEAT_SIGMA_ROW : f->label_dim;
     L->grid_trunk = grid_trunk;
     L->first_k = grid_trunk ? 3 + f->grid_channels : 3;
-    L->kx = grid_trunk ? 3 : 3 + f->grid_channels;
+    L->kx = grid_trunk ? 3 : bridge ? 6 : 3 + f->grid_channels;
     L->kx_pad = (L->kx + 15) / 16 * 16;
+    L->bridge = bridge;
+    L->bridge_res = bridge_res;
     L->label_dim = f->label_dim;
     L->grid_channels = f->grid_channels;
     L->grid_res = f->grid_res;
@@ -150,10 +171,11 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     L->first_img = take(FN_IMG_BYTES);
     for (int l = 0; l < FN_MAX_HIDDEN; ++l) { L->hid_w32[l] = L->hid_b[l] = L->hid_img[l] = 0; }
     for (int l = 0; l < L->n_hidden; ++l) {
-        int k = FN_H + (l == L->color0 ? L->kx_pad : 0);   // the first colour layer's extra rows
+        const bool narrow = bridge && l == L->color0;     // a bridge field's first colour layer: [dir, v] only
+        int k = narrow ? L->kx_pad : FN_H + (l == L->color0 ? L->kx_pad : 0);   // the first colour layer's extra rows
         L->hid_w32[l] = take((size_t)k * FN_H * 4);
         L->hid_b[l] = take(FN_H * 4);
-        L->hid_img[l] = take((size_t)(FN_H / FN_KCHUNK) * FN_IMG_BYTES);
+        L->hid_img[l] = narrow ? 0 : take((size_t)(FN_H / FN_KCHUNK) * FN_IMG_BYTES);
     }
     L->color0_ximg = take(FN_IMG_BYTES);
     L->sigma_w = take((FN_H + 1) * 4);
@@ -174,6 +196,7 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
         if (label_film) L->label.img = take(FN_HEAD_IMG_BYTES(FN_FEAT));
     }
     L->first_img_lo = grid_trunk ? take(FN_IMG_BYTES) : 0;
+    L->bridge_w = bridge ? take((3 * FN_H + 3 + 3 + 1) * 4) : 0;
     L->total = off;
     return 0;
 }

@@ -179,6 +179,89 @@ __global__ void pack_trunk_head_kernel(const float* __restrict__ sw, const float
     }
 }
 
+// ---- bridge fields (FENERF_FIELD_BRIDGE): the first colour layer on [dir, v] and the trunk head with v's rows -------
+// First colour layer, one thread per output n: fp32 copy wt [16][256] (rows dir, v, zero pad), bias, and the input-chunk
+// image: dir in slots 16.., v in slots 32.. (hi, hi, lo each).  w is [256][in_dim]: [dir, v] (in_dim 6), or, with
+// color_layer_pre (pre_w [256][3], pre_b [256]; in_dim 3 + 256), [dir, x] whose x columns are folded with it in double:
+// W_v = W_x W_pre, b = b_c0 + W_x b_pre.
+__global__ void pack_bridge_color0_kernel(const float* __restrict__ w, int in_dim, const float* __restrict__ b,
+                                          const float* __restrict__ pre_w, const float* __restrict__ pre_b,
+                                          float* __restrict__ wt, float* __restrict__ bo, unsigned char* __restrict__ img) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= FN_H) return;
+    float col[6];
+    for (int k = 0; k < 3; ++k) col[k] = w[(size_t)n * in_dim + k];
+    if (pre_w) {
+        double v[3] = {0.0, 0.0, 0.0}, bb = (double)b[n];
+        for (int m = 0; m < FN_H; ++m) {
+            const double x = (double)w[(size_t)n * in_dim + 3 + m];
+            for (int j = 0; j < 3; ++j) v[j] += x * (double)pre_w[m * 3 + j];
+            bb += x * (double)pre_b[m];
+        }
+        for (int j = 0; j < 3; ++j) col[3 + j] = (float)v[j];
+        bo[n] = (float)bb;
+    } else {
+        for (int j = 0; j < 3; ++j) col[3 + j] = w[(size_t)n * in_dim + 3 + j];
+        bo[n] = b[n];
+    }
+    for (int k = 0; k < 16; ++k) wt[k * FN_H + n] = k < 6 ? col[k] : 0.f;
+    for (int k = 0; k < FN_KCHUNK; ++k) *reinterpret_cast<__half*>(img + fn_sw128_offset(n, k)) = __float2half_rn(0.f);
+    for (int s = 0; s < 2; ++s) {
+        const int slot = s == 0 ? FN_SLOT_DIR : FN_SLOT_FEAT;
+        for (int k = 0; k < 3; ++k) {
+            const float v = col[3 * s + k];
+            *reinterpret_cast<__half*>(img + fn_sw128_offset(n, slot + k)) = f16_hi(v);
+            *reinterpret_cast<__half*>(img + fn_sw128_offset(n, slot + 3 + k)) = f16_hi(v);
+            *reinterpret_cast<__half*>(img + fn_sw128_offset(n, slot + 6 + k)) = f16_lo(v);
+        }
+    }
+}
+
+// The trunk head of a bridge field (one block, 256 threads): the sigma copy (zero with the density chain), the image
+// [4][32 rows][64 k] with sigma in row 0 and v's weights in rows 1..3, and the bridge section: v's fp32 weights and
+// bias, then -- with the density chain dw/db ([256][3], [256][256], [256][256], [1][256]) -- a = W4 W3 W2 W1 and
+// c = W4 (W3 (W2 b1 + b2) + b3) + b4, in double.
+__global__ void pack_bridge_head_kernel(const float* __restrict__ sw, const float* __restrict__ sb,
+                                        const float* __restrict__ vw, const float* __restrict__ vb, fenerf_bridge_params ch,
+                                        FnLayout L, unsigned char* __restrict__ packed) {
+    __shared__ double u[3][FN_H];     // W4, W4 W3, W4 W3 W2
+    const int t = threadIdx.x;
+    float* so = reinterpret_cast<float*>(packed + L.sigma_w);
+    float* bw = reinterpret_cast<float*>(packed + L.bridge_w);
+    so[t] = L.bridge_res ? 0.f : sw[t];
+    if (t == 0) so[FN_H] = L.bridge_res ? 0.f : sb[0];
+    for (int i = t; i < 3 * FN_H; i += blockDim.x) bw[i] = vw[i];
+    if (t < 3) bw[3 * FN_H + t] = vb[t];
+    for (int i = t; i < 32 * FN_H; i += blockDim.x) {
+        const int row = i / FN_H, k = i % FN_H;
+        float v = 0.f;
+        if (row == 0 && !L.bridge_res) v = sw[k];
+        else if (row >= 1 && row <= 3) v = vw[(row - 1) * FN_H + k];
+        unsigned char* chunk = packed + L.head_img + (size_t)(k / FN_KCHUNK) * (32 * FN_KCHUNK * 2);
+        *reinterpret_cast<__half*>(chunk + fn_sw128_offset(row, k % FN_KCHUNK)) = __float2half_rn(v);
+    }
+    if (!L.bridge_res) return;
+    u[0][t] = (double)ch.density_w[3][t];
+    __syncthreads();
+    for (int s = 1; s < 3; ++s) {
+        const float* wm = ch.density_w[3 - s];       // W3, then W2: [256][256]
+        double acc = 0.0;
+        for (int m = 0; m < FN_H; ++m) acc += u[s - 1][m] * (double)wm[m * FN_H + t];
+        u[s][t] = acc;
+        __syncthreads();
+    }
+    if (t < 3) {
+        double acc = 0.0;
+        for (int m = 0; m < FN_H; ++m) acc += u[2][m] * (double)ch.density_w[0][m * 3 + t];
+        bw[3 * FN_H + 3 + t] = (float)acc;
+    } else if (t == 3) {
+        double c = (double)ch.density_b[3][0];
+        for (int m = 0; m < FN_H; ++m)
+            c += u[0][m] * (double)ch.density_b[2][m] + u[1][m] * (double)ch.density_b[1][m] + u[2][m] * (double)ch.density_b[0][m];
+        bw[3 * FN_H + 6] = (float)c;
+    }
+}
+
 // ---- grid: (G, D, H, W) channel-major -> [D][H][W][G] channels-last ---------------------------
 // one block per (z, y) line: read G rows of R contiguous x, write R*G contiguous floats
 __global__ void pack_grid_kernel(const float* __restrict__ in, float* __restrict__ out, __half* __restrict__ out16, int R, int G) {
@@ -202,13 +285,16 @@ __global__ void pack_grid_kernel(const float* __restrict__ in, float* __restrict
 
 // ---- fingerprint of the raw parameters (EMA copy_to / restore write through .data without bumping
 // torch's version counter, so the host cannot see that the packed copy went stale) ------------------
+// (40 segments hold every field but the bridge fields, whose extra Linears take a wider instantiation)
+template <int N>
 struct FpSegments {
-    const float* ptr[40];
-    unsigned long long count[40];
+    const float* ptr[N];
+    unsigned long long count[N];
     int n;
 };
 
-__global__ void fingerprint_kernel(FpSegments seg, unsigned long long* __restrict__ out) {
+template <int N>
+__global__ void fingerprint_kernel(FpSegments<N> seg, unsigned long long* __restrict__ out) {
     unsigned long long h0 = 0, h1 = 0;
     const unsigned long long tid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
@@ -237,8 +323,9 @@ __global__ void fingerprint_kernel(FpSegments seg, unsigned long long* __restric
 
 }  // namespace
 
-int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st) {
-    FpSegments seg;
+int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned long long* out, cudaStream_t st,
+                      const fenerf_bridge_params* bridge) {
+    FpSegments<56> seg;
     seg.n = 0;
     auto add = [&](const float* ptr, unsigned long long count) {
         if (ptr && count) { seg.ptr[seg.n] = ptr; seg.count[seg.n] = count; ++seg.n; }
@@ -246,22 +333,38 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
     // (a label FiLM layer takes a hidden slot: it is hashed with the label parameters below, label_w[0])
     const int n_trunk = L.trunk_hidden + 1, n_color = L.n_hidden - L.color0;
     for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? L.first_k : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
-    add(p->sigma_w, FN_H); add(p->sigma_b, 1);
-    for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (unsigned long long)(i == 0 ? L.kx + FN_H : FN_H) * FN_H); add(p->color_b[i], FN_H); }
+    if (!L.bridge_res) { add(p->sigma_w, FN_H); add(p->sigma_b, 1); }
+    // (a bridge field's first colour layer: [dir, v], or [dir, x] before color_layer_pre with the density chain)
+    const unsigned long long c0_in = L.bridge ? (L.bridge_res ? 3 + FN_H : 6) : L.kx + FN_H;
+    for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (i == 0 ? c0_in : FN_H) * FN_H); add(p->color_b[i], FN_H); }
     add(p->rgb_w, (unsigned long long)L.rgb.n_out * FN_H); add(p->rgb_b, L.rgb.n_out);
     if (L.label_dim > 0) {
         add(p->label_w[0], FN_H * FN_H); add(p->label_b[0], FN_H);
         add(p->label_w[1], FN_H * FN_H); add(p->label_b[1], FN_H);
         add(p->label_w[2], (unsigned long long)L.label_dim * FN_H); add(p->label_b[2], L.label_dim);
     }
+    if (L.bridge) { add(p->label_w[0], 3 * FN_H); add(p->label_b[0], 3); }
+    if (L.bridge_res && bridge) {
+        const unsigned long long in[4] = {3, FN_H, FN_H, FN_H}, outs[4] = {FN_H, FN_H, FN_H, 1};
+        for (int i = 0; i < 4; ++i) { add(bridge->density_w[i], in[i] * outs[i]); add(bridge->density_b[i], outs[i]); }
+        add(bridge->pre_w, 3 * FN_H); add(bridge->pre_b, FN_H);
+    }
     if (L.grid_channels > 0) add(p->grid, (unsigned long long)L.grid_channels * L.grid_res * L.grid_res * L.grid_res);
     FN_CUDA_OK(cudaMemsetAsync(out, 0, 16, st));
-    fingerprint_kernel<<<num_sms() * 4, 256, 0, st>>>(seg, out);
+    if (seg.n <= 40) {      // every field but the bridge fields: the instantiation it always had
+        FpSegments<40> s40;
+        s40.n = seg.n;
+        for (int i = 0; i < seg.n; ++i) { s40.ptr[i] = seg.ptr[i]; s40.count[i] = seg.count[i]; }
+        fingerprint_kernel<40><<<num_sms() * 4, 256, 0, st>>>(s40, out);
+    } else {
+        fingerprint_kernel<56><<<num_sms() * 4, 256, 0, st>>>(seg, out);
+    }
     FN_LAUNCH_OK("fingerprint_kernel");
     return 0;
 }
 
-int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, cudaStream_t st) {
+int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, cudaStream_t st,
+               const fenerf_bridge_params* bridge) {
     unsigned char* packed = static_cast<unsigned char*>(packed_v);
     FN_REQUIRE(p->trunk_w[0] && p->trunk_b[0], "trunk_w[0]/trunk_b[0] missing");
     pack_first_kernel<<<1, 256, 0, st>>>(p->trunk_w[0], L.first_k - 3, p->trunk_b[0], (float*)(packed + L.first_w),
@@ -277,6 +380,16 @@ int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, 
         const float* w = l < L.trunk_hidden ? p->trunk_w[l + 1] : is_label ? p->label_w[0] : p->color_w[l - L.color0];
         const float* b = l < L.trunk_hidden ? p->trunk_b[l + 1] : is_label ? p->label_b[0] : p->color_b[l - L.color0];
         FN_REQUIRE(w && b, "weight/bias of hidden layer %d missing", l);
+        if (L.bridge && is_c0) {     // [dir, v] alone: no 256-wide image (layout.h)
+            FN_REQUIRE(!L.bridge_res || (bridge->pre_w && bridge->pre_b), "color_layer_pre missing");
+            pack_bridge_color0_kernel<<<1, 256, 0, st>>>(w, L.bridge_res ? 3 + FN_H : 6, b,
+                                                         L.bridge_res ? bridge->pre_w : nullptr,
+                                                         L.bridge_res ? bridge->pre_b : nullptr,
+                                                         (float*)(packed + L.hid_w32[l]), (float*)(packed + L.hid_b[l]),
+                                                         packed + L.color0_ximg);
+            FN_LAUNCH_OK("pack_bridge_color0_kernel");
+            continue;
+        }
         int in_dim = is_c0 ? L.kx + FN_H : FN_H;
         int x_off = is_c0 ? L.kx : 0;
         int kx = is_c0 ? L.kx : 0, kx_pad = is_c0 ? L.kx_pad : 0;
@@ -289,7 +402,7 @@ int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, 
             FN_LAUNCH_OK("pack_color0_ximg_kernel");
         }
     }
-    FN_REQUIRE(p->sigma_w && p->sigma_b && p->rgb_w && p->rgb_b, "sigma/rgb head parameters missing");
+    FN_REQUIRE((L.bridge_res || (p->sigma_w && p->sigma_b)) && p->rgb_w && p->rgb_b, "sigma/rgb head parameters missing");
     pack_linear_head_kernel<<<1, 256, 0, st>>>(p->rgb_w, p->rgb_b, L.rgb, packed);
     FN_LAUNCH_OK("pack_linear_head_kernel");
     if (L.label_film) {      // no chain to pre-multiply: the head is one Linear
@@ -307,8 +420,20 @@ int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, 
         label_step3_kernel<<<1, 256, 0, st>>>((float*)(packed + L.label_w), L.label_dim);
         FN_LAUNCH_OK("label_step3_kernel");
     }
-    pack_trunk_head_kernel<<<1, 256, 0, st>>>(p->sigma_w, p->sigma_b, L, packed);
-    FN_LAUNCH_OK("pack_trunk_head_kernel");
+    if (L.bridge) {
+        FN_REQUIRE(p->label_w[0] && p->label_b[0], "bridge field: label_w[0] / label_b[0] (the Linear(256 -> 3) to v) missing");
+        fenerf_bridge_params ch{};
+        if (L.bridge_res) {
+            for (int i = 0; i < 4; ++i)
+                FN_REQUIRE(bridge->density_w[i] && bridge->density_b[i], "density chain layer %d missing", i);
+            ch = *bridge;
+        }
+        pack_bridge_head_kernel<<<1, 256, 0, st>>>(p->sigma_w, p->sigma_b, p->label_w[0], p->label_b[0], ch, L, packed);
+        FN_LAUNCH_OK("pack_bridge_head_kernel");
+    } else {
+        pack_trunk_head_kernel<<<1, 256, 0, st>>>(p->sigma_w, p->sigma_b, L, packed);
+        FN_LAUNCH_OK("pack_trunk_head_kernel");
+    }
     if (L.grid_channels > 0) {
         FN_REQUIRE(p->grid, "grid missing");
         int R = L.grid_res, G = L.grid_channels;

@@ -29,6 +29,11 @@
 //
 // Grid-trunk fields (kGridTrunk, FENERF_FIELD_GRID_TRUNK): the first layer sums over the position and the 32 grid features
 // the tile gathered into A rows 259..290, for the density alone as well (GUARD refinement, density grids).
+//
+// Bridge fields (kBridge, FENERF_FIELD_BRIDGE): after the trunk head, v = W_v x + b_v (+ the position with
+// FENERF_FIELD_BRIDGE_RES, whose density is then a . v + c) goes to A rows 259..261 beside the direction; the trunk
+// output is not needed any more, so [dir, v] is copied to A rows 0..15 (zero padded) and the first colour layer is a
+// 16-row k-sum over them.
 #include "siren_common.cuh"
 #include "sm90.cuh"
 
@@ -171,7 +176,8 @@ __device__ __forceinline__ float grid_feature(const float* __restrict__ grid, in
     return out;
 }
 
-template <bool kGather, int P, bool kLabelFilm = false, bool kFeatureHead = false, bool kGridTrunk = false>
+template <bool kGather, int P, bool kLabelFilm = false, bool kFeatureHead = false, bool kGridTrunk = false,
+          bool kBridge = false>
 __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned char* smem_raw) {
     constexpr int TM = 16 * P;
     Smem<P>& s = *reinterpret_cast<Smem<P>*>(smem_raw);
@@ -259,12 +265,30 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                 // heads on the trunk output: sigma, then the pre-multiplied label map
                 const float* sw = reinterpret_cast<const float*>(pk + L.sigma_w);
                 const float* lw = reinterpret_cast<const float*>(pk + L.label_w);
+                const float* bw = reinterpret_cast<const float*>(pk + L.bridge_w);   // kBridge: W_v [3][256], b_v, a, c
+                if constexpr (kBridge) {
+                    // v -> A rows 259..261 (free: a bridge field has no grid); the density of a RES field needs it
+                    if (L.bridge_res || !a.sigma_only) {
+                        for (int it = tid; it < TM * 3; it += NTHREADS) {
+                            const int pt = it % TM, j = it / TM;
+                            float r = __ldg(bw + 3 * FN_H + j);
+                            for (int k = 0; k < FN_H; ++k) r = fmaf(s.A[k][pt], __ldg(bw + j * FN_H + k), r);
+                            // RES: input + coords_res, the warped position plus the Linear's output (siren.py:1072-1073)
+                            s.A[FN_H + 3 + j][pt] = L.bridge_res ? __fadd_rn(s.pos[j][pt], r) : r;
+                        }
+                        __syncthreads();
+                    }
+                }
                 // (a label FiLM field's labels come from its label branch below: no trunk label rows)
                 for (int it = tid; it < TM * (1 + (a.sigma_only ? 0 : L.trunk_labels)); it += NTHREADS) {
                     int pt = it % TM, o = it / TM;
                     const float* w = o == 0 ? sw : lw + (size_t)(o - 1) * FN_H;
                     float r = o == 0 ? __ldg(sw + FN_H) : __ldg(lw + FENERF_MAX_LABEL * FN_H + (o - 1));
-                    for (int k = 0; k < FN_H; ++k) r = fmaf(s.A[k][pt], __ldg(w + k), r);
+                    if (kBridge && L.bridge_res) {       // sigma = a . v + c, the density chain folded at pack time
+                        r = __ldg(bw + 3 * FN_H + 6);
+                        for (int j = 0; j < 3; ++j) r = fmaf(s.A[FN_H + 3 + j][pt], __ldg(bw + 3 * FN_H + 3 + j), r);
+                    } else
+                        for (int k = 0; k < FN_H; ++k) r = fmaf(s.A[k][pt], __ldg(w + k), r);
                     long long flat = s.flat[pt];
                     if (flat >= 0) {
                         if (kGather && a.guard_stats && o == 0) {
@@ -327,7 +351,16 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
                     continue;                                                  // s.A still holds the trunk output
                 }
             }
-            const int K = FN_H + (l == L.color0 ? L.kx_pad : 0);
+            int K = FN_H + (l == L.color0 ? L.kx_pad : 0);
+            if (kBridge && l == L.color0) {
+                // [dir, v] (A rows 256..261) -> rows 0..15, zero padded: the first colour layer reads them alone
+                for (int i = tid; i < L.kx_pad * TM; i += NTHREADS) {
+                    const int k = i / TM, pt = i % TM;
+                    s.A[k][pt] = k < L.kx ? s.A[FN_H + k][pt] : 0.f;
+                }
+                __syncthreads();
+                K = L.kx_pad;
+            }
             init_bias(reinterpret_cast<const float*>(pk + L.hid_b[l]), acc, tid);
             gemm_tile(s, reinterpret_cast<const float*>(pk + L.hid_w32[l]), K, acc, tid);
             film_store(s, a.film, L.n_film, l + 1, acc, tid);
@@ -350,22 +383,22 @@ __device__ __forceinline__ void siren_exact_body(const ExactArgs& a, unsigned ch
     }
 }
 
-template <bool kGather, int P, bool kLabelFilm, bool kFeatureHead = false, bool kGridTrunk = false>
+template <bool kGather, int P, bool kLabelFilm, bool kFeatureHead = false, bool kGridTrunk = false, bool kBridge = false>
 __global__ void __launch_bounds__(NTHREADS, 2) siren_exact_kernel(ExactArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    siren_exact_body<kGather, P, kLabelFilm, kFeatureHead, kGridTrunk>(a, smem_raw);
+    siren_exact_body<kGather, P, kLabelFilm, kFeatureHead, kGridTrunk, kBridge>(a, smem_raw);
 }
 
 // GUARD refinement: the list length is only known on the device.  Short lists (small renders; fields whose densities
 // rarely come near zero) take 16-point tiles -- lowest latency per tile, one wave as long as the list fits
 // 16 x gridDim points -- longer ones 32-point tiles, which keep it to one wave up to twice that and do twice the FFMA
 // per weight slab fetched from L2.
-template <bool kGridTrunk>
+template <bool kGridTrunk, bool kBridge = false>
 __global__ void __launch_bounds__(NTHREADS, 1) siren_exact_guard_kernel(ExactArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int n_only = *a.n_only_dev;
-    if (n_only <= 16 * (int)gridDim.x) siren_exact_body<true, 1, false, false, kGridTrunk>(a, smem_raw);
-    else siren_exact_body<true, 2, false, false, kGridTrunk>(a, smem_raw);
+    if (n_only <= 16 * (int)gridDim.x) siren_exact_body<true, 1, false, false, kGridTrunk, kBridge>(a, smem_raw);
+    else siren_exact_body<true, 2, false, false, kGridTrunk, kBridge>(a, smem_raw);
 }
 
 }  // namespace
@@ -397,7 +430,10 @@ int siren_points_exact(const FnLayout& L, const unsigned char* packed, const flo
     };
     const bool label_film = L.label_film && !sigma_only, feature_head = L.feature_head && !sigma_only;
     int e;
-    if (L.grid_trunk)     // (the density alone too: the trunk needs the grid features)
+    if (L.bridge)         // (the density alone too: a RES field's comes from v)
+        e = gather ? launch(siren_exact_kernel<true, 4, false, false, false, true>)
+                   : launch(siren_exact_kernel<false, 4, false, false, false, true>);
+    else if (L.grid_trunk)     // (the density alone too: the trunk needs the grid features)
         e = gather ? launch(siren_exact_kernel<true, 4, false, false, true>) : launch(siren_exact_kernel<false, 4, false, false, true>);
     else if (feature_head) {
         if (gather) e = label_film ? launch(siren_exact_kernel<true, 4, true, true>) : launch(siren_exact_kernel<true, 4, false, true>);
@@ -470,7 +506,10 @@ int guard_refine(const FnLayout& L, const unsigned char* packed, const float* po
         return 0;
     };
     // (the density of a grid-trunk field needs the grid features: its own instantiation)
-    if (int e = L.grid_trunk ? launch(siren_exact_guard_kernel<true>) : launch(siren_exact_guard_kernel<false>)) return e;
+    // (and a bridge field's, RES's from v: its own as well)
+    if (int e = L.bridge ? launch(siren_exact_guard_kernel<false, true>)
+                         : L.grid_trunk ? launch(siren_exact_guard_kernel<true>) : launch(siren_exact_guard_kernel<false>))
+        return e;
     FN_LAUNCH_OK("siren_exact_kernel(guard)");
     return 0;
 }

@@ -9,6 +9,8 @@ int siren_fast_label_launch(const void* args, int blocks, cudaStream_t st);
 int siren_fast_hd_launch(const void* args, int blocks, bool label_film, cudaStream_t st);
 // the grid-trunk instantiation (siren_fast_grid.cu), the density alone included
 int siren_fast_grid_launch(const void* args, int blocks, cudaStream_t st);
+// the bridge instantiation (siren_fast_bridge.cu), the density alone included
+int siren_fast_bridge_launch(const void* args, int blocks, cudaStream_t st);
 // the debug instantiations (siren_fast_debug.cu): variant 1 = one column pair in four on the software sine, 2 / 3 = the
 // timeline of the production / the variant-1 kernel
 int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st);
@@ -32,6 +34,10 @@ bool build_loads(const FnLayout& L, FastArgs& A, bool sigma_only) {
         if (l == L.trunk_hidden) {
             push(L.head_img, 4 * HEAD_CHUNK);
             if (sigma_only) return A.n_loads <= MAX_LOADS;
+        }
+        if (L.bridge && l == L.color0) {             // [dir, v] alone: the input-chunk image, no 256-wide halves
+            push(L.color0_ximg, 2 * CHUNK);
+            continue;
         }
         push(L.hid_img[l], 2 * CHUNK);               // half 0, k-chunks 0, 1
         push(L.hid_img[l] + 2 * CHUNK, 2 * CHUNK);   // half 0, k-chunks 2, 3
@@ -84,12 +90,14 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     static std::atomic<int> attr_set[kMaxDevices];
     const int blocks = (int)(n_pairs < (long long)num_sms() ? n_pairs : (long long)num_sms());
     if (const int variant = g_variant.load()) {
-        FN_REQUIRE(!L.grid_trunk, "the debug point-network variants do not cover fields with the grid in the trunk");
+        FN_REQUIRE(!L.grid_trunk && !L.bridge,
+                   "the debug point-network variants do not cover fields with the grid in the trunk or a bridge");
         a.trace = g_trace;
         a.trace_ctas = g_trace_ctas;
         return siren_fast_debug_launch(&a, blocks, label_film, feature_head, variant, st);
     }
     if (L.grid_trunk) return siren_fast_grid_launch(&a, blocks, st);
+    if (L.bridge) return siren_fast_bridge_launch(&a, blocks, st);
     if (feature_head) return siren_fast_hd_launch(&a, blocks, label_film, st);
     if (label_film) return siren_fast_label_launch(&a, blocks, st);
     FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<false>, attr_set, (int)SMEM_TOTAL));

@@ -39,10 +39,16 @@
 //                  three times, hi * W_hi + lo * W_hi + hi * W_lo, the low parts of W coming from a second image in the
 //                  weight stream (DESIGN section 5 has the error budget).  The first colour layer takes the direction
 //                  slice only.
+//   kBridge        (FENERF_FIELD_BRIDGE) the trunk head also computes v's three rows (1..3; sigma in row 0).  v is formed
+//                  in fp32 from the accumulators plus the bias (plus the position with FENERF_FIELD_BRIDGE_RES, whose
+//                  density is then a . v + c in fp32), split hi / lo into the staging row's slots 32..40, and the first
+//                  colour layer is one narrow MMA group per half: the direction and v slices against the input-chunk image,
+//                  no 256-wide part.
 //
 // The plain and the label FiLM instantiations live in translation units of their own (siren_fast.cu,
 // siren_fast_label.cu), the two feature-head ones in a third (siren_fast_hd.cu) and the grid-trunk one in a fourth
-// (siren_fast_grid.cu), so that the plain one compiles exactly as it does on its own.  The debug
+// (siren_fast_grid.cu) and the bridge one in a fifth (siren_fast_bridge.cu), so that the plain one compiles exactly as it
+// does on its own.  The debug
 // instantiations -- a share of the sines on the FMA pipe (kSoftSin, soft_sinf) and the clock64 timeline (kTrace) -- live
 // in siren_fast_debug.cu.
 #pragma once
@@ -143,7 +149,7 @@ struct FastArgs {
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
 template <bool kLabelFilm, bool kFeatureHead = false, int kSoftSin = kSoftSinEvery, bool kTrace = false,
-          bool kGridTrunk = false>
+          bool kGridTrunk = false, bool kBridge = false>
 __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_constant__ FastArgs a) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
@@ -466,12 +472,47 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                             const float v = dh[4 * i + 2 * rr + e];
                             if (o < trunk_labels) {
                                 if (!a.sigma_only) a.out[flat * C + o] = fmaf(v, __ldg(lb + FENERF_MAX_LABEL), __ldg(lb + o));
-                            } else if (o == sigma_row) {
+                            } else if (o == sigma_row && !(kBridge && L.bridge_res)) {
                                 const float sig = v + __ldg(sigma_w + FN_H);
                                 a.out[flat * C + (C - 1)] = sig;
                                 if (a.sigma_out) a.sigma_out[flat] = sig;
                             }
                         }
+                }
+                if constexpr (kBridge) {
+                    // v = head rows 1..3 + bias (+ the position): this thread holds rows 2q, 2q + 1 of points r0, r0 + 8; the
+                    // quad's q = 0 thread gathers row 2, 3 from q = 1 and owns the point (every lane shuffles)
+                    const float* bw = reinterpret_cast<const float*>(a.packed + L.bridge_w);
+#pragma unroll
+                    for (int rr = 0; rr < 2; ++rr) {
+                        const float o0 = dh[2 * rr], o1 = dh[2 * rr + 1];
+                        const float p2 = __shfl_xor_sync(0xffffffffu, o0, 1), p3 = __shfl_xor_sync(0xffffffffu, o1, 1);
+                        if (q != 0) continue;
+                        const long long pnt = p0 + r0 + 8 * rr;
+                        float v[3] = {o1 + __ldg(bw + 3 * FN_H), p2 + __ldg(bw + 3 * FN_H + 1), p3 + __ldg(bw + 3 * FN_H + 2)};
+                        if (L.bridge_res) {
+                            if (pnt < a.ppb) {
+                                const long long flat = b * a.ppb + pnt;
+#pragma unroll
+                                for (int j = 0; j < 3; ++j) v[j] += __fmul_rn(a.points[flat * 3 + j], L.input_scale);
+                                float sig = __ldg(bw + 3 * FN_H + 6);
+#pragma unroll
+                                for (int j = 0; j < 3; ++j) sig = fmaf(__ldg(bw + 3 * FN_H + 3 + j), v[j], sig);
+                                a.out[flat * C + (C - 1)] = sig;
+                                if (a.sigma_out) a.sigma_out[flat] = sig;
+                            }
+                        }
+                        if (!a.sigma_only) {
+                            __half* row = xs + (r0 + 8 * rr) * XSTRIDE + FN_SLOT_FEAT;
+#pragma unroll
+                            for (int j = 0; j < 3; ++j) {
+                                __half hi, lo;
+                                split_f16(v[j], hi, lo);
+                                row[j] = hi; row[3 + j] = lo; row[6 + j] = hi;
+                            }
+                        }
+                    }
+                    if (!a.sigma_only) wg_bar(wg);       // v in the staging rows before the first colour layer reads them
                 }
                 if (a.sigma_only) { stop = true; break; }
                 if constexpr (kLabelFilm) {
@@ -543,7 +584,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             }
             // ---- FiLM layer l + 1: weight image halves 64 KB apart, two 32 KB slabs per half ----
             const bool c0 = (l == L.color0);     // first colour layer: + direction / grid-feature slots
-            const int nx = !kGridTrunk && L.grid_channels > 0 ? 3 : 1;     // (a grid-trunk field: the direction alone)
+            const bool narrow = kBridge && c0;   // a bridge field's: the direction and v slices alone
+            // (a grid-trunk field: the direction alone; a bridge field: the direction and v)
+            const int nx = kBridge ? 2 : !kGridTrunk && L.grid_channels > 0 ? 3 : 1;
             uint32_t xf[3][4];
             if (c0)
 #pragma unroll
@@ -552,23 +595,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             const float4* fs = nullptr;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                uint32_t sl[2];
+                uint32_t sl[2] = {0u, 0u};
+                if (narrow && h == 0) w_x = acquire(slot_x);
                 turn_begin();
                 wg_fence();
+                if (!narrow)
 #pragma unroll
-                for (int sb = 0; sb < 2; ++sb) {
-                    const uint32_t w = acquire(sl[sb]);
+                    for (int sb = 0; sb < 2; ++sb) {
+                        const uint32_t w = acquire(sl[sb]);
 #pragma unroll
-                    for (int c = 0; c < 2; ++c)
+                        for (int c = 0; c < 2; ++c)
 #pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            mma_rs_n128(d, act[8 * sb + 4 * c + k], desc_kmajor(w + c * CHUNK + 32 * k), (sb | c | k) ? 1u : 0u);
-                }
+                            for (int k = 0; k < 4; ++k)
+                                mma_rs_n128(d, act[8 * sb + 4 * c + k], desc_kmajor(w + c * CHUNK + 32 * k), (sb | c | k) ? 1u : 0u);
+                    }
                 if (c0) {
-                    if (h == 0) w_x = acquire(slot_x);
+                    if (h == 0 && !narrow) w_x = acquire(slot_x);
 #pragma unroll
                     for (int s = 0; s < 3; ++s)
-                        if (s < nx) mma_rs_n128(d, xf[s], desc_kmajor(w_x + h * CHUNK + 32 * (1 + s)), 1u);
+                        if (s < nx) mma_rs_n128(d, xf[s], desc_kmajor(w_x + h * CHUNK + 32 * (1 + s)), (narrow && s == 0) ? 0u : 1u);
                 }
                 wg_commit();
                 turn_end(c0 ? TG_COLOR0 : TG_HIDDEN);
@@ -577,8 +622,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 fence_regs(d);
                 fence_regs(act);
                 fence_regs(xf);
-                release(sl[0]);
-                release(sl[1]);
+                if (!narrow) {
+                    release(sl[0]);
+                    release(sl[1]);
+                }
                 if (c0 && h == 1) release(slot_x);
                 if (h == 0) fs = film_acquire();
                 if (h == 0) film_epi(fs, 0, nxt);

@@ -40,7 +40,9 @@ def field_desc(spec) -> "_lib.FieldDesc":
                           input_scale=spec.input_scale,
                           reserved=(_lib.FIELD_LABEL_FILM if spec.label_film else 0)
                           | (_lib.FIELD_FEATURE_HEAD if spec.feature_head else 0)
-                          | (_lib.FIELD_GRID_TRUNK if spec.grid_trunk else 0))
+                          | (_lib.FIELD_GRID_TRUNK if spec.grid_trunk else 0)
+                          | (_lib.FIELD_BRIDGE if spec.bridge else 0)
+                          | (_lib.FIELD_BRIDGE_RES if spec.bridge_res else 0))
 
 
 def _f32(t, device):
@@ -51,7 +53,7 @@ def _f32(t, device):
 
 
 def collect_params(module, device):
-    """-> (FieldParams, keepalive list). Parameter order / names per SURVEY.md section 8b."""
+    """-> (FieldParams, BridgeParams or None, keepalive list). Parameter order / names per SURVEY.md section 8b."""
     spec = module.field_spec()
     if getattr(module, "hidden_dim", 256) != _lib.HIDDEN:
         raise ValueError("the sm_90a kernels are specialised for hidden_dim=256 (got %s)" % module.hidden_dim)
@@ -66,8 +68,9 @@ def collect_params(module, device):
     for i, layer in enumerate(module.network):
         p.trunk_w[i] = ptr(layer.layer.weight)
         p.trunk_b[i] = ptr(layer.layer.bias)
-    p.sigma_w = ptr(module.final_layer.weight)
-    p.sigma_b = ptr(module.final_layer.bias)
+    if not spec.bridge_res:      # (RESSIRENDISENTANGLE has no final_layer: its density is a chain on v)
+        p.sigma_w = ptr(module.final_layer.weight)
+        p.sigma_b = ptr(module.final_layer.bias)
     color = module.color_layer_sine
     color = list(color) if isinstance(color, torch.nn.ModuleList) else [color]
     for i, layer in enumerate(color):
@@ -96,7 +99,24 @@ def collect_params(module, device):
             p.label_b[i] = ptr(lin.bias)
     if spec.grid_channels:
         p.grid = ptr(module.spatial_embeddings)
-    return p, keep
+    bridge = None
+    if spec.bridge:
+        # v = Linear(256 -> 3) of the trunk output: color_layer_pre, or res_coord_layer with the density chain
+        lin = module.res_coord_layer if spec.bridge_res else module.color_layer_pre[0]
+        p.label_w[0] = ptr(lin.weight)
+        p.label_b[0] = ptr(lin.bias)
+    if spec.bridge_res:
+        bridge = _lib.BridgeParams()
+        for i, lin in enumerate(module.density_layer_linear):
+            bridge.density_w[i] = ptr(lin.weight)
+            bridge.density_b[i] = ptr(lin.bias)
+        bridge.pre_w = ptr(module.color_layer_pre[0].weight)
+        bridge.pre_b = ptr(module.color_layer_pre[0].bias)
+    return p, bridge, keep
+
+
+def _bridge_ref(bridge):
+    return C.byref(bridge) if bridge is not None else None
 
 
 def pack_field(module) -> PackedField:
@@ -112,9 +132,9 @@ def pack_field(module) -> PackedField:
     with torch.cuda.device(device):
         buf = torch.empty(nbytes + 1024, dtype=torch.uint8, device=device)
         ptr = (buf.data_ptr() + 1023) // 1024 * 1024
-        params, keep = collect_params(module, device)
+        params, bridge, keep = collect_params(module, device)
         stream = torch.cuda.current_stream(device).cuda_stream
-        _lib.check(lib.fenerf_pack_field(C.byref(desc), C.byref(params), ptr, nbytes, stream))
+        _lib.check(lib.fenerf_pack_field_bridge(C.byref(desc), C.byref(params), _bridge_ref(bridge), ptr, nbytes, stream))
         event = torch.cuda.Event()
         event.record()
         del keep
@@ -131,9 +151,9 @@ def fingerprint(module):
     desc = field_desc(module.field_spec())
     with torch.cuda.device(device):
         out = torch.empty(2, dtype=torch.int64, device=device)
-        params, keep = collect_params(module, device)
-        _lib.check(lib.fenerf_field_fingerprint(C.byref(desc), C.byref(params), out.data_ptr(),
-                                                torch.cuda.current_stream(device).cuda_stream))
+        params, bridge, keep = collect_params(module, device)
+        _lib.check(lib.fenerf_field_fingerprint_bridge(C.byref(desc), C.byref(params), _bridge_ref(bridge), out.data_ptr(),
+                                                       torch.cuda.current_stream(device).cuda_stream))
         a, b = out.tolist()
         del keep
     return a, b

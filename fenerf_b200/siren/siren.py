@@ -20,6 +20,8 @@ Reference interfaces mirrored (file:line in the reference tree):
   SPATIALSIRENSEMANTIC                        siren/siren.py:597-671
   SPATIALSIRENBASELINESEMANTIC                siren/siren.py:674-744
   SPATIALSIRENDISENTANGLE                     siren/siren.py:747-813
+  SPATIALSIRENAUGDISENTANGLE                  siren/siren.py:904-979
+  RESSIRENDISENTANGLE                         siren/siren.py:982-1082
   SPATIALSIRENSEMANTICDISENTANGLE             siren/siren.py:1085-1161
   SIRENBASELINESEMANTICDISENTANGLE            siren/siren.py:1163-1229
   TextureEmbeddingPiGAN128SEMANTICDISENTANGLE siren/siren.py:1451-1530
@@ -154,6 +156,10 @@ class FieldSpec:
                    (siren/siren.py:300-301, 1365-1366)
     grid_trunk     the grid features feed the first trunk layer, cat[feat, pos] -> 256, and not the colour branch
                    (siren/siren.py:396-398)
+    bridge         the colour branch reads cat[ray_dir(3), v(3)], v = Linear(256 -> 3)(trunk output), not the trunk's 256
+                   activations (siren/siren.py:965-967)
+    bridge_res     with bridge: v = warped position + Linear(256 -> 3)(trunk output), the density is a chain of four
+                   Linears on v and the first colour layer reads cat[ray_dir, Linear(3 -> 256)(v)] (siren/siren.py:1072-1076)
     out_dim        label_dim + 3 (rgb; 64 features with feature_head) + 1 (sigma); channel order [labels, rgb, sigma]
     """
     trunk_layers: int
@@ -167,6 +173,8 @@ class FieldSpec:
     label_film: bool = False
     feature_head: bool = False
     grid_trunk: bool = False
+    bridge: bool = False
+    bridge_res: bool = False
 
     @property
     def rgb_dim(self):
@@ -716,3 +724,81 @@ class TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_DIM_96(TextureEmbeddingPiGAN12
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs, hidden_dim=256)
         self.spatial_embeddings = nn.Parameter(torch.randn(1, 32, 96, 96, 96) * 0.1)
+
+
+class SPATIALSIRENAUGDISENTANGLE(_DoubleLatentField):
+    """SPATIALSIRENDISENTANGLE with a bridge between trunk and colour branch (siren/siren.py:904-979): v =
+    color_layer_pre(x) is 3 wide, and 8 colour FiLM layers start from FiLM(cat[dir, v], 6 -> 256).  FiLM rows: trunk
+    0..7, colour 8..15; output [rgb, sigma].  color_layer_pre keeps nn.Linear's default init, as in the reference."""
+
+    def __init__(self, input_dim=2, z_geo_dim=100, z_app_dim=100, hidden_dim=256, output_dim=1, device=None):
+        super().__init__()
+        self.device = device
+        self.input_dim = input_dim
+        self.z_geo_dim = z_geo_dim
+        self.z_app_dim = z_app_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+        self.max_batch_size = 2500
+
+        widths = [3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        self.final_layer = nn.Linear(hidden_dim, 1)
+        self.color_layer_pre = nn.Sequential(nn.Linear(hidden_dim, 3))
+        cwidths = [3 + 3] + [hidden_dim] * 8
+        self.color_layer_sine = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(cwidths[:-1], cwidths[1:]))
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 3))
+        self.geo_mapping_network = CustomMappingNetwork(z_geo_dim, 256, len(self.network) * hidden_dim * 2)
+        self.app_mapping_network = CustomMappingNetwork(z_app_dim, 256, len(self.color_layer_sine) * hidden_dim * 2)
+
+        for part in (self.network, self.final_layer, self.color_layer_sine, self.color_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(first_layer_film_sine_init)
+        self.gridwarper = UniformBoxWarp(0.24)
+
+    def field_spec(self):
+        return FieldSpec(trunk_layers=len(self.network), color_layers=len(self.color_layer_sine), label_dim=0,
+                         grid_channels=0, grid_res=0, input_scale=float(self.gridwarper.scale_factor), out_dim=4,
+                         double_latent=True, bridge=True)
+
+
+class RESSIRENDISENTANGLE(_DoubleLatentField):
+    """The residual variant (siren/siren.py:982-1082): v = warped position + res_coord_layer(x); the density is
+    density_layer_linear(v), four Linears without an activation, and 6 colour FiLM layers start from
+    FiLM(cat[dir, color_layer_pre(v)], 259 -> 256).  No final_layer.  FiLM rows: trunk 0..7, colour 8..13; output
+    [rgb, sigma].  res_coord_layer and color_layer_pre keep nn.Linear's default init, and the unused Softmax is kept, as
+    in the reference."""
+
+    def __init__(self, input_dim=2, z_geo_dim=100, z_app_dim=100, hidden_dim=256, output_dim=1, device=None):
+        super().__init__()
+        self.device = device
+        self.input_dim = input_dim
+        self.z_geo_dim = z_geo_dim
+        self.z_app_dim = z_app_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+        self.max_batch_size = 2500
+
+        widths = [3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        self.res_coord_layer = nn.Linear(hidden_dim, 3)
+        self.density_layer_linear = nn.Sequential(
+            nn.Linear(3, hidden_dim), nn.Linear(hidden_dim, hidden_dim), nn.Linear(hidden_dim, hidden_dim),
+            nn.Linear(hidden_dim, 1))
+        self.color_layer_pre = nn.Sequential(nn.Linear(3, hidden_dim))
+        cwidths = [hidden_dim + 3] + [hidden_dim] * 6
+        self.color_layer_sine = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(cwidths[:-1], cwidths[1:]))
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 3))
+        self.geo_mapping_network = CustomMappingNetwork(z_geo_dim, 256, len(self.network) * hidden_dim * 2)
+        self.app_mapping_network = CustomMappingNetwork(z_app_dim, 256, len(self.color_layer_sine) * hidden_dim * 2)
+
+        for part in (self.network, self.density_layer_linear, self.color_layer_sine, self.color_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(first_layer_film_sine_init)
+        self.activation = nn.Softmax(dim=-1)     # unused, as in the reference
+        self.gridwarper = UniformBoxWarp(0.24)
+
+    def field_spec(self):
+        return FieldSpec(trunk_layers=len(self.network), color_layers=len(self.color_layer_sine), label_dim=0,
+                         grid_channels=0, grid_res=0, input_scale=float(self.gridwarper.scale_factor), out_dim=4,
+                         double_latent=True, bridge=True, bridge_res=True)

@@ -65,6 +65,14 @@ extern "C" {
  *   x = FiLM_0(cat[grid_feat(G), x(3)] -> 256)(x); ...;  c = FiLM(cat[dir(3), x(256)] -> 256)
  * EmbeddingPiGAN256 (siren.py:341-410):     trunk 8, color 1, label 0, grid 32 x 64^3 (FENERF_FIELD_GRID_TRUNK),
  *                                scale 2/0.24, out 4.
+ * With FENERF_FIELD_BRIDGE the colour branch does not read the trunk's 256 activations but a 3-vector v taken off them:
+ *   v = Linear(256->3)(x);  c = FiLM(cat[dir(3), v(3)] -> 256); ...      (FENERF_FIELD_BRIDGE alone)
+ *   v = pos * input_scale + Linear(256->3)(x);  sigma = Linear chain 3->256->256->256->1 (no activation)(v);
+ *   c = FiLM(cat[dir(3), Linear(3->256)(v)] -> 256); ...                 (with FENERF_FIELD_BRIDGE_RES)
+ * SPATIALSIRENAUGDISENTANGLE (siren.py:904-979): trunk 8, color 8, label 0, grid 0 (FENERF_FIELD_BRIDGE), scale 2/0.24,
+ *                                out 4.
+ * RESSIRENDISENTANGLE (siren.py:982-1082):   trunk 8, color 6, label 0, grid 0 (FENERF_FIELD_BRIDGE |
+ *                                FENERF_FIELD_BRIDGE_RES), scale 2/0.24, out 4.
  * The hidden width is fixed at 256.                                                            */
 #define FENERF_MAX_TRUNK 8
 #define FENERF_MAX_COLOR 8
@@ -84,6 +92,14 @@ extern "C" {
                                          [256][G+3] in the column order [feat, pos], color_w[0] is [256][3+256] (dir, x).
                                          Only the reference's shape is accepted (EmbeddingPiGAN256): grid_channels 32,
                                          label_dim 0, no other flag.  Anything else with this bit is FENERF_E_UNSUPPORTED. */
+#define FENERF_FIELD_BRIDGE 0x4       /* the colour branch starts from v = Linear(256->3)(x) (label_w[0] [3][256], label_b[0]
+                                         [3]): color_w[0] is [256][3+3] (dir, v).  Only label_dim 0, no grid, out_dim 4,
+                                         alone or with FENERF_FIELD_BRIDGE_RES (SPATIALSIRENAUGDISENTANGLE). */
+#define FENERF_FIELD_BRIDGE_RES 0x10  /* with FENERF_FIELD_BRIDGE: v = pos * input_scale + Linear(256->3)(x), the density is
+                                         a chain of four Linears on v and the first colour layer reads cat[dir,
+                                         Linear(3->256)(v)]: color_w[0] is [256][3+256], sigma_w / sigma_b are unused and
+                                         the chain's parameters come in fenerf_bridge_params, so such a field is packed and
+                                         fingerprinted by the _bridge entry points only (RESSIRENDISENTANGLE). */
 
 typedef struct fenerf_field_desc {
     int32_t trunk_layers;   /* 2..8 */
@@ -133,6 +149,23 @@ int fenerf_pack_field(const fenerf_field_desc* field, const fenerf_field_params*
  * `param.data.copy_`, which torch's version counters do not see. */
 int fenerf_field_fingerprint(const fenerf_field_desc* field, const fenerf_field_params* params,
                              uint64_t* out /* device, 2 x u64 */, void* stream);
+
+/* The parameters a FENERF_FIELD_BRIDGE_RES field has beyond fenerf_field_params (raw torch layout as above):
+ * density_layer_linear [256][3], [256][256], [256][256], [1][256] and its biases, and color_layer_pre [256][3], [256].
+ * The packer folds the chain into sigma = a . v + c and color_layer_pre into the first colour layer's v columns, both in
+ * double on the device.  With `bridge` NULL these two calls are fenerf_pack_field / fenerf_field_fingerprint; a
+ * FENERF_FIELD_BRIDGE_RES field needs it. */
+typedef struct fenerf_bridge_params {
+    const float* density_w[4];
+    const float* density_b[4];
+    const float* pre_w;
+    const float* pre_b;
+} fenerf_bridge_params;
+
+int fenerf_pack_field_bridge(const fenerf_field_desc* field, const fenerf_field_params* params,
+                             const fenerf_bridge_params* bridge, void* packed, size_t packed_bytes, void* stream);
+int fenerf_field_fingerprint_bridge(const fenerf_field_desc* field, const fenerf_field_params* params,
+                                    const fenerf_bridge_params* bridge, uint64_t* out /* device, 2 x u64 */, void* stream);
 
 /* precision modes of the point network */
 #define FENERF_PRECISION_EXACT 0  /* fp32 FFMA + precise sinf everywhere (CUDA cores)            */

@@ -1,6 +1,7 @@
 """256^3 density grid through the point network (extract_double_semantic_shapes.py:59-62 workload):
 density-only entry vs the full evaluation, for both benchmarked models, SPATIALSIRENBASELINE (C) and the grid-trunk
-EmbeddingPiGAN256 (L), whose density needs the grid.  Prints one line per run.
+EmbeddingPiGAN256 (L), whose density needs the grid, and the bridge fields AUG (M, against H) and RES (N, whose
+density comes from v; against G).  Prints one line per run.
 
     python tools/bench_density.py [res] [--models C,L] [--rounds N]     (--rounds: the models N times, alternating)"""
 import os, sys
@@ -9,9 +10,11 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
 import _cases
 import _grid_trunk  # (registers model L)
+import _bridge_fields  # (registers models M, N: the bridge fields AUG and RES)
 from fenerf_b200 import ops
 
-CASE = {"A": "a_small", "B": "b_small", "C": "c_small", "L": "l_small"}
+CASE = {"A": "a_small", "B": "b_small", "C": "c_small", "L": "l_small", "G": "g_small", "H": "h_small",
+        "M": "m_small", "N": "n_small"}
 
 def main():
     import argparse
@@ -23,13 +26,14 @@ def main():
     res = args.res
     print("device: %s" % torch.cuda.get_device_name("cuda:0"))
     for model in args.models.split(",") * args.rounds:
-        case = _cases.CASE_BY_NAME.get(CASE[model]) or _grid_trunk.CASE_BY_NAME[CASE[model]]
+        case = (_cases.CASE_BY_NAME.get(CASE[model]) or _grid_trunk.CASE_BY_NAME.get(CASE[model])
+                or _bridge_fields.CASE_BY_NAME[CASE[model]])
         gen = _cases.build_mirror(case, "cuda:0")
         lin = torch.linspace(-0.15, 0.15, res, device="cuda")
         pts = torch.stack(torch.meshgrid(lin, lin, lin, indexing="ij"), -1).reshape(1, -1, 3).contiguous()
         dirs = torch.zeros(1, 1, 3, device="cuda"); dirs[..., -1] = -1
         with torch.no_grad():
-            if model != "B":
+            if _cases.n_latents(model) == 1:
                 film = gen.siren.film_table(*gen.siren.mapping_network(torch.randn(1, 256, device="cuda")))
             else:
                 fg, pg = gen.siren.geo_mapping_network(torch.randn(1, 256, device="cuda"))
