@@ -24,7 +24,10 @@ backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per
           field (SPATIALSIRENSEMANTIC) recomputes its label layer from the trunk output at FiLM row T and runs it
           backward like a colour layer, its dU diag(f) W joining the trunk's dA.  A bridge field (SPATIALSIRENAUGDISENTANGLE,
           RESSIRENDISENTANGLE) recomputes v = W_v a + b_v (+ the position) off the trunk output and its first colour layer
-          from [dir, v] like a first layer; dv = dU diag(f) W_c0[:, v] (+ dsigma a for RES) joins the trunk as dv W_v.
+          from [dir, v] like a first layer; dv = dU diag(f) W_c0[:, v] (+ dsigma a for RES) joins the trunk as dv W_v:
+          dU diag(f_b) (W_c0[:, v] W_v) through the same per-image product as every other layer, and for RES dsigma a W_v
+          as the trunk's sigma head.  A skinny library product for dv would give each row fp32 values that depend on the
+          chunk's row count, and the fp16 dA would round them differently from chunk layout to chunk layout.
 Gradients flow to the FiLM table (and through torch's autograd into the mapping network / latents /
 frequency offsets) and to every field parameter.  The fp16 gradient stream is scaled by a power of two
 taken from max|d raw| on the device (no host sync) and unscaled at the end.
@@ -256,7 +259,9 @@ class _FieldBackward:
             self.Wl16 = fw.label_film[0][0].detach().to(self.dt).contiguous()
             self.Wchain32.append(fw.label_film[0][0].detach().float())
             self.Wlhead32 = fw.labels[0][0].detach().float().contiguous()                 # (L, 256)
-        self.Wchain32 += [wc0[:, self.kx:]] + [w.detach().float() for w, _ in fw.color[1:]]
+        # a bridge field's first colour layer passes dU diag(f_b) W_c0[:, v] W_v (rank 3) to the trunk
+        wc0_chain = (self.Wc0eff[:, 3:6].double() @ self.Wv32.double()).float() if self.br else wc0[:, self.kx:]
+        self.Wchain32 += [wc0_chain] + [w.detach().float() for w, _ in fw.color[1:]]
         # ... scaled per image once for every chunk: diag(f_b) W, (B, n_film - 1, 256, 256); the NT kernel wants it transposed
         fW = self.film[:, 1:, 0].unsqueeze(3) * torch.stack(self.Wchain32[1:])
         self.fW = fW.transpose(2, 3).to(torch.float16).contiguous() if self.own_gemm else fW.to(self.dt)
@@ -270,8 +275,10 @@ class _FieldBackward:
         if L and not self.lf:      # (a label FiLM field's head acts on the label layer: its rows stay zero here)
             weff, _ = _label_eff(fw.labels)
             heads[:L] = weff
-        if fw.sigma is not None:       # (RES: the density comes from v; its gradient goes there)
+        if fw.sigma is not None:
             heads[L] = fw.sigma[0].detach().float().reshape(-1)
+        elif self.res:                 # sigma = a . v + c with v = W_v h + ...: the trunk's sigma head is a W_v
+            heads[L] = (self.dens_a.double() @ self.Wv32.double()).float()
         self.Wheads32 = heads
         rgbw = torch.zeros((self.n_rgb, 256), dtype=self.dt, device=dev)
         rgbw[:self.spec.rgb_dim] = fw.rgb[0].detach().to(self.dt)
@@ -397,7 +404,8 @@ class _FieldBackward:
                 idx = c0 + j
                 self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dU now
                 if self.br and j == 0:
-                    dA = self._bridge_back(dA, extras, v, A[T - 1], d_sigma, k, ppb, b0, b1)
+                    self._bridge_back(dA, extras, v, A[T - 1], d_sigma, k, ppb, b0, b1)
+                    dA = self._chain(dA, idx, b0, b1, ppb)
                     A[idx], Gt[idx] = None, None
                     break
                 a_in = A[idx - 1] if j else A[T - 1]
@@ -440,7 +448,8 @@ class _FieldBackward:
 
     def _bridge_back(self, dU, extras, v, a_trunk, d_sigma, k, ppb, b0, b1):
         """First colour layer of a bridge field on [dir, v]: its narrow weight gradient, dv = dU diag(f) W_c0[:, v]
-        (+ dsigma a for RES), v's own gradients, and the trunk's dA = dv W_v.  In fp32 (3 columns)."""
+        (+ dsigma a for RES) and v's own gradients, in fp32 (3 columns).  The trunk's share dv W_v goes through _chain
+        and the sigma head instead (see the module docstring)."""
         P = k * ppb
         du = dU.float().view(k, ppb, 256)
         e = torch.zeros((P, self.kx_pad), dtype=torch.float32, device=self.dev)
@@ -454,7 +463,6 @@ class _FieldBackward:
             self.d_c += d_sigma.sum()
         self.d_wv += dv.t() @ a_trunk.float()
         self.d_bv += dv.sum(0)
-        return (dv @ self.Wv32).to(self.dt)
 
     def _grid_grad(self, dU, points, k, ppb, b0, b1):
         """d features = dU diag(f_b) W_feat, (P, G), of the layer the grid feeds, scattered into the grid accumulator."""

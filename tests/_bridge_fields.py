@@ -16,7 +16,8 @@ def _film(layer, h, f, p):
 def restated(siren, pts, film, dirs, fault=None):
     """(B, P, 3) points, (B, L, 2, 256) FiLM table [f, p], (B, P, 3) directions -> (B, P, 4) [rgb, sigma].
     `fault` (the fault checks only): 'no_bridge_bias' drops v's bias, 'no_pos' leaves the position out of RES's v,
-    'swap' swaps the direction and v columns of the first colour layer's input."""
+    'swap' swaps the direction and v columns of the first colour layer's input, 'sigma_from_detached_v' computes RES's
+    density from v.detach() (its gradient then lacks d sigma . a)."""
     x = pts * siren.gridwarper.scale_factor
     h = x
     for i, layer in enumerate(siren.network):
@@ -26,7 +27,7 @@ def restated(siren, pts, film, dirs, fault=None):
     v = h @ lin.weight.t() + (0 if fault == "no_bridge_bias" else lin.bias)
     if res:
         v = v + (0 if fault == "no_pos" else x)
-        sigma = siren.density_layer_linear(v)
+        sigma = siren.density_layer_linear(v.detach() if fault == "sigma_from_detached_v" else v)
         c_in = siren.color_layer_pre(v)
     else:
         sigma = siren.final_layer(h)

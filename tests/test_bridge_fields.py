@@ -1,6 +1,7 @@
 """Bridge fields (SPATIALSIRENAUGDISENTANGLE, RESSIRENDISENTANGLE): the colour branch starts from a 3-wide v taken off the
-trunk output.  CPU: the mirror against the reference's init, the flag rules of the C-ABI, the restatement's faults.
-GPU: both point-network kernels, the density-only entry and the backward against a float64 restatement."""
+trunk output.  CPU: the mirror against the reference's init, the flag rules of the C-ABI, the restatement's faults and
+the faults the backward's bounds catch.  GPU: both point-network kernels under the tile schedules of a real SM count,
+the density-only entries, and the backward under the chunk layouts of production, against a float64 restatement."""
 import copy
 import ctypes
 import gzip
@@ -17,21 +18,24 @@ import torch.nn.functional as F
 import _bridge_fields as BF
 import _cases
 import _harness
-from _fp64 import _film
-from fenerf_b200 import _lib, ops, packing
+import test_gpu_fp64_film_edges as FE
+from _fp64 import _film, _siren, field_ref
+from fenerf_b200 import _lib, backward, ops, packing
 from fenerf_b200.siren import siren as S
+from oracle import render_oracle as oracle
+from test_gpu_fp64_reference import (FIELD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward, _field_points, _forward_inputs,
+                                     _grad_errors, _per_point)
 
 DEV = "cuda:0"
 GOLDEN = _cases.GOLDEN_DIR
-#: point network forward, max |out - fp64| over the rgb / the sigma channels, per model.  Measured on an H100 at up to
-#: 20,000 points per image: exact <= 6.1e-7 (rgb), 8.4e-7 (AUG sigma), 9.6e-6 (RES sigma, scaled chain); fast <= 3.4e-4
-#: (AUG), 1.5e-4 (RES rgb), 1.6e-8 (RES sigma at the reference init, where |a| ~ 1e-6) and 3.6e-3 (RES sigma with the
-#: chain scaled so that a . v is O(1): v's error from the fp16 trunk, times |a| = 1)
+#: point network forward, max |out - fp64| over the rgb / the sigma channels, per model.  Measured on an H100 80GB HBM3
+#: (132 SMs, 400 W power limit) at up to 20,000 points per image and under the four tile schedules (up to 33,691 points
+#: per image): exact <= 1.1e-6 (rgb, AUG at 4sms_minus_1), 8.4e-7 (AUG sigma), 9.7e-6 (RES sigma, scaled chain); fast
+#: <= 3.6e-4 (AUG), 2.0e-4 (RES rgb), 1.6e-8 (RES sigma at the reference init, where |a| ~ 1e-6) and 3.6e-3 (RES sigma
+#: with the chain scaled so that a . v is O(1): v's error from the fp16 trunk, times |a| = 1)
 FWD_BOUND = {"exact": 1e-5, "fast": 5e-3}
 FAST_BOUND = {"aug": (6e-4, 6e-4), "res": (3e-4, 1e-6), "res_scaled": (3e-4, 5e-3)}
 EXACT_BOUND = {"aug": (2e-6, 2e-6), "res": (2e-6, 1e-7), "res_scaled": (2e-6, 2e-5)}
-#: gradients, max |g - fp64| relative to each tensor's largest entry: fp32 streams / fp16 streams
-GRAD_BOUND = {"exact": 5e-4, "default": 2e-2}
 
 
 def _mirror(name, seed=0):
@@ -133,6 +137,53 @@ def test_restatement_runs_the_mirror_forward():
         assert missing == [], missing
 
 
+def _c0_freqs_of_image0(field, points, film, dirs):
+    """The restatement with image 0's frequencies of the first colour row used for every image (a wrong b0 in dv)."""
+    c0 = len(field.network)
+    f = film.clone()
+    f[1:, c0, 0] = film[0, c0, 0]
+    return BF.field_eval(field, points, f, dirs)
+
+
+def _sigma_from_detached_v(field, points, film, dirs):
+    return BF.restated(field, points, film, dirs, fault="sigma_from_detached_v")
+
+
+_BWD_FAULTS = [("aug", "c0_freqs_of_image0"), ("res_scaled", "c0_freqs_of_image0"), ("res_scaled", "sigma_from_detached_v"),
+               ("aug", "dirs_one_ray_off"), ("res_scaled", "dirs_one_ray_off")]
+
+
+@pytest.mark.parametrize("model,fault", _BWD_FAULTS, ids=["%s-%s" % f for f in _BWD_FAULTS])
+def test_backward_faults_exceed_the_bounds(monkeypatch, model, fault):
+    """Faults of the bridge's backward, each applied to the float64 restatement: image 0's colour-row-c0 frequencies
+    used in every image's dv, RES's density from v.detach() (dv without d sigma . a, on the scaled chain where sigma
+    depends on v), and directions sliced one ray off in image 1's second point chunk.  The first two must move some
+    gradient past 10x the default-mode bound; the direction fault past 10x the layout-invariance bound, the check that
+    sees it in default mode, and past the exact-mode bound."""
+    siren = _bridge_siren(model, "cpu")
+    batch, ppb, dir_group = 2, 480, 24
+    pts, dirs = _field_points(batch, ppb, dir_group, 13)
+    film = _film(siren, batch, 13, edges=True)
+    d_raw = torch.randn(batch, ppb, 4, generator=torch.Generator().manual_seed(13)) * 1e-3
+    monkeypatch.setattr(oracle, "field_eval", BF.field_eval)
+    _, film_g, good = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    if fault == "dirs_one_ray_off":
+        shifted = dirs.clone()
+        half = dirs.shape[1] // 2
+        shifted[1, half:-1] = dirs[1, half + 1:]
+        _, film_b, bad = field_ref(siren, monkeypatch, pts, _per_point(shifted, ppb, False), film, d_raw)
+    else:
+        monkeypatch.setattr(oracle, "field_eval", _c0_freqs_of_image0 if fault == "c0_freqs_of_image0" else _sigma_from_detached_v)
+        _, film_b, bad = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    errs = _grad_errors(film_b, bad, film_g, good)
+    worst = max(errs, key=errs.get)
+    print("bridge backward fault %s %s: %s moves %.3g" % (model, fault, worst, errs[worst]))
+    if fault == "dirs_one_ray_off":
+        assert errs[worst] > 10 * LAYOUT_BOUND and errs[worst] > FIELD_BOUND["exact"], errs[worst]
+    else:
+        assert errs[worst] > 10 * FIELD_BOUND["default"], errs[worst]
+
+
 # --------------------------------------------------------------------------------------------
 # GPU: the kernels against the float64 restatement
 # --------------------------------------------------------------------------------------------
@@ -153,7 +204,6 @@ def _gpu_inputs(name, scaled, batch, ppb, seed=7):
 
 
 def _want(siren, film, pts, dirs):
-    import copy
     s64 = copy.deepcopy(siren).double()
     with torch.no_grad():
         return BF.restated(s64, pts.double(), film.double(), dirs.double())
@@ -161,68 +211,104 @@ def _want(siren, film, pts, dirs):
 
 @pytest.mark.gpu
 @torch.no_grad()
-@pytest.mark.parametrize("ppb", [64, 64 * 37 + 5, 20000])          # one tile, an odd count and a ragged last tile
+@pytest.mark.parametrize("shape", [64, 64 * 37 + 5, 20000] + list(_cases.TILE_LAYOUTS))
 @pytest.mark.parametrize("model", MODELS, ids=_IDS)
 @pytest.mark.parametrize("precision", ["exact", "fast"])
-def test_points_match_float64(model, precision, ppb):
-    siren, film, pts, dirs = _gpu_inputs(*model, batch=2, ppb=ppb)
-    want = _want(siren, film, pts, dirs)
-    out = ops.siren_points(siren, pts, film, dirs, precision=precision, dir_group=1)
+def test_points_match_float64(model, precision, shape):
+    """The point network against the float64 restatement per channel, within the model's own bound.  An int shape is
+    points per image with one direction per point (one tile, an odd count, a ragged last tile); a tile layout is one
+    of the schedules derived from the device's SM count, with its direction mode (test_gpu_fp64_reference._FWD_DIRS:
+    per point, one per 24-sample ray, one per image).  A second launch is bit-identical, and the density-only entries
+    (ops.siren_sigma, siren.density) equal the sigma channel bit for bit -- for RES, the density rebuilt from v."""
+    if isinstance(shape, int):
+        siren, film, pts, dirs = _gpu_inputs(*model, batch=2, ppb=shape)
+        dir_group = 1
+    else:
+        siren = _gpu_inputs(*model, batch=1, ppb=64)[0]
+        pts, dirs, film = _forward_inputs(siren, shape, 2400 + MODELS.index(model))
+        dir_group = None
+    want = _want(siren, film, pts, _per_point(dirs, pts.shape[1], False))
+    out = ops.siren_points(siren, pts, film, dirs, precision=precision, dir_group=dir_group)
+    again = ops.siren_points(siren, pts, film, dirs, precision=precision, dir_group=dir_group)
+    sigma = ops.siren_sigma(siren, pts, film, precision=precision)
+    density = siren.density(pts, film, precision=precision)
     torch.cuda.synchronize()
     err = (out.double() - want).abs().amax(dim=(0, 1))
-    print("%s %s ppb %d: max|out - fp64| per channel %s" % (model, precision, ppb, err.tolist()))
+    print("forward %s %s %s (B=%d, ppb %d): max|out - fp64| per channel %s" % (
+        _IDS[MODELS.index(model)], precision, shape, pts.shape[0], pts.shape[1], err.tolist()))
     rgb_bound, sigma_bound = (EXACT_BOUND if precision == "exact" else FAST_BOUND)[_IDS[MODELS.index(model)]]
-    assert err[:3].max() <= rgb_bound and err[3] <= sigma_bound
-    again = ops.siren_points(siren, pts, film, dirs, precision=precision, dir_group=1)
+    assert torch.isfinite(out).all()
+    assert err[:3].max() <= rgb_bound and err[3] <= sigma_bound, err.tolist()
     assert torch.equal(out, again)
+    assert torch.equal(sigma, out[..., -1:]) and torch.equal(density, out[..., -1:])
+
+
+#: backward cases: (layout of test_gpu_fp64_reference._LAYOUTS, model, lock_dirs, planted edge frequencies).  L2 with
+#: planted frequencies on res_scaled: the reference init leaves RES's |a| ~ 1e-6, so only the scaled chain puts the
+#: planted colour-row-c0 columns' dv next to a dsigma a of the same size.  The shared bounds hold for every tensor,
+#: color_layer_pre and the density chain included.  Measured on an H100 80GB HBM3 (400 W power limit): exact <= 1.8e-5
+#: (L4 aug, a FiLM frequency gradient; color_layer_pre <= 1.0e-5, the density chain <= 4.5e-6), default <= 1.24e-2
+#: (L1 aug; color_layer_pre <= 9.4e-3); planted columns 5.0e-6 / 4.4e-3; chunked against one chunk 1.3e-5 (exact) and
+#: 7.8e-6 (default; 2.8e-4 while dv W_v reached the trunk from a skinny library product, see fenerf_b200/backward.py).
+_BWD = ([(lay, m, False, False) for lay in ("L1", "L2", "L3") for m in _IDS]
+        + [("L1", m, True, False) for m in _IDS]
+        + [("L4", m, False, False) for m in ("aug", "res_scaled")]
+        + [("L2", "res_scaled", False, True)])
+
+
+def _bridge_siren(model_id, device):
+    """The generator's field (the seed protocol of _fp64._siren); res_scaled with the density chain scaled."""
+    name, scaled = MODELS[_IDS.index(model_id)]
+    siren = _siren("M" if name == BF.CLASSES[0] else "N", device)
+    return BF.scale_density(siren) if scaled else siren
 
 
 @pytest.mark.gpu
-@torch.no_grad()
-@pytest.mark.parametrize("model", MODELS, ids=_IDS)
-@pytest.mark.parametrize("precision", ["exact", "fast"])
-def test_density_only_is_the_full_evaluations_sigma(model, precision):
-    siren, film, pts, dirs = _gpu_inputs(*model, batch=2, ppb=64 * 37 + 5)
-    full = ops.siren_points(siren, pts, film, dirs, precision=precision, dir_group=1)
-    sigma = siren.density(pts, film, precision=precision)
-    torch.cuda.synchronize()
-    print("%s %s: max|density - full sigma| %g" % (model, precision, (sigma[..., 0] - full[..., -1]).abs().max().item()))
-    assert torch.equal(sigma[..., 0], full[..., -1])
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("model", MODELS, ids=_IDS)
+@pytest.mark.parametrize("layout,model,lock,edges", _BWD,
+                         ids=["%s-%s%s%s" % (lay, m, "-lock_dirs" if k else "", "-edges" if e else "") for lay, m, k, e in _BWD])
 @pytest.mark.parametrize("precision", ["exact", "default"])
-def test_backward_matches_float64_autograd(model, precision):
-    from fenerf_b200 import backward
-    import copy
-    batch, ppb = 2, 3000
-    siren, film, pts, dirs = _gpu_inputs(*model, batch=batch, ppb=ppb)
-    with torch.no_grad():
-        raw = ops.siren_points(siren, pts, film, dirs, precision="exact" if precision == "exact" else "fast", dir_group=1)
-    g = torch.Generator().manual_seed(3)
-    d_raw = (torch.randn(raw.shape, generator=g) * 1e-3).to(DEV)
-    with torch.no_grad():
-        m = d_raw.abs().max()
-        scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)
-        fb = backward._FieldBackward(siren, film, scale, (1.0 / scale).float().reshape(1), exact=precision == "exact")
-        fb.add_points(pts, dirs, 1, False, raw, d_raw)
-        d_film, grads = fb.finish()
-    s64 = copy.deepcopy(siren).double()
-    f64 = film.double().requires_grad_(True)
-    out = BF.restated(s64, pts.double(), f64, dirs.double())
-    (out * d_raw.double()).sum().backward()
-    params = dict(siren.named_parameters())
-    worst = {}
-    for n, p in s64.named_parameters():
-        if "mapping" in n:
-            continue
-        got = grads[id(params[n])].reshape(p.shape).double()
-        ref = p.grad
-        worst[n] = ((got - ref).abs().max() / ref.abs().max().clamp_min(1e-30)).item()
-    worst["film"] = ((d_film.double() - f64.grad).abs().max() / f64.grad.abs().max()).item()
-    print("%s %s: worst relative gradient error %s" % (model, precision, max(worst.items(), key=lambda kv: kv[1])))
-    assert max(worst.values()) <= GRAD_BOUND[precision], worst
+def test_backward_matches_float64_autograd(monkeypatch, layout, model, lock, edges, precision):
+    """``_FieldBackward`` against the float64 VJP of the restatement under the production chunk layouts: every parameter
+    gradient (RES's color_layer_pre and density chain unfolded in finish()) and d film, per tensor and per FiLM layer.
+    L2 has chunks whose image b0 > 0 reads its own colour-row-c0 frequencies in dv; L3 splits each image into point
+    chunks (directions sliced at p0 // dir_group, d a / d c summed over every chunk); L4 is cfg2's pass.  L2 / L3 also
+    run as one chunk, within LAYOUT_BOUND.  With `edges`, f = 0, tiny and large |f| are planted in every FiLM role, and
+    each planted column is checked on its own."""
+    batch, ppb, dir_group, chunk = _LAYOUTS[layout]
+    exact = precision == "exact"
+    if exact:
+        monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)     # exact mode's torch.mm stays fp32
+    monkeypatch.setattr(oracle, "field_eval", BF.field_eval)
+    siren = _bridge_siren(model, DEV)
+    seed = 5000 + 10 * _IDS.index(model) + int(layout[1])
+    pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
+    film, planted = FE._edge_film(siren, batch, seed, FE.BACKWARD_FREQS) if edges else (_film(siren, batch, seed, edges=True), [])
+    d_raw = torch.randn(batch, ppb, 4, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
+    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, lock), film, d_raw)
+    raw = out64.float().contiguous()
+    if chunk:
+        monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
+    d_film, grads = _field_backward(siren, film, pts, dirs, dir_group, lock, raw, d_raw, exact)
+    assert torch.isfinite(d_film).all() and all(torch.isfinite(g).all() for g in grads.values())
+    errs = _grad_errors(d_film, grads, want_film, want)
+    bound = FIELD_BOUND[precision]
+    worst = max(errs, key=errs.get)
+    bridge = {k: "%.2e" % v for k, v in errs.items() if k.split(".")[0] in ("color_layer_pre", "density_layer_linear",
+                                                                           "res_coord_layer", "final_layer")}
+    print("bridge field %s %s %s: worst %s %.3g; bridge tensors %s" % (layout, model, precision, worst, errs[worst], bridge))
+    assert errs[worst] <= bound, {k: "%.2e" % v for k, v in errs.items() if v > bound}
+    if edges:
+        cols = FE._planted_errors(d_film, grads, want_film, want, planted, FE._layer_weights(siren))
+        worst_col = max(cols, key=cols.get)
+        print("bridge edge columns %s %s %s: worst %s %.3g" % (layout, model, precision, worst_col, cols[worst_col]))
+        assert cols[worst_col] <= FIELD_BOUND[precision], {k: "%.2e" % v for k, v in cols.items() if v > FIELD_BOUND[precision]}
+    if chunk:
+        monkeypatch.setattr(backward, "CHUNK_POINTS", 1 << 30)
+        d_film1, grads1 = _field_backward(siren, film, pts, dirs, dir_group, lock, raw, d_raw, exact)
+        inv = _grad_errors(d_film, grads, d_film1, grads1)
+        worst = max(inv, key=inv.get)
+        print("bridge layout %s %s %s: worst %s %.3g" % (layout, model, precision, worst, inv[worst]))
+        assert inv[worst] <= LAYOUT_BOUND, {k: "%.2e" % v for k, v in inv.items() if v > LAYOUT_BOUND}
 
 
 @pytest.mark.gpu
