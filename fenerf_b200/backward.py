@@ -27,7 +27,10 @@ backward  ``fenerf_composite_backward`` (d pixels -> d raw outputs, one warp per
           from [dir, v] like a first layer; dv = dU diag(f) W_c0[:, v] (+ dsigma a for RES) joins the trunk as dv W_v:
           dU diag(f_b) (W_c0[:, v] W_v) through the same per-image product as every other layer, and for RES dsigma a W_v
           as the trunk's sigma head.  A skinny library product for dv would give each row fp32 values that depend on the
-          chunk's row count, and the fp16 dA would round them differently from chunk layout to chunk layout.
+          chunk's row count, and the fp16 dA would round them differently from chunk layout to chunk layout.  The
+          direction-free field (TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96) runs as a grid field whose
+          first colour layer has zero direction columns (finish() drops them from its weight gradient), in the exact
+          mode only: that layer's U(+-1/3) weights at f ~ 30 amplify the fp16 streams' error past any useful bound.
 Gradients flow to the FiLM table (and through torch's autograd into the mapping network / latents /
 frequency offsets) and to every field parameter.  The fp16 gradient stream is scaled by a power of two
 taken from max|d raw| on the device (no host sync) and unscaled at the end.
@@ -66,6 +69,17 @@ def _mm32(a, b):
     if a.dtype == torch.float32:
         return torch.mm(a, b)
     return torch.mm(a, b, out_dtype=torch.float32)
+
+
+class _NoTF32:
+    """Keeps torch's fp32 products fp32 (no TF32) inside the block, whatever the caller's matmul switch says."""
+
+    def __enter__(self):
+        self.prev = torch.backends.cuda.matmul.allow_tf32
+        torch.backends.cuda.matmul.allow_tf32 = False
+
+    def __exit__(self, *exc):
+        torch.backends.cuda.matmul.allow_tf32 = self.prev
 
 
 def _bmm32(a, b):
@@ -228,6 +242,14 @@ class _FieldBackward:
         self.own_gemm = (not exact) and BWD_GEMM == "wgmma"
         self.Wh16 = [None] + [w.detach().to(self.dt).contiguous() for w, _ in fw.trunk[1:]]
         wc0 = fw.color[0][0].detach().float()
+        # a direction-free field's first colour layer reads [feat, x]: zero direction columns give it the [dir, feat, x]
+        # order of the other grid fields (finish() drops them again)
+        self.wd = self.spec.wo_dir
+        if self.wd and not exact:
+            raise RuntimeError("the direction-free field (FENERF_FIELD_WO_DIR) renders and differentiates in "
+                               "precision='exact' only: its first colour layer amplifies the fp16 streams' error")
+        if self.wd:
+            wc0 = torch.cat([torch.zeros((256, 3), dtype=torch.float32, device=dev), wc0], dim=1)
         self.bias = [b.detach().float().contiguous() for _, b in fw.film_layers()]
         if self.br:
             # the first colour layer on [dir, v]; RES: color_layer_pre folded into its v columns and bias (fp64)
@@ -286,6 +308,12 @@ class _FieldBackward:
 
     # ---- one point set: points (B, ppb, 3), dirs (B, ppb/dir_group, 3), raw / d_raw (B, ppb, C) ----
     def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
+        if self.wd:     # the direction-free field: TF32 rounding would be amplified like fp16's (see __init__)
+            with _NoTF32():
+                return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw)
+        return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw)
+
+    def _add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
         B, ppb, _ = points.shape
         if ppb <= CHUNK_POINTS:
             k = max(1, CHUNK_POINTS // ppb)
@@ -474,6 +502,12 @@ class _FieldBackward:
 
     # ---- after every point set: fold the per-image accumulators into parameter / FiLM gradients ----
     def finish(self):
+        if self.wd:
+            with _NoTF32():
+                return self._finish()
+        return self._finish()
+
+    def _finish(self):
         fw, inv = self.fw, self.inv_scale
         film = self.film
         d_film = torch.zeros_like(film)
@@ -490,12 +524,16 @@ class _FieldBackward:
                 w32 = self.Wc0eff                                               # (RES: color_layer_pre folded in)
             elif idx == self.c0:
                 m = torch.cat([self.dWx_b[:, :, :self.kx], self.dW_b[idx]], dim=2)   # column order of the reference: [dir, feat, x]
+                if self.wd:
+                    w32 = torch.cat([torch.zeros_like(w32[:, :3]), w32], dim=1)    # [feat, x] with zero direction columns
             else:
                 m = self.dW_b[idx]                                          # M_b = dU_b^T a
             df = torch.einsum('fk,bfk->bf', w32, m) + self.bias[idx].unsqueeze(0) * dp
             d_film[:, idx, 0] = df * inv
             d_film[:, idx, 1] = dp * inv
             grads[id(w)] = torch.einsum('bf,bfk->fk', f, m) * inv
+            if self.wd and idx == self.c0:
+                grads[id(w)] = grads[id(w)][:, 3:].contiguous()               # the reference's [feat, x]
             grads[id(b)] = (f * dp).sum(0) * inv
         L = self.L
         if fw.sigma is not None:

@@ -80,6 +80,11 @@ int make_layout(const fenerf_field_desc* field, FnLayout* L) {
         return fail(FENERF_E_UNSUPPORTED, "unknown field flag combination 0x%x for this field: FENERF_FIELD_BRIDGE only with "
                     "label_dim 0, no grid and no other flag than FENERF_FIELD_BRIDGE_RES, which needs it (label_dim %d, "
                     "grid %d)", (unsigned)field->reserved, field->label_dim, field->grid_channels);
+    if (r == -6)
+        return fail(FENERF_E_UNSUPPORTED, "unknown field flag combination 0x%x for this field: FENERF_FIELD_WO_DIR only with "
+                    "8 trunk and 8 colour layers, grid_channels 32, label_dim >= 1 and no other flag (trunk %d, colour %d, "
+                    "label_dim %d, grid %d)", (unsigned)field->reserved, field->trunk_layers, field->color_layers,
+                    field->label_dim, field->grid_channels);
     FN_REQUIRE(r == 0, "unsupported field description");
     return 0;
 }

@@ -52,6 +52,9 @@
 //                    position, sigma = a . v + c (a, c: the density chain folded in double, after the bias at bridge_w;
 //                    the trunk head's sigma row is zero), and the first colour layer's v columns and bias are
 //                    W_c0[:, 3:] W_pre and b_c0 + W_c0[:, 3:] b_pre, folded in double as well.
+//   no direction     (FENERF_FIELD_WO_DIR) the first colour layer reads [feat, x]; it is packed in the plain layout
+//                    (kx = 3 + G) with zero direction rows and zero direction slots, so every kernel runs it as a plain
+//                    grid field and no output depends on the direction.
 //
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
@@ -109,18 +112,25 @@ struct FnLayout {
     int32_t bridge;         // the variant flag FENERF_FIELD_BRIDGE: the colour branch reads [dir, v], v off the trunk
     int32_t bridge_res;     // FENERF_FIELD_BRIDGE_RES: v adds the position, the density is a . v + c
     size_t bridge_w;        // bridge: [3][256] f32 weights of v, b[3], then a[3], c (RES; 0 otherwise)
+    int32_t wo_dir;         // the variant flag FENERF_FIELD_WO_DIR: the first colour layer reads [feat, x] (zero direction rows)
 };
 
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head, -4 for the grid in
-// the trunk or -5 for a bridge on a field shape no reference class has, or -1 if the description is outside what the
-// kernels support.
+// the trunk, -5 for a bridge or -6 for a direction-free colour branch on a field shape no reference class has, or -1 if
+// the description is outside what the kernels support.
 static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     if (!f || !L) return -1;
     if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD | FENERF_FIELD_GRID_TRUNK | FENERF_FIELD_BRIDGE |
-                        FENERF_FIELD_BRIDGE_RES))
+                        FENERF_FIELD_BRIDGE_RES | FENERF_FIELD_WO_DIR))
         return -2;
+    const int wo_dir = (f->reserved & FENERF_FIELD_WO_DIR) ? 1 : 0;
+    // TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96: 8 + 8 layers, a 32-channel grid, the label chain, no other
+    // flag
+    if (wo_dir && (f->reserved != FENERF_FIELD_WO_DIR || f->grid_channels != 32 || f->label_dim < 1 || f->trunk_layers != 8 ||
+                   f->color_layers != 8))
+        return -6;
     const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
     const int feature_head = (f->reserved & FENERF_FIELD_FEATURE_HEAD) ? 1 : 0;
     const int grid_trunk = (f->reserved & FENERF_FIELD_GRID_TRUNK) ? 1 : 0;
@@ -197,6 +207,7 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     }
     L->first_img_lo = grid_trunk ? take(FN_IMG_BYTES) : 0;
     L->bridge_w = bridge ? take((3 * FN_H + 3 + 3 + 1) * 4) : 0;
+    L->wo_dir = wo_dir;
     L->total = off;
     return 0;
 }

@@ -88,6 +88,33 @@ __global__ void pack_color0_ximg_kernel(const float* __restrict__ w, int in_dim,
         *reinterpret_cast<__half*>(img + fn_sw128_offset(n, FN_SLOT_FEAT + c)) = __float2half_rn(w[(size_t)n * in_dim + 3 + c]);
 }
 
+// ---- the first colour layer of a direction-free field (FENERF_FIELD_WO_DIR), one block per output n ----------------
+// w is [256][g + 256] in the reference's column order [feat, x].  Packed as a plain grid field's [dir, feat, x] with zero
+// direction columns: the fp32 copy (rows x, then dir = 0, feat, zero pad to kx_pad), the 256-wide f16 image of x, and
+// the input-chunk image with the features in slots 32.. and nothing in the direction slots (layout.h)
+__global__ void pack_wo_dir_color0_kernel(const float* __restrict__ w, int g, int kx_pad, const float* __restrict__ b,
+                                          float* __restrict__ wt, float* __restrict__ bo, unsigned char* __restrict__ img,
+                                          unsigned char* __restrict__ ximg) {
+    const int n = blockIdx.x;
+    const size_t in_dim = (size_t)g + FN_H;
+    for (int k = threadIdx.x; k < FN_H + kx_pad; k += blockDim.x) {
+        float v = 0.f;
+        if (k < FN_H) {
+            v = w[n * in_dim + g + k];
+            *reinterpret_cast<__half*>(img + fn_hidden_img_offset(n, k)) = __float2half_rn(v);
+        } else if (k - FN_H >= 3 && k - FN_H < 3 + g) {
+            v = w[n * in_dim + (k - FN_H - 3)];
+        }
+        wt[(size_t)k * FN_H + n] = v;
+    }
+    for (int k = threadIdx.x; k < FN_KCHUNK; k += blockDim.x) {
+        const int c = k - FN_SLOT_FEAT;
+        const float v = c >= 0 && c < g ? w[n * in_dim + c] : 0.f;
+        *reinterpret_cast<__half*>(ximg + fn_sw128_offset(n, k)) = __float2half_rn(v);
+    }
+    if (threadIdx.x == 0) bo[n] = b[n];
+}
+
 // ---- label chain: Weff = W3 W2 W1, beff = W3 (W2 b1 + b2) + b3, in double ---------------------
 // step 1: U = W3 W2 (L x 256), ub = W3 b2 + b3          grid L blocks x 256 threads
 __global__ void label_step1_kernel(const float* __restrict__ w3, const float* __restrict__ b3,
@@ -285,7 +312,8 @@ __global__ void pack_grid_kernel(const float* __restrict__ in, float* __restrict
 
 // ---- fingerprint of the raw parameters (EMA copy_to / restore write through .data without bumping
 // torch's version counter, so the host cannot see that the packed copy went stale) ------------------
-// (40 segments hold every field but the bridge fields, whose extra Linears take a wider instantiation)
+// (40 segments hold every field but the bridge fields, whose extra Linears take a wider instantiation, and the
+// direction-free field, whose eight colour layers do)
 template <int N>
 struct FpSegments {
     const float* ptr[N];
@@ -335,7 +363,8 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
     for (int i = 0; i < n_trunk; ++i) { add(p->trunk_w[i], (i == 0 ? L.first_k : FN_H) * FN_H); add(p->trunk_b[i], FN_H); }
     if (!L.bridge_res) { add(p->sigma_w, FN_H); add(p->sigma_b, 1); }
     // (a bridge field's first colour layer: [dir, v], or [dir, x] before color_layer_pre with the density chain)
-    const unsigned long long c0_in = L.bridge ? (L.bridge_res ? 3 + FN_H : 6) : L.kx + FN_H;
+    // (a direction-free field's: [feat, x])
+    const unsigned long long c0_in = L.bridge ? (L.bridge_res ? 3 + FN_H : 6) : L.wo_dir ? L.grid_channels + FN_H : L.kx + FN_H;
     for (int i = 0; i < n_color; ++i) { add(p->color_w[i], (i == 0 ? c0_in : FN_H) * FN_H); add(p->color_b[i], FN_H); }
     add(p->rgb_w, (unsigned long long)L.rgb.n_out * FN_H); add(p->rgb_b, L.rgb.n_out);
     if (L.label_dim > 0) {
@@ -351,7 +380,7 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
     }
     if (L.grid_channels > 0) add(p->grid, (unsigned long long)L.grid_channels * L.grid_res * L.grid_res * L.grid_res);
     FN_CUDA_OK(cudaMemsetAsync(out, 0, 16, st));
-    if (seg.n <= 40) {      // every field but the bridge fields: the instantiation it always had
+    if (seg.n <= 40) {      // every field but the bridge and direction-free fields: the instantiation it always had
         FpSegments<40> s40;
         s40.n = seg.n;
         for (int i = 0; i < seg.n; ++i) { s40.ptr[i] = seg.ptr[i]; s40.count[i] = seg.count[i]; }
@@ -388,6 +417,13 @@ int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, 
                                                          (float*)(packed + L.hid_w32[l]), (float*)(packed + L.hid_b[l]),
                                                          packed + L.color0_ximg);
             FN_LAUNCH_OK("pack_bridge_color0_kernel");
+            continue;
+        }
+        if (L.wo_dir && is_c0) {     // [feat, x] as [dir = 0, feat, x] (layout.h)
+            pack_wo_dir_color0_kernel<<<FN_H, 256, 0, st>>>(w, L.grid_channels, L.kx_pad, b, (float*)(packed + L.hid_w32[l]),
+                                                            (float*)(packed + L.hid_b[l]), packed + L.hid_img[l],
+                                                            packed + L.color0_ximg);
+            FN_LAUNCH_OK("pack_wo_dir_color0_kernel");
             continue;
         }
         int in_dim = is_c0 ? L.kx + FN_H : FN_H;

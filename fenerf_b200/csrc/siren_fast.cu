@@ -77,6 +77,12 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     FN_REQUIRE(L.rgb.img < 0xFFFFFFFFull && L.label.img < 0xFFFFFFFFull && L.first_img_lo < 0xFFFFFFFFull,
                "packed weight images beyond 4 GB");
     FN_REQUIRE(((uintptr_t)film & 15) == 0, "the FiLM table must be 16-byte aligned");
+    // a direction-free field's first colour layer (U(+-1/3) weights, f ~ 30) amplifies the fp16 trunk's error to ~2e-2 in
+    // rgb (DESIGN section 5): its colours come from the exact kernel only; its density alone is a plain trunk's
+    if (L.wo_dir && !sigma_only)
+        return fail(FENERF_E_UNSUPPORTED, "FENERF_FIELD_WO_DIR: the wgmma colour branch is not accurate for this field (its "
+                    "first colour layer amplifies the fp16 trunk's error to ~2e-2 in rgb); render it with "
+                    "FENERF_PRECISION_EXACT (the density alone runs in any precision)");
     FastArgs a;
     memset(&a, 0, sizeof(a));
     FN_REQUIRE(build_loads(L, a, sigma_only != 0), "field too deep for the weight stream");

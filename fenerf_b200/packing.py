@@ -42,7 +42,8 @@ def field_desc(spec) -> "_lib.FieldDesc":
                           | (_lib.FIELD_FEATURE_HEAD if spec.feature_head else 0)
                           | (_lib.FIELD_GRID_TRUNK if spec.grid_trunk else 0)
                           | (_lib.FIELD_BRIDGE if spec.bridge else 0)
-                          | (_lib.FIELD_BRIDGE_RES if spec.bridge_res else 0))
+                          | (_lib.FIELD_BRIDGE_RES if spec.bridge_res else 0)
+                          | (_lib.FIELD_WO_DIR if spec.wo_dir else 0))
 
 
 def _f32(t, device):

@@ -26,6 +26,7 @@ Reference interfaces mirrored (file:line in the reference tree):
   SIRENBASELINESEMANTICDISENTANGLE            siren/siren.py:1163-1229
   TextureEmbeddingPiGAN128SEMANTICDISENTANGLE siren/siren.py:1451-1530
   ...256SEMANTICDISENTANGLE / ..._DIM_96      siren/siren.py:1533-1546
+  TextureEmbeddingPiGAN128SEMANTICDISENTANGLE_WO_DIR / ...256..._WO_DIR_DIM_96   siren/siren.py:1549-1640, 1817-1822
 """
 import math
 from dataclasses import dataclass
@@ -160,6 +161,9 @@ class FieldSpec:
                    activations (siren/siren.py:965-967)
     bridge_res     with bridge: v = warped position + Linear(256 -> 3)(trunk output), the density is a chain of four
                    Linears on v and the first colour layer reads cat[ray_dir, Linear(3 -> 256)(v)] (siren/siren.py:1072-1076)
+    wo_dir         the first colour layer reads cat[grid_feat, trunk_out(256)], no ray direction, and carries the U(+-1/3)
+                   init (siren/siren.py:1606, 1626), which amplifies the fp16 trunk's error: the colours come from the exact
+                   kernel only (the density alone runs in any precision)
     out_dim        label_dim + 3 (rgb; 64 features with feature_head) + 1 (sigma); channel order [labels, rgb, sigma]
     """
     trunk_layers: int
@@ -175,6 +179,7 @@ class FieldSpec:
     grid_trunk: bool = False
     bridge: bool = False
     bridge_res: bool = False
+    wo_dir: bool = False
 
     @property
     def rgb_dim(self):
@@ -802,3 +807,57 @@ class RESSIRENDISENTANGLE(_DoubleLatentField):
         return FieldSpec(trunk_layers=len(self.network), color_layers=len(self.color_layer_sine), label_dim=0,
                          grid_channels=0, grid_res=0, input_scale=float(self.gridwarper.scale_factor), out_dim=4,
                          double_latent=True, bridge=True, bridge_res=True)
+
+
+class TextureEmbeddingPiGAN128SEMANTICDISENTANGLE_WO_DIR(_DoubleLatentField):
+    """The direction-free sibling of model B (siren/siren.py:1549-1640): the same trunk, 32 x 96^3 grid and label chain,
+    but EIGHT colour FiLM layers, the first on cat[feat(32), x] with no ray direction and the U(+-1/3)
+    ``modified_first_sine_init`` (:1606).  FiLM rows: trunk 0..7, colour 8..15; output [labels, rgb, sigma].  The 128-wide
+    class is here for name resolution, init and pickling: the kernels take hidden_dim=256 only."""
+
+    def __init__(self, input_dim=2, z_geo_dim=100, z_app_dim=100, hidden_dim=128, output_dim=1, device=None):
+        super().__init__()
+        self.device = device
+        self.input_dim = input_dim
+        self.z_geo_dim = z_geo_dim
+        self.z_app_dim = z_app_dim
+        self.hidden_dim = hidden_dim
+        self.output_dim = output_dim
+
+        widths = [3] + [hidden_dim] * 8
+        self.network = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(widths[:-1], widths[1:]))
+        self.final_layer = nn.Linear(hidden_dim, 1)
+        cwidths = [hidden_dim + 32] + [hidden_dim] * 8
+        self.color_layer_sine = nn.ModuleList(FiLMLayer(a, b) for a, b in zip(cwidths[:-1], cwidths[1:]))
+        self.color_layer_linear = nn.Sequential(nn.Linear(hidden_dim, 3))
+        self.geo_mapping_network = CustomMappingNetwork(z_geo_dim, 256, len(self.network) * hidden_dim * 2)
+        self.app_mapping_network = CustomMappingNetwork(z_app_dim, 256, len(self.color_layer_sine) * hidden_dim * 2)
+        self.label_layer_linear = nn.Sequential(
+            nn.Linear(hidden_dim, hidden_dim), nn.Linear(hidden_dim, hidden_dim),
+            nn.Linear(hidden_dim, self.output_dim - 4))
+
+        for part in (self.network, self.final_layer, self.color_layer_sine, self.color_layer_linear,
+                     self.label_layer_linear):
+            part.apply(frequency_init(25))
+        self.network[0].apply(modified_first_sine_init)
+        self.color_layer_sine[0].apply(modified_first_sine_init)     # U(+-1/3) over all 32 + hidden_dim columns
+
+        self.spatial_embeddings = nn.Parameter(torch.randn(1, 32, 96, 96, 96) * 0.01)
+        self.gridwarper = UniformBoxWarp(0.24)
+
+    def field_spec(self):
+        g = self.spatial_embeddings
+        assert g.shape[2] == g.shape[3] == g.shape[4], "cubic feature grid expected"
+        return FieldSpec(trunk_layers=len(self.network), color_layers=len(self.color_layer_sine),
+                         label_dim=self.output_dim - 4, grid_channels=g.shape[1], grid_res=g.shape[2],
+                         input_scale=float(self.gridwarper.scale_factor), out_dim=self.output_dim,
+                         double_latent=True, wo_dir=True)
+
+
+class TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96(TextureEmbeddingPiGAN128SEMANTICDISENTANGLE_WO_DIR):
+    """The 256-wide production form (siren/siren.py:1817-1822): hidden 256, its own 32 x 96^3 grid (scaled by 0.1) drawn
+    after the base class's (scaled by 0.01)."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs, hidden_dim=256)
+        self.spatial_embeddings = nn.Parameter(torch.randn(1, 32, 96, 96, 96) * 0.1)

@@ -73,6 +73,9 @@ extern "C" {
  *                                out 4.
  * RESSIRENDISENTANGLE (siren.py:982-1082):   trunk 8, color 6, label 0, grid 0 (FENERF_FIELD_BRIDGE |
  *                                FENERF_FIELD_BRIDGE_RES), scale 2/0.24, out 4.
+ * With FENERF_FIELD_WO_DIR the first colour layer reads c = FiLM(cat[grid_feat(G), x(256)] -> 256), no direction:
+ * TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96 (siren.py:1549-1640, 1817-1822):
+ *                                trunk 8, color 8, label 18, grid 32 x 96^3 (FENERF_FIELD_WO_DIR), scale 2/0.24, out 22.
  * The hidden width is fixed at 256.                                                            */
 #define FENERF_MAX_TRUNK 8
 #define FENERF_MAX_COLOR 8
@@ -100,6 +103,14 @@ extern "C" {
                                          Linear(3->256)(v)]: color_w[0] is [256][3+256], sigma_w / sigma_b are unused and
                                          the chain's parameters come in fenerf_bridge_params, so such a field is packed and
                                          fingerprinted by the _bridge entry points only (RESSIRENDISENTANGLE). */
+#define FENERF_FIELD_WO_DIR 0x20      /* the colour branch reads no ray direction: color_w[0] is [256][G+256] in the column
+                                         order (feat, x).  Only the reference's shape is accepted
+                                         (TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96): trunk 8, colour 8,
+                                         grid_channels 32, the label chain (label_dim >= 1), no other flag.  Anything else
+                                         with this bit is FENERF_E_UNSUPPORTED.  The directions are still passed; the
+                                         outputs do not depend on them.  The colours are computed by FENERF_PRECISION_EXACT
+                                         only: FAST / GUARD return FENERF_E_UNSUPPORTED unless FENERF_POINTS_SIGMA_ONLY (the
+                                         first colour layer's U(+-1/3) weights amplify the fp16 trunk's error to ~2e-2). */
 
 typedef struct fenerf_field_desc {
     int32_t trunk_layers;   /* 2..8 */
@@ -120,7 +131,8 @@ typedef struct fenerf_field_params {
     const float* sigma_w;                    /* [1][256] */
     const float* sigma_b;                    /* [1] */
     const float* color_w[FENERF_MAX_COLOR];  /* first [256][3+G+256] (cat order dir, feat, x), rest [256][256];
-                                                FENERF_FIELD_GRID_TRUNK: first [256][3+256] */
+                                                FENERF_FIELD_GRID_TRUNK: first [256][3+256];
+                                                FENERF_FIELD_WO_DIR: first [256][G+256] (feat, x) */
     const float* color_b[FENERF_MAX_COLOR];
     const float* rgb_w;                      /* [3][256]; FENERF_FIELD_FEATURE_HEAD: [64][256] */
     const float* rgb_b;                      /* [3]; FENERF_FIELD_FEATURE_HEAD: [64] */
