@@ -19,7 +19,8 @@ FIELD_BRIDGE = 0x4            # FENERF_FIELD_BRIDGE: the colour branch starts fr
 FIELD_FEATURE_HEAD = 0x8      # FENERF_FIELD_FEATURE_HEAD: Linear(256 -> 64) colour head without the sigmoid
 FIELD_BRIDGE_RES = 0x10       # FENERF_FIELD_BRIDGE_RES: v adds the position, the density is a Linear chain on v
 FIELD_WO_DIR = 0x20           # FENERF_FIELD_WO_DIR: the first colour layer reads [feat, x], no ray direction
-PRECISION = {"exact": 0, "fast": 1, "guard": 2}
+FIELD_SPLIT_IMAGES = 0x40     # FENERF_FIELD_SPLIT_IMAGES: the pack also holds the fp16 low parts of the weight images
+PRECISION = {"exact": 0, "fast": 1, "guard": 2, "split": 3}
 CLAMP = {"relu": 0, "softplus": 1}
 FILL_MODE = {None: 0, "debug": 1, "weight": 2, "weight_debug": 3, "seg_padding_background": 4,
              "eval_seg_padding_background": 5, "eval_white_back": 6}

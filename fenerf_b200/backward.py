@@ -192,14 +192,14 @@ def _linear_chain_grads(chain, d_weff, d_beff):
 class _FieldBackward:
     """Accumulates the gradients of one field over any number of point sets."""
 
-    def __init__(self, module, film, scale, inv_scale, exact=False):
+    def __init__(self, module, film, scale, inv_scale, exact=False, split=False):
         self.module = module
         # stream element type: fp16 (default) or fp32 (parity mode, with precision='exact': plain fp32 GEMMs)
         self.dt = torch.float32 if exact else torch.float16
         self.dtc = 1 if exact else 0
         self.fw = FieldWeights(module)
         self.spec = self.fw.spec
-        self.packed = module.packed()
+        self.packed = module.packed(split=split)       # (split: the pack the forward rendered from; same sections)
         self.film = film.detach().float().contiguous()           # (B, n_film, 2, 256)
         self.scale, self.inv_scale = scale, inv_scale
         dev = self.film.device
@@ -247,7 +247,8 @@ class _FieldBackward:
         self.wd = self.spec.wo_dir
         if self.wd and not exact:
             raise RuntimeError("the direction-free field (FENERF_FIELD_WO_DIR) renders and differentiates in "
-                               "precision='exact' only: its first colour layer amplifies the fp16 streams' error")
+                               "precision='exact' only: its first colour layer amplifies the fp16 streams' error (precision='split' "
+                               "renders it on the tensor cores and differentiates as 'exact')")
         if self.wd:
             wc0 = torch.cat([torch.zeros((256, 3), dtype=torch.float32, device=dev), wc0], dim=1)
         self.bias = [b.detach().float().contiguous() for _, b in fw.film_layers()]
@@ -620,7 +621,10 @@ class RenderFunction(torch.autograd.Function):
                 m = torch.maximum(m, d_raw_f.abs().max())
             scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)
             inv_scale = (1.0 / scale).float().reshape(1)
-            fb = _FieldBackward(module, film, scale, inv_scale, exact=(rd.precision == _lib.PRECISION['exact']))
+            # precision='split' renders forward on the split-precision kernel and differentiates as 'exact' does
+            split = rd.precision == _lib.PRECISION['split']
+            fb = _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'],
+                                split=split)
             lock = bool(rd.lock_view_dependence)
             rays = call.get('grad_rays')
             dirs = st['dirs']

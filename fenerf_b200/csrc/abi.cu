@@ -47,7 +47,7 @@ int check_render_desc(const fenerf_render_desc* rd) {
         return fail(FENERF_E_CLAMP_MODE, "Need to choose clamp mode");
     FN_REQUIRE(rd->fill_mode >= FENERF_FILL_NONE && rd->fill_mode <= FENERF_FILL_EVAL_WHITE_BACK, "unknown fill_mode %d",
                rd->fill_mode);
-    FN_REQUIRE(rd->precision >= FENERF_PRECISION_EXACT && rd->precision <= FENERF_PRECISION_GUARD, "unknown precision %d",
+    FN_REQUIRE(rd->precision >= FENERF_PRECISION_EXACT && rd->precision <= FENERF_PRECISION_SPLIT, "unknown precision %d",
                rd->precision);
     return 0;
 }
@@ -85,6 +85,7 @@ int make_layout(const fenerf_field_desc* field, FnLayout* L) {
                     "8 trunk and 8 colour layers, grid_channels 32, label_dim >= 1 and no other flag (trunk %d, colour %d, "
                     "label_dim %d, grid %d)", (unsigned)field->reserved, field->trunk_layers, field->color_layers,
                     field->label_dim, field->grid_channels);
+    if (r == -7) return fail(FENERF_E_UNSUPPORTED, "%s (flags 0x%x)", kSplitUnsupported, (unsigned)field->reserved);
     FN_REQUIRE(r == 0, "unsupported field description");
     return 0;
 }
@@ -95,6 +96,8 @@ int run_field(const FnLayout& L, const void* packed, const float* points, const 
     const unsigned char* pk = static_cast<const unsigned char*>(packed);
     if (precision == FENERF_PRECISION_EXACT)
         return siren_points_exact(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, nullptr, 0, out, st, sigma_only);
+    if (precision == FENERF_PRECISION_SPLIT)       // the split-precision wgmma kernel (siren_fast_split.cu)
+        return siren_points_split(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
     // the wgmma kernel (siren_fast.cu)
     return siren_points_fast(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
 }
@@ -153,7 +156,7 @@ int fenerf_siren_points(const fenerf_field_desc* field, const void* packed, cons
     FnLayout L;
     const int sigma_only = (precision & FENERF_POINTS_SIGMA_ONLY) ? 1 : 0;
     precision &= 0xff;
-    FN_REQUIRE(precision >= FENERF_PRECISION_EXACT && precision <= FENERF_PRECISION_GUARD, "unknown precision %d", precision);
+    FN_REQUIRE(precision >= FENERF_PRECISION_EXACT && precision <= FENERF_PRECISION_SPLIT, "unknown precision %d", precision);
     if (int e = make_layout(field, &L)) return e;
     FN_REQUIRE(packed && points && film && out, "NULL argument");
     FN_REQUIRE(dirs, "dirs is NULL (pass any (B,P/dir_group,3) tensor; the colour branch consumes it)");
@@ -161,11 +164,14 @@ int fenerf_siren_points(const fenerf_field_desc* field, const void* packed, cons
     FN_REQUIRE(points_per_batch % dir_group == 0, "points_per_batch must be a multiple of dir_group");
     cudaStream_t st = (cudaStream_t)stream;
     if (only_idx) {
+        if (precision == FENERF_PRECISION_SPLIT)
+            return fail(FENERF_E_UNSUPPORTED, "only_idx (the GUARD refinement's exact re-evaluation) does not go with "
+                        "FENERF_PRECISION_SPLIT");
         if (n_only <= 0) return 0;
         return siren_points_exact(L, (const unsigned char*)packed, points, dirs, film, batch, points_per_batch, dir_group,
                                   0, only_idx, n_only, out, st);
     }
-    FN_REQUIRE(precision >= FENERF_PRECISION_EXACT && precision <= FENERF_PRECISION_GUARD, "unknown precision %d", precision);
+    FN_REQUIRE(precision >= FENERF_PRECISION_EXACT && precision <= FENERF_PRECISION_SPLIT, "unknown precision %d", precision);
     return run_field(L, packed, points, dirs, film, batch, points_per_batch, dir_group, 0, precision, out, st, sigma_only);
 }
 

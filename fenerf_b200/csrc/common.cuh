@@ -111,6 +111,14 @@ int field_fingerprint(const FnLayout& L, const fenerf_field_params* p, unsigned 
 int siren_points_fast(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
                       int batch, long long ppb, int dir_group, int lock_dirs, float* out, int sigma_only, cudaStream_t st,
                       float* sigma_out = nullptr);
+// FENERF_PRECISION_SPLIT: the kSplit instantiation of the wgmma kernel (siren_fast_split.cu)
+int siren_points_split(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs, const float* film,
+                       int batch, long long ppb, int dir_group, int lock_dirs, float* out, int sigma_only, cudaStream_t st,
+                       float* sigma_out = nullptr);
+// what FENERF_PRECISION_SPLIT and FENERF_FIELD_SPLIT_IMAGES do not serve
+constexpr const char* kSplitUnsupported =
+    "FENERF_PRECISION_SPLIT / FENERF_FIELD_SPLIT_IMAGES: not built for fields with FENERF_FIELD_LABEL_FILM, "
+    "FENERF_FIELD_FEATURE_HEAD, FENERF_FIELD_GRID_TRUNK or FENERF_FIELD_BRIDGE (render them in exact, fast or guard)";
 // debug: which instantiation siren_points_fast launches (0 production; siren_fast_debug.cu) and the device software sine
 int siren_fast_debug_variant(int variant, unsigned long long* trace, int trace_ctas);
 int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st);

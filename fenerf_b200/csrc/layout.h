@@ -55,6 +55,15 @@
 //   no direction     (FENERF_FIELD_WO_DIR) the first colour layer reads [feat, x]; it is packed in the plain layout
 //                    (kx = 3 + G) with zero direction rows and zero direction slots, so every kernel runs it as a plain
 //                    grid field and no output depends on the direction.
+//   split images     (FENERF_FIELD_SPLIT_IMAGES, for FENERF_PRECISION_SPLIT) appended after every other section, so that
+//                    a pack without the bit is byte for byte what it was.  Every weight matrix M the split kernel reads
+//                    (first layer, hidden layers, the first colour layer's input chunk, trunk head, colour head) is scaled
+//                    by a power of two s_M with max |s_M M| in [0.5, 1), then split hi = f16(s_M w), lo = f16(s_M w - hi):
+//                    unscaled, the hidden layers' frequency_init weights (|w| <= 6.1e-3) leave lo below fp16's normal
+//                    range with a few significant bits.  Sections: the scaled high and the low images, each in the
+//                    layout of its unscaled image, and split_scale = [s_M ..., 1 / s_M ...] (float, M = 0 the first
+//                    layer, 1 + l hidden layer l, n_hidden + 1 the trunk head, n_hidden + 2 the colour head); the
+//                    kernel multiplies the FiLM frequency, or the head output, by 1 / s_M, exactly.
 //
 // "Input chunk" slot order (the 64-wide A chunk the wgmma kernel builds per point):
 //   0..2 pos_hi  3..5 pos_lo  6..8 pos_hi | 16..18 dir_hi 19..21 dir_lo 22..24 dir_hi | 32..63 feat
@@ -72,6 +81,7 @@
 #define FN_SLOT_POS 0
 #define FN_SLOT_DIR 16
 #define FN_SLOT_FEAT 32
+#define FN_SPLIT_SCALES (FN_MAX_HIDDEN + 3)   // split images: first layer, hidden layers, trunk head, colour head
 
 // The f16 image of a head with `rows` rows: [4 chunks][rows][64 k]
 #define FN_HEAD_IMG_BYTES(rows) ((size_t)(FN_H / FN_KCHUNK) * (rows) * FN_KCHUNK * 2)
@@ -113,22 +123,37 @@ struct FnLayout {
     int32_t bridge_res;     // FENERF_FIELD_BRIDGE_RES: v adds the position, the density is a . v + c
     size_t bridge_w;        // bridge: [3][256] f32 weights of v, b[3], then a[3], c (RES; 0 otherwise)
     int32_t wo_dir;         // the variant flag FENERF_FIELD_WO_DIR: the first colour layer reads [feat, x] (zero direction rows)
+    // FENERF_FIELD_SPLIT_IMAGES (see above; 0 otherwise): scaled high (_s) and low (_lo) images, and the scales
+    int32_t split_images;
+    size_t first_img_s;
+    size_t hid_img_s[FN_MAX_HIDDEN], hid_img_lo[FN_MAX_HIDDEN];
+    size_t color0_ximg_s;   // the whole input-chunk image, scaled (its direction slots hi, hi, lo as in color0_ximg)
+    size_t color0_ximg_lo;  // its feature columns' low parts (grid fields)
+    size_t head_img_s, head_img_lo, rgb_img_s, rgb_img_lo;
+    size_t split_scale;     // float [2][FN_SPLIT_SCALES]
 };
 
 static inline size_t fn_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // Returns 0 and fills `L`, -2 if the flags hold an unknown bit, -3 if they ask for a feature head, -4 for the grid in
-// the trunk, -5 for a bridge or -6 for a direction-free colour branch on a field shape no reference class has, or -1 if
-// the description is outside what the kernels support.
+// the trunk, -5 for a bridge or -6 for a direction-free colour branch on a field shape no reference class has, -7 for the
+// split images on a field variant the split kernel does not serve, or -1 if the description is outside what the kernels
+// support.
 static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     if (!f || !L) return -1;
     if (f->reserved & ~(FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD | FENERF_FIELD_GRID_TRUNK | FENERF_FIELD_BRIDGE |
-                        FENERF_FIELD_BRIDGE_RES | FENERF_FIELD_WO_DIR))
+                        FENERF_FIELD_BRIDGE_RES | FENERF_FIELD_WO_DIR | FENERF_FIELD_SPLIT_IMAGES))
         return -2;
-    const int wo_dir = (f->reserved & FENERF_FIELD_WO_DIR) ? 1 : 0;
+    // the split images are a packing option; the field's shape is in the other bits
+    const int split = (f->reserved & FENERF_FIELD_SPLIT_IMAGES) ? 1 : 0;
+    const int32_t shape = f->reserved & ~FENERF_FIELD_SPLIT_IMAGES;
+    if (split && (shape & (FENERF_FIELD_LABEL_FILM | FENERF_FIELD_FEATURE_HEAD | FENERF_FIELD_GRID_TRUNK | FENERF_FIELD_BRIDGE |
+                           FENERF_FIELD_BRIDGE_RES)))
+        return -7;
+    const int wo_dir = (shape & FENERF_FIELD_WO_DIR) ? 1 : 0;
     // TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96: 8 + 8 layers, a 32-channel grid, the label chain, no other
     // flag
-    if (wo_dir && (f->reserved != FENERF_FIELD_WO_DIR || f->grid_channels != 32 || f->label_dim < 1 || f->trunk_layers != 8 ||
+    if (wo_dir && (shape != FENERF_FIELD_WO_DIR || f->grid_channels != 32 || f->label_dim < 1 || f->trunk_layers != 8 ||
                    f->color_layers != 8))
         return -6;
     const int label_film = (f->reserved & FENERF_FIELD_LABEL_FILM) ? 1 : 0;
@@ -208,6 +233,24 @@ static inline int fn_make_layout(const fenerf_field_desc* f, FnLayout* L) {
     L->first_img_lo = grid_trunk ? take(FN_IMG_BYTES) : 0;
     L->bridge_w = bridge ? take((3 * FN_H + 3 + 3 + 1) * 4) : 0;
     L->wo_dir = wo_dir;
+    L->split_images = split ? 1 : 0;
+    for (int l = 0; l < FN_MAX_HIDDEN; ++l) L->hid_img_s[l] = L->hid_img_lo[l] = 0;
+    L->first_img_s = L->color0_ximg_s = L->color0_ximg_lo = L->head_img_s = L->head_img_lo = 0;
+    L->rgb_img_s = L->rgb_img_lo = L->split_scale = 0;
+    if (split) {
+        L->first_img_s = take(FN_IMG_BYTES);
+        for (int l = 0; l < L->n_hidden; ++l) {
+            L->hid_img_s[l] = take((size_t)(FN_H / FN_KCHUNK) * FN_IMG_BYTES);
+            L->hid_img_lo[l] = take((size_t)(FN_H / FN_KCHUNK) * FN_IMG_BYTES);
+        }
+        L->color0_ximg_s = take(FN_IMG_BYTES);
+        if (f->grid_channels > 0) L->color0_ximg_lo = take(FN_IMG_BYTES);
+        L->head_img_s = take(FN_HEAD_IMG_BYTES(32));
+        L->head_img_lo = take(FN_HEAD_IMG_BYTES(32));
+        L->rgb_img_s = take(FN_HEAD_IMG_BYTES(8));
+        L->rgb_img_lo = take(FN_HEAD_IMG_BYTES(8));
+        L->split_scale = take(2 * FN_SPLIT_SCALES * 4);
+    }
     L->total = off;
     return 0;
 }

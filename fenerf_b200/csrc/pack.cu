@@ -289,6 +289,106 @@ __global__ void pack_bridge_head_kernel(const float* __restrict__ sw, const floa
     }
 }
 
+// ---- FENERF_FIELD_SPLIT_IMAGES (layout.h): per weight matrix M a power-of-two scale s_M, then the scaled high and low
+// images, from the pack's own fp32 copies (the values the plain images are rounded from) ---------------------------------
+// matrix m of the split kernel: 0 the first layer [256][3], 1 + l hidden layer l [256][256 (+ kx for the first colour
+// layer)], n_hidden + 1 the trunk head [32][256] (rows as pack_trunk_head_kernel writes them), n_hidden + 2 the colour
+// head [img_rows][256]
+__device__ int split_cols(const FnLayout& L, int m) {
+    return m == 0 ? 3 : (m <= L.n_hidden && m - 1 == L.color0) ? FN_H + L.kx : FN_H;
+}
+__device__ int split_rows(const FnLayout& L, int m) {
+    return m == L.n_hidden + 1 ? 32 : m == L.n_hidden + 2 ? L.rgb.img_rows : FN_H;
+}
+__device__ float split_w(const FnLayout& L, const unsigned char* packed, int m, int n, int k) {
+    if (m == 0) return reinterpret_cast<const float*>(packed + L.first_w)[k * FN_H + n];
+    if (m <= L.n_hidden) return reinterpret_cast<const float*>(packed + L.hid_w32[m - 1])[(size_t)k * FN_H + n];
+    if (m == L.n_hidden + 1) {
+        const float* lw = reinterpret_cast<const float*>(packed + L.label_w);
+        if (n < L.trunk_labels) return lw[n * FN_H + k] * (1.f / lw[FENERF_MAX_LABEL * FN_H + FENERF_MAX_LABEL]);
+        return n == L.sigma_row ? reinterpret_cast<const float*>(packed + L.sigma_w)[k] : 0.f;
+    }
+    return n < L.rgb.n_out ? reinterpret_cast<const float*>(packed + L.rgb.w)[n * FN_H + k] : 0.f;
+}
+
+// one block per matrix: s_M = 2^-e with max |w| = f 2^e, f in [0.5, 1), so that max |s_M w| is in [0.5, 1)
+__global__ void pack_split_scale_kernel(FnLayout L, unsigned char* __restrict__ packed) {
+    __shared__ float smax[256];
+    const int m = blockIdx.x, rows = split_rows(L, m), cols = split_cols(L, m);
+    float mx = 0.f;
+    for (int i = threadIdx.x; i < rows * cols; i += blockDim.x) mx = fmaxf(mx, fabsf(split_w(L, packed, m, i % rows, i / rows)));
+    smax[threadIdx.x] = mx;
+    __syncthreads();
+    for (int s = 128; s > 0; s >>= 1) {
+        if ((int)threadIdx.x < s) smax[threadIdx.x] = fmaxf(smax[threadIdx.x], smax[threadIdx.x + s]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        int e = 0;
+        if (smax[0] > 0.f && isfinite(smax[0])) frexpf(smax[0], &e);
+        float* sc = reinterpret_cast<float*>(packed + L.split_scale);
+        sc[m] = ldexpf(1.f, -e);
+        sc[FN_SPLIT_SCALES + m] = ldexpf(1.f, e);
+    }
+}
+
+__device__ __forceinline__ void put_h(unsigned char* img, uint32_t off, __half v) { *reinterpret_cast<__half*>(img + off) = v; }
+
+// the first layer's input-chunk image, scaled: the position slots hi, hi, lo as in pack_first_kernel (one block)
+__global__ void pack_split_first_kernel(FnLayout L, unsigned char* __restrict__ packed) {
+    const int n = threadIdx.x;
+    const float s = reinterpret_cast<const float*>(packed + L.split_scale)[0];
+    unsigned char* img = packed + L.first_img_s;
+    for (int k = 0; k < FN_KCHUNK; ++k) put_h(img, fn_sw128_offset(n, k), __float2half_rn(0.f));
+    for (int k = 0; k < 3; ++k) {
+        const float v = split_w(L, packed, 0, n, k) * s;
+        put_h(img, fn_sw128_offset(n, FN_SLOT_POS + k), f16_hi(v));
+        put_h(img, fn_sw128_offset(n, FN_SLOT_POS + 3 + k), f16_hi(v));
+        put_h(img, fn_sw128_offset(n, FN_SLOT_POS + 6 + k), f16_lo(v));
+    }
+}
+
+// hidden layer l's scaled 256-wide image and its low parts (one block per output n, one thread per k); for the first
+// colour layer also its scaled input-chunk image (direction hi, hi, lo in slots 16.., features hi in 32..) and the
+// features' low parts
+__global__ void pack_split_hidden_kernel(FnLayout L, int l, unsigned char* __restrict__ packed) {
+    const int n = blockIdx.x, k = threadIdx.x, m = 1 + l;
+    const float s = reinterpret_cast<const float*>(packed + L.split_scale)[m];
+    const float v = split_w(L, packed, m, n, k) * s;
+    put_h(packed + L.hid_img_s[l], fn_hidden_img_offset(n, k), f16_hi(v));
+    put_h(packed + L.hid_img_lo[l], fn_hidden_img_offset(n, k), f16_lo(v));
+    if (l != L.color0 || k >= FN_KCHUNK) return;
+    const int g = L.grid_channels, j = k - FN_SLOT_DIR, c = k - FN_SLOT_FEAT;
+    __half hi = __float2half_rn(0.f), lo = __float2half_rn(0.f);
+    if (j >= 0 && j < 9) {
+        const float d = split_w(L, packed, m, n, FN_H + j % 3) * s;
+        hi = j < 6 ? f16_hi(d) : f16_lo(d);
+    } else if (c >= 0 && c < g) {
+        const float f = split_w(L, packed, m, n, FN_H + 3 + c) * s;
+        hi = f16_hi(f);
+        lo = f16_lo(f);
+    }
+    put_h(packed + L.color0_ximg_s, fn_sw128_offset(n, k), hi);
+    if (g > 0) put_h(packed + L.color0_ximg_lo, fn_sw128_offset(n, k), lo);
+}
+
+// the two heads' scaled images and low parts (one block)
+__global__ void pack_split_heads_kernel(FnLayout L, unsigned char* __restrict__ packed) {
+    const float* sc = reinterpret_cast<const float*>(packed + L.split_scale);
+    for (int h = 0; h < 2; ++h) {
+        const int m = L.n_hidden + 1 + h, rows = split_rows(L, m);
+        unsigned char* hi_img = packed + (h ? L.rgb_img_s : L.head_img_s);
+        unsigned char* lo_img = packed + (h ? L.rgb_img_lo : L.head_img_lo);
+        for (int i = threadIdx.x; i < rows * FN_H; i += blockDim.x) {
+            const int row = i / FN_H, k = i % FN_H;
+            const float v = split_w(L, packed, m, row, k) * sc[m];
+            const size_t chunk = (size_t)(k / FN_KCHUNK) * (rows * FN_KCHUNK * 2);
+            put_h(hi_img + chunk, fn_sw128_offset(row, k % FN_KCHUNK), f16_hi(v));
+            put_h(lo_img + chunk, fn_sw128_offset(row, k % FN_KCHUNK), f16_lo(v));
+        }
+    }
+}
+
 // ---- grid: (G, D, H, W) channel-major -> [D][H][W][G] channels-last ---------------------------
 // one block per (z, y) line: read G rows of R contiguous x, write R*G contiguous floats
 __global__ void pack_grid_kernel(const float* __restrict__ in, float* __restrict__ out, __half* __restrict__ out16, int R, int G) {
@@ -479,6 +579,18 @@ int pack_field(const FnLayout& L, const fenerf_field_params* p, void* packed_v, 
             FN_CUDA_OK(cudaFuncSetAttribute(pack_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         pack_grid_kernel<<<R * R, 256, smem, st>>>(p->grid, (float*)(packed + L.grid), (__half*)(packed + L.grid16), R, G);
         FN_LAUNCH_OK("pack_grid_kernel");
+    }
+    if (L.split_images) {        // (fn_make_layout admits the bit for plain, grid and direction-free fields only)
+        pack_split_scale_kernel<<<L.n_hidden + 3, 256, 0, st>>>(L, packed);
+        FN_LAUNCH_OK("pack_split_scale_kernel");
+        pack_split_first_kernel<<<1, FN_H, 0, st>>>(L, packed);
+        FN_LAUNCH_OK("pack_split_first_kernel");
+        for (int l = 0; l < L.n_hidden; ++l) {
+            pack_split_hidden_kernel<<<FN_H, FN_H, 0, st>>>(L, l, packed);
+            FN_LAUNCH_OK("pack_split_hidden_kernel");
+        }
+        pack_split_heads_kernel<<<1, 256, 0, st>>>(L, packed);
+        FN_LAUNCH_OK("pack_split_heads_kernel");
     }
     return 0;
 }

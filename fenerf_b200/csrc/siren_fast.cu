@@ -82,7 +82,7 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     if (L.wo_dir && !sigma_only)
         return fail(FENERF_E_UNSUPPORTED, "FENERF_FIELD_WO_DIR: the wgmma colour branch is not accurate for this field (its "
                     "first colour layer amplifies the fp16 trunk's error to ~2e-2 in rgb); render it with "
-                    "FENERF_PRECISION_EXACT (the density alone runs in any precision)");
+                    "FENERF_PRECISION_EXACT or FENERF_PRECISION_SPLIT (the density alone runs in any precision)");
     FastArgs a;
     memset(&a, 0, sizeof(a));
     FN_REQUIRE(build_loads(L, a, sigma_only != 0), "field too deep for the weight stream");

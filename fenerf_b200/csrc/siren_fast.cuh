@@ -44,6 +44,11 @@
 //                  density is then a . v + c in fp32), split hi / lo into the staging row's slots 32..40, and the first
 //                  colour layer is one narrow MMA group per half: the direction and v slices against the input-chunk image,
 //                  no 256-wide part.
+//   kSplit         (FENERF_PRECISION_SPLIT, siren_fast_split.cu) every layer half and head issues hi * W_hi (RS), lo * W_hi
+//                  (SS: the activations' low parts from the warpgroup's A_lo region) and hi * W_lo (RS) against the pack's
+//                  power-of-two scaled split images, on a four-slot ring; the first colour layer's input-chunk slices take
+//                  a turn of their own; every sine is soft_sinf, and the epilogue holds half 0's low parts in registers
+//                  until half 1's MMA group has read the current A_lo (DESIGN section 5).
 //
 // The plain and the label FiLM instantiations live in translation units of their own (siren_fast.cu,
 // siren_fast_label.cu), the two feature-head ones in a third (siren_fast_hd.cu) and the grid-trunk one in a fourth
@@ -80,7 +85,22 @@ constexpr uint32_t SMEM_TOTAL = SMEM_BAR + 16 * RING + 16 + 16 * 2 * FRING;
 constexpr uint32_t SMEM_XLO = SMEM_TOTAL;
 constexpr int XLO_STRIDE = 32;
 constexpr uint32_t SMEM_TOTAL_GRID = SMEM_XLO + 2 * TILE * XLO_STRIDE * 2;
+// kSplit: a ring of four slots (one half layer's W_hi and W_lo, 128 KB), then the warpgroups' A_lo regions, then the
+// sections above in their order.  4 x 32 + 2 x 32 (A_lo) + 18 (staging) + 8 (FiLM) + 0.14 (barriers) + 8 (XLO) KB =
+// 231568 B of the 232448
+constexpr int RING_SPLIT = 4;
+constexpr uint32_t ALO_CHUNK = TILE * FN_KCHUNK * 2;                 // one [64 rows][64 k] f16 A chunk, 8 KB
+constexpr uint32_t ALO_BYTES = (FN_H / FN_KCHUNK) * ALO_CHUNK;      // one warpgroup's [4 k-chunks][64 points][64 k]
+constexpr uint32_t SPLIT_SMEM_ALO = RING_SPLIT * SLOT_BYTES;
+constexpr uint32_t SPLIT_SMEM_X = SPLIT_SMEM_ALO + 2 * ALO_BYTES;
+constexpr uint32_t SPLIT_SMEM_FILM = SPLIT_SMEM_X + 2 * TILE * XSTRIDE * 2;
+constexpr uint32_t SPLIT_SMEM_BAR = SPLIT_SMEM_FILM + 2 * FRING * FILM_BYTES;
+constexpr uint32_t SPLIT_SMEM_XLO = SPLIT_SMEM_BAR + 16 * RING_SPLIT + 16 + 16 * 2 * FRING;
+constexpr uint32_t SMEM_TOTAL_SPLIT = SPLIT_SMEM_XLO + 2 * TILE * XLO_STRIDE * 2;
 constexpr int MAX_LOADS = 72;
+// kSplit: per 256-wide layer 8 loads (both halves' W_hi and W_lo), the first colour layer's input-chunk images once
+// per half, both heads twice: 1 + 15 x 8 + 4 + 4 = 129 at most
+constexpr int MAX_LOADS_SPLIT = 132;
 constexpr uint32_t CHUNK = 16384;                   // one [128 rows][64 k] f16 image chunk
 constexpr uint32_t HEAD_CHUNK = 32 * 128;           // one [32 rows][64 k] chunk of the trunk-head image
 constexpr uint32_t RGB_CHUNK = 8 * 128;             // one [8 rows][64 k] chunk of the rgb-head image
@@ -129,8 +149,9 @@ struct Load {
     uint32_t bytes;
 };
 
-struct FastArgs {
-    Load loads[MAX_LOADS];      // one tile's weight stream, in consumption order (build_loads)
+template <int kMaxLoads>
+struct FastArgsT {
+    Load loads[kMaxLoads];      // one tile's weight stream, in consumption order (build_loads)
     int n_loads;
     FnLayout L;
     const unsigned char* packed;
@@ -145,12 +166,21 @@ struct FastArgs {
     unsigned long long* trace;  // kTrace: [trace_ctas][TRACE_WARPS][TRACE_CAP] events of CTAs 0 .. trace_ctas - 1
     int trace_ctas;
 };
+using FastArgs = FastArgsT<MAX_LOADS>;
+using SplitArgs = FastArgsT<MAX_LOADS_SPLIT>;
 
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
 template <bool kLabelFilm, bool kFeatureHead = false, int kSoftSin = kSoftSinEvery, bool kTrace = false,
-          bool kGridTrunk = false, bool kBridge = false>
-__global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_constant__ FastArgs a) {
+          bool kGridTrunk = false, bool kBridge = false, bool kSplit = false>
+__global__ void __launch_bounds__(NTHREADS, 1)
+    siren_fast_kernel(const __grid_constant__ FastArgsT<kSplit ? MAX_LOADS_SPLIT : MAX_LOADS> a) {
+    // the shared-memory plan (kSplit: a smaller ring and the A_lo regions, see SPLIT_SMEM_ALO)
+    constexpr int RING = kSplit ? RING_SPLIT : fn::RING;
+    constexpr uint32_t SMEM_X = kSplit ? SPLIT_SMEM_X : fn::SMEM_X;
+    constexpr uint32_t SMEM_FILM = kSplit ? SPLIT_SMEM_FILM : fn::SMEM_FILM;
+    constexpr uint32_t SMEM_BAR = kSplit ? SPLIT_SMEM_BAR : fn::SMEM_BAR;
+    constexpr uint32_t SMEM_XLO = kSplit ? SPLIT_SMEM_XLO : fn::SMEM_XLO;
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -220,7 +250,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                     for (int k = 0; k < FN_H / 64; ++k) {    // (not unrolled: the producers live on 40 registers)
                         const int cp = lane + 32 * k;        // column pair: columns 2 cp, 2 cp + 1
                         const float2 f = __ldg(row + cp), p = __ldg(row + FN_H / 2 + cp), bb = __ldg(bias + cp);
-                        dst[cp] = make_float4(f.x, f.y, fmaf(f.x, bb.x, p.x), fmaf(f.y, bb.y, p.y));
+                        if constexpr (kSplit) {
+                            // the layer's weights are scaled by s (layout.h, split images): f / s on the accumulator,
+                            // exact for a power of two
+                            const float us = __ldg(reinterpret_cast<const float*>(a.packed + a.L.split_scale) +
+                                                   FN_SPLIT_SCALES + i);
+                            dst[cp] = make_float4(f.x * us, f.y * us, fmaf(f.x, bb.x, p.x), fmaf(f.y, bb.y, p.y));
+                        } else {
+                            dst[cp] = make_float4(f.x, f.y, fmaf(f.x, bb.x, p.x), fmaf(f.y, bb.y, p.y));
+                        }
                     }
                     mbar_arrive(bar_ffull + 8 * e);
                 }
@@ -338,12 +376,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 split_f16(dir[i], hi, lo);
                 slots[FN_SLOT_DIR + i] = hi; slots[FN_SLOT_DIR + 3 + i] = lo; slots[FN_SLOT_DIR + 6 + i] = hi;
             }
-            if constexpr (kGridTrunk) {
-                // the features feed the trunk, the density included: fp32 lookup, split hi / lo like the position
+            if constexpr (kGridTrunk || kSplit) {
+                // the features feed the trunk, the density included (kSplit: the first colour layer): fp32 lookup, split
+                // hi / lo like the position
                 __align__(16) __half lo[32];
 #pragma unroll
                 for (int i = 0; i < 32; ++i) lo[i] = __float2half_rn(0.f);
-                if (valid) {
+                if (valid && (kGridTrunk || (L.grid_channels > 0 && !a.sigma_only))) {
                     float feat[32];
                     grid_features32(reinterpret_cast<const float*>(a.packed + L.grid), L.grid_res, pos[0], pos[1], pos[2], feat);
 #pragma unroll
@@ -382,6 +421,47 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             trace(TR_EPI_DONE);
         };
         auto act_hi = [&]() -> uint32_t (&)[8][4] { return *reinterpret_cast<uint32_t (*)[8][4]>(&act[8]); };
+        // kSplit: the same epilogue with every sine on soft_sinf (sin.approx loses the bits of its own a / 2pi product),
+        // hi = f16(s) into dst and lo = f16(s - hi) into lo, in the same fragment order
+        auto film_epi_split = [&](const float4* fs, int h, uint32_t (&dst)[8][4], uint32_t (&lo)[8][4]) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const float4 e = fs[64 * h + 4 * j + q];
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    const float s0 = soft_sinf(fmaf(e.x, d[4 * j + 2 * rr], e.z));
+                    const float s1 = soft_sinf(fmaf(e.y, d[4 * j + 2 * rr + 1], e.w));
+                    const __half2 hi = __floats2half2_rn(s0, s1);
+                    const float2 hf = __half22float2(hi);
+                    dst[j >> 1][(j & 1) * 2 + rr] = *reinterpret_cast<const uint32_t*>(&hi);
+                    lo[j >> 1][(j & 1) * 2 + rr] = pack_half2(s0 - hf.x, s1 - hf.y);
+                }
+            }
+            trace(TR_EPI_DONE);
+        };
+        // kSplit: this warpgroup's A_lo region holds the low parts of the layer input, K-major and 128B-swizzled like
+        // the weight images: k-slice s at chunk s / 4, + 32 B per slice within it
+        const uint32_t alo_base = sbase + SPLIT_SMEM_ALO + wg * ALO_BYTES;
+        auto alo_desc = [&](int s) { return desc_kmajor(alo_base + (s >> 2) * ALO_CHUNK + 32 * (s & 3)); };
+        // The next layer's low parts, both halves at once: half 0's are produced while half 1's MMA group still has to
+        // read the current ones, so they wait in registers (lo0) until every MMA group on the current A_lo has completed
+        auto alo_store = [&](const uint32_t (&lo0)[8][4], const uint32_t (&lo1)[8][4]) {
+            wg_bar(wg);                              // every warp is past its last wait on the current A_lo
+            unsigned char* base = smem + SPLIT_SMEM_ALO + wg * ALO_BYTES;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int col = 128 * h + 8 * j + 2 * q;
+#pragma unroll
+                    for (int rr = 0; rr < 2; ++rr)
+                        *reinterpret_cast<uint32_t*>(base + (col >> 6) * ALO_CHUNK + fn_sw128_offset(r0 + 8 * rr, col & 63)) =
+                            (h ? lo1 : lo0)[j >> 1][(j & 1) * 2 + rr];
+                }
+            fence_async_smem();                      // the generic-proxy stores, visible to the tensor cores' reads
+            wg_bar(wg);
+        };
+        uint32_t lo0[8][4], lo1[8][4];               // kSplit: the epilogue's low parts of half 0, half 1
 
         // ---- first layer: input slots (k-slice 0) against the [256][64] input image; with the grid in the trunk also the
         // feature slices 2, 3 as hi * W_hi + lo * W_hi + hi * W_lo (the low parts of W: the image after it) ----
@@ -424,12 +504,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 fence_regs(xf);
                 if constexpr (kGridTrunk) { fence_regs(xg); fence_regs(xl); }
                 if (h == 0) fs = film_acquire();
-                if (h == 0) film_epi(fs, 0, nxt);
-                else film_epi(fs, 1, act_hi());
+                if constexpr (kSplit) {
+                    if (h == 0) film_epi_split(fs, 0, nxt, lo0);
+                    else film_epi_split(fs, 1, act_hi(), lo1);
+                } else {
+                    if (h == 0) film_epi(fs, 0, nxt);
+                    else film_epi(fs, 1, act_hi());
+                }
             }
             release(slot);
             if constexpr (kGridTrunk) release(slot_lo);
             film_release();
+            if constexpr (kSplit) alo_store(lo0, lo1);
 #pragma unroll
             for (int s = 0; s < 8; ++s)
 #pragma unroll
@@ -441,14 +527,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             if (l == L.trunk_hidden) {
                 // ---- trunk head: [labels (scaled), sigma] = A . head^T, 32 columns ----
                 float dh[16];
-                uint32_t slot;
+                uint32_t slot, slot_lo = 0, w_lo = 0;
                 const uint32_t w = acquire(slot);
+                if constexpr (kSplit) w_lo = acquire(slot_lo);
                 turn_begin();                        // after acquire: the other order makes ptxas serialize the wgmmas
                 wg_fence();
 #pragma unroll
                 for (int c = 0; c < 4; ++c)
 #pragma unroll
                     for (int k = 0; k < 4; ++k) mma_rs_n32(dh, act[4 * c + k], desc_kmajor(w + c * HEAD_CHUNK + 32 * k), (c | k) ? 1u : 0u);
+                if constexpr (kSplit)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            mma_ss_n32(dh, alo_desc(4 * c + k), desc_kmajor(w + c * HEAD_CHUNK + 32 * k), 1u);
+                            mma_rs_n32(dh, act[4 * c + k], desc_kmajor(w_lo + c * HEAD_CHUNK + 32 * k), 1u);
+                        }
                 wg_commit();
                 turn_end(TG_TRUNK_HEAD);
                 wg_wait<0>();
@@ -456,6 +551,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
                 fence_regs(dh);
                 fence_regs(act);
                 release(slot);
+                if constexpr (kSplit) {
+                    release(slot_lo);
+                    const float us = __ldg(reinterpret_cast<const float*>(a.packed + L.split_scale) + FN_SPLIT_SCALES +
+                                           L.n_hidden + 1);
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) dh[i] *= us;       // the head's scale, undone exactly
+                }
                 // the chain's beff, then its 1/scale, read where a label is written (hoisted out of the layer loop
                 // beside trunk_labels and sigma_row, it cost the hidden layers' MMA issue a uniform register)
                 const float* lb = label_w + FENERF_MAX_LABEL * FN_H;
@@ -584,6 +686,87 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             }
             // ---- FiLM layer l + 1: weight image halves 64 KB apart, two 32 KB slabs per half ----
             const bool c0 = (l == L.color0);     // first colour layer: + direction / grid-feature slots
+            if constexpr (kSplit) {
+                // per half one MMA group on four ring slots (W_hi k-chunks 0, 1 | 2, 3, then W_lo's): hi * W_hi (A in
+                // registers), lo * W_hi (A_lo from shared memory), hi * W_lo.  The first colour layer's input-chunk slices
+                // follow in a turn of their own, against the input-chunk image and, for the grid features, its low parts
+                // (the whole ring is taken by the first group)
+                const bool grid = L.grid_channels > 0;
+                const float4* fs = nullptr;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    uint32_t sl[4], w[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) w[i] = acquire(sl[i]);
+                    turn_begin();
+                    wg_fence();
+#pragma unroll
+                    for (int s = 0; s < 16; ++s)
+                        mma_rs_n128(d, act[s], desc_kmajor(w[s >> 3] + ((s >> 2) & 1) * CHUNK + 32 * (s & 3)), s ? 1u : 0u);
+#pragma unroll
+                    for (int s = 0; s < 16; ++s)
+                        mma_ss_n128(d, alo_desc(s), desc_kmajor(w[s >> 3] + ((s >> 2) & 1) * CHUNK + 32 * (s & 3)), 1u);
+#pragma unroll
+                    for (int s = 0; s < 16; ++s)
+                        mma_rs_n128(d, act[s], desc_kmajor(w[2 + (s >> 3)] + ((s >> 2) & 1) * CHUNK + 32 * (s & 3)), 1u);
+                    wg_commit();
+                    turn_end(c0 ? TG_COLOR0 : TG_HIDDEN);
+                    wg_wait<0>();
+                    trace(TR_MMA_DONE);
+                    fence_regs(d);
+                    fence_regs(act);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) release(sl[i]);
+                    if (c0) {
+                        // direction slice 1 (hi, lo, hi against W_hi, W_hi, W_lo), feature slices 2, 3 as
+                        // hi * W_hi + lo * W_hi + hi * W_lo
+                        uint32_t xf[3][4], xl[2][4], slot_x, slot_xl = 0, w_xl = 0;
+#pragma unroll
+                        for (int s = 0; s < 3; ++s) xfrag(1 + s, xf[s]);
+                        const __half* xlo = reinterpret_cast<const __half*>(smem + SMEM_XLO) + wg * TILE * XLO_STRIDE;
+#pragma unroll
+                        for (int s = 0; s < 2; ++s) {
+                            const __half* p = xlo + r0 * XLO_STRIDE + 16 * s + 2 * q;
+                            xl[s][0] = *reinterpret_cast<const uint32_t*>(p);
+                            xl[s][1] = *reinterpret_cast<const uint32_t*>(p + 8 * XLO_STRIDE);
+                            xl[s][2] = *reinterpret_cast<const uint32_t*>(p + 8);
+                            xl[s][3] = *reinterpret_cast<const uint32_t*>(p + 8 * XLO_STRIDE + 8);
+                        }
+                        const uint32_t w_x = acquire(slot_x);
+                        if (grid) w_xl = acquire(slot_xl);
+                        turn_begin();
+                        wg_fence();
+                        mma_rs_n128(d, xf[0], desc_kmajor(w_x + h * CHUNK + 32), 1u);
+                        if (grid)
+#pragma unroll
+                            for (int s = 0; s < 2; ++s) {
+                                const uint32_t off = h * CHUNK + 32 * (2 + s);
+                                mma_rs_n128(d, xf[1 + s], desc_kmajor(w_x + off), 1u);
+                                mma_rs_n128(d, xl[s], desc_kmajor(w_x + off), 1u);
+                                mma_rs_n128(d, xf[1 + s], desc_kmajor(w_xl + off), 1u);
+                            }
+                        wg_commit();
+                        turn_end(TG_COLOR0);
+                        wg_wait<0>();
+                        trace(TR_MMA_DONE);
+                        fence_regs(d);
+                        fence_regs(xf);
+                        fence_regs(xl);
+                        release(slot_x);
+                        if (grid) release(slot_xl);
+                    }
+                    if (h == 0) fs = film_acquire();
+                    if (h == 0) film_epi_split(fs, 0, nxt, lo0);
+                    else film_epi_split(fs, 1, act_hi(), lo1);
+                }
+                film_release();
+                alo_store(lo0, lo1);
+#pragma unroll
+                for (int s = 0; s < 8; ++s)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) act[s][i] = nxt[s][i];
+                continue;
+            }
             const bool narrow = kBridge && c0;   // a bridge field's: the direction and v slices alone
             // (a grid-trunk field: the direction alone; a bridge field: the direction and v)
             const int nx = kBridge ? 2 : !kGridTrunk && L.grid_channels > 0 ? 3 : 1;
@@ -676,14 +859,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
         // ---- rgb head: sigmoid(A . rgb^T + b), 8 columns of which 3 are used ----
         {
             float dr[4];
-            uint32_t slot;
+            uint32_t slot, slot_lo = 0, w_lo = 0;
             const uint32_t w = acquire(slot);
+            if constexpr (kSplit) w_lo = acquire(slot_lo);
             turn_begin();
             wg_fence();
 #pragma unroll
             for (int c = 0; c < 4; ++c)
 #pragma unroll
                 for (int k = 0; k < 4; ++k) mma_rs_n8(dr, act[4 * c + k], desc_kmajor(w + c * RGB_CHUNK + 32 * k), (c | k) ? 1u : 0u);
+            if constexpr (kSplit)
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        mma_ss_n8(dr, alo_desc(4 * c + k), desc_kmajor(w + c * RGB_CHUNK + 32 * k), 1u);
+                        mma_rs_n8(dr, act[4 * c + k], desc_kmajor(w_lo + c * RGB_CHUNK + 32 * k), 1u);
+                    }
             wg_commit();
             turn_end(TG_OUT_HEAD);
             wg_wait<0>();
@@ -691,6 +883,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) siren_fast_kernel(const __grid_co
             fence_regs(dr);
             fence_regs(act);
             release(slot);
+            if constexpr (kSplit) {
+                release(slot_lo);
+                const float us = __ldg(reinterpret_cast<const float*>(a.packed + L.split_scale) + FN_SPLIT_SCALES +
+                                       L.n_hidden + 2);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) dr[i] *= us;
+            }
             const float* rgb_b = reinterpret_cast<const float*>(a.packed + L.rgb.w) + rgb_rows * FN_H;
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {

@@ -11,7 +11,7 @@ point chunking (SURVEY.md section 8f-2).
 
 Hidden keyword extras (never passed by the reference's callers, used by tests and bench):
   _rng        an RNG source (volumetric_rendering.ReplayRng) instead of the device generator
-  precision   'exact' | 'fast' | 'guard' (default: ops.default_precision())
+  precision   'exact' | 'fast' | 'guard' | 'split' (default: ops.default_precision())
   _debug      dict that receives intermediate tensors (inds, depth, weights_sum, poses)
 """
 import warnings
@@ -36,7 +36,7 @@ class _RenderSkeleton:
         if staged:
             # EMA copy_to / restore write through .data: fingerprint-check the packed weights (host sync; the
             # staged methods end in .cpu() anyway)
-            self.siren.packed(verify=True)
+            self.siren.packed(verify=True, split=ops._precision_code(kwargs.get('precision')) == _lib.PRECISION['split'])
         n_rays = img_size * img_size
         n_samples = num_steps * 2 if hierarchical_sample else num_steps
         with torch.no_grad():

@@ -98,7 +98,8 @@ def siren_points(module, points, film, ray_directions, precision=None, dir_group
     """
     if needs_grad(module, points, film):
         raise NotImplementedError(GRAD_MESSAGE)
-    packed = module.packed()
+    code = _precision_code(precision)
+    packed = module.packed(split=code == _lib.PRECISION['split'])
     device = packed.device
     pts = _prep(points, device)
     flm = _prep(film, device)
@@ -121,7 +122,7 @@ def siren_points(module, points, film, ray_directions, precision=None, dir_group
     with torch.cuda.device(device):
         _lib.check(_lib.lib().fenerf_siren_points(
             C.byref(packed.desc), packed.ptr, _chk(pts, "points"), _chk(dirs, "ray_directions"), _chk(flm, "film"),
-            b, p, dir_group, _precision_code(precision) | (POINTS_SIGMA_ONLY if _sigma_only else 0), idx_ptr, n_only,
+            b, p, dir_group, code | (POINTS_SIGMA_ONLY if _sigma_only else 0), idx_ptr, n_only,
             _chk(out, "out"), _stream(device)))
     return out
 
@@ -283,7 +284,7 @@ def guard_stats(device):
 def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
                    want_depth=True, want_weights_sum=True, want_weights=False, want_inds=False):
     """One call into fenerf_render_forward: the whole render after the mapping network."""
-    packed = module.packed()
+    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
     device = packed.device
     lib = _lib.lib()
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
@@ -318,7 +319,7 @@ def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb
 def render_forward_stages(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f):
     """fenerf_render_forward into a PRIVATE workspace, returned together with typed views of the intermediates
     it leaves there (fenerf_workspace_layout): what the backward consumes (fenerf_b200/backward.py)."""
-    packed = module.packed()
+    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
     device = packed.device
     lib = _lib.lib()
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps

@@ -34,7 +34,7 @@ class PackedField:
                 cur.wait_event(self.event)
 
 
-def field_desc(spec) -> "_lib.FieldDesc":
+def field_desc(spec, split=False) -> "_lib.FieldDesc":
     return _lib.FieldDesc(trunk_layers=spec.trunk_layers, color_layers=spec.color_layers, label_dim=spec.label_dim,
                           grid_channels=spec.grid_channels, grid_res=spec.grid_res, out_dim=spec.out_dim,
                           input_scale=spec.input_scale,
@@ -43,7 +43,8 @@ def field_desc(spec) -> "_lib.FieldDesc":
                           | (_lib.FIELD_GRID_TRUNK if spec.grid_trunk else 0)
                           | (_lib.FIELD_BRIDGE if spec.bridge else 0)
                           | (_lib.FIELD_BRIDGE_RES if spec.bridge_res else 0)
-                          | (_lib.FIELD_WO_DIR if spec.wo_dir else 0))
+                          | (_lib.FIELD_WO_DIR if spec.wo_dir else 0)
+                          | (_lib.FIELD_SPLIT_IMAGES if split else 0))
 
 
 def _f32(t, device):
@@ -120,13 +121,15 @@ def _bridge_ref(bridge):
     return C.byref(bridge) if bridge is not None else None
 
 
-def pack_field(module) -> PackedField:
+def pack_field(module, split=False) -> PackedField:
+    """split=True: the layout with the fp16 low parts of the weight images that precision='split' reads
+    (FENERF_FIELD_SPLIT_IMAGES)."""
     lib = _lib.lib()
     device = next(module.parameters()).device
     if device.type != "cuda":
         raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to an H100 (got %s)" % device)
     spec = module.field_spec()
-    desc = field_desc(spec)
+    desc = field_desc(spec, split)
     nbytes = lib.fenerf_packed_bytes(C.byref(desc))
     if nbytes == 0:
         _lib.check(-1)

@@ -163,7 +163,7 @@ class FieldSpec:
                    Linears on v and the first colour layer reads cat[ray_dir, Linear(3 -> 256)(v)] (siren/siren.py:1072-1076)
     wo_dir         the first colour layer reads cat[grid_feat, trunk_out(256)], no ray direction, and carries the U(+-1/3)
                    init (siren/siren.py:1606, 1626), which amplifies the fp16 trunk's error: the colours come from the exact
-                   kernel only (the density alone runs in any precision)
+                   and the split-precision kernels only (the density alone runs in any precision)
     out_dim        label_dim + 3 (rgb; 64 features with feature_head) + 1 (sigma); channel order [labels, rgb, sigma]
     """
     trunk_layers: int
@@ -216,17 +216,20 @@ class _FieldBase(nn.Module):
     def _weights_version(self):
         return tuple((p.data_ptr(), p._version) for p in self._field_parameters())
 
-    def packed(self, verify=False):
+    def packed(self, verify=False, split=False):
         """Kernel-layout weights.  Repacked when a parameter's (storage, version) changed -- what optimizer
         steps and in-place torch ops bump.  Writes through ``param.data`` (torch_ema ``copy_to`` / ``restore``,
         train_double_latent_semantic.py:464-522) bump nothing: ``verify=True`` compares a device-side
         fingerprint of the raw parameters with the one taken at pack time (one kernel + a 16-byte read-back,
         so a host sync) -- the generators pass it from ``staged_forward*``, the methods the reference renders
         EMA weights through, whose outputs go to the CPU anyway.  :meth:`invalidate_packed` forces a repack.
+        ``split=True``: the pack precision='split' reads, which also holds the fp16 low parts of the weight images
+        (FENERF_FIELD_SPLIT_IMAGES); cached beside the other under the same rules and made on first use only.
         """
         from .. import packing
+        key = '_packed_split_cache' if split else '_packed_cache'
         ver = self._weights_version()
-        cache = self.__dict__.get('_packed_cache')
+        cache = self.__dict__.get(key)
         if cache is not None and cache[0] == ver and verify:
             fp = packing.fingerprint(self)
             if cache[1].fingerprint is None:
@@ -236,20 +239,22 @@ class _FieldBase(nn.Module):
             elif cache[1].fingerprint != fp:
                 cache = None
         if cache is None or cache[0] != ver:
-            cache = (ver, packing.pack_field(self))
+            cache = (ver, packing.pack_field(self, split))
             if verify:
                 cache[1].fingerprint = packing.fingerprint(self)
-            self.__dict__['_packed_cache'] = cache
+            self.__dict__[key] = cache
         cache[1].wait_ready()
         return cache[1]
 
     def invalidate_packed(self):
         """Drop the kernel-layout copy of the weights (next render repacks)."""
         self.__dict__.pop('_packed_cache', None)
+        self.__dict__.pop('_packed_split_cache', None)
 
     def __getstate__(self):
         state = self.__dict__.copy()
         state.pop('_packed_cache', None)  # never pickle device buffers derived from the weights
+        state.pop('_packed_split_cache', None)
         state.pop('_field_plist', None)
         return state
 

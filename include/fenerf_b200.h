@@ -110,7 +110,14 @@ extern "C" {
                                          with this bit is FENERF_E_UNSUPPORTED.  The directions are still passed; the
                                          outputs do not depend on them.  The colours are computed by FENERF_PRECISION_EXACT
                                          only: FAST / GUARD return FENERF_E_UNSUPPORTED unless FENERF_POINTS_SIGMA_ONLY (the
-                                         first colour layer's U(+-1/3) weights amplify the fp16 trunk's error to ~2e-2). */
+                                         first colour layer's U(+-1/3) weights amplify the fp16 trunk's error to ~2e-2).
+                                         FENERF_PRECISION_SPLIT computes them on the tensor cores as well. */
+#define FENERF_FIELD_SPLIT_IMAGES 0x40 /* a packing option, not a field shape: the packed layout also holds the fp16 low
+                                         parts w - f16(w) of every 256-wide layer image, of the first colour layer's feature
+                                         columns and of both heads, appended after every other section (no section moves,
+                                         the fingerprint is the same).  FENERF_PRECISION_SPLIT needs a pack made with it.
+                                         Not built for FENERF_FIELD_LABEL_FILM, _FEATURE_HEAD, _GRID_TRUNK or _BRIDGE
+                                         fields (FENERF_E_UNSUPPORTED). */
 
 typedef struct fenerf_field_desc {
     int32_t trunk_layers;   /* 2..8 */
@@ -185,6 +192,11 @@ int fenerf_field_fingerprint_bridge(const fenerf_field_desc* field, const fenerf
 #define FENERF_PRECISION_GUARD 2  /* FAST, then EXACT re-evaluation of the far sample of every ray
                                      whose |sigma| < guard_tau (the reference's delta=1e10 step,
                                      volumetric_rendering.py:24,32) -- the default                */
+#define FENERF_PRECISION_SPLIT 3  /* fp32-accurate on the tensor cores: fp16 hi / lo operands on wgmma with fp32
+                                     accumulation, three products hi*W_hi + lo*W_hi + hi*W_lo per 256-wide layer and
+                                     per head, every sine through a software sine (2^-20 absolute), no GUARD pass.
+                                     Needs a pack made with FENERF_FIELD_SPLIT_IMAGES; not with only_idx; not for
+                                     label FiLM, feature-head, grid-trunk or bridge fields (FENERF_E_UNSUPPORTED). */
 
 /* Evaluates the field at arbitrary points.
  * Replaces <SIREN>.forward_with_frequencies_phase_shifts (siren/siren.py:164-178, 1509-1530);
