@@ -160,17 +160,35 @@ def _film(linear, x, freq, phase):
 
 
 def grid_lookup(coords, grid):
-    # sample_from_3dgrid, siren.py:314-330
+    # sample_from_3dgrid, siren.py:314-330: in fp32 as the reference samples, except that float64 coordinates (the
+    # float64 references) sample in float64
+    dtype = torch.float64 if coords.dtype == torch.float64 else torch.float32
     b, n, d = coords.shape
-    s = F.grid_sample(grid.float().expand(b, -1, -1, -1, -1), coords.float().reshape(b, 1, 1, -1, d), mode='bilinear',
+    s = F.grid_sample(grid.to(dtype).expand(b, -1, -1, -1, -1), coords.to(dtype).reshape(b, 1, 1, -1, d), mode='bilinear',
                       padding_mode='zeros', align_corners=True)
     nn_, c, h, w, dd = s.shape
     return s.permute(0, 4, 3, 2, 1).reshape(nn_, h * w * dd, c)
 
 
+_FEATURE_HEAD_CLASSES = ("SPATIALSIRENBASELINEHD", "SPATIALSIRENSEMANTICHD")
+_BRIDGE_CLASSES = ("SPATIALSIRENAUGDISENTANGLE", "RESSIRENDISENTANGLE")
+_WO_DIR_CLASSES = ("TextureEmbeddingPiGAN128SEMANTICDISENTANGLE_WO_DIR",
+                   "TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96")
+
+
 def field_eval(field, points, film, dirs):
     """(B,P,3), (B,L,2,256) [15f+30, phase], (B,P,3) -> (B,P,C).  `field` is any module with the
-    reference's attribute names (network, final_layer, color_layer_sine, ...)."""
+    reference's attribute names (network, final_layer, color_layer_sine, ...).  The field families whose
+    attributes do not tell them apart from the stock classes are chosen by class name."""
+    name = type(field).__name__
+    if name in _WO_DIR_CLASSES:
+        return wo_dir_field_eval(field, points, film, dirs)
+    if name in _BRIDGE_CLASSES:
+        return bridge_field_eval(field, points, film, dirs)
+    if name == "EmbeddingPiGAN256":
+        return grid_trunk_field_eval(field, points, film, dirs)
+    if name in _FEATURE_HEAD_CLASSES or hasattr(field, 'label_layer_sine'):
+        return label_film_field_eval(field, points, film, dirs)
     has_grid = hasattr(field, 'spatial_embeddings')
     has_labels = hasattr(field, 'label_layer_linear')
     x = points
@@ -192,6 +210,108 @@ def field_eval(field, points, film, dirs):
         c = _film(layer.layer, c, film[:, n_trunk + j, 0], film[:, n_trunk + j, 1])
     rgb = torch.sigmoid(field.color_layer_linear[0](c))
     return torch.cat([labels, rgb, sigma], dim=-1) if has_labels else torch.cat([rgb, sigma], dim=-1)
+
+
+# The field families below follow the same contract as field_eval.  Their `fault` keywords serve the fault
+# tests only (each applies one mistake the tests' bounds must catch); field_eval never passes one.
+def label_film_field_eval(field, points, film, dirs):
+    """The label FiLM branch (SPATIALSIRENSEMANTIC, siren.py:650-671) and the feature-head classes' 64-wide linear
+    colour head (SPATIALSIRENBASELINEHD, SPATIALSIRENSEMANTICHD, siren.py:298-302, 1358-1367): labels =
+    Linear(FiLM(trunk output; FiLM row len(network))) where the field has a label FiLM layer, the colour layer at the
+    next row; the feature heads take no sigmoid."""
+    x = points * (2 / 0.24)                                              # UniformBoxWarp(0.24), siren.py:653
+    h = x
+    n_trunk = len(field.network)
+    for i, layer in enumerate(field.network):
+        h = _film(layer.layer, h, film[:, i, 0], film[:, i, 1])
+    sigma = field.final_layer(h)
+    row = n_trunk
+    parts = []
+    if hasattr(field, 'label_layer_sine'):
+        parts.append(field.label_layer_linear(_film(field.label_layer_sine.layer, h, film[:, row, 0], film[:, row, 1])))
+        row += 1
+    c = _film(field.color_layer_sine.layer, torch.cat([dirs, h], dim=-1), film[:, row, 0], film[:, row, 1])
+    out = field.color_layer_linear[0](c)
+    parts.append(out if type(field).__name__ in _FEATURE_HEAD_CLASSES else torch.sigmoid(out))
+    return torch.cat(parts + [sigma], dim=-1)
+
+
+def grid_trunk_field_eval(field, points, film, dirs, fault=None):
+    """EmbeddingPiGAN256.forward_with_frequencies_phase_shifts (siren.py:392-408): the grid features sampled at the
+    box-warped position, the first layer on cat[feat, x], the colour layer on cat[dir, trunk output].
+    `fault`: 'no_feat' drops the features from layer 0 (zeros in their place), 'feat_in_colour' sends them to the
+    colour branch instead, 'no_warp' looks the grid up at the unwarped position."""
+    x = points * (2 / 0.24)                                          # UniformBoxWarp(0.24)
+    feats = grid_lookup(points if fault == "no_warp" else x, field.spatial_embeddings)
+    h = torch.cat([torch.zeros_like(feats) if fault in ("no_feat", "feat_in_colour") else feats, x], -1)
+    for i, layer in enumerate(field.network):
+        h = _film(layer.layer, h, film[:, i, 0], film[:, i, 1])
+    sigma = field.final_layer(h)
+    row = len(field.network)
+    c_in = torch.cat([dirs, h], dim=-1)
+    if fault == "feat_in_colour":       # the first colour weights' last 32 columns meet the features instead of h's
+        c_in = torch.cat([dirs, h[..., :-32], feats], dim=-1)
+    c = _film(field.color_layer_sine.layer, c_in, film[:, row, 0], film[:, row, 1])
+    rgb = torch.sigmoid(field.color_layer_linear[0](c))
+    return torch.cat([rgb, sigma], dim=-1)
+
+
+def bridge_field_eval(siren, pts, film, dirs, fault=None):
+    """The bridge fields' forward_with_frequencies_phase_shifts (SPATIALSIRENAUGDISENTANGLE, RESSIRENDISENTANGLE,
+    siren.py:958-979, 1063-1082): the colour branch starts from v, a 3-wide linear map of the trunk output (RES adds
+    the position and takes the density from v).  -> (B, P, 4) [rgb, sigma].
+    `fault`: 'no_bridge_bias' drops v's bias, 'no_pos' leaves the position out of RES's v, 'swap' swaps the direction
+    and v columns of the first colour layer's input, 'sigma_from_detached_v' computes RES's density from v.detach()
+    (its gradient then lacks d sigma . a)."""
+    x = pts * siren.gridwarper.scale_factor
+    h = x
+    for i, layer in enumerate(siren.network):
+        h = _film(layer.layer, h, film[:, i, 0], film[:, i, 1])
+    res = hasattr(siren, "res_coord_layer")
+    lin = siren.res_coord_layer if res else siren.color_layer_pre[0]
+    v = h @ lin.weight.t() + (0 if fault == "no_bridge_bias" else lin.bias)
+    if res:
+        v = v + (0 if fault == "no_pos" else x)
+        sigma = siren.density_layer_linear(v.detach() if fault == "sigma_from_detached_v" else v)
+        c_in = siren.color_layer_pre(v)
+    else:
+        sigma = siren.final_layer(h)
+        c_in = v
+    c = torch.cat([c_in, dirs] if fault == "swap" else [dirs, c_in], dim=-1)
+    row = len(siren.network)
+    for j, layer in enumerate(siren.color_layer_sine):
+        c = _film(layer.layer, c, film[:, row + j, 0], film[:, row + j, 1])
+    return torch.cat([torch.sigmoid(siren.color_layer_linear[0](c)), sigma], dim=-1)
+
+
+def wo_dir_field_eval(siren, pts, film, dirs, fault=None):
+    """The direction-free texture-grid fields' forward_with_frequencies_phase_shifts
+    (TextureEmbeddingPiGAN*SEMANTICDISENTANGLE_WO_DIR*, siren.py:1618-1640): the first colour layer reads cat[feat, h],
+    no direction.  -> (B, P, 22) [labels, rgb, sigma].
+    `fault`: 'fp16_first_colour' rounds both operands of the first colour layer to fp16 (what the plain wgmma path
+    would do), 'with_dir' adds the direction through the layer's first three columns (B's layout read with non-zero
+    direction weights), 'feat_after_x' feeds cat[x, feat] instead of cat[feat, x]."""
+    x = pts * siren.gridwarper.scale_factor
+    feats = grid_lookup(x, siren.spatial_embeddings)
+    h = x
+    for i, layer in enumerate(siren.network):
+        h = _film(layer.layer, h, film[:, i, 0], film[:, i, 1])
+    sigma = siren.final_layer(h)
+    labels = siren.label_layer_linear(h)
+    c = torch.cat([h, feats] if fault == "feat_after_x" else [feats, h], dim=-1)
+    row = len(siren.network)
+    for j, layer in enumerate(siren.color_layer_sine):
+        f, p = film[:, row + j, 0], film[:, row + j, 1]
+        if j == 0 and fault == "fp16_first_colour":
+            w = layer.layer.weight
+            z = c.to(torch.float16).to(c.dtype) @ w.to(torch.float16).to(w.dtype).t() + layer.layer.bias
+            c = torch.sin(f.unsqueeze(1) * z + p.unsqueeze(1))
+        elif j == 0 and fault == "with_dir":
+            z = layer.layer(c) + dirs @ layer.layer.weight[:, :3].t()
+            c = torch.sin(f.unsqueeze(1) * z + p.unsqueeze(1))
+        else:
+            c = _film(layer.layer, c, f, p)
+    return torch.cat([labels, torch.sigmoid(siren.color_layer_linear[0](c)), sigma], dim=-1)
 
 
 # --------------------------------------------------------------------------------------------

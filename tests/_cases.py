@@ -33,6 +33,15 @@ MODELS = {
     "F": ("ImplicitGenerator3d", "SPATIALSIRENBASELINESEMANTIC", 1, 23),
     "G": ("DoubleImplicitGenerator3d", "SPATIALSIRENDISENTANGLE", 2, 4),
     "H": ("DoubleImplicitGenerator3d", "SPATIALSIRENSEMANTICDISENTANGLE", 2, 22),
+    # the field families: label FiLM (23 channels whatever output_dim says), the feature heads (65 / 129 channels
+    # likewise), the grid in the density trunk, the two bridge fields, and B's sibling without the direction
+    "I": ("ImplicitGenerator3d", "SPATIALSIRENSEMANTIC", 1, 23),
+    "J": ("ImplicitGenerator3d", "SPATIALSIRENBASELINEHD", 1, 65),
+    "K": ("ImplicitGenerator3d", "SPATIALSIRENSEMANTICHD", 1, 129),
+    "L": ("ImplicitGenerator3d", "EmbeddingPiGAN256", 1, 4),
+    "M": ("DoubleImplicitGenerator3d", "SPATIALSIRENAUGDISENTANGLE", 2, 4),
+    "N": ("DoubleImplicitGenerator3d", "RESSIRENDISENTANGLE", 2, 4),
+    "P": ("DoubleImplicitGenerator3d", "TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96", 2, 22),
 }
 
 
@@ -57,7 +66,7 @@ class Case:
     seed: int
     cfg: dict = field(default_factory=dict)
     method: str = "forward"        # or "staged_forward"
-    sigma_bias_shift: float = 0.0  # final_layer.bias += shift (opaque-regime fixture, SURVEY.md 7.1)
+    sigma_bias_shift: float = 0.0  # density bias += shift (opaque-regime fixture, SURVEY.md 7.1; apply_weight_edits)
     psi: float = 1.0
 
 
@@ -131,8 +140,91 @@ CASES = [
 #: cases whose CPU oracle run takes tens of seconds: the CPU suite (-m "not gpu") checks them only with
 #: FENERF_SLOW_TESTS=1; the GPU suite always runs them
 BIG_CASES = ("b_cfg2", "a_cfg5")
-CASE_BY_NAME = {c.name: c for c in CASES}
+
+# ---- the field families' cases (each family's tests and golden generator parametrise over its own list) ----
+LABEL_FILM_CASES = [
+    Case("i_small", "I", 2, 71, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("i_small_opaque", "I", 1, 72, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    # (the reference's seg_padding_background fill writes a hard-coded 22-vector, volumetric_rendering.py:77: it cannot
+    # run at this field's 23 channels, so the staged case uses the weight fill)
+    Case("i_staged_softmax", "I", 1, 73, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
+                                              softmax_label=True, fill_mode='weight'), method="staged_forward", psi=0.7),
+    # one cfg2-shaped render (128², 24 + 24); its golden keeps a fixed probe of the pixels (see pixel_probe_index)
+    Case("i_cfg2", "I", 1, 74, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+]
+FEATURE_HEAD_CASES = [
+    Case("j_small", "J", 2, 81, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("j_small_opaque", "J", 1, 82, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    Case("k_small", "K", 2, 91, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("k_small_opaque", "K", 1, 92, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    # softmax over the 125 channels before the last three (the reference's pixels[..., :-3] split) and the weight fill;
+    # the coloured seg-padding / debug fills assign a 22- or 3-vector in the reference and cannot run at these widths
+    Case("k_staged_softmax", "K", 1, 93, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
+                                              softmax_label=True, fill_mode='weight'), method="staged_forward", psi=0.7),
+    # an img_feat_size-like render (64², 24 + 24); its golden keeps a fixed probe of the pixels
+    Case("k_feat64", "K", 1, 94, _cfg(img_size=64, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+]
+GRID_TRUNK_CASES = [
+    Case("l_small", "L", 2, 101, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("l_small_opaque", "L", 1, 102, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    # the fill of the CelebA curriculum's evaluation renders; opaque, so that the field shows through the white fill
+    Case("l_staged_white", "L", 1, 103, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
+                                             fill_mode='eval_white_back'), method="staged_forward", psi=0.7,
+         sigma_bias_shift=0.5),
+    # the benchmarked shape (128², 24 + 24); its golden keeps a fixed probe of the pixels
+    Case("l_cfg2", "L", 1, 104, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+]
+BRIDGE_CASES = [
+    Case("m_small", "M", 2, 201, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("m_small_opaque", "M", 1, 202, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    Case("m_staged_white", "M", 1, 203, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
+                                             fill_mode='eval_white_back'), method="staged_forward", psi=0.7,
+         sigma_bias_shift=0.5),
+    Case("n_small", "N", 2, 211, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    # RES has no final_layer: its opaque fixture shifts the density chain's last bias (apply_weight_edits)
+    Case("n_small_opaque", "N", 1, 212, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    Case("n_staged_white", "N", 1, 213, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
+                                             fill_mode='eval_white_back'), method="staged_forward", psi=0.7,
+         sigma_bias_shift=0.5),
+    # the benchmarked shape (128², 24 + 24); its golden keeps a fixed probe of the pixels
+    Case("n_cfg2", "N", 1, 214, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+]
+WO_DIR_CASES = [
+    Case("p_small", "P", 2, 301, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("p_small_opaque", "P", 1, 302, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
+         sigma_bias_shift=0.5),
+    # (the reference's eval_white_back fill assumes three channels; a labelled field's white fill is the seg-padding one)
+    Case("p_staged_white", "P", 1, 303, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
+                                             fill_mode='eval_seg_padding_background', fill_color='white'),
+         method="staged_forward", psi=0.7, sigma_bias_shift=0.5),
+    # the benchmarked shape (128², 24 + 24); its golden keeps a fixed probe of the pixels
+    Case("p_cfg2", "P", 1, 304, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+]
+#: every case, stock or family, by name
+CASE_BY_NAME = {c.name: c for c in (CASES + LABEL_FILM_CASES + FEATURE_HEAD_CASES + GRID_TRUNK_CASES + BRIDGE_CASES
+                                    + WO_DIR_CASES)}
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+#: entries of the flattened pixels a probed golden (a cfg2-shaped family render) stores instead of every pixel
+PROBE = 32768
+
+
+def pixel_probe_index(numel, n=PROBE):
+    """Fixed pseudo-random flat indices into a rendered frame batch (the probed goldens store only these entries)."""
+    g = torch.Generator().manual_seed(11)
+    return torch.randint(0, numel, (n,), generator=g)
+
+
+def probe_of(pixels):
+    """(B, C, R, R) -> the PROBE entries a probed golden stores."""
+    flat = pixels.reshape(-1)
+    return flat[pixel_probe_index(flat.numel())]
 
 
 def golden_path(case):
@@ -140,9 +232,14 @@ def golden_path(case):
 
 
 def apply_weight_edits(gen, case):
+    """The opaque fixture: the density bias += sigma_bias_shift -- final_layer's, or the last of RES's density chain
+    (RESSIRENDISENTANGLE has no final_layer)."""
     if case.sigma_bias_shift:
         with torch.no_grad():
-            gen.siren.final_layer.bias += case.sigma_bias_shift
+            if hasattr(gen.siren, "final_layer"):
+                gen.siren.final_layer.bias += case.sigma_bias_shift
+            else:
+                gen.siren.density_layer_linear[3].bias += case.sigma_bias_shift
 
 
 def make_latents(case):

@@ -169,20 +169,10 @@ def composite_ref(raw_c, z_c, raw_f, z_f, noise, opt, offset=None, full=False):
     return px, depth[..., 0], wsum[..., 0], weights[..., 0]
 
 
-def _grid_lookup_keep_dtype(coords, grid):
-    """oracle.grid_lookup without its .float() casts (the oracle itself stays pinned bit for bit to the reference)."""
-    b, n, d = coords.shape
-    s = F.grid_sample(grid.expand(b, -1, -1, -1, -1), coords.reshape(b, 1, 1, -1, d), mode='bilinear',
-                      padding_mode='zeros', align_corners=True)
-    nn_, c, h, w, dd = s.shape
-    return s.permute(0, 4, 3, 2, 1).reshape(nn_, h * w * dd, c)
-
-
-def field_ref(siren, monkeypatch, points, dirs_pp, film, d_raw=None, film_rows=None, chunk=1 << 15):
+def field_ref(siren, points, dirs_pp, film, d_raw=None, film_rows=None, chunk=1 << 15):
     """oracle.field_eval on a float64 copy of `siren`, on the tensors' device, in point chunks.
     -> (out (B, P, C) float64, d_film, {parameter name: float64 gradient}); the gradients (the VJP with d_raw, accumulated
     over the chunks) only when d_raw is given.  film_rows: image index whose FiLM rows each image uses (fault checks)."""
-    monkeypatch.setattr(oracle, "grid_lookup", _grid_lookup_keep_dtype)
     ref = copy.deepcopy(siren).double()
     want_grad = d_raw is not None
     film64 = film.double().requires_grad_(want_grad)

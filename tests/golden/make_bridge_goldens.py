@@ -65,7 +65,7 @@ def forward_goldens(ref_generators, ref_siren):
                 pixels, depth = res[0], res[1]
                 extra = {"depth_map": depth.numpy()}
         if case.name in BF.PROBED:
-            extra.update(pixel_probe=BF.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
+            extra.update(pixel_probe=_cases.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
                          pixels_shape=np.array(pixels.shape))
         else:
             extra["pixels"] = pixels.numpy()
@@ -79,7 +79,7 @@ def _loss(pixels):
 
 def grad_goldens(ref_generators, ref_siren):
     for name in BF.GRAD_CASES:
-        case = BF.CASE_BY_NAME[name]
+        case = _cases.CASE_BY_NAME[name]
         gen, _ = make_goldens.build_reference(case, ref_generators, ref_siren)
         latents = tuple(z.clone().requires_grad_(True) for z in _cases.make_latents(case))
         torch.manual_seed(case.seed)
@@ -127,12 +127,11 @@ def dropin_goldens(ref_generators, ref_siren):
 if __name__ == "__main__":
     ref_generators, ref_siren, _ = ref_shim.load()
     which = sys.argv[1:2]
-    with BF.with_bridge():
-        if which in ([], ["--init"]):
-            init_goldens(ref_siren)
-        if which in ([], ["--forward"]):
-            forward_goldens(ref_generators, ref_siren)
-        if which in ([], ["--grads"]):
-            grad_goldens(ref_generators, ref_siren)
-        if which in ([], ["--dropin"]):
-            dropin_goldens(ref_generators, ref_siren)
+    if which in ([], ["--init"]):
+        init_goldens(ref_siren)
+    if which in ([], ["--forward"]):
+        forward_goldens(ref_generators, ref_siren)
+    if which in ([], ["--grads"]):
+        grad_goldens(ref_generators, ref_siren)
+    if which in ([], ["--dropin"]):
+        dropin_goldens(ref_generators, ref_siren)

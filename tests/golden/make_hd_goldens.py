@@ -41,7 +41,7 @@ def forward_goldens(ref_generators, ref_siren):
                 pixels, depth, _ = gen.staged_forward(*latents, **kw)
                 extra = {"depth_map": depth.numpy()}
         if case.name in _hd_fields.PROBED:
-            extra.update(pixel_probe=_hd_fields.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
+            extra.update(pixel_probe=_cases.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
                          pixels_shape=np.array(pixels.shape))
         else:
             extra["pixels"] = pixels.numpy()
@@ -57,7 +57,7 @@ def _loss(pixels):
 
 def grad_goldens(ref_generators, ref_siren):
     for model, name in (("J", "j_small"), ("K", "k_small")):
-        case = _hd_fields.CASE_BY_NAME[name]
+        case = _cases.CASE_BY_NAME[name]
         gen, _ = make_goldens.build_reference(case, ref_generators, ref_siren)
         latents = tuple(z.clone().requires_grad_(True) for z in _cases.make_latents(case))
         torch.manual_seed(case.seed)
@@ -70,7 +70,7 @@ def grad_goldens(ref_generators, ref_siren):
         np.savez_compressed(os.path.join(HERE, "grad_%s.npz" % name), **out)
         print("grad_%s: loss %.6f" % (name, loss.item()))
 
-    case = _hd_fields.CASE_BY_NAME["k_small"]
+    case = _cases.CASE_BY_NAME["k_small"]
     gen, _ = make_goldens.build_reference(case, ref_generators, ref_siren)
     with torch.no_grad():
         fp = [t.clone().requires_grad_(True) for t in gen.siren.mapping_network(_cases.make_latents(case)[0])]

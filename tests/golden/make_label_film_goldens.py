@@ -41,7 +41,7 @@ def forward_goldens(ref_generators, ref_siren):
                 pixels, depth, _ = gen.staged_forward(*latents, **kw)
                 extra = {"depth_map": depth.numpy()}
         if case.name in _label_film.PROBED:
-            extra.update(pixel_probe=_label_film.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
+            extra.update(pixel_probe=_cases.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
                          pixels_shape=np.array(pixels.shape))
         else:
             extra["pixels"] = pixels.numpy()
@@ -56,7 +56,7 @@ def _loss(pixels):
 
 
 def grad_goldens(ref_generators, ref_siren):
-    case = _label_film.CASE_BY_NAME["i_small"]
+    case = _cases.CASE_BY_NAME["i_small"]
     gen, _ = make_goldens.build_reference(case, ref_generators, ref_siren)
     latents = tuple(z.clone().requires_grad_(True) for z in _cases.make_latents(case))
     torch.manual_seed(case.seed)

@@ -36,11 +36,9 @@ def init_goldens(ref_siren):
 
 
 class _Cases:
-    """The shape make_bridge_goldens' forward / gradient writers read (CASES, PROBED, probe_of, GRAD_CASES, ...)."""
+    """The shape make_bridge_goldens' forward / gradient writers read (CASES, PROBED, GRAD_CASES, GRAD_PARAMS)."""
     CASES = WF.CASES
-    CASE_BY_NAME = WF.CASE_BY_NAME
     PROBED = WF.PROBED
-    probe_of = staticmethod(WF.probe_of)
     GRAD_CASES = (WF.GRAD_CASE,)
     GRAD_PARAMS = {"P": WF.GRAD_PARAMS}
 
@@ -49,10 +47,9 @@ if __name__ == "__main__":
     ref_generators, ref_siren, _ = ref_shim.load()
     which = sys.argv[1:2]
     MB.BF = _Cases
-    with WF.with_wo_dir():
-        if which in ([], ["--init"]):
-            init_goldens(ref_siren)
-        if which in ([], ["--forward"]):
-            MB.forward_goldens(ref_generators, ref_siren)
-        if which in ([], ["--grads"]):
-            MB.grad_goldens(ref_generators, ref_siren)
+    if which in ([], ["--init"]):
+        init_goldens(ref_siren)
+    if which in ([], ["--forward"]):
+        MB.forward_goldens(ref_generators, ref_siren)
+    if which in ([], ["--grads"]):
+        MB.grad_goldens(ref_generators, ref_siren)

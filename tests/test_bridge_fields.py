@@ -123,7 +123,8 @@ def test_faults_move_the_restatement_past_the_bounds(name, fault):
     with torch.no_grad():     # a bias of v a dropped one visibly moves (the default init's is U(+-1/16))
         lin = siren.res_coord_layer if name == "RESSIRENDISENTANGLE" else siren.color_layer_pre[0]
         lin.bias.copy_(torch.tensor([0.1, -0.1, 0.1], dtype=lin.bias.dtype))
-        good, bad = BF.restated(siren, pts, film, dirs), BF.restated(siren, pts, film, dirs, fault=fault)
+        good = oracle.bridge_field_eval(siren, pts, film, dirs)
+        bad = oracle.bridge_field_eval(siren, pts, film, dirs, fault=fault)
     assert (good - bad).abs().max() > FWD_BOUND["fast"]
 
 
@@ -131,7 +132,7 @@ def test_restatement_runs_the_mirror_forward():
     """The mirror's module structure is what the restatement reads: every parameter meets the output."""
     for name in BF.CLASSES:
         siren, film, pts, dirs = _cpu_inputs(name, 3, n=8, scaled=name == "RESSIRENDISENTANGLE")
-        out = BF.restated(siren, pts, film, dirs)
+        out = oracle.bridge_field_eval(siren, pts, film, dirs)
         out.sum().backward()
         missing = [n for n, p in siren.named_parameters() if "mapping" not in n and (p.grad is None or p.grad.abs().max() == 0)]
         assert missing == [], missing
@@ -142,11 +143,11 @@ def _c0_freqs_of_image0(field, points, film, dirs):
     c0 = len(field.network)
     f = film.clone()
     f[1:, c0, 0] = film[0, c0, 0]
-    return BF.field_eval(field, points, f, dirs)
+    return oracle.bridge_field_eval(field, points, f, dirs)
 
 
 def _sigma_from_detached_v(field, points, film, dirs):
-    return BF.restated(field, points, film, dirs, fault="sigma_from_detached_v")
+    return oracle.bridge_field_eval(field, points, film, dirs, fault="sigma_from_detached_v")
 
 
 _BWD_FAULTS = [("aug", "c0_freqs_of_image0"), ("res_scaled", "c0_freqs_of_image0"), ("res_scaled", "sigma_from_detached_v"),
@@ -165,16 +166,15 @@ def test_backward_faults_exceed_the_bounds(monkeypatch, model, fault):
     pts, dirs = _field_points(batch, ppb, dir_group, 13)
     film = _film(siren, batch, 13, edges=True)
     d_raw = torch.randn(batch, ppb, 4, generator=torch.Generator().manual_seed(13)) * 1e-3
-    monkeypatch.setattr(oracle, "field_eval", BF.field_eval)
-    _, film_g, good = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    _, film_g, good = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
     if fault == "dirs_one_ray_off":
         shifted = dirs.clone()
         half = dirs.shape[1] // 2
         shifted[1, half:-1] = dirs[1, half + 1:]
-        _, film_b, bad = field_ref(siren, monkeypatch, pts, _per_point(shifted, ppb, False), film, d_raw)
+        _, film_b, bad = field_ref(siren, pts, _per_point(shifted, ppb, False), film, d_raw)
     else:
         monkeypatch.setattr(oracle, "field_eval", _c0_freqs_of_image0 if fault == "c0_freqs_of_image0" else _sigma_from_detached_v)
-        _, film_b, bad = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+        _, film_b, bad = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
     errs = _grad_errors(film_b, bad, film_g, good)
     worst = max(errs, key=errs.get)
     print("bridge backward fault %s %s: %s moves %.3g" % (model, fault, worst, errs[worst]))
@@ -206,7 +206,7 @@ def _gpu_inputs(name, scaled, batch, ppb, seed=7):
 def _want(siren, film, pts, dirs):
     s64 = copy.deepcopy(siren).double()
     with torch.no_grad():
-        return BF.restated(s64, pts.double(), film.double(), dirs.double())
+        return oracle.bridge_field_eval(s64, pts.double(), film.double(), dirs.double())
 
 
 @pytest.mark.gpu
@@ -278,13 +278,12 @@ def test_backward_matches_float64_autograd(monkeypatch, layout, model, lock, edg
     exact = precision == "exact"
     if exact:
         monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)     # exact mode's torch.mm stays fp32
-    monkeypatch.setattr(oracle, "field_eval", BF.field_eval)
     siren = _bridge_siren(model, DEV)
     seed = 5000 + 10 * _IDS.index(model) + int(layout[1])
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film, planted = FE._edge_film(siren, batch, seed, FE.BACKWARD_FREQS) if edges else (_film(siren, batch, seed, edges=True), [])
     d_raw = torch.randn(batch, ppb, 4, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, lock), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, lock), film, d_raw)
     raw = out64.float().contiguous()
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
@@ -354,7 +353,7 @@ def test_oracle_matches_reference_golden(case):
     if case.name in BF.BIG and not os.environ.get("FENERF_SLOW_TESTS") and not torch.cuda.is_available():
         pytest.skip("minutes of CPU oracle (FENERF_SLOW_TESTS=1 runs it)")
     gold = np.load(_cases.golden_path(case))
-    run = BF.oracle_run(case, keep_stages=False)
+    run = _harness.oracle_run(case, keep_stages=False)
     got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
     assert (got - want).abs().max() <= 2e-5
 
@@ -385,8 +384,8 @@ def runs():
 
     def get(name):
         if name not in cache:
-            case = BF.CASE_BY_NAME[name]
-            cache[name] = (case, BF.oracle_run(case))
+            case = _cases.CASE_BY_NAME[name]
+            cache[name] = (case, _harness.oracle_run(case))
         return cache[name]
     return get
 
@@ -399,9 +398,8 @@ def test_end_to_end_against_reference_golden(runs, case, precision, tol):
     from test_hd_fields import _golden_pixels
     gold = np.load(_cases.golden_path(case))
     case, run = runs(case.name)
-    with BF.with_bridge():
-        gen, pixels, poses, depth_map = p._end_to_end(case, run, precision)
-        ill_rays = p._ill_conditioned_pixels(case, run)
+    gen, pixels, poses, depth_map = p._end_to_end(case, run, precision)
+    ill_rays = p._ill_conditioned_pixels(case, run)
     got, want, idx = _golden_pixels(pixels, gold)
     err = (got - want).abs()
     assert int(ill_rays.sum()) <= max(2, 0.002 * ill_rays.numel())
@@ -424,8 +422,7 @@ def test_generator_gradients_match_reference(runs, name, precision):
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
     case, run = runs(name)
     gold = np.load(os.path.join(GOLDEN, "grad_%s.npz" % name))
-    with BF.with_bridge():
-        gen = _cases.build_mirror(case, DEV)
+    gen = _cases.build_mirror(case, DEV)
     latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
     pixels, _ = gen(*latents, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision=precision))
     (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
@@ -443,8 +440,7 @@ def test_inversion_gradients_through_forward_with_frequencies(runs, name):
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
     case, run = runs(name)
     gold = np.load(os.path.join(GOLDEN, "gradfreq_%s.npz" % name))
-    with BF.with_bridge():
-        gen = _cases.build_mirror(case, DEV)
+    gen = _cases.build_mirror(case, DEV)
     with torch.no_grad():
         lat = [p._cuda(z) for z in run["latents"]]
         fp = [t.clone().requires_grad_(True) for t in gen.siren.geo_mapping_network(lat[0]) + gen.siren.app_mapping_network(lat[1])]
@@ -463,9 +459,8 @@ def test_staged_forward_sees_bridge_parameter_writes(name):
     """torch_ema's copy_to writes through param.data without a version bump: a write to v's Linear alone -- and, for RES,
     to color_layer_pre or the density chain alone -- must reach staged_forward (the fingerprint covers them)."""
     model = "M" if name == BF.CLASSES[0] else "N"
-    case = BF.CASE_BY_NAME["%s_small_opaque" % model.lower()]
-    with BF.with_bridge():
-        gen = _cases.build_mirror(case, DEV)
+    case = _cases.CASE_BY_NAME["%s_small_opaque" % model.lower()]
+    gen = _cases.build_mirror(case, DEV)
     s = gen.siren
     targets = [s.color_layer_pre[0].weight] if model == "M" else [s.res_coord_layer.weight, s.color_layer_pre[0].weight,
                                                                    s.density_layer_linear[1].weight]

@@ -19,10 +19,8 @@ case gave NaN FiLM gradients at f = 0 in both precisions.
 import pytest
 import torch
 
-import _bridge_fields as BF        # registers models J, K, L, M, N; its field_eval covers every field class
 from _fp64 import EDGE_FREQS, _film, _siren, field_ref, film_rows, plant_frequencies
 from fenerf_b200 import backward, ops
-from oracle import render_oracle as oracle
 from test_gpu_fp64_reference import (FIELD_BOUND, FWD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward, _field_points,
                                      _grad_errors, _per_point)
 
@@ -81,12 +79,6 @@ def _planted_errors(d_film, grads, want_film, want, planted, layers):
     return errs
 
 
-def _field_eval_for(model):
-    """The restatements' chain (bridge -> grid trunk -> feature head -> label FiLM -> the stock oracle): for models A-H
-    it is the stock oracle itself."""
-    return BF.field_eval
-
-
 def _grad_bounds(names, precision):
     """FIELD_BOUND, except the exact mode's grid gradient of model L (test_grid_trunk.GRID_BOUND_EXACT)."""
     from test_grid_trunk import GRID_BOUND_EXACT
@@ -108,14 +100,13 @@ def test_field_backward_at_edge_frequencies(monkeypatch, layout, model, precisio
     exact = precision == "exact"
     if exact:
         monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
-    monkeypatch.setattr(oracle, "field_eval", _field_eval_for(model))
     siren = _siren(model, DEV)
     seed = 3000 + 10 * MODELS.index(model) + int(layout[1])
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film, planted = _edge_film(siren, batch, seed, BACKWARD_FREQS)
     out_dim = siren.field_spec().out_dim
     d_raw = torch.randn(batch, ppb, out_dim, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
     assert torch.isfinite(want_film).all() and all(torch.isfinite(g).all() for g in want.values())
     raw = out64.float().contiguous()
     if chunk:
@@ -143,10 +134,9 @@ def test_field_backward_at_edge_frequencies(monkeypatch, layout, model, precisio
 
 @gpu
 @pytest.mark.parametrize("model", MODELS)
-def test_point_network_at_edge_frequencies(monkeypatch, model):
+def test_point_network_at_edge_frequencies(model):
     """Both point-network kernels on the planted tables against float64 within FWD_BOUND, per output channel; at |f| =
     150 the pre-activations reach the hundreds (the fast kernel's sin.approx and its fp16 operands)."""
-    monkeypatch.setattr(oracle, "field_eval", _field_eval_for(model))
     siren = _siren(model, DEV)
     seed = 4000 + MODELS.index(model)
     batch, ppb = 2, 6000
@@ -154,7 +144,7 @@ def test_point_network_at_edge_frequencies(monkeypatch, model):
     film, _ = _edge_film(siren, batch, seed)
     with torch.no_grad():
         got = {p: ops.siren_points(siren, pts, film, dirs, precision=p) for p in ("exact", "fast")}
-    want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film)[0]
+    want = field_ref(siren, pts, _per_point(dirs, ppb, False), film)[0]
     err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in got.items()}
     print("edge forward %s: exact %.3g fast %.3g" % (model, err["exact"].max(), err["fast"].max()))
     for k in err:

@@ -33,7 +33,6 @@ import math
 import pytest
 import torch
 
-import _bridge_fields as BF        # registers models M, N
 from _fp64 import PAD_FILL_MODES, _film, _opt, _siren, composite_ref, field_ref
 from fenerf_b200 import _lib, ops
 from fenerf_b200.generators import volumetric_rendering as vr
@@ -290,12 +289,7 @@ def check_resample(x):
 def _far_fp64(name, b, n, s):
     """float64 densities of the far coarse samples of render `name` (its points do not depend on tau)."""
     x = render(name)
-    mp = pytest.MonkeyPatch()
-    try:
-        mp.setattr(oracle, "field_eval", BF.field_eval)         # the stock oracle's for the fields it covers
-        return field_ref(x["siren"], mp, x["points_c"][:, :, -1], x["dirs"], x["film"])[0][..., -1]
-    finally:
-        mp.undo()
+    return field_ref(x["siren"], x["points_c"][:, :, -1], x["dirs"], x["film"])[0][..., -1]
 
 
 def check_guard(x, tau):

@@ -27,7 +27,7 @@ import torch
 import torch.nn.functional as F
 
 import _cases
-from _fp64 import (EDGE_FREQS, _ZeroDraws, _film, _grid_lookup_keep_dtype, _opt, _rel, _siren, composite_ref, field_ref,
+from _fp64 import (EDGE_FREQS, _ZeroDraws, _film, _opt, _rel, _siren, composite_ref, field_ref,
                    noise_offset, plant_frequencies)
 from fenerf_b200 import _lib, backward, ops
 from oracle import render_oracle as oracle
@@ -143,18 +143,22 @@ def test_composite_reference_keeps_the_tie_rule_and_matches_the_oracle():
     assert (px.reshape(-1) - (want.double() * 2 - 1).reshape(-1)).abs().max() <= 1e-6
 
 
-def test_grid_lookup_swap_is_the_oracles_lookup():
+def test_grid_lookup_is_the_references_in_fp32_and_passes_gradcheck_in_float64():
+    """fp32 coordinates take the reference's sample_from_3dgrid (its .float() casts included) bit for bit; float64
+    coordinates sample in float64, which the float64 references differentiate."""
     g = torch.Generator().manual_seed(5)
     grid = torch.randn(1, 3, 4, 4, 4, generator=g)
     coords = torch.rand(2, 7, 3, generator=g) * 2.4 - 1.2
-    assert torch.equal(_grid_lookup_keep_dtype(coords, grid), oracle.grid_lookup(coords, grid))
-    assert torch.autograd.gradcheck(_grid_lookup_keep_dtype, (coords.double().requires_grad_(True),
-                                                            grid.double().requires_grad_(True)))
+    s = F.grid_sample(grid.float().expand(2, -1, -1, -1, -1), coords.float().reshape(2, 1, 1, -1, 3), mode='bilinear',
+                      padding_mode='zeros', align_corners=True)
+    assert torch.equal(s.permute(0, 4, 3, 2, 1).reshape(2, 7, 3), oracle.grid_lookup(coords, grid))
+    assert torch.autograd.gradcheck(oracle.grid_lookup, (coords.double().requires_grad_(True),
+                                                         grid.double().requires_grad_(True)))
 
 
 @pytest.mark.parametrize("model,edges", [("A", False), ("D", False), ("A", True), ("D", True)],
                          ids=["A", "D", "A-zero_tiny_f", "D-zero_tiny_f"])
-def test_field_reference_gradcheck(model, edges, monkeypatch):
+def test_field_reference_gradcheck(model, edges):
     """The float64 field VJP (every parameter and the FiLM table) on 2 points, checked in gradcheck's fast mode
     (random projections of the full Jacobian); with `edges`, every FiLM row also holds f = 0, -0, tiny and large |f|."""
     siren = _siren(model, "cpu")
@@ -162,7 +166,6 @@ def test_field_reference_gradcheck(model, edges, monkeypatch):
     if edges:
         film = plant_frequencies(film, range(film.shape[1]))[0]
     pts, dirs = _field_points(1, 2, 2, 7)
-    monkeypatch.setattr(oracle, "grid_lookup", _grid_lookup_keep_dtype)
     ref = copy.deepcopy(siren).double()
     names = [n for n, p in ref.named_parameters() if "mapping_network" not in n]
     params = dict(ref.named_parameters())
@@ -323,7 +326,7 @@ def test_field_backward_vs_fp64(monkeypatch, layout, model, precision, lock):
     film = _film(siren, batch, seed, edges=True)
     out_dim = siren.field_spec().out_dim
     d_raw = torch.randn(batch, ppb, out_dim, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, lock), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, lock), film, d_raw)
     raw = out64.float().contiguous()
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
@@ -365,7 +368,7 @@ def _forward_inputs(siren, layout, seed):
 @gpu
 @pytest.mark.parametrize("layout", _cases.TILE_LAYOUTS)
 @pytest.mark.parametrize("model", FIELD_MODELS)
-def test_point_network_vs_fp64(monkeypatch, model, layout):
+def test_point_network_vs_fp64(model, layout):
     """Both point-network kernels against oracle.field_eval in float64, per output channel, under tile schedules derived
     from the device's SM count (one pair per CTA, a lone tile in a second pair, two pairs per CTA with the last half
     empty, pairs across image borders); the density-only entry is bit-equal to the full fast evaluation."""
@@ -375,7 +378,7 @@ def test_point_network_vs_fp64(monkeypatch, model, layout):
         exact = ops.siren_points(siren, pts, film, dirs, precision="exact")
         fast = ops.siren_points(siren, pts, film, dirs, precision="fast")
         sigma = ops.siren_sigma(siren, pts, film, precision="fast")
-    want = field_ref(siren, monkeypatch, pts, _per_point(dirs, pts.shape[1], False), film)[0]
+    want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
     err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in (("exact", exact), ("fast", fast))}
     print("forward %s %s: exact %.3g fast %.3g" % (model, layout, err["exact"].max(), err["fast"].max()))
     assert torch.isfinite(fast).all()
@@ -454,19 +457,19 @@ def _cpu_field_case(model):
 
 
 @pytest.mark.parametrize("model", ["A", "D"])
-def test_field_backward_faults_exceed_the_bounds(monkeypatch, model):
+def test_field_backward_faults_exceed_the_bounds(model):
     """Image 0's FiLM rows used for every image (a wrong b0 in gemm_nt_film / _stash / _gate) and directions sliced one ray
     off in image 1's second point chunk (a wrong p0 // dir_group).  Both must exceed the default-mode bound; the
     direction fault must exceed the layout-invariance bound, which is the check that sees it in default mode."""
     siren, pts, dirs, film, d_raw = _cpu_field_case(model)
     batch, ppb = pts.shape[:2]
-    _, film_g, good = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
-    _, film_b, bad = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw, film_rows=[0] * batch)
+    _, film_g, good = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
+    _, film_b, bad = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw, film_rows=[0] * batch)
     moved_film = max(_grad_errors(film_b, bad, film_g, good).values())
     shifted = dirs.clone()
     half = dirs.shape[1] // 2
     shifted[1, half:-1] = dirs[1, half + 1:]
-    _, film_d, bad_d = field_ref(siren, monkeypatch, pts, _per_point(shifted, ppb, False), film, d_raw)
+    _, film_d, bad_d = field_ref(siren, pts, _per_point(shifted, ppb, False), film, d_raw)
     moved_dirs = max(_grad_errors(film_d, bad_d, film_g, good).values())
     print("field faults %s: film rows %.3g, directions %.3g" % (model, moved_film, moved_dirs))
     assert moved_film > 10 * FIELD_BOUND["default"], moved_film
@@ -474,20 +477,20 @@ def test_field_backward_faults_exceed_the_bounds(monkeypatch, model):
 
 
 @pytest.mark.parametrize("model", ["A", "D"])
-def test_forward_faults_exceed_the_bounds(monkeypatch, model):
+def test_forward_faults_exceed_the_bounds(model):
     """The neighbouring image's FiLM rows, and the bias of feature half 1 (features 128-255) left out of every FiLM
     layer: both must move some output channel past the fast kernel's bound."""
     siren, pts, dirs, film, _ = _cpu_field_case(model)
     dirs_pp = _per_point(dirs, pts.shape[1], False)
-    good = field_ref(siren, monkeypatch, pts, dirs_pp, film)[0]
-    swapped = field_ref(siren, monkeypatch, pts, dirs_pp, film, film_rows=[1, 0])[0]
+    good = field_ref(siren, pts, dirs_pp, film)[0]
+    swapped = field_ref(siren, pts, dirs_pp, film, film_rows=[1, 0])[0]
     no_bias = copy.deepcopy(siren)
     with torch.no_grad():
         layers = list(no_bias.network) + (list(no_bias.color_layer_sine) if isinstance(no_bias.color_layer_sine, torch.nn.ModuleList)
                                           else [no_bias.color_layer_sine])
         for layer in layers:
             layer.layer.bias[128:] = 0
-    dropped = field_ref(no_bias, monkeypatch, pts, dirs_pp, film)[0]
+    dropped = field_ref(no_bias, pts, dirs_pp, film)[0]
     moved = {k: float((v - good).abs().amax((0, 1)).max()) for k, v in (("film_rows", swapped), ("bias_half1", dropped))}
     print("forward faults %s: %s" % (model, moved))
     assert min(moved.values()) > 10 * FWD_BOUND["fast"], moved
@@ -529,7 +532,6 @@ def test_film_gradient_algebra_at_edge_frequencies(monkeypatch, model):
     """finish()'s FiLM-gradient algebra, restated from float64 autograd pieces (each layer's input and dL/du), equals
     the autograd gradients of the FiLM table and of every FiLM layer's weight and bias, with f in EDGE_FREQS planted in
     every FiLM row (in all images and in image 1 only).  The algebra that divided by f gives NaN at f = 0 and -0."""
-    import _hd_fields as HD             # registers models J / K; its field_eval covers the label FiLM and plain fields
     siren = copy.deepcopy(_siren(model, "cpu")).double()
     n = 300
     pts, dirs = _field_points(2, n, 3, 21)
@@ -537,9 +539,8 @@ def test_film_gradient_algebra_at_edge_frequencies(monkeypatch, model):
     film0 = _film(_siren(model, "cpu"), 2, 21, edges=True).double()
     film, planted = plant_frequencies(film0, range(film0.shape[1]))
     film.requires_grad_(True)
-    monkeypatch.setattr(oracle, "grid_lookup", _grid_lookup_keep_dtype)
     log = _record_film_layers(monkeypatch)
-    out = HD.field_eval(siren, pts, film, dirs)
+    out = oracle.field_eval(siren, pts, film, dirs)
     d_out = torch.randn(out.shape, generator=torch.Generator().manual_seed(22), dtype=torch.float64)
     (out * d_out).sum().backward()
     assert len(log) == film.shape[1]

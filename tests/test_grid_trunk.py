@@ -2,8 +2,8 @@
 cat[feat, pos] -> 256, and not the colour branch (FENERF_FIELD_GRID_TRUNK), forward and backward.
 
 CPU: the mirror class against the reference (init draws, state-dict keys, parameter names, pickling), the oracle
-(tests/_grid_trunk.py) against the reference's goldens, the flag rules and the packed layout on the host, a float64
-restatement that passes gradcheck, and three faults the bounds must catch.
+(oracle.render_oracle.grid_trunk_field_eval) against the reference's goldens, the flag rules and the packed layout on the
+host, a float64 restatement that passes gradcheck, and three faults the bounds must catch.
 GPU: end to end against the reference's goldens (exact <= 2e-4, default <= 1e-3), both point-network kernels against float64
 over the tile schedules with the density-only entry bit-identical to the sigma channel, the GUARD refinement, the backward
 against float64 and against the reference's autograd (grid probe, the first layer's feature columns), inversion through
@@ -45,7 +45,7 @@ CASES = GT.CASES
 GOLDEN = _cases.GOLDEN_DIR
 TOL = 2e-5          # the oracle against the reference's goldens across hosts (test_oracle.py)
 CHILDREN = ["network", "final_layer", "color_layer_sine", "color_layer_linear", "mapping_network", "gridwarper"]
-SMALL = GT.CASE_BY_NAME["l_small"]
+SMALL = _cases.CASE_BY_NAME["l_small"]
 #: the exact kernel's density carries the fp32 trilinear features through a 35-term first layer at f ~ 30 and then every
 #: trunk layer: measured 1.1e-5 .. 1.3e-5 on sigma (rgb 3e-6 .. 6e-6), against 1e-5 for fields whose trunk sees only the
 #: position; the fast bound is the shared one
@@ -53,7 +53,7 @@ FWD_BOUND_L = {"exact": 3e-5, "fast": FWD_BOUND["fast"]}
 #: the grid's gradient in exact mode reaches the grid through layer 0's fp32 chain and the fp32 scatter-add: measured
 #: 1.1e-4 .. 1.2e-4 of its largest entry (every other tensor within the shared 1e-4)
 GRID_BOUND_EXACT = 3e-4
-GRAD_CASE = GT.CASE_BY_NAME[GT.GRAD_CASE]
+GRAD_CASE = _cases.CASE_BY_NAME[GT.GRAD_CASE]
 
 
 def _gpu_parity():
@@ -130,7 +130,7 @@ def test_oracle_matches_reference_golden(case):
     if case.name in GT.BIG and not os.environ.get("FENERF_SLOW_TESTS") and not torch.cuda.is_available():
         pytest.skip("minutes of CPU oracle (FENERF_SLOW_TESTS=1 runs it)")
     gold = np.load(_cases.golden_path(case))
-    run = GT.oracle_run(case, keep_stages=False)
+    run = _harness.oracle_run(case, keep_stages=False)
     got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
     diff = (got - want).abs()
     assert diff.max() <= TOL, "max|oracle - reference| = %g" % diff.max()
@@ -185,11 +185,11 @@ def _cpu_inputs(seed, n=200, res=None):
 
 
 def test_restatement_is_the_oracle_and_passes_gradcheck():
-    """The restatement equals the oracle's float64 evaluation (tests/_grid_trunk.py) and differentiates
+    """The restatement equals the oracle's float64 evaluation and differentiates
     correctly through the FiLM table, every field parameter and the grid."""
     siren, film, pts, dirs = _cpu_inputs(11)
     with torch.no_grad():
-        assert torch.allclose(_restated(siren, pts, film, dirs), GT.field_eval(siren, pts, film, dirs), rtol=0, atol=1e-12)
+        assert torch.allclose(_restated(siren, pts, film, dirs), oracle.field_eval(siren, pts, film, dirs), rtol=0, atol=1e-12)
     siren, film, pts, dirs = _cpu_inputs(11, n=3, res=5)
     names = [n for n, _ in siren.named_parameters() if "mapping_network" not in n]
     params = dict(siren.named_parameters())
@@ -201,7 +201,7 @@ def test_restatement_is_the_oracle_and_passes_gradcheck():
             m, a = n.rsplit(".", 1) if "." in n else ("", n)
             mods[m]._parameters[a] = p
         try:
-            return GT.field_eval(siren, pts, film_, dirs)
+            return oracle.field_eval(siren, pts, film_, dirs)
         finally:
             for n, d in zip(names, saved):
                 m, a = n.rsplit(".", 1) if "." in n else ("", n)
@@ -220,7 +220,7 @@ def test_faults_exceed_the_bounds(fault):
     res = {}
     for k in (None, fault):
         film.grad = None
-        out = GT.field_eval(siren, pts, film, dirs, fault=k)
+        out = oracle.grid_trunk_field_eval(siren, pts, film, dirs, fault=k)
         (out * d_out).sum().backward()
         res[k] = (out.detach(), film.grad.clone())
     fwd = (res[None][0] - res[fault][0]).abs().amax((0, 1)).max().item()
@@ -239,8 +239,8 @@ def runs():
 
     def get(name):
         if name not in cache:
-            case = GT.CASE_BY_NAME[name]
-            cache[name] = (case, GT.oracle_run(case))
+            case = _cases.CASE_BY_NAME[name]
+            cache[name] = (case, _harness.oracle_run(case))
         return cache[name]
     return get
 
@@ -275,7 +275,7 @@ def test_end_to_end_against_reference_golden(runs, case, precision, tol):
 # --------------------------------------------------------------------------------------------
 @gpu
 @pytest.mark.parametrize("layout", _cases.TILE_LAYOUTS)
-def test_point_network_vs_fp64(monkeypatch, layout):
+def test_point_network_vs_fp64(layout):
     """Both kernels against the oracle's field evaluation in float64 per channel (exact 1e-5, fast 5e-3); back-to-back
     launches are bit-identical, and the density-only entry equals the sigma channel bit for bit in both modes -- the check
     that catches a density path without the grid gather."""
@@ -288,8 +288,7 @@ def test_point_network_vs_fp64(monkeypatch, layout):
         fast2 = ops.siren_points(siren, pts, film, dirs, precision="fast")
         sigma = ops.siren_sigma(siren, pts, film, precision="fast")
         sigma_x = ops.siren_sigma(siren, pts, film, precision="exact")
-    monkeypatch.setattr(oracle, "field_eval", GT.field_eval)
-    want = field_ref(siren, monkeypatch, pts, _per_point(dirs, pts.shape[1], False), film)[0]
+    want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
     err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in (("exact", exact), ("fast", fast))}
     print("forward L %s: exact %.3g fast %.3g (sigma %.3g)" % (layout, err["exact"].max(), err["fast"].max(),
                                                               err["fast"][-1]))
@@ -350,8 +349,7 @@ def test_field_backward_vs_fp64(monkeypatch, layout, precision):
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film = _film(siren, batch, seed, edges=True)
     d_raw = torch.randn(batch, ppb, 4, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    monkeypatch.setattr(oracle, "field_eval", GT.field_eval)
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
     raw = out64.float().contiguous()
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
@@ -426,7 +424,7 @@ def test_inversion_gradients_through_forward_with_frequencies(runs):
 def test_staged_forward_sees_feature_column_writes():
     """torch_ema's copy_to writes through param.data without a version bump: a write to the first layer's feature columns
     alone must reach staged_forward (the fingerprint counts all 35 columns)."""
-    case = GT.CASE_BY_NAME["l_small_opaque"]          # (white-filled at the plain init: nothing would move)
+    case = _cases.CASE_BY_NAME["l_small_opaque"]          # (white-filled at the plain init: nothing would move)
     gen = _cases.build_mirror(case, DEV)
     z = torch.randn(1, 256, generator=torch.Generator().manual_seed(8)).to(DEV)
     kw = dict(case.cfg, psi=0.7, max_batch_size=2400000, precision="exact")

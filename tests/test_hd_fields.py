@@ -2,8 +2,8 @@
 SPATIALSIRENSEMANTICHD (model "K", 129 channels), forward and backward (FENERF_FIELD_FEATURE_HEAD).
 
 CPU: the mirror classes against the reference (init, state-dict keys, parameter order, pickles), the FiLM table, the
-oracle (tests/_hd_fields.py) against the reference's goldens, the flags word and packed sizes on the host, and float64
-restatements of the wide heads and the wide compositor that pass gradcheck.
+oracle (oracle.render_oracle.label_film_field_eval) against the reference's goldens, the flags word and packed sizes on
+the host, and float64 restatements of the wide heads and the wide compositor that pass gradcheck.
 GPU: end to end against the reference's goldens (exact <= 2e-4, default <= 1e-3), both point-network kernels against
 float64 over the tile schedules, the GUARD refinement on a 64-label field, the wide compositor forward and backward
 against float64 up to 64 + 64 samples and 129 channels, the stand-alone compositor bit-identical to the render's, the
@@ -51,7 +51,7 @@ def _gpu_parity():
 # --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("model", ["J", "K"])
 def test_mirror_init_and_state_dict_are_the_references(model):
-    case = HD.CASE_BY_NAME[SMALL[model]]
+    case = _cases.CASE_BY_NAME[SMALL[model]]
     gold = np.load(_cases.golden_path(case))
     gen = _cases.build_mirror(case, "cpu")
     assert _harness.state_digest(gen) == str(gold["state_digest"])
@@ -74,7 +74,7 @@ def test_reference_pickle_loads_under_the_mirror(tmp_path, model):
 
 @pytest.mark.parametrize("model,rows", [("J", 9), ("K", 10)])
 def test_film_table_rows(model, rows):
-    siren = _cases.build_mirror(HD.CASE_BY_NAME[SMALL[model]], "cpu").siren
+    siren = _cases.build_mirror(_cases.CASE_BY_NAME[SMALL[model]], "cpu").siren
     z = torch.randn(3, 256, generator=torch.Generator().manual_seed(5))
     with torch.no_grad():
         film = siren.film_from_latents(z)
@@ -120,7 +120,7 @@ def test_packed_sizes():
     assert lib.fenerf_packed_bytes(ctypes.byref(_desc(FH, 0))) == plain + head
     assert lib.fenerf_packed_bytes(ctypes.byref(_desc(FH | LF, 64))) == label - 4 * 32 * 64 * 2 + 2 * head
     for model in ("J", "K"):
-        spec = _cases.build_mirror(HD.CASE_BY_NAME[SMALL[model]], "cpu").siren.field_spec()
+        spec = _cases.build_mirror(_cases.CASE_BY_NAME[SMALL[model]], "cpu").siren.field_spec()
         d = packing.field_desc(spec)
         assert d.reserved & FH and lib.fenerf_packed_bytes(ctypes.byref(d)) > 0
 
@@ -132,7 +132,7 @@ def _golden_pixels(pixels, gold):
     pixels = pixels.cpu()
     if "pixel_probe" in gold.files:
         assert tuple(pixels.shape) == tuple(gold["pixels_shape"])
-        idx = HD._label_film.pixel_probe_index(pixels.numel())
+        idx = _cases.pixel_probe_index(pixels.numel())
         return pixels.reshape(-1)[idx], torch.from_numpy(gold["pixel_probe"]), idx
     assert tuple(pixels.shape) == gold["pixels"].shape
     return pixels.reshape(-1), torch.from_numpy(gold["pixels"]).reshape(-1), None
@@ -141,7 +141,7 @@ def _golden_pixels(pixels, gold):
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_oracle_matches_reference_golden(case):
     gold = np.load(_cases.golden_path(case))
-    run = HD.oracle_run(case, keep_stages=False)
+    run = _harness.oracle_run(case, keep_stages=False)
     got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
     diff = (got - want).abs()
     assert diff.max() <= TOL, "max|oracle - reference| = %g" % diff.max()
@@ -187,7 +187,7 @@ def _restated(siren, pts, film, dirs, fault=None):
 
 
 def _cpu_inputs(model, seed, n=200):
-    siren = _cases.build_mirror(HD.CASE_BY_NAME[SMALL[model]], "cpu").siren
+    siren = _cases.build_mirror(_cases.CASE_BY_NAME[SMALL[model]], "cpu").siren
     film = _film(siren, 2, seed).double()
     g = torch.Generator().manual_seed(seed)
     pts = ((torch.rand(2, n, 3, generator=g) - 0.5) * 0.24).double()
@@ -197,12 +197,11 @@ def _cpu_inputs(model, seed, n=200):
 
 @pytest.mark.parametrize("model", ["J", "K"])
 def test_restatement_is_the_oracle_and_passes_gradcheck(model):
-    """The oracle's feature-head field evaluation (tests/_hd_fields.py, what the GPU tests compare the kernels and the
-    backward with) equals the written-out restatement, and differentiates correctly through the FiLM table and every
-    field parameter."""
+    """The oracle's feature-head field evaluation (what the GPU tests compare the kernels and the backward with) equals
+    the written-out restatement, and differentiates correctly through the FiLM table and every field parameter."""
     siren, film, pts, dirs = _cpu_inputs(model, 11)
     with torch.no_grad():
-        assert torch.equal(_restated(siren, pts, film, dirs), HD.field_eval(siren, pts, film, dirs))
+        assert torch.equal(_restated(siren, pts, film, dirs), oracle.field_eval(siren, pts, film, dirs))
     pts, dirs = pts[:, :2].contiguous(), dirs[:, :2].contiguous()
     names = [n for n, _ in siren.named_parameters() if "mapping_network" not in n]
     params = dict(siren.named_parameters())
@@ -214,7 +213,7 @@ def test_restatement_is_the_oracle_and_passes_gradcheck(model):
             m, a = n.rsplit(".", 1)
             mods[m]._parameters[a] = p
         try:
-            return HD.field_eval(siren, pts, film_, dirs)
+            return oracle.field_eval(siren, pts, film_, dirs)
         finally:
             for n, d in zip(names, saved):
                 m, a = n.rsplit(".", 1)
@@ -270,8 +269,8 @@ def runs():
 
     def get(name):
         if name not in cache:
-            case = HD.CASE_BY_NAME[name]
-            cache[name] = (case, HD.oracle_run(case))
+            case = _cases.CASE_BY_NAME[name]
+            cache[name] = (case, _harness.oracle_run(case))
         return cache[name]
     return get
 
@@ -308,7 +307,7 @@ def test_end_to_end_against_reference_golden(runs, case, precision, tol):
 @gpu
 @pytest.mark.parametrize("model", ["J", "K"])
 @pytest.mark.parametrize("layout", _cases.TILE_LAYOUTS)
-def test_point_network_vs_fp64(monkeypatch, model, layout):
+def test_point_network_vs_fp64(model, layout):
     """Both kernels against the oracle's field evaluation in float64 per channel (exact 1e-5, fast 5e-3); the fast kernel
     is bit-identical between launches and its density-only entry (the plain instantiation on the trunk view) equals its
     sigma channel."""
@@ -320,8 +319,7 @@ def test_point_network_vs_fp64(monkeypatch, model, layout):
         fast2 = ops.siren_points(siren, pts, film, dirs, precision="fast")
         sigma = ops.siren_sigma(siren, pts, film, precision="fast")
         sigma_x = ops.siren_sigma(siren, pts, film, precision="exact")
-    monkeypatch.setattr(oracle, "field_eval", HD.field_eval)
-    want = field_ref(siren, monkeypatch, pts, _per_point(dirs, pts.shape[1], False), film)[0]
+    want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
     err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in (("exact", exact), ("fast", fast))}
     print("forward %s %s: exact %.3g fast %.3g" % (model, layout, err["exact"].max(), err["fast"].max()))
     assert torch.isfinite(fast).all()
@@ -353,8 +351,7 @@ def test_field_backward_vs_fp64(monkeypatch, layout, model, precision):
     film = _film(siren, batch, seed, edges=True)
     out_dim = siren.field_spec().out_dim
     d_raw = torch.randn(batch, ppb, out_dim, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    monkeypatch.setattr(oracle, "field_eval", HD.field_eval)
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
     raw = out64.float().contiguous()
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
@@ -564,8 +561,8 @@ def test_neural_renderer_generator():
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
     from fenerf_b200.siren import siren as S
     p = _gpu_parity()
-    case = HD.CASE_BY_NAME["k_small"]
-    run = HD.oracle_run(case)
+    case = _cases.CASE_BY_NAME["k_small"]
+    run = _harness.oracle_run(case)
     gold = torch.from_numpy(np.load(_cases.golden_path(case))["pixels"])
     torch.manual_seed(0)
     img_nr, seg_nr = _Upsampler(64, 3), _Upsampler(64, 19)

@@ -61,8 +61,8 @@ def _gpu_parity():
 def test_mirror_init_and_state_dict_are_the_references():
     """Same parameter names, order, shapes and values under manual_seed(0) (the golden's state digest covers keys and
     bytes in order), and the same state_dict keys as the reference-made checkpoint."""
-    gold = np.load(_cases.golden_path(LF.CASE_BY_NAME["i_small"]))
-    gen = _cases.build_mirror(LF.CASE_BY_NAME["i_small"], "cpu")
+    gold = np.load(_cases.golden_path(_cases.CASE_BY_NAME["i_small"]))
+    gen = _cases.build_mirror(_cases.CASE_BY_NAME["i_small"], "cpu")
     assert _harness.state_digest(gen) == str(gold["state_digest"])
     with gzip.open(os.path.join(GOLDEN, "dropin_ref_I.pth.meta.gz"), "rb") as f:
         meta = torch.load(io.BytesIO(f.read()), map_location="cpu", weights_only=False)
@@ -80,7 +80,7 @@ def test_reference_pickle_loads_under_the_mirror(tmp_path):
 
 
 def test_mirror_pickle_carries_no_device_buffers():
-    gen = _cases.build_mirror(LF.CASE_BY_NAME["i_small"], "cpu")
+    gen = _cases.build_mirror(_cases.CASE_BY_NAME["i_small"], "cpu")
     gen.siren.__dict__["_packed_cache"] = ("stand-in",)
     gen.siren.__dict__["_field_plist"] = ("stand-in",)
     buf = io.BytesIO()
@@ -94,7 +94,7 @@ def test_mirror_pickle_carries_no_device_buffers():
 
 def test_film_table_has_ten_rows_in_the_reference_order():
     """Rows 0..7 trunk, 8 label, 9 colour: row r is the mapping output's slice [256 r, 256 (r + 1)) as 15 f + 30."""
-    siren = _cases.build_mirror(LF.CASE_BY_NAME["i_small"], "cpu").siren
+    siren = _cases.build_mirror(_cases.CASE_BY_NAME["i_small"], "cpu").siren
     z = torch.randn(3, 256, generator=torch.Generator().manual_seed(5))
     with torch.no_grad():
         film = siren.film_from_latents(z)
@@ -121,7 +121,7 @@ def test_packed_size_is_computed_on_the_host():
     mine = lib.fenerf_packed_bytes(ctypes.byref(_desc()))
     plain = lib.fenerf_packed_bytes(ctypes.byref(_desc(label_film=False, color_layers=2)))
     assert mine > 0 and mine == plain + 4 * 32 * 64 * 2
-    spec = _cases.build_mirror(LF.CASE_BY_NAME["i_small"], "cpu").siren.field_spec()
+    spec = _cases.build_mirror(_cases.CASE_BY_NAME["i_small"], "cpu").siren.field_spec()
     assert lib.fenerf_packed_bytes(ctypes.byref(packing.field_desc(spec))) == mine
 
 
@@ -149,7 +149,7 @@ def _golden_pixels(pixels, gold):
     pixels = pixels.cpu()
     if "pixel_probe" in gold.files:
         assert tuple(pixels.shape) == tuple(gold["pixels_shape"])
-        idx = LF.pixel_probe_index(pixels.numel())
+        idx = _cases.pixel_probe_index(pixels.numel())
         return pixels.reshape(-1)[idx], torch.from_numpy(gold["pixel_probe"]), idx
     assert tuple(pixels.shape) == gold["pixels"].shape
     return pixels.reshape(-1), torch.from_numpy(gold["pixels"]).reshape(-1), None
@@ -158,7 +158,7 @@ def _golden_pixels(pixels, gold):
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_oracle_matches_reference_golden(case):
     gold = np.load(_cases.golden_path(case))
-    run = LF.oracle_run(case, keep_stages=False)
+    run = _harness.oracle_run(case, keep_stages=False)
     got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
     diff = (got - want).abs()
     assert diff.max() <= TOL, "max|oracle - reference| = %g" % diff.max()
@@ -212,7 +212,7 @@ def _cpu_inputs(seed, n=300):
 def test_restatement_is_the_oracle_and_passes_gradcheck():
     siren, film, pts, dirs = _cpu_inputs(11)
     with torch.no_grad():
-        assert torch.equal(_restated(siren, pts, film, dirs), LF.field_eval(siren, pts, film, dirs))
+        assert torch.equal(_restated(siren, pts, film, dirs), oracle.field_eval(siren, pts, film, dirs))
     pts, dirs = pts[:, :2].contiguous(), dirs[:, :2].contiguous()
     names = [n for n, _ in siren.named_parameters() if "mapping_network" not in n]
     params = dict(siren.named_parameters())
@@ -224,7 +224,7 @@ def test_restatement_is_the_oracle_and_passes_gradcheck():
             m, a = n.rsplit(".", 1)
             mods[m]._parameters[a] = p
         try:
-            return LF.field_eval(siren, pts, film_, dirs)
+            return oracle.field_eval(siren, pts, film_, dirs)
         finally:
             for n, d in zip(names, saved):
                 m, a = n.rsplit(".", 1)
@@ -263,8 +263,8 @@ def runs():
 
     def get(name):
         if name not in cache:
-            case = LF.CASE_BY_NAME[name]
-            cache[name] = (case, LF.oracle_run(case))
+            case = _cases.CASE_BY_NAME[name]
+            cache[name] = (case, _harness.oracle_run(case))
         return cache[name]
     return get
 
@@ -315,7 +315,7 @@ def test_installed_generator_runs_the_class_by_name():
     gen.set_device(DEV)
     l0 = _lib.launch_count()
     with torch.no_grad():
-        px, poses = gen(torch.randn(2, 256, device=DEV), **LF.CASE_BY_NAME["i_small"].cfg)
+        px, poses = gen(torch.randn(2, 256, device=DEV), **_cases.CASE_BY_NAME["i_small"].cfg)
     assert px.shape == (2, 22, 12, 12) and torch.isfinite(px).all() and _lib.launch_count() - l0 >= 5
 
 
@@ -324,7 +324,7 @@ def test_installed_generator_runs_the_class_by_name():
 # --------------------------------------------------------------------------------------------
 @gpu
 @pytest.mark.parametrize("layout", _cases.TILE_LAYOUTS)
-def test_point_network_vs_fp64(monkeypatch, layout):
+def test_point_network_vs_fp64(layout):
     """Both kernels against the oracle's field evaluation (with the label branch) in float64 per channel (exact 1e-5, fast 5e-3); the fast kernel is
     bit-identical between launches and its density-only entry equals its sigma channel."""
     siren = _siren("I", DEV)
@@ -334,8 +334,7 @@ def test_point_network_vs_fp64(monkeypatch, layout):
         fast = ops.siren_points(siren, pts, film, dirs, precision="fast")
         fast2 = ops.siren_points(siren, pts, film, dirs, precision="fast")
         sigma = ops.siren_sigma(siren, pts, film, precision="fast")
-    monkeypatch.setattr(oracle, "field_eval", LF.field_eval)
-    want = field_ref(siren, monkeypatch, pts, _per_point(dirs, pts.shape[1], False), film)[0]
+    want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
     err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in (("exact", exact), ("fast", fast))}
     print("forward I %s: exact %.3g (labels %.3g) fast %.3g (labels %.3g)" % (
         layout, err["exact"].max(), err["exact"][:19].max(), err["fast"].max(), err["fast"][:19].max()))
@@ -351,7 +350,7 @@ def test_guard_refined_rows_match_the_exact_kernel():
     """The GUARD refinement re-evaluates the density of the far samples it lists with the exact kernel's trunk: those
     densities equal the exact kernel's bit for bit, and every other value of the row (labels included) is the fast
     pass's -- the refinement never touches the label branch."""
-    case = LF.CASE_BY_NAME["i_small"]
+    case = _cases.CASE_BY_NAME["i_small"]
     siren = _siren("I", DEV)
     film = _film(siren, 2, 77)
     rd = ops.make_render_desc(batch=2, img_size=24, num_steps=12, hierarchical=False, clamp_mode="relu", nerf_noise=0.0,
@@ -428,8 +427,7 @@ def test_field_backward_vs_fp64(monkeypatch, layout, precision):
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film = _film(siren, batch, seed, edges=True)
     d_raw = torch.randn(batch, ppb, 23, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    monkeypatch.setattr(oracle, "field_eval", LF.field_eval)
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, False), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
     raw = out64.float().contiguous()
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)

@@ -20,8 +20,6 @@ import pytest
 import torch
 
 import _cases
-import _hd_fields  # noqa: F401  (registers models J, K)
-import _label_film  # noqa: F401  (registers model I)
 from _fp64 import _film, _siren, field_ref
 from test_gpu_fp64_reference import FWD_BOUND, _forward_inputs, _per_point
 
@@ -161,7 +159,7 @@ def test_film_fold_is_bit_identical(model):
 @gpu
 @pytest.mark.parametrize("layout", _cases.TILE_LAYOUTS)
 @pytest.mark.parametrize("model", ("A", "B", "C", "D", "H"))
-def test_soft_sine_split_within_fast_bound(monkeypatch, model, layout):
+def test_soft_sine_split_within_fast_bound(model, layout):
     """One column pair in four on soft_sinf (variant 1) and the production kernel against float64, per output channel."""
     from fenerf_b200 import ops
     siren = _siren(model, DEV)
@@ -170,7 +168,7 @@ def test_soft_sine_split_within_fast_bound(monkeypatch, model, layout):
         sfu = ops.siren_points(siren, pts, film, dirs, precision="fast")
         with _Variant(1):
             fast = ops.siren_points(siren, pts, film, dirs, precision="fast")
-    want = field_ref(siren, monkeypatch, pts, _per_point(dirs, pts.shape[1], False), film)[0]
+    want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
     err = (fast.double() - want).abs().amax((0, 1)).max().item()
     err_sfu = (sfu.double() - want).abs().amax((0, 1)).max().item()
     print("split %s %s: soft split %.3g, all-SFU %.3g, max |split - all-SFU| %.3g" % (

@@ -13,16 +13,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import _bridge_fields  # noqa: F401  (registers models M, N)
 import _cases
-import _grid_trunk  # noqa: F401  (model L)
-import _hd_fields  # noqa: F401  (models J, K)
-import _label_film  # noqa: F401  (model I)
+import _harness
 import _wo_dir_fields as WF
 from _fp64 import _film, _siren, field_ref
 from fenerf_b200 import _lib, ops, packing
 from fenerf_b200.generators.volumetric_rendering import ReplayRng
-from oracle import render_oracle as oracle
 from test_gpu_fp64_reference import _forward_inputs, _per_point
 from tools import split_precision as SP
 
@@ -136,12 +132,11 @@ def _gpu_points(model, shape, seed=7):
 @torch.no_grad()
 @pytest.mark.parametrize("model", sorted(GPU_BOUND))
 @pytest.mark.parametrize("shape", _SHAPES)
-def test_points_match_float64(monkeypatch, model, shape):
+def test_points_match_float64(model, shape):
     """Per channel group against float64; a second launch is bit-identical and the density-only entry equals the sigma
     channel."""
-    monkeypatch.setattr(oracle, "field_eval", WF.field_eval)
     siren, film, pts, dirs, dir_group = _gpu_points(model, shape)
-    want, _, _ = field_ref(siren, monkeypatch, pts, _per_point(dirs, pts.shape[1], False), film)
+    want, _, _ = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)
     out = ops.siren_points(siren, pts, film, dirs, precision="split", dir_group=dir_group)
     again = ops.siren_points(siren, pts, film, dirs, precision="split", dir_group=dir_group)
     sigma = siren.density(pts, film, precision="split")
@@ -170,13 +165,8 @@ def runs():
 
     def get(name):
         if name not in cache:
-            if name in WF.CASE_BY_NAME:
-                case = WF.CASE_BY_NAME[name]
-                cache[name] = (case, WF.oracle_run(case))
-            else:
-                import _harness
-                case = _cases.CASE_BY_NAME[name]
-                cache[name] = (case, _harness.oracle_run(case))
+            case = _cases.CASE_BY_NAME[name]
+            cache[name] = (case, _harness.oracle_run(case))
         return cache[name]
     return get
 
@@ -189,15 +179,14 @@ def test_end_to_end_against_reference(runs, name):
     reference's own fp32 forward is up to 5.6e-4 off float64 on this field)."""
     import test_gpu_parity as p
     case, run = runs(name)
-    if name not in WF.CASE_BY_NAME:
+    if case.model != "P":
         gen, pixels, poses, depth_map = p._end_to_end(case, run, "split")
         p._check_pixels(case, run, pixels, 2e-4)
         return
     from test_hd_fields import _golden_pixels
     gold = np.load(_cases.golden_path(case))
-    with WF.with_wo_dir():
-        gen, pixels, poses, depth_map = p._end_to_end(case, run, "split")
-        ill_rays = p._ill_conditioned_pixels(case, run)
+    gen, pixels, poses, depth_map = p._end_to_end(case, run, "split")
+    ill_rays = p._ill_conditioned_pixels(case, run)
     got, want, idx = _golden_pixels(pixels, gold)
     ill = ill_rays.unsqueeze(1).expand_as(pixels).reshape(-1)
     if idx is not None:
@@ -216,8 +205,7 @@ def test_direction_free_gradients_through_a_split_render(runs, golden):
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
     case, run = runs(WF.GRAD_CASE)
     gold = np.load(os.path.join(GOLDEN, "%s_%s.npz" % (golden, WF.GRAD_CASE)))
-    with WF.with_wo_dir():
-        gen = _cases.build_mirror(case, DEV)
+    gen = _cases.build_mirror(case, DEV)
     kw = dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="split")
     if golden == "grad":
         latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
@@ -271,9 +259,8 @@ def test_pack_without_split_images_and_only_idx_are_refused():
 def test_staged_forward_sees_param_data_writes():
     """A param.data write (torch_ema's copy_to) into one hidden layer reaches the next split staged_forward: the
     fingerprint check repacks the split images too."""
-    case = WF.CASE_BY_NAME["p_small_opaque"]
-    with WF.with_wo_dir():
-        gen = _cases.build_mirror(case, DEV)
+    case = _cases.CASE_BY_NAME["p_small_opaque"]
+    gen = _cases.build_mirror(case, DEV)
     g = torch.Generator().manual_seed(8)
     z = [torch.randn(1, 256, generator=g).to(DEV) for _ in range(2)]
     kw = dict(case.cfg, psi=0.7, max_batch_size=2400000, precision="split")

@@ -29,7 +29,7 @@ from test_gpu_fp64_reference import (_LAYOUTS, _field_backward, _field_points, _
 DEV = "cuda:0"
 GOLDEN = _cases.GOLDEN_DIR
 #: exact point network, max |out - fp64| over the (labels, rgb, sigma) channels.  Measured on an H100 80GB HBM3 (700 W
-#: power limit): labels 8.1e-8, rgb 8.3e-5, sigma 7.6e-7.  The wgmma colour path is refused for this field: its rgb error
+#: power limit): labels 8.1e-8, rgb 8.4e-5, sigma 7.6e-7.  The wgmma colour path is refused for this field: its rgb error
 #: was 2.1e-2 at 2 x 2048 points, the fp16 trunk's own error amplified by the first colour layer's U(+-1/3) weights at
 #: f ~ 30 (with those weights zeroed on the trunk columns it was 7.7e-5; DESIGN section 5).  The density alone stays on
 #: the wgmma kernel: 2.9e-4 there.
@@ -126,13 +126,13 @@ def _cpu_inputs(seed, n=1024):
 def test_restatement_is_the_oracle_and_passes_gradcheck():
     siren, film, pts, dirs = _cpu_inputs(3, n=6)
     with torch.no_grad():
-        assert torch.equal(WF.field_eval(siren, pts, film, dirs), WF.restated(siren, pts, film, dirs))
+        assert torch.equal(oracle.field_eval(siren, pts, film, dirs), oracle.wo_dir_field_eval(siren, pts, film, dirs))
     c0 = len(siren.network)
 
     def f(sub):
         fl = film.clone()
         fl[:, c0, :, :3] = sub
-        return WF.restated(siren, pts, fl, dirs)[..., 18:21]
+        return oracle.wo_dir_field_eval(siren, pts, fl, dirs)[..., 18:21]
     sub = film[:, c0, :, :3].clone().requires_grad_(True)
     assert torch.autograd.gradcheck(f, (sub,), eps=1e-6, atol=1e-7)
 
@@ -143,7 +143,8 @@ def test_faults_move_the_colours_past_the_exact_bound(fault):
     and the features after x each move the colours past the exact kernel's rgb bound."""
     siren, film, pts, dirs = _cpu_inputs(5)
     with torch.no_grad():
-        good, bad = WF.restated(siren, pts, film, dirs), WF.restated(siren, pts, film, dirs, fault=fault)
+        good = oracle.wo_dir_field_eval(siren, pts, film, dirs)
+        bad = oracle.wo_dir_field_eval(siren, pts, film, dirs, fault=fault)
     err = (good - bad)[..., 18:21].abs().max().item()
     print("fault %s: max |rgb| move %.3g" % (fault, err))
     assert err > EXACT_BOUND[1]
@@ -155,7 +156,7 @@ def test_oracle_matches_reference_golden(case):
     if case.name in WF.BIG and not os.environ.get("FENERF_SLOW_TESTS") and not torch.cuda.is_available():
         pytest.skip("minutes of CPU oracle (FENERF_SLOW_TESTS=1 runs it)")
     gold = np.load(_cases.golden_path(case))
-    run = WF.oracle_run(case, keep_stages=False)
+    run = _harness.oracle_run(case, keep_stages=False)
     got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
     assert (got - want).abs().max() <= 2e-5
 
@@ -175,7 +176,7 @@ def _gpu_inputs(batch, ppb, seed=7):
 def _want(siren, film, pts, dirs):
     s64 = copy.deepcopy(siren).double()
     with torch.no_grad():
-        return WF.restated(s64, pts.double(), film.double(), dirs.double())
+        return oracle.wo_dir_field_eval(s64, pts.double(), film.double(), dirs.double())
 
 
 @pytest.mark.gpu
@@ -257,14 +258,13 @@ def test_backward_matches_float64_autograd(monkeypatch, layout, lock, edges):
     batch, ppb, dir_group, chunk = _LAYOUTS[layout]
     # TF32 on, a common training setting: the backward keeps this field's products fp32 itself
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", True)
-    monkeypatch.setattr(oracle, "field_eval", WF.field_eval)
     siren = _siren("P", DEV)
     seed = 6000 + int(layout[1])
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film, planted = (FE._edge_film(siren, batch, seed, FE.BACKWARD_FREQS) if edges
                      else (_film(siren, batch, seed, edges=True), []))
     d_raw = torch.randn(batch, ppb, 22, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    out64, want_film, want = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, lock), film, d_raw)
+    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, lock), film, d_raw)
     raw = out64.float().contiguous()
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
@@ -281,7 +281,7 @@ def test_backward_matches_float64_autograd(monkeypatch, layout, lock, edges):
         print("wo_dir edge columns %s: worst %s %.3g" % (layout, worst_col, cols[worst_col]))
         assert cols[worst_col] <= BWD_BOUND, {k: "%.2e" % v for k, v in cols.items() if v > BWD_BOUND}
         film150, _ = FE._edge_film(siren, batch, seed)
-        out150, want_film150, want150 = field_ref(siren, monkeypatch, pts, _per_point(dirs, ppb, lock), film150, d_raw)
+        out150, want_film150, want150 = field_ref(siren, pts, _per_point(dirs, ppb, lock), film150, d_raw)
         d_film150, grads150 = _field_backward(siren, film150, pts, dirs, dir_group, lock, out150.float().contiguous(), d_raw,
                                               True)
         assert torch.isfinite(d_film150).all() and all(torch.isfinite(g).all() for g in grads150.values())
@@ -307,8 +307,8 @@ def runs():
 
     def get(name):
         if name not in cache:
-            case = WF.CASE_BY_NAME[name]
-            cache[name] = (case, WF.oracle_run(case))
+            case = _cases.CASE_BY_NAME[name]
+            cache[name] = (case, _harness.oracle_run(case))
         return cache[name]
     return get
 
@@ -322,9 +322,8 @@ def test_end_to_end_against_reference_golden(runs, case):
     from test_hd_fields import _golden_pixels
     gold = np.load(_cases.golden_path(case))
     case, run = runs(case.name)
-    with WF.with_wo_dir():
-        gen, pixels, poses, depth_map = p._end_to_end(case, run, "exact")
-        ill_rays = p._ill_conditioned_pixels(case, run)
+    gen, pixels, poses, depth_map = p._end_to_end(case, run, "exact")
+    ill_rays = p._ill_conditioned_pixels(case, run)
     got, want, idx = _golden_pixels(pixels, gold)
     err = (got - want).abs()
     assert int(ill_rays.sum()) <= max(2, 0.002 * ill_rays.numel())
@@ -345,8 +344,7 @@ def test_generator_gradients_match_reference(runs):
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
     case, run = runs(WF.GRAD_CASE)
     gold = np.load(os.path.join(GOLDEN, "grad_%s.npz" % WF.GRAD_CASE))
-    with WF.with_wo_dir():
-        gen = _cases.build_mirror(case, DEV)
+    gen = _cases.build_mirror(case, DEV)
     latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
     pixels, _ = gen(*latents, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="exact"))
     (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
@@ -363,8 +361,7 @@ def test_inversion_gradients_through_forward_with_frequencies(runs):
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
     case, run = runs(WF.GRAD_CASE)
     gold = np.load(os.path.join(GOLDEN, "gradfreq_%s.npz" % WF.GRAD_CASE))
-    with WF.with_wo_dir():
-        gen = _cases.build_mirror(case, DEV)
+    gen = _cases.build_mirror(case, DEV)
     with torch.no_grad():
         lat = [p._cuda(z) for z in run["latents"]]
         fp = [t.clone().requires_grad_(True) for t in gen.siren.geo_mapping_network(lat[0]) + gen.siren.app_mapping_network(lat[1])]
@@ -381,9 +378,8 @@ def test_inversion_gradients_through_forward_with_frequencies(runs):
 def test_staged_forward_sees_first_colour_layer_writes():
     """torch_ema's copy_to writes through param.data without a version bump: a write to color_layer_sine[0] alone -- its
     feature columns alone, too -- must reach staged_forward (the fingerprint covers all 288 columns)."""
-    case = WF.CASE_BY_NAME["p_small_opaque"]
-    with WF.with_wo_dir():
-        gen = _cases.build_mirror(case, DEV)
+    case = _cases.CASE_BY_NAME["p_small_opaque"]
+    gen = _cases.build_mirror(case, DEV)
     s = gen.siren
     g = torch.Generator().manual_seed(8)
     z = [torch.randn(1, 256, generator=g).to(DEV) for _ in range(2)]

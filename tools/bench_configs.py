@@ -9,8 +9,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
 import _cases
-import _grid_trunk  # (registers model L)
-import _bridge_fields  # (registers models M, N: the bridge fields AUG and RES)
 
 # C: A's layers; L: C's plus 32 more inputs of the first layer; G / H: 8 + 3 / 8 + 8 FiLM layers; M (AUG): H's trunk, 7
 # wide colour layers and a 6-wide first one; N (RES): 7 + 5 wide layers, the narrow first layers and heads
@@ -34,8 +32,7 @@ def main():
     print("device: %s" % torch.cuda.get_device_name(dev))
     rows = [r for r in ROWS if not args.models or r[1] in args.models.split(",")]
     for label, model, batch, img, steps in rows * args.rounds:
-        case = (_cases.CASE_BY_NAME.get(CASE[model]) or _grid_trunk.CASE_BY_NAME.get(CASE[model])
-                or _bridge_fields.CASE_BY_NAME[CASE[model]])
+        case = _cases.CASE_BY_NAME[CASE[model]]
         gen = _cases.build_mirror(case, dev)
         md = dict(_cases.BASE, img_size=img, num_steps=steps, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)
         lat = [torch.randn(batch, 256, device=dev) for _ in range(_cases.n_latents(model))]

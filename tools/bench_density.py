@@ -9,8 +9,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
 import _cases
-import _grid_trunk  # (registers model L)
-import _bridge_fields  # (registers models M, N: the bridge fields AUG and RES)
 from fenerf_b200 import ops
 
 CASE = {"A": "a_small", "B": "b_small", "C": "c_small", "L": "l_small", "G": "g_small", "H": "h_small",
@@ -26,8 +24,7 @@ def main():
     res = args.res
     print("device: %s" % torch.cuda.get_device_name("cuda:0"))
     for model in args.models.split(",") * args.rounds:
-        case = (_cases.CASE_BY_NAME.get(CASE[model]) or _grid_trunk.CASE_BY_NAME.get(CASE[model])
-                or _bridge_fields.CASE_BY_NAME[CASE[model]])
+        case = _cases.CASE_BY_NAME[CASE[model]]
         gen = _cases.build_mirror(case, "cuda:0")
         lin = torch.linspace(-0.15, 0.15, res, device="cuda")
         pts = torch.stack(torch.meshgrid(lin, lin, lin, indexing="ij"), -1).reshape(1, -1, 3).contiguous()

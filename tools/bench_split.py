@@ -15,7 +15,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 
 import _cases  # noqa: E402
-import _wo_dir_fields as WF  # noqa: E402
 from _fp64 import _film  # noqa: E402
 from fenerf_b200 import ops  # noqa: E402
 from fenerf_b200.graphs import GraphedRender  # noqa: E402
@@ -54,9 +53,7 @@ def main():
     print("device: %s (%s)" % (torch.cuda.get_device_name(dev), q.stdout.strip() or "nvidia-smi unavailable"))
     setups = {}
     for model in args.models.split(","):
-        case = _cases.CASE_BY_NAME.get(CASE[model]) or WF.CASE_BY_NAME[CASE[model]]
-        with WF.with_wo_dir():
-            gen = _cases.build_mirror(case, dev)
+        gen = _cases.build_mirror(_cases.CASE_BY_NAME[CASE[model]], dev)
         md = dict(_cases.BASE, img_size=IMG, num_steps=STEPS, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)
         g = torch.Generator().manual_seed(1)
         lat = [torch.randn(BATCH, 256, generator=g).to(dev) for _ in range(_cases.n_latents(model))]

@@ -34,7 +34,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for _p in (ROOT, os.path.join(ROOT, "tests")):
     if _p not in sys.path:
         sys.path.insert(0, _p)
-import _wo_dir_fields as WF  # noqa: E402
 from _fp64 import _film, _siren  # noqa: E402
 from oracle import render_oracle as oracle  # noqa: E402
 
@@ -113,13 +112,11 @@ def patch_split(setattr_, fault=None, args=None):
             return f32(_SIN64(f32(a)))
         return approx_sin(a) if fault == "sinf" else soft_sin(a)
 
-    def grid(coords, g):
-        if fault == "fp16_grid":       # the fast path's copy: fp16 voxels, the interpolated feature rounded to fp16
-            return f16(_lookup64(coords, f16(g)))
-        return _lookup64(coords, g)
     setattr_(torch.nn.Linear, "forward", linear)
     setattr_(torch, "sin", sine)
-    setattr_(oracle, "grid_lookup", grid)
+    if fault == "fp16_grid":           # the fast path's copy: fp16 voxels, the interpolated feature rounded to fp16
+        lookup = oracle.grid_lookup
+        setattr_(oracle, "grid_lookup", lambda coords, g: f16(lookup(coords, f16(g))))
 
 
 class Patcher:
@@ -141,13 +138,6 @@ class Patcher:
         self.saved.clear()
 
 
-def _lookup64(coords, grid):
-    b, n, d = coords.shape
-    s = F.grid_sample(grid.expand(b, -1, -1, -1, -1), coords.reshape(b, 1, 1, -1, d), mode='bilinear', padding_mode='zeros',
-                      align_corners=True)
-    return s.reshape(b, grid.shape[1], -1).transpose(1, 2)
-
-
 def inputs(model, latents=2, points=4096, seed=3):
     siren = _siren(model, "cpu")
     film = _film(siren, latents, seed).double()
@@ -161,12 +151,11 @@ def evaluate(setattr_, siren, film, pts, dirs, mode=None, fault=None, args=None)
     """mode None: float64 (sine arguments into `args`); 'split': the split kernel's arithmetic (with `fault`)."""
     with torch.no_grad():
         if mode is None:
-            setattr_(oracle, "grid_lookup", _lookup64)
             if args is not None:
                 setattr_(torch, "sin", lambda a: (args.append(a.detach().reshape(-1)), _SIN64(a))[1])
         else:
             patch_split(setattr_, fault, args)
-        return WF.field_eval(siren, pts, film, dirs)
+        return oracle.field_eval(siren, pts, film, dirs)
 
 
 def errors(siren, film, pts, dirs, fault=None, setattr_=None):
