@@ -37,6 +37,7 @@ EXPORTS = (
     "fenerf_workspace_layout", "fenerf_mask2color", "fenerf_frames_to_u8", "fenerf_mapping_film",
     "fenerf_guard_stats", "fenerf_debug_stage_times", "fenerf_debug_fast_variant", "fenerf_debug_soft_sine",
     "fenerf_gemm_nt_f16", "fenerf_gemm_nt_film", "fenerf_gemm_tn_f16",
+    "fenerf_gemm_nt_split", "fenerf_gemm_nt_film_split", "fenerf_gemm_tn_split", "fenerf_absmax_f32",
     "fenerf_pack_field_bridge", "fenerf_field_fingerprint_bridge",
 )
 
@@ -134,6 +135,14 @@ def _declare(lib):
     lib.fenerf_gemm_nt_film.argtypes = [vp, vp, i64, vp, vp, i64, i64, vp, vp, vp, vp, vp]
     lib.fenerf_gemm_tn_f16.restype = C.c_int
     lib.fenerf_gemm_tn_f16.argtypes = [vp, vp, i32, i64, i32, vp, vp, vp]
+    lib.fenerf_gemm_nt_split.restype = C.c_int
+    lib.fenerf_gemm_nt_split.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp]
+    lib.fenerf_gemm_nt_film_split.restype = C.c_int
+    lib.fenerf_gemm_nt_film_split.argtypes = [vp, vp, vp, i64, vp, vp, vp, i64, i64, vp, vp, vp]
+    lib.fenerf_gemm_tn_split.restype = C.c_int
+    lib.fenerf_gemm_tn_split.argtypes = [vp, vp, i32, i64, i32, vp, vp, vp, vp]
+    lib.fenerf_absmax_f32.restype = C.c_int
+    lib.fenerf_absmax_f32.argtypes = [vp, i64, vp, vp]
     lib.fenerf_debug_stage_times.restype = C.c_int
     lib.fenerf_debug_stage_times.argtypes = [i32, vp]
     lib.fenerf_debug_fast_variant.restype = C.c_int

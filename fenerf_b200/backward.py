@@ -38,7 +38,8 @@ taken from max|d raw| on the device (no host sync) and unscaled at the end.
 The three 256-wide products per layer run on wgmma (csrc/gemm.cu: ``fenerf_gemm_nt_film`` -- the recompute with its FiLM
 epilogue fused, ``fenerf_gemm_nt_f16`` for dA' = dU diag(f_b) W, ``fenerf_gemm_tn_f16`` split-K for the per-image M_b); only the narrow
 products (heads, the 3 / 35-wide inputs) go to the library.  ``FENERF_B200_BWD_GEMM=cublas`` switches the wide ones back
-(A/B timing); ``precision='exact'`` always uses fp32 library GEMMs.  (The kernels can also fold the next layer's gate multiply
+(A/B timing); ``precision='exact'`` uses fp32 library GEMMs, or, with ``grad_precision='split'``, the split kernels of
+csrc/gemm_split.cu on the same fp32 streams (fp16 hi / lo operands scaled by powers of two, fp32-grade results).  (The kernels can also fold the next layer's gate multiply
 into the dA product's epilogue and produce the bias column sums from the dW kernel's staged tiles -- measured: the gate kernel's
 17 ms disappear but the two GEMMs slow down by as much, both being HBM-bound; the chain below keeps the separate gate kernel.)
 """
@@ -189,11 +190,50 @@ def _linear_chain_grads(chain, d_weff, d_beff):
     return out
 
 
+#: the render keyword ``grad_precision``: None (the backward of the forward precision) or 'split'
+GRAD_PRECISIONS = (None, "split")
+_GRAD_SPLIT_STREAMS = ("grad_precision='split' differentiates precision='split' or 'exact' renders only: it runs on their "
+                       "fp32 streams (precision='fast' / 'guard' keep the fp16 backward)")
+
+
+def _grad_split_refusal(spec):
+    """Why grad_precision='split' cannot differentiate a field of this spec (None: it can).  The same variants as the split
+    forward (FENERF_PRECISION_SPLIT) refuses."""
+    kinds = [name for name, on in (("a label FiLM layer", spec.label_film), ("a feature head", spec.feature_head),
+                                   ("grid features in the trunk", spec.grid_trunk), ("a bridge colour branch", spec.bridge))
+             if on]
+    if not kinds:
+        return None
+    return ("grad_precision='split' is not built for fields with %s (FENERF_FIELD_LABEL_FILM, FENERF_FIELD_FEATURE_HEAD, "
+            "FENERF_FIELD_GRID_TRUNK, FENERF_FIELD_BRIDGE); differentiate them without grad_precision" % " and ".join(kinds))
+
+
+def check_grad_precision(module, grad_precision, precision):
+    """Raises unless a differentiable render of `module` in forward precision `precision` (name or code) can take
+    `grad_precision`: ValueError for an unknown name, RuntimeError with the reason for a refused combination."""
+    if grad_precision not in GRAD_PRECISIONS:
+        raise ValueError("grad_precision must be one of %s (got %r)" % (GRAD_PRECISIONS, grad_precision))
+    if grad_precision is None:
+        return
+    if ops._precision_code(precision) not in (_lib.PRECISION["split"], _lib.PRECISION["exact"]):
+        raise RuntimeError(_GRAD_SPLIT_STREAMS)
+    reason = _grad_split_refusal(module.field_spec())
+    if reason:
+        raise RuntimeError(reason)
+
+
 class _FieldBackward:
     """Accumulates the gradients of one field over any number of point sets."""
 
-    def __init__(self, module, film, scale, inv_scale, exact=False, split=False):
+    def __init__(self, module, film, scale, inv_scale, exact=False, split=False, grad_split=False):
         self.module = module
+        # grad_split (grad_precision='split'): the fp32 streams of the exact mode, the 256-wide products on the split
+        # kernels of csrc/gemm_split.cu
+        self.gs = bool(grad_split)
+        if self.gs and not exact:
+            raise RuntimeError(_GRAD_SPLIT_STREAMS)
+        if self.gs and _grad_split_refusal(module.field_spec()):
+            raise RuntimeError(_grad_split_refusal(module.field_spec()))
         # stream element type: fp16 (default) or fp32 (parity mode, with precision='exact': plain fp32 GEMMs)
         self.dt = torch.float32 if exact else torch.float16
         self.dtc = 1 if exact else 0
@@ -272,6 +312,8 @@ class _FieldBackward:
             wc0 = torch.cat([self.Wc0eff, torch.zeros((256, 256), dtype=torch.float32, device=dev)], dim=1)
         self.Wc0x_narrow = wc0[:, :self.kx].contiguous()                          # (256, 3 + G) fp32
         self.Wc16 = [wc0[:, self.kx:].to(self.dt).contiguous()] + [w.detach().to(self.dt).contiguous() for w, _ in fw.color[1:]]
+        # grad_split: the recompute's 256-wide weights by FiLM row (trunk 1.., colour c0..), split as (hi, lo, amax)
+        self.Wsplit = [None] + [ops.split_weights(w) for w in self.Wh16[1:] + self.Wc16] if self.gs else None
         # the weights the grid features meet, (256, G): the first colour layer's, or the first layer's with the grid in
         # the trunk, whose FiLM row is then 0
         self.feat_row = 0 if self.gt else self.c0
@@ -287,7 +329,11 @@ class _FieldBackward:
         self.Wchain32 += [wc0_chain] + [w.detach().float() for w, _ in fw.color[1:]]
         # ... scaled per image once for every chunk: diag(f_b) W, (B, n_film - 1, 256, 256); the NT kernel wants it transposed
         fW = self.film[:, 1:, 0].unsqueeze(3) * torch.stack(self.Wchain32[1:])
-        self.fW = fW.transpose(2, 3).to(torch.float16).contiguous() if self.own_gemm else fW.to(self.dt)
+        if self.gs:     # per image and layer, (diag(f_b) W)^T scaled by its own power of two and split
+            self.fW_hi, self.fW_lo, self.fW_amax = ops.split_weights(fW.transpose(2, 3))
+            self.fW = None
+        else:
+            self.fW = fW.transpose(2, 3).to(torch.float16).contiguous() if self.own_gemm else fW.to(self.dt)
         del fW
         self.fWfeat = (self.film[:, self.feat_row, 0].unsqueeze(2) * self.Wfeat32).to(self.dt) if G else None    # (B, 256, G)
         if self.own_gemm:
@@ -309,8 +355,8 @@ class _FieldBackward:
 
     # ---- one point set: points (B, ppb, 3), dirs (B, ppb/dir_group, 3), raw / d_raw (B, ppb, C) ----
     def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
-        if self.wd:     # the direction-free field: TF32 rounding would be amplified like fp16's (see __init__)
-            with _NoTF32():
+        if self.wd or self.gs:     # the direction-free field: TF32 rounding would be amplified like fp16's (see __init__);
+            with _NoTF32():          # grad_split: its narrow products stay fp32
                 return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw)
         return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw)
 
@@ -345,9 +391,17 @@ class _FieldBackward:
         _lib.check(_lib.lib().fenerf_gate_backward(dA.data_ptr(), gate.data_ptr(), P, ppb, tmp.data_ptr(), self.dtc, _stream(self.dev)))
         cs += tmp
 
-    def _chain(self, dU, idx, b0, b1, ppb):
-        """dU diag(f_b) W of FiLM row idx for each image b of the chunk: the gradient of the layer's input (P, 256)."""
+    def _chain(self, dU, idx, b0, b1, ppb, amax=None):
+        """dU diag(f_b) W of FiLM row idx for each image b of the chunk: the gradient of the layer's input (P, 256).
+        amax: max |dU| on the device (grad_split)."""
         k = b1 - b0
+        if self.gs:
+            out = torch.empty_like(dU)
+            for i in range(k):
+                rows = slice(i * ppb, (i + 1) * ppb)
+                ops.gemm_nt_split(dU[rows], self.fW_hi[b0 + i, idx - 1], self.fW_lo[b0 + i, idx - 1],
+                                  self.fW_amax[b0 + i, idx - 1], a_amax=amax, out=out[rows])
+            return out
         if not self.own_gemm:
             return torch.bmm(dU.view(k, ppb, 256), self.fW[b0:b1, idx - 1]).view(k * ppb, 256)
         out = torch.empty_like(dU)
@@ -383,6 +437,8 @@ class _FieldBackward:
             for l in range(1, T):
                 if own:     # z = a W^T with the FiLM epilogue fused: z never leaves the SM
                     A[l], Gt[l] = ops.gemm_nt_film(A[l - 1], self.Wh16[l], self.bias[l], self.film, b0, l, ppb)
+                elif self.gs:
+                    A[l], Gt[l] = ops.gemm_nt_film_split(A[l - 1], *self.Wsplit[l], self.bias[l], self.film, b0, l, ppb)
                 else:
                     A[l], Gt[l] = self._stash(_mm32(A[l - 1], self.Wh16[l].t()), l, b0, P, ppb)
             if self.lf:     # the label FiLM layer, on the trunk output
@@ -404,11 +460,16 @@ class _FieldBackward:
                                                  narrow_w=self.Wn64)
                 del e64
             else:
-                A[c0], Gt[c0] = self._stash(_mm32(A[T - 1], self.Wc16[0].t()), c0, b0, P, ppb, xin=extras, wx=self.Wc0x_narrow)
+                z = ops.gemm_nt_split(A[T - 1], *self.Wsplit[c0]) if self.gs else _mm32(A[T - 1], self.Wc16[0].t())
+                A[c0], Gt[c0] = self._stash(z, c0, b0, P, ppb, xin=extras, wx=self.Wc0x_narrow)
+                del z
             for j in range(1, Cn):
                 if own:
                     A[c0 + j], Gt[c0 + j] = ops.gemm_nt_film(A[c0 + j - 1], self.Wc16[j], self.bias[c0 + j], self.film, b0, c0 + j,
                                                              ppb)
+                elif self.gs:
+                    A[c0 + j], Gt[c0 + j] = ops.gemm_nt_film_split(A[c0 + j - 1], *self.Wsplit[c0 + j], self.bias[c0 + j], self.film,
+                                                                   b0, c0 + j, ppb)
                 else:
                     A[c0 + j], Gt[c0 + j] = self._stash(_mm32(A[c0 + j - 1], self.Wc16[j].t()), c0 + j, b0, P, ppb)
             # ---- head gradients ----
@@ -439,14 +500,18 @@ class _FieldBackward:
                     break
                 a_in = A[idx - 1] if j else A[T - 1]
                 du3 = dA.view(k, ppb, 256).transpose(1, 2)
-                self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(du3, a_in.view(k, ppb, 256))
+                amax = ops.absmax(dA) if self.gs else None      # (grad_split: the scale of this layer's dU, on the device)
+                if self.gs:
+                    self.dW_b[idx][b0:b1] += ops.gemm_tn_split(dA, a_in, k, ppb, x_amax=amax)
+                else:
+                    self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(du3, a_in.view(k, ppb, 256))
                 if j == 0:
                     e16 = torch.zeros((P, self.kx_pad), dtype=self.dt, device=dev)
                     e16[:, :self.kx] = extras
                     self.dWx_b[b0:b1] += _bmm32(du3, e16.view(k, ppb, self.kx_pad))
                     if G and not self.gt:
                         self._grid_grad(dA, points, k, ppb, b0, b1)
-                dA = self._chain(dA, idx, b0, b1, ppb)
+                dA = self._chain(dA, idx, b0, b1, ppb, amax)
                 A[idx], Gt[idx] = None, None
             # ---- trunk: colour-branch gradient + sigma / label heads ----
             dA += torch.mm(dH.float(), self.Wheads32)
@@ -462,11 +527,14 @@ class _FieldBackward:
                 A[T], Gt[T] = None, None
             for l in range(T - 1, 0, -1):
                 self._gate(dA, Gt[l], l, b0, b1, P, ppb)
+                amax = ops.absmax(dA) if self.gs else None
                 if own:
                     self.dW_b[l][b0:b1] += ops.gemm_tn(dA, A[l - 1], k, ppb)
+                elif self.gs:
+                    self.dW_b[l][b0:b1] += ops.gemm_tn_split(dA, A[l - 1], k, ppb, x_amax=amax)
                 else:
                     self.dW_b[l][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), A[l - 1].view(k, ppb, 256))
-                dA = self._chain(dA, l, b0, b1, ppb)
+                dA = self._chain(dA, l, b0, b1, ppb, amax)
                 A[l], Gt[l] = None, None
             self._gate(dA, Gt[0], 0, b0, b1, P, ppb)
             if self.gt:
@@ -503,7 +571,7 @@ class _FieldBackward:
 
     # ---- after every point set: fold the per-image accumulators into parameter / FiLM gradients ----
     def finish(self):
-        if self.wd:
+        if self.wd or self.gs:
             with _NoTF32():
                 return self._finish()
         return self._finish()
@@ -624,7 +692,7 @@ class RenderFunction(torch.autograd.Function):
             # precision='split' renders forward on the split-precision kernel and differentiates as 'exact' does
             split = rd.precision == _lib.PRECISION['split']
             fb = _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'],
-                                split=split)
+                                split=split, grad_split=call.get('grad_precision') == 'split')
             lock = bool(rd.lock_view_dependence)
             rays = call.get('grad_rays')
             dirs = st['dirs']
@@ -651,11 +719,15 @@ class RenderFunction(torch.autograd.Function):
 
 
 def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
-                     grad_rays=None):
+                     grad_rays=None, grad_precision=None):
     """Differentiable render: (B, C-1, R, R) pixels with autograd edges to `film` and the field parameters.
-    `grad_rays`: optional int64 ray indices -- only these rays carry the gradient (part_forward)."""
+    `grad_rays`: optional int64 ray indices -- only these rays carry the gradient (part_forward).
+    `grad_precision`: None (the backward of the forward precision) or 'split' (fp32 streams, the 256-wide products on the
+    split kernels of csrc/gemm_split.cu; forward precision 'split' or 'exact', the fields the split forward serves)."""
+    check_grad_precision(module, grad_precision, rd.precision)
     fw = FieldWeights(module)
     params = fw.parameters()
     call = dict(module=module, rd=rd, x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world, rng_perturb=rng_perturb,
-                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_rays=grad_rays)
+                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_rays=grad_rays,
+                grad_precision=grad_precision)
     return RenderFunction.apply(film, call, *params)

@@ -386,6 +386,37 @@ int fenerf_gemm_tn_f16(const void* X, const void* Y, int32_t batch, int64_t poin
     return gemm_tn(X, Y, batch, points_per_batch, slices, partial, (cudaStream_t)stream, colsum);
 }
 
+int fenerf_gemm_nt_split(const float* A, const void* B_hi, const void* B_lo, int64_t M, const float* a_amax, const float* b_amax,
+                         float* c_f32, void* stream) {
+    FN_REQUIRE(A && B_hi && B_lo && b_amax && c_f32 && M >= 0, "bad argument");
+    FN_REQUIRE((((uintptr_t)A | (uintptr_t)B_hi | (uintptr_t)B_lo | (uintptr_t)c_f32) & 15) == 0, "operands must be 16-byte aligned");
+    return gemm_nt_split(A, B_hi, B_lo, M, a_amax, b_amax, c_f32, nullptr, nullptr, nullptr, nullptr, 0, 1, (cudaStream_t)stream);
+}
+
+int fenerf_gemm_nt_film_split(const float* A, const void* W_hi, const void* W_lo, int64_t M, const float* w_amax,
+                              const float* bias, const float* film_layer, int64_t film_batch_stride, int64_t points_per_batch,
+                              float* a_out, float* gate_out, void* stream) {
+    FN_REQUIRE(A && W_hi && W_lo && w_amax && bias && film_layer && a_out && gate_out && M >= 0 && points_per_batch >= 1,
+               "bad argument");
+    FN_REQUIRE((((uintptr_t)A | (uintptr_t)W_hi | (uintptr_t)W_lo | (uintptr_t)a_out | (uintptr_t)gate_out) & 15) == 0,
+               "operands must be 16-byte aligned");
+    return gemm_nt_split(A, W_hi, W_lo, M, nullptr, w_amax, nullptr, a_out, gate_out, bias, film_layer, film_batch_stride,
+                         points_per_batch, (cudaStream_t)stream);
+}
+
+int fenerf_gemm_tn_split(const float* X, const float* Y, int32_t batch, int64_t points_per_batch, int32_t slices,
+                         const float* x_amax, const float* y_amax, float* partial, void* stream) {
+    FN_REQUIRE(X && Y && partial && batch >= 1 && points_per_batch >= 1 && slices >= 1, "bad argument");
+    FN_REQUIRE((((uintptr_t)X | (uintptr_t)Y | (uintptr_t)partial) & 15) == 0, "operands must be 16-byte aligned");
+    return gemm_tn_split(X, Y, batch, points_per_batch, slices, x_amax, y_amax, partial, (cudaStream_t)stream);
+}
+
+int fenerf_absmax_f32(const float* x, int64_t n, float* amax, void* stream) {
+    FN_REQUIRE(x && amax && n >= 0, "bad argument");
+    FN_REQUIRE(((uintptr_t)x & 15) == 0, "x must be 16-byte aligned");
+    return absmax_f32(x, n, amax, (cudaStream_t)stream);
+}
+
 int fenerf_composite_backward(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse, const float* z_coarse,
                               const float* raw_fine, const float* z_fine, const float* rng_noise, const float* d_pixels,
                               float* d_raw_coarse, float* d_raw_fine, void* stream) {

@@ -150,6 +150,13 @@ int gemm_nt(const void* A, const void* B, long long M, float* c32, void* c16, vo
             const void* A2 = nullptr, const void* B2 = nullptr);
 int gemm_tn(const void* X, const void* Y, int batch, long long ppb, int slices, float* partial, cudaStream_t st,
             float* colsum = nullptr);
+// gemm_split.cu
+int gemm_nt_split(const float* A, const void* B_hi, const void* B_lo, long long M, const float* a_amax, const float* b_amax,
+                  float* c32, float* a_out, float* gate_out, const float* bias, const float* film, long long film_stride,
+                  long long ppb, cudaStream_t st);
+int gemm_tn_split(const float* X, const float* Y, int batch, long long ppb, int slices, const float* x_amax, const float* y_amax,
+                  float* partial, cudaStream_t st);
+int absmax_f32(const float* x, long long n, float* amax, cudaStream_t st);
 // mapping.cu
 int mapping_film(const float* const* w, const float* const* b, const float* z, int B, int z_dim, int n_layers, int layer0,
                  int n_film_total, const float* avg_f, const float* avg_p, float psi, float* h_scratch, float* film,

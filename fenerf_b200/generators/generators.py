@@ -12,6 +12,8 @@ point chunking (SURVEY.md section 8f-2).
 Hidden keyword extras (never passed by the reference's callers, used by tests and bench):
   _rng        an RNG source (volumetric_rendering.ReplayRng) instead of the device generator
   precision   'exact' | 'fast' | 'guard' | 'split' (default: ops.default_precision())
+  grad_precision  None | 'split': the backward of a differentiable 'exact' / 'split' render on the split kernels
+              (backward.render_with_grad); ignored without autograd
   _debug      dict that receives intermediate tensors (inds, depth, weights_sum, poses)
 """
 import warnings
@@ -111,7 +113,8 @@ class _RenderSkeleton:
             # the differentiable call (G step, inversion): same kernels forward, backward in fenerf_b200/backward.py
             from .. import backward
             pixels = backward.render_with_grad(self.siren, rd, film, x_lin, y_lin, z_lin, cam2world,
-                                               rng_perturb.contiguous(), rng_noise_c, rng_u, rng_noise_f, grad_rays=grad_rays)
+                                               rng_perturb.contiguous(), rng_noise_c, rng_u, rng_noise_f, grad_rays=grad_rays,
+                                               grad_precision=kwargs.get('grad_precision'))
             depth = wsum = weights = None
         return pixels, depth, wsum, weights, pitch, yaw
 

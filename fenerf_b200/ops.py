@@ -429,3 +429,80 @@ def gemm_tn(x16, y16, batch, ppb, slices=None, colsum=False):
                                                  ppb, slices, partial.data_ptr(), cs.data_ptr() if colsum else 0, _stream(dev)))
     out = partial.sum(1) if slices > 1 else partial[:, 0]
     return (out, cs.sum(1)) if colsum else out
+
+
+# --------------------------------------------------------------------------------------------
+# split-precision GEMMs of the backward (csrc/gemm_split.cu; grad_precision='split')
+# --------------------------------------------------------------------------------------------
+def split_scale_exp(amax):
+    """Exponent of the power-of-two scale the split kernels give an operand whose largest magnitude is `amax`: 15 - e for
+    amax = m 2^e, m in [0.5, 1), clamped to [-126, 126] (include/fenerf_b200.h)."""
+    return (15 - torch.frexp(amax).exponent).clamp(-126, 126)
+
+
+def split_weights(w):
+    """(..., 256, 256) fp32 -> (hi, lo, amax): each matrix scaled by its own power of two (split_scale_exp of its max |w|,
+    amax (...,)) and split into fp16 hi = f16(s w) and lo = f16(s w - hi).  On the device, no host sync."""
+    w = w.float()
+    amax = w.abs().amax(dim=(-2, -1))
+    s = torch.ldexp(torch.ones_like(amax), split_scale_exp(amax))
+    ws = w * s[..., None, None]
+    hi = ws.to(torch.float16)
+    lo = (ws - hi.float()).to(torch.float16)
+    return hi.contiguous(), lo.contiguous(), amax.contiguous()
+
+
+def absmax(x, out=None):
+    """max |x| of an fp32 tensor as a one-element device tensor (fenerf_absmax_f32; no host sync)."""
+    dev = x.device
+    if out is None:
+        out = torch.empty(1, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().fenerf_absmax_f32(_chk(x, "x", dev), x.numel(), out.data_ptr(), _stream(dev)))
+    return out
+
+
+def gemm_nt_split(a32, b_hi, b_lo, b_amax, a_amax=None, out=None):
+    """(M, 256) fp32 . B^T with B pre-split by split_weights (256, 256) -> (M, 256) fp32 (fenerf_gemm_nt_split).
+    a_amax: max |a| as a device scalar (None: |a| <= 1).  `out`: a contiguous (M, 256) fp32 tensor to write into."""
+    dev = a32.device
+    m = a32.shape[0]
+    if out is None:
+        out = torch.empty((m, 256), dtype=torch.float32, device=dev)
+    elif out.shape != (m, 256) or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError("out must be a contiguous (%d, 256) float32 tensor" % m)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().fenerf_gemm_nt_split(
+            _chk(a32, "A", dev), _chk(b_hi, "B_hi", dev, torch.float16), _chk(b_lo, "B_lo", dev, torch.float16), m,
+            _chk(a_amax, "a_amax", dev), b_amax.data_ptr(), out.data_ptr(), _stream(dev)))
+    return out
+
+
+def gemm_nt_film_split(a32, w_hi, w_lo, w_amax, bias, film, b0, layer, ppb):
+    """One FiLM layer's recompute from fp32 sine activations with the epilogue fused (fenerf_gemm_nt_film_split):
+    -> (a, gate), both (M, 256) fp32."""
+    dev = a32.device
+    m = a32.shape[0]
+    a_out = torch.empty((m, 256), dtype=torch.float32, device=dev)
+    g_out = torch.empty((m, 256), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().fenerf_gemm_nt_film_split(
+            _chk(a32, "A", dev), _chk(w_hi, "W_hi", dev, torch.float16), _chk(w_lo, "W_lo", dev, torch.float16), m,
+            w_amax.data_ptr(), _chk(bias, "bias", dev), film[b0, layer].data_ptr(), film.stride(0), ppb, a_out.data_ptr(),
+            g_out.data_ptr(), _stream(dev)))
+    return a_out, g_out
+
+
+def gemm_tn_split(x32, y32, batch, ppb, x_amax=None, y_amax=None, slices=None):
+    """Per image b: X_b^T Y_b with X, Y (batch * ppb, 256) fp32 -> (batch, 256, 256) fp32 (fenerf_gemm_tn_split; the
+    split-K partials are summed here).  x_amax / y_amax: max |X| / |Y| as device scalars (None: at most 1)."""
+    dev = x32.device
+    if slices is None:
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        slices = max(1, min((ppb + 63) // 64, (sms + batch - 1) // batch))
+    partial = torch.empty((batch, slices, 256, 256), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().fenerf_gemm_tn_split(_chk(x32, "X", dev), _chk(y32, "Y", dev), batch, ppb, slices,
+                                                   _chk(x_amax, "x_amax", dev), _chk(y_amax, "y_amax", dev),
+                                                   partial.data_ptr(), _stream(dev)))
+    return partial.sum(1) if slices > 1 else partial[:, 0]

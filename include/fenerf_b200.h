@@ -425,6 +425,28 @@ int fenerf_gemm_nt_film(const void* A, const void* W, int64_t M, const float* bi
 int fenerf_gemm_tn_f16(const void* X, const void* Y, int32_t batch, int64_t points_per_batch, int32_t slices, float* partial,
                        float* colsum, void* stream);
 
+/* The same three products with fp32-grade results (csrc/gemm_split.cu; the backward of grad_precision='split').  Every
+ * operand is scaled by the power of two 2^(15 - e), where m 2^e (m in [0.5, 1)) is its largest magnitude `*_amax` (a
+ * device scalar; NULL: at most 1, as for sine activations), and split into fp16 hi = f16(s x), lo = f16(s x - hi); each
+ * product is hi.hi + lo.hi + hi.lo with fp32 accumulation and the scales are taken out exactly.  The fp32 streams are
+ * split while they are loaded; B / W come pre-split by the caller, scaled by the power of two of b_amax / w_amax.
+ *   fenerf_gemm_nt_split       c_f32 (M, 256) = A (M, 256) fp32 . B^T, B_hi / B_lo (256, 256) fp16
+ *   fenerf_gemm_nt_film_split  the recompute with its epilogue fused, A (M, 256) fp32 sine activations: a_out =
+ *                              sin(f (z + bias) + p), gate_out = cos(f (z + bias) + p), both (M, 256) fp32 (precise
+ *                              sincosf); film_layer / film_batch_stride / points_per_batch as in fenerf_gemm_nt_film
+ *   fenerf_gemm_tn_split       partial (batch, slices, 256, 256) fp32 as fenerf_gemm_tn_f16, X and Y (batch *
+ *                              points_per_batch, 256) fp32 (no column sums: the split backward takes them from
+ *                              fenerf_gate_backward)
+ *   fenerf_absmax_f32          *amax = max |x| over n fp32 values, on the stream (no host sync)                        */
+int fenerf_gemm_nt_split(const float* A, const void* B_hi, const void* B_lo, int64_t M, const float* a_amax, const float* b_amax,
+                         float* c_f32, void* stream);
+int fenerf_gemm_nt_film_split(const float* A, const void* W_hi, const void* W_lo, int64_t M, const float* w_amax,
+                              const float* bias, const float* film_layer, int64_t film_batch_stride, int64_t points_per_batch,
+                              float* a_out, float* gate_out, void* stream);
+int fenerf_gemm_tn_split(const float* X, const float* Y, int32_t batch, int64_t points_per_batch, int32_t slices,
+                         const float* x_amax, const float* y_amax, float* partial, void* stream);
+int fenerf_absmax_f32(const float* x, int64_t n, float* amax, void* stream);
+
 /* d pixels (B, C-1, H, W) -> d raw outputs.  Backward of the merge + fancy_integration + softmax / *2-1
  * epilogue (generators.py:85-104, volumetric_rendering.py:18-50); same arguments as fenerf_composite.
  * d_raw_fine / raw_fine / z_fine NULL when !hierarchical.  fill modes are staged_forward-only (no_grad).
