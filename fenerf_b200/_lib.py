@@ -39,6 +39,7 @@ EXPORTS = (
     "fenerf_gemm_nt_f16", "fenerf_gemm_nt_film", "fenerf_gemm_tn_f16",
     "fenerf_gemm_nt_split", "fenerf_gemm_nt_film_split", "fenerf_gemm_tn_split", "fenerf_absmax_f32",
     "fenerf_pack_field_bridge", "fenerf_field_fingerprint_bridge",
+    "fenerf_render_rays", "fenerf_rays_workspace_bytes", "fenerf_rays_workspace_layout", "fenerf_composite_backward_rays",
 )
 
 
@@ -83,6 +84,10 @@ class WorkspaceOffsets(C.Structure):
                                           "points_fine", "raw_fine", "total")]
 
 
+class RaysWorkspaceOffsets(C.Structure):
+    _fields_ = [(n, C.c_size_t) for n in ("raw_coarse", "z_fine", "points_fine", "dirs_fine", "raw_fine", "total")]
+
+
 _lib = None
 
 
@@ -115,6 +120,14 @@ def _declare(lib):
     lib.fenerf_workspace_layout.argtypes = [P(RenderDesc), P(FieldDesc), P(WorkspaceOffsets)]
     lib.fenerf_render_forward.restype = C.c_int
     lib.fenerf_render_forward.argtypes = [P(RenderDesc), P(FieldDesc)] + [vp] * 15 + [vp, sz, vp]
+    lib.fenerf_render_rays.restype = C.c_int
+    lib.fenerf_render_rays.argtypes = [P(RenderDesc), P(FieldDesc), vp, vp, vp, vp, i32] + [vp] * 9 + [vp, sz, vp]
+    lib.fenerf_rays_workspace_bytes.restype = sz
+    lib.fenerf_rays_workspace_bytes.argtypes = [P(RenderDesc), P(FieldDesc), i32]
+    lib.fenerf_rays_workspace_layout.restype = C.c_int
+    lib.fenerf_rays_workspace_layout.argtypes = [P(RenderDesc), P(FieldDesc), i32, P(RaysWorkspaceOffsets)]
+    lib.fenerf_composite_backward_rays.restype = C.c_int
+    lib.fenerf_composite_backward_rays.argtypes = [P(RenderDesc), i32] + [vp] * 9
     lib.fenerf_composite_backward.restype = C.c_int
     lib.fenerf_composite_backward.argtypes = [P(RenderDesc), i32] + [vp] * 9
     lib.fenerf_film_forward_stash.restype = C.c_int

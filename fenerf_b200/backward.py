@@ -718,6 +718,95 @@ class RenderFunction(torch.autograd.Function):
         return tuple(out)
 
 
+class RaysRenderFunction(torch.autograd.Function):
+    """pixels (B, N, C-1) = render of caller-supplied rays (fenerf_render_rays; DoubleImplicitGenerator3d.point_forward),
+    differentiable w.r.t. `film` and the field parameters.  The ray tensors are inputs without gradient: the backward
+    below is RenderFunction's with the ray-major compositing backward and the caller's directions."""
+
+    @staticmethod
+    @torch.amp.custom_fwd(device_type='cuda', cast_inputs=torch.float32)
+    def forward(ctx, film, call, *params):
+        module, rd = call['module'], call['rd']
+        st = ops.render_rays_stages(module, rd, film, call['points'], call['dirs'], call['origins'], call['ray_dirs'],
+                                    call['z_vals'], call['rng_noise_c'], call['rng_u'], call['rng_noise_f'])
+        ctx.call, ctx.stages = call, st
+        ctx.save_for_backward(film, *params)
+        ctx.param_ids = [id(p) for p in call['params']]
+        return st['pixels']
+
+    @staticmethod
+    @torch.amp.custom_bwd(device_type='cuda')
+    def backward(ctx, d_pixels):
+        call, st = ctx.call, ctx.stages
+        film = ctx.saved_tensors[0]
+        module, rd = call['module'], call['rd']
+        dev = film.device
+        B, s = rd.batch, rd.num_steps
+        c = st['raw_c'].shape[-1]
+        hier = bool(rd.hierarchical)
+        d_pixels = d_pixels.float().contiguous()
+        with torch.cuda.device(dev), torch.no_grad():
+            d_raw_c = torch.empty_like(st['raw_c'])
+            d_raw_f = torch.empty_like(st['raw_f']) if hier else None
+            noise = call['rng_noise_f'] if rd.noise_std != 0.0 else None
+            _lib.check(_lib.lib().fenerf_composite_backward_rays(
+                C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
+                _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
+                _stream(dev)))
+            m = d_raw_c.abs().max()
+            if hier:
+                m = torch.maximum(m, d_raw_f.abs().max())
+            scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)
+            inv_scale = (1.0 / scale).float().reshape(1)
+            split = rd.precision == _lib.PRECISION['split']
+            fb = _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'],
+                                split=split, grad_split=call.get('grad_precision') == 'split')
+            g = st['dir_group']
+            if hier:
+                # the fine pass: the fine samples' own directions (per-sample), the per-ray ones, or (0, 0, -1)
+                lock = bool(rd.lock_view_dependence)
+                dirs_f = st['dirs_f'] if st['dirs_f'] is not None else st['dirs']
+                fb.add_points(st['points_f'].reshape(B, -1, 3), dirs_f, g, lock, st['raw_f'].reshape(B, -1, c),
+                              d_raw_f.reshape(B, -1, c))
+            # the coarse pass keeps the caller's directions whatever lock_view_dependence says
+            fb.add_points(st['points_c'].reshape(B, -1, 3), st['dirs'], g, False, st['raw_c'].reshape(B, -1, c),
+                          d_raw_c.reshape(B, -1, c))
+            d_film, grads = fb.finish()
+        out = [d_film if ctx.needs_input_grad[0] else None, None]
+        for i, pid in enumerate(ctx.param_ids):
+            gr = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
+            if gr is not None:
+                gr = gr.reshape(ctx.saved_tensors[1 + i].shape)
+            out.append(gr)
+        return tuple(out)
+
+
+#: what a rays-in render refuses to differentiate
+RAYS_GRAD_MESSAGE = ("fenerf_b200: point_forward differentiates w.r.t. the latents and the field parameters only; gradients "
+                     "w.r.t. the sample points, directions, origins or depths are not built (%s requires grad): detach it")
+
+
+def check_rays_no_grad(**tensors):
+    """RuntimeError naming the first ray tensor that requires grad (under autograd): no gradient is silently dropped."""
+    if not torch.is_grad_enabled():
+        return
+    for name, t in tensors.items():
+        if t is not None and t.requires_grad:
+            raise RuntimeError(RAYS_GRAD_MESSAGE % name)
+
+
+def render_rays_with_grad(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f,
+                          grad_precision=None):
+    """Differentiable render of caller-supplied rays (rd from ops.make_rays_desc): (B, N, C-1) pixels with autograd
+    edges to `film` and the field parameters.  `grad_precision` as render_with_grad."""
+    check_grad_precision(module, grad_precision, rd.precision)
+    check_rays_no_grad(points=points, directions=dirs, origins=origins, ray_directions=ray_dirs, z_vals=z_vals)
+    params = FieldWeights(module).parameters()
+    call = dict(module=module, rd=rd, points=points, dirs=dirs, origins=origins, ray_dirs=ray_dirs, z_vals=z_vals,
+                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_precision=grad_precision)
+    return RaysRenderFunction.apply(film, call, *params)
+
+
 def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
                      grad_rays=None, grad_precision=None):
     """Differentiable render: (B, C-1, R, R) pixels with autograd edges to `film` and the field parameters.

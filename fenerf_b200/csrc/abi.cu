@@ -38,6 +38,30 @@ Workspace plan_workspace(const fenerf_render_desc* rd, int C) {
     return w;
 }
 
+// fenerf_render_rays: the coarse inputs are the caller's; dirs_f holds the fine samples' per-sample directions
+struct RaysWorkspace {
+    size_t stats, raw_c, z_f, points_f, dirs_f, raw_f, guard, sigma_c, total;
+};
+
+RaysWorkspace plan_rays_workspace(const fenerf_render_desc* rd, int C, int dir_group) {
+    RaysWorkspace w;
+    size_t n_rays = (size_t)rd->batch * rd->img_h * rd->img_w;
+    size_t pc = n_rays * rd->num_steps;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = fn_align_up(off + bytes, 256); return o; };
+    const bool dirs_f = rd->hierarchical && dir_group == 1 && !rd->lock_view_dependence;
+    w.stats = take(64);               // always at offset 0: fenerf_guard_stats
+    w.raw_c = take(pc * C * 4);
+    w.z_f = take(rd->hierarchical ? pc * 4 : 4);
+    w.points_f = take(rd->hierarchical ? pc * 3 * 4 : 4);
+    w.dirs_f = take(dirs_f ? pc * 3 * 4 : 4);
+    w.raw_f = take(rd->hierarchical ? pc * C * 4 : 4);
+    w.guard = take((n_rays + 1) * 4);
+    w.sigma_c = take(pc * 4);
+    w.total = off;
+    return w;
+}
+
 int check_render_desc(const fenerf_render_desc* rd) {
     FN_REQUIRE(rd, "render desc is NULL");
     FN_REQUIRE(rd->batch >= 1 && rd->img_h >= 1 && rd->img_w >= 1, "bad batch/img size %d %dx%d", rd->batch, rd->img_h,
@@ -335,6 +359,76 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
     return rc;
 }
 
+size_t fenerf_rays_workspace_bytes(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group) {
+    if (!rd || !field) return 0;
+    return plan_rays_workspace(rd, field->out_dim, dir_group).total;
+}
+
+int fenerf_rays_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
+                                 fenerf_rays_workspace_offsets* out) {
+    if (int e = check_render_desc(rd)) return e;
+    FN_REQUIRE(field && out, "NULL argument");
+    RaysWorkspace w = plan_rays_workspace(rd, field->out_dim, dir_group);
+    out->raw_coarse = w.raw_c; out->z_fine = w.z_f; out->points_fine = w.points_f; out->dirs_fine = w.dirs_f;
+    out->raw_fine = w.raw_f; out->total = w.total;
+    return 0;
+}
+
+int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
+                       const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
+                       const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f,
+                       float* pixels, float* depth, float* weights_sum, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+    if (int e = check_render_desc(rd)) return e;
+    FnLayout L;
+    if (int e = make_layout(field, &L)) return e;
+    FN_REQUIRE(rd->img_h == 1, "rays-in render: img_h must be 1 and img_w the number of rays per image (img_h %d)", rd->img_h);
+    FN_REQUIRE(rd->fill_mode == FENERF_FILL_NONE, "rays-in render: no fill modes (fill_mode %d)", rd->fill_mode);
+    FN_REQUIRE(packed && film && points && dirs && z_vals && pixels && workspace, "NULL argument");
+    FN_REQUIRE(dir_group == 1 || dir_group == rd->num_steps, "dir_group %d: 1 (a direction per sample) or num_steps %d "
+               "(one per ray)", dir_group, rd->num_steps);
+    FN_REQUIRE(!rd->hierarchical || (origins && ray_dirs), "hierarchical render needs the per-ray origins and ray_dirs");
+    FN_REQUIRE(!rd->hierarchical || rng_u, "hierarchical render needs rng_u");
+    FN_REQUIRE(!rd->hierarchical || rd->num_steps >= 3, "hierarchical render needs num_steps >= 3");
+    FN_REQUIRE(rd->noise_std == 0.f || (rng_noise_f && (!rd->hierarchical || rng_noise_c)), "noise_std != 0 needs the noise draws");
+    FN_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const int C = L.out_dim;
+    RaysWorkspace w = plan_rays_workspace(rd, C, dir_group);
+    if (workspace_bytes < w.total) return fail(FENERF_E_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, w.total);
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    float* raw_c = (float*)(ws + w.raw_c);
+    float* z_f = (float*)(ws + w.z_f);
+    float* points_f = (float*)(ws + w.points_f);
+    float* dirs_f = (float*)(ws + w.dirs_f);
+    float* raw_f = (float*)(ws + w.raw_f);
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long rays = rd->img_w;
+    const long long ppb = rays * rd->num_steps;
+    const float* noise_c = rd->noise_std != 0.f ? rng_noise_c : nullptr;
+    const float* noise_f = rd->noise_std != 0.f ? rng_noise_f : nullptr;
+
+    // the coarse pass keeps the caller's directions whatever lock_view_dependence says (generators.py:810)
+    float* sigma_c = (rd->hierarchical && rd->precision != FENERF_PRECISION_EXACT) ? (float*)(ws + w.sigma_c) : nullptr;
+    if (int e = run_field(L, packed, points, dirs, film, rd->batch, ppb, dir_group, 0, rd->precision, raw_c, st, 0, sigma_c))
+        return e;
+    if (rd->precision == FENERF_PRECISION_GUARD) {
+        float tau = rd->guard_tau > 0.f ? rd->guard_tau : 1.5e-3f;
+        const int n_samples = rd->hierarchical ? 2 * rd->num_steps : rd->num_steps;
+        if (int e = guard_refine(L, (const unsigned char*)packed, points, dirs, film, rd->batch, rays, rd->num_steps, 0, tau,
+                                 noise_f ? noise_f + (n_samples - 1) : nullptr, n_samples, rd->noise_std, raw_c,
+                                 (int32_t*)(ws + w.guard), (int32_t*)(ws + w.stats), st, dir_group)) return e;
+    }
+    if (rd->hierarchical) {
+        const bool per_sample = dir_group == 1 && !rd->lock_view_dependence;
+        if (int e = resample_rays(rd, C, raw_c, z_vals, ray_dirs, origins, noise_c, rng_u, z_f, points_f,
+                                  per_sample ? dirs : nullptr, per_sample ? dirs_f : nullptr, sigma_c, st)) return e;
+        if (int e = run_field(L, packed, points_f, per_sample ? dirs_f : dirs, film, rd->batch, ppb, dir_group,
+                              rd->lock_view_dependence, rd->precision, raw_f, st)) return e;
+    }
+    return composite_rays(rd, C, raw_c, z_vals, rd->hierarchical ? raw_f : nullptr, rd->hierarchical ? z_f : nullptr, noise_f,
+                          pixels, depth, weights_sum, st);
+}
+
 int fenerf_mapping_film(const fenerf_mapping_params* net, const float* z, int32_t batch, int32_t n_layers, int32_t first_layer,
                         int32_t n_film_total, const float* avg_frequencies, const float* avg_phase_shifts, float psi,
                         float* h_scratch, float* film, void* stream) {
@@ -425,6 +519,16 @@ int fenerf_composite_backward(const fenerf_render_desc* rd, int32_t out_dim, con
     FN_REQUIRE(rd->noise_std == 0.f || rng_noise, "noise_std != 0 needs rng_noise");
     return composite_backward(rd, out_dim, raw_coarse, z_coarse, raw_fine, z_fine, rd->noise_std != 0.f ? rng_noise : nullptr,
                               d_pixels, d_raw_coarse, d_raw_fine, (cudaStream_t)stream);
+}
+
+int fenerf_composite_backward_rays(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse,
+                                   const float* z_coarse, const float* raw_fine, const float* z_fine, const float* rng_noise,
+                                   const float* d_pixels, float* d_raw_coarse, float* d_raw_fine, void* stream) {
+    if (int e = check_render_desc(rd)) return e;
+    FN_REQUIRE(raw_coarse && z_coarse && d_pixels && d_raw_coarse, "NULL argument");
+    FN_REQUIRE(rd->noise_std == 0.f || rng_noise, "noise_std != 0 needs rng_noise");
+    return composite_backward(rd, out_dim, raw_coarse, z_coarse, raw_fine, z_fine, rd->noise_std != 0.f ? rng_noise : nullptr,
+                              d_pixels, d_raw_coarse, d_raw_fine, (cudaStream_t)stream, 1);
 }
 
 int fenerf_film_forward_stash(const float* z, const float* bias, const float* film_layer, int64_t film_batch_stride,

@@ -122,10 +122,11 @@ constexpr const char* kSplitUnsupported =
 // debug: which instantiation siren_points_fast launches (0 production; siren_fast_debug.cu) and the device software sine
 int siren_fast_debug_variant(int variant, unsigned long long* trace, int trace_ctas);
 int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st);
+// dir_group: points per direction of `dirs` (0: num_steps, one per ray; 1: one per sample, fenerf_render_rays)
 int guard_refine(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
                  const float* film, int batch, long long rays_per_batch, int num_steps, int lock_dirs, float tau,
                  const float* noise_far, long long noise_stride, float noise_std,
-                 float* raw, int32_t* scratch_idx, int32_t* stats, cudaStream_t st);
+                 float* raw, int32_t* scratch_idx, int32_t* stats, cudaStream_t st, int dir_group = 0);
 int camera_poses(int n, int mode, float h_std, float v_std, float h_mean, float v_mean, const float* draw_theta,
                  const float* draw_phi, float* c2w, float* pitch, float* yaw, cudaStream_t st);
 int ray_setup(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
@@ -134,15 +135,25 @@ int ray_setup(const fenerf_render_desc* rd, const float* x_lin, const float* y_l
 int resample(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* dirs,
              const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
              long long* inds, cudaStream_t st, int sort_fine = 0, const float* sigma_compact = nullptr);
+// fenerf_render_rays' resampler (resample_rays.cu): per-ray origins (B, N, 3); the fine samples depth-sorted.  With
+// dirs_sample (B, N, S, 3) (per-sample directions), fine sample k of sample_pdf's order takes direction slot k and
+// dirs_fine (B, N, S, 3) receives those directions in the sorted order
+int resample_rays(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* ray_dirs,
+                  const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
+                  const float* dirs_sample, float* dirs_fine, const float* sigma_compact, cudaStream_t st);
 int composite_sorted(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                      const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
                      cudaStream_t st);
 int composite(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
               const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
               int32_t* sort_idx, cudaStream_t st);
+// rays = 1: d_pixels ray-major (B, N, C-1) of pixels in [0, 1] (fenerf_composite_backward_rays)
 int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                        const float* z_f, const float* noise, const float* d_pixels, float* d_raw_c, float* d_raw_f,
-                       cudaStream_t st);
+                       cudaStream_t st, int rays = 0);
+// fenerf_render_rays' compositor: both lists depth-sorted, pixels ray-major (B, N, C-1) in [0, 1]
+int composite_rays(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
+                   const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, cudaStream_t st);
 
 // gemm.cu
 int gemm_nt(const void* A, const void* B, long long M, float* c32, void* c16, void* a_out, void* gate_out, const float* bias,

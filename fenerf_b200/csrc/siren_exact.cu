@@ -479,7 +479,7 @@ __global__ void guard_scan_kernel(const float* __restrict__ raw, long long n_ray
 int guard_refine(const FnLayout& L, const unsigned char* packed, const float* points, const float* dirs,
                  const float* film, int batch, long long rays_per_batch, int num_steps, int lock_dirs, float tau,
                  const float* noise_far, long long noise_stride, float noise_std,
-                 float* raw, int32_t* scratch_idx, int32_t* stats, cudaStream_t st) {
+                 float* raw, int32_t* scratch_idx, int32_t* stats, cudaStream_t st, int dir_group) {
     long long n_rays = rays_per_batch * batch;
     FN_REQUIRE(n_rays * num_steps < 2147483647LL, "too many points for the 32-bit guard list");
     FN_CUDA_OK(cudaMemsetAsync(scratch_idx, 0, sizeof(int32_t), st));
@@ -493,7 +493,7 @@ int guard_refine(const FnLayout& L, const unsigned char* packed, const float* po
     ExactArgs a;
     a.L = L; a.packed = packed; a.points = points; a.dirs = dirs; a.film = film; a.out = raw;
     a.only_idx = scratch_idx + 1; a.n_only_dev = scratch_idx; a.n_only = 0; a.n_items = 0;
-    a.ppb = rays_per_batch * num_steps; a.tiles_per_batch = 1; a.dir_group = num_steps; a.lock_dirs = lock_dirs;
+    a.ppb = rays_per_batch * num_steps; a.tiles_per_batch = 1; a.dir_group = dir_group > 0 ? dir_group : num_steps; a.lock_dirs = lock_dirs;
     a.sigma_only = 1;      // only the sign of the far sample's density matters; its colour stays the wgmma one
     a.guard_stats = stats;
     // (stats[0..2] were zeroed and stats[3] = tau written by guard_scan_kernel's launch above: no host memory is

@@ -349,6 +349,50 @@ class DoubleImplicitGenerator3d(_RenderSkeleton, nn.Module):
             hierarchical_sample, sample_dist, lock_view_dependence, kwargs, staged=False)
         return pixels, torch.cat([pitch, yaw], -1)
 
+    def point_forward(self, transformed_points, transformed_ray_directions_expanded, transformed_ray_origins,
+                      transformed_ray_directions, z_vals, z_geo, z_app, num_steps, hierarchical_sample,
+                      lock_view_dependence=False, **kwargs):
+        """The render of caller-supplied rays (generators.py:800-856): coarse points (B, N, S, 3) used as given, their
+        directions (B, N, S, 3) or (B, N*S, 3), per-ray origins and directions (B, N, 3) for the fine points, depths
+        (B, N, S, 1); any N.  Returns the pixels (B, N, C-1), ray-major in [0, 1] (no permute, no *2-1).
+        lock_view_dependence locks the FINE pass's directions only, as the reference does.  Differentiable w.r.t. the
+        latents and the field; a ray tensor that requires grad is refused (RuntimeError).  One fenerf_render_rays call;
+        directions that are an expand() of per-ray ones (stride 0 along S) go in once per ray."""
+        from .. import backward
+        backward.check_rays_no_grad(transformed_points=transformed_points,
+                                    transformed_ray_directions_expanded=transformed_ray_directions_expanded,
+                                    transformed_ray_origins=transformed_ray_origins,
+                                    transformed_ray_directions=transformed_ray_directions, z_vals=z_vals)
+        clamp_mode, noise_std = kwargs['clamp_mode'], kwargs['nerf_noise']
+        device = torch.device(self.device)
+        if device.type != 'cuda':
+            raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to an H100 (got %s)" % device)
+        rng = kwargs.get('_rng') or vr.DeviceRng(device)
+        batch_size, n_rays = transformed_points.shape[:2]
+        dirs = transformed_ray_directions_expanded
+        if dirs.dim() == 4 and dirs.shape[2] == num_steps and dirs.stride(2) == 0:
+            dirs = dirs[:, :, 0]            # the same direction for every sample of a ray: one per ray (dir_group S)
+        film = self.siren.film_from_latents(z_geo, z_app)
+        with torch.no_grad():
+            rng_noise_c = rng_u = None
+            if hierarchical_sample:
+                rng_noise_c = rng.randn(batch_size, n_rays, num_steps, 1)              # draw #4
+                rng_u = rng.rand(batch_size * n_rays, num_steps)                       # draw #5
+            n_samples = 2 * num_steps if hierarchical_sample else num_steps
+            rng_noise_f = rng.randn(batch_size, n_rays, n_samples, 1)                  # draw #6
+            rd = ops.make_rays_desc(
+                batch=batch_size, n_rays=n_rays, num_steps=num_steps, hierarchical=hierarchical_sample,
+                clamp_mode=clamp_mode, nerf_noise=noise_std, last_back=kwargs.get('last_back', False),
+                white_back=kwargs.get('white_back', False), black_back=kwargs.get('black_back', False),
+                softmax_label=self.softmax_label, lock_view_dependence=lock_view_dependence,
+                precision=kwargs.get('precision'), guard_tau=kwargs.get('guard_tau', getattr(self.siren, '_guard_tau', 0.0)))
+        args = (transformed_points, dirs, transformed_ray_origins, transformed_ray_directions, z_vals, rng_noise_c, rng_u,
+                rng_noise_f)
+        if ops.needs_grad(self.siren, film):
+            return backward.render_rays_with_grad(self.siren, rd, film, *args, grad_precision=kwargs.get('grad_precision'))
+        with torch.no_grad():
+            return ops.render_rays(self.siren, rd, film, *args)[0]
+
     def part_forward(self, z_geo, z_app, img_size, fov, ray_start, ray_end, num_steps, h_stddev, v_stddev, h_mean,
                      v_mean, hierarchical_sample, sample_dist=None, lock_view_dependence=False, **kwargs):
         """Ray-subset training (generators.py:858-910): every ray is rendered, `grad_points` randomly chosen ones carry

@@ -352,6 +352,126 @@ def render_forward_stages(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_
     return st
 
 
+# --------------------------------------------------------------------------------------------
+# rays-in render (fenerf_render_rays): DoubleImplicitGenerator3d.point_forward after the mapping networks
+# --------------------------------------------------------------------------------------------
+def make_rays_desc(*, batch, n_rays, num_steps, hierarchical, clamp_mode, nerf_noise, last_back=False, white_back=False,
+                   black_back=False, softmax_label=False, lock_view_dependence=False, precision=None, guard_tau=0.0):
+    """The render descriptor of a rays-in render: img_h = 1, img_w = the rays per image; no fill mode, no field of view."""
+    rd = make_render_desc(batch=batch, img_size=1, num_steps=num_steps, hierarchical=hierarchical, clamp_mode=clamp_mode,
+                          nerf_noise=nerf_noise, fov=0.0, last_back=last_back, white_back=white_back, black_back=black_back,
+                          softmax_label=softmax_label, lock_view_dependence=lock_view_dependence, precision=precision,
+                          guard_tau=guard_tau)
+    rd.img_w = int(n_rays)
+    return rd
+
+
+def rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device):
+    """Checks and lays out the ray tensors of a rays-in render -> (points (B,N,S,3), dirs, dir_group, origins, ray_dirs,
+    z_vals (B,N,S)).  dirs (B,N,S,3) / (B,N*S,3) is one direction per sample (dir_group 1), (B,N,3) one per ray
+    (dir_group S).  origins / ray_dirs (B,N,3) are only read by a hierarchical render (None otherwise)."""
+    b, n, s = rd.batch, rd.img_w, rd.num_steps
+    pts = _prep(points, device)
+    if pts.shape != (b, n, s, 3):
+        raise ValueError("points must be (B, N, S, 3) = %s, got %s" % ((b, n, s, 3), tuple(pts.shape)))
+    d = _prep(dirs, device)
+    if d.numel() == b * n * s * 3:
+        d, dir_group = d.reshape(b, n * s, 3), 1
+    elif d.numel() == b * n * 3:
+        d, dir_group = d.reshape(b, n, 3), s
+    else:
+        raise ValueError("directions must be (B, N, S, 3), (B, N*S, 3) or (B, N, 3), got %s" % (tuple(dirs.shape),))
+    z = _prep(z_vals, device)
+    if z.numel() != b * n * s:
+        raise ValueError("z_vals must be (B, N, S[, 1]) = %s, got %s" % ((b, n, s), tuple(z_vals.shape)))
+    z = z.reshape(b, n, s)
+    o = rdir = None
+    if rd.hierarchical:
+        o, rdir = _prep(origins, device), _prep(ray_dirs, device)
+        for t, name in ((o, "origins"), (rdir, "ray_dirs")):
+            if t.numel() != b * n * 3:
+                raise ValueError("%s must be (B, N, 3) = %s, got %s" % (name, (b, n, 3), tuple(t.shape)))
+        o, rdir = o.reshape(b, n, 3), rdir.reshape(b, n, 3)
+    return pts, d, dir_group, o, rdir, z
+
+
+def _rays_call(lib, rd, packed, film, pts, dirs, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, depth,
+               wsum, ws_ptr, ws_bytes, device):
+    _lib.check(lib.fenerf_render_rays(
+        C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device), _chk(pts, "points", device),
+        _chk(dirs, "dirs", device), dir_group, _chk(o, "origins", device), _chk(rdir, "ray_dirs", device),
+        _chk(z, "z_vals", device), _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device),
+        _chk(rng_noise_f, "rng_noise_f", device), pixels.data_ptr(), depth.data_ptr() if depth is not None else 0,
+        wsum.data_ptr() if wsum is not None else 0, ws_ptr, ws_bytes, _stream(device)))
+
+
+def _film_for(packed, film, device, b):
+    packed_desc = packed.desc
+    film = _prep(film, device)
+    n_film = packed_desc.trunk_layers + packed_desc.color_layers + (1 if packed_desc.reserved & _lib.FIELD_LABEL_FILM else 0)
+    if film.shape != (b, n_film, 2, _lib.HIDDEN):
+        raise ValueError("film table has shape %s" % (tuple(film.shape),))
+    return film
+
+
+def render_rays(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f,
+                want_depth=False, want_weights_sum=False):
+    """One call into fenerf_render_rays (rd from make_rays_desc): the render of caller-supplied rays.
+    Returns (pixels (B, N, C-1) ray-major in [0, 1], depth (B, N, 1) or None, weights_sum (B, N, 1) or None)."""
+    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
+    device = packed.device
+    lib = _lib.lib()
+    b, n = rd.batch, rd.img_w
+    c = packed.desc.out_dim
+    film = _film_for(packed, film, device, b)
+    pts, d, dir_group, o, rdir, z = rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device)
+    pixels = torch.empty((b, n, c - 1), dtype=torch.float32, device=device)
+    depth = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_depth else None
+    wsum = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_weights_sum else None
+    with torch.cuda.device(device):
+        nbytes = lib.fenerf_rays_workspace_bytes(C.byref(rd), C.byref(packed.desc), dir_group)
+        ws = _workspace(device, nbytes)
+        ws_ptr = (ws.data_ptr() + 255) // 256 * 256
+        _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, depth, wsum,
+                   ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()), device)
+    return pixels, depth, wsum
+
+
+def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f):
+    """fenerf_render_rays into a PRIVATE workspace, returned with typed views of what it leaves there
+    (fenerf_rays_workspace_layout) and the laid-out inputs: what the backward consumes (fenerf_b200/backward.py)."""
+    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
+    device = packed.device
+    lib = _lib.lib()
+    b, n, s = rd.batch, rd.img_w, rd.num_steps
+    c = packed.desc.out_dim
+    film = _film_for(packed, film, device, b)
+    pts, d, dir_group, o, rdir, z = rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device)
+    pixels = torch.empty((b, n, c - 1), dtype=torch.float32, device=device)
+    off = _lib.RaysWorkspaceOffsets()
+    with torch.cuda.device(device):
+        _lib.check(lib.fenerf_rays_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off)))
+        ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
+        base = (ws.data_ptr() + 255) // 256 * 256 - ws.data_ptr()
+        _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, None, None,
+                   ws.data_ptr() + base, ws.numel() - base, device)
+
+    def view(offset, shape):
+        numel = 1
+        for e in shape:
+            numel *= e
+        return ws[base + offset: base + offset + numel * 4].view(torch.float32).view(shape)
+
+    st = dict(pixels=pixels, workspace=ws, points_c=pts, z_c=z, dirs=d, dir_group=dir_group,
+              raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None, dirs_f=None)
+    if rd.hierarchical:
+        st.update(points_f=view(off.points_fine, (b, n, s, 3)), z_f=view(off.z_fine, (b, n, s)),
+                  raw_f=view(off.raw_fine, (b, n, s, c)))
+        if dir_group == 1 and not rd.lock_view_dependence:
+            st.update(dirs_f=view(off.dirs_fine, (b, n * s, 3)))
+    return st
+
+
 def mapping_film(net, z, film, first_layer, n_layers, avg=None, psi=1.0):
     """fenerf_mapping_film: CustomMappingNetwork + `15 f + 30` (+ psi truncation towards `avg` = (avg_frequencies,
     avg_phase_shifts)) written straight into layers [first_layer, first_layer + n_layers) of the FiLM table

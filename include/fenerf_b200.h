@@ -365,6 +365,48 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
                           int64_t* inds_dbg, void* workspace, size_t workspace_bytes,
                           void* stream);
 
+/* ---- rays-in render ------------------------------------------------------------------------------
+ * The render of caller-supplied rays: DoubleImplicitGenerator3d.point_forward (generators/generators.py:800-856) after
+ * the mapping networks -- patch or crop rendering, custom camera models, ray subsets.  No ray set-up runs: the coarse
+ * points, depths and directions go to the point network and the compositor as given (the points are NOT recomputed
+ * from origin + dir * z).  rd->img_h = 1 and rd->img_w = N, any number of rays per image; rd->fill_mode must be
+ * FENERF_FILL_NONE.
+ *   points      (B, N, S, 3) coarse sample points
+ *   dirs        (B, N*S/dir_group, 3): dir_group 1, one direction per sample (the reference's expanded directions), or
+ *               dir_group S, one per ray.  The coarse pass always reads them; rd->lock_view_dependence replaces the
+ *               directions with (0, 0, -1) for the FINE pass only, as the reference does (generators.py:830-833)
+ *   origins     (B, N, 3) per-ray origins and ray_dirs (B, N, 3) per-ray directions: the fine points are
+ *               origins + ray_dirs * z_fine (generators.py:828); NULL when !rd->hierarchical
+ *   z_vals      (B, N, S) coarse depths, ascending along each ray (as every camera's stratified samples are; the
+ *               compositor merges the fine samples into them and the GUARD refinement takes sample S-1 as the far one --
+ *               not checked)
+ *   rng_noise_c (B, N, S) #4, rng_u (B*N, S) #5, rng_noise_f (B, N, S') #6, as fenerf_render_forward
+ *   pixels      (B, N, C-1) ray-major, in [0, 1]: no *2-1 (softmax over the label channels with rd->softmax_label)
+ *   depth / weights_sum (B, N) or NULL
+ * Fine sample k of sample_pdf's order takes direction slot k (dir_group 1): the resampler carries the slot through its
+ * depth sort and leaves the fine samples' directions in the workspace (dirs_fine below).                            */
+int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
+                       const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
+                       const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f,
+                       float* pixels, float* depth, float* weights_sum, void* workspace, size_t workspace_bytes,
+                       void* stream);
+
+/* Scratch of fenerf_render_rays and where it leaves its intermediates (byte offsets; the coarse inputs are the
+ * caller's own tensors): what the backward needs.  fenerf_guard_stats reads the same workspace.  The fine entries only
+ * when rd->hierarchical; dirs_fine only with dir_group 1 and without rd->lock_view_dependence (else the fine pass reads
+ * the caller's `dirs`, or none). */
+typedef struct fenerf_rays_workspace_offsets {
+    size_t raw_coarse;     /* (B,N,S,C) after the GUARD refinement */
+    size_t z_fine;         /* (B,N,S)   depth-sorted */
+    size_t points_fine;    /* (B,N,S,3) */
+    size_t dirs_fine;      /* (B,N,S,3) */
+    size_t raw_fine;       /* (B,N,S,C) */
+    size_t total;
+} fenerf_rays_workspace_offsets;
+size_t fenerf_rays_workspace_bytes(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group);
+int fenerf_rays_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
+                                 fenerf_rays_workspace_offsets* out);
+
 /* ---- mapping network -> FiLM table -------------------------------------------------------------------
  * CustomMappingNetwork (siren/siren.py:82-102: Linear(z, 256) + LeakyReLU(0.2), 3 x [Linear(256, 256) + LeakyReLU],
  * Linear(256, n_layers * 512)), the halves split into frequencies / phase shifts (:100-101), the `15 f + 30`
@@ -455,6 +497,13 @@ int fenerf_composite_backward(const fenerf_render_desc* rd, int32_t out_dim, con
                               const float* z_coarse, const float* raw_fine, const float* z_fine,
                               const float* rng_noise, const float* d_pixels,
                               float* d_raw_coarse, float* d_raw_fine, void* stream);
+
+/* The same backward for fenerf_render_rays' ray-major pixels: d_pixels (B, N, C-1) of pixels in [0, 1] (no *2-1
+ * factor); N = rd->img_h * rd->img_w.  Otherwise as fenerf_composite_backward. */
+int fenerf_composite_backward_rays(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse,
+                                   const float* z_coarse, const float* raw_fine, const float* z_fine,
+                                   const float* rng_noise, const float* d_pixels, float* d_raw_coarse, float* d_raw_fine,
+                                   void* stream);
 
 /* One FiLM layer's forward values for the backward (siren/siren.py:113-123): from the GEMM output
  * z (n_points, 256) fp32 (NULL for the first layer) plus optional narrow inputs narrow_in (n_points, w) fp32
