@@ -141,7 +141,7 @@ def _fill(out, wsum, fill_mode, fill_color):
     return out
 
 
-def composite_ref(raw_c, z_c, raw_f, z_f, noise, opt, offset=None, full=False):
+def composite_ref(raw_c, z_c, raw_f, z_f, noise, opt, offset=None, full=False, ray_major=False):
     """float64 pixels (B, C_img, R, R) of the final compositing.  raw_* float64 (B, N, S, C), possibly requiring grad;
     z_* (B, N, S) and noise (B, N, n) are the kernel's own fp32 inputs (noise is in merged-sample order).
 
@@ -149,7 +149,8 @@ def composite_ref(raw_c, z_c, raw_f, z_f, noise, opt, offset=None, full=False):
     function must stay smooth under perturbation), so the relu sees the same sign as in the kernel.  Then
     oracle.alpha_composite in float64, the fill mode (C_img = C - 1, or C with the seg-padding background channel), the
     label softmax over the channels before the last three (so over [background, labels] with padding) and `* 2 - 1` to
-    NCHW.  full: -> (pixels, depth (B, N), weights_sum (B, N), weights (B, N, n)) instead."""
+    NCHW.  ray_major: the rays-in render's pixels instead, (B, N, C - 1) in [0, 1] for any N (no `* 2 - 1`, no
+    reshape).  full: -> (pixels, depth (B, N), weights_sum (B, N), weights (B, N, n)) instead."""
     raw, z = _merge(raw_c, z_c, raw_f, z_f)
     sig = raw[..., -1]
     if noise is not None:
@@ -161,9 +162,10 @@ def composite_ref(raw_c, z_c, raw_f, z_f, noise, opt, offset=None, full=False):
     px = _fill(px, wsum[..., 0], opt.get("fill_mode"), opt.get("fill_color", "black"))
     if opt["softmax"]:
         px = torch.cat([torch.softmax(px[..., :-3], -1), px[..., -3:]], -1)
-    b, n = px.shape[:2]
-    r = math.isqrt(n)
-    px = px.reshape(b, r, r, -1).permute(0, 3, 1, 2) * 2 - 1
+    if not ray_major:
+        b, n = px.shape[:2]
+        r = math.isqrt(n)
+        px = px.reshape(b, r, r, -1).permute(0, 3, 1, 2) * 2 - 1
     if not full:
         return px
     return px, depth[..., 0], wsum[..., 0], weights[..., 0]

@@ -141,7 +141,9 @@ def restate_point_forward(field, film, points, dirs_expanded, origins, ray_dirs,
     order, every draw through the oracle's recorder) on the caller's rays: points (B,N,S,3) used as given, dirs_expanded
     (B,N,S,3) or (B,N*S,3), per-ray origins / ray_dirs (B,N,3) for the fine points, z_vals (B,N,S,1).  cfg keys:
     num_steps hierarchical_sample clamp_mode nerf_noise [lock_view_dependence last_back white_back black_back
-    softmax_label].  Returns a dict: pixels (B,N,C-1) in [0,1], ray-major; draws.
+    softmax_label].  Returns a dict: pixels (B,N,C-1) in [0,1], ray-major; draws; stages: the intermediates (per-point
+    directions (B,N*S,3) and raw outputs (B,N,S,C) of the coarse pass; hierarchical: fine depths (B,N,S) in sample_pdf's
+    order, the fine points, their directions and raw outputs).
     fault (the fault tests only): 'sorted_dirs' pairs the fine samples with the directions in depth order instead of
     sample_pdf's order; 'lock_coarse' locks the coarse pass's directions too."""
     draws = draws or oracle.Draws()
@@ -154,6 +156,7 @@ def restate_point_forward(field, film, points, dirs_expanded, origins, ray_dirs,
             dirs_pp = torch.zeros_like(dirs_pp)
             dirs_pp[..., -1] = -1
         coarse = oracle.field_eval(field, pts, film, dirs_pp).reshape(b, n, s, -1)
+        stages = dict(dirs_coarse=dirs_pp, raw_coarse=coarse)
         if cfg['hierarchical_sample']:
             _, _, w, _ = oracle.alpha_composite(coarse, z_vals, draws, cfg['nerf_noise'], cfg['clamp_mode'])   # draw 4
             w = w.reshape(-1, s) + 1e-5
@@ -171,6 +174,7 @@ def restate_point_forward(field, film, points, dirs_expanded, origins, ray_dirs,
                 rank = torch.argsort(order, dim=-1, stable=True)       # fine sample k gets the slot of its depth rank
                 dirs_f = torch.gather(dirs_pp.reshape(b, n, s, 3), 2, rank.unsqueeze(-1).expand(-1, -1, -1, 3)).reshape(b, -1, 3)
             fine = oracle.field_eval(field, pts_f.reshape(b, -1, 3), film, dirs_f).reshape(b, n, s, -1)
+            stages.update(z_fine=z_fine[..., 0], points_fine=pts_f, dirs_fine=dirs_f, raw_fine=fine)
             all_raw = torch.cat([fine, coarse], dim=-2)
             all_z = torch.cat([z_fine, z_vals], dim=-2)
             _, order = torch.sort(all_z, dim=-2)
@@ -183,7 +187,7 @@ def restate_point_forward(field, film, points, dirs_expanded, origins, ray_dirs,
                                              black_back=cfg.get('black_back', False))                          # draw 6
         if cfg.get('softmax_label', False):
             px = torch.cat([torch.nn.Softmax(dim=-1)(px[..., :-3]), px[..., -3:]], dim=-1)
-    return dict(pixels=px, draws=draws.log)
+    return dict(pixels=px, draws=draws.log, stages=stages)
 
 
 def oracle_run(case, rays=None, fault=None):

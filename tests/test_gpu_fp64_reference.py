@@ -4,7 +4,9 @@ The parity tests elsewhere compare whole renders at 12²-16² pixels with 9-12 s
 checked on its own against a float64 restatement of the same operation, at the shapes where it changes behaviour:
 
   A. ``fenerf_composite_backward`` with 8-128 merged samples (the 32-sample scan chunks and their carry, the dynamic
-     shared-memory opt-in beyond 48 KB), 4-32 channels, every compositing option, exact depth ties;
+     shared-memory opt-in beyond 48 KB), 4-32 channels, every compositing option, exact depth ties; and, as a second
+     entry ('-rays'), ``fenerf_composite_backward_rays`` (ray-major pixels in [0, 1]: its own kernel and opt-in), bit
+     for bit the NCHW entry's result on the same upstream value (measured: 2.3e-6 at n = 128, C = 22, softplus + noise);
   B. ``_FieldBackward`` for every field class under the chunk layouts of production: several images per chunk
      (FiLM rows of image b0 > 0) and one image split into point chunks (directions sliced at p0 // dir_group);
   C. the point network forward (exact and fast kernels) under the tile schedules of a real SM count.
@@ -88,10 +90,10 @@ def _per_point(dirs, ppb, lock):
 # --------------------------------------------------------------------------------------------
 # 0. float64 references
 # --------------------------------------------------------------------------------------------
-def composite_vjp(raw_c, z_c, raw_f, z_f, noise, opt, d_pixels):
-    """(d raw_c, d raw_f) in float64 for the upstream gradient d_pixels."""
+def composite_vjp(raw_c, z_c, raw_f, z_f, noise, opt, d_pixels, ray_major=False):
+    """(d raw_c, d raw_f) in float64 for the upstream gradient d_pixels (NCHW, or (B, N, C - 1) with ray_major)."""
     leaves = [raw_c.double().requires_grad_(True)] + ([raw_f.double().requires_grad_(True)] if raw_f is not None else [])
-    px = composite_ref(leaves[0], z_c, leaves[1] if raw_f is not None else None, z_f, noise, opt)
+    px = composite_ref(leaves[0], z_c, leaves[1] if raw_f is not None else None, z_f, noise, opt, ray_major=ray_major)
     grads = torch.autograd.grad((px * d_pixels.double()).sum(), leaves)
     return grads[0], (grads[1] if raw_f is not None else None)
 
@@ -211,6 +213,14 @@ _COMPOSITE += [(n, hier, c, o, opaque) for n, hier in [(33, False), (96, True), 
                                     (22, "relu_softmax", False), (23, "softplus_noise_softmax", True)]]
 _COMPOSITE_MODEL = {4: "A", 22: "D", 23: "E", 32: "D32"}
 _B, _R = 3, 37          # 37² rays per image: not a multiple of the 8 rays of a composite_backward block
+#: the two entries of the compositing backward: NCHW pixels * 2 - 1 (fenerf_composite_backward, the ids without a
+#: suffix) and ray-major pixels in [0, 1] (fenerf_composite_backward_rays, the rays-in render's; ids '-rays')
+ENTRIES = ("nchw", "rays")
+
+
+def with_entries(cases, ids):
+    """Every case on both compositing-backward entries; the NCHW entry keeps the case's id."""
+    return [pytest.param(*case, e, id=i + ("" if e == "nchw" else "-" + e)) for case, i in zip(cases, ids) for e in ENTRIES]
 
 
 @functools.lru_cache(maxsize=None)
@@ -236,40 +246,67 @@ def _composite_inputs(c, steps, hier, opaque):
     return out
 
 
-def _composite_backward(opt, steps, hier, x, noise, d_pixels):
+def _composite_backward(opt, steps, hier, x, noise, d_pixels, entry="nchw", batch=_B, img=_R):
+    """One entry of the compositing backward; the gradient buffers start as NaN (an entry not written stays NaN).
+    'rays': the rays-in render's descriptor, img_h = 1 and img_w = the img² rays per image."""
     c = x["raw_c"].shape[-1]
-    rd = ops.make_render_desc(batch=_B, img_size=_R, num_steps=steps, hierarchical=hier, clamp_mode=opt["clamp"],
+    rd = ops.make_render_desc(batch=batch, img_size=img, num_steps=steps, hierarchical=hier, clamp_mode=opt["clamp"],
                               nerf_noise=opt["noise"], fov=12, last_back=opt["last_back"], white_back=opt["white_back"],
                               black_back=opt["black_back"], softmax_label=opt["softmax"])
-    d_c = torch.empty_like(x["raw_c"])
-    d_f = torch.empty_like(x["raw_f"]) if hier else None
+    lib = _lib.lib()
+    fn = lib.fenerf_composite_backward
+    if entry == "rays":
+        rd.img_h, rd.img_w = 1, img * img
+        fn = lib.fenerf_composite_backward_rays
+    d_c = torch.full_like(x["raw_c"], float("nan"))
+    d_f = torch.full_like(x["raw_f"], float("nan")) if hier else None
     p = lambda t: t.data_ptr() if t is not None else 0                  # noqa: E731
-    _lib.check(_lib.lib().fenerf_composite_backward(
-        ctypes.byref(rd), c, p(x["raw_c"]), p(x["z_c"]), p(x["raw_f"]), p(x["z_f"]), p(noise), p(d_pixels), p(d_c), p(d_f),
-        torch.cuda.current_stream().cuda_stream))
+    _lib.check(fn(ctypes.byref(rd), c, p(x["raw_c"]), p(x["z_c"]), p(x["raw_f"]), p(x["z_f"]), p(noise), p(d_pixels), p(d_c),
+                  p(d_f), torch.cuda.current_stream().cuda_stream))
     return d_c, d_f
 
 
+def composite_backward_errors(o, steps, hier, x, noise, g, entry, batch=_B, img=_R):
+    """The compositing backward of `entry` on a d_pixels drawn from `g`, against composite_vjp -> (dict of the kernel's
+    d_c, d_f and the float64 w_c, w_f; relative errors).
+    'rays' is also run on the NCHW entry with d_pixels permuted to NCHW and halved: that entry doubles what it reads, so
+    both kernels see the same upstream value exactly, and their results must agree bit for bit."""
+    c = x["raw_c"].shape[-1]
+    if entry == "nchw":
+        d_pixels = torch.randn(batch, c - 1, img, img, generator=g).to(DEV)
+    else:
+        d_pixels = torch.randn(batch, img * img, c - 1, generator=g).to(DEV)
+    d_c, d_f = _composite_backward(o, steps, hier, x, noise, d_pixels, entry, batch, img)
+    w_c, w_f = composite_vjp(x["raw_c"], x["z_c"], x["raw_f"], x["z_f"], noise, o, d_pixels, ray_major=entry == "rays")
+    if entry == "rays":
+        nchw = (0.5 * d_pixels).permute(0, 2, 1).reshape(batch, c - 1, img, img).contiguous()
+        e_c, e_f = _composite_backward(o, steps, hier, x, noise, nchw, "nchw", batch, img)
+        assert torch.equal(d_c, e_c), "ray-major d_raw_c differs from the NCHW entry's on the same upstream value"
+        assert not hier or torch.equal(d_f, e_f), "ray-major d_raw_f differs from the NCHW entry's on the same upstream value"
+    errs = {"d_raw_c": _rel(d_c, w_c)}
+    if hier:
+        errs["d_raw_f"] = _rel(d_f, w_f)
+    assert all(v == v for v in errs.values()), errs          # (NaN: an entry was not written)
+    return dict(d_c=d_c, d_f=d_f, w_c=w_c, w_f=w_f), errs
+
+
+_COMPOSITE_IDS = ["n%d-%s-C%d-%s%s" % (n, "hier" if h else "flat", c, o, "-opaque" if q else "") for n, h, c, o, q in _COMPOSITE]
+
+
 @gpu
-@pytest.mark.parametrize("n,hier,c,opt,opaque", _COMPOSITE,
-                         ids=["n%d-%s-C%d-%s%s" % (n, "hier" if h else "flat", c, o, "-opaque" if q else "")
-                              for n, h, c, o, q in _COMPOSITE])
-def test_composite_backward_vs_fp64(n, hier, c, opt, opaque):
-    """``fenerf_composite_backward`` as RenderFunction.backward calls it, against the float64 VJP of the compositing:
-    B = 3, 37² rays, n merged samples (more than 32 carry the transmittance scan from chunk to chunk; the shared memory
-    of n = 48 with C = 32 and of n >= 96 with C >= 22 is beyond 48 KB and needs the opt-in)."""
+@pytest.mark.parametrize("n,hier,c,opt,opaque,entry", with_entries(_COMPOSITE, _COMPOSITE_IDS))
+def test_composite_backward_vs_fp64(n, hier, c, opt, opaque, entry):
+    """``fenerf_composite_backward`` as RenderFunction.backward calls it, and ``fenerf_composite_backward_rays`` as
+    RaysRenderFunction.backward does, against the float64 VJP of the compositing: B = 3, 37² rays, n merged samples
+    (more than 32 carry the transmittance scan from chunk to chunk; the shared memory of n = 48 with C = 32 and of
+    n >= 96 with C >= 22 is beyond 48 KB and needs the opt-in, which each entry's kernel makes for itself)."""
     steps = n // 2 if hier else n
     x = _composite_inputs(c, steps, hier, opaque)
     o = _OPTS[opt]
     g = torch.Generator().manual_seed(n * 64 + c)
     noise = torch.randn(_B, _R * _R, n, generator=g).to(DEV) if o["noise"] else None
-    d_pixels = torch.randn(_B, c - 1, _R, _R, generator=g).to(DEV)
-    d_c, d_f = _composite_backward(o, steps, hier, x, noise, d_pixels)
-    w_c, w_f = composite_vjp(x["raw_c"], x["z_c"], x["raw_f"], x["z_f"], noise, o, d_pixels)
-    errs = {"d_raw_c": _rel(d_c, w_c)}
-    if hier:
-        errs["d_raw_f"] = _rel(d_f, w_f)
-    print("composite n=%d C=%d %s: %s" % (n, c, opt, errs))
+    errs = composite_backward_errors(o, steps, hier, x, noise, g, entry)[1]
+    print("composite %s n=%d C=%d %s: %s" % (entry, n, c, opt, errs))
     assert max(errs.values()) <= COMPOSITE_BOUND, errs
 
 

@@ -28,7 +28,8 @@ from fenerf_b200 import _lib, ops, packing
 from oracle import render_oracle as oracle
 from test_dropin import _LOAD_WITH_MIRROR, _reference_checkpoint, _run
 from test_gpu_fp64_reference import (COMPOSITE_BOUND, FIELD_BOUND, FWD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward,
-                                     _field_points, _forward_inputs, _grad_errors, _per_point, _render_points, composite_vjp)
+                                     _field_points, _forward_inputs, _grad_errors, _per_point, _render_points,
+                                     composite_backward_errors, with_entries)
 
 DEV = "cuda:0"
 gpu = pytest.mark.gpu
@@ -430,12 +431,13 @@ def _wide_inputs(c, steps, hier, seed):
 
 
 @gpu
-@pytest.mark.parametrize("n,hier,c,opt", _WIDE, ids=["n%d-%s-C%d-%s" % (n, "hier" if h else "flat", c, o)
-                                                      for n, h, c, o in _WIDE])
-def test_wide_composite_vs_fp64(n, hier, c, opt):
+@pytest.mark.parametrize("n,hier,c,opt,entry", with_entries(_WIDE, ["n%d-%s-C%d-%s" % (n, "hier" if h else "flat", c, o)
+                                                                    for n, h, c, o in _WIDE]))
+def test_wide_composite_vs_fp64(n, hier, c, opt, entry):
     """fenerf_composite (unsorted: the render's samples shuffled) and fenerf_composite_backward at 33 .. 129 channels
     against the float64 compositing and its VJP.  The gradient buffers start as NaN, and the density column is compared
-    on its own as well: every entry must be written."""
+    on its own as well: every entry must be written.  '-rays': fenerf_composite_backward_rays (ray-major d_pixels) in
+    place of fenerf_composite_backward, bit for bit the NCHW entry's result on the same upstream value."""
     steps = n // 2 if hier else n
     o = _WOPTS[opt]
     x = _wide_inputs(c, steps, hier, 7 * n + c)
@@ -452,19 +454,12 @@ def test_wide_composite_vs_fp64(n, hier, c, opt):
     src = shuf if hier else x
     want = composite_ref(src["raw_c"].double(), src["z_c"], src["raw_f"].double() if hier else None, src["z_f"], noise, o)
     fwd = _rel(px, want)
-    d_pixels = torch.randn(_WB, c - 1, _WR, _WR, generator=g).to(DEV)
-    d_c = torch.full_like(x["raw_c"], float("nan"))
-    d_f = torch.full_like(x["raw_f"], float("nan")) if hier else None
-    p = lambda t: t.data_ptr() if t is not None else 0                  # noqa: E731
-    _lib.check(_lib.lib().fenerf_composite_backward(
-        ctypes.byref(rd), c, p(x["raw_c"]), p(x["z_c"]), p(x["raw_f"]), p(x["z_f"]), p(noise), p(d_pixels), p(d_c), p(d_f),
-        torch.cuda.current_stream().cuda_stream))
-    w_c, w_f = composite_vjp(x["raw_c"], x["z_c"], x["raw_f"], x["z_f"], noise, o, d_pixels)
-    errs = {"forward": fwd, "d_raw_c": _rel(d_c, w_c), "d_sigma_c": _rel(d_c[..., -1], w_c[..., -1])}
+    t, errs = composite_backward_errors(o, steps, hier, x, noise, g, entry, batch=_WB, img=_WR)
+    errs.update(forward=fwd, d_sigma_c=_rel(t["d_c"][..., -1], t["w_c"][..., -1]))
     if hier:
-        errs.update(d_raw_f=_rel(d_f, w_f), d_sigma_f=_rel(d_f[..., -1], w_f[..., -1]))
+        errs["d_sigma_f"] = _rel(t["d_f"][..., -1], t["w_f"][..., -1])
     assert all(v == v for v in errs.values()), errs          # (NaN: an entry was not written)
-    print("wide composite n=%d C=%d %s: %s" % (n, c, opt, errs))
+    print("wide composite %s n=%d C=%d %s: %s" % (entry, n, c, opt, errs))
     assert max(errs.values()) <= COMPOSITE_BOUND, errs
 
 
