@@ -66,7 +66,7 @@ int check_render_desc(const fenerf_render_desc* rd) {
     FN_REQUIRE(rd, "render desc is NULL");
     FN_REQUIRE(rd->batch >= 1 && rd->img_h >= 1 && rd->img_w >= 1, "bad batch/img size %d %dx%d", rd->batch, rd->img_h,
                rd->img_w);
-    FN_REQUIRE(rd->num_steps >= 2 && rd->num_steps <= 64, "num_steps %d outside [2, 64]", rd->num_steps);
+    FN_REQUIRE(rd->num_steps >= 2 && rd->num_steps <= 256, "num_steps %d outside [2, 256]", rd->num_steps);
     if (rd->clamp_mode != FENERF_CLAMP_RELU && rd->clamp_mode != FENERF_CLAMP_SOFTPLUS)
         return fail(FENERF_E_CLAMP_MODE, "Need to choose clamp mode");
     FN_REQUIRE(rd->fill_mode >= FENERF_FILL_NONE && rd->fill_mode <= FENERF_FILL_EVAL_WHITE_BACK, "unknown fill_mode %d",

@@ -14,7 +14,8 @@
 //                               and the transmittance scan, then the reverse scan (C <= 32: one lane per channel and
 //                               one for sigma)
 //   composite_backward_wide_kernel  the same for 32 < C <= 129 (composite_wide.cu): channels looped per lane, the raw
-//                               rows read from global memory instead of staged in shared memory
+//                               rows read from global memory instead of staged in shared memory; also the narrow
+//                               fields' backward where their staged rows do not fit (n C large, composite_backward())
 // The ray-major instantiations of all three (fenerf_render_rays, fenerf_composite_backward_rays) live in
 // composite_rays.cu; this file plans their launches as it does for the NCHW ones.
 #include "composite.cuh"
@@ -66,16 +67,24 @@ int composite_forward(const fenerf_render_desc* rd, int C, const float* raw_c, c
     const long long want = (A.n_rays * tpr + kThreads - 1) / kThreads;
     const long long cap = (long long)num_sms() * 16;
     const int blocks = (int)(want < cap ? want : cap);
-    const size_t smem = unsorted ? (size_t)A.n_samples * kThreads : 0;      // the sort positions, <= 16 KB
+    const size_t smem = unsorted ? (size_t)A.n_samples * kThreads : 0;      // the sort positions, <= 64 KB
     void (*kernel)(CompositeArgs);
     if (rays) return composite_rays_launch(A, blocks, st);
     if (wide) return composite_wide_launch(A, unsorted, blocks, smem, st);
-    if (C == 4 && (((uintptr_t)raw_c | (uintptr_t)raw_f) & 15) == 0)
+    int variant;
+    if (C == 4 && (((uintptr_t)raw_c | (uintptr_t)raw_f) & 15) == 0) {
         kernel = unsorted ? composite_ray_kernel<3, 1, true> : composite_ray_kernel<3, 1, false>;
-    else if (C <= 8)
+        variant = 0;
+    } else if (C <= 8) {
         kernel = unsorted ? composite_ray_kernel<7, 1, true> : composite_ray_kernel<7, 1, false>;
-    else
+        variant = 1;
+    } else {
         kernel = unsorted ? composite_ray_kernel<8, 4, true> : composite_ray_kernel<8, 4, false>;
+        variant = 2;
+    }
+    // (only UNSORTED takes shared memory: above n = 384 samples its positions need the opt-in, one per instantiation)
+    static std::atomic<int> smem_set[3][kMaxDevices];
+    if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(kernel, smem_set[variant], (int)smem));
     kernel<<<blocks, kThreads, smem, st>>>(A);
     FN_LAUNCH_OK("composite_ray_kernel");
     return 0;
@@ -109,17 +118,21 @@ int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, 
     if (rd->hierarchical) FN_REQUIRE(d_raw_f, "hierarchical render needs d_raw_fine");
     A.d_pixels = d_pixels; A.d_raw_c = d_raw_c; A.d_raw_f = d_raw_f;
     A.n_pad = (A.n_samples + 3) & ~3;
-    const bool wide = C > 32;      // composite_backward_kernel: lanes 0..C-2 the channels, lane C-1 sigma
-    A.warp_floats = wide ? 7 * A.n_pad + kWideCh * 32 : (7 * A.n_pad + 64 + A.n_samples * C + 3) & ~3;
+    // composite_backward_kernel (lanes 0..C-2 the channels, lane C-1 sigma) stages each warp's raw block of n C floats;
+    // where eight such blocks do not fit a block's shared memory (n = 256 at C >= 22, n = 512 at C >= 8), the wide
+    // kernel, which reads the raw rows from global memory, takes the narrow fields too
+    const int narrow_floats = (7 * A.n_pad + 64 + A.n_samples * C + 3) & ~3;
+    const bool wide = C > 32 || (size_t)kRaysPerBlock * narrow_floats * sizeof(float) > (size_t)kMaxBlockSmem;
+    A.warp_floats = wide ? 7 * A.n_pad + kWideCh * 32 : narrow_floats;
     const size_t smem = (size_t)kRaysPerBlock * A.warp_floats * sizeof(float);
     long long groups = (A.n_rays + kRaysPerBlock - 1) / kRaysPerBlock;
     int per_sm = (int)(200 * 1024 / (smem + 1024));
     per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
     int blocks = (int)(groups < (long long)num_sms() * per_sm ? groups : (long long)num_sms() * per_sm);
     if (rays) return composite_backward_rays_launch(A, wide, blocks < 1 ? 1 : blocks, smem, st);
+    if (wide) return composite_backward_wide_launch(A, blocks < 1 ? 1 : blocks, smem, st);
     static std::atomic<int> smem_set[kMaxDevices];
     if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(composite_backward_kernel, smem_set, (int)smem));
-    if (wide) return composite_backward_wide_launch(A, blocks < 1 ? 1 : blocks, smem, st);
     composite_backward_kernel<<<blocks < 1 ? 1 : blocks, kRaysPerBlock * 32, smem, st>>>(A);
     FN_LAUNCH_OK("composite_backward_kernel");
     return 0;

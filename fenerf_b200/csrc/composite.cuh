@@ -5,7 +5,8 @@
 
 namespace fn {
 
-constexpr int kMaxSamples = 128;   // 2 * 64; the forward's sort positions are bytes
+constexpr int kMaxSamples = 512;   // 2 * 256; the forward's sort positions (within one list of S) are bytes
+constexpr int kMaxBlockSmem = 227 * 1024;   // the dynamic shared memory a block can opt in to (sm_90)
 constexpr int kThreads = 128;      // forward block
 constexpr int kRaysPerBlock = 8;   // backward: one warp per ray
 constexpr int kMaxC = 129;         // 64 labels + 64 features + sigma (SPATIALSIRENSEMANTICHD)

@@ -39,6 +39,8 @@ int composite_rays_launch(const CompositeArgs& A, int blocks, cudaStream_t st) {
 
 int composite_backward_rays_launch(const CompositeBwdArgs& A, bool wide, int blocks, size_t smem, cudaStream_t st) {
     if (wide) {
+        static std::atomic<int> smem_set[kMaxDevices];
+        if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(composite_backward_wide_rays_kernel, smem_set, (int)smem));
         composite_backward_wide_rays_kernel<<<blocks, kRaysPerBlock * 32, smem, st>>>(A);
         FN_LAUNCH_OK("composite_backward_wide_rays_kernel");
         return 0;

@@ -14,13 +14,20 @@ __global__ void __launch_bounds__(kRaysPerBlock * 32) composite_backward_wide_ke
 }  // namespace
 
 int composite_wide_launch(const CompositeArgs& A, bool unsorted, int blocks, size_t smem, cudaStream_t st) {
-    if (unsorted) composite_ray_kernel<kWideCh, 32, true><<<blocks, kThreads, smem, st>>>(A);
-    else composite_ray_kernel<kWideCh, 32, false><<<blocks, kThreads, smem, st>>>(A);
+    if (unsorted) {
+        static std::atomic<int> smem_set[kMaxDevices];
+        if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(composite_ray_kernel<kWideCh, 32, true>, smem_set, (int)smem));
+        composite_ray_kernel<kWideCh, 32, true><<<blocks, kThreads, smem, st>>>(A);
+    } else {
+        composite_ray_kernel<kWideCh, 32, false><<<blocks, kThreads, smem, st>>>(A);
+    }
     FN_LAUNCH_OK("composite_ray_kernel<wide>");
     return 0;
 }
 
 int composite_backward_wide_launch(const CompositeBwdArgs& A, int blocks, size_t smem, cudaStream_t st) {
+    static std::atomic<int> smem_set[kMaxDevices];      // above 48 KB from n = 204 samples
+    if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(composite_backward_wide_kernel, smem_set, (int)smem));
     composite_backward_wide_kernel<<<blocks, kRaysPerBlock * 32, smem, st>>>(A);
     FN_LAUNCH_OK("composite_backward_wide_kernel");
     return 0;

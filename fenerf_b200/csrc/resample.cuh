@@ -7,7 +7,11 @@ namespace fn {
 
 namespace {
 
-constexpr int kMaxS = 64;
+constexpr int kMaxS = 256;
+// Rays per block: the per-thread arrays take 3 S NT floats (+ S NT bytes of draw slots for RAYS), which must fit the
+// 227 KB a block can have.  128 up to S = 128 (212,992 B with the slots), 64 above (the same 212,992 B at S = 256).
+constexpr int kMaxSWide = 128;
+__host__ __device__ constexpr int resample_block(int S) { return S <= kMaxSWide ? 128 : 64; }
 
 // ONE THREAD PER RAY: every product and sum runs in the reference's left-to-right order (torch.cumprod, torch.cumsum;
 // the pdf normaliser is a sequential sum -- torch.sum's vectorised order is host-ISA dependent and is not
@@ -16,10 +20,11 @@ constexpr int kMaxS = 64;
 // fenerf_render_forward also wants the fine samples depth-sorted (stable insertion sort) for the two-pointer merge
 // in composite.cu; the stand-alone entry keeps them in draw order.
 // RAYS (fenerf_render_rays): one origin per ray (B, N, 3) instead of one per image (B, 3); and, with dirs_sample
-// (B, N, S, 3), the depth sort carries each fine sample's draw slot k (a [S][128] byte array after the three float
+// (B, N, S, 3), the depth sort carries each fine sample's draw slot k (a [S][NT] byte array after the three float
 // arrays) so that dirs_fine receives, in the sorted order, the direction of slot k: the reference pairs fine sample k of
 // sample_pdf's order with expanded direction k (generators.py:822-835).
-template <bool RAYS>
+// NT rays per block (resample_block(S)); the slots are bytes, so S <= 256.
+template <bool RAYS, int NT>
 __device__ __forceinline__ void
 resample_ray_body(long long n_rays, long long rays_per_batch, int S, int C, int clamp_mode, float noise_std,
                   const float* __restrict__ raw, const float* __restrict__ z_vals, const float* __restrict__ dirs,
@@ -29,13 +34,13 @@ resample_ray_body(long long n_rays, long long rays_per_batch, int S, int C, int 
                   float* __restrict__ dirs_fine) {
     // per-thread arrays live in shared memory as [index][thread]: whatever index a lane uses, its bank is its lane id,
     // so the data-dependent accesses of the binary search and the insertion sort never conflict (thread-local arrays
-    // would be 768 B of local memory per thread: ~340 KB per SM, thrashing the L1).  The block's 128 rays are
+    // would be 768 B of local memory per thread: ~340 KB per SM, thrashing the L1).  The block's NT rays are
     // contiguous in every global array, so inputs and outputs move through these arrays with coalesced accesses.
     extern __shared__ float s_arr[];
-    const int nt = 128, tid = threadIdx.x;
-    float* const z_ = s_arr;                              // depths                       [S][128]
-    float* const cdf_ = s_arr + (size_t)S * nt;           // weights, then the CDF        [S][128]
-    float* const zf_ = s_arr + (size_t)2 * S * nt;        // uniform draws, then z_fine   [S][128]
+    const int nt = NT, tid = threadIdx.x;
+    float* const z_ = s_arr;                              // depths                       [S][NT]
+    float* const cdf_ = s_arr + (size_t)S * nt;           // weights, then the CDF        [S][NT]
+    float* const zf_ = s_arr + (size_t)2 * S * nt;        // uniform draws, then z_fine   [S][NT]
     unsigned char* const slot_ = reinterpret_cast<unsigned char*>(s_arr + (size_t)3 * S * nt);   // RAYS: draw slots
 #define z(i) z_[(i) * nt + tid]
 #define cdf(i) cdf_[(i) * nt + tid]

@@ -239,7 +239,7 @@ int fenerf_siren_points(const fenerf_field_desc* field, const void* packed,
 typedef struct fenerf_render_desc {
     int32_t batch;
     int32_t img_h, img_w;       /* reference always renders square; kept separate for clarity */
-    int32_t num_steps;          /* S, coarse samples per ray (2..64) */
+    int32_t num_steps;          /* S, coarse samples per ray (2..256) */
     int32_t hierarchical;       /* 1: resample S fine points per ray (generators.py:58-89) */
     int32_t clamp_mode;         /* FENERF_CLAMP_* ; anything else -> FENERF_E_CLAMP_MODE */
     int32_t last_back, white_back, black_back;
