@@ -177,7 +177,8 @@ def field_ref(siren, points, dirs_pp, film, d_raw=None, film_rows=None, chunk=1 
     over the chunks) only when d_raw is given.  film_rows: image index whose FiLM rows each image uses (fault checks)."""
     ref = copy.deepcopy(siren).double()
     want_grad = d_raw is not None
-    film64 = film.double().requires_grad_(want_grad)
+    # a copy even of a float64 film: two calls must not accumulate into one .grad of the caller's tensor
+    film64 = film.detach().to(torch.float64, copy=True).requires_grad_(want_grad)
     for p in ref.parameters():
         p.requires_grad_(want_grad)
     outs = []

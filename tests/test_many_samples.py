@@ -22,8 +22,9 @@ import _point_forward as pf
 import test_gpu_fp64_forward_stages as fs
 import test_gpu_fp64_rays as fr
 import test_gpu_fp64_reference as fref
+import test_gpu_fp64_train_grads as tg
 from _fp64 import _film, _opt, _siren, composite_ref
-from fenerf_b200 import _lib, backward, ops
+from fenerf_b200 import _lib, ops
 from fenerf_b200.generators import volumetric_rendering as vr
 
 gpu = pytest.mark.gpu
@@ -389,19 +390,19 @@ def test_rays_gradients_vs_fp64(monkeypatch, model, s):
 
 
 @gpu
-def test_camera_render_with_grad_at_256_steps():
-    """backward.render_with_grad at S = 256 (512 merged): the differentiable render's pixels are the no_grad render's,
-    and every gradient is finite and non-zero."""
-    siren = fs._field("B")
-    with _registered(fs, "grad256", ("B", 1, 32, 256, True, _opt("relu"), "exact", False)):
-        x = fs.render("grad256")
-    f = x["film"].clone().requires_grad_(True)
-    px = backward.render_with_grad(siren, x["rd"], f, x["x_lin"], x["y_lin"], x["z_lin"], x["c2w"], x["perturb"].unsqueeze(-1),
-                                   x["noise_c"].unsqueeze(-1), x["u"], x["noise_f"].unsqueeze(-1))
-    assert torch.equal(px.detach(), x["pixels"])
-    params = backward.FieldWeights(siren).parameters()
-    gr = torch.autograd.grad((px * torch.randn_like(px)).sum(), [f] + params)
-    assert all(torch.isfinite(t).all() and t.abs().max() > 0 for t in gr)
+def test_camera_render_with_grad_at_256_steps(monkeypatch):
+    """backward.render_with_grad at S = 256 (512 merged: the compositing backward reads the raw rows from global
+    memory), model B, one image of 32², in exact and default precision: the differentiable render's pixels are the
+    no_grad render's, and d film and every parameter gradient are within FIELD_BOUND of the float64 VJP of the camera
+    render's chain on its own intermediates (test_gpu_fp64_train_grads.py)."""
+    monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
+    for precision in ("exact", "guard"):
+        x = tg.make_render("B", 1, 32, 256, _opt("relu"), precision, False, False, 256)
+        px, d_film, grads = tg.camera_grads(x, x["d_pixels"])
+        st = tg.stages(x)
+        assert torch.equal(st["pixels"], px), "render_forward_stages differs from the differentiable render"
+        want_film, want = tg.chain(x, st, x["d_pixels"])
+        tg.check_against_chain(x, "S=256 %s" % precision, d_film, grads, want_film, want)
 
 
 @gpu
