@@ -84,6 +84,16 @@ def plant_frequencies(film, rows, freqs=EDGE_FREQS):
     return film.contiguous(), planted
 
 
+def pass_dirs(dirs, s, lock):
+    """(B, N * S, 3) per-point directions of one pass of a camera render: each ray's direction (B, N, 3) repeated over
+    its S samples, or (0, 0, -1) under lock_view_dependence."""
+    if lock:
+        d = torch.zeros((dirs.shape[0], dirs.shape[1] * s, 3), dtype=dirs.dtype, device=dirs.device)
+        d[..., 2] = -1
+        return d
+    return dirs.repeat_interleave(s, dim=1)
+
+
 def _rel(got, want):
     s = want.abs().max().item()
     return (got.double() - want.double()).abs().max().item() / (s if s > 0 else 1.0)

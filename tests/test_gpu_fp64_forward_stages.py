@@ -3,9 +3,11 @@
 Every render here runs the whole pipeline into a private workspace; each stage is then checked against a float64
 restatement computed from the kernel's OWN fp32 inputs, read from that workspace, so no upstream error enters:
 
-  (a) ray_setup_kernel: points, depths, directions, origins;
-  (b) resample_ray_kernel (sort_fine = 1; in default and fast precision it reads the point network's compact density
-      copy): bit for bit against the stand-alone resampler on the same raw_c, and in CDF space against the float64
+  (a) ray_setup_kernel: points, depths, directions, origins; the point network's raw_c and raw_f on a fixed random
+      subset of at most POINT_RAYS rays (check_points), against field_ref on the render's own points with the
+      directions each pass used, within FWD_BOUND['exact'] in exact and split, FWD_BOUND['fast'] in fast and guard;
+  (b) resample_ray_kernel (sort_fine = 1; in default, fast and split precision it reads the point network's compact
+      density copy): bit for bit against the stand-alone resampler on the same raw_c, and in CDF space against the float64
       inverse CDF -- |F64(z) - u| <= CDF_A S 2^-24 / W + CDF_B 2^-24 |z| p / delta, the fp32 CDF's accumulated rounding
       plus the rounding of the depth itself (W the ray's weight total, p / delta the density of the depth's bin);
   (c) the GUARD refinement: which far samples are re-evaluated, their values, and fenerf_guard_stats, with 16-point
@@ -19,7 +21,12 @@ device it runs on, so every grid-stride loop takes a second pass.  The 'straddle
 multiple of the resampler's 128-ray blocks: blocks hold rays of two images.  The 'cfg2-M' and 'cfg2-N' renders run
 the bridge fields at the benchmarked shape; RES's resampling and GUARD read a density computed from v.  Measured for
 them on an H100 80GB HBM3 (400 W power limit): rays 2.7e-7, CDF ratio 0.23, refined far densities 8.2e-7, compositor
-1.6e-6, all within the constants below.
+1.6e-6, all within the constants below.  The '-split' rows run the same checks in precision='split' (the benchmarked
+shapes, the loop, the straddle, lock_view_dependence, a flat render, D32 at S = 64 and S = 256); bit-equality of the
+render's z_f and inds with the stand-alone resampler on raw_c pins the split kernel's compact density copy.  Measured on
+an H100 80GB HBM3 (700 W power limit), the point network inside renders: split <= 2.5e-6 (cfg2-B-split), guard and
+fast <= 5.4e-4 (cfg2-M), exact 8.8e-7 (flat64-F); the split rows' other stages within the same constants (CDF ratio
+<= 0.25, compositor <= 4.8e-6 at S = 256).
 
 CPU tests show that the float64 references reproduce the fp32 oracle, and that typical faults, applied to the float64
 reference, exceed each bound at least tenfold.
@@ -33,7 +40,7 @@ import math
 import pytest
 import torch
 
-from _fp64 import PAD_FILL_MODES, _film, _opt, _siren, composite_ref, field_ref
+from _fp64 import PAD_FILL_MODES, _film, _opt, _siren, composite_ref, field_ref, pass_dirs
 from fenerf_b200 import _lib, ops
 from fenerf_b200.generators import volumetric_rendering as vr
 from oracle import render_oracle as oracle
@@ -165,6 +172,17 @@ _RENDERS = {
 for _colour in ("black", "grey", "white", "light_grey", "teal"):      # teal: no fill colour of the reference's table
     _RENDERS["fill-B-seg_padding-" + _colour] = ("B", 2, 96, 24, True,
                                                  _opt(fill_mode="seg_padding_background", fill_color=_colour), "guard", False)
+# precision='split': the resampler reads the split kernel's compact density copy, lock_view_dependence its lock_dirs
+_RENDERS.update({
+    "cfg2-A-split": ("A", 4, 128, 24, True, _opt("relu"), "split", False),
+    "cfg2-B-split": ("B", 4, 128, 24, True, _opt("relu"), "split", False),
+    "loop-B-split": ("B", None, 256, 48, True, _opt("softplus", noise=0.5, softmax=True), "split", False),
+    "straddle-D-split": ("D", 3, 200, 24, True, _opt("relu", noise=0.3), "split", False),
+    "lock-A-split": ("A", 2, 96, 24, True, _opt("relu"), "split", True),
+    "flat63-A-split": ("A", 3, 37, 63, False, _opt("relu", noise=0.5, black_back=True), "split", True),
+    "max-D32-split": ("D32", 2, 72, 64, True, _opt("relu", noise=0.5, softmax=True, last_back=True), "split", False),
+    "s256-B-split": ("B", 2, 24, 256, True, _opt("relu", noise=0.5), "split", False),
+})
 
 
 def _sms():
@@ -208,14 +226,15 @@ def render(name, guard_tau=0.0, seed=None):
                               softmax_label=o["softmax"], lock_view_dependence=lock, precision=precision, guard_tau=guard_tau)
     g = torch.Generator(device=DEV).manual_seed(seed)
     n, ns = r * r, (2 * s if hier else s)
-    x = dict(name=name, siren=siren, rd=rd, opt=o, b=batch, n=n, s=s, ns=ns, hier=hier, film=_film(siren, batch, seed))
+    x = dict(name=name, siren=siren, rd=rd, opt=o, b=batch, n=n, s=s, ns=ns, hier=hier, lock=lock, precision=precision,
+             film=_film(siren, batch, seed))
     x["x_lin"], x["y_lin"], x["z_lin"] = vr.ray_tables(r, s, 0.88, 1.12, DEV)
     x["c2w"] = ops.camera_poses(batch, "gaussian", 0.3, 0.155, math.pi / 2, math.pi / 2, _DeviceDraws(g), torch.device(DEV))[0]
     x["perturb"] = torch.rand(batch, n, s, generator=g, device=DEV)
     x["noise_c"] = torch.randn(batch, n, s, generator=g, device=DEV)
     x["u"] = torch.rand(batch * n, s, generator=g, device=DEV)
     x["noise_f"] = torch.randn(batch, n, ns, generator=g, device=DEV)
-    packed = siren.packed()
+    packed = siren.packed(split=precision == "split")
     c = packed.desc.out_dim
     c_img = c - 1 + (1 if o["fill_mode"] in PAD_FILL_MODES else 0)
     out = dict(pixels=torch.empty((batch, c_img, r, r), device=DEV), depth=torch.empty((batch, n), device=DEV),
@@ -283,6 +302,45 @@ def check_resample(x):
     assert ratio.max().item() <= 1.0, msg
     assert adjacent and tie <= 1.0, msg
     return dict(cdf_ratio=ratio.max().item(), a=a_meas, b=b_meas, inds_mismatch=n_mis, tie=tie)
+
+
+#: rays per render whose point-network outputs check_points compares with float64 (a fixed random subset)
+POINT_RAYS = 1 << 16
+
+
+def point_refs(siren, film, st, lock, rays, lock_coarse=None, film_rows=None):
+    """float64 point-network outputs of each pass of a camera render on rays `rays` (indices into every image's rays):
+    field_ref on the pass's own points (st: points_c, dirs, points_f or None) with the directions it used (pass_dirs).
+    lock_coarse and film_rows exist for the fault checks.  -> [coarse (B, len(rays), S, C), fine or None]"""
+    b, s = st["points_c"].shape[0], st["points_c"].shape[2]
+    out = []
+    for pts, locked in ((st["points_c"], lock if lock_coarse is None else lock_coarse), (st["points_f"], lock)):
+        if pts is None:
+            out.append(None)
+            continue
+        want = field_ref(siren, pts[:, rays].reshape(b, -1, 3), pass_dirs(st["dirs"][:, rays], s, locked), film,
+                         film_rows=film_rows)[0]
+        out.append(want.reshape(b, len(rays), s, -1))
+    return out
+
+
+def point_errors(raws, wants):
+    """max |raw - fp64| over the passes present."""
+    return max((r.double() - w).abs().max().item() for r, w in zip(raws, wants) if w is not None)
+
+
+def check_points(x):
+    """raw_c and raw_f against field_ref on the render's own points, on at most POINT_RAYS rays: within
+    FWD_BOUND['exact'] in exact and split, FWD_BOUND['fast'] in fast and guard."""
+    rays = torch.randperm(x["n"], generator=torch.Generator().manual_seed(17))[:max(1, POINT_RAYS // x["b"])].to(DEV)
+    st = dict(points_c=x["points_c"], dirs=x["dirs"], points_f=x["points_f"])
+    wants = point_refs(x["siren"], x["film"], st, x["lock"], rays)
+    raws = [t[:, rays] if t is not None else None for t in (x["raw_c"], x["raw_f"])]
+    err = point_errors(raws, wants)
+    bound = FWD_BOUND["exact" if x["precision"] in ("exact", "split") else "fast"]
+    print("%s points (%d rays per image): max |raw - fp64| %.3g (bound %g)" % (x["name"], len(rays), err, bound))
+    assert err <= bound, "raw_c / raw_f: max |kernel - fp64| = %.3g" % err
+    return err
 
 
 @functools.lru_cache(maxsize=2)
@@ -362,7 +420,7 @@ def test_forward_stages_vs_fp64(name):
     if name.startswith("loop"):
         caps = one_pass_rays(_sms(), x["raw_c"].shape[-1])
         assert all(x["b"] * x["n"] > v for v in caps.values()), (x["b"], x["n"], caps)
-    res = dict(rays=check_ray_setup(x))
+    res = dict(rays=check_ray_setup(x), points=check_points(x))
     if x["hier"]:
         res.update(check_resample(x))
     if x["rd"].precision == _lib.PRECISION["guard"]:

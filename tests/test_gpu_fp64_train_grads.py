@@ -44,7 +44,8 @@ the whole batch, so an image whose upstream gradient is 1e-3 of the batch's larg
 own d film, relative to its own largest entry, measured up to 6.3e-2 (train-B-noise; cfg2-A 6.2e-2, bridge-N 3.2e-2)
 while the images at the top of the spread stay near 1e-2.  FIELD_BOUND, per tensor over the batch, holds; a caller who
 needs each image's FiLM gradient to 2e-2 of itself (an inversion whose images' losses differ by decades) differentiates
-in exact, or renders those images in separate calls.
+in exact, or a precision='split' render with grad_precision='split' (each image's d film within 7.3e-5 of itself under
+the same spread, test_gpu_fp64_split.py), or renders those images in separate calls.
 """
 import copy
 import functools
@@ -53,7 +54,7 @@ import math
 import pytest
 import torch
 
-from _fp64 import _film, _opt, _rel, _siren, composite_ref, field_ref, noise_offset
+from _fp64 import _film, _opt, _rel, _siren, composite_ref, field_ref, noise_offset, pass_dirs
 from fenerf_b200 import backward, ops
 from fenerf_b200.generators import volumetric_rendering as vr
 from oracle import render_oracle as oracle
@@ -70,16 +71,6 @@ CHAIN_ROWS = 1 << 17
 # --------------------------------------------------------------------------------------------
 # the float64 chain of the camera render
 # --------------------------------------------------------------------------------------------
-def pass_dirs(dirs, s, lock):
-    """(B, N * S, 3) per-point directions of one pass of a camera render: each ray's direction (B, N, 3) repeated over
-    its S samples, or (0, 0, -1) under lock_view_dependence."""
-    if lock:
-        d = torch.zeros((dirs.shape[0], dirs.shape[1] * s, 3), dtype=dirs.dtype, device=dirs.device)
-        d[..., 2] = -1
-        return d
-    return dirs.repeat_interleave(s, dim=1)
-
-
 def camera_chain(siren, film, st, lock, opt, noise, offset=None):
     """float64 pixels (B, C - 1, R, R) of the camera render from the FiLM table: field_ref on both passes (directions as
     pass_dirs), then composite_ref.  st: points_c, z_c, dirs, points_f, z_f (the render's own).  Differentiable in film
@@ -186,13 +177,13 @@ def render_case(name):
     return make_render(model, b, r, s, o, precision, lock, opaque, sum(map(ord, name)))
 
 
-def camera_grads(x, d_pixels, grad_rays=None):
+def camera_grads(x, d_pixels, grad_rays=None, grad_precision=None):
     """render_with_grad and the gradients of sum(pixels * d_pixels): (pixels, d film, {parameter name: gradient})."""
     siren = x["siren"]
     params = backward.FieldWeights(siren).parameters()
     names = {id(p): k for k, p in siren.named_parameters()}
     f = x["film"].clone().requires_grad_(True)
-    px = backward.render_with_grad(siren, x["rd"], f, *x["args"], grad_rays=grad_rays)
+    px = backward.render_with_grad(siren, x["rd"], f, *x["args"], grad_rays=grad_rays, grad_precision=grad_precision)
     gr = torch.autograd.grad((px * d_pixels).sum(), [f] + params)
     return px.detach(), gr[0], {names[id(p)]: t for p, t in zip(params, gr[1:])}
 
@@ -208,16 +199,18 @@ def chain(x, st, d_pixels):
 
 
 def bound_of(precision):
-    return FIELD_BOUND["exact" if precision == "exact" else "default"]
+    """A 'split' render's backward runs on fp32 streams, with or without grad_precision='split'."""
+    return FIELD_BOUND["exact" if precision in ("exact", "split") else "default"]
 
 
-def check_against_chain(x, tag, d_film, grads, want_film, want):
-    """Every parameter tensor and each FiLM layer's frequency and phase gradient within the precision's bound."""
+def check_against_chain(x, tag, d_film, grads, want_film, want, bound=None):
+    """Every parameter tensor and each FiLM layer's frequency and phase gradient within `bound` (None: the precision's
+    bound)."""
     assert set(want) <= set(grads), sorted(set(want) - set(grads))
     errs = _grad_errors(d_film, {k: grads[k] for k in want}, want_film, want)
     worst = max(errs, key=errs.get)
     per_image = film_errors_per_image(d_film, want_film)
-    bound = bound_of(x["precision"])
+    bound = bound_of(x["precision"]) if bound is None else bound
     print("train grads %s: worst %s %.3g (bound %g); d film per image %.3g %s" % (
         tag, worst, errs[worst], bound, per_image.max().item(), ["%.2g" % v for v in per_image.tolist()]))
     assert errs[worst] <= bound, {k: "%.2e" % v for k, v in errs.items() if v > bound}

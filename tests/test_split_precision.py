@@ -3,8 +3,11 @@ matrix scaled by a power of two before its split (layout.h, FENERF_FIELD_SPLIT_I
 
 CPU: the precision name, the packed layout with and without the split images, the refused field variants, and the
 restatement of tools/split_precision.py against float64 with the faults its bounds catch.  GPU: the point network
-against float64 for models A, B, C and P under the tile schedules, renders against the reference's goldens, P's
-gradients through a split render, the refusals, repacking after param.data writes and CUDA-graph replay."""
+against float64 for every field it serves (A-H, D32 and P) under the tile schedules, with one direction per point
+and per 24-point ray, renders of A-H, S and P against
+the reference's goldens, P's gradients through a split render, the refusals, repacking after param.data writes and
+CUDA-graph replay.  Edge FiLM frequencies, the render's stages and the training backward in split are in
+test_gpu_fp64_split.py and test_gpu_fp64_forward_stages.py."""
 import ctypes
 import os
 
@@ -111,19 +114,25 @@ def test_faults_move_the_restatement_past_the_bound(monkeypatch, cpu_fields, fau
 # GPU: the point network against float64
 # --------------------------------------------------------------------------------------------
 #: max |out - fp64| per (labels, rgb, sigma) of the split kernel.  A / B / C: 20x the restatement's bound (the kernel
-#: also sums in fp32); P: the exact kernel's bound for this field (test_wo_dir_fields.EXACT_BOUND).
-GPU_BOUND = {"A": (1e-5, 1e-5, 1e-5), "B": (1e-5, 1e-5, 1e-5), "C": (1e-5, 1e-5, 1e-5), "P": (1e-5, 2e-4, 1e-5)}
+#: also sums in fp32), and the same for every other plain field: D (22 labels), E and F (19), G, H (the deepest weight
+#: stream: 127 bulk loads of the 132 the split kernel allows) and D32 (sigma in row 31, the last the 32-column trunk
+#: head holds); P: the exact kernel's bound for this field (test_wo_dir_fields.EXACT_BOUND).  Measured on an H100 80GB
+#: HBM3 (700 W power limit): A-H and D32 <= 2.4e-6 (model H), P 1.67e-4 in rgb.
+GPU_BOUND = dict({m: (1e-5, 1e-5, 1e-5) for m in ("A", "B", "C", "D", "E", "F", "G", "H", "D32")}, P=(1e-5, 2e-4, 1e-5))
 _SHAPES = [64, 64 * 37 + 5, 20000] + list(_cases.TILE_LAYOUTS)
 
 
-def _gpu_points(model, shape, seed=7):
+def _gpu_points(model, shape, seed=7, dir_group=1):
+    """Integer shapes: 2 images of `shape` points, one direction per dir_group points (the point count rounded up to a
+    multiple of dir_group, which fenerf_siren_points requires); tile layouts: _forward_inputs."""
     siren = _siren(model, DEV)
     if isinstance(shape, int):
         film = _film(siren, 2, seed).contiguous()
         g = torch.Generator().manual_seed(seed)
-        pts = ((torch.rand(2, shape, 3, generator=g) - 0.5) * 0.24).to(DEV)
-        dirs = F.normalize(torch.randn(2, shape, 3, generator=g), dim=-1).to(DEV)
-        return siren, film, pts, dirs, 1
+        n = -(-shape // dir_group) * dir_group
+        pts = ((torch.rand(2, n, 3, generator=g) - 0.5) * 0.24).to(DEV)
+        dirs = F.normalize(torch.randn(2, n // dir_group, 3, generator=g), dim=-1).to(DEV)
+        return siren, film, pts, dirs, dir_group
     pts, dirs, film = _forward_inputs(siren, shape, 2600)
     return siren, film, pts, dirs, None
 
@@ -135,7 +144,20 @@ def _gpu_points(model, shape, seed=7):
 def test_points_match_float64(model, shape):
     """Per channel group against float64; a second launch is bit-identical and the density-only entry equals the sigma
     channel."""
-    siren, film, pts, dirs, dir_group = _gpu_points(model, shape)
+    _check_points(*_gpu_points(model, shape), model, shape)
+
+
+@pytest.mark.gpu
+@torch.no_grad()
+@pytest.mark.parametrize("model", sorted(GPU_BOUND))
+@pytest.mark.parametrize("shape", [s for s in _SHAPES if isinstance(s, int)])
+def test_points_match_float64_one_direction_per_ray(model, shape):
+    """As test_points_match_float64 with one direction per 24-point ray (dir_group 24) at the integer shapes, rounded up
+    to 72, 2376 and 20016 points; two of the tile layouts run dir_group 24 already (_FWD_DIRS)."""
+    _check_points(*_gpu_points(model, shape, dir_group=24), model, shape)
+
+
+def _check_points(siren, film, pts, dirs, dir_group, model, shape):
     want, _, _ = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)
     out = ops.siren_points(siren, pts, film, dirs, precision="split", dir_group=dir_group)
     again = ops.siren_points(siren, pts, film, dirs, precision="split", dir_group=dir_group)
@@ -144,8 +166,8 @@ def test_points_match_float64(model, shape):
     err = (out.double() - want).abs().amax(dim=(0, 1))
     n_lab = out.shape[-1] - 4
     groups = (err[:n_lab].max().item() if n_lab else 0.0, err[n_lab:n_lab + 3].max().item(), err[-1].item())
-    print("forward %s split %s (B=%d, ppb %d): max|out - fp64| labels / rgb / sigma %s" % (
-        model, shape, pts.shape[0], pts.shape[1], ["%.3g" % e for e in groups]))
+    print("forward %s split %s (B=%d, ppb %d, %d directions): max|out - fp64| labels / rgb / sigma %s" % (
+        model, shape, pts.shape[0], pts.shape[1], dirs.shape[1], ["%.3g" % e for e in groups]))
     assert torch.isfinite(out).all()
     assert all(e <= b for e, b in zip(groups, GPU_BOUND[model])), groups
     assert torch.equal(out, again)
@@ -156,7 +178,8 @@ def test_points_match_float64(model, shape):
 # GPU: renders and gradients against the reference
 # --------------------------------------------------------------------------------------------
 _RENDER = ["a_small", "a_cfg2", "a_cfg5", "b_small", "b_cfg2", "c_small", "a_nohier_softplus", "b_staged_segpad",
-           "p_small", "p_small_opaque", "p_cfg2", "p_staged_white"]
+           "d_small", "d_staged_softmax", "d_b2", "e_staged_debug", "e_staged_weight_debug", "f_small", "g_small", "h_small",
+           "s_small", "s_staged_weight", "p_small", "p_small_opaque", "p_cfg2", "p_staged_white"]
 
 
 @pytest.fixture(scope="module")
@@ -174,7 +197,7 @@ def runs():
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", _RENDER)
 def test_end_to_end_against_reference(runs, name):
-    """Split renders with the far-sigma exclusion rule of test_gpu_parity.py: A / B / C within the exact mode's 2e-4 of the
+    """Split renders with the far-sigma exclusion rule of test_gpu_parity.py: A-H and S within the exact mode's 2e-4 of the
     oracle run (which matches the reference's goldens); P within its exact mode's 1e-3 of the reference's goldens (the
     reference's own fp32 forward is up to 5.6e-4 off float64 on this field)."""
     import test_gpu_parity as p
