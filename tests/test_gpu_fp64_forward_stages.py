@@ -76,14 +76,17 @@ def one_pass_rays(sms, c):
 # --------------------------------------------------------------------------------------------
 # float64 references
 # --------------------------------------------------------------------------------------------
-def ray_setup_ref(x_lin, y_lin, z_lin, tan_half, c2w, perturb, fault=None):
+def ray_setup_ref(x_lin, y_lin, z_lin, tan_half, c2w, perturb, fault=None, rays=None):
     """get_initial_rays_trig + perturb_points + transform_sampled_points in float64 from the kernel's inputs.
-    -> points (B, N, S, 3), depths (B, N, S), directions (B, N, 3), origins (B, 3).  Ray p = row * R + col."""
+    -> points (B, N, S, 3), depths (B, N, S), directions (B, N, 3), origins (B, 3).  Ray p = row * R + col.
+    rays: only these rays of every image (N = len(rays))."""
     x, y, zl = x_lin.double(), y_lin.double(), z_lin.double()
     r = x.numel()
     gx, gy = x.repeat(r), y.repeat_interleave(r)
     if fault == "row_col_swapped":
         gx, gy = x.repeat_interleave(r), y.repeat(r)
+    if rays is not None:
+        gx, gy, perturb = gx[rays], gy[rays], perturb[:, rays]
     d = torch.stack([gx, gy, torch.full_like(gx, -1.0 / tan_half)], -1)
     d = d / d.norm(dim=-1, keepdim=True)
     u = perturb.double()
@@ -212,11 +215,12 @@ def _field(model):
     return _siren(model, DEV)
 
 
-def render(name, guard_tau=0.0, seed=None):
+def render(name, guard_tau=0.0, seed=None, spec=None, inputs=None):
     """fenerf_render_forward of render `name` into a private workspace: every output (pixels, depth, weights_sum,
     weights, inds), views of the intermediates it leaves there (fenerf_workspace_layout), the aligned workspace pointer
-    and every input the stages consumed."""
-    model, batch, r, s, hier, o, precision, lock = _RENDERS[name]
+    and every input the stages consumed.  spec: a row of the _RENDERS form for a render not in that table; inputs:
+    {film, c2w, perturb (B, N, S), noise_c (B, N, S), u (B N, S), noise_f (B, N, n)} replacing the drawn ones."""
+    model, batch, r, s, hier, o, precision, lock = spec or _RENDERS[name]
     siren = _field(model)
     batch = batch or loop_batch(_sms(), r, siren.field_spec().out_dim)
     seed = seed if seed is not None else sum(map(ord, name))
@@ -234,6 +238,7 @@ def render(name, guard_tau=0.0, seed=None):
     x["noise_c"] = torch.randn(batch, n, s, generator=g, device=DEV)
     x["u"] = torch.rand(batch * n, s, generator=g, device=DEV)
     x["noise_f"] = torch.randn(batch, n, ns, generator=g, device=DEV)
+    x.update(inputs or {})
     packed = siren.packed(split=precision == "split")
     c = packed.desc.out_dim
     c_img = c - 1 + (1 if o["fill_mode"] in PAD_FILL_MODES else 0)
@@ -268,16 +273,25 @@ def render(name, guard_tau=0.0, seed=None):
 # --------------------------------------------------------------------------------------------
 # the checks of one render
 # --------------------------------------------------------------------------------------------
-def check_ray_setup(x):
-    pts, z, dirs, org = ray_setup_ref(x["x_lin"], x["y_lin"], x["z_lin"], x["rd"].tan_half_fov, x["c2w"], x["perturb"])
+def _rays_of(t, rays):
+    """t (B, N, ...) on rays `rays` of every image (all of them for None)."""
+    return t if rays is None else t[:, rays]
+
+
+def check_ray_setup(x, rays=None):
+    """rays: compare on these rays of every image only (the float64 reference is evaluated on them alone)."""
+    pts, z, dirs, org = ray_setup_ref(x["x_lin"], x["y_lin"], x["z_lin"], x["rd"].tan_half_fov, x["c2w"], x["perturb"],
+                                      rays=rays)
     err = max((a.double() - b).abs().max().item() for a, b in
-              ((x["points_c"], pts), (x["z_c"], z), (x["dirs"], dirs), (x["origins"], org)))
+              ((_rays_of(x["points_c"], rays), pts), (_rays_of(x["z_c"], rays), z), (_rays_of(x["dirs"], rays), dirs),
+               (x["origins"], org)))
     print("%s ray set-up: %.3g" % (x["name"], err))
     assert err <= RAY_BOUND, "ray set-up: max |kernel - fp64| = %.3g" % err
     return err
 
 
-def check_resample(x):
+def check_resample(x, rays=None):
+    """The plumbing bit for bit on the whole buffers; the float64 CDF on rays `rays` of every image (None: all)."""
     b, n, s, o = x["b"], x["n"], x["s"], x["opt"]
     rd = x["rd"]
     z_sa, _, inds_sa = ops.resample(rd, x["raw_c"], x["z_c"], x["dirs"], x["origins"], x["noise_c"], x["u"], want_inds=True)
@@ -287,14 +301,16 @@ def check_resample(x):
     assert torch.equal(x["inds"], inds_sa), "render inds != stand-alone inds"
     pts = x["origins"][:, None, None, :] + x["dirs"][:, :, None, :] * x["z_f"].unsqueeze(-1)
     assert torch.equal(pts, x["points_f"]), "points_f != origins + dirs * z_f"
-    sig = x["raw_c"][..., -1].reshape(b * n, s)
+    rows = slice(None) if rays is None else (torch.arange(b, device=rays.device)[:, None] * n + rays).reshape(-1)
+    sig = x["raw_c"][..., -1].reshape(b * n, s)[rows]
     if o["noise"]:
-        sig = sig + x["noise_c"].reshape(b * n, s) * o["noise"]
-    ref = resample_ref(sig, x["z_c"].reshape(b * n, s), o["clamp"], x["u"])
-    ratio, err, t1, t2 = cdf_errors(ref, z_sa, x["u"])
+        sig = sig + x["noise_c"].reshape(b * n, s)[rows] * o["noise"]
+    u = x["u"][rows]
+    ref = resample_ref(sig, x["z_c"].reshape(b * n, s)[rows], o["clamp"], u)
+    ratio, err, t1, t2 = cdf_errors(ref, z_sa[rows], u)
     a_meas = (err / t1)[t2 < 0.1 * t1].max().item() if (t2 < 0.1 * t1).any() else 0.0
     b_meas = (err / t2)[t1 < 0.1 * t2].max().item() if (t1 < 0.1 * t2).any() else 0.0
-    adjacent, tie, n_mis = inds_near_ties(ref, x["inds"].reshape(b * n, s), x["u"])
+    adjacent, tie, n_mis = inds_near_ties(ref, x["inds"].reshape(b * n, s)[rows], u)
     msg = "resample: |F64(z) - u| / bound %.3g (a %.3g where the first term dominates, b %.3g where the second does); " \
           "%d inds differ from searchsorted(cdf64, u), worst |u - cdf64[edge]| / bound %.3g" % (
               ratio.max().item(), a_meas, b_meas, n_mis, tie)
@@ -329,10 +345,11 @@ def point_errors(raws, wants):
     return max((r.double() - w).abs().max().item() for r, w in zip(raws, wants) if w is not None)
 
 
-def check_points(x):
-    """raw_c and raw_f against field_ref on the render's own points, on at most POINT_RAYS rays: within
+def check_points(x, rays=None):
+    """raw_c and raw_f against field_ref on the render's own points, on at most POINT_RAYS rays (or on `rays`): within
     FWD_BOUND['exact'] in exact and split, FWD_BOUND['fast'] in fast and guard."""
-    rays = torch.randperm(x["n"], generator=torch.Generator().manual_seed(17))[:max(1, POINT_RAYS // x["b"])].to(DEV)
+    if rays is None:
+        rays = torch.randperm(x["n"], generator=torch.Generator().manual_seed(17))[:max(1, POINT_RAYS // x["b"])].to(DEV)
     st = dict(points_c=x["points_c"], dirs=x["dirs"], points_f=x["points_f"])
     wants = point_refs(x["siren"], x["film"], st, x["lock"], rays)
     raws = [t[:, rays] if t is not None else None for t in (x["raw_c"], x["raw_f"])]
@@ -350,20 +367,35 @@ def _far_fp64(name, b, n, s):
     return field_ref(x["siren"], x["points_c"][:, :, -1], x["dirs"], x["film"])[0][..., -1]
 
 
-def check_guard(x, tau):
-    """Which far samples the GUARD refinement re-evaluated, their values, and fenerf_guard_stats."""
+def guard_refined(fast, pre, tau):
+    """(B, N) mask of the rays whose far sample the GUARD refinement re-evaluates: fast-pass far densities `fast`, with
+    the noise added `pre`, within tau of the relu step or not finite, and the probe rays (every (B N / 128)-th)."""
+    n_rays = fast.numel()
+    ray = torch.arange(n_rays, device=fast.device).reshape(fast.shape)
+    return (pre.abs() < tau) | ~torch.isfinite(fast) | (ray % max(1, n_rays // 128) == 0)
+
+
+def check_guard(x, tau, refined_only=False):
+    """Which far samples the GUARD refinement re-evaluated, their values, and fenerf_guard_stats.  refined_only: the
+    float64 reference on the refined far samples alone (the ones it is compared on), not on every ray."""
     b, n, s, o = x["b"], x["n"], x["s"], x["opt"]
     with torch.no_grad():
         fast = ops.siren_points(x["siren"], x["points_c"].reshape(b, n * s, 3), x["film"], x["dirs"], precision="fast")
     fast = fast.reshape(b, n, s, -1)[:, :, -1, -1]
     pre = fast + x["noise_f"][..., -1] * o["noise"] if o["noise"] else fast
-    n_rays = b * n
-    ray = torch.arange(n_rays, device=DEV).reshape(b, n)
-    sel = (pre.abs() < tau) | ~torch.isfinite(fast) | (ray % max(1, n_rays // 128) == 0)
+    sel = guard_refined(fast, pre, tau)
     got = x["raw_c"][:, :, -1, -1]
     assert torch.equal(got[~sel], fast[~sel]), "a far density outside the refined set differs from the fast pass"
-    want = _far_fp64(x["name"], b, n, s)
-    err = (got.double() - want).abs()[sel].max().item()
+    if refined_only:
+        err = 0.0
+        for i in range(b):
+            if sel[i].any():
+                want = field_ref(x["siren"], x["points_c"][i:i + 1, sel[i], -1], x["dirs"][i:i + 1, sel[i]],
+                                 x["film"][i:i + 1])[0][0, :, -1]
+                err = max(err, (got[i, sel[i]].double() - want).abs().max().item())
+    else:
+        want = _far_fp64(x["name"], b, n, s)
+        err = (got.double() - want).abs()[sel].max().item()
     assert err <= FWD_BOUND["exact"], "refined far densities: max |kernel - fp64| = %.3g" % err
     rep = _lib.GuardReport()
     _lib.check(_lib.lib().fenerf_guard_stats(ctypes.c_void_p(x["ws_ptr"]), ctypes.byref(rep),
@@ -378,26 +410,40 @@ def check_guard(x, tau):
     return dict(refined=n_sel, tiles=16 if n_sel <= 16 * _sms() else 32, flips=flips, max_abs_delta=delta, fp64=err)
 
 
-def check_composite(x):
-    """pixels, depth, weights_sum, weights against composite_ref, one image at a time."""
+def composite_subset_ref(x, i, rays):
+    """composite_ref of image i of render x on rays `rays` (None: all): (pixels (1, C_img, N') NCHW-scaled, depth,
+    weights_sum, weights)."""
     o, hier = x["opt"], x["hier"]
+    sl = slice(i, i + 1)
+    sub = lambda t: None if t is None else _rays_of(t[sl], rays)          # noqa: E731
+    px, depth, wsum, w = composite_ref(sub(x["raw_c"]).double(), sub(x["z_c"]), sub(x["raw_f"]).double() if hier else None,
+                                       sub(x["z_f"]) if hier else None, sub(x["noise_f"]) if o["noise"] else None, o,
+                                       full=True, ray_major=True)
+    return (px * 2 - 1).transpose(1, 2), depth, wsum, w
+
+
+def check_composite(x, rays=None):
+    """pixels, depth, weights_sum, weights against composite_ref, one image at a time, on rays `rays` of every image
+    (None: all); the stand-alone compositor bit for bit on the whole buffers."""
+    o = x["opt"]
     errs = dict(pixels=0.0, depth=0.0, weights_sum=0.0, weights=0.0)
     skipped = 0
+    n_cmp = x["n"] if rays is None else len(rays)
     for i in range(x["b"]):
         sl = slice(i, i + 1)
-        px, depth, wsum, w = composite_ref(x["raw_c"][sl].double(), x["z_c"][sl], x["raw_f"][sl].double() if hier else None,
-                                           x["z_f"][sl] if hier else None, x["noise_f"][sl] if o["noise"] else None, o, full=True)
+        px, depth, wsum, w = composite_subset_ref(x, i, rays)
         keep = torch.ones_like(wsum, dtype=torch.bool)
         if o["fill_mode"] is not None:
             keep = (wsum - 0.9).abs() >= FILL_TIE
             skipped += int((~keep).sum())
-        pe = (x["pixels"][sl].double() - px).abs().amax(1).reshape(1, -1)
+        got_px = x["pixels"][sl].flatten(2)
+        pe = (_rays_of(got_px.transpose(1, 2), rays).transpose(1, 2).double() - px).abs().amax(1)
         errs["pixels"] = max(errs["pixels"], pe[keep].max().item())
-        errs["depth"] = max(errs["depth"], (x["depth"][sl].double() - depth).abs().max().item())
-        errs["weights_sum"] = max(errs["weights_sum"], (x["wsum"][sl].double() - wsum).abs().max().item())
-        errs["weights"] = max(errs["weights"], (x["weights"][sl].double() - w).abs().max().item())
+        errs["depth"] = max(errs["depth"], (_rays_of(x["depth"][sl], rays).double() - depth).abs().max().item())
+        errs["weights_sum"] = max(errs["weights_sum"], (_rays_of(x["wsum"][sl], rays).double() - wsum).abs().max().item())
+        errs["weights"] = max(errs["weights"], (_rays_of(x["weights"][sl], rays).double() - w).abs().max().item())
     print("%s composite: %s, %d rays skipped" % (x["name"], errs, skipped))
-    assert skipped <= FILL_TIE_FRACTION * x["b"] * x["n"], "%d rays within %g of weights_sum = 0.9" % (skipped, FILL_TIE)
+    assert skipped <= FILL_TIE_FRACTION * x["b"] * n_cmp, "%d rays within %g of weights_sum = 0.9" % (skipped, FILL_TIE)
     assert max(errs.values()) <= COMPOSITE_FWD_BOUND, errs
     # the public entry on the render's own inputs (raw_c after GUARD, draw #6) is the render's computation, bit for bit
     px, depth, wsum, w, _ = ops.composite(x["rd"], x["raw_c"], x["z_c"], x["raw_f"], x["z_f"],

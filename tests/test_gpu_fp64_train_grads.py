@@ -74,10 +74,14 @@ CHAIN_ROWS = 1 << 17
 def camera_chain(siren, film, st, lock, opt, noise, offset=None):
     """float64 pixels (B, C - 1, R, R) of the camera render from the FiLM table: field_ref on both passes (directions as
     pass_dirs), then composite_ref.  st: points_c, z_c, dirs, points_f, z_f (the render's own).  Differentiable in film
-    where film requires grad; `offset` fixes the fp32 noise offset (noise_offset) for gradcheck."""
+    where film requires grad; `offset` fixes the fp32 noise offset (noise_offset) for gradcheck.  A flat render has
+    points_f None."""
     b, n, s = st["z_c"].shape
     outs = []
     for pts, locked in ((st["points_c"], lock), (st["points_f"], lock)):
+        if pts is None:
+            outs.append(None)
+            continue
         d = pass_dirs(st["dirs"], s, locked).double()
         outs.append(oracle.field_eval(siren, pts.reshape(b, -1, 3).double(), film, d).reshape(b, n, s, -1))
     return composite_ref(outs[0], st["z_c"], outs[1], st["z_f"], noise, opt, offset)
@@ -87,13 +91,15 @@ def camera_chain_vjp(siren, film, st, lock, opt, noise, d_pixels, lock_coarse=No
     """The float64 VJP of the camera render on its own intermediates st (points_c, z_c, dirs, raw_c, points_f, z_f,
     raw_f): composite_vjp of the NCHW pixels, then field_ref on each pass with the directions it used.  lock_coarse and
     film_rows exist for the fault checks (a coarse pass locked otherwise than the fine one; image i reading the FiLM rows
-    of image film_rows[i]).  -> (d film, {parameter name: gradient})."""
+    of image film_rows[i]).  A flat render has points_f, z_f and raw_f None.  -> (d film, {parameter name: gradient})."""
     b, n, s, c = st["raw_c"].shape
     d_c, d_f = composite_vjp(st["raw_c"], st["z_c"], st["raw_f"], st["z_f"], noise, opt, d_pixels)
     lock_c = lock if lock_coarse is None else lock_coarse
     chunk = max(1, CHAIN_ROWS // b)
     _, film_c, want = field_ref(siren, st["points_c"].reshape(b, -1, 3), pass_dirs(st["dirs"], s, lock_c), film,
                                 d_c.reshape(b, -1, c), film_rows, chunk)
+    if st["points_f"] is None:
+        return film_c, want
     _, film_f, want_f = field_ref(siren, st["points_f"].reshape(b, -1, 3), pass_dirs(st["dirs"], s, lock), film,
                                   d_f.reshape(b, -1, c), film_rows, chunk)
     for k, v in want_f.items():
@@ -351,17 +357,19 @@ def test_grad_rays_vs_fp64(fp32_products, precision):
 # CPU: the chain reproduces the oracle, is the derivative of its forward, and its bound catches faults
 # --------------------------------------------------------------------------------------------
 @functools.lru_cache(maxsize=None)
-def _oracle_render(lock):
+def _oracle_render(lock, hier=True):
     """The fp32 oracle's render of model D (2 images, 8² rays, 12 + 12 samples, noise 0.5), as test_gpu_fp64_forward_
-    stages._cpu_render, with or without lock_view_dependence; its stages in the chain's names."""
+    stages._cpu_render, with or without lock_view_dependence, or flat (12 samples); its stages in the chain's names."""
     siren = _siren("D", "cpu")
     film = _film(siren, 2, 21)
     torch.manual_seed(21)
-    out = oracle.render(siren, film, dict(_CPU_CFG, lock_view_dependence=lock), keep_stages=True)
+    out = oracle.render(siren, film, dict(_CPU_CFG, lock_view_dependence=lock, hierarchical_sample=hier), keep_stages=True)
     s = out["stages"]
     st = dict(points_c=s["points_coarse"], z_c=s["z_coarse"][..., 0], dirs=s["dirs"], raw_c=s["raw_coarse"],
-              points_f=s["points_fine"], z_f=s["z_fine"][..., 0], raw_f=s["raw_fine"])
-    noise = out["draws"][5][1][..., 0]
+              points_f=None, z_f=None, raw_f=None)
+    if hier:
+        st.update(points_f=s["points_fine"], z_f=s["z_fine"][..., 0], raw_f=s["raw_fine"])
+    noise = out["draws"][-1][1][..., 0]            # the compositor's draw, the last one
     return siren, film, st, noise, out["pixels"]
 
 
@@ -373,17 +381,28 @@ def test_camera_chain_matches_the_oracle(lock):
     """field_ref on both passes with pass_dirs reproduces the oracle's raw outputs within FWD_BOUND['exact'] (under
     lock_view_dependence, both passes locked, as the oracle's and the reference's camera render lock them), and the
     chain's pixels reproduce the oracle's."""
-    siren, film, st, noise, pixels = _oracle_render(lock)
+    _check_chain_against_the_oracle(lock, True)
+
+
+def test_flat_camera_chain_matches_the_oracle():
+    """The same for a flat render (no fine pass: points_f None), the inversion's render."""
+    _check_chain_against_the_oracle(False, False)
+
+
+def _check_chain_against_the_oracle(lock, hier):
+    siren, film, st, noise, pixels = _oracle_render(lock, hier)
     b, n, s, c = st["raw_c"].shape
     errs = {}
     for tag, pts, raw in (("coarse", st["points_c"], st["raw_c"]), ("fine", st["points_f"], st["raw_f"])):
+        if pts is None:
+            continue
         out = field_ref(siren, pts.reshape(b, -1, 3), pass_dirs(st["dirs"], s, lock), film)[0]
         errs[tag] = (out - raw.reshape(b, -1, c).double()).abs().max().item()
     with torch.no_grad():
         px = camera_chain(copy_double(siren), film.double(), st, lock, _CPU_OPT, noise)
     errs["pixels"] = (px - pixels.double()).abs().max().item()
-    print("camera chain vs oracle (%s): %s" % ("locked" if lock else "free", errs))
-    assert max(errs["coarse"], errs["fine"]) <= FWD_BOUND["exact"], errs
+    print("camera chain vs oracle (%s, %s): %s" % ("locked" if lock else "free", "hierarchical" if hier else "flat", errs))
+    assert max(v for k, v in errs.items() if k != "pixels") <= FWD_BOUND["exact"], errs
     assert errs["pixels"] <= COMPOSITE_FWD_BOUND, errs
 
 
@@ -391,30 +410,43 @@ def copy_double(siren):
     return copy.deepcopy(siren).double()
 
 
-def _tiny_chain_inputs():
-    """Model A on 1 image of 3² rays, 4 + 4 samples from the oracle's set-up, its float64 field outputs as raw."""
+def _tiny_chain_inputs(hier=True):
+    """Model A on 1 image of 3² rays, 4 + 4 samples (or 4, flat) from the oracle's set-up, its float64 field outputs as
+    raw."""
     siren = _siren("A", "cpu")
     film = _film(siren, 1, 31).double()
-    cfg = dict(_CPU_CFG, img_size=3, num_steps=4)
+    cfg = dict(_CPU_CFG, img_size=3, num_steps=4, hierarchical_sample=hier)
     torch.manual_seed(31)
     out = oracle.render(siren, film.float(), cfg, keep_stages=True)
     s = out["stages"]
-    st = dict(points_c=s["points_coarse"], z_c=s["z_coarse"][..., 0], dirs=s["dirs"], points_f=s["points_fine"],
-              z_f=s["z_fine"][..., 0])
+    st = dict(points_c=s["points_coarse"], z_c=s["z_coarse"][..., 0], dirs=s["dirs"], points_f=None, z_f=None, raw_f=None)
+    if hier:
+        st.update(points_f=s["points_fine"], z_f=s["z_fine"][..., 0])
     b, n, k = st["z_c"].shape
     ref = copy_double(siren)
     for tag, pts in (("c", st["points_c"]), ("f", st["points_f"])):
+        if pts is None:
+            continue
         with torch.no_grad():
             st["raw_" + tag] = oracle.field_eval(ref, pts.reshape(b, -1, 3).double(), film,
                                                  pass_dirs(st["dirs"], k, False).double()).reshape(b, n, k, -1)
-    noise = out["draws"][5][1][..., 0]
+    noise = out["draws"][-1][1][..., 0]            # the compositor's draw, the last one
     return siren, ref, film, st, noise
 
 
 def test_camera_chain_gradcheck():
     """The chain's forward passes gradcheck in the FiLM table (fast mode), and camera_chain_vjp is its derivative: d film
     and every parameter gradient equal the float64 autograd of the whole chain to 1e-10."""
-    siren, ref, film, st, noise = _tiny_chain_inputs()
+    _check_chain_gradcheck(True)
+
+
+def test_flat_camera_chain_gradcheck():
+    """The same for a flat render (points_f None), the inversion's render."""
+    _check_chain_gradcheck(False)
+
+
+def _check_chain_gradcheck(hier):
+    siren, ref, film, st, noise = _tiny_chain_inputs(hier)
     off = noise_offset(st["raw_c"], st["z_c"], st["raw_f"], st["z_f"], noise, _CPU_OPT["noise"])
     fn = lambda f: camera_chain(ref, f, st, False, _CPU_OPT, noise, off)       # noqa: E731
     assert torch.autograd.gradcheck(fn, (film.clone().requires_grad_(True),), fast_mode=True, eps=1e-7, atol=1e-6,

@@ -11,14 +11,19 @@ The reference's last compositing interval is 1e10 wide, so a pixel is a step fun
 sign(sigma_far): rays whose oracle |sigma_far| is below ILL_TAU are ill-conditioned for ANY fp32
 implementation (an ulp of summation order flips them) and are excluded, with their count bounded.
 """
+import copy
+import functools
+
 import numpy as np
 import pytest
 import torch
 
 import _cases
 import _harness
+from _fp64 import _rel
 from fenerf_b200 import _lib, ops
 from fenerf_b200.generators.volumetric_rendering import ReplayRng
+from fenerf_b200.siren import siren as siren_mod
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -618,16 +623,68 @@ def test_render_script_call_sequence(runs, tmp_path):
     assert rgb.shape[1] == 3 and segmap.shape[1] == img.shape[1] - 3
 
 
-@pytest.mark.parametrize("name,batch", [("a_small", 3), ("b_small", 2), ("h_small", 5), ("a_small", 37)])
-def test_fused_mapping_network_matches_the_modules(name, batch):
-    """fenerf_mapping_film (cluster kernel + wide last layer) against CustomMappingNetwork + film_table in PyTorch,
-    with and without the psi truncation of staged_forward."""
+#: model A built with another latent width (ImplicitGenerator3d(TALLSIREN, z_dim, 4)): 512 is the `CelebA` curriculum's
+#: latent_dim (the first layer's K = 512 loads fill the kernel's 512-float rows), 4 the narrowest accepted, 36 and 508
+#: not multiples of the 128 floats one pass of a warp's loads covers
+_Z_DIMS = {"a_z512": 512, "a_z4": 4, "a_z36": 36, "a_z508": 508}
+
+
+@functools.lru_cache(maxsize=None)
+def _generator_with_z_dim(z_dim):
+    from fenerf_b200.generators import generators as g
+    from fenerf_b200.siren import siren as s
+    with torch.random.fork_rng(devices=[]):          # seeded initialisation; the session's RNG stream is left alone
+        torch.manual_seed(0)
+        gen = g.ImplicitGenerator3d(s.TALLSIREN, z_dim, 4)
+    gen.eval()
+    return gen
+
+
+def _mapping_case_generator(name):
+    if name in _Z_DIMS:
+        gen = copy.deepcopy(_generator_with_z_dim(_Z_DIMS[name])).to(DEV)
+        gen.device = gen.siren.device = DEV
+        return gen, "A", _Z_DIMS[name]
     case = _cases.CASE_BY_NAME[name]
-    gen = _cases.build_mirror(case, DEV)
+    return _cases.build_mirror(case, DEV), case.model, 256
+
+
+def _film64(sir, zs, psi=1.0, avg=None):
+    """The FiLM table of the mapping network(s) in float64, with the psi truncation towards `avg` (film_from_latents'
+    order of the averages)."""
+    ref = copy.deepcopy(sir).double()
+    if len(zs) == 1:
+        f, p = ref.mapping_network(zs[0].double())
+        if avg is not None:
+            f, p = avg[0].double() + psi * (f - avg[0].double()), avg[1].double() + psi * (p - avg[1].double())
+        return torch.stack([(f * 15 + 30).reshape(f.shape[0], -1, 256), p.reshape(f.shape[0], -1, 256)], 2)
+    fg, pg = ref.geo_mapping_network(zs[0].double())
+    fa, pa = ref.app_mapping_network(zs[1].double())
+    if avg is not None:
+        a = [t.double() for t in avg]
+        fg, pg, fa, pa = a[0] + psi * (fg - a[0]), a[1] + psi * (pg - a[1]), a[2] + psi * (fa - a[2]), a[3] + psi * (pa - a[3])
+    b = fg.shape[0]
+    f = torch.cat([(fg * 15 + 30).reshape(b, -1, 256), (fa * 15 + 30).reshape(b, -1, 256)], 1)
+    return torch.stack([f, torch.cat([pg.reshape(b, -1, 256), pa.reshape(b, -1, 256)], 1)], 2)
+
+
+@pytest.mark.parametrize("name,batch", [("a_small", 3), ("b_small", 2), ("h_small", 5), ("a_small", 37), ("a_z512", 1),
+                                        ("a_z512", 32), ("a_z512", 37), ("a_z4", 3), ("a_z36", 5), ("a_z508", 33)])
+def test_fused_mapping_network_matches_the_modules(name, batch):
+    """fenerf_mapping_film (cluster kernel + wide last layer) against CustomMappingNetwork + film_table in PyTorch, and
+    against the mapping network in float64, with and without the psi truncation of staged_forward: within 2e-5 of the
+    table's largest entry.  Measured against float64 on an H100 80GB HBM3 (700 W power limit): at most 1.3e-7 of it,
+    z_dim 512 included.  The a_z* rows are model A with another latent width (_Z_DIMS); at z_dim 512 one no_grad
+    forward of the generator must equal render_forward on the same draws with the table the fused kernel wrote, bit
+    for bit (test_fused_mapping_at_z_dim_512_feeds_the_render)."""
+    gen, model, z_dim = _mapping_case_generator(name)
     sir = gen.siren
     g = torch.Generator(device=DEV).manual_seed(1)
-    zs = [torch.randn(batch, 256, device=DEV, generator=g) for _ in range(_cases.n_latents(case.model))]
+    zs = [torch.randn(batch, z_dim, device=DEV, generator=g) for _ in range(_cases.n_latents(model))]
+    nets = [sir.mapping_network] if len(zs) == 1 else [sir.geo_mapping_network, sir.app_mapping_network]
     with torch.no_grad():
+        assert all(siren_mod._fused_mapping_ok(n, z) for n, z in zip(nets, zs)), "the fused mapping path is not taken"
+        print("%s: z_dim %d on the fused mapping path (fenerf_mapping_film)" % (name, z_dim))
         got = sir.film_from_latents(*zs)
         if len(zs) == 1:
             f, p = sir.mapping_network(zs[0])
@@ -644,17 +701,25 @@ def test_fused_mapping_network_matches_the_modules(name, batch):
     assert got.shape == want.shape
     assert (got - want).abs().max() <= 2e-5 * want.abs().max(), float((got - want).abs().max())
     assert (got_t - want_t).abs().max() <= 2e-5 * want_t.abs().max(), float((got_t - want_t).abs().max())
+    w64, w64_t = _film64(sir, zs), _film64(sir, zs, 0.7, avg)
+    e64, e64_t = _rel(got, w64), _rel(got_t, w64_t)
+    print("%s B=%d z_dim %d: fused mapping vs float64 %.3g, with psi %.3g (of the table's maximum)" % (name, batch, z_dim,
+                                                                                                       e64, e64_t))
+    assert max(e64, e64_t) <= 2e-5, (e64, e64_t)
     # with autograd on, the PyTorch modules run (the latent / mapping network must stay differentiable)
     z = zs[0].clone().requires_grad_(True)
     film = sir.film_from_latents(z, *zs[1:])
     assert film.requires_grad
 
 
-@pytest.mark.parametrize("m", [128, 1000, 128 * 149 + 17])
+@pytest.mark.parametrize("m", [1, 24, 63, 128, 128 + 24, 1000, 128 * 149 + 17])
 def test_wgmma_gemm_nt_cos_gate_against_fp32_matmul(m):
     """fenerf_gemm_nt_f16 (fp32 / fp16 output, the optional output * gate epilogue, and row ranges of one output written by
     separate launches, as the backward's per-image chain products do) and fenerf_gemm_nt_film, whose gate is cos(u) --
-    no factor f, so that no FiLM gradient has to divide by it."""
+    no factor f, so that no FiLM gradient has to divide by it.  M = 1, 24 and 63 fill less than one 64-row half of a
+    128-row tile (24: the one-ray trailing chunk of a flat 24-step 256² backward, backward.CHUNK_POINTS), 128 + 24 a
+    second tile with that ragged tail.  The FiLM epilogue runs on two images of (M + 1) / 2 rows and on one image of M
+    rows: at M = 24 that is the trailing chunk's own shape."""
     g = torch.Generator(device=DEV).manual_seed(m)
     a = (torch.randn(m, 256, device=DEV, generator=g) * 0.5).half()
     w = (torch.randn(256, 256, device=DEV, generator=g) * 0.1).half()
@@ -673,28 +738,32 @@ def test_wgmma_gemm_nt_cos_gate_against_fp32_matmul(m):
     gate = (torch.randn(m, 256, device=DEV, generator=g) * 5).half()      # optional epilogue: output * gate
     gated = ops.gemm_nt(a, w, torch.float16, gate=gate)
     assert (gated.float() - want * gate.float()).abs().max() <= 2e-3 * (want * gate.float()).abs().max()
-    # the fused FiLM epilogue
-    B, ppb = 2, (m + 1) // 2
-    mm = B * ppb
-    a2 = (torch.randn(mm, 256, device=DEV, generator=g) * 0.5).half()
-    film = torch.stack([torch.rand(B, 3, 256, device=DEV, generator=g) * 40 + 10, torch.randn(B, 3, 256, device=DEV, generator=g)], 2).contiguous()
-    bias = torch.randn(256, device=DEV, generator=g) * 0.1
-    act, gate = ops.gemm_nt_film(a2, w, bias, film, 0, 1, ppb)
-    z = (a2.float() @ w.float().t() + bias).reshape(B, ppb, 256)
-    u = film[:, 1, 0].unsqueeze(1) * z + film[:, 1, 1].unsqueeze(1)
-    assert (act.float().reshape(B, ppb, 256) - torch.sin(u)).abs().max() <= 2e-3
-    assert (gate.float().reshape(B, ppb, 256) - torch.cos(u)).abs().max() <= 2e-3              # the gate is cos(u), without f
-    # ... with a narrow fifth k-chunk (35 of 64 columns used)
-    xn = torch.zeros(mm, 64, device=DEV).half(); xn[:, :35] = (torch.randn(mm, 35, device=DEV, generator=g) * 0.3).half()
-    wn = torch.zeros(256, 64, device=DEV).half(); wn[:, :35] = (torch.randn(256, 35, device=DEV, generator=g) * 0.1).half()
-    act2, gate2 = ops.gemm_nt_film(a2, w, bias, film, 0, 1, ppb, narrow_in=xn, narrow_w=wn)
-    u2 = film[:, 1, 0].unsqueeze(1) * (z + (xn.float() @ wn.float().t()).reshape(B, ppb, 256)) + film[:, 1, 1].unsqueeze(1)
-    assert (act2.float().reshape(B, ppb, 256) - torch.sin(u2)).abs().max() <= 2e-3
-    assert (gate2.float().reshape(B, ppb, 256) - torch.cos(u2)).abs().max() <= 2e-3
+    # the fused FiLM epilogue, on two images and on one image of m rows (m = 24: the trailing chunk's one ray)
+    for B, ppb in ((2, (m + 1) // 2), (1, m)):
+        mm = B * ppb
+        a2 = (torch.randn(mm, 256, device=DEV, generator=g) * 0.5).half()
+        film = torch.stack([torch.rand(B, 3, 256, device=DEV, generator=g) * 40 + 10, torch.randn(B, 3, 256, device=DEV, generator=g)], 2).contiguous()
+        bias = torch.randn(256, device=DEV, generator=g) * 0.1
+        act, gate = ops.gemm_nt_film(a2, w, bias, film, 0, 1, ppb)
+        z = (a2.float() @ w.float().t() + bias).reshape(B, ppb, 256)
+        u = film[:, 1, 0].unsqueeze(1) * z + film[:, 1, 1].unsqueeze(1)
+        assert (act.float().reshape(B, ppb, 256) - torch.sin(u)).abs().max() <= 2e-3
+        assert (gate.float().reshape(B, ppb, 256) - torch.cos(u)).abs().max() <= 2e-3              # the gate is cos(u), without f
+        # ... with a narrow fifth k-chunk (35 of 64 columns used)
+        xn = torch.zeros(mm, 64, device=DEV).half(); xn[:, :35] = (torch.randn(mm, 35, device=DEV, generator=g) * 0.3).half()
+        wn = torch.zeros(256, 64, device=DEV).half(); wn[:, :35] = (torch.randn(256, 35, device=DEV, generator=g) * 0.1).half()
+        act2, gate2 = ops.gemm_nt_film(a2, w, bias, film, 0, 1, ppb, narrow_in=xn, narrow_w=wn)
+        u2 = film[:, 1, 0].unsqueeze(1) * (z + (xn.float() @ wn.float().t()).reshape(B, ppb, 256)) + film[:, 1, 1].unsqueeze(1)
+        assert (act2.float().reshape(B, ppb, 256) - torch.sin(u2)).abs().max() <= 2e-3
+        assert (gate2.float().reshape(B, ppb, 256) - torch.cos(u2)).abs().max() <= 2e-3
 
 
-@pytest.mark.parametrize("batch,ppb,slices", [(1, 64, 1), (2, 200, 3), (3, 4096 * 3 + 5, None)])
+@pytest.mark.parametrize("batch,ppb,slices", [(1, 1, None), (1, 24, None), (2, 24, 3), (3, 63, None), (1, 64, 1), (2, 200, 3),
+                                              (3, 4096 * 3 + 5, None)])
 def test_tcgen05_gemm_tn_against_fp32_bmm(batch, ppb, slices):
+    """Per-image X_b^T Y_b and the column sums of X.  ppb = 1, 24 and 63 fill less than one 64-point stage (24: the
+    one-ray trailing chunk of a flat 24-step 256² backward); (2, 24, 3) leaves two slices of each image without a stage,
+    so their partials must be zero."""
     g = torch.Generator(device=DEV).manual_seed(ppb)
     x = (torch.randn(batch * ppb, 256, device=DEV, generator=g) * 0.5).half()
     y = (torch.randn(batch * ppb, 256, device=DEV, generator=g) * 0.5).half()
@@ -706,6 +775,35 @@ def test_tcgen05_gemm_tn_against_fp32_bmm(batch, ppb, slices):
     assert torch.equal(got2, got)
     want_cs = x.float().reshape(batch, ppb, 256).sum(1)
     assert (cs - want_cs).abs().max() <= 1e-4 * max(1.0, float(want_cs.abs().max()))
+
+
+def test_fused_mapping_at_z_dim_512_feeds_the_render():
+    """Model A built with z_dim 512 (the `CelebA` curriculum's latent_dim): one no_grad forward of the generator equals,
+    bit for bit, render_forward on the same draws with the FiLM table the fused mapping kernel wrote -- the render takes
+    the fused table, not the PyTorch modules' (which differ from it in the last bits)."""
+    gen, _, z_dim = _mapping_case_generator("a_z512")
+    sir = gen.siren
+    cfg = dict(_cases.BASE, img_size=32, num_steps=12, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.5)
+    b, n, s = 2, 32 * 32, 12
+    g = torch.Generator(device=DEV).manual_seed(512)
+    z = torch.randn(b, z_dim, device=DEV, generator=g)
+    draws = [("rand", torch.rand(b, n, s, 1, device=DEV, generator=g)), ("randn", torch.randn(b, 1, device=DEV, generator=g)),
+             ("randn", torch.randn(b, 1, device=DEV, generator=g)), ("randn", torch.randn(b, n, s, 1, device=DEV, generator=g)),
+             ("rand", torch.rand(b * n, s, device=DEV, generator=g)), ("randn", torch.randn(b, n, 2 * s, 1, device=DEV, generator=g))]
+    with torch.no_grad():
+        assert siren_mod._fused_mapping_ok(sir.mapping_network, z)
+        px, _ = gen(z, _rng=ReplayRng(draws, DEV), **cfg)
+        film = sir.film_from_latents(z)
+        f, p = sir.mapping_network(z)
+        assert not torch.equal(film, sir.film_table(f, p)), "the fused and the PyTorch tables agree bit for bit: no witness"
+        rd = ops.make_render_desc(batch=b, img_size=32, num_steps=s, hierarchical=True, clamp_mode="relu", nerf_noise=0.5, fov=12)
+        c2w = ops.camera_poses(b, "gaussian", 0.3, 0.155, cfg["h_mean"], cfg["v_mean"], ReplayRng(draws[1:3], DEV),
+                               torch.device(DEV))[0]
+        x_lin, y_lin, z_lin = ops.ray_tables(32, s, 0.88, 1.12, DEV)
+        want = ops.render_forward(sir, rd, film, x_lin, y_lin, z_lin, c2w, draws[0][1].contiguous(), draws[3][1], draws[4][1],
+                                  draws[5][1])[0]
+    print("z_dim 512: generator forward on the fused mapping path, frame bit-identical to render_forward on its table")
+    assert torch.equal(px, want), float((px - want).abs().max())
 
 
 def test_frame_consumers_match_the_reference_loops():
