@@ -40,6 +40,8 @@ EXPORTS = (
     "fenerf_gemm_nt_split", "fenerf_gemm_nt_film_split", "fenerf_gemm_tn_split", "fenerf_absmax_f32",
     "fenerf_pack_field_bridge", "fenerf_field_fingerprint_bridge",
     "fenerf_render_rays", "fenerf_rays_workspace_bytes", "fenerf_rays_workspace_layout", "fenerf_composite_backward_rays",
+    "fenerf_gate_backward_det", "fenerf_absmax_finite", "fenerf_grid_scatter_det_workspace_bytes",
+    "fenerf_grid_scatter_add_det", "fenerf_det_launch_count",
 )
 
 
@@ -142,6 +144,16 @@ def _declare(lib):
     lib.fenerf_grid_scatter_add.argtypes = [P(FieldDesc), vp, vp, i32, i64, vp, i32, vp]
     lib.fenerf_grid_unpack_grad.restype = C.c_int
     lib.fenerf_grid_unpack_grad.argtypes = [P(FieldDesc), vp, vp, vp, vp]
+    lib.fenerf_gate_backward_det.restype = C.c_int
+    lib.fenerf_gate_backward_det.argtypes = [vp, vp, i64, i64, vp, sz, vp, i32, vp]
+    lib.fenerf_absmax_finite.restype = C.c_int
+    lib.fenerf_absmax_finite.argtypes = [vp, i64, i32, i64, i32, vp, vp]
+    lib.fenerf_grid_scatter_det_workspace_bytes.restype = sz
+    lib.fenerf_grid_scatter_det_workspace_bytes.argtypes = [P(FieldDesc)]
+    lib.fenerf_grid_scatter_add_det.restype = C.c_int
+    lib.fenerf_grid_scatter_add_det.argtypes = [P(FieldDesc), vp, vp, i32, i64, vp, sz, vp, i32, vp]
+    lib.fenerf_det_launch_count.restype = i64
+    lib.fenerf_det_launch_count.argtypes = []
     lib.fenerf_gemm_nt_f16.restype = C.c_int
     lib.fenerf_gemm_nt_f16.argtypes = [vp, vp, i64, vp, vp, vp, vp]
     lib.fenerf_gemm_nt_film.restype = C.c_int
@@ -212,3 +224,8 @@ def check(code):
 
 def launch_count():
     return int(lib().fenerf_launch_count())
+
+
+def det_launch_count():
+    """Kernels launched by the deterministic backward's entries (the *_det ones) since load."""
+    return int(lib().fenerf_det_launch_count())

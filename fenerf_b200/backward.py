@@ -276,6 +276,13 @@ class _FieldBackward:
         if G:
             r = self.spec.grid_res
             self.grid_grad_cl = torch.zeros((r, r, r, G), dtype=torch.float32, device=dev)
+        # torch.use_deterministic_algorithms(True): the column sums and the grid scatter in a fixed order
+        # (csrc/backward_det.cu) instead of float atomics; the fixed-point grid scatter's workspace (2.5x the accumulator)
+        self.det = torch.are_deterministic_algorithms_enabled()
+        self.grid_det_ws = None
+        if G and self.det:
+            nbytes = _lib.lib().fenerf_grid_scatter_det_workspace_bytes(C.byref(self.packed.desc))
+            self.grid_det_ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         # fp16 / fp32 weight views for the GEMMs
         fw = self.fw
         self.W0 = fw.trunk[0][0].detach().float().contiguous()                    # (256, 3); grid trunk (256, G + 3)
@@ -388,7 +395,13 @@ class _FieldBackward:
     def _gate(self, dA, gate, idx, b0, b1, P, ppb):
         cs = self.colsum[b0:b1, idx]
         tmp = torch.zeros((b1 - b0, 256), dtype=torch.float32, device=self.dev)
-        _lib.check(_lib.lib().fenerf_gate_backward(dA.data_ptr(), gate.data_ptr(), P, ppb, tmp.data_ptr(), self.dtc, _stream(self.dev)))
+        if self.det:     # each 512-point slab's sums to its own row, added in a fixed order
+            part = torch.empty(P // ppb * ((ppb + 511) // 512) * 256, dtype=torch.float32, device=self.dev)
+            _lib.check(_lib.lib().fenerf_gate_backward_det(dA.data_ptr(), gate.data_ptr(), P, ppb, part.data_ptr(),
+                                                           part.numel() * 4, tmp.data_ptr(), self.dtc, _stream(self.dev)))
+        else:
+            _lib.check(_lib.lib().fenerf_gate_backward(dA.data_ptr(), gate.data_ptr(), P, ppb, tmp.data_ptr(), self.dtc,
+                                                       _stream(self.dev)))
         cs += tmp
 
     def _chain(self, dU, idx, b0, b1, ppb, amax=None):
@@ -565,6 +578,12 @@ class _FieldBackward:
         """d features = dU diag(f_b) W_feat, (P, G), of the layer the grid feeds, scattered into the grid accumulator."""
         P = k * ppb
         d_feat = torch.bmm(dU.view(k, ppb, 256), self.fWfeat[b0:b1]).view(P, -1).contiguous()
+        if self.det:     # 64-bit fixed point at a scale taken from this point set's max |d feat|, integer atomics
+            ws = self.grid_det_ws
+            _lib.check(_lib.lib().fenerf_grid_scatter_add_det(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
+                                                              d_feat.shape[1], P, ws.data_ptr(), ws.numel(),
+                                                              self.grid_grad_cl.data_ptr(), self.dtc, _stream(self.dev)))
+            return
         _lib.check(_lib.lib().fenerf_grid_scatter_add(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
                                                       d_feat.shape[1], P, self.grid_grad_cl.data_ptr(), self.dtc,
                                                       _stream(self.dev)))

@@ -134,6 +134,7 @@ extern "C" {
 const char* fenerf_last_error(void) { return g_err; }
 int32_t fenerf_abi_version(void) { return FENERF_ABI_VERSION; }
 int64_t fenerf_launch_count(void) { return (int64_t)g_launches.load(); }
+int64_t fenerf_det_launch_count(void) { return (int64_t)g_det_launches.load(); }
 
 size_t fenerf_packed_bytes(const fenerf_field_desc* field) {
     FnLayout L;
@@ -581,6 +582,43 @@ int fenerf_grid_unpack_grad(const fenerf_field_desc* field, const float* grad_ch
     FN_REQUIRE(L.grid_channels > 0, "field has no grid");
     FN_REQUIRE(grad_channels_last && out && inv_scale, "bad argument");
     return grid_unpack_grad(L, grad_channels_last, out, inv_scale, (cudaStream_t)stream);
+}
+
+int fenerf_gate_backward_det(void* dA, const void* gate, int64_t n_points, int64_t points_per_batch, float* partial,
+                             size_t partial_bytes, float* colsum, int32_t dtype, void* stream) {
+    FN_REQUIRE(dA && gate && partial && colsum && n_points > 0 && points_per_batch > 0, "bad argument");
+    FN_REQUIRE(n_points % points_per_batch == 0, "n_points must be a whole number of images");
+    FN_REQUIRE(dtype == FENERF_DTYPE_F16 || dtype == FENERF_DTYPE_F32, "dtype");
+    const size_t need = (size_t)gate_det_partial_floats(n_points, points_per_batch) * sizeof(float);
+    if (partial_bytes < need) return fail(FENERF_E_WORKSPACE, "partial buffer too small: %zu < %zu", partial_bytes, need);
+    return gate_backward_det(dA, gate, n_points, points_per_batch, partial, colsum, dtype, (cudaStream_t)stream);
+}
+
+int fenerf_absmax_finite(const void* x, int64_t rows, int32_t cols, int64_t ld, int32_t dtype, float* amax, void* stream) {
+    FN_REQUIRE(x && amax && rows >= 0 && cols >= 0 && ld >= cols, "bad argument");
+    FN_REQUIRE(dtype == FENERF_DTYPE_F16 || dtype == FENERF_DTYPE_F32, "dtype");
+    return absmax_finite(x, rows, cols, ld, amax, dtype, (cudaStream_t)stream);
+}
+
+size_t fenerf_grid_scatter_det_workspace_bytes(const fenerf_field_desc* field) {
+    FnLayout L;
+    if (make_layout(field, &L) != 0) return 0;
+    if (L.grid_channels == 0) return 0;
+    return grid_det_workspace_bytes(L);
+}
+
+int fenerf_grid_scatter_add_det(const fenerf_field_desc* field, const float* points, const void* d_feat, int32_t ld,
+                                int64_t n_points, void* workspace, size_t workspace_bytes, float* grad_channels_last,
+                                int32_t dtype, void* stream) {
+    FnLayout L;
+    if (int e = make_layout(field, &L)) return e;
+    FN_REQUIRE(L.grid_channels > 0, "field has no grid");
+    FN_REQUIRE(points && d_feat && workspace && grad_channels_last && n_points > 0 && ld >= 32, "bad argument");
+    FN_REQUIRE(((uintptr_t)workspace & 7) == 0, "workspace must be 8-byte aligned");
+    FN_REQUIRE(dtype == FENERF_DTYPE_F16 || dtype == FENERF_DTYPE_F32, "dtype");
+    const size_t need = grid_det_workspace_bytes(L);
+    if (workspace_bytes < need) return fail(FENERF_E_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, need);
+    return grid_scatter_add_det(L, points, d_feat, ld, n_points, workspace, grad_channels_last, dtype, (cudaStream_t)stream);
 }
 
 #pragma GCC visibility pop

@@ -21,6 +21,7 @@
 //   (u = f z + p, z = W a + b, dU = dL/du = dA cos(u)).
 #include "common.cuh"
 #include "siren_common.cuh"
+#include "vec8.cuh"
 
 namespace fn {
 
@@ -29,28 +30,6 @@ namespace {
 // ---- FiLM layer: forward values the backward needs --------------------------------------------------
 // thread = (point, 8 consecutive features).  z may be NULL (first layer: only the narrow inputs), xin may be
 // NULL (plain hidden layer).  out: a (fp16, the next GEMM's input) and gate = cos(f z + p) (fp16).
-template <typename T> struct Vec8;
-template <> struct Vec8<__half> {
-    __align__(16) __half v[8];
-    __device__ __forceinline__ void set(int i, float x) { v[i] = __float2half_rn(x); }
-    __device__ __forceinline__ float get(int i) const { return __half2float(v[i]); }
-    __device__ __forceinline__ void load(const __half* p) { *reinterpret_cast<uint4*>(v) = *reinterpret_cast<const uint4*>(p); }
-    __device__ __forceinline__ void store(__half* p) const { *reinterpret_cast<uint4*>(p) = *reinterpret_cast<const uint4*>(v); }
-};
-template <> struct Vec8<float> {
-    __align__(16) float v[8];
-    __device__ __forceinline__ void set(int i, float x) { v[i] = x; }
-    __device__ __forceinline__ float get(int i) const { return v[i]; }
-    __device__ __forceinline__ void load(const float* p) {
-        reinterpret_cast<float4*>(v)[0] = reinterpret_cast<const float4*>(p)[0];
-        reinterpret_cast<float4*>(v)[1] = reinterpret_cast<const float4*>(p)[1];
-    }
-    __device__ __forceinline__ void store(float* p) const {
-        reinterpret_cast<float4*>(p)[0] = reinterpret_cast<const float4*>(v)[0];
-        reinterpret_cast<float4*>(p)[1] = reinterpret_cast<const float4*>(v)[1];
-    }
-};
-
 template <typename T>
 __global__ void __launch_bounds__(256) film_forward_stash_kernel(
     const float* __restrict__ z, const float* __restrict__ bias, const float* __restrict__ film_l /* layer's [2][256] of image 0 */,

@@ -14,6 +14,7 @@ namespace fn {
 
 extern thread_local char g_err[512];
 extern std::atomic<long long> g_launches;
+extern std::atomic<long long> g_det_launches;     // the deterministic backward's launches (backward_det.cu)
 
 inline int fail(int code, const char* fmt, ...) {
     va_list ap;
@@ -187,5 +188,13 @@ int extras_gather(const FnLayout& L, const unsigned char* packed, const float* p
 int grid_scatter_add(const FnLayout& L, const float* points, const void* d_feat, int ld, long long P, float* grad_cl,
                      int f32, cudaStream_t st);
 int grid_unpack_grad(const FnLayout& L, const float* grad_cl, float* out, const float* inv_scale, cudaStream_t st);
+// backward_det.cu: the deterministic variants (torch.use_deterministic_algorithms)
+long long gate_det_partial_floats(long long P, long long ppb);
+int gate_backward_det(void* dA, const void* gate, long long P, long long ppb, float* partial, float* colsum, int f32,
+                      cudaStream_t st);
+int absmax_finite(const void* x, long long rows, int cols, long long ld, float* amax, int f32, cudaStream_t st);
+size_t grid_det_workspace_bytes(const FnLayout& L);
+int grid_scatter_add_det(const FnLayout& L, const float* points, const void* d_feat, int ld, long long P, void* workspace,
+                         float* grad_cl, int f32, cudaStream_t st);
 
 }  // namespace fn

@@ -542,6 +542,31 @@ int fenerf_grid_scatter_add(const fenerf_field_desc* field, const float* points,
 int fenerf_grid_unpack_grad(const fenerf_field_desc* field, const float* grad_channels_last, float* out,
                             const float* inv_scale, void* stream);
 
+/* Deterministic variants of the two backward sums that fenerf_gate_backward and fenerf_grid_scatter_add form with float
+ * atomics (the order-dependent last bits): the same inputs give the same bits from call to call and process to process
+ * on the same GPU model (torch.use_deterministic_algorithms(True) in fenerf_b200/backward.py).
+ *   fenerf_gate_backward_det      fenerf_gate_backward's dU and column sums: each 512-point slab writes its 256 sums to
+ *                                 partial, at least (n_points / points_per_batch) * ceil(points_per_batch / 512) * 256 fp32
+ *                                 (partial_bytes), and colsum += their per-image sums in an order fixed by the slab count
+ *   fenerf_absmax_finite          *amax = max |x| over the FINITE entries of x (rows, cols) of `dtype` with leading
+ *                                 dimension ld >= cols (0 when there are none), on the stream (no host sync)
+ *   fenerf_grid_scatter_add_det   fenerf_grid_scatter_add in 64-bit fixed point: every contribution w d is rounded to a
+ *                                 multiple of 2^-s, s = 62 - ceil(log2(amax n_points)) with amax = max finite |d feat|, and
+ *                                 summed with integer atomics; then grad_channels_last += sum 2^-s.  An element that
+ *                                 receives a NaN, or both +inf and -inf, gains a NaN, one that receives one infinity gains
+ *                                 it.  Error per element <= n_v 2^-(s+1), n_v the contributions it receives.  workspace:
+ *                                 fenerf_grid_scatter_det_workspace_bytes(field), 8-byte aligned (0 for a field without a
+ *                                 grid); one call at a time per workspace, which the call zeroes itself
+ *   fenerf_det_launch_count       kernels these entries launched since load (also counted by fenerf_launch_count) */
+int fenerf_gate_backward_det(void* dA, const void* gate, int64_t n_points, int64_t points_per_batch, float* partial,
+                             size_t partial_bytes, float* colsum, int32_t dtype, void* stream);
+int fenerf_absmax_finite(const void* x, int64_t rows, int32_t cols, int64_t ld, int32_t dtype, float* amax, void* stream);
+size_t fenerf_grid_scatter_det_workspace_bytes(const fenerf_field_desc* field);
+int fenerf_grid_scatter_add_det(const fenerf_field_desc* field, const float* points, const void* d_feat, int32_t ld,
+                                int64_t n_points, void* workspace, size_t workspace_bytes, float* grad_channels_last,
+                                int32_t dtype, void* stream);
+int64_t fenerf_det_launch_count(void);
+
 /* Per-thread message for the last non-zero return. */
 const char* fenerf_last_error(void);
 
