@@ -42,6 +42,8 @@ EXPORTS = (
     "fenerf_render_rays", "fenerf_rays_workspace_bytes", "fenerf_rays_workspace_layout", "fenerf_composite_backward_rays",
     "fenerf_gate_backward_det", "fenerf_absmax_finite", "fenerf_grid_scatter_det_workspace_bytes",
     "fenerf_grid_scatter_add_det", "fenerf_det_launch_count",
+    "fenerf_render_rays_grad", "fenerf_rays_grad_workspace_layout", "fenerf_composite_backward_rays_dz",
+    "fenerf_grid_coord_grad", "fenerf_ray_dir_grad",
 )
 
 
@@ -128,6 +130,16 @@ def _declare(lib):
     lib.fenerf_rays_workspace_bytes.argtypes = [P(RenderDesc), P(FieldDesc), i32]
     lib.fenerf_rays_workspace_layout.restype = C.c_int
     lib.fenerf_rays_workspace_layout.argtypes = [P(RenderDesc), P(FieldDesc), i32, P(RaysWorkspaceOffsets)]
+    lib.fenerf_render_rays_grad.restype = C.c_int
+    lib.fenerf_render_rays_grad.argtypes = [P(RenderDesc), P(FieldDesc), vp, vp, vp, vp, i32] + [vp] * 9 + [vp, sz, vp]
+    lib.fenerf_rays_grad_workspace_layout.restype = C.c_int
+    lib.fenerf_rays_grad_workspace_layout.argtypes = [P(RenderDesc), P(FieldDesc), i32, P(RaysWorkspaceOffsets), P(sz)]
+    lib.fenerf_composite_backward_rays_dz.restype = C.c_int
+    lib.fenerf_composite_backward_rays_dz.argtypes = [P(RenderDesc), i32] + [vp] * 7
+    lib.fenerf_grid_coord_grad.restype = C.c_int
+    lib.fenerf_grid_coord_grad.argtypes = [P(FieldDesc), vp, vp, vp, i32, i64, vp, i32, vp]
+    lib.fenerf_ray_dir_grad.restype = C.c_int
+    lib.fenerf_ray_dir_grad.argtypes = [i64, i32, i32, vp, vp, vp, vp, vp, vp]
     lib.fenerf_composite_backward_rays.restype = C.c_int
     lib.fenerf_composite_backward_rays.argtypes = [P(RenderDesc), i32] + [vp] * 9
     lib.fenerf_composite_backward.restype = C.c_int

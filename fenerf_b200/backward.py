@@ -361,26 +361,33 @@ class _FieldBackward:
         self.Wrgb16 = rgbw
 
     # ---- one point set: points (B, ppb, 3), dirs (B, ppb/dir_group, 3), raw / d_raw (B, ppb, C) ----
-    def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
+    # ray_grad: optional (B, ppb, 3) fp32 outputs 'dx' (d points, coarse pass) and 'ddir' (d direction per point), in the
+    # scaled stream units (times `scale`, without input_scale); None: the backward runs exactly as without them
+    def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad=None):
         if self.wd or self.gs:     # the direction-free field: TF32 rounding would be amplified like fp16's (see __init__);
             with _NoTF32():          # grad_split: its narrow products stay fp32
-                return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw)
-        return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw)
+                return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad)
+        return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad)
 
-    def _add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw):
+    def _add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad=None):
         B, ppb, _ = points.shape
+
+        def outs(rows, cols):
+            return None if ray_grad is None else {k: (v[rows, cols] if v is not None else None) for k, v in ray_grad.items()}
+
         if ppb <= CHUNK_POINTS:
             k = max(1, CHUNK_POINTS // ppb)
             for b0 in range(0, B, k):
                 b1 = min(B, b0 + k)
-                self._chunk(points[b0:b1], dirs[b0:b1], dir_group, lock_dirs, raw[b0:b1], d_raw[b0:b1], b0, b1)
+                self._chunk(points[b0:b1], dirs[b0:b1], dir_group, lock_dirs, raw[b0:b1], d_raw[b0:b1], b0, b1,
+                            outs(slice(b0, b1), slice(None)))
         else:
             step = CHUNK_POINTS // dir_group * dir_group
             for b in range(B):
                 for p0 in range(0, ppb, step):
                     p1 = min(ppb, p0 + step)
                     self._chunk(points[b:b + 1, p0:p1], dirs[b:b + 1, p0 // dir_group:p1 // dir_group], dir_group, lock_dirs,
-                                raw[b:b + 1, p0:p1], d_raw[b:b + 1, p0:p1], b, b + 1)
+                                raw[b:b + 1, p0:p1], d_raw[b:b + 1, p0:p1], b, b + 1, outs(slice(b, b + 1), slice(p0, p1)))
 
     def _stash(self, z, idx, b0, P, ppb, xin=None, wx=None):
         a = torch.empty((P, 256), dtype=self.dt, device=self.dev)
@@ -423,8 +430,11 @@ class _FieldBackward:
             ops.gemm_nt(dU[rows], self.fW[b0 + i, idx - 1], torch.float16, out=out[rows])
         return out
 
-    def _chunk(self, points, dirs, dir_group, lock_dirs, raw, d_raw, b0, b1):
+    def _chunk(self, points, dirs, dir_group, lock_dirs, raw, d_raw, b0, b1, ray_grad=None):
         lib = _lib.lib()
+        want_dx = ray_grad is not None and ray_grad.get('dx') is not None
+        want_dir = ray_grad is not None and ray_grad.get('ddir') is not None
+        dx_grid = dx_res = None
         dev, spec = self.dev, self.spec
         k, ppb = points.shape[0], points.shape[1]
         P = k * ppb
@@ -507,7 +517,11 @@ class _FieldBackward:
                 idx = c0 + j
                 self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dU now
                 if self.br and j == 0:
-                    self._bridge_back(dA, extras, v, A[T - 1], d_sigma, k, ppb, b0, b1)
+                    dv = self._bridge_back(dA, extras, v, A[T - 1], d_sigma, k, ppb, b0, b1)
+                    if want_dir:
+                        ray_grad['ddir'].copy_(self._narrow_grad(dA, self.Wc0eff[:, 0:3], c0, k, ppb, b0, b1))
+                    if want_dx and self.res:      # v = x + res_coord_layer(a): dv (with dsigma a) reaches x
+                        dx_res = dv
                     dA = self._chain(dA, idx, b0, b1, ppb)
                     A[idx], Gt[idx] = None, None
                     break
@@ -523,7 +537,11 @@ class _FieldBackward:
                     e16[:, :self.kx] = extras
                     self.dWx_b[b0:b1] += _bmm32(du3, e16.view(k, ppb, self.kx_pad))
                     if G and not self.gt:
-                        self._grid_grad(dA, points, k, ppb, b0, b1)
+                        d_feat = self._grid_grad(dA, points, k, ppb, b0, b1)
+                        if want_dx:
+                            dx_grid = self._coord_grad(d_feat, points, P)
+                    if want_dir:
+                        ray_grad['ddir'].copy_(self._narrow_grad(dA, self.Wc0x_narrow[:, 0:3], c0, k, ppb, b0, b1))
                 dA = self._chain(dA, idx, b0, b1, ppb, amax)
                 A[idx], Gt[idx] = None, None
             # ---- trunk: colour-branch gradient + sigma / label heads ----
@@ -551,7 +569,16 @@ class _FieldBackward:
                 A[l], Gt[l] = None, None
             self._gate(dA, Gt[0], 0, b0, b1, P, ppb)
             if self.gt:
-                self._grid_grad(dA, points, k, ppb, b0, b1)
+                d_feat = self._grid_grad(dA, points, k, ppb, b0, b1)
+                if want_dx:
+                    dx_grid = self._coord_grad(d_feat, points, P)
+            if want_dx:     # x = points * input_scale: the first layer's position columns, the grid term, RES's dv
+                dx = self._narrow_grad(dA, self.W0[:, self.k0 - 3:self.k0], 0, k, ppb, b0, b1)
+                if dx_grid is not None:
+                    dx += dx_grid.view(k, ppb, 3)
+                if dx_res is not None:
+                    dx += dx_res.view(k, ppb, 3)
+                ray_grad['dx'].copy_(dx)
             x16 = torch.zeros((P, self.k0_pad), dtype=self.dt, device=dev)
             x16[:, :self.k0] = x
             self.dW_b[0][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), x16.view(k, ppb, self.k0_pad))
@@ -573,6 +600,21 @@ class _FieldBackward:
             self.d_c += d_sigma.sum()
         self.d_wv += dv.t() @ a_trunk.float()
         self.d_bv += dv.sum(0)
+        return dv
+
+    def _narrow_grad(self, dU, w, row, k, ppb, b0, b1):
+        """dU diag(f_b) w of FiLM row `row` for a narrow slice w (256, 3) of the layer's input columns: the gradient of
+        those inputs, (k, ppb, 3) fp32 (ray_grad)."""
+        with _NoTF32():
+            return torch.bmm(dU.view(k, ppb, 256).float(), self.film[b0:b1, row, 0].unsqueeze(2) * w)
+
+    def _coord_grad(self, d_feat, points, P):
+        """The grid term of the sample points' gradient, (P, 3) fp32 w.r.t. the box-warped coordinate (ray_grad)."""
+        out = torch.empty((P, 3), dtype=torch.float32, device=self.dev)
+        _lib.check(_lib.lib().fenerf_grid_coord_grad(C.byref(self.packed.desc), self.packed.ptr, points.data_ptr(),
+                                                     d_feat.data_ptr(), d_feat.shape[1], P, out.data_ptr(),
+                                                     1 if d_feat.dtype == torch.float32 else 0, _stream(self.dev)))
+        return out
 
     def _grid_grad(self, dU, points, k, ppb, b0, b1):
         """d features = dU diag(f_b) W_feat, (P, G), of the layer the grid feeds, scattered into the grid accumulator."""
@@ -583,10 +625,11 @@ class _FieldBackward:
             _lib.check(_lib.lib().fenerf_grid_scatter_add_det(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
                                                               d_feat.shape[1], P, ws.data_ptr(), ws.numel(),
                                                               self.grid_grad_cl.data_ptr(), self.dtc, _stream(self.dev)))
-            return
+            return d_feat
         _lib.check(_lib.lib().fenerf_grid_scatter_add(C.byref(self.packed.desc), points.data_ptr(), d_feat.data_ptr(),
                                                       d_feat.shape[1], P, self.grid_grad_cl.data_ptr(), self.dtc,
                                                       _stream(self.dev)))
+        return d_feat
 
     # ---- after every point set: fold the per-image accumulators into parameter / FiLM gradients ----
     def finish(self):
@@ -739,18 +782,27 @@ class RenderFunction(torch.autograd.Function):
 
 class RaysRenderFunction(torch.autograd.Function):
     """pixels (B, N, C-1) = render of caller-supplied rays (fenerf_render_rays; DoubleImplicitGenerator3d.point_forward),
-    differentiable w.r.t. `film` and the field parameters.  The ray tensors are inputs without gradient: the backward
-    below is RenderFunction's with the ray-major compositing backward and the caller's directions."""
+    differentiable w.r.t. `film` and the field parameters; with call['ray_grad'] the ray tensors (points, dirs, origins,
+    ray_dirs, z_vals) follow the parameters as inputs and get the reference's gradients: the coarse points, the
+    directions (both passes; the fine samples' through their draw slots), the depths without hierarchical sampling, and
+    None for the per-ray origins and directions.  The backward is RenderFunction's with the ray-major compositing
+    backward and the caller's directions."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type='cuda', cast_inputs=torch.float32)
-    def forward(ctx, film, call, *params):
+    def forward(ctx, film, call, *inputs):
         module, rd = call['module'], call['rd']
-        st = ops.render_rays_stages(module, rd, film, call['points'], call['dirs'], call['origins'], call['ray_dirs'],
-                                    call['z_vals'], call['rng_noise_c'], call['rng_u'], call['rng_noise_f'])
+        n_params = len(call['params'])
+        rays = inputs[n_params:] if call.get('ray_grad') else None
+        points, dirs, origins, ray_dirs, z_vals = rays if rays else (call[k] for k in RAY_INPUTS)
+        # the fine samples' draw slots: only for a backward w.r.t. the directions
+        slots = bool(rays) and ctx.needs_input_grad[2 + n_params + 1]
+        st = ops.render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, call['rng_noise_c'],
+                                    call['rng_u'], call['rng_noise_f'], slots=slots)
         ctx.call, ctx.stages = call, st
-        ctx.save_for_backward(film, *params)
+        ctx.save_for_backward(film, *inputs[:n_params])
         ctx.param_ids = [id(p) for p in call['params']]
+        ctx.ray_meta = [(t.shape, t.dtype) if t is not None else None for t in rays] if rays else None
         return st['pixels']
 
     @staticmethod
@@ -763,15 +815,27 @@ class RaysRenderFunction(torch.autograd.Function):
         B, s = rd.batch, rd.num_steps
         c = st['raw_c'].shape[-1]
         hier = bool(rd.hierarchical)
+        n_params = len(ctx.param_ids)
+        need = ctx.needs_input_grad[2 + n_params:] if ctx.ray_meta else (False,) * len(RAY_INPUTS)
+        spec = module.field_spec()
+        want_points, want_z = need[0], need[4] and not hier
+        want_dirs = need[1] and not spec.wo_dir        # the direction-free field never reads them
         d_pixels = d_pixels.float().contiguous()
         with torch.cuda.device(dev), torch.no_grad():
             d_raw_c = torch.empty_like(st['raw_c'])
             d_raw_f = torch.empty_like(st['raw_f']) if hier else None
             noise = call['rng_noise_f'] if rd.noise_std != 0.0 else None
-            _lib.check(_lib.lib().fenerf_composite_backward_rays(
-                C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
-                _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
-                _stream(dev)))
+            d_z = None
+            if want_z:     # the same d raw, and the depth gradient beside it
+                d_z = torch.empty_like(st['z_c'])
+                _lib.check(_lib.lib().fenerf_composite_backward_rays_dz(
+                    C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(noise), d_pixels.data_ptr(),
+                    d_raw_c.data_ptr(), d_z.data_ptr(), _stream(dev)))
+            else:
+                _lib.check(_lib.lib().fenerf_composite_backward_rays(
+                    C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
+                    _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
+                    _stream(dev)))
             m = d_raw_c.abs().max()
             if hier:
                 m = torch.maximum(m, d_raw_f.abs().max())
@@ -781,28 +845,56 @@ class RaysRenderFunction(torch.autograd.Function):
             fb = _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'],
                                 split=split, grad_split=call.get('grad_precision') == 'split')
             g = st['dir_group']
+            lock = bool(rd.lock_view_dependence)
+            pc = B * rd.img_w * s
+
+            def buf():
+                return torch.zeros((B, pc // B, 3), dtype=torch.float32, device=dev)
+
+            dir_f = buf() if want_dirs and hier and not lock else None
+            dir_c = buf() if want_dirs else None
+            dx = buf() if want_points else None
             if hier:
                 # the fine pass: the fine samples' own directions (per-sample), the per-ray ones, or (0, 0, -1)
-                lock = bool(rd.lock_view_dependence)
                 dirs_f = st['dirs_f'] if st['dirs_f'] is not None else st['dirs']
                 fb.add_points(st['points_f'].reshape(B, -1, 3), dirs_f, g, lock, st['raw_f'].reshape(B, -1, c),
-                              d_raw_f.reshape(B, -1, c))
+                              d_raw_f.reshape(B, -1, c), ray_grad=dict(ddir=dir_f) if dir_f is not None else None)
             # the coarse pass keeps the caller's directions whatever lock_view_dependence says
             fb.add_points(st['points_c'].reshape(B, -1, 3), st['dirs'], g, False, st['raw_c'].reshape(B, -1, c),
-                          d_raw_c.reshape(B, -1, c))
+                          d_raw_c.reshape(B, -1, c),
+                          ray_grad=dict(dx=dx, ddir=dir_c) if (dx is not None or dir_c is not None) else None)
             d_film, grads = fb.finish()
+            ray_grads = [None] * len(RAY_INPUTS)
+            if dx is not None:
+                ray_grads[0] = dx * inv_scale * spec.input_scale
+            if dir_c is not None:
+                d_dirs = torch.empty((B * rd.img_w * s // g, 3), dtype=torch.float32, device=dev)
+                _lib.check(_lib.lib().fenerf_ray_dir_grad(B * rd.img_w, s, g, dir_c.data_ptr(), _ptr(dir_f),
+                                                          _ptr(st['slots_f']) if dir_f is not None else 0,
+                                                          inv_scale.data_ptr(), d_dirs.data_ptr(), _stream(dev)))
+                ray_grads[1] = d_dirs
+            if d_z is not None:
+                ray_grads[4] = d_z
         out = [d_film if ctx.needs_input_grad[0] else None, None]
         for i, pid in enumerate(ctx.param_ids):
             gr = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
             if gr is not None:
                 gr = gr.reshape(ctx.saved_tensors[1 + i].shape)
             out.append(gr)
+        if ctx.ray_meta:
+            for gr, meta, want in zip(ray_grads, ctx.ray_meta, need):
+                out.append(gr.reshape(meta[0]).to(meta[1]) if gr is not None and want else None)
         return tuple(out)
+
+
+#: the ray tensors of a rays-in render, in the order RaysRenderFunction takes them with ray_grad
+RAY_INPUTS = ("points", "dirs", "origins", "ray_dirs", "z_vals")
 
 
 #: what a rays-in render refuses to differentiate
 RAYS_GRAD_MESSAGE = ("fenerf_b200: point_forward differentiates w.r.t. the latents and the field parameters only; gradients "
-                     "w.r.t. the sample points, directions, origins or depths are not built (%s requires grad): detach it")
+                     "w.r.t. the sample points, directions, origins or depths are not built (%s requires grad): detach it, "
+                     "or pass ray_grad=True")
 
 
 def check_rays_no_grad(**tensors):
@@ -815,15 +907,19 @@ def check_rays_no_grad(**tensors):
 
 
 def render_rays_with_grad(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f,
-                          grad_precision=None):
+                          grad_precision=None, ray_grad=False):
     """Differentiable render of caller-supplied rays (rd from ops.make_rays_desc): (B, N, C-1) pixels with autograd
-    edges to `film` and the field parameters.  `grad_precision` as render_with_grad."""
+    edges to `film` and the field parameters.  `grad_precision` as render_with_grad.  ray_grad=True: also to the ray
+    tensors (RaysRenderFunction); without it a ray tensor that requires grad is refused."""
     check_grad_precision(module, grad_precision, rd.precision)
-    check_rays_no_grad(points=points, directions=dirs, origins=origins, ray_directions=ray_dirs, z_vals=z_vals)
+    if not ray_grad:
+        check_rays_no_grad(points=points, directions=dirs, origins=origins, ray_directions=ray_dirs, z_vals=z_vals)
     params = FieldWeights(module).parameters()
     call = dict(module=module, rd=rd, points=points, dirs=dirs, origins=origins, ray_dirs=ray_dirs, z_vals=z_vals,
-                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_precision=grad_precision)
-    return RaysRenderFunction.apply(film, call, *params)
+                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_precision=grad_precision,
+                ray_grad=bool(ray_grad))
+    rays = (points, dirs, origins, ray_dirs, z_vals) if ray_grad else ()
+    return RaysRenderFunction.apply(film, call, *params, *rays)
 
 
 def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,

@@ -39,11 +39,12 @@ Workspace plan_workspace(const fenerf_render_desc* rd, int C) {
 }
 
 // fenerf_render_rays: the coarse inputs are the caller's; dirs_f holds the fine samples' per-sample directions
+// fine_slots (fenerf_render_rays_grad only): each fine sample's draw slot, appended after the other sections
 struct RaysWorkspace {
-    size_t stats, raw_c, z_f, points_f, dirs_f, raw_f, guard, sigma_c, total;
+    size_t stats, raw_c, z_f, points_f, dirs_f, raw_f, guard, sigma_c, total, fine_slots;
 };
 
-RaysWorkspace plan_rays_workspace(const fenerf_render_desc* rd, int C, int dir_group) {
+RaysWorkspace plan_rays_workspace(const fenerf_render_desc* rd, int C, int dir_group, bool grad = false) {
     RaysWorkspace w;
     size_t n_rays = (size_t)rd->batch * rd->img_h * rd->img_w;
     size_t pc = n_rays * rd->num_steps;
@@ -58,6 +59,7 @@ RaysWorkspace plan_rays_workspace(const fenerf_render_desc* rd, int C, int dir_g
     w.raw_f = take(rd->hierarchical ? pc * C * 4 : 4);
     w.guard = take((n_rays + 1) * 4);
     w.sigma_c = take(pc * 4);
+    w.fine_slots = grad && dirs_f ? take(pc) : 0;
     w.total = off;
     return w;
 }
@@ -375,11 +377,26 @@ int fenerf_rays_workspace_layout(const fenerf_render_desc* rd, const fenerf_fiel
     return 0;
 }
 
-int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
-                       const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
-                       const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f,
-                       float* pixels, float* depth, float* weights_sum, void* workspace, size_t workspace_bytes,
-                       void* stream) {
+int fenerf_rays_grad_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
+                                      fenerf_rays_workspace_offsets* out, size_t* fine_slots) {
+    if (int e = check_render_desc(rd)) return e;
+    FN_REQUIRE(field && out && fine_slots, "NULL argument");
+    RaysWorkspace w = plan_rays_workspace(rd, field->out_dim, dir_group, true);
+    out->raw_coarse = w.raw_c; out->z_fine = w.z_f; out->points_fine = w.points_f; out->dirs_fine = w.dirs_f;
+    out->raw_fine = w.raw_f; out->total = w.total;
+    *fine_slots = w.fine_slots;
+    return 0;
+}
+
+}  // extern "C"
+
+namespace {
+
+// fenerf_render_rays; grad: fenerf_render_rays_grad (the fine samples' draw slots into the workspace)
+int render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
+                const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
+                const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f, float* pixels,
+                float* depth, float* weights_sum, void* workspace, size_t workspace_bytes, void* stream, bool grad) {
     if (int e = check_render_desc(rd)) return e;
     FnLayout L;
     if (int e = make_layout(field, &L)) return e;
@@ -394,7 +411,7 @@ int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* fi
     FN_REQUIRE(rd->noise_std == 0.f || (rng_noise_f && (!rd->hierarchical || rng_noise_c)), "noise_std != 0 needs the noise draws");
     FN_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
     const int C = L.out_dim;
-    RaysWorkspace w = plan_rays_workspace(rd, C, dir_group);
+    RaysWorkspace w = plan_rays_workspace(rd, C, dir_group, grad);
     if (workspace_bytes < w.total) return fail(FENERF_E_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, w.total);
     unsigned char* ws = static_cast<unsigned char*>(workspace);
     float* raw_c = (float*)(ws + w.raw_c);
@@ -421,13 +438,38 @@ int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* fi
     }
     if (rd->hierarchical) {
         const bool per_sample = dir_group == 1 && !rd->lock_view_dependence;
-        if (int e = resample_rays(rd, C, raw_c, z_vals, ray_dirs, origins, noise_c, rng_u, z_f, points_f,
-                                  per_sample ? dirs : nullptr, per_sample ? dirs_f : nullptr, sigma_c, st)) return e;
+        if (grad && per_sample) {
+            if (int e = resample_rays_slots(rd, C, raw_c, z_vals, ray_dirs, origins, noise_c, rng_u, z_f, points_f, dirs, dirs_f,
+                                            sigma_c, ws + w.fine_slots, st)) return e;
+        } else if (int e = resample_rays(rd, C, raw_c, z_vals, ray_dirs, origins, noise_c, rng_u, z_f, points_f,
+                                         per_sample ? dirs : nullptr, per_sample ? dirs_f : nullptr, sigma_c, st)) return e;
         if (int e = run_field(L, packed, points_f, per_sample ? dirs_f : dirs, film, rd->batch, ppb, dir_group,
                               rd->lock_view_dependence, rd->precision, raw_f, st)) return e;
     }
     return composite_rays(rd, C, raw_c, z_vals, rd->hierarchical ? raw_f : nullptr, rd->hierarchical ? z_f : nullptr, noise_f,
                           pixels, depth, weights_sum, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
+                       const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
+                       const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f,
+                       float* pixels, float* depth, float* weights_sum, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+    return render_rays(rd, field, packed, film, points, dirs, dir_group, origins, ray_dirs, z_vals, rng_noise_c, rng_u,
+                       rng_noise_f, pixels, depth, weights_sum, workspace, workspace_bytes, stream, false);
+}
+
+int fenerf_render_rays_grad(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed,
+                            const float* film, const float* points, const float* dirs, int32_t dir_group, const float* origins,
+                            const float* ray_dirs, const float* z_vals, const float* rng_noise_c, const float* rng_u,
+                            const float* rng_noise_f, float* pixels, float* depth, float* weights_sum, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    return render_rays(rd, field, packed, film, points, dirs, dir_group, origins, ray_dirs, z_vals, rng_noise_c, rng_u,
+                       rng_noise_f, pixels, depth, weights_sum, workspace, workspace_bytes, stream, true);
 }
 
 int fenerf_mapping_film(const fenerf_mapping_params* net, const float* z, int32_t batch, int32_t n_layers, int32_t first_layer,
@@ -532,6 +574,18 @@ int fenerf_composite_backward_rays(const fenerf_render_desc* rd, int32_t out_dim
                               d_pixels, d_raw_coarse, d_raw_fine, (cudaStream_t)stream, 1);
 }
 
+int fenerf_composite_backward_rays_dz(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse,
+                                      const float* z_coarse, const float* rng_noise, const float* d_pixels,
+                                      float* d_raw_coarse, float* d_z, void* stream) {
+    if (int e = check_render_desc(rd)) return e;
+    FN_REQUIRE(!rd->hierarchical, "the depth gradient is built for non-hierarchical renders only (hierarchical sampling "
+               "composites the depths without a gradient)");
+    FN_REQUIRE(raw_coarse && z_coarse && d_pixels && d_raw_coarse && d_z, "NULL argument");
+    FN_REQUIRE(rd->noise_std == 0.f || rng_noise, "noise_std != 0 needs rng_noise");
+    return composite_backward(rd, out_dim, raw_coarse, z_coarse, nullptr, nullptr, rd->noise_std != 0.f ? rng_noise : nullptr,
+                              d_pixels, d_raw_coarse, nullptr, (cudaStream_t)stream, 1, d_z);
+}
+
 int fenerf_film_forward_stash(const float* z, const float* bias, const float* film_layer, int64_t film_batch_stride,
                               int64_t n_points, int64_t points_per_batch, const float* narrow_in, int32_t narrow_width,
                               const float* narrow_w, void* a_out, void* gate_out, int32_t dtype, void* stream) {
@@ -573,6 +627,26 @@ int fenerf_grid_scatter_add(const fenerf_field_desc* field, const float* points,
     FN_REQUIRE(points && d_feat && grad_channels_last && n_points > 0 && ld >= 32 && ld % 8 == 0, "bad argument");
     FN_REQUIRE(dtype == FENERF_DTYPE_F16 || dtype == FENERF_DTYPE_F32, "dtype");
     return grid_scatter_add(L, points, d_feat, ld, n_points, grad_channels_last, dtype, (cudaStream_t)stream);
+}
+
+int fenerf_grid_coord_grad(const fenerf_field_desc* field, const void* packed, const float* points, const void* d_feat,
+                           int32_t ld, int64_t n_points, float* d_coord, int32_t dtype, void* stream) {
+    FnLayout L;
+    if (int e = make_layout(field, &L)) return e;
+    FN_REQUIRE(L.grid_channels > 0, "field has no grid");
+    FN_REQUIRE(packed && points && d_feat && d_coord && n_points > 0 && ld >= 32 && ld % 8 == 0, "bad argument");
+    FN_REQUIRE(dtype == FENERF_DTYPE_F16 || dtype == FENERF_DTYPE_F32, "dtype");
+    return grid_coord_grad(L, (const unsigned char*)packed, points, d_feat, ld, n_points, d_coord, dtype, (cudaStream_t)stream);
+}
+
+int fenerf_ray_dir_grad(int64_t n_rays, int32_t num_steps, int32_t dir_group, const float* d_dir_coarse,
+                        const float* d_dir_fine, const uint8_t* fine_slots, const float* inv_scale, float* d_dirs,
+                        void* stream) {
+    FN_REQUIRE(d_dir_coarse && inv_scale && d_dirs && n_rays > 0 && num_steps >= 1 && num_steps <= 256, "bad argument");
+    FN_REQUIRE(dir_group == 1 || dir_group == num_steps, "dir_group %d: 1 or num_steps %d", dir_group, num_steps);
+    FN_REQUIRE(!(d_dir_fine && dir_group == 1) || fine_slots, "per-sample fine directions need their draw slots");
+    return ray_dir_grad(n_rays, num_steps, dir_group, d_dir_coarse, d_dir_fine, fine_slots, inv_scale, d_dirs,
+                        (cudaStream_t)stream);
 }
 
 int fenerf_grid_unpack_grad(const fenerf_field_desc* field, const float* grad_channels_last, float* out,

@@ -142,16 +142,23 @@ int resample(const fenerf_render_desc* rd, int C, const float* raw, const float*
 int resample_rays(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* ray_dirs,
                   const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
                   const float* dirs_sample, float* dirs_fine, const float* sigma_compact, cudaStream_t st);
+// resample_rays with per-sample directions that also writes fine_slots (B, N, S) uint8, each fine sample's draw slot k in
+// the sorted order (resample_rays_slots.cu; fenerf_render_rays_grad)
+int resample_rays_slots(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* ray_dirs,
+                        const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
+                        const float* dirs_sample, float* dirs_fine, const float* sigma_compact, unsigned char* fine_slots,
+                        cudaStream_t st);
 int composite_sorted(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                      const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
                      cudaStream_t st);
 int composite(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
               const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
               int32_t* sort_idx, cudaStream_t st);
-// rays = 1: d_pixels ray-major (B, N, C-1) of pixels in [0, 1] (fenerf_composite_backward_rays)
+// rays = 1: d_pixels ray-major (B, N, C-1) of pixels in [0, 1] (fenerf_composite_backward_rays); d_z (B, N, S): also the
+// depth gradient of a non-hierarchical rays-in render (fenerf_composite_backward_rays_dz)
 int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                        const float* z_f, const float* noise, const float* d_pixels, float* d_raw_c, float* d_raw_f,
-                       cudaStream_t st, int rays = 0);
+                       cudaStream_t st, int rays = 0, float* d_z = nullptr);
 // fenerf_render_rays' compositor: both lists depth-sorted, pixels ray-major (B, N, C-1) in [0, 1]
 int composite_rays(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                    const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, cudaStream_t st);
@@ -188,6 +195,11 @@ int extras_gather(const FnLayout& L, const unsigned char* packed, const float* p
 int grid_scatter_add(const FnLayout& L, const float* points, const void* d_feat, int ld, long long P, float* grad_cl,
                      int f32, cudaStream_t st);
 int grid_unpack_grad(const FnLayout& L, const float* grad_cl, float* out, const float* inv_scale, cudaStream_t st);
+// ray_grads.cu: the gradients w.r.t. a rays-in render's own inputs (ray_grad=True)
+int grid_coord_grad(const FnLayout& L, const unsigned char* packed, const float* points, const void* d_feat, int ld,
+                    long long P, float* d_coord, int f32, cudaStream_t st);
+int ray_dir_grad(long long n_rays, int S, int dir_group, const float* d_dir_coarse, const float* d_dir_fine,
+                 const unsigned char* fine_slots, const float* inv_scale, float* d_dirs, cudaStream_t st);
 // backward_det.cu: the deterministic variants (torch.use_deterministic_algorithms)
 long long gate_det_partial_floats(long long P, long long ppb);
 int gate_backward_det(void* dA, const void* gate, long long P, long long ppb, float* partial, float* colsum, int f32,

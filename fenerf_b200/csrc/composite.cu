@@ -111,7 +111,7 @@ int composite(const fenerf_render_desc* rd, int C, const float* raw_c, const flo
 
 int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                        const float* z_f, const float* noise, const float* d_pixels, float* d_raw_c, float* d_raw_f,
-                       cudaStream_t st, int rays) {
+                       cudaStream_t st, int rays, float* d_z) {
     CompositeBwdArgs A;
     if (int e = composite_args(rd, C, raw_c, z_c, raw_f, z_f, noise, A)) return e;
     FN_REQUIRE(rd->fill_mode == FENERF_FILL_NONE, "fill modes belong to staged_forward (no_grad)");
@@ -129,6 +129,10 @@ int composite_backward(const fenerf_render_desc* rd, int C, const float* raw_c, 
     int per_sm = (int)(200 * 1024 / (smem + 1024));
     per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
     int blocks = (int)(groups < (long long)num_sms() * per_sm ? groups : (long long)num_sms() * per_sm);
+    if (d_z) {
+        FN_REQUIRE(rays && !rd->hierarchical, "the depth gradient is built for non-hierarchical rays-in renders only");
+        return composite_backward_rays_dz_launch(A, wide, blocks < 1 ? 1 : blocks, smem, d_z, st);
+    }
     if (rays) return composite_backward_rays_launch(A, wide, blocks < 1 ? 1 : blocks, smem, st);
     if (wide) return composite_backward_wide_launch(A, blocks < 1 ? 1 : blocks, smem, st);
     static std::atomic<int> smem_set[kMaxDevices];

@@ -225,11 +225,39 @@ __global__ void __launch_bounds__(kThreads) composite_ray_kernel(CompositeArgs A
 }
 
 
+// ---- depth gradient of a non-hierarchical ray (DZ: fenerf_composite_backward_rays_dz) ----------------------------
+// delta_j = z[ord[j + 1]] - z[ord[j]] in depth order and the far interval is the constant kFarDelta, so
+// d delta_j = d alpha_j act_j exp(-delta_j act_j) (act = relu / softplus of sigma + noise) and the sample at ord[j]
+// receives d delta_{j-1} - d delta_j.  d_alpha[] holds d alpha_j from the reverse scan, dd[] is scratch of n floats;
+// each sample's d z is written once by one lane: no atomics.
+template <typename SigmaOf>
+__device__ __forceinline__ void depth_backward(const CompositeBwdArgs& A, long long ray, long long base, int n, int lane,
+                                               const int* ord, const float* d_alpha, float* dd, SigmaOf sigma_of,
+                                               float* d_z) {
+    for (int j = lane; j < n; j += 32) {
+        float v = 0.f;
+        if (j < n - 1) {
+            float sig = sigma_of(ord[j]);
+            if (A.noise) sig = __fadd_rn(sig, __fmul_rn(A.noise[ray * n + j], A.noise_std));
+            const float act = density_act(sig, A.clamp_mode);
+            const float delta = __fsub_rn(A.z_c[base + ord[j + 1]], A.z_c[base + ord[j]]);
+            float e;
+            sample_alpha(delta, act, &e);
+            v = __fmul_rn(__fmul_rn(d_alpha[j], act), e);
+        }
+        dd[j] = v;
+    }
+    __syncwarp();
+    for (int j = lane; j < n; j += 32) d_z[base + ord[j]] = __fsub_rn(j > 0 ? dd[j - 1] : 0.f, dd[j]);
+    __syncwarp();
+}
+
 // ---- backward: ONE WARP PER RAY ----------------------------------------------------------------------------------
 // Per-warp shared memory: z[n_pad] zs[n_pad] w[n_pad] ord[n_pad] al[n_pad] tt[n_pad] r[n_pad] raw[n*C] g[32] o[32]
 // RAYS (fenerf_composite_backward_rays): d_pixels is ray-major (B, N, C-1) of pixels in [0, 1] (no *2-1 factor).
-template <bool RAYS>
-__device__ __forceinline__ void composite_backward_body(const CompositeBwdArgs& A) {
+// DZ (non-hierarchical RAYS only): also d_z (B, N, S), the gradient w.r.t. the depths (depth_backward).
+template <bool RAYS, bool DZ = false>
+__device__ __forceinline__ void composite_backward_body(const CompositeBwdArgs& A, float* d_z = nullptr) {
     extern __shared__ __align__(16) float dyn[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n = A.n_samples, S = A.S, C = A.C, np = A.n_pad;
@@ -362,9 +390,11 @@ __device__ __forceinline__ void composite_backward_body(const CompositeBwdArgs& 
                 const float d_alpha = z[j] * (zs[j] - U);
                 U = fmaf(tt[j], U, zs[j] * al[j]);
                 rr[j] = d_alpha * rr[j];            // dL/dsigma_j
+                if constexpr (DZ) tt[j] = d_alpha;  // (tt[j] is not read again)
             }
         }
         __syncwarp();
+        if constexpr (DZ) depth_backward(A, ray, base, n, lane, ord, tt, al, [&](int oi) { return raw[oi * C + (C - 1)]; }, d_z);
         // scatter: d raw[ord[j]][c] = w'_j g_c (c < C-1), [C-1] = d sigma
         for (int j = 0; j < n; ++j) {
             const int oi = ord[j];
@@ -389,8 +419,8 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-template <bool RAYS>
-__device__ __forceinline__ void composite_backward_wide_body(const CompositeBwdArgs& A) {
+template <bool RAYS, bool DZ = false>
+__device__ __forceinline__ void composite_backward_wide_body(const CompositeBwdArgs& A, float* d_z = nullptr) {
     extern __shared__ __align__(16) float dyn[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n = A.n_samples, S = A.S, C = A.C, np = A.n_pad;
@@ -528,9 +558,11 @@ __device__ __forceinline__ void composite_backward_wide_body(const CompositeBwdA
                 const float d_alpha = z[j] * (zs[j] - U);
                 U = fmaf(tt[j], U, zs[j] * al[j]);
                 rr[j] = d_alpha * rr[j];
+                if constexpr (DZ) tt[j] = d_alpha;
             }
         }
         __syncwarp();
+        if constexpr (DZ) depth_backward(A, ray, base, n, lane, ord, tt, al, [&](int oi) { return row(oi)[C - 1]; }, d_z);
         for (int j = 0; j < n; ++j) {
             const int oi = ord[j];
             float wj = w[j];
@@ -554,5 +586,7 @@ int composite_backward_wide_launch(const CompositeBwdArgs& A, int blocks, size_t
 // the ray-major launches of composite_rays.cu (fenerf_render_rays, fenerf_composite_backward_rays)
 int composite_rays_launch(const CompositeArgs& A, int blocks, cudaStream_t st);
 int composite_backward_rays_launch(const CompositeBwdArgs& A, bool wide, int blocks, size_t smem, cudaStream_t st);
+// the depth-gradient instantiations of composite_rays_dz.cu (fenerf_composite_backward_rays_dz)
+int composite_backward_rays_dz_launch(const CompositeBwdArgs& A, bool wide, int blocks, size_t smem, float* d_z, cudaStream_t st);
 
 }  // namespace fn

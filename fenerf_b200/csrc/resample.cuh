@@ -23,15 +23,17 @@ __host__ __device__ constexpr int resample_block(int S) { return S <= kMaxSWide 
 // (B, N, S, 3), the depth sort carries each fine sample's draw slot k (a [S][NT] byte array after the three float
 // arrays) so that dirs_fine receives, in the sorted order, the direction of slot k: the reference pairs fine sample k of
 // sample_pdf's order with expanded direction k (generators.py:822-835).
-// NT rays per block (resample_block(S)); the slots are bytes, so S <= 256.
-template <bool RAYS, int NT>
+// NT rays per block (resample_block(S)); the slots are bytes, so S <= 256.  SLOTS (resample_rays_slots.cu): the slots
+// also leave, in the sorted order, to fine_slots (B, N, S) -- what the backward needs to return the fine samples'
+// direction gradients to the caller's slots.
+template <bool RAYS, int NT, bool SLOTS = false>
 __device__ __forceinline__ void
 resample_ray_body(long long n_rays, long long rays_per_batch, int S, int C, int clamp_mode, float noise_std,
                   const float* __restrict__ raw, const float* __restrict__ z_vals, const float* __restrict__ dirs,
                   const float* __restrict__ origins, const float* __restrict__ noise, const float* __restrict__ u,
                   float* __restrict__ z_fine, float* __restrict__ pts_fine, long long* __restrict__ inds, int sort_fine,
                   const float* __restrict__ sigma_compact, const float* __restrict__ dirs_sample,
-                  float* __restrict__ dirs_fine) {
+                  float* __restrict__ dirs_fine, unsigned char* __restrict__ fine_slots = nullptr) {
     // per-thread arrays live in shared memory as [index][thread]: whatever index a lane uses, its bank is its lane id,
     // so the data-dependent accesses of the binary search and the insertion sort never conflict (thread-local arrays
     // would be 768 B of local memory per thread: ~340 KB per SM, thrashing the L1).  The block's NT rays are
@@ -137,6 +139,7 @@ resample_ray_body(long long n_rays, long long rays_per_batch, int S, int C, int 
                 const float* d = dirs_sample + (rr * S + slot_[ss * nt + r]) * 3;
                 float* df = dirs_fine + (ray0 * S + i) * 3;
                 df[0] = __ldg(d + 0); df[1] = __ldg(d + 1); df[2] = __ldg(d + 2);
+                if constexpr (SLOTS) fine_slots[ray0 * S + i] = slot_[ss * nt + r];
             }
         }
         __syncthreads();

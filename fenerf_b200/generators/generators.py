@@ -351,18 +351,22 @@ class DoubleImplicitGenerator3d(_RenderSkeleton, nn.Module):
 
     def point_forward(self, transformed_points, transformed_ray_directions_expanded, transformed_ray_origins,
                       transformed_ray_directions, z_vals, z_geo, z_app, num_steps, hierarchical_sample,
-                      lock_view_dependence=False, **kwargs):
+                      lock_view_dependence=False, ray_grad=False, **kwargs):
         """The render of caller-supplied rays (generators.py:800-856): coarse points (B, N, S, 3) used as given, their
         directions (B, N, S, 3) or (B, N*S, 3), per-ray origins and directions (B, N, 3) for the fine points, depths
         (B, N, S, 1); any N.  Returns the pixels (B, N, C-1), ray-major in [0, 1] (no permute, no *2-1).
         lock_view_dependence locks the FINE pass's directions only, as the reference does.  Differentiable w.r.t. the
-        latents and the field; a ray tensor that requires grad is refused (RuntimeError).  One fenerf_render_rays call;
-        directions that are an expand() of per-ray ones (stride 0 along S) go in once per ray."""
+        latents and the field; without ray_grad a ray tensor that requires grad is refused (RuntimeError).  ray_grad=True
+        differentiates the ray tensors too, where the reference does: the coarse points, the directions, and the depths
+        without hierarchical sampling (the origins and per-ray directions only place the fine points, under no_grad
+        there).  One fenerf_render_rays call; directions that are an expand() of per-ray ones (stride 0 along S) go in
+        once per ray (their gradient is the per-ray sum)."""
         from .. import backward
-        backward.check_rays_no_grad(transformed_points=transformed_points,
-                                    transformed_ray_directions_expanded=transformed_ray_directions_expanded,
-                                    transformed_ray_origins=transformed_ray_origins,
-                                    transformed_ray_directions=transformed_ray_directions, z_vals=z_vals)
+        if not ray_grad:
+            backward.check_rays_no_grad(transformed_points=transformed_points,
+                                        transformed_ray_directions_expanded=transformed_ray_directions_expanded,
+                                        transformed_ray_origins=transformed_ray_origins,
+                                        transformed_ray_directions=transformed_ray_directions, z_vals=z_vals)
         clamp_mode, noise_std = kwargs['clamp_mode'], kwargs['nerf_noise']
         device = torch.device(self.device)
         if device.type != 'cuda':
@@ -388,8 +392,9 @@ class DoubleImplicitGenerator3d(_RenderSkeleton, nn.Module):
                 precision=kwargs.get('precision'), guard_tau=kwargs.get('guard_tau', getattr(self.siren, '_guard_tau', 0.0)))
         args = (transformed_points, dirs, transformed_ray_origins, transformed_ray_directions, z_vals, rng_noise_c, rng_u,
                 rng_noise_f)
-        if ops.needs_grad(self.siren, film):
-            return backward.render_rays_with_grad(self.siren, rd, film, *args, grad_precision=kwargs.get('grad_precision'))
+        if ops.needs_grad(self.siren, film, *(args[:5] if ray_grad else ())):
+            return backward.render_rays_with_grad(self.siren, rd, film, *args, grad_precision=kwargs.get('grad_precision'),
+                                                  ray_grad=ray_grad)
         with torch.no_grad():
             return ops.render_rays(self.siren, rd, film, *args)[0]
 

@@ -396,8 +396,8 @@ def rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device):
 
 
 def _rays_call(lib, rd, packed, film, pts, dirs, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, depth,
-               wsum, ws_ptr, ws_bytes, device):
-    _lib.check(lib.fenerf_render_rays(
+               wsum, ws_ptr, ws_bytes, device, slots=False):
+    _lib.check((lib.fenerf_render_rays_grad if slots else lib.fenerf_render_rays)(
         C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device), _chk(pts, "points", device),
         _chk(dirs, "dirs", device), dir_group, _chk(o, "origins", device), _chk(rdir, "ray_dirs", device),
         _chk(z, "z_vals", device), _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device),
@@ -437,9 +437,12 @@ def render_rays(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_n
     return pixels, depth, wsum
 
 
-def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f):
+def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f,
+                       slots=False):
     """fenerf_render_rays into a PRIVATE workspace, returned with typed views of what it leaves there
-    (fenerf_rays_workspace_layout) and the laid-out inputs: what the backward consumes (fenerf_b200/backward.py)."""
+    (fenerf_rays_workspace_layout) and the laid-out inputs: what the backward consumes (fenerf_b200/backward.py).
+    slots=True (a backward w.r.t. the directions): fenerf_render_rays_grad, which also leaves the fine samples' draw
+    slots, 'slots_f' (B, N, S) uint8, where the fine pass reads per-sample directions (None elsewhere)."""
     packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
     device = packed.device
     lib = _lib.lib()
@@ -449,12 +452,17 @@ def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals
     pts, d, dir_group, o, rdir, z = rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device)
     pixels = torch.empty((b, n, c - 1), dtype=torch.float32, device=device)
     off = _lib.RaysWorkspaceOffsets()
+    slots_off = C.c_size_t(0)
     with torch.cuda.device(device):
-        _lib.check(lib.fenerf_rays_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off)))
+        if slots:
+            _lib.check(lib.fenerf_rays_grad_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off),
+                                                             C.byref(slots_off)))
+        else:
+            _lib.check(lib.fenerf_rays_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off)))
         ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
         base = (ws.data_ptr() + 255) // 256 * 256 - ws.data_ptr()
         _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, None, None,
-                   ws.data_ptr() + base, ws.numel() - base, device)
+                   ws.data_ptr() + base, ws.numel() - base, device, slots=slots)
 
     def view(offset, shape):
         numel = 1
@@ -463,12 +471,14 @@ def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals
         return ws[base + offset: base + offset + numel * 4].view(torch.float32).view(shape)
 
     st = dict(pixels=pixels, workspace=ws, points_c=pts, z_c=z, dirs=d, dir_group=dir_group,
-              raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None, dirs_f=None)
+              raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None, dirs_f=None, slots_f=None)
     if rd.hierarchical:
         st.update(points_f=view(off.points_fine, (b, n, s, 3)), z_f=view(off.z_fine, (b, n, s)),
                   raw_f=view(off.raw_fine, (b, n, s, c)))
         if dir_group == 1 and not rd.lock_view_dependence:
             st.update(dirs_f=view(off.dirs_fine, (b, n * s, 3)))
+            if slots:
+                st.update(slots_f=ws[base + slots_off.value: base + slots_off.value + b * n * s].view(b, n, s))
     return st
 
 

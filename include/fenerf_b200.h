@@ -407,6 +407,19 @@ size_t fenerf_rays_workspace_bytes(const fenerf_render_desc* rd, const fenerf_fi
 int fenerf_rays_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
                                  fenerf_rays_workspace_offsets* out);
 
+/* fenerf_render_rays for a render that will be differentiated w.r.t. per-sample directions (point_forward with
+ * ray_grad=True): the same arguments, kernels and results, and with dir_group 1 in a hierarchical render without
+ * rd->lock_view_dependence also each fine sample's draw slot k (B, N, S) uint8, in the depth-sorted order of z_fine,
+ * at byte offset *fine_slots of the workspace.  fenerf_rays_grad_workspace_layout: fenerf_rays_workspace_layout with
+ * that section appended (out->total includes it; *fine_slots = 0 when the render writes no slots). */
+int fenerf_render_rays_grad(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed,
+                            const float* film, const float* points, const float* dirs, int32_t dir_group, const float* origins,
+                            const float* ray_dirs, const float* z_vals, const float* rng_noise_c, const float* rng_u,
+                            const float* rng_noise_f, float* pixels, float* depth, float* weights_sum, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int fenerf_rays_grad_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
+                                      fenerf_rays_workspace_offsets* out, size_t* fine_slots);
+
 /* ---- mapping network -> FiLM table -------------------------------------------------------------------
  * CustomMappingNetwork (siren/siren.py:82-102: Linear(z, 256) + LeakyReLU(0.2), 3 x [Linear(256, 256) + LeakyReLU],
  * Linear(256, n_layers * 512)), the halves split into frequencies / phase shifts (:100-101), the `15 f + 30`
@@ -505,6 +518,14 @@ int fenerf_composite_backward_rays(const fenerf_render_desc* rd, int32_t out_dim
                                    const float* rng_noise, const float* d_pixels, float* d_raw_coarse, float* d_raw_fine,
                                    void* stream);
 
+/* fenerf_composite_backward_rays of a non-hierarchical render that also returns d_z (B, N, S), the gradient w.r.t. the
+ * depths z_coarse: d delta_j = d alpha_j act_j exp(-delta_j act_j) over the depth-ordered intervals (the far one is the
+ * constant 1e10), d z_i = d delta_{i-1} - d delta_i.  d_raw_coarse bit for bit as fenerf_composite_backward_rays.
+ * One write per sample, no atomics. */
+int fenerf_composite_backward_rays_dz(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse,
+                                      const float* z_coarse, const float* rng_noise, const float* d_pixels,
+                                      float* d_raw_coarse, float* d_z, void* stream);
+
 /* One FiLM layer's forward values for the backward (siren/siren.py:113-123): from the GEMM output
  * z (n_points, 256) fp32 (NULL for the first layer) plus optional narrow inputs narrow_in (n_points, w) fp32
  * against narrow_w (256, w) fp32 (positions; [dir, grid features] of the first colour layer):
@@ -541,6 +562,23 @@ int fenerf_grid_scatter_add(const fenerf_field_desc* field, const float* points,
                             int64_t n_points, float* grad_channels_last, int32_t dtype, void* stream);
 int fenerf_grid_unpack_grad(const fenerf_field_desc* field, const float* grad_channels_last, float* out,
                             const float* inv_scale, void* stream);
+
+/* Gradients w.r.t. a rays-in render's own inputs (point_forward with ray_grad=True); one thread per point / ray, no
+ * atomics.
+ *   fenerf_grid_coord_grad  d_coord (n_points, 3) fp32 = d feat . d feat / d x of the trilinear lookup at
+ *                           x = points * input_scale (grid_sample's align_corners=True: the factor (R - 1) / 2; zero
+ *                           padding; x -> W, y -> H, z -> D), d feat (n_points, ld >= 32) of `dtype`; the 8 corners x 32
+ *                           channels of the packed fp32 channels-last grid are gathered per point (1 KB)
+ *   fenerf_ray_dir_grad     d_dirs (n_rays * num_steps / dir_group, 3) = (coarse + fine) * *inv_scale (a DEVICE scalar)
+ *                           from the per-point direction gradients d_dir_coarse and d_dir_fine (n_rays, num_steps, 3);
+ *                           dir_group 1: fine sample j goes to slot fine_slots[j] (a permutation per ray; from
+ *                           fenerf_render_rays_grad), dir_group num_steps: per-ray sums in index order.  d_dir_fine NULL:
+ *                           the fine pass read no caller direction */
+int fenerf_grid_coord_grad(const fenerf_field_desc* field, const void* packed, const float* points, const void* d_feat,
+                           int32_t ld, int64_t n_points, float* d_coord, int32_t dtype, void* stream);
+int fenerf_ray_dir_grad(int64_t n_rays, int32_t num_steps, int32_t dir_group, const float* d_dir_coarse,
+                        const float* d_dir_fine, const uint8_t* fine_slots, const float* inv_scale, float* d_dirs,
+                        void* stream);
 
 /* Deterministic variants of the two backward sums that fenerf_gate_backward and fenerf_grid_scatter_add form with float
  * atomics (the order-dependent last bits): the same inputs give the same bits from call to call and process to process
