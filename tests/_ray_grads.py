@@ -38,7 +38,21 @@ CASES = {
     "rg_n_vardirs": (pf.PointCase("rg_n_vardirs", "N", 1, 414, vary_dirs=1.0, cfg=dict(_KW)), False),
     "rg_n_nohier": (pf.PointCase("rg_n_nohier", "N", 1, 415, vary_dirs=1.0, hierarchical=False, cfg=dict(_KW)), False),
     "rg_p_vardirs": (pf.PointCase("rg_p_vardirs", "P", 1, 416, vary_dirs=1.0, cfg=dict(_KW)), False),
+    # without hierarchical sampling: the depth gradient under each compositing option
+    "rg_b_nohier_white": (pf.PointCase("rg_b_nohier_white", "B", 1, 431, vary_dirs=1.0, hierarchical=False,
+                                       cfg=dict(_KW, white_back=True)), False),
+    "rg_b_nohier_black": (pf.PointCase("rg_b_nohier_black", "B", 1, 432, vary_dirs=1.0, hierarchical=False,
+                                       cfg=dict(_KW, black_back=True)), False),
+    "rg_b_nohier_softmax": (pf.PointCase("rg_b_nohier_softmax", "B", 1, 433, vary_dirs=1.0, hierarchical=False,
+                                         softmax_label=True, cfg=dict(_KW)), False),
+    "rg_b_nohier_softplus_noise": (pf.PointCase("rg_b_nohier_softplus_noise", "B", 1, 434, vary_dirs=1.0,
+                                                hierarchical=False, cfg=dict(_KW, clamp_mode='softplus', nerf_noise=0.5)),
+                                   False),
+    "rg_b_nohier_dup_z": (pf.PointCase("rg_b_nohier_dup_z", "B", 1, 435, vary_dirs=1.0, hierarchical=False,
+                                       cfg=dict(_KW)), False),
 }
+#: cases whose depths hold exact duplicates (zero-width intervals): see make_rays
+DUP_Z = {"rg_b_nohier_dup_z"}
 #: fields the reference has no point_forward for (single-latent generators): checked against chain() only, through
 #: backward.render_rays_with_grad.  L: the grid in the trunk; K: 129 channels (the wide compositing bodies), non-hierarchical
 #: so that the wide depth-gradient body runs
@@ -77,6 +91,11 @@ def make_rays(name):
     rays = pf.load_rays(case) if case.name in pf.CASE_BY_NAME else pf.make_rays(case)
     if expand:
         rays["dirs"] = rays["ray_dirs"].unsqueeze(2).expand(-1, -1, case.num_steps, -1)
+    if name in DUP_Z:      # every 3rd sample repeats its predecessor's depth on every other ray; the last two equal on all
+        z = rays["z_vals"].clone()
+        z[:, ::2, 3::3] = z[:, ::2, 2:-1:3][:, :, :z[:, ::2, 3::3].shape[2]]
+        z[:, :, -1] = z[:, :, -2]
+        rays["z_vals"] = z
     return rays
 
 

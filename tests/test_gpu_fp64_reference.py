@@ -7,6 +7,9 @@ checked on its own against a float64 restatement of the same operation, at the s
      shared-memory opt-in beyond 48 KB), 4-32 channels, every compositing option, exact depth ties; and, as a second
      entry ('-rays'), ``fenerf_composite_backward_rays`` (ray-major pixels in [0, 1]: its own kernel and opt-in), bit
      for bit the NCHW entry's result on the same upstream value (measured: 2.3e-6 at n = 128, C = 22, softplus + noise);
+     and on flat renders a third ('-rays_dz'), ``fenerf_composite_backward_rays_dz``: the same d raw bit for bit, and the
+     gradient w.r.t. the coarse depths against float64 autograd, from S = 2 up to the 256-step limit on both sides of
+     the narrow body's shared-memory limit (248 / 249 samples at C = 22);
   B. ``_FieldBackward`` for every field class under the chunk layouts of production: several images per chunk
      (FiLM rows of image b0 > 0) and one image split into point chunks (directions sliced at p0 // dir_group);
   C. the point network forward (exact and fast kernels) under the tile schedules of a real SM count.
@@ -40,6 +43,11 @@ gpu = pytest.mark.gpu
 #: composite backward, max |d_raw - fp64| / max |d_raw fp64| per tensor (coarse and fine).  Measured: 2.5e-6 (n = 128,
 #: C = 22, softplus + noise); 1.6e-6 at n = 96, 9.9e-7 at n = 48, <= 8.3e-7 up to 33.  The faults of D move it by >= 4.4e-3.
 COMPOSITE_BOUND = 1e-5
+#: the depth gradient of fenerf_composite_backward_rays_dz, max |d z - fp64| / max |d z fp64|.  Measured: 6.7e-5 (n = 256,
+#: C = 4, opaque, black_back), 3.2e-5 at n = 248, <= 1.0e-5 up to n = 64: each sample's d z is the difference of its two
+#: intervals' terms d alpha act exp(-delta act), which cancel where the density is high and the intervals short, so
+#: d alpha's fp32 rounding (COMPOSITE_BOUND's) grows relative to d z with S.
+DEPTH_BOUND = 2e-4
 #: field backward, max |grad - fp64| / max |grad fp64| per parameter tensor, the whole grid and each FiLM layer's
 #: frequency and phase gradients.  Measured: exact 3.1e-5 (model H, L1: d film of colour layer 5), 1.0e-5 at L4;
 #: default 1.21e-2 (model H, L1), 5.5e-3 at L4 -- the fp16 streams (u = f z + p recomputed from them, f ~ 30) set it.
@@ -90,12 +98,15 @@ def _per_point(dirs, ppb, lock):
 # --------------------------------------------------------------------------------------------
 # 0. float64 references
 # --------------------------------------------------------------------------------------------
-def composite_vjp(raw_c, z_c, raw_f, z_f, noise, opt, d_pixels, ray_major=False):
-    """(d raw_c, d raw_f) in float64 for the upstream gradient d_pixels (NCHW, or (B, N, C - 1) with ray_major)."""
+def composite_vjp(raw_c, z_c, raw_f, z_f, noise, opt, d_pixels, ray_major=False, want_z=False):
+    """(d raw_c, d raw_f) in float64 for the upstream gradient d_pixels (NCHW, or (B, N, C - 1) with ray_major);
+    want_z (no fine samples): (d raw_c, d z_c), the coarse depths a float64 leaf as well."""
+    assert not (want_z and raw_f is not None), "the depth gradient is that of a non-hierarchical render"
     leaves = [raw_c.double().requires_grad_(True)] + ([raw_f.double().requires_grad_(True)] if raw_f is not None else [])
+    z_c = z_c.double().requires_grad_(True) if want_z else z_c
     px = composite_ref(leaves[0], z_c, leaves[1] if raw_f is not None else None, z_f, noise, opt, ray_major=ray_major)
-    grads = torch.autograd.grad((px * d_pixels.double()).sum(), leaves)
-    return grads[0], (grads[1] if raw_f is not None else None)
+    grads = torch.autograd.grad((px * d_pixels.double()).sum(), leaves + ([z_c] if want_z else []))
+    return grads[0], grads[1] if (raw_f is not None or want_z) else None
 
 
 # --------------------------------------------------------------------------------------------
@@ -203,24 +214,45 @@ def _eval_with(ref, names, ps, pts, film, dirs):
 _OPTS = {"relu": _opt("relu"), "softplus_noise": _opt("softplus", noise=0.5), "softplus_last_back": _opt("softplus", last_back=True),
          "relu_white_back": _opt("relu", white_back=True), "relu_black_back": _opt("relu", black_back=True),
          "relu_softmax": _opt("relu", softmax=True), "softplus_noise_softmax": _opt("softplus", noise=0.5, softmax=True)}
-#: merged samples per ray: flat n = S, up to the library's limit of 64 steps; hierarchical n = 2 S (12+12, cfg2's 24+24,
-#: cfg5's 48+48, the 64+64 maximum)
-_SAMPLES = [(8, False), (31, False), (32, False), (33, False), (64, False), (24, True), (48, True), (96, True), (128, True)]
+#: merged samples per ray: flat n = S from the descriptor's least 2 steps; hierarchical n = 2 S (12+12, cfg2's 24+24,
+#: cfg5's 48+48, 64+64)
+_SAMPLES = [(2, False), (3, False), (8, False), (31, False), (32, False), (33, False), (64, False), (24, True), (48, True),
+            (96, True), (128, True)]
 _COMPOSITE = [(n, hier, c, o, opaque) for n, hier in _SAMPLES
               for c, o, opaque in [(4, "relu", False), (22, "softplus_noise", False), (32, "relu", True)]]
 _COMPOSITE += [(n, hier, c, o, opaque) for n, hier in [(33, False), (96, True), (128, True)]
                for c, o, opaque in [(23, "softplus_last_back", False), (4, "relu_white_back", True), (22, "relu_black_back", False),
                                     (22, "relu_softmax", False), (23, "softplus_noise_softmax", True)]]
+#: the flat ends of the library's 256 steps: C = 22's narrow body at S = 248 and its spill to the wide one at 249
+#: (narrow_pass_limit), S = 256 narrow at C = 4 and wide at C = 22
+_COMPOSITE += [(248, False, 22, "softplus_noise", False), (249, False, 22, "relu_white_back", False),
+               (256, False, 4, "relu_black_back", True), (256, False, 22, "relu_softmax", False)]
 _COMPOSITE_MODEL = {4: "A", 22: "D", 23: "E", 32: "D32"}
 _B, _R = 3, 37          # 37² rays per image: not a multiple of the 8 rays of a composite_backward block
-#: the two entries of the compositing backward: NCHW pixels * 2 - 1 (fenerf_composite_backward, the ids without a
-#: suffix) and ray-major pixels in [0, 1] (fenerf_composite_backward_rays, the rays-in render's; ids '-rays')
-ENTRIES = ("nchw", "rays")
+#: the entries of the compositing backward: NCHW pixels * 2 - 1 (fenerf_composite_backward, the ids without a suffix),
+#: ray-major pixels in [0, 1] (fenerf_composite_backward_rays, the rays-in render's; ids '-rays') and the same with the
+#: depth gradient of a non-hierarchical render (fenerf_composite_backward_rays_dz, point_forward(..., ray_grad=True)'s;
+#: ids '-rays_dz')
+ENTRIES = ("nchw", "rays", "rays_dz")
+
+
+def entries(hier):
+    """The compositing-backward entries a case runs on: the depth gradient is built for flat renders only."""
+    return ENTRIES if not hier else ENTRIES[:2]
 
 
 def with_entries(cases, ids):
-    """Every case on both compositing-backward entries; the NCHW entry keeps the case's id."""
-    return [pytest.param(*case, e, id=i + ("" if e == "nchw" else "-" + e)) for case, i in zip(cases, ids) for e in ENTRIES]
+    """Every case (n, hier, ...) on each of its compositing-backward entries; the NCHW entry keeps the case's id."""
+    return [pytest.param(*case, e, id=i + ("" if e == "nchw" else "-" + e)) for case, i in zip(cases, ids)
+            for e in entries(case[1])]
+
+
+def narrow_pass_limit(c):
+    """The most merged samples whose raw blocks, eight warps' of them, composite_backward stages in the narrow body's
+    227 KB of shared memory at C channels; beyond, the wide body reads rows from global memory.  A restatement of
+    composite_backward's plan (csrc/composite.cu: narrow_floats and the `wide` test after it): keep the two in step."""
+    fits = lambda n: 8 * ((7 * ((n + 3) & ~3) + 64 + n * c + 3) & ~3) * 4 <= 227 * 1024      # noqa: E731
+    return max(n for n in range(1, 513) if fits(n))
 
 
 @functools.lru_cache(maxsize=None)
@@ -248,21 +280,27 @@ def _composite_inputs(c, steps, hier, opaque):
 
 def _composite_backward(opt, steps, hier, x, noise, d_pixels, entry="nchw", batch=_B, img=_R):
     """One entry of the compositing backward; the gradient buffers start as NaN (an entry not written stays NaN).
-    'rays': the rays-in render's descriptor, img_h = 1 and img_w = the img² rays per image."""
+    'rays' / 'rays_dz': the rays-in render's descriptor, img_h = 1 and img_w = the img² rays per image; 'rays_dz'
+    returns (d raw_c, d z_c)."""
     c = x["raw_c"].shape[-1]
     rd = ops.make_render_desc(batch=batch, img_size=img, num_steps=steps, hierarchical=hier, clamp_mode=opt["clamp"],
                               nerf_noise=opt["noise"], fov=12, last_back=opt["last_back"], white_back=opt["white_back"],
                               black_back=opt["black_back"], softmax_label=opt["softmax"])
     lib = _lib.lib()
-    fn = lib.fenerf_composite_backward
-    if entry == "rays":
-        rd.img_h, rd.img_w = 1, img * img
-        fn = lib.fenerf_composite_backward_rays
     d_c = torch.full_like(x["raw_c"], float("nan"))
-    d_f = torch.full_like(x["raw_f"], float("nan")) if hier else None
     p = lambda t: t.data_ptr() if t is not None else 0                  # noqa: E731
+    stream = torch.cuda.current_stream().cuda_stream
+    if entry != "nchw":
+        rd.img_h, rd.img_w = 1, img * img
+    if entry == "rays_dz":
+        d_z = torch.full_like(x["z_c"], float("nan"))
+        _lib.check(lib.fenerf_composite_backward_rays_dz(ctypes.byref(rd), c, p(x["raw_c"]), p(x["z_c"]), p(noise),
+                                                         p(d_pixels), p(d_c), p(d_z), stream))
+        return d_c, d_z
+    fn = lib.fenerf_composite_backward_rays if entry == "rays" else lib.fenerf_composite_backward
+    d_f = torch.full_like(x["raw_f"], float("nan")) if hier else None
     _lib.check(fn(ctypes.byref(rd), c, p(x["raw_c"]), p(x["z_c"]), p(x["raw_f"]), p(x["z_f"]), p(noise), p(d_pixels), p(d_c),
-                  p(d_f), torch.cuda.current_stream().cuda_stream))
+                  p(d_f), stream))
     return d_c, d_f
 
 
@@ -270,27 +308,45 @@ def composite_backward_errors(o, steps, hier, x, noise, g, entry, batch=_B, img=
     """The compositing backward of `entry` on a d_pixels drawn from `g`, against composite_vjp -> (dict of the kernel's
     d_c, d_f and the float64 w_c, w_f; relative errors).
     'rays' is also run on the NCHW entry with d_pixels permuted to NCHW and halved: that entry doubles what it reads, so
-    both kernels see the same upstream value exactly, and their results must agree bit for bit."""
+    both kernels see the same upstream value exactly, and their results must agree bit for bit.  'rays_dz' must give the
+    'rays' entry's d raw bit for bit, and its depth gradient ('d_z', in place of d_f) is checked against float64 autograd
+    w.r.t. the coarse depths."""
     c = x["raw_c"].shape[-1]
     if entry == "nchw":
         d_pixels = torch.randn(batch, c - 1, img, img, generator=g).to(DEV)
     else:
         d_pixels = torch.randn(batch, img * img, c - 1, generator=g).to(DEV)
     d_c, d_f = _composite_backward(o, steps, hier, x, noise, d_pixels, entry, batch, img)
-    w_c, w_f = composite_vjp(x["raw_c"], x["z_c"], x["raw_f"], x["z_f"], noise, o, d_pixels, ray_major=entry == "rays")
+    w_c, w_f = composite_vjp(x["raw_c"], x["z_c"], x["raw_f"], x["z_f"], noise, o, d_pixels, ray_major=entry != "nchw",
+                             want_z=entry == "rays_dz")
     if entry == "rays":
         nchw = (0.5 * d_pixels).permute(0, 2, 1).reshape(batch, c - 1, img, img).contiguous()
         e_c, e_f = _composite_backward(o, steps, hier, x, noise, nchw, "nchw", batch, img)
         assert torch.equal(d_c, e_c), "ray-major d_raw_c differs from the NCHW entry's on the same upstream value"
         assert not hier or torch.equal(d_f, e_f), "ray-major d_raw_f differs from the NCHW entry's on the same upstream value"
+    if entry == "rays_dz":
+        e_c = _composite_backward(o, steps, hier, x, noise, d_pixels, "rays", batch, img)[0]
+        assert torch.equal(d_c, e_c), "the depth-gradient entry's d_raw_c differs from the ray-major entry's"
     errs = {"d_raw_c": _rel(d_c, w_c)}
-    if hier:
-        errs["d_raw_f"] = _rel(d_f, w_f)
+    if hier or entry == "rays_dz":
+        errs["d_z" if entry == "rays_dz" else "d_raw_f"] = _rel(d_f, w_f)
     assert all(v == v for v in errs.values()), errs          # (NaN: an entry was not written)
     return dict(d_c=d_c, d_f=d_f, w_c=w_c, w_f=w_f), errs
 
 
+def over_bounds(errs):
+    """The entries of a composite_backward_errors() result past their bound: DEPTH_BOUND for d z, COMPOSITE_BOUND else."""
+    return {k: v for k, v in errs.items() if v > (DEPTH_BOUND if k == "d_z" else COMPOSITE_BOUND)}
+
+
 _COMPOSITE_IDS = ["n%d-%s-C%d-%s%s" % (n, "hier" if h else "flat", c, o, "-opaque" if q else "") for n, h, c, o, q in _COMPOSITE]
+
+
+def test_flat_cases_straddle_the_narrow_body_limit():
+    """The flat cases put C = 22 on both sides of the narrow body's limit and S = 256 in the narrow body at C = 4."""
+    assert narrow_pass_limit(22) == 248 and narrow_pass_limit(4) >= 256
+    flat22 = {n for n, hier, c, _, _ in _COMPOSITE if c == 22 and not hier}
+    assert {248, 249, 256} <= flat22 and (256, False, 4) in {case[:3] for case in _COMPOSITE}
 
 
 @gpu
@@ -307,7 +363,7 @@ def test_composite_backward_vs_fp64(n, hier, c, opt, opaque, entry):
     noise = torch.randn(_B, _R * _R, n, generator=g).to(DEV) if o["noise"] else None
     errs = composite_backward_errors(o, steps, hier, x, noise, g, entry)[1]
     print("composite %s n=%d C=%d %s: %s" % (entry, n, c, opt, errs))
-    assert max(errs.values()) <= COMPOSITE_BOUND, errs
+    assert not over_bounds(errs), errs
 
 
 # --------------------------------------------------------------------------------------------

@@ -29,7 +29,7 @@ from oracle import render_oracle as oracle
 from test_dropin import _LOAD_WITH_MIRROR, _reference_checkpoint, _run
 from test_gpu_fp64_reference import (COMPOSITE_BOUND, FIELD_BOUND, FWD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward,
                                      _field_points, _forward_inputs, _grad_errors, _per_point, _render_points,
-                                     composite_backward_errors, with_entries)
+                                     composite_backward_errors, over_bounds, with_entries)
 
 DEV = "cuda:0"
 gpu = pytest.mark.gpu
@@ -460,7 +460,7 @@ def test_wide_composite_vs_fp64(n, hier, c, opt, entry):
         errs["d_sigma_f"] = _rel(t["d_f"][..., -1], t["w_f"][..., -1])
     assert all(v == v for v in errs.values()), errs          # (NaN: an entry was not written)
     print("wide composite %s n=%d C=%d %s: %s" % (entry, n, c, opt, errs))
-    assert max(errs.values()) <= COMPOSITE_BOUND, errs
+    assert not over_bounds(errs), errs
 
 
 @gpu

@@ -37,11 +37,38 @@ DEV = "cuda:0"
 # ---------------------------------------------------------------------------------------------------------------------
 # CPU: the grid coordinate gradient
 # ---------------------------------------------------------------------------------------------------------------------
-def grid_coord_grad_ref(grid, x, d_feat, fault=None):
+def fp32_cell_index(points, scale, R):
+    """The grid index of each axis as the kernels form it in fp32 (csrc/siren_common.cuh: trilinear), and as ATen's fp32
+    grid_sample does: fp32(fp32(fp32(p s) + 1) 0.5) (R - 1), for fp32 points p (any shape, last axis xyz)."""
+    p = np.asarray(points, dtype=np.float32)
+    x = p * np.float32(scale)
+    return ((x + np.float32(1)) * np.float32(0.5)) * np.float32(R - 1)
+
+
+def plant_on_index(values, target, scale, R, span=64):
+    """fp32 values near `values` (float64 array) whose fp32 index (fp32_cell_index) is exactly the integer `target` (same
+    shape), found among the 2 span + 1 fp32 neighbours -> (values, found mask)."""
+    v = np.asarray(values, dtype=np.float32)
+    out, found = v.copy(), np.zeros(v.shape, dtype=bool)
+    cand = v.copy()
+    down = v.copy()
+    for _ in range(span + 1):
+        for c in (cand, down):
+            hit = ~found & (fp32_cell_index(c, scale, R) == np.asarray(target, dtype=np.float32))
+            out[hit], found[hit] = c[hit], True
+        cand = np.nextafter(cand, np.float32(np.inf))
+        down = np.nextafter(down, np.float32(-np.inf))
+    return out, found
+
+
+def grid_coord_grad_ref(grid, x, d_feat, fault=None, cell=None):
     """d feat . d feat / d x of grid_sample(align_corners=True, zeros) at x (P, 3), grid (1, G, D, H, W), d_feat (P, G):
     the 8 corners' features dotted with d feat, the other two axes' weights, the per-axis sign and (R - 1) / 2 (what
-    grid_coord_grad_kernel computes).  fault: 'swap_axes' reads x -> D and z -> W, 'no_half' drops (R - 1) / 2,
-    'align_false' takes align_corners=False's coordinate map and factor R / 2."""
+    grid_coord_grad_kernel computes).  cell: the base cell (P, 3) to use (the floor of the kernel's fp32 index, which
+    decides the side of a one-sided derivative on a cell face); default the floor of x's own index.
+    fault: 'swap_axes' reads x -> D and z -> W, 'no_half' drops (R - 1) / 2, 'align_false' takes align_corners=False's
+    coordinate map and factor R / 2, 'clamp_upper_cell' keeps the cell below R - 1 (cell R - 2 at x = +1, the left-hand
+    derivative there), 'ceil_on_face' takes the cell below a face (ceil(i) - 1: the left-hand derivative on every face)."""
     g = grid[0].permute(1, 2, 3, 0)                                   # (D, H, W, G)
     R = g.shape[0]
     xs = x.flip(-1) if fault == "swap_axes" else x
@@ -51,13 +78,17 @@ def grid_coord_grad_ref(grid, x, d_feat, fault=None):
     else:
         i = (xs + 1) / 2 * (R - 1)
         half = 1.0 if fault == "no_half" else (R - 1) / 2
-    i0 = torch.floor(i)
+    i0 = torch.floor(i) if cell is None else cell.to(i.dtype)
+    if fault == "clamp_upper_cell":
+        i0 = i0.clamp(max=R - 2)
+    elif fault == "ceil_on_face":
+        i0 = torch.where(i0 == i, i0 - 1, i0)
     w1 = i - i0
     w = torch.stack([1 - w1, w1], -1)                                  # (P, 3, 2)
     out = torch.zeros_like(x)
     for k in range(8):
         e = [k & 1, (k >> 1) & 1, k >> 2]
-        idx = i0.long() + torch.tensor(e)
+        idx = i0.long() + torch.tensor(e, device=x.device)
         inside = ((idx >= 0) & (idx < R)).all(-1)
         ic = idx.clamp(0, R - 1)
         feat = g[ic[:, 2], ic[:, 1], ic[:, 0]] * inside.unsqueeze(-1)
@@ -102,6 +133,117 @@ def test_the_grid_comparison_catches(fault):
     want = _grid_sample_grad(grid, x, d_feat)
     err = (grid_coord_grad_ref(grid, x, d_feat, fault=fault) - want).abs().max().item() / want.abs().max().item()
     assert err > 5 * GRID_BOUND, err
+
+
+def plant_face_points(g, P, scale, R):
+    """fp32 points (P, 3) of a grid of R³ cells behind a box warp `scale`, in five classes of P / 5 rows, each row with
+    one planted axis a (the others random inside): an interior cell face (fp32 index an exact integer 1 .. R - 2), the
+    box boundary (x s = +-1 exactly: index 0 or R - 1), straddling the boundary (index in (-1, 0) or (R - 1, R): half the
+    corners outside), fully outside (index below -1 or above R), random inside.  -> (points, class per row (0 .. 4),
+    planted axis per row)."""
+    k = P // 5
+    cls = torch.arange(P) // k
+    cls[cls > 4] = 4
+    axis = torch.randint(0, 3, (P,), generator=g)
+    idx = torch.rand((P, 3), generator=g, dtype=torch.float64) * (R - 1)
+    u = torch.rand(P, generator=g, dtype=torch.float64)
+    side = torch.rand(P, generator=g) < 0.5
+    target = torch.randint(1, R - 1, (P,), generator=g).double()
+    target[cls == 1] = torch.where(side, 0.0, R - 1.0).double()[cls == 1]
+    planted = idx.gather(1, axis[:, None])[:, 0]
+    planted = torch.where(cls <= 1, target, planted)
+    planted = torch.where(cls == 2, torch.where(side, -u, R - 1 + u), planted)
+    planted = torch.where(cls == 3, torch.where(side, -1.5 - 4 * u, R + 0.5 + 4 * u), planted)
+    idx.scatter_(1, axis[:, None], planted[:, None])
+    pts = ((idx / (R - 1)) * 2 - 1) / scale
+    out = pts.float().numpy().copy()
+    face = (cls <= 1).numpy()
+    rows = np.nonzero(face)[0]
+    a = axis.numpy()[rows]
+    v, found = plant_on_index(pts.numpy()[rows, a], target.numpy()[rows], scale, R)
+    out[rows, a] = v
+    keep = np.ones(P, dtype=bool)
+    keep[rows[~found]] = False                 # no fp32 value of that index: the row is dropped
+    return torch.from_numpy(out)[keep], cls[keep], axis[keep]
+
+
+def fp32_cells(points, scale, R):
+    return torch.from_numpy(np.floor(fp32_cell_index(points.numpy(), scale, R))).long()
+
+
+def _one_sided(grid, x, d_feat, axis, h=1e-6):
+    """(f(y + h e_axis) - f(y)) / h, f = sum(grid_sample(y) * d feat), in float64: the right-hand derivative along `axis`
+    at y = x moved onto the nearest face along that axis in float64 (x s itself may lie 1e-7 cells to either side of it;
+    the derivative along an axis is the same everywhere in a cell)."""
+    def f(y):
+        return (F.grid_sample(grid, y.reshape(1, 1, 1, -1, 3), mode='bilinear', padding_mode='zeros',
+                              align_corners=True).reshape(grid.shape[1], -1).t() * d_feat).sum(-1)
+    R = grid.shape[-1]
+    rows = torch.arange(x.shape[0])
+    y = x.clone()
+    k = ((x[rows, axis] + 1) / 2 * (R - 1)).round()
+    y[rows, axis] = k / (R - 1) * 2 - 1
+    step = torch.zeros_like(x)
+    step[rows, axis] = h
+    return (f(y + step) - f(y)) / h
+
+
+#: the grid reference on planted points: against grid_sample's float64 autograd off the faces, against the one-sided
+#: finite difference (of a function linear along the axis within a cell: rounding only) on them
+GRID_FD_BOUND = 1e-7
+_FACE_SCALE, _FACE_R = 1 / 0.24 * 2, 9
+
+
+def _face_case():
+    g = torch.Generator().manual_seed(11)
+    pts, cls, axis = plant_face_points(g, 5000, _FACE_SCALE, _FACE_R)
+    grid = torch.randn((1, 32, _FACE_R, _FACE_R, _FACE_R), generator=g, dtype=torch.float64)
+    d_feat = torch.randn((pts.shape[0], 32), generator=g, dtype=torch.float64)
+    return grid, pts, cls, axis, d_feat
+
+
+def test_planted_points_hit_their_classes():
+    """Each class keeps most of its rows, and every face / boundary row's fp32 index is an exact integer."""
+    _, pts, cls, axis, _ = _face_case()
+    idx = torch.from_numpy(fp32_cell_index(pts.numpy(), _FACE_SCALE, _FACE_R)).double()
+    planted = idx.gather(1, axis[:, None])[:, 0]
+    assert all((cls == c).sum().item() >= 700 for c in range(5))
+    assert torch.equal(planted[cls <= 1], planted[cls <= 1].round())
+    assert ((planted[cls == 1] == 0) | (planted[cls == 1] == _FACE_R - 1)).all()
+    assert ((planted[cls == 2] > -1) & (planted[cls == 2] < 0) | (planted[cls == 2] > _FACE_R - 1) & (planted[cls == 2] < _FACE_R)).all()
+    assert ((planted[cls == 3] < -1) | (planted[cls == 3] > _FACE_R)).all()
+
+
+def test_grid_reference_on_faces_is_the_one_sided_derivative():
+    """With the kernel's fp32 cells the reference is grid_sample's float64 autograd away from faces and the right-hand
+    finite difference along the planted axis on interior faces and on the box boundary (x s = +-1)."""
+    grid, pts, cls, axis, d_feat = _face_case()
+    x = pts.double() * _FACE_SCALE
+    cells = fp32_cells(pts, _FACE_SCALE, _FACE_R)
+    got = grid_coord_grad_ref(grid, x, d_feat, cell=cells)
+    off = cls >= 2
+    want = _grid_sample_grad(grid, x[off], d_feat[off])
+    assert (got[off] - want).abs().max().item() <= GRID_BOUND * want.abs().max().item()
+    assert torch.count_nonzero(got[cls == 3]).item() == 0                # fully outside: no corner inside
+    on = cls <= 1
+    fd = _one_sided(grid, x[on], d_feat[on], axis[on])
+    g_axis = got[on].gather(1, axis[on][:, None])[:, 0]
+    err = (g_axis - fd).abs().max().item() / fd.abs().max().item()
+    assert err <= GRID_FD_BOUND, err
+
+
+@pytest.mark.parametrize("fault", ["clamp_upper_cell", "ceil_on_face"])
+def test_the_face_comparison_catches(fault):
+    """A cell clamped below R - 1 at x s = +1, or the cell below every face: the left-hand derivative where the kernels
+    take the right-hand one, past 5x the bound of the face comparison."""
+    grid, pts, cls, axis, d_feat = _face_case()
+    x = pts.double() * _FACE_SCALE
+    on = cls <= 1
+    fd = _one_sided(grid, x[on], d_feat[on], axis[on])
+    bad = grid_coord_grad_ref(grid, x, d_feat, fault=fault, cell=fp32_cells(pts, _FACE_SCALE, _FACE_R))
+    g_axis = bad[on].gather(1, axis[on][:, None])[:, 0]
+    err = (g_axis - fd).abs().max().item() / fd.abs().max().item()
+    assert err > 5 * GRID_FD_BOUND, err
 
 
 # ---------------------------------------------------------------------------------------------------------------------
