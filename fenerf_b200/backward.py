@@ -37,24 +37,21 @@ taken from max|d raw| on the device (no host sync) and unscaled at the end.
 
 The three 256-wide products per layer run on wgmma (csrc/gemm.cu: ``fenerf_gemm_nt_film`` -- the recompute with its FiLM
 epilogue fused, ``fenerf_gemm_nt_f16`` for dA' = dU diag(f_b) W, ``fenerf_gemm_tn_f16`` split-K for the per-image M_b); only the narrow
-products (heads, the 3 / 35-wide inputs) go to the library.  ``FENERF_B200_BWD_GEMM=cublas`` switches the wide ones back
-(A/B timing); ``precision='exact'`` uses fp32 library GEMMs, or, with ``grad_precision='split'``, the split kernels of
-csrc/gemm_split.cu on the same fp32 streams (fp16 hi / lo operands scaled by powers of two, fp32-grade results).  (The kernels can also fold the next layer's gate multiply
+products (heads, the 3 / 35-wide inputs) go to the library.  ``precision='exact'`` uses fp32 library GEMMs, or, with
+``grad_precision='split'``, the split kernels of csrc/gemm_split.cu on the same fp32 streams (fp16 hi / lo operands scaled
+by powers of two, fp32-grade results).  One stream object per backward (_Stream) holds its weight forms
+and forms these three products.  (The kernels can also fold the next layer's gate multiply
 into the dA product's epilogue and produce the bias column sums from the dW kernel's staged tiles -- measured: the gate kernel's
 17 ms disappear but the two GEMMs slow down by as much, both being HBM-bound; the chain below keeps the separate gate kernel.)
 """
+import contextlib
 import ctypes as C
 
 import torch
 
 from . import _lib, ops, packing
 
-import os
-
 CHUNK_POINTS = 1 << 19
-#: the 256-wide products: 'wgmma' = csrc/gemm.cu (default), 'cublas' = torch.mm / bmm (kept for A/B timing and as the
-#: fp32 path of precision='exact')
-BWD_GEMM = os.environ.get("FENERF_B200_BWD_GEMM", "wgmma")
 
 
 def _ptr(t):
@@ -222,21 +219,97 @@ def check_grad_precision(module, grad_precision, precision):
         raise RuntimeError(reason)
 
 
+class _Stream:
+    """The gradient stream of a backward: its weight forms and its three 256-wide products per FiLM layer.
+      'fp16'   the default: fp16 activations, gates and dU; the products on the wgmma kernels of csrc/gemm.cu
+      'exact'  precision='exact' (and 'split' renders): fp32 activations, gates and dU; the products as fp32 torch GEMMs
+      'split'  grad_precision='split': the exact stream's tensors, the products on the split kernels of csrc/gemm_split.cu;
+               every weight and every image's (diag(f_b) W)^T split as (hi, lo, amax), and max |dU| as dU's scale
+    `film`, `bias`: the FiLM table and the biases by FiLM row; `narrow_w`: the first colour layer's fp32 weights of its
+    [dir, grid features]; `rows`: the recompute's fp32 (256, 256) weights by FiLM row (None at row 0: its inputs are the
+    points); `fW`: the chain products' diag(f_b) W, (B, n_film - 1, 256, 256) fp32.  (It keeps no reference to the
+    _FieldBackward: no cycle, so the backward's device buffers are freed the moment it returns.)"""
+
+    def __init__(self, kind, film, bias, narrow_w, rows, fW):
+        self.kind, self.film, self.bias, self.narrow_w = kind, film, bias, narrow_w
+        # element type of the activations, gates and dU, and its code in the C-ABI
+        self.dt, self.dtc = (torch.float16, 0) if kind == 'fp16' else (torch.float32, 1)
+        if kind == 'fp16':
+            self.W = [None if w is None else w.to(torch.float16).contiguous() for w in rows]
+            self.fW = fW.transpose(2, 3).to(torch.float16).contiguous()          # the NT kernel wants it transposed
+            self.Wn64 = torch.zeros((256, 64), dtype=torch.float16, device=film.device)
+            self.Wn64[:, :narrow_w.shape[1]] = narrow_w
+            return
+        self.W = [None if w is None else w.float().contiguous() for w in rows]
+        self.fW = fW
+        if kind == 'split':
+            self.W = [None] + [ops.split_weights(w) for w in self.W[1:]]
+            self.fW = ops.split_weights(fW.transpose(2, 3))
+
+    def stash(self, z, row, b0, P, ppb, xin=None, wx=None):
+        """(a, gate) of FiLM row `row` from its pre-activation z (None: zero) plus the narrow inputs xin wx^T
+        (fenerf_film_forward_stash): the first layer, a bridge field's first colour layer, the exact / split recompute."""
+        dev = self.film.device
+        a = torch.empty((P, 256), dtype=self.dt, device=dev)
+        g = torch.empty((P, 256), dtype=self.dt, device=dev)
+        kx = 0 if xin is None else xin.shape[1]
+        _lib.check(_lib.lib().fenerf_film_forward_stash(
+            _ptr(z), self.bias[row].data_ptr(), self.film[b0, row].data_ptr(), self.film.stride(0), P, ppb,
+            _ptr(xin), kx, _ptr(wx), a.data_ptr(), g.data_ptr(), self.dtc, _stream(dev)))
+        return a, g
+
+    def recompute(self, row, a_prev, b0, ppb, narrow=None):
+        """(a, gate) of FiLM row `row` from the previous layer's activations.  `narrow`: the first colour layer's other
+        inputs [dir, grid features]; on fp16 they ride as a fifth 64-wide k-chunk of the same kernel."""
+        if self.kind == 'fp16':     # z = a W^T with the FiLM epilogue fused: z never leaves the SM
+            if narrow is None:
+                return ops.gemm_nt_film(a_prev, self.W[row], self.bias[row], self.film, b0, row, ppb)
+            e64 = torch.zeros((a_prev.shape[0], 64), dtype=torch.float16, device=self.film.device)
+            e64[:, :self.narrow_w.shape[1]] = narrow
+            return ops.gemm_nt_film(a_prev, self.W[row], self.bias[row], self.film, b0, row, ppb, narrow_in=e64, narrow_w=self.Wn64)
+        if self.kind == 'split' and narrow is None:
+            return ops.gemm_nt_film_split(a_prev, *self.W[row], self.bias[row], self.film, b0, row, ppb)
+        z = ops.gemm_nt_split(a_prev, *self.W[row]) if self.kind == 'split' else torch.mm(a_prev, self.W[row].t())
+        return self.stash(z, row, b0, a_prev.shape[0], ppb, xin=narrow, wx=None if narrow is None else self.narrow_w)
+
+    def chain(self, dU, row, b0, b1, ppb, amax):
+        """dU diag(f_b) W of FiLM row `row` for each image b of the chunk: the gradient of the layer's input (P, 256)."""
+        k = b1 - b0
+        if self.kind == 'exact':
+            return torch.bmm(dU.view(k, ppb, 256), self.fW[b0:b1, row - 1]).view(k * ppb, 256)
+        out = torch.empty_like(dU)
+        for i in range(k):
+            rows = slice(i * ppb, (i + 1) * ppb)
+            if self.kind == 'fp16':
+                ops.gemm_nt(dU[rows], self.fW[b0 + i, row - 1], torch.float16, out=out[rows])
+            else:
+                hi, lo, w_amax = (t[b0 + i, row - 1] for t in self.fW)
+                ops.gemm_nt_split(dU[rows], hi, lo, w_amax, a_amax=amax, out=out[rows])
+        return out
+
+    def weight_product(self, dU, a_in, k, ppb, amax):
+        """The per-image M_b = dU_b^T a_in, (k, 256, 256) fp32."""
+        if self.kind == 'fp16':
+            return ops.gemm_tn(dU, a_in, k, ppb)
+        if self.kind == 'split':
+            return ops.gemm_tn_split(dU, a_in, k, ppb, x_amax=amax)
+        return torch.bmm(dU.view(k, ppb, 256).transpose(1, 2), a_in.view(k, ppb, 256))
+
+    def scale(self, dU):
+        """max |dU| on the device for the split products; None on the other streams."""
+        return ops.absmax(dU) if self.kind == 'split' else None
+
+
 class _FieldBackward:
     """Accumulates the gradients of one field over any number of point sets."""
 
     def __init__(self, module, film, scale, inv_scale, exact=False, split=False, grad_split=False):
-        self.module = module
         # grad_split (grad_precision='split'): the fp32 streams of the exact mode, the 256-wide products on the split
         # kernels of csrc/gemm_split.cu
-        self.gs = bool(grad_split)
-        if self.gs and not exact:
+        if grad_split and not exact:
             raise RuntimeError(_GRAD_SPLIT_STREAMS)
-        if self.gs and _grad_split_refusal(module.field_spec()):
+        if grad_split and _grad_split_refusal(module.field_spec()):
             raise RuntimeError(_grad_split_refusal(module.field_spec()))
-        # stream element type: fp16 (default) or fp32 (parity mode, with precision='exact': plain fp32 GEMMs)
-        self.dt = torch.float32 if exact else torch.float16
-        self.dtc = 1 if exact else 0
         self.fw = FieldWeights(module)
         self.spec = self.fw.spec
         self.packed = module.packed(split=split)       # (split: the pack the forward rendered from; same sections)
@@ -247,7 +320,7 @@ class _FieldBackward:
         B = self.film.shape[0]
         T, Cn = len(self.fw.trunk), len(self.fw.color)
         self.lf = len(self.fw.label_film)                          # 1: a label FiLM layer at row T, colour from T + 1
-        self.T, self.Cn, self.c0, self.n_film = T, Cn, T + self.lf, T + self.lf + Cn
+        self.T, self.c0, self.n_film = T, T + self.lf, T + self.lf + Cn
         G = self.spec.grid_channels
         # narrow inputs: the first layer's [pos] -- [feat, pos] with the grid in the trunk (EmbeddingPiGAN256) -- and the
         # first colour layer's [dir, feat] -- [dir] with the grid in the trunk
@@ -283,11 +356,9 @@ class _FieldBackward:
         if G and self.det:
             nbytes = _lib.lib().fenerf_grid_scatter_det_workspace_bytes(C.byref(self.packed.desc))
             self.grid_det_ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        # fp16 / fp32 weight views for the GEMMs
+        # the narrow products' weights and the 256-wide weights of the gradient stream
         fw = self.fw
         self.W0 = fw.trunk[0][0].detach().float().contiguous()                    # (256, 3); grid trunk (256, G + 3)
-        self.own_gemm = (not exact) and BWD_GEMM == "wgmma"
-        self.Wh16 = [None] + [w.detach().to(self.dt).contiguous() for w, _ in fw.trunk[1:]]
         wc0 = fw.color[0][0].detach().float()
         # a direction-free field's first colour layer reads [feat, x]: zero direction columns give it the [dir, feat, x]
         # order of the other grid fields (finish() drops them again)
@@ -318,34 +389,29 @@ class _FieldBackward:
             self.d_bv = torch.zeros(3, dtype=torch.float32, device=dev)
             wc0 = torch.cat([self.Wc0eff, torch.zeros((256, 256), dtype=torch.float32, device=dev)], dim=1)
         self.Wc0x_narrow = wc0[:, :self.kx].contiguous()                          # (256, 3 + G) fp32
-        self.Wc16 = [wc0[:, self.kx:].to(self.dt).contiguous()] + [w.detach().to(self.dt).contiguous() for w, _ in fw.color[1:]]
-        # grad_split: the recompute's 256-wide weights by FiLM row (trunk 1.., colour c0..), split as (hi, lo, amax)
-        self.Wsplit = [None] + [ops.split_weights(w) for w in self.Wh16[1:] + self.Wc16] if self.gs else None
         # the weights the grid features meet, (256, G): the first colour layer's, or the first layer's with the grid in
         # the trunk, whose FiLM row is then 0
         self.feat_row = 0 if self.gt else self.c0
         self.Wfeat32 = (self.W0[:, :G] if self.gt else wc0[:, 3:self.kx].contiguous()) if G else None
-        # fp32 weights of the chain products dA' = dU diag(f_b) W, by FiLM row (row 0 has none: its inputs are the points)
-        self.Wchain32 = [None] + [w.detach().float() for w, _ in fw.trunk[1:]]
         if self.lf:
-            self.Wl16 = fw.label_film[0][0].detach().to(self.dt).contiguous()
-            self.Wchain32.append(fw.label_film[0][0].detach().float())
             self.Wlhead32 = fw.labels[0][0].detach().float().contiguous()                 # (L, 256)
-        # a bridge field's first colour layer passes dU diag(f_b) W_c0[:, v] W_v (rank 3) to the trunk
-        wc0_chain = (self.Wc0eff[:, 3:6].double() @ self.Wv32.double()).float() if self.br else wc0[:, self.kx:]
-        self.Wchain32 += [wc0_chain] + [w.detach().float() for w, _ in fw.color[1:]]
-        # ... scaled per image once for every chunk: diag(f_b) W, (B, n_film - 1, 256, 256); the NT kernel wants it transposed
-        fW = self.film[:, 1:, 0].unsqueeze(3) * torch.stack(self.Wchain32[1:])
-        if self.gs:     # per image and layer, (diag(f_b) W)^T scaled by its own power of two and split
-            self.fW_hi, self.fW_lo, self.fW_amax = ops.split_weights(fW.transpose(2, 3))
-            self.fW = None
-        else:
-            self.fW = fW.transpose(2, 3).to(torch.float16).contiguous() if self.own_gemm else fW.to(self.dt)
-        del fW
+        # the 256-wide weights by FiLM row (row 0 has none: its inputs are the points): trunk, label FiLM layer, colour
+        wide = ([None] + [w.detach() for w, _ in fw.trunk[1:] + fw.label_film] + [wc0[:, self.kx:]]
+                + [w.detach() for w, _ in fw.color[1:]])
+        # the chain products dA' = dU diag(f_b) W use the same weights, except a bridge field's first colour layer: it
+        # passes dU diag(f_b) W_c0[:, v] W_v (rank 3) to the trunk
+        chain = list(wide)
+        if self.br:
+            chain[self.c0] = (self.Wc0eff[:, 3:6].double() @ self.Wv32.double()).float()
+        # ... scaled per image once for every chunk: diag(f_b) W, (B, n_film - 1, 256, 256)
+        fW = self.film[:, 1:, 0].unsqueeze(3) * torch.stack([w.float() for w in chain[1:]])
+        self.stream = _Stream('split' if grad_split else 'exact' if exact else 'fp16', self.film, self.bias, self.Wc0x_narrow,
+                              wide, fW)
+        self.dt, self.dtc = self.stream.dt, self.stream.dtc       # fp16, or fp32 with precision='exact' / 'split'
         self.fWfeat = (self.film[:, self.feat_row, 0].unsqueeze(2) * self.Wfeat32).to(self.dt) if G else None    # (B, 256, G)
-        if self.own_gemm:
-            self.Wn64 = torch.zeros((256, 64), dtype=torch.float16, device=dev)
-            self.Wn64[:, :self.kx] = self.Wc0x_narrow
+        # the direction-free field: TF32 rounding would be amplified like fp16's (see above); grad_split: its narrow
+        # products stay fp32
+        self._narrow_precision = _NoTF32 if self.wd or grad_split else contextlib.nullcontext
         self.L = L
         heads = torch.zeros((self.n_heads, 256), dtype=torch.float32, device=dev)
         if L and not self.lf:      # (a label FiLM field's head acts on the label layer: its rows stay zero here)
@@ -364,40 +430,25 @@ class _FieldBackward:
     # ray_grad: optional (B, ppb, 3) fp32 outputs 'dx' (d points, coarse pass) and 'ddir' (d direction per point), in the
     # scaled stream units (times `scale`, without input_scale); None: the backward runs exactly as without them
     def add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad=None):
-        if self.wd or self.gs:     # the direction-free field: TF32 rounding would be amplified like fp16's (see __init__);
-            with _NoTF32():          # grad_split: its narrow products stay fp32
-                return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad)
-        return self._add_points(points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad)
-
-    def _add_points(self, points, dirs, dir_group, lock_dirs, raw, d_raw, ray_grad=None):
         B, ppb, _ = points.shape
 
         def outs(rows, cols):
             return None if ray_grad is None else {k: (v[rows, cols] if v is not None else None) for k, v in ray_grad.items()}
 
-        if ppb <= CHUNK_POINTS:
-            k = max(1, CHUNK_POINTS // ppb)
-            for b0 in range(0, B, k):
-                b1 = min(B, b0 + k)
-                self._chunk(points[b0:b1], dirs[b0:b1], dir_group, lock_dirs, raw[b0:b1], d_raw[b0:b1], b0, b1,
-                            outs(slice(b0, b1), slice(None)))
-        else:
+        with self._narrow_precision():
+            if ppb <= CHUNK_POINTS:
+                k = max(1, CHUNK_POINTS // ppb)
+                for b0 in range(0, B, k):
+                    b1 = min(B, b0 + k)
+                    self._chunk(points[b0:b1], dirs[b0:b1], dir_group, lock_dirs, raw[b0:b1], d_raw[b0:b1], b0, b1,
+                                outs(slice(b0, b1), slice(None)))
+                return
             step = CHUNK_POINTS // dir_group * dir_group
             for b in range(B):
                 for p0 in range(0, ppb, step):
                     p1 = min(ppb, p0 + step)
                     self._chunk(points[b:b + 1, p0:p1], dirs[b:b + 1, p0 // dir_group:p1 // dir_group], dir_group, lock_dirs,
                                 raw[b:b + 1, p0:p1], d_raw[b:b + 1, p0:p1], b, b + 1, outs(slice(b, b + 1), slice(p0, p1)))
-
-    def _stash(self, z, idx, b0, P, ppb, xin=None, wx=None):
-        a = torch.empty((P, 256), dtype=self.dt, device=self.dev)
-        g = torch.empty((P, 256), dtype=self.dt, device=self.dev)
-        film_l = self.film[b0, idx]
-        kx = 0 if xin is None else xin.shape[1]
-        _lib.check(_lib.lib().fenerf_film_forward_stash(
-            _ptr(z), self.bias[idx].data_ptr(), film_l.data_ptr(), self.film.stride(0), P, ppb,
-            _ptr(xin), kx, _ptr(wx), a.data_ptr(), g.data_ptr(), self.dtc, _stream(self.dev)))
-        return a, g
 
     def _gate(self, dA, gate, idx, b0, b1, P, ppb):
         cs = self.colsum[b0:b1, idx]
@@ -411,25 +462,6 @@ class _FieldBackward:
                                                        _stream(self.dev)))
         cs += tmp
 
-    def _chain(self, dU, idx, b0, b1, ppb, amax=None):
-        """dU diag(f_b) W of FiLM row idx for each image b of the chunk: the gradient of the layer's input (P, 256).
-        amax: max |dU| on the device (grad_split)."""
-        k = b1 - b0
-        if self.gs:
-            out = torch.empty_like(dU)
-            for i in range(k):
-                rows = slice(i * ppb, (i + 1) * ppb)
-                ops.gemm_nt_split(dU[rows], self.fW_hi[b0 + i, idx - 1], self.fW_lo[b0 + i, idx - 1],
-                                  self.fW_amax[b0 + i, idx - 1], a_amax=amax, out=out[rows])
-            return out
-        if not self.own_gemm:
-            return torch.bmm(dU.view(k, ppb, 256), self.fW[b0:b1, idx - 1]).view(k * ppb, 256)
-        out = torch.empty_like(dU)
-        for i in range(k):
-            rows = slice(i * ppb, (i + 1) * ppb)
-            ops.gemm_nt(dU[rows], self.fW[b0 + i, idx - 1], torch.float16, out=out[rows])
-        return out
-
     def _chunk(self, points, dirs, dir_group, lock_dirs, raw, d_raw, b0, b1, ray_grad=None):
         lib = _lib.lib()
         want_dx = ray_grad is not None and ray_grad.get('dx') is not None
@@ -438,14 +470,15 @@ class _FieldBackward:
         dev, spec = self.dev, self.spec
         k, ppb = points.shape[0], points.shape[1]
         P = k * ppb
-        T, Cn, c0 = self.T, self.Cn, self.c0
+        T, c0 = self.T, self.c0
+        stream = self.stream
         points = points.contiguous()
         dirs = dirs.contiguous()
         raw = raw.contiguous()
         d_raw = d_raw.contiguous()
         with torch.cuda.device(dev):
             st = _stream(dev)
-            # ---- recompute the forward, stashing activations and gates (fp16) ----
+            # ---- recompute the forward, stashing activations and gates ----
             x = (points.reshape(P, 3) * spec.input_scale).contiguous() if spec.input_scale != 1.0 else points.reshape(P, 3)
             G = spec.grid_channels
             extras = torch.empty((P, 3 + G), dtype=torch.float32, device=dev)     # [dir, feat]
@@ -455,46 +488,20 @@ class _FieldBackward:
                 x = torch.cat([extras[:, 3:], x], dim=1).contiguous()
                 extras = extras[:, :3].contiguous()
             A, Gt = [None] * self.n_film, [None] * self.n_film
-            own = self.own_gemm
-            A[0], Gt[0] = self._stash(None, 0, b0, P, ppb, xin=x, wx=self.W0)
-            for l in range(1, T):
-                if own:     # z = a W^T with the FiLM epilogue fused: z never leaves the SM
-                    A[l], Gt[l] = ops.gemm_nt_film(A[l - 1], self.Wh16[l], self.bias[l], self.film, b0, l, ppb)
-                elif self.gs:
-                    A[l], Gt[l] = ops.gemm_nt_film_split(A[l - 1], *self.Wsplit[l], self.bias[l], self.film, b0, l, ppb)
-                else:
-                    A[l], Gt[l] = self._stash(_mm32(A[l - 1], self.Wh16[l].t()), l, b0, P, ppb)
-            if self.lf:     # the label FiLM layer, on the trunk output
-                if own:
-                    A[T], Gt[T] = ops.gemm_nt_film(A[T - 1], self.Wl16, self.bias[T], self.film, b0, T, ppb)
-                else:
-                    A[T], Gt[T] = self._stash(_mm32(A[T - 1], self.Wl16.t()), T, b0, P, ppb)
+            A[0], Gt[0] = stream.stash(None, 0, b0, P, ppb, xin=x, wx=self.W0)
+            for l in range(1, c0):     # the trunk, then the label FiLM layer on the trunk output
+                A[l], Gt[l] = stream.recompute(l, A[l - 1], b0, ppb)
             v = None
             if self.br:     # v off the trunk output (fp32), then the first colour layer on [dir, v] like a first layer
                 v = _mm32(A[T - 1], self.Wv32.t().to(self.dt)) + self.bv32
                 if self.res:
                     v = v + x
                 extras = torch.cat([extras, v], dim=1).contiguous()
-                A[c0], Gt[c0] = self._stash(None, c0, b0, P, ppb, xin=extras, wx=self.Wc0eff)
-            elif own:     # the narrow inputs [dir, grid features] ride as a fifth 64-wide k-chunk of the same kernel
-                e64 = torch.zeros((P, 64), dtype=torch.float16, device=dev)
-                e64[:, :self.kx] = extras
-                A[c0], Gt[c0] = ops.gemm_nt_film(A[T - 1], self.Wc16[0], self.bias[c0], self.film, b0, c0, ppb, narrow_in=e64,
-                                                 narrow_w=self.Wn64)
-                del e64
+                A[c0], Gt[c0] = stream.stash(None, c0, b0, P, ppb, xin=extras, wx=self.Wc0eff)
             else:
-                z = ops.gemm_nt_split(A[T - 1], *self.Wsplit[c0]) if self.gs else _mm32(A[T - 1], self.Wc16[0].t())
-                A[c0], Gt[c0] = self._stash(z, c0, b0, P, ppb, xin=extras, wx=self.Wc0x_narrow)
-                del z
-            for j in range(1, Cn):
-                if own:
-                    A[c0 + j], Gt[c0 + j] = ops.gemm_nt_film(A[c0 + j - 1], self.Wc16[j], self.bias[c0 + j], self.film, b0, c0 + j,
-                                                             ppb)
-                elif self.gs:
-                    A[c0 + j], Gt[c0 + j] = ops.gemm_nt_film_split(A[c0 + j - 1], *self.Wsplit[c0 + j], self.bias[c0 + j], self.film,
-                                                                   b0, c0 + j, ppb)
-                else:
-                    A[c0 + j], Gt[c0 + j] = self._stash(_mm32(A[c0 + j - 1], self.Wc16[j].t()), c0 + j, b0, P, ppb)
+                A[c0], Gt[c0] = stream.recompute(c0, A[T - 1], b0, ppb, narrow=extras)
+            for l in range(c0 + 1, self.n_film):
+                A[l], Gt[l] = stream.recompute(l, A[l - 1], b0, ppb)
             # ---- head gradients ----
             dH = torch.empty((P, self.n_heads), dtype=self.dt, device=dev)
             dRGB = torch.empty((P, self.n_rgb), dtype=self.dt, device=dev)
@@ -513,36 +520,29 @@ class _FieldBackward:
             self.d_heads_b += dH.float().sum(0)
             # ---- colour branch, top down ----
             dA = torch.mm(dRGB, self.Wrgb16)                                   # (P, 256) fp16
-            for j in range(Cn - 1, -1, -1):
-                idx = c0 + j
+            for idx in range(self.n_film - 1, c0 - 1, -1):
                 self._gate(dA, Gt[idx], idx, b0, b1, P, ppb)                   # dA is dU now
-                if self.br and j == 0:
+                amax = stream.scale(dA)
+                if self.br and idx == c0:
                     dv = self._bridge_back(dA, extras, v, A[T - 1], d_sigma, k, ppb, b0, b1)
                     if want_dir:
                         ray_grad['ddir'].copy_(self._narrow_grad(dA, self.Wc0eff[:, 0:3], c0, k, ppb, b0, b1))
                     if want_dx and self.res:      # v = x + res_coord_layer(a): dv (with dsigma a) reaches x
                         dx_res = dv
-                    dA = self._chain(dA, idx, b0, b1, ppb)
-                    A[idx], Gt[idx] = None, None
-                    break
-                a_in = A[idx - 1] if j else A[T - 1]
-                du3 = dA.view(k, ppb, 256).transpose(1, 2)
-                amax = ops.absmax(dA) if self.gs else None      # (grad_split: the scale of this layer's dU, on the device)
-                if self.gs:
-                    self.dW_b[idx][b0:b1] += ops.gemm_tn_split(dA, a_in, k, ppb, x_amax=amax)
                 else:
-                    self.dW_b[idx][b0:b1] += ops.gemm_tn(dA, a_in, k, ppb) if own else _bmm32(du3, a_in.view(k, ppb, 256))
-                if j == 0:
-                    e16 = torch.zeros((P, self.kx_pad), dtype=self.dt, device=dev)
-                    e16[:, :self.kx] = extras
-                    self.dWx_b[b0:b1] += _bmm32(du3, e16.view(k, ppb, self.kx_pad))
-                    if G and not self.gt:
-                        d_feat = self._grid_grad(dA, points, k, ppb, b0, b1)
-                        if want_dx:
-                            dx_grid = self._coord_grad(d_feat, points, P)
-                    if want_dir:
-                        ray_grad['ddir'].copy_(self._narrow_grad(dA, self.Wc0x_narrow[:, 0:3], c0, k, ppb, b0, b1))
-                dA = self._chain(dA, idx, b0, b1, ppb, amax)
+                    a_in = A[idx - 1] if idx > c0 else A[T - 1]
+                    self.dW_b[idx][b0:b1] += stream.weight_product(dA, a_in, k, ppb, amax)
+                    if idx == c0:     # the narrow inputs [dir, grid features]: their weights, the grid, d dir
+                        e16 = torch.zeros((P, self.kx_pad), dtype=self.dt, device=dev)
+                        e16[:, :self.kx] = extras
+                        self.dWx_b[b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), e16.view(k, ppb, self.kx_pad))
+                        if G and not self.gt:
+                            d_feat = self._grid_grad(dA, points, k, ppb, b0, b1)
+                            if want_dx:
+                                dx_grid = self._coord_grad(d_feat, points, P)
+                        if want_dir:
+                            ray_grad['ddir'].copy_(self._narrow_grad(dA, self.Wc0x_narrow[:, 0:3], c0, k, ppb, b0, b1))
+                dA = stream.chain(dA, idx, b0, b1, ppb, amax)
                 A[idx], Gt[idx] = None, None
             # ---- trunk: colour-branch gradient + sigma / label heads ----
             dA += torch.mm(dH.float(), self.Wheads32)
@@ -550,22 +550,15 @@ class _FieldBackward:
                 # (P, 256), formed in fp32: an fp16 product's reduction order depends on the chunk's row count
                 dAl = torch.mm(dH[:, :self.L].float(), self.Wlhead32).to(self.dt)
                 self._gate(dAl, Gt[T], T, b0, b1, P, ppb)
-                if own:
-                    self.dW_b[T][b0:b1] += ops.gemm_tn(dAl, A[T - 1], k, ppb)
-                else:
-                    self.dW_b[T][b0:b1] += _bmm32(dAl.view(k, ppb, 256).transpose(1, 2), A[T - 1].view(k, ppb, 256))
-                dA += self._chain(dAl, T, b0, b1, ppb)
+                amax = stream.scale(dAl)
+                self.dW_b[T][b0:b1] += stream.weight_product(dAl, A[T - 1], k, ppb, amax)
+                dA += stream.chain(dAl, T, b0, b1, ppb, amax)
                 A[T], Gt[T] = None, None
             for l in range(T - 1, 0, -1):
                 self._gate(dA, Gt[l], l, b0, b1, P, ppb)
-                amax = ops.absmax(dA) if self.gs else None
-                if own:
-                    self.dW_b[l][b0:b1] += ops.gemm_tn(dA, A[l - 1], k, ppb)
-                elif self.gs:
-                    self.dW_b[l][b0:b1] += ops.gemm_tn_split(dA, A[l - 1], k, ppb, x_amax=amax)
-                else:
-                    self.dW_b[l][b0:b1] += _bmm32(dA.view(k, ppb, 256).transpose(1, 2), A[l - 1].view(k, ppb, 256))
-                dA = self._chain(dA, l, b0, b1, ppb, amax)
+                amax = stream.scale(dA)
+                self.dW_b[l][b0:b1] += stream.weight_product(dA, A[l - 1], k, ppb, amax)
+                dA = stream.chain(dA, l, b0, b1, ppb, amax)
                 A[l], Gt[l] = None, None
             self._gate(dA, Gt[0], 0, b0, b1, P, ppb)
             if self.gt:
@@ -585,8 +578,8 @@ class _FieldBackward:
 
     def _bridge_back(self, dU, extras, v, a_trunk, d_sigma, k, ppb, b0, b1):
         """First colour layer of a bridge field on [dir, v]: its narrow weight gradient, dv = dU diag(f) W_c0[:, v]
-        (+ dsigma a for RES) and v's own gradients, in fp32 (3 columns).  The trunk's share dv W_v goes through _chain
-        and the sigma head instead (see the module docstring)."""
+        (+ dsigma a for RES) and v's own gradients, in fp32 (3 columns).  The trunk's share dv W_v goes through the chain
+        product and the sigma head instead (see the module docstring)."""
         P = k * ppb
         du = dU.float().view(k, ppb, 256)
         e = torch.zeros((P, self.kx_pad), dtype=torch.float32, device=self.dev)
@@ -633,10 +626,8 @@ class _FieldBackward:
 
     # ---- after every point set: fold the per-image accumulators into parameter / FiLM gradients ----
     def finish(self):
-        if self.wd or self.gs:
-            with _NoTF32():
-                return self._finish()
-        return self._finish()
+        with self._narrow_precision():
+            return self._finish()
 
     def _finish(self):
         fw, inv = self.fw, self.inv_scale
@@ -707,6 +698,38 @@ class _FieldBackward:
         return d_film, grads
 
 
+def _save_inputs(ctx, call, film, params):
+    ctx.call = call
+    ctx.save_for_backward(film, *params)
+    ctx.param_ids = [id(p) for p in call['params']]
+
+
+def _field_backward(call, film, d_raw_c, d_raw_f):
+    """The _FieldBackward of a render: its precision and grad_precision, the fp16 stream's scale a power of two taken from
+    max |d raw| on the device (no host sync)."""
+    module, rd = call['module'], call['rd']
+    m = d_raw_c.abs().max()
+    if d_raw_f is not None:
+        m = torch.maximum(m, d_raw_f.abs().max())
+    scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)
+    inv_scale = (1.0 / scale).float().reshape(1)
+    # precision='split' renders forward on the split-precision kernel and differentiates as 'exact' does
+    split = rd.precision == _lib.PRECISION['split']
+    return _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'], split=split,
+                          grad_split=call.get('grad_precision') == 'split')
+
+
+def _input_grads(ctx, d_film, grads):
+    """The backward's outputs for film, call and the field parameters."""
+    out = [d_film if ctx.needs_input_grad[0] else None, None]
+    for i, pid in enumerate(ctx.param_ids):
+        g = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
+        if g is not None:
+            g = g.reshape(ctx.saved_tensors[1 + i].shape)
+        out.append(g)
+    return out
+
+
 class RenderFunction(torch.autograd.Function):
     """pixels = render(film, field parameters); see the module docstring."""
 
@@ -716,9 +739,8 @@ class RenderFunction(torch.autograd.Function):
         module, rd = call['module'], call['rd']
         st = ops.render_forward_stages(module, rd, film, call['x_lin'], call['y_lin'], call['z_lin'], call['cam2world'],
                                        call['rng_perturb'], call['rng_noise_c'], call['rng_u'], call['rng_noise_f'])
-        ctx.call, ctx.stages = call, st
-        ctx.save_for_backward(film, *params)
-        ctx.param_ids = [id(p) for p in call['params']]
+        ctx.stages = st
+        _save_inputs(ctx, call, film, params)
         return st['pixels']
 
     @staticmethod
@@ -726,7 +748,7 @@ class RenderFunction(torch.autograd.Function):
     def backward(ctx, d_pixels):
         call, st = ctx.call, ctx.stages
         film = ctx.saved_tensors[0]
-        module, rd = call['module'], call['rd']
+        rd = call['rd']
         dev = film.device
         lib = _lib.lib()
         B, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
@@ -746,15 +768,7 @@ class RenderFunction(torch.autograd.Function):
                 C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
                 _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
                 _stream(dev)))
-            m = d_raw_c.abs().max()
-            if hier:
-                m = torch.maximum(m, d_raw_f.abs().max())
-            scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)
-            inv_scale = (1.0 / scale).float().reshape(1)
-            # precision='split' renders forward on the split-precision kernel and differentiates as 'exact' does
-            split = rd.precision == _lib.PRECISION['split']
-            fb = _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'],
-                                split=split, grad_split=call.get('grad_precision') == 'split')
+            fb = _field_backward(call, film, d_raw_c, d_raw_f)
             lock = bool(rd.lock_view_dependence)
             rays = call.get('grad_rays')
             dirs = st['dirs']
@@ -771,13 +785,7 @@ class RenderFunction(torch.autograd.Function):
                 fb.add_points(pick(st['points_f'], 3), dirs, s, lock, pick(st['raw_f'], c), pick(d_raw_f, c))
             fb.add_points(pick(st['points_c'], 3), dirs, s, lock, pick(st['raw_c'], c), pick(d_raw_c, c))
             d_film, grads = fb.finish()
-        out = [d_film if ctx.needs_input_grad[0] else None, None]
-        for i, pid in enumerate(ctx.param_ids):
-            g = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
-            if g is not None:
-                g = g.reshape(ctx.saved_tensors[1 + i].shape)
-            out.append(g)
-        return tuple(out)
+        return tuple(_input_grads(ctx, d_film, grads))
 
 
 class RaysRenderFunction(torch.autograd.Function):
@@ -799,9 +807,8 @@ class RaysRenderFunction(torch.autograd.Function):
         slots = bool(rays) and ctx.needs_input_grad[2 + n_params + 1]
         st = ops.render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, call['rng_noise_c'],
                                     call['rng_u'], call['rng_noise_f'], slots=slots)
-        ctx.call, ctx.stages = call, st
-        ctx.save_for_backward(film, *inputs[:n_params])
-        ctx.param_ids = [id(p) for p in call['params']]
+        ctx.stages = st
+        _save_inputs(ctx, call, film, inputs[:n_params])
         ctx.ray_meta = [(t.shape, t.dtype) if t is not None else None for t in rays] if rays else None
         return st['pixels']
 
@@ -836,14 +843,7 @@ class RaysRenderFunction(torch.autograd.Function):
                     C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
                     _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
                     _stream(dev)))
-            m = d_raw_c.abs().max()
-            if hier:
-                m = torch.maximum(m, d_raw_f.abs().max())
-            scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)
-            inv_scale = (1.0 / scale).float().reshape(1)
-            split = rd.precision == _lib.PRECISION['split']
-            fb = _FieldBackward(module, film, scale, inv_scale, exact=split or rd.precision == _lib.PRECISION['exact'],
-                                split=split, grad_split=call.get('grad_precision') == 'split')
+            fb = _field_backward(call, film, d_raw_c, d_raw_f)
             g = st['dir_group']
             lock = bool(rd.lock_view_dependence)
             pc = B * rd.img_w * s
@@ -866,21 +866,16 @@ class RaysRenderFunction(torch.autograd.Function):
             d_film, grads = fb.finish()
             ray_grads = [None] * len(RAY_INPUTS)
             if dx is not None:
-                ray_grads[0] = dx * inv_scale * spec.input_scale
+                ray_grads[0] = dx * fb.inv_scale * spec.input_scale
             if dir_c is not None:
                 d_dirs = torch.empty((B * rd.img_w * s // g, 3), dtype=torch.float32, device=dev)
                 _lib.check(_lib.lib().fenerf_ray_dir_grad(B * rd.img_w, s, g, dir_c.data_ptr(), _ptr(dir_f),
                                                           _ptr(st['slots_f']) if dir_f is not None else 0,
-                                                          inv_scale.data_ptr(), d_dirs.data_ptr(), _stream(dev)))
+                                                          fb.inv_scale.data_ptr(), d_dirs.data_ptr(), _stream(dev)))
                 ray_grads[1] = d_dirs
             if d_z is not None:
                 ray_grads[4] = d_z
-        out = [d_film if ctx.needs_input_grad[0] else None, None]
-        for i, pid in enumerate(ctx.param_ids):
-            gr = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
-            if gr is not None:
-                gr = gr.reshape(ctx.saved_tensors[1 + i].shape)
-            out.append(gr)
+        out = _input_grads(ctx, d_film, grads)
         if ctx.ray_meta:
             for gr, meta, want in zip(ray_grads, ctx.ray_meta, need):
                 out.append(gr.reshape(meta[0]).to(meta[1]) if gr is not None and want else None)
@@ -929,8 +924,7 @@ def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_pertu
     `grad_precision`: None (the backward of the forward precision) or 'split' (fp32 streams, the 256-wide products on the
     split kernels of csrc/gemm_split.cu; forward precision 'split' or 'exact', the fields the split forward serves)."""
     check_grad_precision(module, grad_precision, rd.precision)
-    fw = FieldWeights(module)
-    params = fw.parameters()
+    params = FieldWeights(module).parameters()
     call = dict(module=module, rd=rd, x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world, rng_perturb=rng_perturb,
                 rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_rays=grad_rays,
                 grad_precision=grad_precision)

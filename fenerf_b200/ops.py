@@ -6,6 +6,7 @@ current CUDA stream to the library, wrap the outputs.  No arithmetic of the hot 
 Python or in torch ops.
 """
 import ctypes as C
+import functools
 import math
 import os
 
@@ -255,6 +256,21 @@ def composite(rd, raw_coarse, z_coarse, raw_fine=None, z_fine=None, rng_noise=No
 _WORKSPACES = {}
 
 
+def _aligned(ws):
+    """The first 256-byte aligned address in workspace `ws`."""
+    return (ws.data_ptr() + 255) // 256 * 256
+
+
+def _packed(module, rd):
+    """The kernel-layout weights a render of precision rd.precision reads."""
+    return module.packed(split=rd.precision == _lib.PRECISION['split'])
+
+
+def _stage_view(ws, base, offset, shape):
+    """fp32 view of shape `shape` at byte `offset` past `base` in a private render workspace."""
+    return ws[base + offset: base + offset + math.prod(shape) * 4].view(torch.float32).view(shape)
+
+
 def _workspace(device, nbytes):
     """One grow-only scratch buffer per (device, stream): the C-ABI never allocates."""
     key = (device, torch.cuda.current_stream(device).cuda_stream)
@@ -277,23 +293,32 @@ def guard_stats(device):
         return None
     rep = _lib.GuardReport()
     with torch.cuda.device(device):
-        _lib.check(_lib.lib().fenerf_guard_stats((ws.data_ptr() + 255) // 256 * 256, C.byref(rep), _stream(device)))
+        _lib.check(_lib.lib().fenerf_guard_stats(_aligned(ws), C.byref(rep), _stream(device)))
     return dict(refined=rep.refined, max_abs_delta=rep.max_abs_delta, sign_flips=rep.sign_flips, tau=rep.tau)
+
+
+def _forward_call(lib, rd, packed, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f, pixels,
+                  depth, wsum, weights, inds, ws_ptr, ws_bytes, device):
+    _lib.check(lib.fenerf_render_forward(
+        C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device),
+        _chk(x_lin, "x_lin", device), _chk(y_lin, "y_lin", device), _chk(z_lin, "z_lin", device),
+        _chk(cam2world, "cam2world", device), _chk(rng_perturb, "rng_perturb", device),
+        _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device), _chk(rng_noise_f, "rng_noise_f", device),
+        pixels.data_ptr(), depth.data_ptr() if depth is not None else 0, wsum.data_ptr() if wsum is not None else 0,
+        weights.data_ptr() if weights is not None else 0, inds.data_ptr() if inds is not None else 0, ws_ptr, ws_bytes,
+        _stream(device)))
 
 
 def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
                    want_depth=True, want_weights_sum=True, want_weights=False, want_inds=False):
     """One call into fenerf_render_forward: the whole render after the mapping network."""
-    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
+    packed = _packed(module, rd)
     device = packed.device
     lib = _lib.lib()
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
     ns = 2 * s if rd.hierarchical else s
     c = packed.desc.out_dim
-    film = _prep(film, device)
-    n_film = packed.desc.trunk_layers + packed.desc.color_layers + (1 if packed.desc.reserved & _lib.FIELD_LABEL_FILM else 0)
-    if film.shape != (b, n_film, 2, _lib.HIDDEN):
-        raise ValueError("film table has shape %s" % (tuple(film.shape),))
+    film = _film_for(packed, film, device, b)
     pixels = torch.empty((b, _image_channels(rd, c), rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     depth = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_depth else None
     wsum = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_weights_sum else None
@@ -302,48 +327,30 @@ def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb
     with torch.cuda.device(device):
         nbytes = lib.fenerf_workspace_bytes(C.byref(rd), C.byref(packed.desc))
         ws = _workspace(device, nbytes)
-        ws_ptr = (ws.data_ptr() + 255) // 256 * 256
-        _lib.check(lib.fenerf_render_forward(
-            C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device),
-            _chk(x_lin, "x_lin", device), _chk(y_lin, "y_lin", device), _chk(z_lin, "z_lin", device),
-            _chk(cam2world, "cam2world", device), _chk(rng_perturb, "rng_perturb", device),
-            _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device),
-            _chk(rng_noise_f, "rng_noise_f", device),
-            pixels.data_ptr(), depth.data_ptr() if depth is not None else 0,
-            wsum.data_ptr() if wsum is not None else 0, weights.data_ptr() if weights is not None else 0,
-            inds.data_ptr() if inds is not None else 0, ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()),
-            _stream(device)))
+        ws_ptr = _aligned(ws)
+        _forward_call(lib, rd, packed, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
+                      pixels, depth, wsum, weights, inds, ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()), device)
     return pixels, depth, wsum, weights, inds
 
 
 def render_forward_stages(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f):
     """fenerf_render_forward into a PRIVATE workspace, returned together with typed views of the intermediates
     it leaves there (fenerf_workspace_layout): what the backward consumes (fenerf_b200/backward.py)."""
-    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
+    packed = _packed(module, rd)
     device = packed.device
     lib = _lib.lib()
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
     c = packed.desc.out_dim
-    film = _prep(film, device)
+    film = _film_for(packed, film, device, b)
     pixels = torch.empty((b, c - 1, rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     off = _lib.WorkspaceOffsets()
     with torch.cuda.device(device):
         _lib.check(lib.fenerf_workspace_layout(C.byref(rd), C.byref(packed.desc), C.byref(off)))
         ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
-        base = (ws.data_ptr() + 255) // 256 * 256 - ws.data_ptr()
-        _lib.check(lib.fenerf_render_forward(
-            C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device),
-            _chk(x_lin, "x_lin", device), _chk(y_lin, "y_lin", device), _chk(z_lin, "z_lin", device),
-            _chk(cam2world, "cam2world", device), _chk(rng_perturb, "rng_perturb", device),
-            _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device), _chk(rng_noise_f, "rng_noise_f", device),
-            pixels.data_ptr(), 0, 0, 0, 0, ws.data_ptr() + base, ws.numel() - base, _stream(device)))
-
-    def view(offset, shape):
-        numel = 1
-        for d in shape:
-            numel *= d
-        return ws[base + offset: base + offset + numel * 4].view(torch.float32).view(shape)
-
+        base = _aligned(ws) - ws.data_ptr()
+        _forward_call(lib, rd, packed, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
+                      pixels, None, None, None, None, ws.data_ptr() + base, ws.numel() - base, device)
+    view = functools.partial(_stage_view, ws, base)
     st = dict(pixels=pixels, workspace=ws, points_c=view(off.points_coarse, (b, n, s, 3)), z_c=view(off.z_coarse, (b, n, s)),
               dirs=view(off.dirs, (b, n, 3)), raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None)
     if rd.hierarchical:
@@ -406,6 +413,7 @@ def _rays_call(lib, rd, packed, film, pts, dirs, dir_group, o, rdir, z, rng_nois
 
 
 def _film_for(packed, film, device, b):
+    """`film` on `device`, checked to be the (B, FiLM rows, 2, 256) table the pack reads."""
     packed_desc = packed.desc
     film = _prep(film, device)
     n_film = packed_desc.trunk_layers + packed_desc.color_layers + (1 if packed_desc.reserved & _lib.FIELD_LABEL_FILM else 0)
@@ -418,7 +426,7 @@ def render_rays(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_n
                 want_depth=False, want_weights_sum=False):
     """One call into fenerf_render_rays (rd from make_rays_desc): the render of caller-supplied rays.
     Returns (pixels (B, N, C-1) ray-major in [0, 1], depth (B, N, 1) or None, weights_sum (B, N, 1) or None)."""
-    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
+    packed = _packed(module, rd)
     device = packed.device
     lib = _lib.lib()
     b, n = rd.batch, rd.img_w
@@ -431,7 +439,7 @@ def render_rays(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_n
     with torch.cuda.device(device):
         nbytes = lib.fenerf_rays_workspace_bytes(C.byref(rd), C.byref(packed.desc), dir_group)
         ws = _workspace(device, nbytes)
-        ws_ptr = (ws.data_ptr() + 255) // 256 * 256
+        ws_ptr = _aligned(ws)
         _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, depth, wsum,
                    ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()), device)
     return pixels, depth, wsum
@@ -443,7 +451,7 @@ def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals
     (fenerf_rays_workspace_layout) and the laid-out inputs: what the backward consumes (fenerf_b200/backward.py).
     slots=True (a backward w.r.t. the directions): fenerf_render_rays_grad, which also leaves the fine samples' draw
     slots, 'slots_f' (B, N, S) uint8, where the fine pass reads per-sample directions (None elsewhere)."""
-    packed = module.packed(split=rd.precision == _lib.PRECISION['split'])
+    packed = _packed(module, rd)
     device = packed.device
     lib = _lib.lib()
     b, n, s = rd.batch, rd.img_w, rd.num_steps
@@ -460,16 +468,10 @@ def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals
         else:
             _lib.check(lib.fenerf_rays_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off)))
         ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
-        base = (ws.data_ptr() + 255) // 256 * 256 - ws.data_ptr()
+        base = _aligned(ws) - ws.data_ptr()
         _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, None, None,
                    ws.data_ptr() + base, ws.numel() - base, device, slots=slots)
-
-    def view(offset, shape):
-        numel = 1
-        for e in shape:
-            numel *= e
-        return ws[base + offset: base + offset + numel * 4].view(torch.float32).view(shape)
-
+    view = functools.partial(_stage_view, ws, base)
     st = dict(pixels=pixels, workspace=ws, points_c=pts, z_c=z, dirs=d, dir_group=dir_group,
               raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None, dirs_f=None, slots_f=None)
     if rd.hierarchical:
@@ -545,13 +547,17 @@ def gemm_nt_film(a16, w16, bias, film, b0, layer, ppb, narrow_in=None, narrow_w=
     return a_out, g_out
 
 
+def _tn_slices(dev, batch, ppb):
+    """Default split-K of the per-image X_b^T Y_b products: enough CTAs to fill the SMs, at least 64 rows per slice."""
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    return max(1, min((ppb + 63) // 64, (sms + batch - 1) // batch))
+
+
 def gemm_tn(x16, y16, batch, ppb, slices=None, colsum=False):
     """Per image b: X_b^T Y_b with X, Y (batch * ppb, 256) fp16 -> (batch, 256, 256) fp32 (fenerf_gemm_tn_f16; the
     split-K partials of the CTAs are summed here).  colsum=True also returns the column sums of X per image (batch, 256)."""
     dev = x16.device
-    if slices is None:
-        sms = torch.cuda.get_device_properties(dev).multi_processor_count
-        slices = max(1, min((ppb + 63) // 64, (sms + batch - 1) // batch))
+    slices = _tn_slices(dev, batch, ppb) if slices is None else slices
     partial = torch.empty((batch, slices, 256, 256), dtype=torch.float32, device=dev)
     cs = torch.empty((batch, slices, 256), dtype=torch.float32, device=dev) if colsum else None
     with torch.cuda.device(dev):
@@ -627,9 +633,7 @@ def gemm_tn_split(x32, y32, batch, ppb, x_amax=None, y_amax=None, slices=None):
     """Per image b: X_b^T Y_b with X, Y (batch * ppb, 256) fp32 -> (batch, 256, 256) fp32 (fenerf_gemm_tn_split; the
     split-K partials are summed here).  x_amax / y_amax: max |X| / |Y| as device scalars (None: at most 1)."""
     dev = x32.device
-    if slices is None:
-        sms = torch.cuda.get_device_properties(dev).multi_processor_count
-        slices = max(1, min((ppb + 63) // 64, (sms + batch - 1) // batch))
+    slices = _tn_slices(dev, batch, ppb) if slices is None else slices
     partial = torch.empty((batch, slices, 256, 256), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().fenerf_gemm_tn_split(_chk(x32, "X", dev), _chk(y32, "Y", dev), batch, ppb, slices,

@@ -13,6 +13,8 @@ implementation (an ulp of summation order flips them) and are excluded, with the
 """
 import copy
 import functools
+import gc
+import weakref
 
 import numpy as np
 import pytest
@@ -900,3 +902,31 @@ def test_neural_renderer_modules_run_on_the_unit_frame(runs):
     g = gen.siren.final_layer.weight.grad
     assert g is not None and torch.isfinite(g).all() and g.abs().sum() > 0
     assert up[1].weight.grad is not None and up[1].weight.grad.abs().sum() > 0
+
+
+@pytest.mark.parametrize("name,kw", [("a_small", {}), ("b_small", dict(precision="exact")),
+                                     ("b_small", dict(precision="split", grad_precision="split"))])
+def test_backward_state_is_freed_without_the_cycle_collector(name, kw, monkeypatch):
+    """The render backward's per-call state (_FieldBackward: the per-image accumulators, the stream's weight forms, the
+    grid accumulator) is in no reference cycle: reference counting frees it, and its device memory, as soon as
+    loss.backward() returns, so a training loop does not wait for Python's cycle collector to get that memory back."""
+    from fenerf_b200 import backward
+    case = _cases.CASE_BY_NAME[name]
+    gen = _cases.build_mirror(case, DEV)
+    zs = [torch.randn(case.batch, 256, device=DEV) for _ in range(_cases.n_latents(case.model))]
+    made = []
+    init = backward._FieldBackward.__init__
+
+    def spy(self, *args, **kwargs):
+        init(self, *args, **kwargs)
+        made.append(weakref.ref(self))
+
+    monkeypatch.setattr(backward._FieldBackward, "__init__", spy)
+    gc.collect()
+    gc.disable()
+    try:
+        px, _ = gen(*zs, **dict(case.cfg, **kw))
+        px.sum().backward()
+        assert len(made) == 1 and made[0]() is None
+    finally:
+        gc.enable()
