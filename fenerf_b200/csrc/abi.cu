@@ -227,8 +227,8 @@ int fenerf_resample(const fenerf_render_desc* rd, int32_t out_dim, const float* 
     FN_REQUIRE(raw_coarse && z_vals && dirs && origins && rng_u && z_fine && points_fine, "NULL argument");
     FN_REQUIRE(out_dim >= 2 && out_dim <= 129, "out_dim %d unsupported", out_dim);
     FN_REQUIRE(rd->noise_std == 0.f || rng_noise, "noise_std != 0 needs rng_noise");
-    return resample(rd, out_dim, raw_coarse, z_vals, dirs, origins, rd->noise_std != 0.f ? rng_noise : nullptr, rng_u,
-                    z_fine, points_fine, (long long*)inds, (cudaStream_t)stream);
+    return resample(rd, out_dim, raw_coarse, z_vals, dirs, origins, nullptr, rd->noise_std != 0.f ? rng_noise : nullptr, rng_u,
+                    nullptr, z_fine, points_fine, (cudaStream_t)stream, (long long*)inds);
 }
 
 int fenerf_composite(const fenerf_render_desc* rd, int32_t out_dim, const float* raw_coarse, const float* z_coarse,
@@ -346,8 +346,8 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
     }
     stage_mark(3, st);
     if (rd->hierarchical) {
-        if (int e = resample(rd, C, raw_c, z_c, dirs, origins, noise_c, rng_u, z_f, points_f, (long long*)inds_dbg, st,
-                             /*sort_fine=*/1, sigma_c)) return e;
+        if (int e = resample(rd, C, raw_c, z_c, dirs, origins, nullptr, noise_c, rng_u, sigma_c, z_f, points_f, st,
+                             (long long*)inds_dbg, /*sort_fine=*/1)) return e;
         stage_mark(4, st);
         if (int e = run_field(L, packed, points_f, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
                               rd->precision, raw_f, st)) return e;
@@ -438,11 +438,9 @@ int render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, co
     }
     if (rd->hierarchical) {
         const bool per_sample = dir_group == 1 && !rd->lock_view_dependence;
-        if (grad && per_sample) {
-            if (int e = resample_rays_slots(rd, C, raw_c, z_vals, ray_dirs, origins, noise_c, rng_u, z_f, points_f, dirs, dirs_f,
-                                            sigma_c, ws + w.fine_slots, st)) return e;
-        } else if (int e = resample_rays(rd, C, raw_c, z_vals, ray_dirs, origins, noise_c, rng_u, z_f, points_f,
-                                         per_sample ? dirs : nullptr, per_sample ? dirs_f : nullptr, sigma_c, st)) return e;
+        if (int e = resample(rd, C, raw_c, z_vals, ray_dirs, nullptr, origins, noise_c, rng_u, sigma_c, z_f, points_f, st,
+                             nullptr, 1, per_sample ? dirs : nullptr, per_sample ? dirs_f : nullptr,
+                             grad && per_sample ? ws + w.fine_slots : nullptr)) return e;
         if (int e = run_field(L, packed, points_f, per_sample ? dirs_f : dirs, film, rd->batch, ppb, dir_group,
                               rd->lock_view_dependence, rd->precision, raw_f, st)) return e;
     }

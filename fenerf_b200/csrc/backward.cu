@@ -320,11 +320,7 @@ int grid_scatter_add(const FnLayout& L, const float* points, const void* d_feat,
 int grid_unpack_grad(const FnLayout& L, const float* grad_cl, float* out, const float* inv_scale, cudaStream_t st) {
     const int R = L.grid_res, G = L.grid_channels;
     const size_t smem = (size_t)G * (R + 1) * sizeof(float);
-    static std::atomic<int> smem_set[kMaxDevices];
-    if (smem > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(grid_unpack_grad_kernel, smem_set, (int)smem));
-    grid_unpack_grad_kernel<<<R * R, 256, smem, st>>>(grad_cl, out, R, G, inv_scale);
-    FN_LAUNCH_OK("grid_unpack_grad_kernel");
-    return 0;
+    return launch<grid_unpack_grad_kernel>("grid_unpack_grad_kernel", R * R, 256, smem, st, grad_cl, out, R, G, inv_scale);
 }
 
 }  // namespace fn

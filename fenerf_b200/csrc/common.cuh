@@ -68,15 +68,23 @@ inline int num_sms() {
     return n;
 }
 
-// cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): remember the largest value set on each
-// device (`state` is one array per kernel instantiation) and raise it when a launch needs more.
-template <typename F>
-inline cudaError_t ensure_dynamic_smem(F kernel, std::atomic<int>* state /*[kMaxDevices]*/, int bytes) {
-    const int dev = current_device();
-    if (state[dev].load(std::memory_order_acquire) >= bytes) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess) state[dev].store(bytes, std::memory_order_release);
-    return e;
+// Kernel<<<grid, block, smem, st>>>(args...), counted.  Above the default 48 KB of dynamic shared memory a kernel has to
+// opt in, and cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): the state is one array per kernel --
+// keyed on the kernel itself, not its signature, which kernels share -- holding the largest value set on each device,
+// raised when a launch needs more.
+template <auto Kernel, typename... Args>
+inline int launch(const char* name, dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args&... args) {
+    if (smem > 48 * 1024) {
+        static std::atomic<int> opted_in[kMaxDevices];
+        std::atomic<int>& state = opted_in[current_device()];
+        if (state.load(std::memory_order_acquire) < (int)smem) {
+            FN_CUDA_OK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            state.store((int)smem, std::memory_order_release);
+        }
+    }
+    Kernel<<<grid, block, smem, st>>>(args...);
+    FN_LAUNCH_OK(name);
+    return 0;
 }
 
 // ---- the per-sample terms of fancy_integration (volumetric_rendering.py:18-38): compositors and resampler ----
@@ -133,21 +141,15 @@ int camera_poses(int n, int mode, float h_std, float v_std, float h_mean, float 
 int ray_setup(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
               const float* cam2world, const float* rng_perturb, float* points, float* z_vals, float* dirs,
               float* origins, cudaStream_t st);
-int resample(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* dirs,
-             const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
-             long long* inds, cudaStream_t st, int sort_fine = 0, const float* sigma_compact = nullptr);
-// fenerf_render_rays' resampler (resample_rays.cu): per-ray origins (B, N, 3); the fine samples depth-sorted.  With
-// dirs_sample (B, N, S, 3) (per-sample directions), fine sample k of sample_pdf's order takes direction slot k and
-// dirs_fine (B, N, S, 3) receives those directions in the sorted order
-int resample_rays(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* ray_dirs,
-                  const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
-                  const float* dirs_sample, float* dirs_fine, const float* sigma_compact, cudaStream_t st);
-// resample_rays with per-sample directions that also writes fine_slots (B, N, S) uint8, each fine sample's draw slot k in
-// the sorted order (resample_rays_slots.cu; fenerf_render_rays_grad)
-int resample_rays_slots(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* ray_dirs,
-                        const float* origins, const float* noise, const float* u, float* z_fine, float* pts_fine,
-                        const float* dirs_sample, float* dirs_fine, const float* sigma_compact, unsigned char* fine_slots,
-                        cudaStream_t st);
+// The resampler.  origins: one per image (B, 3), the camera render's (fenerf_resample, fenerf_render_forward: inds,
+// sort_fine) -- or ray_origins: one per ray (B, N, 3), the rays-in render's (fenerf_render_rays), whose fine samples are
+// always depth-sorted.  Rays-in with dirs_sample (B, N, S, 3) (per-sample directions), fine sample k of sample_pdf's
+// order takes direction slot k and dirs_fine (B, N, S, 3) receives those directions in the sorted order; fine_slots
+// (B, N, S) uint8, if given, each fine sample's draw slot k in the sorted order (fenerf_render_rays_grad)
+int resample(const fenerf_render_desc* rd, int C, const float* raw, const float* z, const float* dirs, const float* origins,
+             const float* ray_origins, const float* noise, const float* u, const float* sigma_compact, float* z_fine,
+             float* pts_fine, cudaStream_t st, long long* inds = nullptr, int sort_fine = 0,
+             const float* dirs_sample = nullptr, float* dirs_fine = nullptr, unsigned char* fine_slots = nullptr);
 int composite_sorted(const fenerf_render_desc* rd, int C, const float* raw_c, const float* z_c, const float* raw_f,
                      const float* z_f, const float* noise, float* pixels, float* depth, float* wsum, float* weights,
                      cudaStream_t st);

@@ -264,24 +264,16 @@ int gemm_nt(const void* A, const void* B, long long M, float* c32, void* c16, vo
     a.gate_out = (__half*)gate_out; a.gate_mul = (const __half*)gate_mul; a.A2 = (const __half*)A2; a.B2 = (const __half*)B2;
     a.bias = bias; a.film = film; a.film_stride = film_stride; a.ppb = ppb > 0 ? ppb : 1; a.M = M;
     if (M <= 0) return 0;
-    static std::atomic<int> set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(gemm_nt_kernel, set, (int)NT_SMEM));
     const long long tiles = (M + 127) / 128;
     const int blocks = (int)(tiles < (long long)num_sms() ? tiles : (long long)num_sms());
-    gemm_nt_kernel<<<blocks, kThreads, NT_SMEM, st>>>(a);
-    FN_LAUNCH_OK("gemm_nt_kernel");
-    return 0;
+    return launch<gemm_nt_kernel>("gemm_nt_kernel", blocks, kThreads, NT_SMEM, st, a);
 }
 
 int gemm_tn(const void* X, const void* Y, int batch, long long ppb, int slices, float* partial, cudaStream_t st, float* colsum) {
     static_assert(TN_SMEM <= 232448, "gemm_tn shared memory");
     TnArgs a;
     a.X = (const __half*)X; a.Y = (const __half*)Y; a.partial = partial; a.colsum = colsum; a.ppb = ppb; a.slices = slices;
-    static std::atomic<int> set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(gemm_tn_kernel, set, (int)TN_SMEM));
-    gemm_tn_kernel<<<dim3(slices, batch, 2), kThreads, TN_SMEM, st>>>(a);
-    FN_LAUNCH_OK("gemm_tn_kernel");
-    return 0;
+    return launch<gemm_tn_kernel>("gemm_tn_kernel", dim3(slices, batch, 2), kThreads, TN_SMEM, st, a);
 }
 
 }  // namespace fn

@@ -330,14 +330,10 @@ int gemm_nt_split(const float* A, const void* B_hi, const void* B_lo, long long 
     a.a_out = a_out; a.gate_out = gate_out; a.bias = bias; a.film = film; a.film_stride = film_stride;
     a.ppb = ppb > 0 ? ppb : 1; a.M = M;
     if (M <= 0) return 0;
-    static std::atomic<int> set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(split_nt_kernel, set, (int)SNT_SMEM));
     const long long tiles = (M + 127) / 128;
     const int half = num_sms() / 2;
     const int blocks = (int)(tiles < (long long)half ? tiles : (long long)half);
-    split_nt_kernel<<<dim3(blocks, 2), kThreads, SNT_SMEM, st>>>(a);
-    FN_LAUNCH_OK("split_nt_kernel");
-    return 0;
+    return launch<split_nt_kernel>("split_nt_kernel", dim3(blocks, 2), kThreads, SNT_SMEM, st, a);
 }
 
 int gemm_tn_split(const float* X, const float* Y, int batch, long long ppb, int slices, const float* x_amax, const float* y_amax,
@@ -345,11 +341,7 @@ int gemm_tn_split(const float* X, const float* Y, int batch, long long ppb, int 
     static_assert(STN_SMEM <= 232448, "split_tn shared memory");
     SplitTnArgs a;
     a.X = X; a.Y = Y; a.x_amax = x_amax; a.y_amax = y_amax; a.partial = partial; a.ppb = ppb; a.slices = slices;
-    static std::atomic<int> set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(split_tn_kernel, set, (int)STN_SMEM));
-    split_tn_kernel<<<dim3(slices, batch, 2), kThreads, STN_SMEM, st>>>(a);
-    FN_LAUNCH_OK("split_tn_kernel");
-    return 0;
+    return launch<split_tn_kernel>("split_tn_kernel", dim3(slices, batch, 2), kThreads, STN_SMEM, st, a);
 }
 
 int absmax_f32(const float* x, long long n, float* amax, cudaStream_t st) {

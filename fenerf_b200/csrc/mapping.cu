@@ -155,10 +155,7 @@ int mapping_film(const float* const* w, const float* const* b, const float* z, i
         for (int i = 0; i < 4; ++i) { ha.w[i] = w[i]; ha.b[i] = b[i]; }
         ha.z = z + (size_t)b0 * z_dim; ha.h_out = h_scratch; ha.B = nb; ha.z_dim = z_dim;
         const size_t smem_h = (size_t)2 * nb * 512 * sizeof(float);
-        static std::atomic<int> set_h[kMaxDevices];
-        if (smem_h > 48 * 1024) FN_CUDA_OK(ensure_dynamic_smem(mapping_hidden_kernel, set_h, (int)smem_h));
-        mapping_hidden_kernel<<<1, 256, smem_h, st>>>(ha);
-        FN_LAUNCH_OK("mapping_hidden_kernel");
+        if (int e = launch<mapping_hidden_kernel>("mapping_hidden_kernel", 1, 256, smem_h, st, ha)) return e;
         OutArgs oa;
         oa.w = w[4]; oa.b = b[4]; oa.h = h_scratch; oa.avg_f = avg_f; oa.avg_p = avg_p;
         oa.film = film + (size_t)b0 * n_film_total * 512; oa.B = nb; oa.n_layers = n_layers; oa.layer0 = layer0;

@@ -4,7 +4,8 @@
 namespace fn {
 
 // the label FiLM instantiation (siren_fast_label.cu) and the feature-head ones (siren_fast_hd.cu); `args` is this file's
-// FastArgs
+// FastArgs (a type of the header's anonymous namespace, so each translation unit has its own and a typed declaration
+// would not link)
 int siren_fast_label_launch(const void* args, int blocks, cudaStream_t st);
 int siren_fast_hd_launch(const void* args, int blocks, bool label_film, cudaStream_t st);
 // the grid-trunk instantiation (siren_fast_grid.cu), the density alone included
@@ -93,7 +94,6 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     if (a.n_tiles <= 0) return 0;
     FN_REQUIRE(ppb % a.dir_group == 0, "points_per_batch %lld not a multiple of dir_group %d", ppb, a.dir_group);
     const long long n_pairs = (a.n_tiles + 1) / 2;
-    static std::atomic<int> attr_set[kMaxDevices];
     const int blocks = (int)(n_pairs < (long long)num_sms() ? n_pairs : (long long)num_sms());
     if (const int variant = g_variant.load()) {
         FN_REQUIRE(!L.grid_trunk && !L.bridge,
@@ -106,10 +106,7 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     if (L.bridge) return siren_fast_bridge_launch(&a, blocks, st);
     if (feature_head) return siren_fast_hd_launch(&a, blocks, label_film, st);
     if (label_film) return siren_fast_label_launch(&a, blocks, st);
-    FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<false>, attr_set, (int)SMEM_TOTAL));
-    siren_fast_kernel<false><<<blocks, NTHREADS, SMEM_TOTAL, st>>>(a);
-    FN_LAUNCH_OK("siren_fast_kernel");
-    return 0;
+    return launch<siren_fast_kernel<false>>("siren_fast_kernel", blocks, NTHREADS, SMEM_TOTAL, st, a);
 }
 
 }  // namespace fn

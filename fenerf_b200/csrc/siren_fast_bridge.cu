@@ -8,12 +8,8 @@ namespace fn {
 
 int siren_fast_bridge_launch(const void* args, int blocks, cudaStream_t st) {
     const FastArgs& a = *static_cast<const FastArgs*>(args);
-    constexpr auto kernel = siren_fast_kernel<false, false, kSoftSinEvery, false, false, true>;
-    static std::atomic<int> attr_set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(kernel, attr_set, (int)SMEM_TOTAL));
-    kernel<<<blocks, NTHREADS, SMEM_TOTAL, st>>>(a);
-    FN_LAUNCH_OK("siren_fast_kernel<bridge>");
-    return 0;
+    return launch<siren_fast_kernel<false, false, kSoftSinEvery, false, false, true>>("siren_fast_kernel<bridge>", blocks,
+                                                                                    NTHREADS, SMEM_TOTAL, st, a);
 }
 
 }  // namespace fn

@@ -11,12 +11,9 @@ namespace fn {
 namespace {
 
 template <bool kLabelFilm, bool kFeatureHead, int kSoftSin, bool kTrace>
-int launch(const FastArgs& a, int blocks, cudaStream_t st) {
-    static std::atomic<int> attr_set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace>, attr_set, (int)SMEM_TOTAL));
-    siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace><<<blocks, NTHREADS, SMEM_TOTAL, st>>>(a);
-    FN_LAUNCH_OK("siren_fast_kernel<debug>");
-    return 0;
+int debug_launch(const FastArgs& a, int blocks, cudaStream_t st) {
+    return launch<siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace>>("siren_fast_kernel<debug>", blocks, NTHREADS,
+                                                                                SMEM_TOTAL, st, a);
 }
 
 __global__ void soft_sine_kernel(const float* a, float* out, long long n) {
@@ -29,12 +26,12 @@ __global__ void soft_sine_kernel(const float* a, float* out, long long n) {
 int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st) {
     const FastArgs& a = *static_cast<const FastArgs*>(args);
     if (variant == 1) {
-        if (feature_head) return label_film ? launch<true, true, kSoftSinSplit, false>(a, blocks, st) : launch<false, true, kSoftSinSplit, false>(a, blocks, st);
-        return label_film ? launch<true, false, kSoftSinSplit, false>(a, blocks, st) : launch<false, false, kSoftSinSplit, false>(a, blocks, st);
+        if (feature_head) return label_film ? debug_launch<true, true, kSoftSinSplit, false>(a, blocks, st) : debug_launch<false, true, kSoftSinSplit, false>(a, blocks, st);
+        return label_film ? debug_launch<true, false, kSoftSinSplit, false>(a, blocks, st) : debug_launch<false, false, kSoftSinSplit, false>(a, blocks, st);
     }
     FN_REQUIRE(!label_film && !feature_head, "the point-network timeline covers plain fields only");
-    if (variant == 2) return launch<false, false, kSoftSinEvery, true>(a, blocks, st);
-    return launch<false, false, kSoftSinSplit, true>(a, blocks, st);
+    if (variant == 2) return debug_launch<false, false, kSoftSinEvery, true>(a, blocks, st);
+    return debug_launch<false, false, kSoftSinSplit, true>(a, blocks, st);
 }
 
 int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st) {

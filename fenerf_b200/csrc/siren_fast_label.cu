@@ -7,11 +7,7 @@ namespace fn {
 
 int siren_fast_label_launch(const void* args, int blocks, cudaStream_t st) {
     const FastArgs& a = *static_cast<const FastArgs*>(args);
-    static std::atomic<int> attr_set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(siren_fast_kernel<true>, attr_set, (int)SMEM_TOTAL));
-    siren_fast_kernel<true><<<blocks, NTHREADS, SMEM_TOTAL, st>>>(a);
-    FN_LAUNCH_OK("siren_fast_kernel<label FiLM>");
-    return 0;
+    return launch<siren_fast_kernel<true>>("siren_fast_kernel<label FiLM>", blocks, NTHREADS, SMEM_TOTAL, st, a);
 }
 
 }  // namespace fn

@@ -66,12 +66,8 @@ int siren_points_split(const FnLayout& L, const unsigned char* packed, const flo
     FN_REQUIRE(ppb % a.dir_group == 0, "points_per_batch %lld not a multiple of dir_group %d", ppb, a.dir_group);
     const long long n_pairs = (a.n_tiles + 1) / 2;
     const int blocks = (int)(n_pairs < (long long)num_sms() ? n_pairs : (long long)num_sms());
-    constexpr auto kernel = siren_fast_kernel<false, false, 0, false, false, false, true>;
-    static std::atomic<int> attr_set[kMaxDevices];
-    FN_CUDA_OK(ensure_dynamic_smem(kernel, attr_set, (int)SMEM_TOTAL_SPLIT));
-    kernel<<<blocks, NTHREADS, SMEM_TOTAL_SPLIT, st>>>(a);
-    FN_LAUNCH_OK("siren_fast_kernel<split>");
-    return 0;
+    return launch<siren_fast_kernel<false, false, 0, false, false, false, true>>("siren_fast_kernel<split>", blocks, NTHREADS,
+                                                                               SMEM_TOTAL_SPLIT, st, a);
 }
 
 }  // namespace fn
