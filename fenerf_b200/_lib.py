@@ -44,6 +44,7 @@ EXPORTS = (
     "fenerf_grid_scatter_add_det", "fenerf_det_launch_count",
     "fenerf_render_rays_grad", "fenerf_rays_grad_workspace_layout", "fenerf_composite_backward_rays_dz",
     "fenerf_grid_coord_grad", "fenerf_ray_dir_grad",
+    "fenerf_mc_workspace_bytes", "fenerf_mc_count", "fenerf_mc_emit",
 )
 
 
@@ -194,6 +195,12 @@ def _declare(lib):
     lib.fenerf_mask2color.argtypes = [vp, i32, i32, i64, vp, vp]
     lib.fenerf_frames_to_u8.restype = C.c_int
     lib.fenerf_frames_to_u8.argtypes = [vp, i32, i32, i32, i32, i64, vp, vp]
+    lib.fenerf_mc_workspace_bytes.restype = sz
+    lib.fenerf_mc_workspace_bytes.argtypes = [i32]
+    lib.fenerf_mc_count.restype = C.c_int
+    lib.fenerf_mc_count.argtypes = [vp, i32, C.c_float, vp, sz, vp, vp]
+    lib.fenerf_mc_emit.restype = C.c_int
+    lib.fenerf_mc_emit.argtypes = [vp, i32, C.c_float, P(C.c_float), C.c_float, vp, sz, i64, i64, vp, vp, vp]
     lib.fenerf_last_error.restype = C.c_char_p
     lib.fenerf_last_error.argtypes = []
     lib.fenerf_abi_version.restype = i32

@@ -640,3 +640,55 @@ def gemm_tn_split(x32, y32, batch, ppb, x_amax=None, y_amax=None, slices=None):
                                                    _chk(x_amax, "x_amax", dev), _chk(y_amax, "y_amax", dev),
                                                    partial.data_ptr(), _stream(dev)))
     return partial.sum(1) if slices > 1 else partial[:, 0]
+
+
+# --------------------------------------------------------------------------------------------
+# marching cubes over a density grid (csrc/mesh.cu)
+# --------------------------------------------------------------------------------------------
+def _mc_grid(sigma, level):
+    """Checks a (N, N, N) fp32 CUDA grid and a finite level -> (N, level as a float)."""
+    if sigma.dim() != 3 or not (sigma.shape[0] == sigma.shape[1] == sigma.shape[2]):
+        raise ValueError("sigma must be an (N, N, N) grid, got %s" % (tuple(sigma.shape),))
+    _chk(sigma, "sigma")
+    level = float(level)
+    if not math.isfinite(level):
+        raise ValueError("level must be finite, got %r" % level)
+    return sigma.shape[0], level
+
+
+def mc_count(sigma, level):
+    """fenerf_mc_count: classify the grid's cells and scan the counts -> (workspace, counts (2,) int64 [V, F] on the
+    device).  No host sync; mc_emit reads the workspace."""
+    n, level = _mc_grid(sigma, level)
+    device = sigma.device
+    with torch.cuda.device(device):
+        nbytes = _lib.lib().fenerf_mc_workspace_bytes(n)
+        if nbytes == 0:
+            _lib.check(_lib.lib().fenerf_mc_count(sigma.data_ptr(), n, level, 0, 0, 0, _stream(device)))
+        ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=device)
+        counts = torch.empty(2, dtype=torch.int64, device=device)
+        _lib.check(_lib.lib().fenerf_mc_count(sigma.data_ptr(), n, level, _aligned(ws), nbytes, counts.data_ptr(),
+                                              _stream(device)))
+    return ws, counts
+
+
+def mc_emit(sigma, level, origin, voxel_size, ws, n_vertices, n_triangles):
+    """fenerf_mc_emit into new tensors -> (vertices (V, 3) fp32, faces (F, 3) int32)."""
+    n, level = _mc_grid(sigma, level)
+    device = sigma.device
+    verts = torch.empty((n_vertices, 3), dtype=torch.float32, device=device)
+    faces = torch.empty((n_triangles, 3), dtype=torch.int32, device=device)
+    org = (C.c_float * 3)(*[float(o) for o in origin])
+    with torch.cuda.device(device):
+        _lib.check(_lib.lib().fenerf_mc_emit(
+            sigma.data_ptr(), n, level, org, float(voxel_size), _aligned(ws), ws.numel() - (_aligned(ws) - ws.data_ptr()),
+            n_vertices, n_triangles, verts.data_ptr(), faces.data_ptr(), _stream(device)))
+    return verts, faces
+
+
+def marching_cubes(sigma, level, origin, voxel_size):
+    """The mesh of the (N, N, N) fp32 grid `sigma` at `level` (inside: sigma >= level) -> (vertices (V, 3) fp32, faces
+    (F, 3) int32), grid point (i, j, k) at origin + (i, j, k) voxel_size.  Reads the two counts back (one host sync)."""
+    ws, counts = mc_count(sigma, level)
+    n_vertices, n_triangles = (int(c) for c in counts.tolist())
+    return mc_emit(sigma, level, origin, voxel_size, ws, n_vertices, n_triangles)

@@ -605,6 +605,32 @@ int fenerf_grid_scatter_add_det(const fenerf_field_desc* field, const float* poi
                                 int32_t dtype, void* stream);
 int64_t fenerf_det_launch_count(void);
 
+/* ---- marching cubes over a density grid ------------------------------------------------------------
+ * The mesh of the shape scripts' density grid (extract_double_semantic_shapes.py writes the 256^3 grid of sigma to an
+ * .mrc file and meshes it on the CPU), on the device.
+ *   sigma      (N, N, N) fp32, the scripts' index order: grid point (i, j, k) at i N^2 + j N + k, k fastest; 2 <= N,
+ *              N^3 + 1 <= 2^31 - 1.  A point is inside when sigma >= level (NaN is outside); level must be finite
+ *   workspace  fenerf_mc_workspace_bytes(N) bytes, 256-byte aligned (0: N out of range); fenerf_mc_count fills it and
+ *              fenerf_mc_emit reads it, so the two share it with the same sigma, N and level
+ *   counts     (2,) int64, device: the vertex count V, then the triangle count F.  Reading them back is the one host
+ *              sync of an extraction: the caller sizes the outputs from them
+ *   origin     host, 3 floats: the position of grid point (0, 0, 0); point (i, j, k) is at origin + (i, j, k) voxel_size,
+ *              each coordinate rounded as a product, then a sum
+ *   vertices   (V, 3) fp32: one vertex per grid edge sigma crosses level on, at a + t (b - a), t = (level - sigma_a) /
+ *              (sigma_b - sigma_a), a the lower-index end (t = 0.5 when an end is NaN or infinite).  Ordered by the
+ *              edge's lower end (linear index), then its axis 0, 1, 2
+ *   faces      (F, 3) int32 vertex indices; normals (b - a) x (c - a) point from inside to outside (towards lower
+ *              sigma).  Ordered by cell (linear index of its lowest corner), then the case table's order.  Cells that
+ *              share a face cut it the same way, so the mesh is closed away from the grid's boundary
+ * n_vertices / n_triangles are the counts fenerf_mc_count wrote; more than 2^31 - 1 of either is refused (the indices
+ * are int32).  Every pointer but origin must be device memory (FENERF_E_ARG otherwise). */
+size_t fenerf_mc_workspace_bytes(int32_t n);
+int fenerf_mc_count(const float* sigma, int32_t n, float level, void* workspace, size_t workspace_bytes, int64_t* counts,
+                    void* stream);
+int fenerf_mc_emit(const float* sigma, int32_t n, float level, const float* origin /* host, 3 */, float voxel_size,
+                   const void* workspace, size_t workspace_bytes, int64_t n_vertices, int64_t n_triangles, float* vertices,
+                   int32_t* faces, void* stream);
+
 /* Per-thread message for the last non-zero return. */
 const char* fenerf_last_error(void);
 
