@@ -785,6 +785,8 @@ class RenderFunction(torch.autograd.Function):
                 fb.add_points(pick(st['points_f'], 3), dirs, s, lock, pick(st['raw_f'], c), pick(d_raw_f, c))
             fb.add_points(pick(st['points_c'], 3), dirs, s, lock, pick(st['raw_c'], c), pick(d_raw_c, c))
             d_film, grads = fb.finish()
+            if call.get('grad_reduce') is not None:
+                call['grad_reduce']([d_film] + list(grads.values()))
         return tuple(_input_grads(ctx, d_film, grads))
 
 
@@ -918,14 +920,16 @@ def render_rays_with_grad(module, rd, film, points, dirs, origins, ray_dirs, z_v
 
 
 def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
-                     grad_rays=None, grad_precision=None):
+                     grad_rays=None, grad_precision=None, grad_reduce=None):
     """Differentiable render: (B, C-1, R, R) pixels with autograd edges to `film` and the field parameters.
     `grad_rays`: optional int64 ray indices -- only these rays carry the gradient (part_forward).
     `grad_precision`: None (the backward of the forward precision) or 'split' (fp32 streams, the 256-wide products on the
-    split kernels of csrc/gemm_split.cu; forward precision 'split' or 'exact', the fields the split forward serves)."""
+    split kernels of csrc/gemm_split.cu; forward precision 'split' or 'exact', the fields the split forward serves).
+    `grad_reduce`: optional callable given [d film, every parameter gradient] before they leave the backward; it may
+    modify them in place (a ray-sharded render sums them over its ranks there, dist.RayShard.reduce)."""
     check_grad_precision(module, grad_precision, rd.precision)
     params = FieldWeights(module).parameters()
     call = dict(module=module, rd=rd, x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world, rng_perturb=rng_perturb,
                 rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_rays=grad_rays,
-                grad_precision=grad_precision)
+                grad_precision=grad_precision, grad_reduce=grad_reduce)
     return RenderFunction.apply(film, call, *params)

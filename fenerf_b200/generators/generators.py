@@ -15,6 +15,8 @@ Hidden keyword extras (never passed by the reference's callers, used by tests an
   grad_precision  None | 'split': the backward of a differentiable 'exact' / 'split' render on the split kernels
               (backward.render_with_grad); ignored without autograd
   _debug      dict that receives intermediate tensors (inds, depth, weights_sum, poses)
+  _ray_shard  a dist.RayShard: render only its pixel rows of every image and return what its gather makes of them
+              (dist.render_sharded_rays)
 """
 import warnings
 
@@ -74,6 +76,16 @@ class _RenderSkeleton:
                     rng_noise_f[:, idx] = rng.randn(batch_size, idx.numel(), n_samples, 1)
                 if hierarchical_sample:
                     rng_u = rng_u.reshape(batch_size * n_rays, num_steps)
+            shard = kwargs.get('_ray_shard')
+            if shard is not None:
+                # a window of whole pixel rows is itself a camera image, rows x img_size, whose y table is a slice of the
+                # full one: the full draws are taken above, so the RNG stream stays the unsharded render's
+                if grad_rays is not None:
+                    raise ValueError("fenerf_b200: a ray-sharded render does not take grad_points")
+                r0, r1 = shard.rows(img_size)
+                y_lin = y_lin[r0:r1]
+                rng_perturb, rng_noise_c, rng_u, rng_noise_f = vr.window_draws(
+                    batch_size, n_rays, r0 * img_size, r1 * img_size, rng_perturb, rng_noise_c, rng_u, rng_noise_f)
             rd = ops.make_render_desc(
                 batch=batch_size, img_size=img_size, num_steps=num_steps, hierarchical=hierarchical_sample,
                 clamp_mode=clamp_mode, nerf_noise=noise_std, fov=fov, last_back=kwargs.get('last_back', False),
@@ -82,6 +94,8 @@ class _RenderSkeleton:
                 fill_color=kwargs.get('fill_color', 'black'), softmax_label=self.softmax_label,
                 lock_view_dependence=lock_view_dependence, precision=kwargs.get('precision'),
                 guard_tau=kwargs.get('guard_tau', getattr(self.siren, '_guard_tau', 0.0)))
+            if shard is not None:
+                rd.img_h = r1 - r0
             debug = kwargs.get('_debug')
             fill_mode = kwargs.get('fill_mode', None) if staged else None
             wants_per_sample_weights = staged and fill_mode in (None, 'debug', 'seg_padding_background')
@@ -97,6 +111,8 @@ class _RenderSkeleton:
                     # reference's random initialisation; if the measured error eats more than a third of it, widen it (it
                     # sticks to this field for later calls) and render this call again.
                     rep = ops.guard_stats(device)
+                    if rep is not None and shard is not None:
+                        rep = shard.guard_report(rep, device)    # every rank decides on the whole image's measurement
                     if rep is not None and rep['refined'] > 0 and rep['max_abs_delta'] > rep['tau'] / 3:
                         new_tau = max(4.0 * rep['max_abs_delta'], rep['tau'])
                         warnings.warn("fenerf_b200: fp16 density error %.3g is within 3x of guard_tau %.3g on these weights; "
@@ -114,8 +130,15 @@ class _RenderSkeleton:
             from .. import backward
             pixels = backward.render_with_grad(self.siren, rd, film, x_lin, y_lin, z_lin, cam2world,
                                                rng_perturb.contiguous(), rng_noise_c, rng_u, rng_noise_f, grad_rays=grad_rays,
-                                               grad_precision=kwargs.get('grad_precision'))
+                                               grad_precision=kwargs.get('grad_precision'),
+                                               grad_reduce=shard.reduce if shard is not None else None)
             depth = wsum = weights = None
+        if shard is not None:
+            # pixels (B, C, rows, R) gather along their rows; depth, weights_sum and weights (B, rows * R, ...) along rays
+            pixels = shard.gather(pixels, 2, img_size)
+            with torch.no_grad():
+                depth, wsum, weights = (None if t is None else shard.gather(t, 1, img_size, ray_major=True)
+                                        for t in (depth, wsum, weights))
         return pixels, depth, wsum, weights, pitch, yaw
 
     def _finish_pixels(self, pixels):

@@ -73,6 +73,16 @@ class ReplayRng:
         return t.to(self.device)
 
 
+def window_draws(batch, n_rays, p0, p1, perturb, noise_c, u, noise_f):
+    """Rays [p0, p1) of every image of a camera render's per-ray draws: #1 perturb (B,N,S,1), #4 noise_c (B,N,S,1),
+    #5 u (B*N,S), #6 noise_f (B,N,S',1) -> the same layouts over p1 - p0 rays per image, contiguous (None stays None).
+    A ray-sharded render draws the whole tensors, in the reference's order, and renders with its window of them."""
+    def win(t):
+        return None if t is None else t[:, p0:p1].contiguous()
+    u = None if u is None else win(u.reshape(batch, n_rays, -1)).reshape(-1, u.shape[-1])
+    return win(perturb), win(noise_c), u, win(noise_f)
+
+
 # --------------------------------------------------------------------------------------------
 # tables
 # --------------------------------------------------------------------------------------------
