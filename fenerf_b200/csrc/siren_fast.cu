@@ -7,14 +7,15 @@ namespace fn {
 // FastArgs (a type of the header's anonymous namespace, so each translation unit has its own and a typed declaration
 // would not link)
 int siren_fast_label_launch(const void* args, int blocks, cudaStream_t st);
-int siren_fast_hd_launch(const void* args, int blocks, bool label_film, cudaStream_t st);
+// (the feature-head ones size their grids themselves: the one without the label FiLM branch runs WG_PLAIN warpgroups)
+int siren_fast_hd_launch(const void* args, bool label_film, cudaStream_t st);
 // the grid-trunk instantiation (siren_fast_grid.cu), the density alone included
 int siren_fast_grid_launch(const void* args, int blocks, cudaStream_t st);
 // the bridge instantiation (siren_fast_bridge.cu), the density alone included
 int siren_fast_bridge_launch(const void* args, int blocks, cudaStream_t st);
 // the debug instantiations (siren_fast_debug.cu): variant 1 = one column pair in four on the software sine, 2 / 3 = the
-// timeline of the production / the variant-1 kernel
-int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st);
+// timeline of the production / the variant-1 kernel; each sizes its grid for its own number of consumer warpgroups
+int siren_fast_debug_launch(const void* args, bool label_film, bool feature_head, int variant, cudaStream_t st);
 
 namespace {
 
@@ -66,7 +67,7 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
                       int batch, long long ppb, int dir_group, int lock_dirs, float* out, int sigma_only, cudaStream_t st,
                       float* sigma_out) {
     static_assert(sizeof(FastArgs) <= 4000, "kernel parameter block too large");
-    static_assert(SMEM_TOTAL <= 232448, "one CTA per SM: 227 KB of shared memory");
+    static_assert(SMEM_TOTAL <= 232448 && SMEM3_TOTAL <= 232448, "one CTA per SM: 227 KB of shared memory");
     static_assert(FN_HEAD_IMG_BYTES(FN_FEAT) == SLOT_BYTES, "a feature-head image is one ring slot");
     // a feature-head field's density alone runs the plain instantiation: it stops after the trunk head, whose sigma row
     // is 0 (layout.h)
@@ -93,20 +94,26 @@ int siren_points_fast(const FnLayout& L, const unsigned char* packed, const floa
     a.dir_group = dir_group < 1 ? 1 : dir_group; a.lock_dirs = lock_dirs;
     if (a.n_tiles <= 0) return 0;
     FN_REQUIRE(ppb % a.dir_group == 0, "points_per_batch %lld not a multiple of dir_group %d", ppb, a.dir_group);
-    const long long n_pairs = (a.n_tiles + 1) / 2;
-    const int blocks = (int)(n_pairs < (long long)num_sms() ? n_pairs : (long long)num_sms());
+    // the plain and the feature-head instantiations without the label FiLM branch, and their debug variants, run WG_PLAIN
+    // consumer warpgroups with 32-bit tile and point indices
+    if (!L.grid_trunk && !L.bridge && !label_film)
+        FN_REQUIRE(a.n_tiles < (1ll << 31) - WG_PLAIN && ppb < (1ll << 31) - TILE,
+                   "the fast point network indexes tiles and points in 32 bits: %lld tiles of 64 points over the batch "
+                   "(at most 2^31 - %d), %lld points per image (at most 2^31 - %d)", a.n_tiles, WG_PLAIN + 1, ppb, TILE + 1);
     if (const int variant = g_variant.load()) {
         FN_REQUIRE(!L.grid_trunk && !L.bridge,
                    "the debug point-network variants do not cover fields with the grid in the trunk or a bridge");
         a.trace = g_trace;
         a.trace_ctas = g_trace_ctas;
-        return siren_fast_debug_launch(&a, blocks, label_film, feature_head, variant, st);
+        return siren_fast_debug_launch(&a, label_film, feature_head, variant, st);
     }
+    const int blocks = fast_ctas(a.n_tiles, 2);      // the other instantiations run two
     if (L.grid_trunk) return siren_fast_grid_launch(&a, blocks, st);
     if (L.bridge) return siren_fast_bridge_launch(&a, blocks, st);
-    if (feature_head) return siren_fast_hd_launch(&a, blocks, label_film, st);
+    if (feature_head) return siren_fast_hd_launch(&a, label_film, st);
     if (label_film) return siren_fast_label_launch(&a, blocks, st);
-    return launch<siren_fast_kernel<false>>("siren_fast_kernel", blocks, NTHREADS, SMEM_TOTAL, st, a);
+    return launch<siren_fast_kernel<false, false, kSoftSinEvery, false, false, false, false, WG_PLAIN>>(
+        "siren_fast_kernel", fast_ctas(a.n_tiles, WG_PLAIN), fast_threads(WG_PLAIN), fast_smem(WG_PLAIN), st, a);
 }
 
 }  // namespace fn

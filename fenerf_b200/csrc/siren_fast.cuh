@@ -1,28 +1,34 @@
 // Point network, FAST mode (wgmma, sm_90a): fp16 operands, fp32 accumulation, activations held in registers.
 //
-// One persistent CTA per SM, 384 threads = three warpgroups:
-//   warps 0..3, 4..7   two consumer warpgroups; each evaluates the whole network for its own tile of 64 points
-//   warp 8             weight producer (its warpgroup gives its registers to the consumers): bulk copies of the packed weight images (layout.h) into a ring of six
-//                      32 KB slots, in the order the consumers read them; both warpgroups read every slot
-//   warps 9, 10        FiLM producers, one per consumer warpgroup: each fills a two-entry ring of that warpgroup with
-//                      every layer's FiLM constants already folded, per column pair {f_c, f_c+1, f_c b_c + p_c, ...}
-//                      (2 KB, one LDS.128 per four epilogue elements), so that the epilogue does no f b + p
+// One persistent CTA per SM, kWG consumer warpgroups and one producer warpgroup.  kWG = 3 (WG_PLAIN: the plain
+// instantiation, the feature-head one without the label FiLM branch, and the debug ones built from them) runs 512
+// threads; the label FiLM, grid-trunk, bridge and split instantiations run kWG = 2, 384 threads (DESIGN section 5):
+//   warps 0 .. 4 kWG - 1   the consumer warpgroups; each evaluates the whole network for its own tile of 64 points
+//   warp 4 kWG             weight producer (its warpgroup gives its registers to the consumers): bulk copies of the packed
+//                          weight images (layout.h) into a ring of 32 KB slots (six for kWG = 2, four for kWG = 3), in
+//                          the order the consumers read them; every consumer warpgroup reads every slot
+//   the next kWG warps     FiLM producers, one per consumer warpgroup: each fills a two-entry ring of that warpgroup with
+//                          every layer's FiLM constants already folded, per column pair {f_c, f_c+1, f_c b_c + p_c, ...}
+//                          (2 KB, one LDS.128 per four epilogue elements), so that the epilogue does no f b + p
 //
 // A layer is D[64 points x 256] = A[64 x 256] . W^T with A in registers (wgmma m64n128k16, one feature half at a
 // time) and W from the ring.  The accumulator fragment of wgmma is the register A fragment of the next layer
 // (sm90.cuh), so the FiLM epilogue sin(f z + (f b + p)) turns half h of the accumulator into k-slices 8h .. 8h+7
-// of the next layer's A operand without touching shared memory.  Registers per consumer thread: 64 (A) + 64
-// (accumulator) + 32 (half of the next A) + the input slots of the first colour layer, within the 232 that setmaxnreg
-// grants.
+// of the next layer's A operand.  Registers per consumer thread, kWG = 2: 64 (A) + 64 (accumulator) + 32 (half 0 of
+// the next A, `nxt`, while half 1 is computed) + the input slots of the first colour layer, within the 232 that
+// setmaxnreg grants.  kWG = 3 has 160: half 0 of the next A waits in the warpgroup's park region in shared memory
+// instead of `nxt` and is read back once half 1's MMA group has completed, and the input slices are SS operands from
+// a 128B-swizzled staging chunk instead of register fragments (SMEM3_*).
 //
-// The two consumer warpgroups take turns at the tensor cores (ping-pong): a warpgroup waits for its turn, issues one
-// MMA group (a half layer with the colour-layer input slices, a first-layer half, or a head), commits it and hands the
-// turn to the other warpgroup; only then does it wait for its own MMAs and run their epilogue.  The tensor cores
-// execute the MMA groups in issue order, so one warpgroup's sin epilogue runs under the other's MMAs instead of both
-// warpgroups computing sines at once while the tensor cores idle.  The turns are a pair of mbarriers (bounded waits).
+// The consumer warpgroups take turns at the tensor cores in strict rotation (kWG = 2: ping-pong): a warpgroup waits for
+// its turn, issues one MMA group (a half layer with the colour-layer input slices, a first-layer half, or a head),
+// commits it and hands the turn to the next warpgroup; only then does it wait for its own MMAs and run their epilogue.
+// The tensor cores execute the MMA groups in issue order, so a warpgroup's sin epilogue runs under the others' MMAs
+// instead of all warpgroups computing sines at once while the tensor cores idle.  The turns are one mbarrier per
+// warpgroup (bounded waits).
 //
 // The input slots of a point (layout.h: positions, view direction and grid features, hi / lo split in fp16) are
-// built once per tile by one thread per point into a small staging buffer and read from there as A fragments.
+// built once per tile by one thread per point into a small staging buffer and read from there as A operands.
 //
 // The kernel reads where sigma and the labels sit, and where each head's bias is, from the layout (layout.h); the
 // feature-head instantiations take these as the constants fn_make_layout writes for their fields (see the trunk head).
@@ -89,6 +95,25 @@ constexpr uint32_t SMEM_TOTAL_GRID = SMEM_XLO + 2 * TILE * XLO_STRIDE * 2;
 // sections above in their order.  4 x 32 + 2 x 32 (A_lo) + 18 (staging) + 8 (FiLM) + 0.14 (barriers) + 8 (XLO) KB =
 // 231568 B of the 232448
 constexpr int RING_SPLIT = 4;
+// Three consumer warpgroups (kWG = 3; the plain instantiation and the debug ones built from it): 512 threads, so the
+// register file gives the consumers 160 per thread.  A ring of four slots (two half layers), then one 16 KB park region
+// per warpgroup (half 0's epilogue output, [8 k-slices][128 threads] uint4, until half 1's MMA group has completed), the
+// staging rows as one [64 points][64 slots] 128B-swizzled K-major chunk per warpgroup (the input slices are SS operands,
+// so they take no registers), the FiLM entries and the barriers: 131072 + 49152 + 24576 + 12288 + 184 = 217272 B of
+// the 232448
+constexpr int WG_PLAIN = 3;
+constexpr int RING3 = 4;
+constexpr uint32_t PARK_BYTES = 128 * 8 * 16;
+constexpr uint32_t X3_BYTES = TILE * 64 * 2;
+constexpr uint32_t SMEM3_PARK = RING3 * SLOT_BYTES;
+constexpr uint32_t SMEM3_X = SMEM3_PARK + 3 * PARK_BYTES;
+constexpr uint32_t SMEM3_FILM = SMEM3_X + 3 * X3_BYTES;
+constexpr uint32_t SMEM3_BAR = SMEM3_FILM + 3 * FRING * FILM_BYTES;
+// full[RING3], empty[RING3], turn[3], film_full[3 * FRING], film_empty[3 * FRING]
+constexpr uint32_t SMEM3_TOTAL = SMEM3_BAR + 16 * RING3 + 8 * 3 + 16 * 3 * FRING;
+static_assert(SMEM3_TOTAL == 217272 && SMEM3_X % 1024 == 0, "three warpgroups: the shared-memory plan");
+constexpr int fast_threads(int wgs) { return 128 * (wgs + 1); }
+constexpr uint32_t fast_smem(int wgs) { return wgs == 3 ? SMEM3_TOTAL : SMEM_TOTAL; }
 constexpr uint32_t ALO_CHUNK = TILE * FN_KCHUNK * 2;                 // one [64 rows][64 k] f16 A chunk, 8 KB
 constexpr uint32_t ALO_BYTES = (FN_H / FN_KCHUNK) * ALO_CHUNK;      // one warpgroup's [4 k-chunks][64 points][64 k]
 constexpr uint32_t SPLIT_SMEM_ALO = RING_SPLIT * SLOT_BYTES;
@@ -116,7 +141,7 @@ constexpr int kSoftSinEvery = FENERF_SOFT_SIN_EVERY;
 constexpr int kSoftSinSplit = 4;
 // timeline (kTrace): 64-bit events per traced warp, {kind 8 bits, group 8 bits, clock64 48 bits}
 constexpr int TRACE_CAP = 1024;
-constexpr int TRACE_WARPS = 11;
+constexpr int TRACE_WARPS = 16;
 enum TraceEvent {
     TR_PAIR = 1, TR_TURN_WAIT, TR_TURN_DONE, TR_ACQ_WAIT, TR_ACQ_DONE, TR_COMMIT, TR_MMA_DONE, TR_EPI_DONE,
     TR_FILM_WAIT, TR_FILM_DONE, TR_EMPTY_WAIT, TR_EMPTY_DONE,
@@ -171,53 +196,67 @@ using SplitArgs = FastArgsT<MAX_LOADS_SPLIT>;
 
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
+// CTAs of a launch with `wgs` consumer warpgroups: a CTA takes a group of `wgs` tiles at a time, at most one CTA per SM
+inline int fast_ctas(long long n_tiles, int wgs) {
+    const long long n_groups = (n_tiles + wgs - 1) / wgs;
+    return (int)(n_groups < (long long)num_sms() ? n_groups : (long long)num_sms());
+}
+
 template <bool kLabelFilm, bool kFeatureHead = false, int kSoftSin = kSoftSinEvery, bool kTrace = false,
-          bool kGridTrunk = false, bool kBridge = false, bool kSplit = false>
-__global__ void __launch_bounds__(NTHREADS, 1)
+          bool kGridTrunk = false, bool kBridge = false, bool kSplit = false, int kWG = 2>
+__global__ void __launch_bounds__(fast_threads(kWG), 1)
     siren_fast_kernel(const __grid_constant__ FastArgsT<kSplit ? MAX_LOADS_SPLIT : MAX_LOADS> a) {
-    // the shared-memory plan (kSplit: a smaller ring and the A_lo regions, see SPLIT_SMEM_ALO)
-    constexpr int RING = kSplit ? RING_SPLIT : fn::RING;
-    constexpr uint32_t SMEM_X = kSplit ? SPLIT_SMEM_X : fn::SMEM_X;
-    constexpr uint32_t SMEM_FILM = kSplit ? SPLIT_SMEM_FILM : fn::SMEM_FILM;
-    constexpr uint32_t SMEM_BAR = kSplit ? SPLIT_SMEM_BAR : fn::SMEM_BAR;
+    static_assert(kWG == 2 || (kWG == 3 && !kSplit), "two consumer warpgroups, or three without the A_lo regions");
+    // the shared-memory plan (kSplit: a smaller ring and the A_lo regions, see SPLIT_SMEM_ALO; kWG = 3: SMEM3_TOTAL)
+    constexpr int RING = kSplit ? RING_SPLIT : kWG == 3 ? RING3 : fn::RING;
+    constexpr int PROD_WARP = 4 * kWG;
+    constexpr uint32_t SMEM_X = kSplit ? SPLIT_SMEM_X : kWG == 3 ? SMEM3_X : fn::SMEM_X;
+    constexpr uint32_t SMEM_FILM = kSplit ? SPLIT_SMEM_FILM : kWG == 3 ? SMEM3_FILM : fn::SMEM_FILM;
+    constexpr uint32_t SMEM_BAR = kSplit ? SPLIT_SMEM_BAR : kWG == 3 ? SMEM3_BAR : fn::SMEM_BAR;
     constexpr uint32_t SMEM_XLO = kSplit ? SPLIT_SMEM_XLO : fn::SMEM_XLO;
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t sbase = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * RING, bar_turn = bar_empty + 8 * RING;
-    const uint32_t bar_ffull = bar_turn + 16, bar_fempty = bar_ffull + 8 * 2 * FRING;
+    const uint32_t bar_ffull = bar_turn + 8 * kWG, bar_fempty = bar_ffull + 8 * kWG * FRING;
     // timeline: lane 0 of every warp of the first trace_ctas CTAs appends {kind, group, clock64} until its buffer is full
-    unsigned long long* tbuf = nullptr;
-    uint32_t tn = 0;
+    // (the others start full; the buffer's address is formed at each event, which keeps the consumers' registers)
+    uint32_t tn = TRACE_CAP;
     if constexpr (kTrace)
-        if (lane == 0 && (int)blockIdx.x < a.trace_ctas) tbuf = a.trace + ((size_t)blockIdx.x * TRACE_WARPS + warp) * TRACE_CAP;
+        if (lane == 0 && (int)blockIdx.x < a.trace_ctas) tn = 0;
     auto trace = [&](int kind, int group = 0) {
         if constexpr (kTrace)
-            if (tbuf && tn < TRACE_CAP)
-                tbuf[tn++] = ((unsigned long long)kind << 56) | ((unsigned long long)group << 48) |
-                             ((unsigned long long)clock64() & ((1ull << 48) - 1));
+            if (tn < TRACE_CAP)
+                a.trace[((size_t)blockIdx.x * TRACE_WARPS + (threadIdx.x >> 5)) * TRACE_CAP + tn++] =
+                    ((unsigned long long)kind << 56) | ((unsigned long long)group << 48) |
+                    ((unsigned long long)clock64() & ((1ull << 48) - 1));
     };
     if (threadIdx.x == 0) {
         for (int i = 0; i < RING; ++i) {
             mbar_init(bar_full + 8 * i, 1);
-            mbar_init(bar_empty + 8 * i, 8);        // one arrival per consumer warp
+            mbar_init(bar_empty + 8 * i, 4 * kWG);  // one arrival per consumer warp
         }
-        for (int g = 0; g < 2; ++g) mbar_init(bar_turn + 8 * g, 4);     // warpgroup g's turn: one arrival per warp of the other
-        for (int e = 0; e < 2 * FRING; ++e) {
+        // warpgroup g's turn: one arrival per warp of the warpgroup before it
+        for (int g = 0; g < kWG; ++g) mbar_init(bar_turn + 8 * g, 4);
+        for (int e = 0; e < kWG * FRING; ++e) {
             mbar_init(bar_ffull + 8 * e, 32);       // one arrival per lane of the entry's FiLM producer
             mbar_init(bar_fempty + 8 * e, 4);       // one arrival per warp of the entry's warpgroup
         }
         fence_barrier_init();
     }
     __syncthreads();
-    const long long n_pairs = (a.n_tiles + 1) / 2;
+    // tile and point indices (kWG = 3: 32-bit, which saves the consumers registers; the launch checks the bounds)
+    using Idx = std::conditional_t<kWG == 3, int, long long>;
+    const Idx n_groups = (Idx)((a.n_tiles + kWG - 1) / kWG);     // groups of kWG tiles, one per consumer warpgroup
 
-    // registers are allocated per warpgroup: the producer warpgroup keeps 40 per thread, the consumers get 232
+    // registers are allocated per warpgroup: the producer warpgroup keeps 40 per thread, the consumers get 232 (kWG = 3:
+    // 32 and 160, 128 x 32 + 384 x 160 = 65536)
     if (warp >= PROD_WARP) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+        if constexpr (kWG == 3) asm volatile("setmaxnreg.dec.sync.aligned.u32 32;\n" ::: "memory");
+        else asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
         if (warp == PROD_WARP && lane == 0) {
             uint32_t it = 0;
-            for (long long pair = blockIdx.x; pair < n_pairs; pair += gridDim.x)
+            for (Idx grp = blockIdx.x; grp < n_groups; grp += gridDim.x)
                 for (int i = 0; i < a.n_loads; ++i, ++it) {
                     const uint32_t slot = it % RING;
                     trace(TR_EMPTY_WAIT);
@@ -226,7 +265,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
                     mbar_arrive_expect_tx(bar_full + 8 * slot, a.loads[i].bytes);
                     bulk_g2s(sbase + slot * SLOT_BYTES, a.packed + a.loads[i].src, a.loads[i].bytes, bar_full + 8 * slot);
                 }
-        } else if (warp == PROD_WARP + 1 || warp == PROD_WARP + 2) {
+        } else if (warp == PROD_WARP + 1 || warp == PROD_WARP + 2 || (kWG == 3 && warp == PROD_WARP + 3)) {
             // the FiLM layers of consumer warpgroup g's tiles, in the order its epilogues use them: the first layer, then
             // hidden layers 0 .. n - 1 (n = trunk_hidden when the network stops after the trunk head).  Each lane folds
             // four column pairs, c = f b + p with the expression the epilogue used to evaluate (the same bits), and
@@ -234,9 +273,9 @@ __global__ void __launch_bounds__(NTHREADS, 1)
             const int g = warp - PROD_WARP - 1;
             const int n_film = 1 + (a.sigma_only ? a.L.trunk_hidden : a.L.n_hidden);
             uint32_t it = 0;
-            for (long long pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
-                const long long tile = pair * 2 + g;
-                const long long b = tile < a.n_tiles ? tile / a.tiles_per_batch : 0;
+            for (Idx grp = blockIdx.x; grp < n_groups; grp += gridDim.x) {
+                const Idx tile = grp * kWG + g;
+                const Idx b = tile < a.n_tiles ? tile / a.tiles_per_batch : 0;
                 const float* film_b = a.film + (size_t)b * a.L.n_film * 2 * FN_H;
                 for (int i = 0; i < n_film; ++i, ++it) {
                     const uint32_t e = g * FRING + it % FRING;
@@ -268,7 +307,8 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     }
 
     // ================= consumers =================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    if constexpr (kWG == 3) asm volatile("setmaxnreg.inc.sync.aligned.u32 160;\n" ::: "memory");
+    else asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     const int wg = warp >> 2, q = lane & 3;
     const int tid = threadIdx.x & 127;
     const int r0 = (warp & 3) * 16 + (lane >> 2);   // this thread's rows of the tile: r0 and r0 + 8
@@ -284,6 +324,9 @@ __global__ void __launch_bounds__(NTHREADS, 1)
     const int rgb_rows = kFeatureHead ? FN_FEAT : L.rgb.w_rows;
     const int label_rows = kFeatureHead ? FN_FEAT : L.label.w_rows;
     __half* xs = reinterpret_cast<__half*>(smem + SMEM_X) + wg * TILE * XSTRIDE;
+    // kWG = 3: the staging chunk, k-slice s of the input slots at + 32 s (the A operand of the input MMAs, SS)
+    unsigned char* const xs3 = smem + SMEM_X + wg * X3_BYTES;
+    const uint32_t xs3_addr = sbase + SMEM_X + wg * X3_BYTES;
     uint32_t it = 0;
     // the next load of the stream: wait until it has landed, return its slot's shared-memory address
     auto acquire = [&](uint32_t& slot) -> uint32_t {
@@ -298,12 +341,14 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_empty + 8 * slot);
     };
-    // MMA turns, strictly alternating and warpgroup 0 first: turn n of warpgroup 1 waits for phase n of its barrier, turn
-    // n of warpgroup 0 for phase n - 1 of its own (its first turn passes at once).  Invariant: both warpgroups take the
-    // same number of turns for every tile pair -- they run the same sequence of layers, the warpgroup without a tile in a
-    // CTA's last pair included, and the sigma_only stop comes after the same trunk-head turn in both.  A warpgroup that
-    // took one turn more would wait for a handover that never comes (and trap).
+    // MMA turns, in strict rotation and warpgroup 0 first: turn n of warpgroup g > 0 waits for phase n of its barrier (the
+    // end of turn n of warpgroup g - 1), turn n of warpgroup 0 for phase n - 1 of its own (the end of the last
+    // warpgroup's turn n - 1; its first turn passes at once).  Invariant: every warpgroup takes the same number of turns
+    // for every tile group -- they run the same sequence of layers, a warpgroup without a tile in a CTA's last group
+    // included, and the sigma_only stop comes after the same trunk-head turn in all.  A warpgroup that took one turn more
+    // would wait for a handover that never comes (and trap).
     uint32_t turns = 0;
+    const int next_wg = kWG == 2 ? (wg ^ 1) : (wg + 1) % kWG;
     // this warpgroup's FiLM entries (filled by its FiLM producer), one per layer, in layer order
     uint32_t fit = 0;
     auto film_acquire = [&]() -> const float4* {
@@ -328,7 +373,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         trace(TR_COMMIT, group);
         ++turns;
         __syncwarp();
-        if (lane == 0) mbar_arrive(bar_turn + 8 * (wg ^ 1));
+        if (lane == 0) mbar_arrive(bar_turn + 8 * next_wg);
     };
     // A fragment of k-slice s of the staged input slots
     auto xfrag = [&](int s, uint32_t (&f)[4]) {
@@ -339,13 +384,13 @@ __global__ void __launch_bounds__(NTHREADS, 1)
         f[3] = *reinterpret_cast<const uint32_t*>(p + 8 * XSTRIDE + 8);
     };
 
-    for (long long pair = blockIdx.x; pair < n_pairs; pair += gridDim.x) {
-        const long long tile = pair * 2 + wg;
-        // a CTA's last pair may hold a single tile: the other warpgroup still consumes the weight stream, on rows that
-        // are all past the end (nothing is stored)
+    for (Idx grp = blockIdx.x; grp < n_groups; grp += gridDim.x) {
+        const Idx tile = grp * kWG + wg;
+        // a CTA's last group may hold fewer tiles than warpgroups: the others still consume the weight stream, on rows
+        // that are all past the end (nothing is stored)
         const bool tile_ok = tile < a.n_tiles;
-        const long long b = tile_ok ? tile / a.tiles_per_batch : 0;
-        const long long p0 = tile_ok ? (tile % a.tiles_per_batch) * TILE : a.ppb;
+        const Idx b = tile_ok ? tile / a.tiles_per_batch : 0;
+        const Idx p0 = tile_ok ? (tile % a.tiles_per_batch) * TILE : a.ppb;
         trace(TR_PAIR);
 
         // ---- input slots of the tile's points (layout.h), one thread per point ----
@@ -397,9 +442,16 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 #pragma unroll
                 for (int i = 0; i < 32; ++i) slots[FN_SLOT_FEAT + i] = __float2half_rn(feat[i]);
             }
+            if constexpr (kWG == 3) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i)
-                reinterpret_cast<uint4*>(xs + tid * XSTRIDE)[i] = reinterpret_cast<const uint4*>(slots)[i];
+                for (int i = 0; i < 8; ++i)
+                    *reinterpret_cast<uint4*>(xs3 + fn_sw128_offset(tid, 8 * i)) = reinterpret_cast<const uint4*>(slots)[i];
+                fence_async_smem();                  // the generic-proxy stores, visible to the tensor cores' reads
+            } else {
+#pragma unroll
+                for (int i = 0; i < 8; ++i)
+                    reinterpret_cast<uint4*>(xs + tid * XSTRIDE)[i] = reinterpret_cast<const uint4*>(slots)[i];
+            }
         }
         wg_bar(wg);
 
@@ -421,6 +473,24 @@ __global__ void __launch_bounds__(NTHREADS, 1)
             trace(TR_EPI_DONE);
         };
         auto act_hi = [&]() -> uint32_t (&)[8][4] { return *reinterpret_cast<uint32_t (*)[8][4]>(&act[8]); };
+        // kWG = 3: half 0's epilogue output waits in the warpgroup's park region (k-slice s of thread tid at [s][tid])
+        // instead of `nxt`, until half 1's MMA group has completed and act[0..7] are free again
+        uint4* const park = reinterpret_cast<uint4*>(smem + SMEM3_PARK + wg * PARK_BYTES) + tid;
+        auto park_store = [&]() {
+            if constexpr (kWG == 3) {
+#pragma unroll
+                for (int s = 0; s < 8; ++s) park[128 * s] = make_uint4(nxt[s][0], nxt[s][1], nxt[s][2], nxt[s][3]);
+            }
+        };
+        auto park_load = [&]() {
+            if constexpr (kWG == 3) {
+#pragma unroll
+                for (int s = 0; s < 8; ++s) {
+                    const uint4 v = park[128 * s];
+                    act[s][0] = v.x; act[s][1] = v.y; act[s][2] = v.z; act[s][3] = v.w;
+                }
+            }
+        };
         // kSplit: the same epilogue with every sine on soft_sinf (sin.approx loses the bits of its own a / 2pi product),
         // hi = f16(s) into dst and lo = f16(s - hi) into lo, in the same fragment order
         auto film_epi_split = [&](const float4* fs, int h, uint32_t (&dst)[8][4], uint32_t (&lo)[8][4]) {
@@ -469,7 +539,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
             uint32_t xf[4], slot, slot_lo = 0, w_lo = 0;
             uint32_t xg[2][4], xl[2][4];             // kGridTrunk: feature slots 32..63, hi and lo
             const float4* fs = nullptr;
-            xfrag(0, xf);
+            if constexpr (kWG == 2) xfrag(0, xf);
             if constexpr (kGridTrunk) {
                 const __half* xlo = reinterpret_cast<const __half*>(smem + SMEM_XLO) + wg * TILE * XLO_STRIDE;
 #pragma unroll
@@ -488,7 +558,8 @@ __global__ void __launch_bounds__(NTHREADS, 1)
             for (int h = 0; h < 2; ++h) {
                 turn_begin();
                 wg_fence();
-                mma_rs_n128(d, xf, desc_kmajor(w + h * CHUNK), 0u);
+                if constexpr (kWG == 3) mma_ss_n128(d, desc_kmajor(xs3_addr), desc_kmajor(w + h * CHUNK), 0u);
+                else mma_rs_n128(d, xf, desc_kmajor(w + h * CHUNK), 0u);
                 if constexpr (kGridTrunk)
 #pragma unroll
                     for (int s = 0; s < 2; ++s) {
@@ -501,25 +572,27 @@ __global__ void __launch_bounds__(NTHREADS, 1)
                 wg_wait<0>();
                 trace(TR_MMA_DONE);
                 fence_regs(d);
-                fence_regs(xf);
+                if constexpr (kWG == 2) fence_regs(xf);     // (kWG = 3: the input slices are SS operands)
                 if constexpr (kGridTrunk) { fence_regs(xg); fence_regs(xl); }
                 if (h == 0) fs = film_acquire();
                 if constexpr (kSplit) {
                     if (h == 0) film_epi_split(fs, 0, nxt, lo0);
                     else film_epi_split(fs, 1, act_hi(), lo1);
                 } else {
-                    if (h == 0) film_epi(fs, 0, nxt);
-                    else film_epi(fs, 1, act_hi());
+                    if (h == 0) { film_epi(fs, 0, nxt); park_store(); }
+                    else { park_load(); film_epi(fs, 1, act_hi()); }
                 }
             }
             release(slot);
             if constexpr (kGridTrunk) release(slot_lo);
             film_release();
             if constexpr (kSplit) alo_store(lo0, lo1);
+            if constexpr (kWG == 2) {
 #pragma unroll
-            for (int s = 0; s < 8; ++s)
+                for (int s = 0; s < 8; ++s)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) act[s][i] = nxt[s][i];
+                    for (int i = 0; i < 4; ++i) act[s][i] = nxt[s][i];
+            }
         }
 
         bool stop = false;
@@ -771,9 +844,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
             // (a grid-trunk field: the direction alone; a bridge field: the direction and v)
             const int nx = kBridge ? 2 : !kGridTrunk && L.grid_channels > 0 ? 3 : 1;
             uint32_t xf[3][4];
-            if (c0)
+            if constexpr (kWG == 2) {
+                if (c0)
 #pragma unroll
-                for (int s = 0; s < 3; ++s) xfrag(1 + s, xf[s]);
+                    for (int s = 0; s < 3; ++s) xfrag(1 + s, xf[s]);
+            }
             uint32_t slot_x = 0, w_x = 0;
             const float4* fs = nullptr;
 #pragma unroll
@@ -796,7 +871,11 @@ __global__ void __launch_bounds__(NTHREADS, 1)
                     if (h == 0 && !narrow) w_x = acquire(slot_x);
 #pragma unroll
                     for (int s = 0; s < 3; ++s)
-                        if (s < nx) mma_rs_n128(d, xf[s], desc_kmajor(w_x + h * CHUNK + 32 * (1 + s)), (narrow && s == 0) ? 0u : 1u);
+                        if (s < nx) {
+                            const uint64_t wd = desc_kmajor(w_x + h * CHUNK + 32 * (1 + s));
+                            if constexpr (kWG == 3) mma_ss_n128(d, desc_kmajor(xs3_addr + 32 * (1 + s)), wd, (narrow && s == 0) ? 0u : 1u);
+                            else mma_rs_n128(d, xf[s], wd, (narrow && s == 0) ? 0u : 1u);
+                        }
                 }
                 wg_commit();
                 turn_end(c0 ? TG_COLOR0 : TG_HIDDEN);
@@ -804,21 +883,23 @@ __global__ void __launch_bounds__(NTHREADS, 1)
                 trace(TR_MMA_DONE);
                 fence_regs(d);
                 fence_regs(act);
-                fence_regs(xf);
+                if constexpr (kWG == 2) fence_regs(xf);
                 if (!narrow) {
                     release(sl[0]);
                     release(sl[1]);
                 }
                 if (c0 && h == 1) release(slot_x);
                 if (h == 0) fs = film_acquire();
-                if (h == 0) film_epi(fs, 0, nxt);
-                else film_epi(fs, 1, act_hi());
+                if (h == 0) { film_epi(fs, 0, nxt); park_store(); }
+                else { park_load(); film_epi(fs, 1, act_hi()); }
             }
             film_release();
+            if constexpr (kWG == 2) {
 #pragma unroll
-            for (int s = 0; s < 8; ++s)
+                for (int s = 0; s < 8; ++s)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) act[s][i] = nxt[s][i];
+                    for (int i = 0; i < 4; ++i) act[s][i] = nxt[s][i];
+            }
         }
         if (stop) continue;
 

@@ -10,10 +10,13 @@ namespace fn {
 
 namespace {
 
+// each variant runs as many consumer warpgroups as its production kernel: WG_PLAIN without the label FiLM branch, two
+// with it
 template <bool kLabelFilm, bool kFeatureHead, int kSoftSin, bool kTrace>
-int debug_launch(const FastArgs& a, int blocks, cudaStream_t st) {
-    return launch<siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace>>("siren_fast_kernel<debug>", blocks, NTHREADS,
-                                                                                SMEM_TOTAL, st, a);
+int debug_launch(const FastArgs& a, cudaStream_t st) {
+    constexpr int kWG = kLabelFilm ? 2 : WG_PLAIN;
+    return launch<siren_fast_kernel<kLabelFilm, kFeatureHead, kSoftSin, kTrace, false, false, false, kWG>>(
+        "siren_fast_kernel<debug>", fast_ctas(a.n_tiles, kWG), fast_threads(kWG), fast_smem(kWG), st, a);
 }
 
 __global__ void soft_sine_kernel(const float* a, float* out, long long n) {
@@ -23,15 +26,15 @@ __global__ void soft_sine_kernel(const float* a, float* out, long long n) {
 
 }  // namespace
 
-int siren_fast_debug_launch(const void* args, int blocks, bool label_film, bool feature_head, int variant, cudaStream_t st) {
+int siren_fast_debug_launch(const void* args, bool label_film, bool feature_head, int variant, cudaStream_t st) {
     const FastArgs& a = *static_cast<const FastArgs*>(args);
     if (variant == 1) {
-        if (feature_head) return label_film ? debug_launch<true, true, kSoftSinSplit, false>(a, blocks, st) : debug_launch<false, true, kSoftSinSplit, false>(a, blocks, st);
-        return label_film ? debug_launch<true, false, kSoftSinSplit, false>(a, blocks, st) : debug_launch<false, false, kSoftSinSplit, false>(a, blocks, st);
+        if (feature_head) return label_film ? debug_launch<true, true, kSoftSinSplit, false>(a, st) : debug_launch<false, true, kSoftSinSplit, false>(a, st);
+        return label_film ? debug_launch<true, false, kSoftSinSplit, false>(a, st) : debug_launch<false, false, kSoftSinSplit, false>(a, st);
     }
     FN_REQUIRE(!label_film && !feature_head, "the point-network timeline covers plain fields only");
-    if (variant == 2) return debug_launch<false, false, kSoftSinEvery, true>(a, blocks, st);
-    return debug_launch<false, false, kSoftSinSplit, true>(a, blocks, st);
+    if (variant == 2) return debug_launch<false, false, kSoftSinEvery, true>(a, st);
+    return debug_launch<false, false, kSoftSinSplit, true>(a, st);
 }
 
 int soft_sine_eval(const float* a, float* out, long long n, cudaStream_t st) {

@@ -648,8 +648,9 @@ int fenerf_debug_stage_times(int32_t enable, float* ms_out /* host, 6 floats */)
  * that FAST mode launches from then on: 0 the production kernel (every FiLM sine on the SFU); 1 one column pair in four of
  * the epilogue on the software sine (FMA pipe); 2 / 3 the production / the variant-1 kernel recording a clock64 timeline
  * (plain fields only).  The timeline
- * variants write into trace, a device buffer of trace_ctas x 11 x 1024 uint64 events (CTAs 0 .. trace_ctas - 1, warps
- * 0 .. 10, lane 0), each {kind bits 63..56, MMA group bits 55..48, clock64 bits 47..0}, zero past a warp's last event;
+ * variants write into trace, a device buffer of trace_ctas x 16 x 1024 uint64 events (CTAs 0 .. trace_ctas - 1, warps
+ * 0 .. 15, lane 0; the traced kernel runs three consumer warpgroups: warps 0 .. 11 consume, warp 12 streams the weights,
+ * warps 13 .. 15 fold the FiLM rows), each {kind bits 63..56, MMA group bits 55..48, clock64 bits 47..0}, zero past a warp's last event;
  * tools/siren_timeline.py decodes them.  fenerf_debug_soft_sine evaluates the epilogue's software sine on n device
  * floats. */
 int fenerf_debug_fast_variant(int32_t variant, void* trace, int32_t trace_ctas);

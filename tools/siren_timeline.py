@@ -7,16 +7,18 @@ kernel (every sine on the SFU) and of the traced kernel with one column pair in 
 (fenerf_debug_fast_variant 2 / 3), lane 0 of every warp of the first --ctas
 CTAs recording {event, clock64} (csrc/siren_fast.cuh, TraceEvent).  Per variant it reports, over those CTAs:
 
-  tensor idle   share of clocks between a CTA's first MMA issue and its last MMA completion in which neither consumer
+  tensor idle   share of clocks between a CTA's first MMA issue and its last MMA completion in which no consumer
                 warpgroup has an MMA group in flight (its turn taken, its wg_wait not yet returned)
-  per group     MMA group duration (its completion minus the later of its turn and the other warpgroup's previous
-                completion) and the epilogue after it (wg_wait returned -> FiLM epilogue done), median / p90 clocks
+  per group     MMA group duration (its completion minus the later of its turn and the other warpgroups' latest
+                completion before it) and the epilogue after it (wg_wait returned -> FiLM epilogue done), median / p90
+                clocks
   waits         consumer clocks in turn waits, weight-slot waits (acquire) and FiLM-entry waits, as shares of the
                 window; the producers' empty-slot waits
 
 Clock stamps cost a few instructions each; the traced kernels run slightly slower than the production ones.
 """
 import argparse
+import bisect
 import ctypes
 import json
 import os
@@ -33,7 +35,9 @@ import bench  # noqa: E402
 from fenerf_b200 import _lib, ops  # noqa: E402
 from fenerf_b200.generators import volumetric_rendering as vr  # noqa: E402
 
-WARPS, CAP = 11, 1024
+WARPS, CAP = 16, 1024
+CONSUMER_WGS = 3                      # warps 0..11; warp 12 streams the weights, warps 13..15 fold the FiLM rows
+WEIGHT_WARP = 4 * CONSUMER_WGS
 (PAIR, TURN_WAIT, TURN_DONE, ACQ_WAIT, ACQ_DONE, COMMIT, MMA_DONE, EPI_DONE, FILM_WAIT, FILM_DONE, EMPTY_WAIT,
  EMPTY_DONE) = range(1, 13)
 GROUPS = ["first", "hidden", "color0", "trunk_head", "label_layer", "label_head", "out_head"]
@@ -118,11 +122,11 @@ def analyse(buf):
     producer_clocks = 0
     for cta in range(buf.shape[0]):
         evs = [decode(buf[cta, w]) for w in range(WARPS)]
-        if not evs[0] or not evs[4]:
+        if any(not evs[4 * g] for g in range(CONSUMER_WGS)):
             continue
-        # warps 0 and 4 stand for their warpgroups (all four warps of a warpgroup wait for the same MMA group)
-        g0, g1 = consumer_groups(evs[0]), consumer_groups(evs[4])
-        ivs = sorted([(c, d) for _, c, d, _ in g0 + g1])
+        # warp 4 g stands for warpgroup g (all four warps of a warpgroup wait for the same MMA group)
+        wgs = [consumer_groups(evs[4 * g]) for g in range(CONSUMER_WGS)]
+        ivs = sorted([(c, d) for groups in wgs for _, c, d, _ in groups])
         lo, hi = ivs[0][0], max(d for _, d in ivs)
         busy, cur_s, cur_e = 0, None, None
         for s, e in ivs:
@@ -135,15 +139,15 @@ def analyse(buf):
         busy += cur_e - cur_s
         idle += (hi - lo) - busy
         window += hi - lo
-        done_other = {0: [d for _, _, d, _ in g1], 1: [d for _, _, d, _ in g0]}
-        for wg, groups in ((0, g0), (1, g1)):
+        for wg, groups in enumerate(wgs):
+            done_other = sorted(d for o, other in enumerate(wgs) if o != wg for _, _, d, _ in other)
             for grp, c, d, e in groups:
-                prev = [x for x in done_other[wg] if x <= d]
-                start = max(c, prev[-1]) if prev else c
+                i = bisect.bisect_right(done_other, d)
+                start = max(c, done_other[i - 1]) if i else c
                 mma.setdefault(GROUPS[grp], []).append(d - start)
                 if e is not None:
                     epi.setdefault(GROUPS[grp], []).append(e - d)
-        for w in range(8):
+        for w in range(WEIGHT_WARP):
             ev = evs[w]
             if not ev:
                 continue
@@ -151,7 +155,7 @@ def analyse(buf):
             waits["turn"] += wait_clocks(ev, TURN_WAIT, TURN_DONE)
             waits["weight_slot"] += wait_clocks(ev, ACQ_WAIT, ACQ_DONE)
             waits["film_entry"] += wait_clocks(ev, FILM_WAIT, FILM_DONE)
-        for w, key in ((8, "weight_empty"), (9, "film_empty"), (10, "film_empty")):
+        for w, key in [(WEIGHT_WARP, "weight_empty")] + [(WEIGHT_WARP + 1 + g, "film_empty") for g in range(CONSUMER_WGS)]:
             ev = evs[w]
             if ev:
                 producer_clocks += ev[-1][2] - ev[0][2]
