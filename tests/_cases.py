@@ -313,6 +313,49 @@ def tile_layout(name, sms, dir_group=1):
     return batch, ppb - ppb % dir_group
 
 
+#: consumer warpgroups of the plain instantiation of the fast kernel and of the ones built from it (csrc/siren_fast.cuh):
+#: a CTA takes a group of three tiles per round, CTAs = min(groups, SMs), tiles are never shared between images
+WG_PLAIN = 3
+
+#: launch shapes of the three-warpgroup schedule, name -> what it reaches (wg3_layout gives their sizes)
+WG3_LAYOUTS = {
+    "one_group_per_cta": "3 SMs tiles: every CTA runs exactly one group; the last tile holds 1 point",
+    "one_tile_in_second_group": "3 SMs + 1 tiles: CTA 0 comes back for a group whose warpgroups 1 and 2 have no tile "
+                                "(they stream the weights on rows past the end); the last tile holds 63 points",
+    "two_tiles_in_second_group": "3 SMs + 2 tiles: CTA 0's second group leaves warpgroup 2 without a tile; last tile 27",
+    "one_cta_short": "3 (SMs - 1) tiles: one CTA fewer than the SMs, one full group each; last tile 63",
+    "five_rounds": "15 SMs + 2 tiles: every CTA runs five rounds, CTA 0 a sixth one holding two tiles, so the weight ring, "
+                   "the turn barriers and the FiLM rings wrap their phases many times; last tile 1",
+    "tiny_1": "3 SMs + 1 images of 1 point: a group covers three images, every warpgroup works on a tail, CTA 0 comes "
+              "back for the last image alone",
+    "tiny_37": "3 SMs + 1 images of 37 points, as tiny_1",
+    "tiny_63": "3 SMs + 1 images of 63 points, as tiny_1",
+    "tiny_64": "3 SMs + 1 images of 64 points: full tiles, a group covers three images",
+    "tiny_65": "3 SMs + 1 images of 65 points: two tiles per image, the second of 1 point; groups straddle two images, "
+               "three rounds for CTA 0",
+}
+
+
+def wg3_layout(name, sms, dir_group=1):
+    """-> (batch, points per image) of a WG3_LAYOUTS entry on a GPU with `sms` SMs.  The points per image are a multiple
+    of dir_group; when the layout's tail is not, the nearest multiple that keeps the tile count is taken."""
+    g = WG_PLAIN
+    tiny = g * sms + 1
+    batch, tiles, tail = {"one_group_per_cta": (1, g * sms, 1),
+                          "one_tile_in_second_group": (1, g * sms + 1, 63),
+                          "two_tiles_in_second_group": (1, g * sms + 2, 27),
+                          "one_cta_short": (1, g * (sms - 1), 63),
+                          "five_rounds": (1, 5 * g * sms + 2, 1),
+                          "tiny_1": (tiny, 1, 1),
+                          "tiny_37": (tiny, 1, 37),
+                          "tiny_63": (tiny, 1, 63),
+                          "tiny_64": (tiny, 1, 64),
+                          "tiny_65": (tiny, 2, 1)}[name]
+    ppb = (tiles - 1) * 64 + tail
+    up = -(-ppb // dir_group) * dir_group
+    return batch, up if up <= tiles * 64 else up - dir_group
+
+
 def grid_probe_index(numel, n):
     """Fixed pseudo-random flat indices into the feature grid (the gradient goldens store only these entries)."""
     g = torch.Generator().manual_seed(7)

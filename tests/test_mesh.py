@@ -4,7 +4,8 @@ CPU: the tables regenerate to the checked-in header and follow their rule case b
 extraction (tests/_mesh.py) gives closed, consistently oriented meshes of the right topology and area on synthetic grids;
 write_ply round-trips.  GPU: the library's faces equal the restatement's exactly on those grids; on the fields' own
 grids (models A, B, L, N) the density grid is the shape script's, the mesh is closed away from the box, every vertex
-lies on its grid edge, and the per-vertex attributes are the point network's at the vertices.
+lies on its grid edge and equals the restatement's, and the per-vertex attributes are the point network's at the vertices
+(test_gpu_fp64_wg3.py compares them with float64).
 """
 import ctypes as C
 import math
@@ -216,6 +217,7 @@ def test_field_mesh(model, n):
     boundary = M.check_closed(vn, fn_, origin, voxel, n)
     want_v, want_f, owner, axis = M.extract(sig, level, origin, voxel, with_edges=True)
     assert np.array_equal(fn_, want_f)
+    assert np.abs(vn - want_v).max() <= 1e-6 * CUBE, "vertices off the float64 restatement's"
     idx = np.stack(np.unravel_index(owner, (n, n, n)), axis=1)
     lat = M.lattice(origin, voxel, n)
     rows = np.arange(len(owner))
