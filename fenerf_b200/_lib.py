@@ -45,6 +45,7 @@ EXPORTS = (
     "fenerf_render_rays_grad", "fenerf_rays_grad_workspace_layout", "fenerf_composite_backward_rays_dz",
     "fenerf_grid_coord_grad", "fenerf_ray_dir_grad",
     "fenerf_mc_workspace_bytes", "fenerf_mc_count", "fenerf_mc_emit",
+    "fenerf_camera_poses_dev", "fenerf_cam2world_grad_workspace_bytes", "fenerf_cam2world_grad",
 )
 
 
@@ -113,6 +114,12 @@ def _declare(lib):
     lib.fenerf_siren_points.argtypes = [P(FieldDesc), vp, vp, vp, vp, i32, i64, i32, i32, vp, i32, vp, vp]
     lib.fenerf_camera_poses.restype = C.c_int
     lib.fenerf_camera_poses.argtypes = [i32, i32, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp]
+    lib.fenerf_camera_poses_dev.restype = C.c_int
+    lib.fenerf_camera_poses_dev.argtypes = [i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]
+    lib.fenerf_cam2world_grad_workspace_bytes.restype = sz
+    lib.fenerf_cam2world_grad_workspace_bytes.argtypes = [P(RenderDesc)]
+    lib.fenerf_cam2world_grad.restype = C.c_int
+    lib.fenerf_cam2world_grad.argtypes = [P(RenderDesc)] + [vp] * 7 + [C.c_float, vp, sz, vp, vp]
     lib.fenerf_ray_setup.restype = C.c_int
     lib.fenerf_ray_setup.argtypes = [P(RenderDesc)] + [vp] * 10
     lib.fenerf_resample.restype = C.c_int

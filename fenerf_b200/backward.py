@@ -731,16 +731,19 @@ def _input_grads(ctx, d_film, grads):
 
 
 class RenderFunction(torch.autograd.Function):
-    """pixels = render(film, field parameters); see the module docstring."""
+    """pixels = render(film, field parameters); see the module docstring.  With call['pose_grad'] the cam2world matrices
+    follow the parameters as an input and get the gradient of the coarse sample points R p_cam + T and of the ray
+    directions R d_cam of both passes (fenerf_cam2world_grad); the fine points, the depths and the origins carry none, as
+    in the reference."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type='cuda', cast_inputs=torch.float32)
-    def forward(ctx, film, call, *params):
+    def forward(ctx, film, call, *inputs):
         module, rd = call['module'], call['rd']
         st = ops.render_forward_stages(module, rd, film, call['x_lin'], call['y_lin'], call['z_lin'], call['cam2world'],
                                        call['rng_perturb'], call['rng_noise_c'], call['rng_u'], call['rng_noise_f'])
         ctx.stages = st
-        _save_inputs(ctx, call, film, params)
+        _save_inputs(ctx, call, film, inputs[:len(call['params'])])
         return st['pixels']
 
     @staticmethod
@@ -781,13 +784,49 @@ class RenderFunction(torch.autograd.Function):
 
             if rays is not None:
                 dirs = dirs.index_select(1, rays).contiguous()
+            # the pose gradient: d sample points of the coarse pass, d direction per point of both passes (none under
+            # lock_view_dependence or for the direction-free field)
+            pose = bool(call.get('pose_grad')) and ctx.needs_input_grad[2 + len(ctx.param_ids)]
+            dx = dir_c = dir_f = None
+            if pose:
+                dx = torch.zeros((B, n * s, 3), dtype=torch.float32, device=dev)
+                if not lock and not fb.spec.wo_dir:
+                    dir_c = torch.zeros_like(dx)
+                    dir_f = torch.zeros_like(dx) if hier else None
             if hier:
-                fb.add_points(pick(st['points_f'], 3), dirs, s, lock, pick(st['raw_f'], c), pick(d_raw_f, c))
-            fb.add_points(pick(st['points_c'], 3), dirs, s, lock, pick(st['raw_c'], c), pick(d_raw_c, c))
+                fb.add_points(pick(st['points_f'], 3), dirs, s, lock, pick(st['raw_f'], c), pick(d_raw_f, c),
+                              ray_grad=dict(ddir=dir_f) if dir_f is not None else None)
+            fb.add_points(pick(st['points_c'], 3), dirs, s, lock, pick(st['raw_c'], c), pick(d_raw_c, c),
+                          ray_grad=dict(dx=dx, ddir=dir_c) if pose else None)
             d_film, grads = fb.finish()
+            d_c2w = _cam2world_grad(call, fb, dx, dir_c, dir_f) if pose else None
             if call.get('grad_reduce') is not None:
-                call['grad_reduce']([d_film] + list(grads.values()))
-        return tuple(_input_grads(ctx, d_film, grads))
+                call['grad_reduce']([d_film] + list(grads.values()) + [d_c2w])
+        out = _input_grads(ctx, d_film, grads)
+        if call.get('pose_grad'):
+            out.append(d_c2w)
+        return tuple(out)
+
+
+def _cam2world_grad(call, fb, dx, dir_c, dir_f):
+    """d cam2world (B, 4, 4) of a camera render from the coarse pass's d points `dx` and the per-point direction
+    gradients of both passes (scaled stream units): the directions' per-ray sums (fenerf_ray_dir_grad), then
+    fenerf_cam2world_grad, which recomputes the camera-space samples."""
+    rd, dev = call['rd'], fb.dev
+    B, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
+    lib = _lib.lib()
+    d_dirs = None
+    if dir_c is not None:
+        d_dirs = torch.empty((B * n, 3), dtype=torch.float32, device=dev)
+        _lib.check(lib.fenerf_ray_dir_grad(B * n, s, s, dir_c.data_ptr(), _ptr(dir_f), 0, fb.inv_scale.data_ptr(),
+                                           d_dirs.data_ptr(), _stream(dev)))
+    ws = torch.empty(lib.fenerf_cam2world_grad_workspace_bytes(C.byref(rd)), dtype=torch.uint8, device=dev)
+    d_c2w = torch.empty((B, 4, 4), dtype=torch.float32, device=dev)
+    _lib.check(lib.fenerf_cam2world_grad(
+        C.byref(rd), call['x_lin'].data_ptr(), call['y_lin'].data_ptr(), call['z_lin'].data_ptr(),
+        call['rng_perturb'].data_ptr(), dx.data_ptr(), _ptr(d_dirs), fb.inv_scale.data_ptr(), fb.spec.input_scale,
+        ws.data_ptr(), ws.numel(), d_c2w.data_ptr(), _stream(dev)))
+    return d_c2w
 
 
 class RaysRenderFunction(torch.autograd.Function):
@@ -925,11 +964,15 @@ def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_pertu
     `grad_rays`: optional int64 ray indices -- only these rays carry the gradient (part_forward).
     `grad_precision`: None (the backward of the forward precision) or 'split' (fp32 streams, the 256-wide products on the
     split kernels of csrc/gemm_split.cu; forward precision 'split' or 'exact', the fields the split forward serves).
-    `grad_reduce`: optional callable given [d film, every parameter gradient] before they leave the backward; it may
-    modify them in place (a ray-sharded render sums them over its ranks there, dist.RayShard.reduce)."""
+    `grad_reduce`: optional callable given [d film, every parameter gradient, d cam2world or None] before they leave the
+    backward; it may modify them in place (a ray-sharded render sums them over its ranks there, dist.RayShard.reduce).
+    A `cam2world` that requires grad (a pose input of forward_with_frequencies that does) gets its gradient."""
     check_grad_precision(module, grad_precision, rd.precision)
     params = FieldWeights(module).parameters()
-    call = dict(module=module, rd=rd, x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world, rng_perturb=rng_perturb,
-                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_rays=grad_rays,
-                grad_precision=grad_precision, grad_reduce=grad_reduce)
-    return RenderFunction.apply(film, call, *params)
+    pose_grad = torch.is_grad_enabled() and cam2world.requires_grad
+    if pose_grad and grad_rays is not None:
+        raise ValueError("fenerf_b200: the pose gradient is not built for ray subsets (grad_rays)")
+    call = dict(module=module, rd=rd, x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world.detach(),
+                rng_perturb=rng_perturb, rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params,
+                grad_rays=grad_rays, grad_precision=grad_precision, grad_reduce=grad_reduce, pose_grad=pose_grad)
+    return RenderFunction.apply(film, call, *params, *((cam2world,) if pose_grad else ()))

@@ -212,6 +212,35 @@ int fenerf_camera_poses(int32_t n, int32_t mode, float h_stddev, float v_stddev,
                         (cudaStream_t)stream);
 }
 
+int fenerf_camera_poses_dev(int32_t n, int32_t mode, const float* h_stddev, const float* v_stddev, const float* h_mean,
+                            const float* v_mean, int32_t per_image, const float* draw_theta, const float* draw_phi,
+                            float* cam2world, float* pitch, float* yaw, void* stream) {
+    FN_REQUIRE(n >= 1 && h_stddev && v_stddev && h_mean && v_mean && cam2world && pitch && yaw, "bad argument");
+    FN_REQUIRE(per_image >= 0 && per_image <= 15, "per_image %d: a mask of bits 0..3", per_image);
+    FN_REQUIRE(mode >= FENERF_CAMERA_FIXED && mode <= FENERF_CAMERA_SPHERICAL_UNIFORM, "unsupported camera mode %d", mode);
+    FN_REQUIRE(mode == FENERF_CAMERA_FIXED || (draw_theta && draw_phi), "camera mode %d needs the two random draws", mode);
+    return camera_poses_dev(n, mode, h_stddev, v_stddev, h_mean, v_mean, per_image, draw_theta, draw_phi, cam2world, pitch,
+                            yaw, (cudaStream_t)stream);
+}
+
+size_t fenerf_cam2world_grad_workspace_bytes(const fenerf_render_desc* rd) {
+    if (!rd || check_render_desc(rd)) return 0;
+    return cam2world_grad_workspace_bytes(rd);
+}
+
+int fenerf_cam2world_grad(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
+                          const float* rng_perturb, const float* d_points, const float* d_dirs, const float* inv_scale,
+                          float input_scale, void* workspace, size_t workspace_bytes, float* d_cam2world, void* stream) {
+    if (int e = check_render_desc(rd)) return e;
+    FN_REQUIRE(x_lin && y_lin && z_lin && rng_perturb && d_points && inv_scale && workspace && d_cam2world, "NULL argument");
+    FN_REQUIRE(rd->num_steps >= 2, "num_steps %d: the perturbation needs two depths", rd->num_steps);
+    FN_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "workspace must be 8-byte aligned");
+    FN_REQUIRE(workspace_bytes >= cam2world_grad_workspace_bytes(rd), "workspace too small: %zu < %zu", workspace_bytes,
+               cam2world_grad_workspace_bytes(rd));
+    return cam2world_grad(rd, x_lin, y_lin, z_lin, rng_perturb, d_points, d_dirs, inv_scale, input_scale, (double*)workspace,
+                          d_cam2world, (cudaStream_t)stream);
+}
+
 int fenerf_ray_setup(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
                      const float* cam2world, const float* rng_perturb, float* points, float* z_vals, float* dirs,
                      float* origins, void* stream) {

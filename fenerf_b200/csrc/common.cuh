@@ -141,6 +141,13 @@ int camera_poses(int n, int mode, float h_std, float v_std, float h_mean, float 
 int ray_setup(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
               const float* cam2world, const float* rng_perturb, float* points, float* z_vals, float* dirs,
               float* origins, cudaStream_t st);
+int camera_poses_dev(int n, int mode, const float* h_std, const float* v_std, const float* h_mean, const float* v_mean,
+                     int per_image, const float* draw_theta, const float* draw_phi, float* c2w, float* pitch, float* yaw,
+                     cudaStream_t st);
+size_t cam2world_grad_workspace_bytes(const fenerf_render_desc* rd);
+int cam2world_grad(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
+                   const float* rng_perturb, const float* d_points, const float* d_dirs, const float* inv_scale,
+                   float input_scale, double* partial, float* d_cam2world, cudaStream_t st);
 // The resampler.  origins: one per image (B, 3), the camera render's (fenerf_resample, fenerf_render_forward: inds,
 // sort_fine) -- or ray_origins: one per ray (B, N, 3), the rays-in render's (fenerf_render_rays), whose fine samples are
 // always depth-sorted.  Rays-in with dirs_sample (B, N, S, 3) (per-sample directions), fine sample k of sample_pdf's

@@ -16,6 +16,8 @@ every rank, and the backward sums d FiLM and the field's parameter gradients ove
 import torch
 import torch.distributed as dist
 
+from . import ops
+
 
 def shard_bounds(total, rank, world):
     """Contiguous near-even split; the first `total % world` ranks get one extra image."""
@@ -74,11 +76,14 @@ class FrameGatherer:
 
 def render_sharded(generator, latents, metadata, group=None):
     """Rank-sharded ``generator(*latents, **metadata)``: every rank passes the FULL latent batch
-    (same on all ranks), renders its shard and returns all frames and poses."""
+    (same on all ranks), renders its shard and returns all frames and poses.  Per-image (B, 1) pose tensors in
+    `metadata` are sliced with the latents."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     total = latents[0].shape[0]
     lo, hi = shard_bounds(total, rank, world)
+    metadata = {k: (v[lo:hi] if k in ops.POSE_ARGS and isinstance(v, torch.Tensor) and tuple(v.shape) == (total, 1) else v)
+                for k, v in metadata.items()}
     with torch.no_grad():
         frames, poses = generator(*[z[lo:hi] for z in latents], **metadata)
     return gather_frames(frames, group), gather_frames(poses, group)

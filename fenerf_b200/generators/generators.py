@@ -18,6 +18,7 @@ Hidden keyword extras (never passed by the reference's callers, used by tests an
   _ray_shard  a dist.RayShard: render only its pixel rows of every image and return what its gather makes of them
               (dist.render_sharded_rays)
 """
+import contextlib
 import warnings
 
 import torch
@@ -31,12 +32,19 @@ class _RenderSkeleton:
     """The one render skeleton all reference methods share (generators.py:41-104 etc.)."""
 
     def _render(self, film, batch_size, img_size, fov, ray_start, ray_end, num_steps, h_stddev, v_stddev, h_mean,
-                v_mean, hierarchical_sample, sample_dist, lock_view_dependence, kwargs, staged, grad_points=None):
+                v_mean, hierarchical_sample, sample_dist, lock_view_dependence, kwargs, staged, grad_points=None,
+                pose_grad=False):
+        """pose_grad (forward_with_frequencies): a pose argument that requires grad gets the pose gradient, and makes the
+        render differentiable; elsewhere the poses are read without autograd, as the reference builds them."""
+        poses = (h_stddev, v_stddev, h_mean, v_mean)
+        for name, v in zip(ops.POSE_ARGS, poses):
+            ops.pose_value(name, v, batch_size)
         device = torch.device(self.device)
         if device.type != 'cuda':
             raise RuntimeError("fenerf_b200 renders on CUDA only; move the generator to an H100 (got %s)" % device)
+        pose_grad = pose_grad and ops.pose_requires_grad(*poses)
         rng = kwargs.get('_rng') or vr.DeviceRng(device)
-        with_grad = (not staged) and ops.needs_grad(self.siren, film)
+        with_grad = (not staged) and (pose_grad or ops.needs_grad(self.siren, film))
         if staged:
             # EMA copy_to / restore write through .data: fingerprint-check the packed weights (host sync; the
             # staged methods end in .cpu() anyway)
@@ -46,8 +54,10 @@ class _RenderSkeleton:
         with torch.no_grad():
             # draw #1, then the camera draws (transform_sampled_points, volumetric_rendering.py:147-153)
             rng_perturb = rng.rand(batch_size, n_rays, num_steps, 1)
+        with contextlib.nullcontext() if pose_grad else torch.no_grad():
             cam2world, pitch, yaw = ops.camera_poses(batch_size, sample_dist, h_stddev, v_stddev, h_mean, v_mean, rng,
                                                      device)
+        with torch.no_grad():
             x_lin, y_lin, z_lin = ops.ray_tables(img_size, num_steps, ray_start, ray_end, device)
             rng_noise_c = rng_u = None
             grad_rays = None
@@ -126,7 +136,8 @@ class _RenderSkeleton:
                 if debug is not None:
                     debug.update(depth=depth, weights_sum=wsum, inds=inds, pitch=pitch, yaw=yaw, cam2world=cam2world)
         if with_grad:
-            # the differentiable call (G step, inversion): same kernels forward, backward in fenerf_b200/backward.py
+            # the differentiable call (G step, inversion): same kernels forward, backward in fenerf_b200/backward.py; a
+            # cam2world that requires grad (pose_grad) is one of its inputs
             from .. import backward
             pixels = backward.render_with_grad(self.siren, rd, film, x_lin, y_lin, z_lin, cam2world,
                                                rng_perturb.contiguous(), rng_noise_c, rng_u, rng_noise_f, grad_rays=grad_rays,
@@ -251,7 +262,7 @@ class ImplicitGenerator3d(_RenderSkeleton, nn.Module):
         pixels, _, _, _, pitch, yaw = self._render(
             self._film(frequencies, phase_shifts), frequencies.shape[0], img_size, fov, ray_start, ray_end, num_steps,
             h_stddev, v_stddev, h_mean, v_mean, hierarchical_sample, sample_dist, lock_view_dependence, kwargs,
-            staged=False)
+            staged=False, pose_grad=True)
         return self._finish_pixels(pixels), torch.cat([pitch, yaw], -1)
 
 
@@ -369,7 +380,7 @@ class DoubleImplicitGenerator3d(_RenderSkeleton, nn.Module):
         film = self.siren.film_table(frequencies_geo, frequencies_app, phase_shifts_geo, phase_shifts_app)
         pixels, _, _, _, pitch, yaw = self._render(
             film, batch_size, img_size, fov, ray_start, ray_end, num_steps, h_stddev, v_stddev, h_mean, v_mean,
-            hierarchical_sample, sample_dist, lock_view_dependence, kwargs, staged=False)
+            hierarchical_sample, sample_dist, lock_view_dependence, kwargs, staged=False, pose_grad=True)
         return pixels, torch.cat([pitch, yaw], -1)
 
     def point_forward(self, transformed_points, transformed_ray_directions_expanded, transformed_ray_origins,

@@ -145,17 +145,29 @@ def needs_grad(module, *tensors):
 # --------------------------------------------------------------------------------------------
 # render stages (exposed for stage-level parity tests and for callers that bring their own rays)
 # --------------------------------------------------------------------------------------------
-def camera_poses(n, mode, h_stddev, v_stddev, h_mean, v_mean, rng, device):
-    """Camera pose sampling + look-at matrix in one launch (sample_camera_positions + create_cam2world_matrix,
-    generators/volumetric_rendering.py:170-248).  The draws are made here with `rng` in the reference's order
-    (theta then phi; 'hybrid' first flips Python's `random.random()`); every mode the reference names is
-    covered, anything else means "the mean pose" as in the reference's else-branch.
-    Returns (cam2world (n,4,4), pitch (n,1), yaw (n,1))."""
-    code = _lib.CAMERA_MODE.get(mode, 0)
-    h_stddev, v_stddev, h_mean, v_mean = float(h_stddev), float(v_stddev), float(h_mean), float(v_mean)
+POSE_ARGS = ("h_stddev", "v_stddev", "h_mean", "v_mean")
+
+
+def pose_value(name, v, n):
+    """A camera pose argument of a render of n images: a Python number (-> float), or a tensor of one element or of
+    shape (n, 1) (-> the tensor).  Anything else is a ValueError naming the argument: the reference's (n,) would
+    broadcast to (n, n)."""
+    if not isinstance(v, torch.Tensor):
+        return float(v)
+    if not v.is_floating_point() or not (v.numel() == 1 or tuple(v.shape) == (n, 1)):
+        raise ValueError("%s must be a number, or a floating-point tensor of one element or of shape (B, 1) = (%d, 1); "
+                         "got %s of shape %s" % (name, n, v.dtype, tuple(v.shape)))
+    return v
+
+
+def camera_draws(n, mode, rng):
+    """The camera draws of sample_camera_positions in the reference's order -> (kernel mode, doubled, draw_theta,
+    draw_phi): 'hybrid' flips Python's `random.random()` first and is then 'uniform' with doubled stddevs (doubled=True)
+    or 'gaussian'; a mode the reference does not name is the mean pose (no draws)."""
+    code, doubled = _lib.CAMERA_MODE.get(mode, 0), False
     if mode == "hybrid":
         if rng.coin() < 0.5:
-            code, h_stddev, v_stddev = 1, 2 * h_stddev, 2 * v_stddev
+            code, doubled = 1, True
         else:
             code = 2
     d_theta = d_phi = None
@@ -165,18 +177,73 @@ def camera_poses(n, mode, h_stddev, v_stddev, h_mean, v_mean, rng, device):
         d_theta, d_phi = rng.randn(n, 1), rng.randn(n, 1)
     elif code == 3:
         d_theta, d_phi = rng.randn(n, 1, 4), rng.randn(n, 1, 4)
-    if code == 4:
-        v_stddev, v_mean = v_stddev / math.pi, v_mean / math.pi
+    return code, doubled, d_theta, d_phi
+
+
+def camera_kernel_values(code, doubled, values, device):
+    """The four pose values (POSE_ARGS order; numbers or tensors) as fenerf_camera_poses_dev reads them: float32 device
+    tensors of one entry or one per image, hybrid's stddevs doubled, spherical_uniform's v_stddev and v_mean divided by
+    pi -- on each tensor's own device and dtype, as the reference's tensor arithmetic does -> (tensors, per_image mask)."""
+    out, per_image = [], 0
+    for k, v in enumerate(values):
+        if doubled and k < 2:
+            v = 2 * v
+        if code == 4 and k % 2 == 1:
+            v = v / math.pi
+        if isinstance(v, torch.Tensor):
+            t = v.detach().to(device=device, dtype=torch.float32).reshape(-1).contiguous()
+        else:
+            t = torch.tensor([v], dtype=torch.float32, device=device)
+        if t.numel() > 1:
+            per_image |= 1 << k
+        out.append(t)
+    return out, per_image
+
+
+def camera_poses_launch(n, code, doubled, values, d_theta, d_phi, device):
+    """One camera_kernel launch -> (cam2world (n,4,4), pitch (n,1), yaw (n,1)).  All-number poses go through
+    fenerf_camera_poses as arguments, any tensor through fenerf_camera_poses_dev (no host read)."""
     c2w = torch.empty((n, 4, 4), dtype=torch.float32, device=device)
     pitch = torch.empty((n, 1), dtype=torch.float32, device=device)
     yaw = torch.empty((n, 1), dtype=torch.float32, device=device)
+    draws = (_chk(d_theta.contiguous(), "draw_theta", device) if d_theta is not None else 0,
+             _chk(d_phi.contiguous(), "draw_phi", device) if d_phi is not None else 0)
     with torch.cuda.device(device):
-        _lib.check(_lib.lib().fenerf_camera_poses(
-            n, code, h_stddev, v_stddev, h_mean, v_mean,
-            _chk(d_theta.contiguous(), "draw_theta", device) if d_theta is not None else 0,
-            _chk(d_phi.contiguous(), "draw_phi", device) if d_phi is not None else 0,
-            c2w.data_ptr(), pitch.data_ptr(), yaw.data_ptr(), _stream(device)))
+        if not any(isinstance(v, torch.Tensor) for v in values):
+            h_stddev, v_stddev, h_mean, v_mean = values
+            if doubled:
+                h_stddev, v_stddev = 2 * h_stddev, 2 * v_stddev
+            if code == 4:
+                v_stddev, v_mean = v_stddev / math.pi, v_mean / math.pi
+            _lib.check(_lib.lib().fenerf_camera_poses(n, code, h_stddev, v_stddev, h_mean, v_mean, *draws, c2w.data_ptr(),
+                                                      pitch.data_ptr(), yaw.data_ptr(), _stream(device)))
+        else:
+            vals, per_image = camera_kernel_values(code, doubled, values, device)
+            _lib.check(_lib.lib().fenerf_camera_poses_dev(n, code, *[t.data_ptr() for t in vals], per_image, *draws,
+                                                          c2w.data_ptr(), pitch.data_ptr(), yaw.data_ptr(), _stream(device)))
     return c2w, pitch, yaw
+
+
+def camera_poses(n, mode, h_stddev, v_stddev, h_mean, v_mean, rng, device):
+    """Camera pose sampling + look-at matrix in one launch (sample_camera_positions + create_cam2world_matrix,
+    generators/volumetric_rendering.py:170-248).  The draws are made here with `rng` in the reference's order
+    (theta then phi; 'hybrid' first flips Python's `random.random()`); every mode the reference names is
+    covered, anything else means "the mean pose" as in the reference's else-branch.
+    Each pose argument is a Python number, a one-element tensor or an (n, 1) tensor (one value per image); tensors are
+    read on the device.  Under autograd, a tensor that requires grad gets the gradient of cam2world, pitch and yaw
+    (fenerf_b200.poses.CameraPoses).  Returns (cam2world (n,4,4), pitch (n,1), yaw (n,1))."""
+    values = tuple(pose_value(k, v, n) for k, v in zip(POSE_ARGS, (h_stddev, v_stddev, h_mean, v_mean)))
+    code, doubled, d_theta, d_phi = camera_draws(n, mode, rng)
+    if pose_requires_grad(*values):
+        from . import poses
+        return poses.CameraPoses.apply(dict(n=n, code=code, doubled=doubled, d_theta=d_theta, d_phi=d_phi, device=device),
+                                       *values)
+    return camera_poses_launch(n, code, doubled, values, d_theta, d_phi, device)
+
+
+def pose_requires_grad(*values):
+    """True when a pose argument is a tensor that autograd would differentiate."""
+    return torch.is_grad_enabled() and any(isinstance(v, torch.Tensor) and v.requires_grad for v in values)
 
 
 _TABLES = {}

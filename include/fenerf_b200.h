@@ -274,6 +274,12 @@ typedef struct fenerf_render_desc {
 int fenerf_camera_poses(int32_t n, int32_t mode, float h_stddev, float v_stddev, float h_mean, float v_mean,
                         const float* draw_theta, const float* draw_phi, float* cam2world, float* pitch, float* yaw,
                         void* stream);
+/* fenerf_camera_poses with the pose values in DEVICE memory (no host read): h_stddev, v_stddev, h_mean, v_mean each hold
+ * one value, or one per image when bit 0, 1, 2, 3 of per_image is set.  The same arithmetic as fenerf_camera_poses (one
+ * device function), so equal values give equal bits; SPHERICAL_UNIFORM's v_stddev, v_mean come pre-divided by pi. */
+int fenerf_camera_poses_dev(int32_t n, int32_t mode, const float* h_stddev, const float* v_stddev, const float* h_mean,
+                            const float* v_mean, int32_t per_image, const float* draw_theta, const float* draw_phi,
+                            float* cam2world, float* pitch, float* yaw, void* stream);
 
 /* Camera rays, stratified perturbation and camera-to-world transform.
  * Replaces get_initial_rays_trig + perturb_points + the three bmm of transform_sampled_points
@@ -285,6 +291,22 @@ int fenerf_camera_poses(int32_t n, int32_t mode, float h_stddev, float v_stddev,
 int fenerf_ray_setup(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin,
                      const float* z_lin, const float* cam2world, const float* rng_perturb,
                      float* points, float* z_vals, float* dirs, float* origins, void* stream);
+
+/* Gradient of a camera render w.r.t. its cam2world matrices (forward_with_frequencies with a pose that requires grad).
+ * Per image b: d cam2world_b = [dR | dT] over rows 0..2 (row 3 written 0), with
+ *   dR = sum_samples dx p_cam^T + sum_rays d_dir d_cam^T,   dT = sum_samples dx
+ * where p_cam, d_cam are the camera-space sample point and ray direction, recomputed from x_lin, y_lin, z_lin and
+ * rng_perturb with fenerf_ray_setup's operations (rd, x_lin ... rng_perturb: its arguments).
+ *   d_points  (B, N, S, 3) the gradient of the coarse sample points times 1 / (*inv_scale) / input_scale (the backward's
+ *             scaled stream, before the point network's input_scale); multiplied back here
+ *   d_dirs    (B, N, 3) the gradient of the world ray directions (fenerf_ray_dir_grad with dir_group num_steps), or NULL
+ *   workspace fenerf_cam2world_grad_workspace_bytes(rd) bytes, 8-byte aligned
+ * Sums run in fp64 in a fixed order (no atomics): the same inputs give the same bits from call to call.  A window of
+ * pixel rows (img_h rows, y_lin its slice) gives that window's share. */
+size_t fenerf_cam2world_grad_workspace_bytes(const fenerf_render_desc* rd);
+int fenerf_cam2world_grad(const fenerf_render_desc* rd, const float* x_lin, const float* y_lin, const float* z_lin,
+                          const float* rng_perturb, const float* d_points, const float* d_dirs, const float* inv_scale,
+                          float input_scale, void* workspace, size_t workspace_bytes, float* d_cam2world, void* stream);
 
 /* Coarse weights + inverse-CDF resampling + fine points.
  * Replaces fancy_integration(coarse) -> weights, the resample prep and sample_pdf
