@@ -698,12 +698,6 @@ class _FieldBackward:
         return d_film, grads
 
 
-def _save_inputs(ctx, call, film, params):
-    ctx.call = call
-    ctx.save_for_backward(film, *params)
-    ctx.param_ids = [id(p) for p in call['params']]
-
-
 def _field_backward(call, film, d_raw_c, d_raw_f):
     """The _FieldBackward of a render: its precision and grad_precision, the fp16 stream's scale a power of two taken from
     max |d raw| on the device (no host sync)."""
@@ -719,31 +713,43 @@ def _field_backward(call, film, d_raw_c, d_raw_f):
                           grad_split=call.get('grad_precision') == 'split')
 
 
-def _input_grads(ctx, d_film, grads):
-    """The backward's outputs for film, call and the field parameters."""
-    out = [d_film if ctx.needs_input_grad[0] else None, None]
-    for i, pid in enumerate(ctx.param_ids):
-        g = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
-        if g is not None:
-            g = g.reshape(ctx.saved_tensors[1 + i].shape)
-        out.append(g)
-    return out
+#: the ray set-up inputs of a camera render, and the ray tensors of a rays-in render in the order RenderFunction takes them
+#: with ray_grad
+CAMERA_INPUTS = ("x_lin", "y_lin", "z_lin", "cam2world", "rng_perturb")
+RAY_INPUTS = ("points", "dirs", "origins", "ray_dirs", "z_vals")
 
 
 class RenderFunction(torch.autograd.Function):
-    """pixels = render(film, field parameters); see the module docstring.  With call['pose_grad'] the cam2world matrices
-    follow the parameters as an input and get the gradient of the coarse sample points R p_cam + T and of the ray
-    directions R d_cam of both passes (fenerf_cam2world_grad); the fine points, the depths and the origins carry none, as
-    in the reference."""
+    """pixels = render(film, field parameters); see the module docstring.  One node for both renders:
+      camera   (call from render_with_grad) fenerf_render_forward, NCHW pixels.  A cam2world that requires grad follows the
+               parameters as an input and gets the gradient of the coarse sample points R p_cam + T
+               and of the ray directions R d_cam of both passes (fenerf_cam2world_grad); the fine points, the depths and
+               the origins carry none, as in the reference.
+      rays-in  (call from render_rays_with_grad) fenerf_render_rays, (B, N, C-1) ray-major pixels
+               (DoubleImplicitGenerator3d.point_forward).  With ray_grad the ray tensors (RAY_INPUTS) follow the
+               parameters as inputs and get the reference's gradients: the coarse points, the directions (both passes;
+               the fine samples' through their draw slots), the depths without hierarchical sampling, and None for the
+               per-ray origins and directions.
+    The two differ in where the rays come from, the compositing backward of their pixel layout, which passes
+    lock_view_dependence locks and where the ray gradients go; the rest of the backward is one path."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type='cuda', cast_inputs=torch.float32)
     def forward(ctx, film, call, *inputs):
         module, rd = call['module'], call['rd']
-        st = ops.render_forward_stages(module, rd, film, call['x_lin'], call['y_lin'], call['z_lin'], call['cam2world'],
-                                       call['rng_perturb'], call['rng_noise_c'], call['rng_u'], call['rng_noise_f'])
-        ctx.stages = st
-        _save_inputs(ctx, call, film, inputs[:len(call['params'])])
+        n_params = len(call['params'])
+        extra = inputs[n_params:]           # the cam2world that requires grad, or the ray tensors (ray_grad)
+        draws = (call['rng_noise_c'], call['rng_u'], call['rng_noise_f'])
+        if 'cam2world' in call:
+            st = ops.render_forward_stages(module, rd, film, *(call[k] for k in CAMERA_INPUTS), *draws)
+        else:
+            # the fine samples' draw slots: only for a backward w.r.t. the directions
+            slots = bool(extra) and ctx.needs_input_grad[2 + n_params + 1]
+            st = ops.render_rays_stages(module, rd, film, *(extra or (call[k] for k in RAY_INPUTS)), *draws, slots=slots)
+        ctx.call, ctx.stages = call, st
+        ctx.save_for_backward(film, *inputs[:n_params])
+        ctx.param_ids = [id(p) for p in call['params']]
+        ctx.extra_meta = [(t.shape, t.dtype) if t is not None else None for t in extra]
         return st['pixels']
 
     @staticmethod
@@ -754,27 +760,45 @@ class RenderFunction(torch.autograd.Function):
         rd = call['rd']
         dev = film.device
         lib = _lib.lib()
+        camera = 'cam2world' in call
         B, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
         c = st['raw_c'].shape[-1]
         hier = bool(rd.hierarchical)
+        n_params = len(ctx.param_ids)
+        need = ctx.needs_input_grad[2 + n_params:] + (False,) * len(RAY_INPUTS)     # (inputs the call lacks want none)
+        spec = call['module'].field_spec()
+        rays = call.get('grad_rays')
+        # the consumer of the ray gradients: d cam2world reads d points and d directions; a rays-in render's caller takes
+        # each ray tensor that requires grad (the direction-free field never reads directions; the depths get a gradient
+        # only without hierarchical sampling)
+        want_dx = need[0]
+        want_dirs = need[0 if camera else 1] and not spec.wo_dir
+        want_z = not camera and need[4] and not hier
+        # lock_view_dependence locks both passes of a camera render, only the fine pass of a rays-in render: the coarse
+        # pass keeps the caller's directions whatever it says (generators.py:810)
+        lock_f = bool(rd.lock_view_dependence)
+        lock_c = lock_f and camera
         d_pixels = d_pixels.float().contiguous()
         with torch.cuda.device(dev), torch.no_grad():
             d_raw_c = torch.empty_like(st['raw_c'])
             d_raw_f = torch.empty_like(st['raw_f']) if hier else None
             noise = call['rng_noise_f'] if rd.noise_std != 0.0 else None
-            if call.get('grad_rays') is not None:
+            if rays is not None:
                 # gradient only through the chosen rays: the others were rendered under no_grad in the reference
                 mask = torch.zeros(n, dtype=torch.bool, device=dev)
-                mask[call['grad_rays']] = True
+                mask[rays] = True
                 d_pixels = d_pixels * mask.reshape(1, 1, rd.img_h, rd.img_w)
-            _lib.check(lib.fenerf_composite_backward(
-                C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
-                _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
-                _stream(dev)))
+            d_z = None
+            if want_z:     # the same d raw, and the depth gradient beside it
+                d_z = torch.empty_like(st['z_c'])
+                _lib.check(lib.fenerf_composite_backward_rays_dz(
+                    C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(noise), d_pixels.data_ptr(),
+                    d_raw_c.data_ptr(), d_z.data_ptr(), _stream(dev)))
+            else:
+                _lib.check((lib.fenerf_composite_backward if camera else lib.fenerf_composite_backward_rays)(
+                    C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']), _ptr(st['z_f']),
+                    _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f), _stream(dev)))
             fb = _field_backward(call, film, d_raw_c, d_raw_f)
-            lock = bool(rd.lock_view_dependence)
-            rays = call.get('grad_rays')
-            dirs = st['dirs']
 
             def pick(t, last):
                 # (B, n, s, last) -> (B, n' * s, last): every ray, or only the rays that carry a gradient (part_forward)
@@ -782,149 +806,58 @@ class RenderFunction(torch.autograd.Function):
                     t = t.index_select(1, rays)
                 return t.reshape(B, -1, last)
 
-            if rays is not None:
-                dirs = dirs.index_select(1, rays).contiguous()
-            # the pose gradient: d sample points of the coarse pass, d direction per point of both passes (none under
-            # lock_view_dependence or for the direction-free field)
-            pose = bool(call.get('pose_grad')) and ctx.needs_input_grad[2 + len(ctx.param_ids)]
-            dx = dir_c = dir_f = None
-            if pose:
-                dx = torch.zeros((B, n * s, 3), dtype=torch.float32, device=dev)
-                if not lock and not fb.spec.wo_dir:
-                    dir_c = torch.zeros_like(dx)
-                    dir_f = torch.zeros_like(dx) if hier else None
+            dirs_c = st['dirs'] if rays is None else st['dirs'].index_select(1, rays).contiguous()
+            # the fine pass: a rays-in render's fine samples' own directions (per-sample), else the coarse pass's
+            dirs_f = st['dirs_f'] if st['dirs_f'] is not None else dirs_c
+            g = st['dir_group']
+
+            def buf():
+                return torch.zeros((B, n * s, 3), dtype=torch.float32, device=dev)
+
+            # d points of the coarse pass, d direction per point of each pass that reads unlocked directions
+            dx = buf() if want_dx else None
+            dir_c = buf() if want_dirs and not lock_c else None
+            dir_f = buf() if want_dirs and hier and not lock_f else None
             if hier:
-                fb.add_points(pick(st['points_f'], 3), dirs, s, lock, pick(st['raw_f'], c), pick(d_raw_f, c),
+                fb.add_points(pick(st['points_f'], 3), dirs_f, g, lock_f, pick(st['raw_f'], c), pick(d_raw_f, c),
                               ray_grad=dict(ddir=dir_f) if dir_f is not None else None)
-            fb.add_points(pick(st['points_c'], 3), dirs, s, lock, pick(st['raw_c'], c), pick(d_raw_c, c),
-                          ray_grad=dict(dx=dx, ddir=dir_c) if pose else None)
+            fb.add_points(pick(st['points_c'], 3), dirs_c, g, lock_c, pick(st['raw_c'], c), pick(d_raw_c, c),
+                          ray_grad=dict(dx=dx, ddir=dir_c) if (dx is not None or dir_c is not None) else None)
             d_film, grads = fb.finish()
-            d_c2w = _cam2world_grad(call, fb, dx, dir_c, dir_f) if pose else None
+            d_dirs = None
+            if dir_c is not None:     # the directions' gradients per ray (dir_group S) or per sample
+                d_dirs = torch.empty((B * n * s // g, 3), dtype=torch.float32, device=dev)
+                _lib.check(lib.fenerf_ray_dir_grad(B * n, s, g, dir_c.data_ptr(), _ptr(dir_f),
+                                                   _ptr(st['slots_f']) if dir_f is not None else 0,
+                                                   fb.inv_scale.data_ptr(), d_dirs.data_ptr(), _stream(dev)))
+            if camera:
+                extra = [_cam2world_grad(call, fb, dx, d_dirs) if want_dx else None]
+            else:
+                extra = [dx * fb.inv_scale * spec.input_scale if dx is not None else None, d_dirs, None, None, d_z]
             if call.get('grad_reduce') is not None:
-                call['grad_reduce']([d_film] + list(grads.values()) + [d_c2w])
-        out = _input_grads(ctx, d_film, grads)
-        if call.get('pose_grad'):
-            out.append(d_c2w)
+                call['grad_reduce']([d_film] + list(grads.values()) + [extra[0] if camera else None])
+        out = [d_film if ctx.needs_input_grad[0] else None, None]
+        for i, pid in enumerate(ctx.param_ids):
+            gr = grads.get(pid) if ctx.needs_input_grad[2 + i] else None
+            out.append(gr.reshape(ctx.saved_tensors[1 + i].shape) if gr is not None else None)
+        for gr, meta, want in zip(extra, ctx.extra_meta, need):
+            out.append(gr.reshape(meta[0]).to(meta[1]) if gr is not None and want else None)
         return tuple(out)
 
 
-def _cam2world_grad(call, fb, dx, dir_c, dir_f):
-    """d cam2world (B, 4, 4) of a camera render from the coarse pass's d points `dx` and the per-point direction
-    gradients of both passes (scaled stream units): the directions' per-ray sums (fenerf_ray_dir_grad), then
+def _cam2world_grad(call, fb, dx, d_dirs):
+    """d cam2world (B, 4, 4) of a camera render from the coarse pass's d points `dx` (scaled stream units) and the
+    directions' per-ray gradients d_dirs (fenerf_ray_dir_grad; None: no direction is differentiated):
     fenerf_cam2world_grad, which recomputes the camera-space samples."""
     rd, dev = call['rd'], fb.dev
-    B, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
     lib = _lib.lib()
-    d_dirs = None
-    if dir_c is not None:
-        d_dirs = torch.empty((B * n, 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.fenerf_ray_dir_grad(B * n, s, s, dir_c.data_ptr(), _ptr(dir_f), 0, fb.inv_scale.data_ptr(),
-                                           d_dirs.data_ptr(), _stream(dev)))
     ws = torch.empty(lib.fenerf_cam2world_grad_workspace_bytes(C.byref(rd)), dtype=torch.uint8, device=dev)
-    d_c2w = torch.empty((B, 4, 4), dtype=torch.float32, device=dev)
+    d_c2w = torch.empty((rd.batch, 4, 4), dtype=torch.float32, device=dev)
     _lib.check(lib.fenerf_cam2world_grad(
         C.byref(rd), call['x_lin'].data_ptr(), call['y_lin'].data_ptr(), call['z_lin'].data_ptr(),
         call['rng_perturb'].data_ptr(), dx.data_ptr(), _ptr(d_dirs), fb.inv_scale.data_ptr(), fb.spec.input_scale,
         ws.data_ptr(), ws.numel(), d_c2w.data_ptr(), _stream(dev)))
     return d_c2w
-
-
-class RaysRenderFunction(torch.autograd.Function):
-    """pixels (B, N, C-1) = render of caller-supplied rays (fenerf_render_rays; DoubleImplicitGenerator3d.point_forward),
-    differentiable w.r.t. `film` and the field parameters; with call['ray_grad'] the ray tensors (points, dirs, origins,
-    ray_dirs, z_vals) follow the parameters as inputs and get the reference's gradients: the coarse points, the
-    directions (both passes; the fine samples' through their draw slots), the depths without hierarchical sampling, and
-    None for the per-ray origins and directions.  The backward is RenderFunction's with the ray-major compositing
-    backward and the caller's directions."""
-
-    @staticmethod
-    @torch.amp.custom_fwd(device_type='cuda', cast_inputs=torch.float32)
-    def forward(ctx, film, call, *inputs):
-        module, rd = call['module'], call['rd']
-        n_params = len(call['params'])
-        rays = inputs[n_params:] if call.get('ray_grad') else None
-        points, dirs, origins, ray_dirs, z_vals = rays if rays else (call[k] for k in RAY_INPUTS)
-        # the fine samples' draw slots: only for a backward w.r.t. the directions
-        slots = bool(rays) and ctx.needs_input_grad[2 + n_params + 1]
-        st = ops.render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, call['rng_noise_c'],
-                                    call['rng_u'], call['rng_noise_f'], slots=slots)
-        ctx.stages = st
-        _save_inputs(ctx, call, film, inputs[:n_params])
-        ctx.ray_meta = [(t.shape, t.dtype) if t is not None else None for t in rays] if rays else None
-        return st['pixels']
-
-    @staticmethod
-    @torch.amp.custom_bwd(device_type='cuda')
-    def backward(ctx, d_pixels):
-        call, st = ctx.call, ctx.stages
-        film = ctx.saved_tensors[0]
-        module, rd = call['module'], call['rd']
-        dev = film.device
-        B, s = rd.batch, rd.num_steps
-        c = st['raw_c'].shape[-1]
-        hier = bool(rd.hierarchical)
-        n_params = len(ctx.param_ids)
-        need = ctx.needs_input_grad[2 + n_params:] if ctx.ray_meta else (False,) * len(RAY_INPUTS)
-        spec = module.field_spec()
-        want_points, want_z = need[0], need[4] and not hier
-        want_dirs = need[1] and not spec.wo_dir        # the direction-free field never reads them
-        d_pixels = d_pixels.float().contiguous()
-        with torch.cuda.device(dev), torch.no_grad():
-            d_raw_c = torch.empty_like(st['raw_c'])
-            d_raw_f = torch.empty_like(st['raw_f']) if hier else None
-            noise = call['rng_noise_f'] if rd.noise_std != 0.0 else None
-            d_z = None
-            if want_z:     # the same d raw, and the depth gradient beside it
-                d_z = torch.empty_like(st['z_c'])
-                _lib.check(_lib.lib().fenerf_composite_backward_rays_dz(
-                    C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(noise), d_pixels.data_ptr(),
-                    d_raw_c.data_ptr(), d_z.data_ptr(), _stream(dev)))
-            else:
-                _lib.check(_lib.lib().fenerf_composite_backward_rays(
-                    C.byref(rd), c, st['raw_c'].data_ptr(), st['z_c'].data_ptr(), _ptr(st['raw_f']) if hier else 0,
-                    _ptr(st['z_f']) if hier else 0, _ptr(noise), d_pixels.data_ptr(), d_raw_c.data_ptr(), _ptr(d_raw_f),
-                    _stream(dev)))
-            fb = _field_backward(call, film, d_raw_c, d_raw_f)
-            g = st['dir_group']
-            lock = bool(rd.lock_view_dependence)
-            pc = B * rd.img_w * s
-
-            def buf():
-                return torch.zeros((B, pc // B, 3), dtype=torch.float32, device=dev)
-
-            dir_f = buf() if want_dirs and hier and not lock else None
-            dir_c = buf() if want_dirs else None
-            dx = buf() if want_points else None
-            if hier:
-                # the fine pass: the fine samples' own directions (per-sample), the per-ray ones, or (0, 0, -1)
-                dirs_f = st['dirs_f'] if st['dirs_f'] is not None else st['dirs']
-                fb.add_points(st['points_f'].reshape(B, -1, 3), dirs_f, g, lock, st['raw_f'].reshape(B, -1, c),
-                              d_raw_f.reshape(B, -1, c), ray_grad=dict(ddir=dir_f) if dir_f is not None else None)
-            # the coarse pass keeps the caller's directions whatever lock_view_dependence says
-            fb.add_points(st['points_c'].reshape(B, -1, 3), st['dirs'], g, False, st['raw_c'].reshape(B, -1, c),
-                          d_raw_c.reshape(B, -1, c),
-                          ray_grad=dict(dx=dx, ddir=dir_c) if (dx is not None or dir_c is not None) else None)
-            d_film, grads = fb.finish()
-            ray_grads = [None] * len(RAY_INPUTS)
-            if dx is not None:
-                ray_grads[0] = dx * fb.inv_scale * spec.input_scale
-            if dir_c is not None:
-                d_dirs = torch.empty((B * rd.img_w * s // g, 3), dtype=torch.float32, device=dev)
-                _lib.check(_lib.lib().fenerf_ray_dir_grad(B * rd.img_w, s, g, dir_c.data_ptr(), _ptr(dir_f),
-                                                          _ptr(st['slots_f']) if dir_f is not None else 0,
-                                                          fb.inv_scale.data_ptr(), d_dirs.data_ptr(), _stream(dev)))
-                ray_grads[1] = d_dirs
-            if d_z is not None:
-                ray_grads[4] = d_z
-        out = _input_grads(ctx, d_film, grads)
-        if ctx.ray_meta:
-            for gr, meta, want in zip(ray_grads, ctx.ray_meta, need):
-                out.append(gr.reshape(meta[0]).to(meta[1]) if gr is not None and want else None)
-        return tuple(out)
-
-
-#: the ray tensors of a rays-in render, in the order RaysRenderFunction takes them with ray_grad
-RAY_INPUTS = ("points", "dirs", "origins", "ray_dirs", "z_vals")
 
 
 #: what a rays-in render refuses to differentiate
@@ -946,16 +879,15 @@ def render_rays_with_grad(module, rd, film, points, dirs, origins, ray_dirs, z_v
                           grad_precision=None, ray_grad=False):
     """Differentiable render of caller-supplied rays (rd from ops.make_rays_desc): (B, N, C-1) pixels with autograd
     edges to `film` and the field parameters.  `grad_precision` as render_with_grad.  ray_grad=True: also to the ray
-    tensors (RaysRenderFunction); without it a ray tensor that requires grad is refused."""
+    tensors (RenderFunction); without it a ray tensor that requires grad is refused."""
     check_grad_precision(module, grad_precision, rd.precision)
     if not ray_grad:
         check_rays_no_grad(points=points, directions=dirs, origins=origins, ray_directions=ray_dirs, z_vals=z_vals)
     params = FieldWeights(module).parameters()
     call = dict(module=module, rd=rd, points=points, dirs=dirs, origins=origins, ray_dirs=ray_dirs, z_vals=z_vals,
-                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_precision=grad_precision,
-                ray_grad=bool(ray_grad))
+                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params, grad_precision=grad_precision)
     rays = (points, dirs, origins, ray_dirs, z_vals) if ray_grad else ()
-    return RaysRenderFunction.apply(film, call, *params, *rays)
+    return RenderFunction.apply(film, call, *params, *rays)
 
 
 def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
@@ -974,5 +906,5 @@ def render_with_grad(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_pertu
         raise ValueError("fenerf_b200: the pose gradient is not built for ray subsets (grad_rays)")
     call = dict(module=module, rd=rd, x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world.detach(),
                 rng_perturb=rng_perturb, rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f, params=params,
-                grad_rays=grad_rays, grad_precision=grad_precision, grad_reduce=grad_reduce, pose_grad=pose_grad)
+                grad_rays=grad_rays, grad_precision=grad_precision, grad_reduce=grad_reduce)
     return RenderFunction.apply(film, call, *params, *((cam2world,) if pose_grad else ()))

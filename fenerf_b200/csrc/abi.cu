@@ -13,53 +13,37 @@ using namespace fn;
 
 namespace {
 
+// The workspace of every render.  A camera render (fenerf_render_forward) keeps its ray set-up there: points_c, z_c,
+// dirs, origins.  A rays-in render (fenerf_render_rays, `rays`) reads those from the caller and keeps the fine samples'
+// per-sample directions in dirs_f instead (per_sample_f); fine_slots (fenerf_render_rays_grad only): each
+// fine sample's draw slot, appended after the other sections (0: none).  Sections a render lacks stay at offset 0.
 struct Workspace {
-    size_t stats, points_c, z_c, dirs, origins, raw_c, z_f, points_f, raw_f, guard, sigma_c, total;
+    size_t stats, points_c, z_c, dirs, origins, raw_c, z_f, points_f, dirs_f, raw_f, guard, sigma_c, fine_slots, total;
+    bool per_sample_f;
 };
 
-Workspace plan_workspace(const fenerf_render_desc* rd, int C) {
-    Workspace w;
+Workspace plan_workspace(const fenerf_render_desc* rd, int C, bool rays = false, int dir_group = 0, bool grad = false) {
+    Workspace w{};
     size_t n_rays = (size_t)rd->batch * rd->img_h * rd->img_w;
     size_t pc = n_rays * rd->num_steps;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = fn_align_up(off + bytes, 256); return o; };
+    w.per_sample_f = rays && rd->hierarchical && dir_group == 1 && !rd->lock_view_dependence;
     w.stats = take(64);               // always at offset 0: fenerf_guard_stats
-    w.points_c = take(pc * 3 * 4);
-    w.z_c = take(pc * 4);
-    w.dirs = take(n_rays * 3 * 4);
-    w.origins = take((size_t)rd->batch * 3 * 4);
+    if (!rays) {
+        w.points_c = take(pc * 3 * 4);
+        w.z_c = take(pc * 4);
+        w.dirs = take(n_rays * 3 * 4);
+        w.origins = take((size_t)rd->batch * 3 * 4);
+    }
     w.raw_c = take(pc * C * 4);
     w.z_f = take(rd->hierarchical ? pc * 4 : 4);
     w.points_f = take(rd->hierarchical ? pc * 3 * 4 : 4);
+    if (rays) w.dirs_f = take(w.per_sample_f ? pc * 3 * 4 : 4);
     w.raw_f = take(rd->hierarchical ? pc * C * 4 : 4);
     w.guard = take((n_rays + 1) * 4);
     w.sigma_c = take(pc * 4);
-    w.total = off;
-    return w;
-}
-
-// fenerf_render_rays: the coarse inputs are the caller's; dirs_f holds the fine samples' per-sample directions
-// fine_slots (fenerf_render_rays_grad only): each fine sample's draw slot, appended after the other sections
-struct RaysWorkspace {
-    size_t stats, raw_c, z_f, points_f, dirs_f, raw_f, guard, sigma_c, total, fine_slots;
-};
-
-RaysWorkspace plan_rays_workspace(const fenerf_render_desc* rd, int C, int dir_group, bool grad = false) {
-    RaysWorkspace w;
-    size_t n_rays = (size_t)rd->batch * rd->img_h * rd->img_w;
-    size_t pc = n_rays * rd->num_steps;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off = fn_align_up(off + bytes, 256); return o; };
-    const bool dirs_f = rd->hierarchical && dir_group == 1 && !rd->lock_view_dependence;
-    w.stats = take(64);               // always at offset 0: fenerf_guard_stats
-    w.raw_c = take(pc * C * 4);
-    w.z_f = take(rd->hierarchical ? pc * 4 : 4);
-    w.points_f = take(rd->hierarchical ? pc * 3 * 4 : 4);
-    w.dirs_f = take(dirs_f ? pc * 3 * 4 : 4);
-    w.raw_f = take(rd->hierarchical ? pc * C * 4 : 4);
-    w.guard = take((n_rays + 1) * 4);
-    w.sigma_c = take(pc * 4);
-    w.fine_slots = grad && dirs_f ? take(pc) : 0;
+    if (grad && w.per_sample_f) w.fine_slots = take(pc);
     w.total = off;
     return w;
 }
@@ -126,6 +110,105 @@ int run_field(const FnLayout& L, const void* packed, const float* points, const 
         return siren_points_split(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
     // the wgmma kernel (siren_fast.cu)
     return siren_points_fast(L, pk, points, dirs, film, batch, ppb, dir_group, lock_dirs, out, sigma_only, st, sigma_out);
+}
+
+// The checks every render makes after its own, and the size of its workspace
+int check_pipeline(const fenerf_render_desc* rd, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f,
+                   const void* workspace, size_t workspace_bytes, const Workspace& w) {
+    FN_REQUIRE(!rd->hierarchical || rng_u, "hierarchical render needs rng_u");
+    FN_REQUIRE(!rd->hierarchical || rd->num_steps >= 3, "hierarchical render needs num_steps >= 3");
+    FN_REQUIRE(rd->noise_std == 0.f || (rng_noise_f && (!rd->hierarchical || rng_noise_c)), "noise_std != 0 needs the noise draws");
+    FN_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    if (workspace_bytes < w.total) return fail(FENERF_E_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, w.total);
+    return 0;
+}
+
+// The coarse samples a render starts from: a camera render's ray_setup outputs in the workspace, or the caller's rays
+struct CoarseRays {
+    const float* points;        // (B, N, S, 3)
+    const float* z;             // (B, N, S)
+    const float* dirs;          // (B, N*S/dir_group, 3)
+    int dir_group;
+    int lock;                   // lock_view_dependence of the coarse pass: a camera render's; a rays-in render keeps the
+                                // caller's directions there whatever it says (generators.py:810)
+    const float* origins;       // the fine points' origins: (B, 3) one per image, or NULL and
+    const float* ray_origins;   //   (B, N, 3) one per ray
+    const float* ray_dirs;      // (B, N, 3) the fine points' directions
+};
+
+// The render after ray set-up: coarse field, GUARD refinement, resampling, fine field, compositing.  Outputs as
+// fenerf_composite (NCHW x2-1, fill modes, per-sample weights; stage timing marks 2..6 of fenerf_render_forward), or with
+// ray_major as fenerf_render_rays: (B, N, C-1) in [0, 1].
+int render_pipeline(const fenerf_render_desc* rd, const FnLayout& L, const void* packed, const float* film,
+                    const CoarseRays& r, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f,
+                    unsigned char* ws, const Workspace& w, bool ray_major, float* pixels, float* depth, float* weights_sum,
+                    float* weights, int64_t* inds, cudaStream_t st) {
+    const int C = L.out_dim;
+    const long long rays = (long long)rd->img_h * rd->img_w;
+    const long long ppb = rays * rd->num_steps;
+    const float* noise_c = rd->noise_std != 0.f ? rng_noise_c : nullptr;
+    const float* noise_f = rd->noise_std != 0.f ? rng_noise_f : nullptr;
+    float* raw_c = (float*)(ws + w.raw_c);
+    float* z_f = (float*)(ws + w.z_f);
+    float* points_f = (float*)(ws + w.points_f);
+    float* dirs_f = w.per_sample_f ? (float*)(ws + w.dirs_f) : nullptr;
+    float* raw_f = (float*)(ws + w.raw_f);
+    auto mark = [&](int i) { if (!ray_major) stage_mark(i, st); };
+
+    // the wgmma pass also leaves the densities as one float per point for the resampler (which never reads the far
+    // sample, so the GUARD refinement of raw_c below does not concern that copy)
+    float* sigma_c = (rd->hierarchical && rd->precision != FENERF_PRECISION_EXACT) ? (float*)(ws + w.sigma_c) : nullptr;
+    if (int e = run_field(L, packed, r.points, r.dirs, film, rd->batch, ppb, r.dir_group, r.lock, rd->precision, raw_c, st, 0,
+                          sigma_c)) return e;
+    mark(2);
+    if (rd->precision == FENERF_PRECISION_GUARD) {
+        float tau = rd->guard_tau > 0.f ? rd->guard_tau : 1.5e-3f;
+        const int n_samples = rd->hierarchical ? 2 * rd->num_steps : rd->num_steps;
+        if (int e = guard_refine(L, (const unsigned char*)packed, r.points, r.dirs, film, rd->batch, rays, rd->num_steps,
+                                 r.lock, tau, noise_f ? noise_f + (n_samples - 1) : nullptr, n_samples, rd->noise_std, raw_c,
+                                 (int32_t*)(ws + w.guard), (int32_t*)(ws + w.stats), st, r.dir_group)) return e;
+    }
+    mark(3);
+    if (rd->hierarchical) {
+        // with per-sample directions each fine sample takes its draw slot's (dirs_f); else the fine pass reads r.dirs
+        if (int e = resample(rd, C, raw_c, r.z, r.ray_dirs, r.origins, r.ray_origins, noise_c, rng_u, sigma_c, z_f, points_f,
+                             st, (long long*)inds, /*sort_fine=*/1, dirs_f ? r.dirs : nullptr, dirs_f,
+                             w.fine_slots ? ws + w.fine_slots : nullptr)) return e;
+        mark(4);
+        if (int e = run_field(L, packed, points_f, dirs_f ? dirs_f : r.dirs, film, rd->batch, ppb, r.dir_group,
+                              rd->lock_view_dependence, rd->precision, raw_f, st)) return e;
+    } else {
+        mark(4);
+    }
+    mark(5);
+    // both sample lists are depth-sorted here: one thread per ray, accumulators in registers (composite.cu)
+    const float* rf = rd->hierarchical ? raw_f : nullptr;
+    const float* zf = rd->hierarchical ? z_f : nullptr;
+    const int rc = ray_major ? composite_rays(rd, C, raw_c, r.z, rf, zf, noise_f, pixels, depth, weights_sum, st)
+                             : composite_sorted(rd, C, raw_c, r.z, rf, zf, noise_f, pixels, depth, weights_sum, weights, st);
+    mark(6);
+    return rc;
+}
+
+// fenerf_render_rays; grad: fenerf_render_rays_grad (the fine samples' draw slots into the workspace)
+int render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
+                const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
+                const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f, float* pixels,
+                float* depth, float* weights_sum, void* workspace, size_t workspace_bytes, void* stream, bool grad) {
+    if (int e = check_render_desc(rd)) return e;
+    FnLayout L;
+    if (int e = make_layout(field, &L)) return e;
+    FN_REQUIRE(rd->img_h == 1, "rays-in render: img_h must be 1 and img_w the number of rays per image (img_h %d)", rd->img_h);
+    FN_REQUIRE(rd->fill_mode == FENERF_FILL_NONE, "rays-in render: no fill modes (fill_mode %d)", rd->fill_mode);
+    FN_REQUIRE(packed && film && points && dirs && z_vals && pixels && workspace, "NULL argument");
+    FN_REQUIRE(dir_group == 1 || dir_group == rd->num_steps, "dir_group %d: 1 (a direction per sample) or num_steps %d "
+               "(one per ray)", dir_group, rd->num_steps);
+    FN_REQUIRE(!rd->hierarchical || (origins && ray_dirs), "hierarchical render needs the per-ray origins and ray_dirs");
+    const Workspace w = plan_workspace(rd, L.out_dim, true, dir_group, grad);
+    if (int e = check_pipeline(rd, rng_noise_c, rng_u, rng_noise_f, workspace, workspace_bytes, w)) return e;
+    const CoarseRays r{points, z_vals, dirs, dir_group, 0, nullptr, origins, ray_dirs};
+    return render_pipeline(rd, L, packed, film, r, rng_noise_c, rng_u, rng_noise_f, static_cast<unsigned char*>(workspace), w,
+                           true, pixels, depth, weights_sum, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 }  // namespace
@@ -334,152 +417,45 @@ int fenerf_render_forward(const fenerf_render_desc* rd, const fenerf_field_desc*
     FnLayout L;
     if (int e = make_layout(field, &L)) return e;
     FN_REQUIRE(packed && film && x_lin && y_lin && z_lin && cam2world && rng_perturb && pixels && workspace, "NULL argument");
-    FN_REQUIRE(!rd->hierarchical || rng_u, "hierarchical render needs rng_u");
-    FN_REQUIRE(!rd->hierarchical || rd->num_steps >= 3, "hierarchical render needs num_steps >= 3");
-    FN_REQUIRE(rd->noise_std == 0.f || (rng_noise_f && (!rd->hierarchical || rng_noise_c)), "noise_std != 0 needs the noise draws");
-    FN_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
-    const int C = L.out_dim;
-    Workspace w = plan_workspace(rd, C);
-    if (workspace_bytes < w.total) return fail(FENERF_E_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, w.total);
+    const Workspace w = plan_workspace(rd, L.out_dim);
+    if (int e = check_pipeline(rd, rng_noise_c, rng_u, rng_noise_f, workspace, workspace_bytes, w)) return e;
     unsigned char* ws = static_cast<unsigned char*>(workspace);
-    float* points_c = (float*)(ws + w.points_c);
-    float* z_c = (float*)(ws + w.z_c);
+    float* points = (float*)(ws + w.points_c);
+    float* z = (float*)(ws + w.z_c);
     float* dirs = (float*)(ws + w.dirs);
     float* origins = (float*)(ws + w.origins);
-    float* raw_c = (float*)(ws + w.raw_c);
-    float* z_f = (float*)(ws + w.z_f);
-    float* points_f = (float*)(ws + w.points_f);
-    float* raw_f = (float*)(ws + w.raw_f);
-    int32_t* guard = (int32_t*)(ws + w.guard);
     cudaStream_t st = (cudaStream_t)stream;
-    const long long rays = (long long)rd->img_h * rd->img_w;
-    const long long ppb = rays * rd->num_steps;
-    const float* noise_c = rd->noise_std != 0.f ? rng_noise_c : nullptr;
-    const float* noise_f = rd->noise_std != 0.f ? rng_noise_f : nullptr;
-
     stage_mark(0, st);
-    if (int e = ray_setup(rd, x_lin, y_lin, z_lin, cam2world, rng_perturb, points_c, z_c, dirs, origins, st)) return e;
+    if (int e = ray_setup(rd, x_lin, y_lin, z_lin, cam2world, rng_perturb, points, z, dirs, origins, st)) return e;
     stage_mark(1, st);
-    // the wgmma pass also leaves the densities as one float per point for the resampler (which never reads the far
-    // sample, so the GUARD refinement of raw_c below does not concern that copy)
-    float* sigma_c = (rd->hierarchical && rd->precision != FENERF_PRECISION_EXACT) ? (float*)(ws + w.sigma_c) : nullptr;
-    if (int e = run_field(L, packed, points_c, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
-                          rd->precision, raw_c, st, 0, sigma_c)) return e;
-    stage_mark(2, st);
-    if (rd->precision == FENERF_PRECISION_GUARD) {
-        float tau = rd->guard_tau > 0.f ? rd->guard_tau : 1.5e-3f;
-        const int n_samples = rd->hierarchical ? 2 * rd->num_steps : rd->num_steps;
-        if (int e = guard_refine(L, (const unsigned char*)packed, points_c, dirs, film, rd->batch, rays, rd->num_steps,
-                                 rd->lock_view_dependence, tau, noise_f ? noise_f + (n_samples - 1) : nullptr, n_samples,
-                                 rd->noise_std, raw_c, guard, (int32_t*)(ws + w.stats), st)) return e;
-    }
-    stage_mark(3, st);
-    if (rd->hierarchical) {
-        if (int e = resample(rd, C, raw_c, z_c, dirs, origins, nullptr, noise_c, rng_u, sigma_c, z_f, points_f, st,
-                             (long long*)inds_dbg, /*sort_fine=*/1)) return e;
-        stage_mark(4, st);
-        if (int e = run_field(L, packed, points_f, dirs, film, rd->batch, ppb, rd->num_steps, rd->lock_view_dependence,
-                              rd->precision, raw_f, st)) return e;
-    } else {
-        stage_mark(4, st);
-    }
-    stage_mark(5, st);
-    // both sample lists are depth-sorted here: one thread per ray, accumulators in registers (composite.cu)
-    const int rc = composite_sorted(rd, C, raw_c, z_c, rd->hierarchical ? raw_f : nullptr, rd->hierarchical ? z_f : nullptr,
-                                    noise_f, pixels, depth, weights_sum, weights, st);
-    stage_mark(6, st);
-    return rc;
+    const CoarseRays r{points, z, dirs, rd->num_steps, rd->lock_view_dependence, origins, nullptr, dirs};
+    return render_pipeline(rd, L, packed, film, r, rng_noise_c, rng_u, rng_noise_f, ws, w, false, pixels, depth, weights_sum,
+                           weights, inds_dbg, st);
 }
 
 size_t fenerf_rays_workspace_bytes(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group) {
     if (!rd || !field) return 0;
-    return plan_rays_workspace(rd, field->out_dim, dir_group).total;
-}
-
-int fenerf_rays_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
-                                 fenerf_rays_workspace_offsets* out) {
-    if (int e = check_render_desc(rd)) return e;
-    FN_REQUIRE(field && out, "NULL argument");
-    RaysWorkspace w = plan_rays_workspace(rd, field->out_dim, dir_group);
-    out->raw_coarse = w.raw_c; out->z_fine = w.z_f; out->points_fine = w.points_f; out->dirs_fine = w.dirs_f;
-    out->raw_fine = w.raw_f; out->total = w.total;
-    return 0;
+    return plan_workspace(rd, field->out_dim, true, dir_group).total;
 }
 
 int fenerf_rays_grad_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
                                       fenerf_rays_workspace_offsets* out, size_t* fine_slots) {
     if (int e = check_render_desc(rd)) return e;
     FN_REQUIRE(field && out && fine_slots, "NULL argument");
-    RaysWorkspace w = plan_rays_workspace(rd, field->out_dim, dir_group, true);
+    const Workspace w = plan_workspace(rd, field->out_dim, true, dir_group, true);
     out->raw_coarse = w.raw_c; out->z_fine = w.z_f; out->points_fine = w.points_f; out->dirs_fine = w.dirs_f;
     out->raw_fine = w.raw_f; out->total = w.total;
     *fine_slots = w.fine_slots;
     return 0;
 }
 
-}  // extern "C"
-
-namespace {
-
-// fenerf_render_rays; grad: fenerf_render_rays_grad (the fine samples' draw slots into the workspace)
-int render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
-                const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,
-                const float* z_vals, const float* rng_noise_c, const float* rng_u, const float* rng_noise_f, float* pixels,
-                float* depth, float* weights_sum, void* workspace, size_t workspace_bytes, void* stream, bool grad) {
-    if (int e = check_render_desc(rd)) return e;
-    FnLayout L;
-    if (int e = make_layout(field, &L)) return e;
-    FN_REQUIRE(rd->img_h == 1, "rays-in render: img_h must be 1 and img_w the number of rays per image (img_h %d)", rd->img_h);
-    FN_REQUIRE(rd->fill_mode == FENERF_FILL_NONE, "rays-in render: no fill modes (fill_mode %d)", rd->fill_mode);
-    FN_REQUIRE(packed && film && points && dirs && z_vals && pixels && workspace, "NULL argument");
-    FN_REQUIRE(dir_group == 1 || dir_group == rd->num_steps, "dir_group %d: 1 (a direction per sample) or num_steps %d "
-               "(one per ray)", dir_group, rd->num_steps);
-    FN_REQUIRE(!rd->hierarchical || (origins && ray_dirs), "hierarchical render needs the per-ray origins and ray_dirs");
-    FN_REQUIRE(!rd->hierarchical || rng_u, "hierarchical render needs rng_u");
-    FN_REQUIRE(!rd->hierarchical || rd->num_steps >= 3, "hierarchical render needs num_steps >= 3");
-    FN_REQUIRE(rd->noise_std == 0.f || (rng_noise_f && (!rd->hierarchical || rng_noise_c)), "noise_std != 0 needs the noise draws");
-    FN_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
-    const int C = L.out_dim;
-    RaysWorkspace w = plan_rays_workspace(rd, C, dir_group, grad);
-    if (workspace_bytes < w.total) return fail(FENERF_E_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, w.total);
-    unsigned char* ws = static_cast<unsigned char*>(workspace);
-    float* raw_c = (float*)(ws + w.raw_c);
-    float* z_f = (float*)(ws + w.z_f);
-    float* points_f = (float*)(ws + w.points_f);
-    float* dirs_f = (float*)(ws + w.dirs_f);
-    float* raw_f = (float*)(ws + w.raw_f);
-    cudaStream_t st = (cudaStream_t)stream;
-    const long long rays = rd->img_w;
-    const long long ppb = rays * rd->num_steps;
-    const float* noise_c = rd->noise_std != 0.f ? rng_noise_c : nullptr;
-    const float* noise_f = rd->noise_std != 0.f ? rng_noise_f : nullptr;
-
-    // the coarse pass keeps the caller's directions whatever lock_view_dependence says (generators.py:810)
-    float* sigma_c = (rd->hierarchical && rd->precision != FENERF_PRECISION_EXACT) ? (float*)(ws + w.sigma_c) : nullptr;
-    if (int e = run_field(L, packed, points, dirs, film, rd->batch, ppb, dir_group, 0, rd->precision, raw_c, st, 0, sigma_c))
-        return e;
-    if (rd->precision == FENERF_PRECISION_GUARD) {
-        float tau = rd->guard_tau > 0.f ? rd->guard_tau : 1.5e-3f;
-        const int n_samples = rd->hierarchical ? 2 * rd->num_steps : rd->num_steps;
-        if (int e = guard_refine(L, (const unsigned char*)packed, points, dirs, film, rd->batch, rays, rd->num_steps, 0, tau,
-                                 noise_f ? noise_f + (n_samples - 1) : nullptr, n_samples, rd->noise_std, raw_c,
-                                 (int32_t*)(ws + w.guard), (int32_t*)(ws + w.stats), st, dir_group)) return e;
-    }
-    if (rd->hierarchical) {
-        const bool per_sample = dir_group == 1 && !rd->lock_view_dependence;
-        if (int e = resample(rd, C, raw_c, z_vals, ray_dirs, nullptr, origins, noise_c, rng_u, sigma_c, z_f, points_f, st,
-                             nullptr, 1, per_sample ? dirs : nullptr, per_sample ? dirs_f : nullptr,
-                             grad && per_sample ? ws + w.fine_slots : nullptr)) return e;
-        if (int e = run_field(L, packed, points_f, per_sample ? dirs_f : dirs, film, rd->batch, ppb, dir_group,
-                              rd->lock_view_dependence, rd->precision, raw_f, st)) return e;
-    }
-    return composite_rays(rd, C, raw_c, z_vals, rd->hierarchical ? raw_f : nullptr, rd->hierarchical ? z_f : nullptr, noise_f,
-                          pixels, depth, weights_sum, st);
+int fenerf_rays_workspace_layout(const fenerf_render_desc* rd, const fenerf_field_desc* field, int32_t dir_group,
+                                 fenerf_rays_workspace_offsets* out) {
+    size_t fine_slots;
+    if (int e = fenerf_rays_grad_workspace_layout(rd, field, dir_group, out, &fine_slots)) return e;
+    if (fine_slots) out->total = fine_slots;     // the slots are the last section: the layout without them ends there
+    return 0;
 }
-
-}  // namespace
-
-extern "C" {
 
 int fenerf_render_rays(const fenerf_render_desc* rd, const fenerf_field_desc* field, const void* packed, const float* film,
                        const float* points, const float* dirs, int32_t dir_group, const float* origins, const float* ray_dirs,

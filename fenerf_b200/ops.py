@@ -364,66 +364,90 @@ def guard_stats(device):
     return dict(refined=rep.refined, max_abs_delta=rep.max_abs_delta, sign_flips=rep.sign_flips, tau=rep.tau)
 
 
-def _forward_call(lib, rd, packed, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f, pixels,
-                  depth, wsum, weights, inds, ws_ptr, ws_bytes, device):
-    _lib.check(lib.fenerf_render_forward(
-        C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device),
-        _chk(x_lin, "x_lin", device), _chk(y_lin, "y_lin", device), _chk(z_lin, "z_lin", device),
-        _chk(cam2world, "cam2world", device), _chk(rng_perturb, "rng_perturb", device),
-        _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device), _chk(rng_noise_f, "rng_noise_f", device),
-        pixels.data_ptr(), depth.data_ptr() if depth is not None else 0, wsum.data_ptr() if wsum is not None else 0,
-        weights.data_ptr() if weights is not None else 0, inds.data_ptr() if inds is not None else 0, ws_ptr, ws_bytes,
-        _stream(device)))
+def _render_call(entry, rd, packed, film, args, outs, ws_ptr, ws_bytes, device):
+    """One render entry of the C-ABI into the workspace at ws_ptr: fenerf_render_forward, `args` its ray set-up inputs
+    (_camera_render), or fenerf_render_rays[_grad], `args` the laid-out rays (_rays_render); then the three draws.
+    `args` by name, in the entry's order (numbers go as they are); `outs` its output tensors (None: not wanted)."""
+    ptrs = [v if isinstance(v, int) else _chk(v, k, device) for k, v in args.items()]
+    _lib.check(entry(C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device), *ptrs,
+                     *(0 if t is None else t.data_ptr() for t in outs), ws_ptr, ws_bytes, _stream(device)))
+
+
+def _camera_render(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f):
+    """The pack, FiLM table, frame (B, C_img, H, W) and arguments of fenerf_render_forward."""
+    packed = _packed(module, rd)
+    c = packed.desc.out_dim
+    film = _film_for(packed, film, packed.device, rd.batch)
+    pixels = torch.empty((rd.batch, _image_channels(rd, c), rd.img_h, rd.img_w), dtype=torch.float32, device=packed.device)
+    args = dict(x_lin=x_lin, y_lin=y_lin, z_lin=z_lin, cam2world=cam2world, rng_perturb=rng_perturb,
+                rng_noise_c=rng_noise_c, rng_u=rng_u, rng_noise_f=rng_noise_f)
+    return packed, film, pixels, args
+
+
+def _render_shared(entry, nbytes, rd, packed, film, args, outs):
+    """_render_call into the grow-only workspace of the current stream (where guard_stats reads)."""
+    device = packed.device
+    with torch.cuda.device(device):
+        ws = _workspace(device, nbytes)
+        ws_ptr = _aligned(ws)
+        _render_call(entry, rd, packed, film, args, outs, ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()), device)
+
+
+def _render_stages(entry, off, rd, packed, film, pixels, args, outs, slots_off=0):
+    """_render_call into a PRIVATE workspace laid out as `off`, returned with typed views of what the render leaves there:
+    what the backward consumes (fenerf_b200/backward.py).  The coarse samples are a camera render's ray set-up in the
+    workspace, or the caller's rays (args); the fine samples' directions and draw slots only where a rays-in render keeps
+    them (fenerf_rays_workspace_offsets)."""
+    device = packed.device
+    b, n, s, c = rd.batch, rd.img_h * rd.img_w, rd.num_steps, packed.desc.out_dim
+    with torch.cuda.device(device):
+        ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
+        base = _aligned(ws) - ws.data_ptr()
+        _render_call(entry, rd, packed, film, args, (pixels,) + outs, ws.data_ptr() + base, ws.numel() - base, device)
+    view = functools.partial(_stage_view, ws, base)
+    if "points" in args:
+        coarse = args["points"], args["z_vals"], args["dirs"], args["dir_group"]
+    else:
+        coarse = view(off.points_coarse, (b, n, s, 3)), view(off.z_coarse, (b, n, s)), view(off.dirs, (b, n, 3)), s
+    st = dict(pixels=pixels, workspace=ws, points_c=coarse[0], z_c=coarse[1], dirs=coarse[2], dir_group=coarse[3],
+              raw_c=view(off.raw_coarse, (b, n, s, c)), points_f=None, z_f=None, raw_f=None, dirs_f=None, slots_f=None)
+    if rd.hierarchical:
+        st.update(points_f=view(off.points_fine, (b, n, s, 3)), z_f=view(off.z_fine, (b, n, s)),
+                  raw_f=view(off.raw_fine, (b, n, s, c)))
+        if st["dir_group"] == 1 and not rd.lock_view_dependence:
+            st.update(dirs_f=view(off.dirs_fine, (b, n * s, 3)))
+            if slots_off:
+                st.update(slots_f=ws[base + slots_off: base + slots_off + b * n * s].view(b, n, s))
+    return st
 
 
 def render_forward(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
                    want_depth=True, want_weights_sum=True, want_weights=False, want_inds=False):
     """One call into fenerf_render_forward: the whole render after the mapping network."""
-    packed = _packed(module, rd)
+    packed, film, pixels, args = _camera_render(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c,
+                                                rng_u, rng_noise_f)
     device = packed.device
-    lib = _lib.lib()
     b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
     ns = 2 * s if rd.hierarchical else s
-    c = packed.desc.out_dim
-    film = _film_for(packed, film, device, b)
-    pixels = torch.empty((b, _image_channels(rd, c), rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     depth = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_depth else None
     wsum = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_weights_sum else None
     weights = torch.empty((b, n, ns, 1), dtype=torch.float32, device=device) if want_weights else None
     inds = torch.empty((b * n, s), dtype=torch.int64, device=device) if (want_inds and rd.hierarchical) else None
-    with torch.cuda.device(device):
-        nbytes = lib.fenerf_workspace_bytes(C.byref(rd), C.byref(packed.desc))
-        ws = _workspace(device, nbytes)
-        ws_ptr = _aligned(ws)
-        _forward_call(lib, rd, packed, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
-                      pixels, depth, wsum, weights, inds, ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()), device)
+    lib = _lib.lib()
+    _render_shared(lib.fenerf_render_forward, lib.fenerf_workspace_bytes(C.byref(rd), C.byref(packed.desc)), rd, packed,
+                   film, args, (pixels, depth, wsum, weights, inds))
     return pixels, depth, wsum, weights, inds
 
 
 def render_forward_stages(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f):
     """fenerf_render_forward into a PRIVATE workspace, returned together with typed views of the intermediates
-    it leaves there (fenerf_workspace_layout): what the backward consumes (fenerf_b200/backward.py)."""
-    packed = _packed(module, rd)
-    device = packed.device
+    it leaves there (fenerf_workspace_layout): _render_stages."""
+    packed, film, pixels, args = _camera_render(module, rd, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c,
+                                                rng_u, rng_noise_f)
     lib = _lib.lib()
-    b, n, s = rd.batch, rd.img_h * rd.img_w, rd.num_steps
-    c = packed.desc.out_dim
-    film = _film_for(packed, film, device, b)
-    pixels = torch.empty((b, c - 1, rd.img_h, rd.img_w), dtype=torch.float32, device=device)
     off = _lib.WorkspaceOffsets()
-    with torch.cuda.device(device):
-        _lib.check(lib.fenerf_workspace_layout(C.byref(rd), C.byref(packed.desc), C.byref(off)))
-        ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
-        base = _aligned(ws) - ws.data_ptr()
-        _forward_call(lib, rd, packed, film, x_lin, y_lin, z_lin, cam2world, rng_perturb, rng_noise_c, rng_u, rng_noise_f,
-                      pixels, None, None, None, None, ws.data_ptr() + base, ws.numel() - base, device)
-    view = functools.partial(_stage_view, ws, base)
-    st = dict(pixels=pixels, workspace=ws, points_c=view(off.points_coarse, (b, n, s, 3)), z_c=view(off.z_coarse, (b, n, s)),
-              dirs=view(off.dirs, (b, n, 3)), raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None)
-    if rd.hierarchical:
-        st.update(points_f=view(off.points_fine, (b, n, s, 3)), z_f=view(off.z_fine, (b, n, s)),
-                  raw_f=view(off.raw_fine, (b, n, s, c)))
-    return st
+    _lib.check(lib.fenerf_workspace_layout(C.byref(rd), C.byref(packed.desc), C.byref(off)))
+    return _render_stages(lib.fenerf_render_forward, off, rd, packed, film, pixels, args, (None,) * 4)
 
 
 # --------------------------------------------------------------------------------------------
@@ -469,14 +493,27 @@ def rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device):
     return pts, d, dir_group, o, rdir, z
 
 
+#: the arguments of fenerf_render_rays before its outputs, as _render_call takes them by name
+_RAYS_ARGS = ("points", "dirs", "dir_group", "origins", "ray_dirs", "z_vals", "rng_noise_c", "rng_u", "rng_noise_f")
+
+
 def _rays_call(lib, rd, packed, film, pts, dirs, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, depth,
                wsum, ws_ptr, ws_bytes, device, slots=False):
-    _lib.check((lib.fenerf_render_rays_grad if slots else lib.fenerf_render_rays)(
-        C.byref(rd), C.byref(packed.desc), packed.ptr, _chk(film, "film", device), _chk(pts, "points", device),
-        _chk(dirs, "dirs", device), dir_group, _chk(o, "origins", device), _chk(rdir, "ray_dirs", device),
-        _chk(z, "z_vals", device), _chk(rng_noise_c, "rng_noise_c", device), _chk(rng_u, "rng_u", device),
-        _chk(rng_noise_f, "rng_noise_f", device), pixels.data_ptr(), depth.data_ptr() if depth is not None else 0,
-        wsum.data_ptr() if wsum is not None else 0, ws_ptr, ws_bytes, _stream(device)))
+    """fenerf_render_rays (slots: fenerf_render_rays_grad) on rays laid out by rays_inputs, into the workspace at ws_ptr."""
+    args = dict(zip(_RAYS_ARGS, (pts, dirs, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f)))
+    _render_call(lib.fenerf_render_rays_grad if slots else lib.fenerf_render_rays, rd, packed, film, args,
+                 (pixels, depth, wsum), ws_ptr, ws_bytes, device)
+
+
+def _rays_render(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f):
+    """The pack, FiLM table, frame (B, N, C-1) and arguments of fenerf_render_rays."""
+    packed = _packed(module, rd)
+    device = packed.device
+    film = _film_for(packed, film, device, rd.batch)
+    args = dict(zip(_RAYS_ARGS, (*rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device), rng_noise_c, rng_u,
+                                 rng_noise_f)))
+    pixels = torch.empty((rd.batch, rd.img_w, packed.desc.out_dim - 1), dtype=torch.float32, device=device)
+    return packed, film, pixels, args
 
 
 def _film_for(packed, film, device, b):
@@ -493,62 +530,35 @@ def render_rays(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_n
                 want_depth=False, want_weights_sum=False):
     """One call into fenerf_render_rays (rd from make_rays_desc): the render of caller-supplied rays.
     Returns (pixels (B, N, C-1) ray-major in [0, 1], depth (B, N, 1) or None, weights_sum (B, N, 1) or None)."""
-    packed = _packed(module, rd)
-    device = packed.device
-    lib = _lib.lib()
+    packed, film, pixels, args = _rays_render(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u,
+                                              rng_noise_f)
     b, n = rd.batch, rd.img_w
-    c = packed.desc.out_dim
-    film = _film_for(packed, film, device, b)
-    pts, d, dir_group, o, rdir, z = rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device)
-    pixels = torch.empty((b, n, c - 1), dtype=torch.float32, device=device)
-    depth = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_depth else None
-    wsum = torch.empty((b, n, 1), dtype=torch.float32, device=device) if want_weights_sum else None
-    with torch.cuda.device(device):
-        nbytes = lib.fenerf_rays_workspace_bytes(C.byref(rd), C.byref(packed.desc), dir_group)
-        ws = _workspace(device, nbytes)
-        ws_ptr = _aligned(ws)
-        _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, depth, wsum,
-                   ws_ptr, ws.numel() - (ws_ptr - ws.data_ptr()), device)
+    depth = torch.empty((b, n, 1), dtype=torch.float32, device=packed.device) if want_depth else None
+    wsum = torch.empty((b, n, 1), dtype=torch.float32, device=packed.device) if want_weights_sum else None
+    lib = _lib.lib()
+    nbytes = lib.fenerf_rays_workspace_bytes(C.byref(rd), C.byref(packed.desc), args["dir_group"])
+    _render_shared(lib.fenerf_render_rays, nbytes, rd, packed, film, args, (pixels, depth, wsum))
     return pixels, depth, wsum
 
 
 def render_rays_stages(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u, rng_noise_f,
                        slots=False):
     """fenerf_render_rays into a PRIVATE workspace, returned with typed views of what it leaves there
-    (fenerf_rays_workspace_layout) and the laid-out inputs: what the backward consumes (fenerf_b200/backward.py).
+    (fenerf_rays_workspace_layout) and the laid-out inputs: _render_stages.
     slots=True (a backward w.r.t. the directions): fenerf_render_rays_grad, which also leaves the fine samples' draw
     slots, 'slots_f' (B, N, S) uint8, where the fine pass reads per-sample directions (None elsewhere)."""
-    packed = _packed(module, rd)
-    device = packed.device
+    packed, film, pixels, args = _rays_render(module, rd, film, points, dirs, origins, ray_dirs, z_vals, rng_noise_c, rng_u,
+                                              rng_noise_f)
     lib = _lib.lib()
-    b, n, s = rd.batch, rd.img_w, rd.num_steps
-    c = packed.desc.out_dim
-    film = _film_for(packed, film, device, b)
-    pts, d, dir_group, o, rdir, z = rays_inputs(rd, points, dirs, origins, ray_dirs, z_vals, device)
-    pixels = torch.empty((b, n, c - 1), dtype=torch.float32, device=device)
     off = _lib.RaysWorkspaceOffsets()
     slots_off = C.c_size_t(0)
-    with torch.cuda.device(device):
-        if slots:
-            _lib.check(lib.fenerf_rays_grad_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off),
-                                                             C.byref(slots_off)))
-        else:
-            _lib.check(lib.fenerf_rays_workspace_layout(C.byref(rd), C.byref(packed.desc), dir_group, C.byref(off)))
-        ws = torch.empty(off.total + 256, dtype=torch.uint8, device=device)
-        base = _aligned(ws) - ws.data_ptr()
-        _rays_call(lib, rd, packed, film, pts, d, dir_group, o, rdir, z, rng_noise_c, rng_u, rng_noise_f, pixels, None, None,
-                   ws.data_ptr() + base, ws.numel() - base, device, slots=slots)
-    view = functools.partial(_stage_view, ws, base)
-    st = dict(pixels=pixels, workspace=ws, points_c=pts, z_c=z, dirs=d, dir_group=dir_group,
-              raw_c=view(off.raw_coarse, (b, n, s, c)), raw_f=None, z_f=None, points_f=None, dirs_f=None, slots_f=None)
-    if rd.hierarchical:
-        st.update(points_f=view(off.points_fine, (b, n, s, 3)), z_f=view(off.z_fine, (b, n, s)),
-                  raw_f=view(off.raw_fine, (b, n, s, c)))
-        if dir_group == 1 and not rd.lock_view_dependence:
-            st.update(dirs_f=view(off.dirs_fine, (b, n * s, 3)))
-            if slots:
-                st.update(slots_f=ws[base + slots_off.value: base + slots_off.value + b * n * s].view(b, n, s))
-    return st
+    if slots:
+        _lib.check(lib.fenerf_rays_grad_workspace_layout(C.byref(rd), C.byref(packed.desc), args["dir_group"], C.byref(off),
+                                                         C.byref(slots_off)))
+    else:
+        _lib.check(lib.fenerf_rays_workspace_layout(C.byref(rd), C.byref(packed.desc), args["dir_group"], C.byref(off)))
+    return _render_stages(lib.fenerf_render_rays_grad if slots else lib.fenerf_render_rays, off, rd, packed, film, pixels,
+                          args, (None, None), slots_off.value)
 
 
 def mapping_film(net, z, film, first_layer, n_layers, avg=None, psi=1.0):

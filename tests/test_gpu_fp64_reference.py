@@ -352,10 +352,11 @@ def test_flat_cases_straddle_the_narrow_body_limit():
 @gpu
 @pytest.mark.parametrize("n,hier,c,opt,opaque,entry", with_entries(_COMPOSITE, _COMPOSITE_IDS))
 def test_composite_backward_vs_fp64(n, hier, c, opt, opaque, entry):
-    """``fenerf_composite_backward`` as RenderFunction.backward calls it, and ``fenerf_composite_backward_rays`` as
-    RaysRenderFunction.backward does, against the float64 VJP of the compositing: B = 3, 37² rays, n merged samples
-    (more than 32 carry the transmittance scan from chunk to chunk; the shared memory of n = 48 with C = 32 and of
-    n >= 96 with C >= 22 is beyond 48 KB and needs the opt-in, which each entry's kernel makes for itself)."""
+    """``fenerf_composite_backward`` as RenderFunction.backward calls it for a camera render, and
+    ``fenerf_composite_backward_rays`` as it does for a rays-in render, against the float64 VJP of the compositing:
+    B = 3, 37² rays, n merged samples (more than 32 carry the transmittance scan from chunk to chunk; the shared memory
+    of n = 48 with C = 32 and of n >= 96 with C >= 22 is beyond 48 KB and needs the opt-in, which each entry's kernel
+    makes for itself)."""
     steps = n // 2 if hier else n
     x = _composite_inputs(c, steps, hier, opaque)
     o = _OPTS[opt]
@@ -384,7 +385,7 @@ _FIELD = ([(lay, m, p, False) for lay in ("L1", "L2", "L3") for m in FIELD_MODEL
 def _field_backward(siren, film, pts, dirs, dir_group, lock, raw, d_raw, exact):
     with torch.no_grad():
         m = d_raw.abs().max()
-        scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)   # as RenderFunction.backward
+        scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)   # as backward._field_backward
         fb = backward._FieldBackward(siren, film, scale, (1.0 / scale).float().reshape(1), exact=exact)
         fb.add_points(pts, dirs, dir_group, lock, raw, d_raw)
         d_film, grads = fb.finish()

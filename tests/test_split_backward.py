@@ -248,7 +248,7 @@ _FIELD = ([(lay, m) for lay in ("L1", "L2", "L3") for m in FIELD_MODELS + ("P",)
 def _field_backward(siren, film, pts, dirs, dir_group, raw, d_raw, grad_split=True):
     with torch.no_grad(), backward._NoTF32():
         m = d_raw.abs().max()
-        scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)   # as RenderFunction.backward
+        scale = torch.exp2(4.0 - torch.ceil(torch.log2(m.clamp_min(1e-30)))).float().reshape(1)   # as backward._field_backward
         fb = backward._FieldBackward(siren, film, scale, (1.0 / scale).float().reshape(1), exact=True, grad_split=grad_split)
         fb.add_points(pts, dirs, dir_group, False, raw, d_raw)
         d_film, grads = fb.finish()
