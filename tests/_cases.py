@@ -68,6 +68,8 @@ class Case:
     method: str = "forward"        # or "staged_forward"
     sigma_bias_shift: float = 0.0  # density bias += shift (opaque-regime fixture, SURVEY.md 7.1; apply_weight_edits)
     psi: float = 1.0
+    probed: bool = False           # the golden stores `pixel_probe` (PROBE entries of the pixels) and their abs-sum
+    big: bool = False              # the CPU oracle run takes tens of seconds or minutes
 
 
 def _cfg(**kw):
@@ -134,15 +136,9 @@ CASES = [
     Case("h_small", "H", 1, 57, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
     # ---- the benchmarked shapes themselves (BASELINE.json configs[1] and the configs[4] shape), one face each ----
     Case("a_cfg2", "A", 1, 61, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-    Case("b_cfg2", "B", 1, 62, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-    Case("a_cfg5", "A", 1, 63, _cfg(img_size=256, num_steps=48, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-]
-#: cases whose CPU oracle run takes tens of seconds: the CPU suite (-m "not gpu") checks them only with
-#: FENERF_SLOW_TESTS=1; the GPU suite always runs them
-BIG_CASES = ("b_cfg2", "a_cfg5")
-
-# ---- the field families' cases (each family's tests and golden generator parametrise over its own list) ----
-LABEL_FILM_CASES = [
+    Case("b_cfg2", "B", 1, 62, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0), big=True),
+    Case("a_cfg5", "A", 1, 63, _cfg(img_size=256, num_steps=48, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0), big=True),
+    # ---- the field families: label FiLM (I), feature heads (J, K), grid trunk (L), bridge (M, N), direction-free (P) ----
     Case("i_small", "I", 2, 71, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
     Case("i_small_opaque", "I", 1, 72, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
          sigma_bias_shift=0.5),
@@ -151,9 +147,8 @@ LABEL_FILM_CASES = [
     Case("i_staged_softmax", "I", 1, 73, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
                                               softmax_label=True, fill_mode='weight'), method="staged_forward", psi=0.7),
     # one cfg2-shaped render (128², 24 + 24); its golden keeps a fixed probe of the pixels (see pixel_probe_index)
-    Case("i_cfg2", "I", 1, 74, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-]
-FEATURE_HEAD_CASES = [
+    Case("i_cfg2", "I", 1, 74, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0),
+         probed=True),
     Case("j_small", "J", 2, 81, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
     Case("j_small_opaque", "J", 1, 82, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
          sigma_bias_shift=0.5),
@@ -165,9 +160,8 @@ FEATURE_HEAD_CASES = [
     Case("k_staged_softmax", "K", 1, 93, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0,
                                               softmax_label=True, fill_mode='weight'), method="staged_forward", psi=0.7),
     # an img_feat_size-like render (64², 24 + 24); its golden keeps a fixed probe of the pixels
-    Case("k_feat64", "K", 1, 94, _cfg(img_size=64, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-]
-GRID_TRUNK_CASES = [
+    Case("k_feat64", "K", 1, 94, _cfg(img_size=64, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0),
+         probed=True),
     Case("l_small", "L", 2, 101, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
     Case("l_small_opaque", "L", 1, 102, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
          sigma_bias_shift=0.5),
@@ -176,9 +170,8 @@ GRID_TRUNK_CASES = [
                                              fill_mode='eval_white_back'), method="staged_forward", psi=0.7,
          sigma_bias_shift=0.5),
     # the benchmarked shape (128², 24 + 24); its golden keeps a fixed probe of the pixels
-    Case("l_cfg2", "L", 1, 104, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-]
-BRIDGE_CASES = [
+    Case("l_cfg2", "L", 1, 104, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0),
+         probed=True, big=True),
     Case("m_small", "M", 2, 201, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
     Case("m_small_opaque", "M", 1, 202, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
          sigma_bias_shift=0.5),
@@ -193,9 +186,8 @@ BRIDGE_CASES = [
                                              fill_mode='eval_white_back'), method="staged_forward", psi=0.7,
          sigma_bias_shift=0.5),
     # the benchmarked shape (128², 24 + 24); its golden keeps a fixed probe of the pixels
-    Case("n_cfg2", "N", 1, 214, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
-]
-WO_DIR_CASES = [
+    Case("n_cfg2", "N", 1, 214, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0),
+         probed=True, big=True),
     Case("p_small", "P", 2, 301, _cfg(img_size=12, num_steps=9, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
     Case("p_small_opaque", "P", 1, 302, _cfg(img_size=12, num_steps=10, h_stddev=0.0, v_stddev=0.0, nerf_noise=0.0),
          sigma_bias_shift=0.5),
@@ -204,12 +196,187 @@ WO_DIR_CASES = [
                                              fill_mode='eval_seg_padding_background', fill_color='white'),
          method="staged_forward", psi=0.7, sigma_bias_shift=0.5),
     # the benchmarked shape (128², 24 + 24); its golden keeps a fixed probe of the pixels
-    Case("p_cfg2", "P", 1, 304, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0)),
+    Case("p_cfg2", "P", 1, 304, _cfg(img_size=128, num_steps=24, h_stddev=0.3, v_stddev=0.155, nerf_noise=0.0),
+         probed=True, big=True),
 ]
-#: every case, stock or family, by name
-CASE_BY_NAME = {c.name: c for c in (CASES + LABEL_FILM_CASES + FEATURE_HEAD_CASES + GRID_TRUNK_CASES + BRIDGE_CASES
-                                    + WO_DIR_CASES)}
+#: every case by name
+CASE_BY_NAME = {c.name: c for c in CASES}
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+_TRUNK = ["siren.network.0.layer.weight", "siren.network.7.layer.bias", "siren.final_layer.weight"]
+_LABEL_FILM = ["siren.label_layer_sine.layer.weight", "siren.label_layer_sine.layer.bias",
+               "siren.label_layer_linear.0.weight", "siren.label_layer_linear.0.bias"]
+_DOUBLE_MAPPING = ["siren.geo_mapping_network.network.8.bias", "siren.app_mapping_network.network.8.bias"]
+
+#: parameters whose gradients grad_<case>.npz stores (besides the latents'), for each gradient-golden case: a
+#: cross-section of trunk, heads, colour branch and mapping network.  The family cases that are opaque are so, so that
+#: the render (and with it every gradient) is not the empty background's
+GRAD_PARAMS = {
+    "a_small": _TRUNK + ["siren.color_layer_sine.layer.bias", "siren.color_layer_linear.0.weight",
+                         "siren.mapping_network.network.8.bias"],
+    "d_small": _TRUNK + ["siren.color_layer_sine.2.layer.bias", "siren.color_layer_linear.0.weight",
+                         "siren.label_layer_linear.1.weight"] + _DOUBLE_MAPPING,
+    "b_small": ["siren.network.0.layer.weight", "siren.network.3.layer.weight", "siren.network.7.layer.bias",
+                "siren.final_layer.weight", "siren.final_layer.bias", "siren.color_layer_sine.0.layer.weight",
+                "siren.color_layer_sine.2.layer.bias", "siren.color_layer_linear.0.weight",
+                "siren.color_layer_linear.0.bias", "siren.label_layer_linear.0.weight",
+                "siren.label_layer_linear.1.bias", "siren.label_layer_linear.2.weight"] + _DOUBLE_MAPPING,
+    "i_small": _TRUNK + _LABEL_FILM + ["siren.color_layer_sine.layer.bias", "siren.color_layer_linear.0.weight",
+                                       "siren.mapping_network.network.8.bias"],
+    "j_small": _TRUNK + ["siren.color_layer_sine.layer.bias", "siren.color_layer_linear.0.weight",
+                         "siren.color_layer_linear.0.bias", "siren.mapping_network.network.8.bias"],
+    "k_small": _TRUNK + _LABEL_FILM + ["siren.color_layer_sine.layer.bias", "siren.color_layer_linear.0.weight",
+                                       "siren.color_layer_linear.0.bias", "siren.mapping_network.network.8.bias"],
+    "l_small_opaque": ["siren.network.0.layer.weight", "siren.network.0.layer.bias", "siren.network.7.layer.bias",
+                       "siren.final_layer.weight", "siren.color_layer_sine.layer.weight",
+                       "siren.color_layer_linear.0.weight", "siren.mapping_network.network.8.bias"],
+    "m_small_opaque": _TRUNK + ["siren.color_layer_pre.0.weight", "siren.color_layer_pre.0.bias",
+                                "siren.color_layer_sine.0.layer.weight", "siren.color_layer_linear.0.weight"]
+    + _DOUBLE_MAPPING,
+    "n_small_opaque": ["siren.network.0.layer.weight", "siren.network.7.layer.bias", "siren.res_coord_layer.weight",
+                       "siren.res_coord_layer.bias", "siren.density_layer_linear.0.weight",
+                       "siren.density_layer_linear.1.weight", "siren.density_layer_linear.3.weight",
+                       "siren.density_layer_linear.3.bias", "siren.color_layer_pre.0.weight",
+                       "siren.color_layer_pre.0.bias", "siren.color_layer_sine.0.layer.weight",
+                       "siren.color_layer_linear.0.weight"] + _DOUBLE_MAPPING,
+    # (the grid's 113 MB gradient is left to the float64 tests)
+    "p_small_opaque": _TRUNK + ["siren.label_layer_linear.0.weight", "siren.color_layer_sine.0.layer.weight",
+                                "siren.color_layer_sine.0.layer.bias", "siren.color_layer_sine.7.layer.weight",
+                                "siren.color_layer_linear.0.weight"] + _DOUBLE_MAPPING,
+}
+GRAD_PARAMS["d_staged_softmax"] = GRAD_PARAMS["d_small"]
+GRAD_PARAMS["a_hier_softplus"] = GRAD_PARAMS["a_small"]
+#: entries of a grid's gradient a gradient golden stores: model B a fixed random projection (grid_probe_index); model L
+#: its largest entries with their indices (grid_probe_idx: a small render touches few voxels, so a random probe of the
+#: 8.4 M entries would hold zeros only); both with the absolute sum
+GRID_PROBE = 4096
+
+#: the inversion goldens (gradfreq_<case>.npz: d L / d (frequencies, phase shifts) through forward_with_frequencies) ->
+#: the FiLM rows [r0, r1) that are also held to the bound on their own (the label FiLM row, the feature heads' rows)
+GRADFREQ = {"a_small": None, "d_small": None, "i_small": (8, 9), "k_small": (8, 10), "l_small_opaque": None,
+            "m_small_opaque": None, "n_small_opaque": None, "p_small_opaque": None}
+
+#: per-model facts of the tests and the golden maker; a model without an entry takes the defaults of `model_data`
+#:   grid_probe  how its gradient golden samples the grid's gradient: "random", "largest" (see GRID_PROBE) or None
+#:   freq_order  "mapping": its inversion golden stores a double latent's gradients as the mapping networks return them
+#:               (geo f, geo p, app f, app p); otherwise in forward_with_frequencies' order (geo f, app f, geo p, app p)
+#:   dropin      dropin_ref_<model>.* written from the reference's classes: "full" (a whole-module checkpoint with
+#:               step / epoch, and .meta: parameter names and state dict), "bare" (the checkpoint alone) or "shapes"
+#:               (.meta alone: names and state-dict shapes; the 32 x 64^3 grid is not stored)
+#:   third       its staged goldens also keep staged_forward's third output
+#:   precisions  the render precisions it serves (P: the fp16 colour path is refused, DESIGN section 5)
+#:   repack      (parameter, columns, factor): writes through param.data that staged_forward must see
+#:   guard       (image size, bound of the self-check's max |delta| or None): the GUARD refinement test
+#:   fwd_seed, bwd_seed  seeds of its point-network and _FieldBackward float64 tests (test_gpu_fp64_reference), where
+#:               they are not the stock models' 2000 + index and 1000 + 10 index (+ the layout's number)
+#:   bounds      overrides of BOUNDS
+_STOCK = dict(third=True)
+MODEL_DATA = {
+    "A": dict(_STOCK, dropin="full"),
+    "B": dict(_STOCK, grid_probe="random"),
+    "C": _STOCK, "D": dict(_STOCK, dropin="full"), "E": _STOCK, "S": _STOCK, "F": _STOCK, "G": _STOCK, "H": _STOCK,
+    "I": dict(dropin="full", repack=[("siren.label_layer_sine.layer.weight", None, 1.5),
+                                     ("siren.color_layer_sine.layer.weight", None, 1.5)],
+              # the default mode's label channels at cfg2 (128², 24 + 24): unlike rgb they pass through no sigmoid, so
+              # the fp16 label layer's error reaches the pixels undamped.  Measured 1.0e-3 (every other case and channel:
+              # <= 6.1e-4)
+              bounds={"render_guard_cfg2_labels": 1.5e-3},
+              # the refinement never touches the label branch (every ray refined: no self-check bound)
+              guard=(24, None), fwd_seed=2100, bwd_seed=3100),
+    "J": dict(dropin="full", fwd_seed=2200, bwd_seed=3200),
+    # a 64-label field: the refinement runs through the plain exact kernel on the trunk view
+    "K": dict(dropin="full", guard=(16, 1e-2), fwd_seed=2200, bwd_seed=3210),
+    # the self-check stays under tau / 3 of the default tau (1.5e-3), so the generators never widen tau for this field
+    "L": dict(grid_probe="largest", dropin="shapes", guard=(16, 1.5e-3 / 3), fwd_seed=2300, bwd_seed=3300,
+              # the feature columns alone: the fingerprint counts all 35 columns
+              repack=[("siren.network.0.layer.weight", slice(0, 32), -1.0)],
+              bounds={
+                  # the exact kernel's density carries the fp32 trilinear features through a 35-term first layer at
+                  # f ~ 30 and then every trunk layer: measured 1.1e-5 .. 1.3e-5 on sigma (rgb 3e-6 .. 6e-6), against
+                  # 1e-5 for fields whose trunk sees only the position; the fast bound is the shared one
+                  "fwd_exact": 3e-5,
+                  # the grid's gradient in exact mode reaches the grid through layer 0's fp32 chain and the fp32
+                  # scatter-add: measured 1.1e-4 .. 1.2e-4 of its largest entry (every other tensor within the shared
+                  # 1e-4)
+                  "grid_exact": 3e-4,
+                  # the grid's absolute sum in the default mode: measured 5.3e-5 (exact 1.8e-5)
+                  "grid_abs_sum_guard": 2e-2}),
+    "M": dict(freq_order="mapping", dropin="bare", repack=[("siren.color_layer_pre.0.weight", None, -3.0)]),
+    "N": dict(freq_order="mapping", dropin="bare", repack=[("siren.res_coord_layer.weight", None, -3.0),
+                                                           ("siren.color_layer_pre.0.weight", None, -3.0),
+                                                           ("siren.density_layer_linear.1.weight", None, -3.0)]),
+    "P": dict(freq_order="mapping", precisions=("exact",),
+              # the whole first colour layer, and its feature columns alone: the fingerprint covers all 288 columns
+              repack=[("siren.color_layer_sine.0.layer.weight", None, -3.0),
+                      ("siren.color_layer_sine.0.layer.weight", slice(0, 32), -3.0)],
+              bounds={
+                  # exact renders against the reference's: measured on an H100 80GB HBM3 (700 W) <= 5.6e-4 (p_cfg2;
+                  # 2.5e-4 .. 3.4e-4 on the small cases) -- the reference's own fp32 forward differs from float64 by
+                  # the same amplification of its rounding (the first colour layer's U(+-1/3) weights at f ~ 30)
+                  "render_exact": 1e-3,
+                  # gradients and inversion against the reference's autograd, exact mode: measured <= 6.6e-3 and 5.9e-3
+                  "grad_exact": 1e-2, "kink_exact": 1e-2}),
+}
+
+#: bounds of the shared tests, overridden per model by MODEL_DATA[m]["bounds"]
+BOUNDS = {
+    "render_exact": 2e-4, "render_guard": 1e-3,        # end to end, against the oracle and the reference's goldens
+    "render_guard_cfg2_labels": 1e-3,                  # the label channels of a probed (cfg2-shaped) case, default mode
+    # gradients against the reference's autograd, relative to each tensor's max; the density head's `kink` bound
+    # (test_gpu_parity.KINK_KEYS)
+    "grad_exact": 5e-4, "grad_guard": 2e-2, "kink_exact": 1e-2, "kink_guard": 0.3,
+    "grid_abs_sum_exact": 5e-3, "grid_abs_sum_guard": 5e-3,
+    "fwd_exact": 1e-5, "fwd_fast": 5e-3,               # point network against float64 (test_gpu_fp64_reference)
+    "grid_exact": 1e-4,                                # _FieldBackward's grid gradient against float64, exact mode
+}
+
+
+def model_data(model, key):
+    d = MODEL_DATA.get(model, {})
+    if key == "bounds":
+        return dict(BOUNDS, **d.get("bounds", {}))
+    return d.get(key, {"precisions": ("exact", "guard")}.get(key))
+
+
+def bound(model, name):
+    return model_data(model, "bounds")[name]
+
+
+#: class-level init goldens of field classes (bridge_init.json, wo_dir_init.json): file -> (constructor arguments,
+#: classes); per class the state digest, parameter names, state-dict shapes, child names and the RNG's next draw
+INIT_GOLDENS = {
+    # (input_dim, z_geo_dim, z_app_dim, hidden_dim, output_dim): the double-latent curriculum's shapes
+    "bridge_init.json": (((3, 256, 256, 256, 4), {}), ("SPATIALSIRENAUGDISENTANGLE", "RESSIRENDISENTANGLE")),
+    # the texture-embedding curriculum's shapes (18 labels); each class keeps its own hidden_dim
+    "wo_dir_init.json": (((), dict(input_dim=3, z_geo_dim=256, z_app_dim=256, output_dim=22)),
+                         ("TextureEmbeddingPiGAN128SEMANTICDISENTANGLE_WO_DIR",
+                          "TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96")),
+}
+INIT_CLASSES = {name: (f, args) for f, (args, names) in INIT_GOLDENS.items() for name in names}
+
+
+def construct_field(siren_mod, name):
+    """A field class of INIT_GOLDENS with its arguments (the caller seeds the RNG)."""
+    args, kwargs = INIT_CLASSES[name][1]
+    return getattr(siren_mod, name)(*args, **kwargs)
+
+
+def scale_density(siren):
+    """Scales RES's last density Linear so that max |a| = 1 and shifts its bias so that c = 0 (sigma = a . v + c, the chain
+    folded): at the reference's init |a| is ~1e-6 and the density hardly depends on v, so the sigma-from-v path would go
+    untested."""
+    def fold():
+        a, c = None, None
+        for lin in siren.density_layer_linear:
+            w, b = lin.weight.double(), lin.bias.double()
+            a, c = (w, b) if a is None else (w @ a, w @ c + b)
+        return a, c
+    with torch.no_grad():
+        a, _ = fold()
+        siren.density_layer_linear[3].weight.mul_(1.0 / a.abs().max().item())
+        _, c = fold()
+        siren.density_layer_linear[3].bias.sub_(c.to(siren.density_layer_linear[3].bias.dtype))
+    return siren
 
 #: entries of the flattened pixels a probed golden (a cfg2-shaped family render) stores instead of every pixel
 PROBE = 32768
@@ -360,3 +527,15 @@ def grid_probe_index(numel, n):
     """Fixed pseudo-random flat indices into the feature grid (the gradient goldens store only these entries)."""
     g = torch.Generator().manual_seed(7)
     return torch.randint(0, numel, (n,), generator=g)
+
+
+def frequency_leaves(siren, latents, model):
+    """The mapping networks' outputs for the inversion call, in the order its golden stores their gradients (arg0, arg1,
+    ...) -> (outputs, the order forward_with_frequencies takes them in)."""
+    if len(latents) == 1:
+        return list(siren.mapping_network(latents[0])), (0, 1)
+    fg, pg = siren.geo_mapping_network(latents[0])
+    fa, pa = siren.app_mapping_network(latents[1])
+    if model_data(model, "freq_order") == "mapping":
+        return [fg, pg, fa, pa], (0, 2, 1, 3)
+    return [fg, fa, pg, pa], (0, 1, 2, 3)

@@ -1,10 +1,17 @@
 """Generates tests/golden/*.npz by running the UNMODIFIED reference (a checkout of it named by $FENERF_REFERENCE_ROOT).
 
-    python tests/golden/make_goldens.py [--grads | --zero-freq | --part | --dropin]
+    python tests/golden/make_goldens.py [case ...] | --grads | --zero-freq | --part | --dropin | --init
 
 The reference holds no golden vectors for the render path (SURVEY.md section 4), so the pin of the
 oracle is the reference's own forward on fixed seeds, captured here.  The .npz files travel with
-the repository; the reference does not.
+the repository; the reference does not.  What each flag writes, from tests/_cases.py's tables:
+  (none)       <case>.npz for every case of CASES (or the named ones): forward / staged_forward outputs; a probed case
+               stores a fixed probe of the pixels and their abs-sum
+  --grads      grad_<case>.npz (GRAD_PARAMS), gradfreq_<case>.npz (GRADFREQ) and gradfreq_a_small_zero_f.npz
+  --zero-freq  gradfreq_a_small_zero_f.npz alone
+  --part       part_d_small.npz (ray-subset training)
+  --dropin     dropin_ref_<model>.* for every model with MODEL_DATA[m]["dropin"], and dropin_ref_layout.json
+  --init       bridge_init.json and wo_dir_init.json (INIT_GOLDENS)
 
 Seed protocol (shared with tests/_cases.py):
   torch.manual_seed(0)            -> construct the generator (reference init order)
@@ -14,7 +21,10 @@ Seed protocol (shared with tests/_cases.py):
   torch.manual_seed(case.seed)    -> the forward under test  (+ random.seed(case.seed): the 'hybrid' camera
                                      mode flips Python's global coin, volumetric_rendering.py:199)
 """
+import gzip
 import hashlib
+import io
+import json
 import os
 import random
 import sys
@@ -68,60 +78,55 @@ def main():
                 res = gen.staged_forward(*latents, **kw)
                 pixels = res[0]
                 extra = {"depth_map": res[1].numpy()}
-                if len(res) > 2:
+                if len(res) > 2 and _cases.model_data(case.model, "third"):
                     extra["third"] = res[2].numpy()
             else:
                 raise ValueError(case.method)
-        path = os.path.join(out_dir, case.name + ".npz")
-        np.savez_compressed(path, pixels=pixels.cpu().numpy(), state_digest=np.array(digest), **extra)
+        if case.probed:
+            extra.update(pixel_probe=_cases.probe_of(pixels).numpy(), pixels_abs_sum=np.array(pixels.abs().sum().item()),
+                         pixels_shape=np.array(pixels.shape))
+        else:
+            extra["pixels"] = pixels.cpu().numpy()
+        path = _cases.golden_path(case)
+        np.savez_compressed(path, state_digest=np.array(digest), **extra)
         print("%-28s pixels %s  mean|x| %.6f  -> %s (%.1f KB)" % (
             case.name, tuple(pixels.shape), float(pixels.abs().mean()), os.path.basename(path), os.path.getsize(path) / 1024))
 
 
 # ---- gradients of the differentiable call (the reference's G step / inversion path) -----------------
-GRAD_CASES = ("a_small", "d_small", "b_small", "d_staged_softmax", "a_hier_softplus")
-#: parameters whose gradients are stored (a cross-section of trunk, heads, colour branch, mapping network)
-GRAD_PARAMS = {
-    "A": ["siren.network.0.layer.weight", "siren.network.7.layer.bias", "siren.final_layer.weight",
-          "siren.color_layer_sine.layer.bias", "siren.color_layer_linear.0.weight",
-          "siren.mapping_network.network.8.bias"],
-    "D": ["siren.network.0.layer.weight", "siren.network.7.layer.bias", "siren.final_layer.weight",
-          "siren.color_layer_sine.2.layer.bias", "siren.color_layer_linear.0.weight",
-          "siren.label_layer_linear.1.weight", "siren.geo_mapping_network.network.8.bias",
-          "siren.app_mapping_network.network.8.bias"],
-    "B": ["siren.network.0.layer.weight", "siren.network.3.layer.weight", "siren.network.7.layer.bias",
-          "siren.final_layer.weight", "siren.final_layer.bias", "siren.color_layer_sine.0.layer.weight",
-          "siren.color_layer_sine.2.layer.bias", "siren.color_layer_linear.0.weight", "siren.color_layer_linear.0.bias",
-          "siren.label_layer_linear.0.weight", "siren.label_layer_linear.1.bias", "siren.label_layer_linear.2.weight",
-          "siren.geo_mapping_network.network.8.bias", "siren.app_mapping_network.network.8.bias"],
-}
-#: model B's grid gradient is 113 MB: stored as a fixed random projection (and its abs-sum)
-GRID_PROBE = 4096
+def _loss(pixels):
+    return (pixels * _cases.loss_weights(pixels.shape)).sum()
 
 
 def grad_goldens():
-    """tests/golden/grad_<case>.npz: d L / d (latents, selected parameters) of the reference's forward with
-    autograd on, same seed protocol (and therefore the same random draws) as the forward goldens."""
+    """tests/golden/grad_<case>.npz: d L / d (latents, GRAD_PARAMS[case]) of the reference's forward with autograd on,
+    same seed protocol (and therefore the same random draws) as the forward goldens; a grid's gradient as
+    MODEL_DATA[m]["grid_probe"] says."""
     ref_generators, ref_siren, _ = ref_shim.load()
     out_dir = os.path.dirname(os.path.abspath(__file__))
-    for name in GRAD_CASES:
+    for name, keys in _cases.GRAD_PARAMS.items():
         case = _cases.CASE_BY_NAME[name]
         gen, _ = build_reference(case, ref_generators, ref_siren)
         latents = tuple(z.clone().requires_grad_(True) for z in _cases.make_latents(case))
         torch.manual_seed(case.seed)
         kw = {k: v for k, v in case.cfg.items() if k != "fill_mode"}      # forward() of a staged case: same config
         pixels, _ = gen(*latents, **kw)
-        loss = (pixels * _cases.loss_weights(pixels.shape)).sum()
+        loss = _loss(pixels)
         loss.backward()
         params = dict(gen.named_parameters())
         out = {"loss": np.array(loss.item())}
         for i, z in enumerate(latents):
             out["latent%d" % i] = z.grad.numpy()
-        for k in GRAD_PARAMS[case.model]:
+        for k in keys:
             out[k] = params[k].grad.numpy()
-        if "siren.spatial_embeddings" in params:
+        probe = _cases.model_data(case.model, "grid_probe")
+        if probe:
             g = params["siren.spatial_embeddings"].grad.reshape(-1)
-            idx = _cases.grid_probe_index(g.numel(), GRID_PROBE)
+            if probe == "random":
+                idx = _cases.grid_probe_index(g.numel(), _cases.GRID_PROBE)
+            else:
+                idx = g.abs().topk(_cases.GRID_PROBE).indices.sort().values
+                out["grid_probe_idx"] = idx.numpy()
             out["grid_probe"] = g[idx].numpy()
             out["grid_abs_sum"] = np.array(g.abs().sum().item())
         path = os.path.join(out_dir, "grad_%s.npz" % name)
@@ -131,25 +136,19 @@ def grad_goldens():
 
 
 def frequency_grad_goldens():
-    """tests/golden/gradfreq_a_small.npz: the inversion call -- d L / d (frequencies, phase_shifts) through
+    """tests/golden/gradfreq_<case>.npz: the inversion call -- d L / d (frequencies, phase_shifts) through
     forward_with_frequencies (inverse_render_double_semantic.py:385-407, generators.py:353-431)."""
     ref_generators, ref_siren, _ = ref_shim.load()
     out_dir = os.path.dirname(os.path.abspath(__file__))
-    for name in ("a_small", "d_small"):
+    for name in _cases.GRADFREQ:
         case = _cases.CASE_BY_NAME[name]
         gen, _ = build_reference(case, ref_generators, ref_siren)
-        latents = _cases.make_latents(case)
         with torch.no_grad():
-            if case.model == "A":
-                fp = list(gen.siren.mapping_network(latents[0]))
-            else:
-                fg, pg = gen.siren.geo_mapping_network(latents[0])
-                fa, pa = gen.siren.app_mapping_network(latents[1])
-                fp = [fg, fa, pg, pa]
-        fp = [t.clone().requires_grad_(True) for t in fp]
+            leaves, order = _cases.frequency_leaves(gen.siren, _cases.make_latents(case), case.model)
+        fp = [t.clone().requires_grad_(True) for t in leaves]
         torch.manual_seed(case.seed)
-        pixels, _ = gen.forward_with_frequencies(*fp, **case.cfg)
-        loss = (pixels * _cases.loss_weights(pixels.shape)).sum()
+        pixels, _ = gen.forward_with_frequencies(*[fp[i] for i in order], **case.cfg)
+        loss = _loss(pixels)
         loss.backward()
         out = {"loss": np.array(loss.item())}
         for i, t in enumerate(fp):
@@ -249,7 +248,7 @@ def part_forward_goldens():
         out["draw%d_%s" % (i, kind)] = t.numpy()
     for i, z in enumerate(latents):
         out["g_latent%d" % i] = z.grad.numpy()
-    for k in GRAD_PARAMS[case.model]:
+    for k in _cases.GRAD_PARAMS[case.name]:
         out["g_" + k] = params[k].grad.numpy()
     path = os.path.join(out_dir, "part_d_small.npz")
     np.savez_compressed(path, **out)
@@ -257,35 +256,46 @@ def part_forward_goldens():
                                                         os.path.getsize(path) / 1024))
 
 
+def _write_gz(path, obj):
+    buf = io.BytesIO()
+    torch.save(obj, buf)
+    # (mtime 0: the gzip header carries no time stamp, so regenerating gives the same bytes)
+    with open(path, "wb") as raw, gzip.GzipFile(filename="", mode="wb", compresslevel=9, fileobj=raw, mtime=0) as f:
+        f.write(buf.getvalue())
+
+
 def dropin_goldens():
-    """What tests/test_dropin.py needs from the reference, so that it runs without it:
-      dropin_ref_<model>.pth.gz (+ .meta.gz)  whole-module checkpoints written by the reference's classes
-          (torch.save(generator), train_double_latent_semantic.py:523 style) and the parameter names / state_dict beside
-          them; every state_dict tensor is filled with its own constant (i + 1) / 64 so that the files compress to a few KB
-          and a key mix-up still shows
+    """What the drop-in tests need from the reference, so that they run without it, for every model with
+    MODEL_DATA[m]["dropin"]:
+      dropin_ref_<model>.pth.gz  a whole-module checkpoint written by the reference's classes (torch.save(generator),
+          train_double_latent_semantic.py:523 style); every state_dict tensor is filled with its own constant
+          (i + 1) / 64 so that the file compresses to a few KB and a key mix-up still shows.  "full" sets step and epoch
+      dropin_ref_<model>.pth.meta.gz  ("full") the parameter names and the state_dict beside it; ("shapes", no
+          checkpoint) the parameter names and the state-dict shapes of the unfilled generator
       dropin_ref_layout.json  the module names of the reference's generators / siren packages and the model / generator
           names of three curriculums"""
-    import gzip
-    import io
-    import json
     ref_generators, ref_siren, ref_curriculums = ref_shim.load()
     out_dir = os.path.dirname(os.path.abspath(__file__))
-    for model in ("A", "D"):
+    for model in _cases.MODELS:
+        kind = _cases.model_data(model, "dropin")
+        if not kind:
+            continue
         torch.manual_seed(0)
-        if model == "A":
-            gen = ref_generators.ImplicitGenerator3d(ref_siren.TALLSIREN, 256, 4)
-        else:
-            gen = ref_generators.DoubleImplicitGenerator3d(ref_siren.SIRENBASELINESEMANTICDISENTANGLE, 256, 256, 22)
+        gen = _cases.construct(ref_generators, ref_siren, model)
         gen.set_device("cpu")
-        gen.step, gen.epoch = 1234, 7
+        path = os.path.join(out_dir, "dropin_ref_%s.pth" % model)
+        if kind == "shapes":
+            _write_gz(path + ".meta.gz", {"names": [n for n, _ in gen.named_parameters()],
+                                          "state": {k: tuple(v.shape) for k, v in gen.state_dict().items()}})
+            continue
+        if kind == "full":
+            gen.step, gen.epoch = 1234, 7
         with torch.no_grad():
             for i, t in enumerate(gen.state_dict().values()):
                 t.fill_((i + 1) / 64.0)
-        for suffix, obj in (("", gen), (".meta", {"names": [n for n, _ in gen.named_parameters()], "state": gen.state_dict()})):
-            buf = io.BytesIO()
-            torch.save(obj, buf)
-            with gzip.open(os.path.join(out_dir, "dropin_ref_%s.pth%s.gz" % (model, suffix)), "wb", compresslevel=9) as f:
-                f.write(buf.getvalue())
+        _write_gz(path + ".gz", gen)
+        if kind == "full":
+            _write_gz(path + ".meta.gz", {"names": [n for n, _ in gen.named_parameters()], "state": gen.state_dict()})
     root = ref_shim.REFERENCE_ROOT
 
     def modules(pkg):
@@ -301,9 +311,30 @@ def dropin_goldens():
         f.write("\n")
 
 
+def init_goldens():
+    """INIT_GOLDENS: per field class, built under torch.manual_seed(0) with its arguments, the state digest
+    (tests/_harness.py), parameter names, state-dict keys and shapes, child names, and the first draw of the RNG after the
+    constructor (the init consumed exactly the reference's draws)."""
+    _, ref_siren, _ = ref_shim.load()
+    out_dir = os.path.dirname(os.path.abspath(__file__))
+    for fname, (_, names) in _cases.INIT_GOLDENS.items():
+        out = {}
+        for name in names:
+            torch.manual_seed(0)
+            siren = _cases.construct_field(ref_siren, name)
+            out[name] = {"digest": state_digest(siren), "names": [n for n, _ in siren.named_parameters()],
+                         "state": {k: list(v.shape) for k, v in siren.state_dict().items()},
+                         "children": [n for n, _ in siren.named_children()], "next_draw": torch.rand(1).item()}
+        with open(os.path.join(out_dir, fname), "w") as f:
+            json.dump(out, f, indent=1, sort_keys=True)
+        print(fname, {k: v["digest"][:12] for k, v in out.items()})
+
+
 if __name__ == "__main__":
     if sys.argv[1:2] == ["--dropin"]:
         dropin_goldens()
+    elif sys.argv[1:2] == ["--init"]:
+        init_goldens()
     elif sys.argv[1:2] == ["--part"]:
         part_forward_goldens()
     elif sys.argv[1:2] == ["--grads"]:

@@ -1,23 +1,17 @@
 """Bridge fields (SPATIALSIRENAUGDISENTANGLE, RESSIRENDISENTANGLE): the colour branch starts from a 3-wide v taken off the
-trunk output.  CPU: the mirror against the reference's init, the flag rules of the C-ABI, the restatement's faults and
-the faults the backward's bounds catch.  GPU: both point-network kernels under the tile schedules of a real SM count,
-the density-only entries, and the backward under the chunk layouts of production, against a float64 restatement."""
+trunk output.  CPU: the field spec, the flag rules of the C-ABI, the restatement's faults and the faults the backward's
+bounds catch.  GPU: both point-network kernels under the tile schedules of a real SM count, the density-only entries, the
+GUARD refinement, and the backward under the chunk layouts of production, against a float64 restatement.  The init,
+oracle, drop-in, end-to-end, gradient, inversion and repack checks of these fields run with every other field's, in
+test_oracle.py, test_dropin.py and test_gpu_parity.py."""
 import copy
 import ctypes
-import gzip
-import io
-import json
-import os
-
-import numpy as np
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-import _bridge_fields as BF
 import _cases
-import _harness
 import test_gpu_fp64_film_edges as FE
 from _fp64 import _film, _siren, field_ref
 from fenerf_b200 import _lib, backward, ops, packing
@@ -27,7 +21,7 @@ from test_gpu_fp64_reference import (FIELD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field
                                      _grad_errors, _per_point)
 
 DEV = "cuda:0"
-GOLDEN = _cases.GOLDEN_DIR
+CLASSES = _cases.INIT_GOLDENS["bridge_init.json"][1]
 #: point network forward, max |out - fp64| over the rgb / the sigma channels, per model.  Measured on an H100 80GB HBM3
 #: (132 SMs, 400 W power limit) at up to 20,000 points per image and under the four tile schedules (up to 33,691 points
 #: per image): exact <= 1.1e-6 (rgb, AUG at 4sms_minus_1), 8.4e-7 (AUG sigma), 9.7e-6 (RES sigma, scaled chain); fast
@@ -40,40 +34,18 @@ EXACT_BOUND = {"aug": (2e-6, 2e-6), "res": (2e-6, 1e-7), "res_scaled": (2e-6, 2e
 
 def _mirror(name, seed=0):
     torch.manual_seed(seed)
-    return getattr(S, name)(*BF.ARGS)
+    return _cases.construct_field(S, name)
+
+
+@pytest.mark.parametrize("name", CLASSES)
+def test_field_spec(name):
+    spec = _mirror(name).field_spec()
+    assert spec.bridge and spec.bridge_res == (name == "RESSIRENDISENTANGLE") and spec.out_dim == 4
 
 
 # --------------------------------------------------------------------------------------------
 # CPU: the mirror classes
 # --------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name", BF.CLASSES)
-def test_mirror_init_and_state_dict_are_the_references(name):
-    with open(os.path.join(GOLDEN, "bridge_init.json")) as f:
-        gold = json.load(f)[name]
-    siren = _mirror(name)
-    assert torch.rand(1).item() == gold["next_draw"]          # the init drew exactly what the reference's draws
-    assert _harness.state_digest(siren) == gold["digest"]
-    assert [n for n, _ in siren.named_parameters()] == gold["names"]
-    assert {k: list(v.shape) for k, v in siren.state_dict().items()} == gold["state"]
-    assert [n for n, _ in siren.named_children()] == gold["children"]
-    spec = siren.field_spec()
-    assert spec.bridge and spec.bridge_res == (name == "RESSIRENDISENTANGLE") and spec.out_dim == 4
-
-
-@pytest.mark.parametrize("name", BF.CLASSES)
-def test_mirror_pickles_and_resolves_by_name(name):
-    import fenerf_b200
-    fenerf_b200.install()
-    import siren.siren as installed
-    assert getattr(installed, name) is getattr(S, name)
-    siren = _mirror(name)
-    buf = io.BytesIO()
-    torch.save(siren, buf)
-    back = torch.load(io.BytesIO(buf.getvalue()), map_location="cpu", weights_only=False)
-    assert type(back) is getattr(S, name)
-    assert all(torch.equal(a, b) for a, b in zip(siren.state_dict().values(), back.state_dict().values()))
-
-
 def _desc(flags, label_dim=0, grid=0, color=8):
     return _lib.FieldDesc(trunk_layers=8, color_layers=color, label_dim=label_dim, grid_channels=grid,
                           grid_res=64 if grid else 0, out_dim=label_dim + 4, input_scale=2 / 0.24, reserved=flags)
@@ -95,7 +67,7 @@ def test_bridge_bits_only_in_the_reference_shapes():
     aligned = (ctypes.addressof(buf) + 1023) // 1024 * 1024
     assert lib.fenerf_pack_field(ctypes.byref(_desc(BR | RES, color=6)), ctypes.byref(params), aligned, 1, None) == -1
     assert b"fenerf_bridge_params" in lib.fenerf_last_error()
-    for name in BF.CLASSES:
+    for name in CLASSES:
         d = packing.field_desc(_mirror(name).field_spec())
         assert d.reserved == (BR | RES if name == "RESSIRENDISENTANGLE" else BR)
         assert lib.fenerf_packed_bytes(ctypes.byref(d)) > 0
@@ -104,7 +76,7 @@ def test_bridge_bits_only_in_the_reference_shapes():
 def _cpu_inputs(name, seed, n=64, scaled=False):
     siren = _mirror(name, seed).double()
     if scaled:
-        BF.scale_density(siren)
+        _cases.scale_density(siren)
     film = _film(siren.float(), 2, seed).double()
     siren.double()
     g = torch.Generator().manual_seed(seed)
@@ -130,7 +102,7 @@ def test_faults_move_the_restatement_past_the_bounds(name, fault):
 
 def test_restatement_runs_the_mirror_forward():
     """The mirror's module structure is what the restatement reads: every parameter meets the output."""
-    for name in BF.CLASSES:
+    for name in CLASSES:
         siren, film, pts, dirs = _cpu_inputs(name, 3, n=8, scaled=name == "RESSIRENDISENTANGLE")
         out = oracle.bridge_field_eval(siren, pts, film, dirs)
         out.sum().backward()
@@ -194,7 +166,7 @@ _IDS = ["aug", "res", "res_scaled"]
 def _gpu_inputs(name, scaled, batch, ppb, seed=7):
     siren = _mirror(name, seed)
     if scaled:
-        BF.scale_density(siren)
+        _cases.scale_density(siren)
     siren = siren.to(DEV)
     film = _film(siren, batch, seed).contiguous()
     g = torch.Generator().manual_seed(seed)
@@ -259,8 +231,8 @@ _BWD = ([(lay, m, False, False) for lay in ("L1", "L2", "L3") for m in _IDS]
 def _bridge_siren(model_id, device):
     """The generator's field (the seed protocol of _fp64._siren); res_scaled with the density chain scaled."""
     name, scaled = MODELS[_IDS.index(model_id)]
-    siren = _siren("M" if name == BF.CLASSES[0] else "N", device)
-    return BF.scale_density(siren) if scaled else siren
+    siren = _siren("M" if name == CLASSES[0] else "N", device)
+    return _cases.scale_density(siren) if scaled else siren
 
 
 @pytest.mark.gpu
@@ -347,134 +319,3 @@ def test_guard_refinement(model):
 # --------------------------------------------------------------------------------------------
 # render level: the oracle and the library against the reference's goldens
 # --------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", BF.CASES, ids=lambda c: c.name)
-def test_oracle_matches_reference_golden(case):
-    from test_hd_fields import _golden_pixels
-    if case.name in BF.BIG and not os.environ.get("FENERF_SLOW_TESTS") and not torch.cuda.is_available():
-        pytest.skip("minutes of CPU oracle (FENERF_SLOW_TESTS=1 runs it)")
-    gold = np.load(_cases.golden_path(case))
-    run = _harness.oracle_run(case, keep_stages=False)
-    got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
-    assert (got - want).abs().max() <= 2e-5
-
-
-@pytest.mark.parametrize("model", sorted(BF.MODELS))
-def test_reference_checkpoint_loads_under_the_mirror(model):
-    """A generator saved with torch.save by the reference's classes loads after install() into the mirror classes, with
-    the reference's parameter order and state_dict; the mirror's own checkpoint has the same layout."""
-    import fenerf_b200
-    fenerf_b200.install()
-    with gzip.open(os.path.join(GOLDEN, "dropin_ref_%s.pth.gz" % model), "rb") as f:
-        gen = torch.load(io.BytesIO(f.read()), map_location="cpu", weights_only=False)
-    name = BF.MODELS[model][1]
-    assert type(gen.siren) is getattr(S, name)
-    mine = _cases.build_mirror(_cases.Case("x", model, 1, 0), "cpu")
-    assert [n for n, _ in gen.named_parameters()] == [n for n, _ in mine.named_parameters()]
-    assert list(gen.state_dict()) == list(mine.state_dict())
-    for i, t in enumerate(gen.state_dict().values()):
-        assert torch.all(t == (i + 1) / 64.0)
-    with torch.no_grad():
-        gen.siren.load_state_dict(mine.siren.state_dict())       # the loaded object is a working mirror
-    assert gen.siren.field_spec() == mine.siren.field_spec()
-
-
-@pytest.fixture(scope="module")
-def runs():
-    cache = {}
-
-    def get(name):
-        if name not in cache:
-            case = _cases.CASE_BY_NAME[name]
-            cache[name] = (case, _harness.oracle_run(case))
-        return cache[name]
-    return get
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("case", BF.CASES, ids=lambda c: c.name)
-@pytest.mark.parametrize("precision,tol", [("exact", 2e-4), ("guard", 1e-3)])
-def test_end_to_end_against_reference_golden(runs, case, precision, tol):
-    import test_gpu_parity as p
-    from test_hd_fields import _golden_pixels
-    gold = np.load(_cases.golden_path(case))
-    case, run = runs(case.name)
-    gen, pixels, poses, depth_map = p._end_to_end(case, run, precision)
-    ill_rays = p._ill_conditioned_pixels(case, run)
-    got, want, idx = _golden_pixels(pixels, gold)
-    err = (got - want).abs()
-    assert int(ill_rays.sum()) <= max(2, 0.002 * ill_rays.numel())
-    ill = ill_rays.unsqueeze(1).expand_as(pixels).reshape(-1)
-    if idx is not None:
-        ill = ill[idx]
-    print("%s %s: max err %.3g" % (case.name, precision, err[~ill].max()))
-    assert err[~ill].max() <= tol
-    if poses is not None:
-        assert (poses - torch.from_numpy(gold["poses"])).abs().max() <= 1e-5
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", BF.GRAD_CASES)
-@pytest.mark.parametrize("precision", ["exact", "guard"])
-def test_generator_gradients_match_reference(runs, name, precision):
-    """forward() with autograd (the RenderFunction, parameters mapped by identity) against the reference's autograd on the
-    opaque case: <= 5e-4 of each tensor's max in exact mode, <= 2e-2 in the default mode."""
-    import test_gpu_parity as p
-    from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    case, run = runs(name)
-    gold = np.load(os.path.join(GOLDEN, "grad_%s.npz" % name))
-    gen = _cases.build_mirror(case, DEV)
-    latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
-    pixels, _ = gen(*latents, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision=precision))
-    (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-    got = {"latent%d" % i: z.grad for i, z in enumerate(latents)}
-    got.update({k: q.grad for k, q in gen.named_parameters()})
-    worst = p._compare_grads(gold, got, rel=5e-4 if precision == "exact" else 2e-2,
-                             kink_rel=1e-2 if precision == "exact" else 0.3)
-    print("gradients %s %s: %s" % (name, precision, {k: "%.1e" % v for k, v in worst.items()}))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", BF.GRAD_CASES)
-def test_inversion_gradients_through_forward_with_frequencies(runs, name):
-    import test_gpu_parity as p
-    from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    case, run = runs(name)
-    gold = np.load(os.path.join(GOLDEN, "gradfreq_%s.npz" % name))
-    gen = _cases.build_mirror(case, DEV)
-    with torch.no_grad():
-        lat = [p._cuda(z) for z in run["latents"]]
-        fp = [t.clone().requires_grad_(True) for t in gen.siren.geo_mapping_network(lat[0]) + gen.siren.app_mapping_network(lat[1])]
-    for q in gen.parameters():
-        q.requires_grad_(False)
-    pixels, _ = gen.forward_with_frequencies(fp[0], fp[2], fp[1], fp[3],
-                                             **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="exact"))
-    (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-    worst = p._compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=5e-4)
-    print("inversion %s: %s" % (name, worst))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", BF.CLASSES)
-def test_staged_forward_sees_bridge_parameter_writes(name):
-    """torch_ema's copy_to writes through param.data without a version bump: a write to v's Linear alone -- and, for RES,
-    to color_layer_pre or the density chain alone -- must reach staged_forward (the fingerprint covers them)."""
-    model = "M" if name == BF.CLASSES[0] else "N"
-    case = _cases.CASE_BY_NAME["%s_small_opaque" % model.lower()]
-    gen = _cases.build_mirror(case, DEV)
-    s = gen.siren
-    targets = [s.color_layer_pre[0].weight] if model == "M" else [s.res_coord_layer.weight, s.color_layer_pre[0].weight,
-                                                                   s.density_layer_linear[1].weight]
-    g = torch.Generator().manual_seed(8)
-    z = [torch.randn(1, 256, generator=g).to(DEV) for _ in range(2)]
-    kw = dict(case.cfg, psi=0.7, max_batch_size=2400000, precision="exact")
-
-    def render():
-        torch.manual_seed(1)
-        return torch.cat([t.reshape(-1).cpu() for t in gen.staged_forward(*z, **kw)[:2]])
-    with torch.no_grad():
-        for w in targets:
-            a = render()
-            w.data.copy_(w.detach() * -3.0)
-            b = render()
-            s.invalidate_packed()
-            assert not torch.equal(a, b) and torch.equal(b, render())

@@ -1,7 +1,7 @@
 """The drop-in boundary, proven with the reference's own call sequence (SURVEY.md section 8b).
 
-CPU part (this file, ``-m "not gpu"``): every test runs in a fresh interpreter, because ``install()``
-edits ``sys.modules``.
+CPU part (this file, ``-m "not gpu"``): the call sequences run in a fresh interpreter, because ``install()``
+edits ``sys.modules``; the per-model checkpoint and pickle checks run in this one.
   * stand-alone install (no reference on sys.path): the two submodule names resolve to the mirror;
   * next to a tree with the reference's package layout (its module names, recorded in
     tests/golden/dropin_ref_layout.json): after ``install()`` the reference's sibling modules stay importable
@@ -12,12 +12,15 @@ edits ``sys.modules``.
     tests/golden/dropin_ref_*.pth.gz) loads under the mirror with an identical state_dict and the same parameter
     order, so torch_ema's positional ``copy_to`` / ``restore`` (``param.data.copy_``) lands on the right tensors;
   * a checkpoint written under the mirror references the same classes and carries the same attributes and
-    state_dict layout as the reference's own.
-tests/golden/make_goldens.py --dropin records those files from the unmodified reference.
+    state_dict layout as the reference's own;
+  * every field class with a reference file pickles without its device buffers and resolves by name after install().
+tests/golden/make_goldens.py --dropin records those files from the unmodified reference, for every model of
+tests/_cases.py's MODEL_DATA with a `dropin` entry.
 GPU part: tests/test_gpu_parity.py::test_render_script_call_sequence replays
 render_multiview_images_double_semantic.py:43-65 against a golden.
 """
 import gzip
+import io
 import json
 import os
 import shutil
@@ -25,6 +28,9 @@ import subprocess
 import sys
 
 import pytest
+import torch
+
+import _cases
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -138,10 +144,64 @@ print("ok")
 '''
 
 
-@pytest.mark.parametrize("model", ["A", "D"])
+def _models_with(*kinds):
+    return [m for m in _cases.MODELS if _cases.model_data(m, "dropin") in kinds]
+
+
+@pytest.mark.parametrize("model", _models_with("full"))
 def test_reference_pickle_loads_under_the_mirror(tmp_path, model):
     out = _run(_LOAD_WITH_MIRROR, _reference_checkpoint(tmp_path, model))
     assert "ok" in out
+
+
+@pytest.mark.parametrize("model", _models_with("full", "bare"))
+def test_reference_checkpoint_loads_under_the_mirror(model):
+    """A generator saved with torch.save by the reference's classes loads after install() into the mirror classes, with
+    the reference's parameter order and state_dict; the mirror's own checkpoint has the same layout."""
+    import fenerf_b200
+    from fenerf_b200.siren import siren as S
+    fenerf_b200.install()
+    with gzip.open(os.path.join(GOLDEN, "dropin_ref_%s.pth.gz" % model), "rb") as f:
+        gen = torch.load(io.BytesIO(f.read()), map_location="cpu", weights_only=False)
+    assert type(gen.siren) is getattr(S, _cases.MODELS[model][1])
+    mine = _cases.build_mirror(_cases.Case("x", model, 1, 0), "cpu")
+    assert [n for n, _ in gen.named_parameters()] == [n for n, _ in mine.named_parameters()]
+    assert list(gen.state_dict()) == list(mine.state_dict())
+    for i, t in enumerate(gen.state_dict().values()):
+        assert torch.all(t == (i + 1) / 64.0)
+    with torch.no_grad():
+        gen.siren.load_state_dict(mine.siren.state_dict())       # the loaded object is a working mirror
+    assert gen.siren.field_spec() == mine.siren.field_spec()
+
+
+#: the field classes whose reference checkpoint or init golden the tests hold
+_PICKLED = [_cases.MODELS[m][1] for m in _models_with("full", "bare", "shapes")] + list(_cases.INIT_CLASSES)
+
+
+@pytest.mark.parametrize("name", _PICKLED)
+def test_mirror_pickles_and_resolves_by_name(name):
+    """The mirror field pickles without its device buffers, loads back as the same class, and install() resolves the
+    class by its name in the reference's module."""
+    import fenerf_b200
+    from fenerf_b200.siren import siren as S
+    fenerf_b200.install()
+    import siren.siren as installed
+    assert getattr(installed, name) is getattr(S, name)
+    if name in _cases.INIT_CLASSES:
+        torch.manual_seed(0)
+        field = _cases.construct_field(S, name)
+    else:
+        model = next(m for m, row in _cases.MODELS.items() if row[1] == name)
+        field = _cases.build_mirror(_cases.Case("x", model, 1, 0), "cpu").siren
+    field.__dict__["_packed_cache"] = ("stand-in",)
+    field.__dict__["_field_plist"] = ("stand-in",)
+    buf = io.BytesIO()
+    torch.save(field, buf)
+    assert b"_packed_cache" not in buf.getvalue() and b"_field_plist" not in buf.getvalue()
+    back = torch.load(io.BytesIO(buf.getvalue()), map_location="cpu", weights_only=False)
+    assert type(back) is getattr(S, name)
+    assert list(back.state_dict()) == list(field.state_dict())
+    assert all(torch.equal(a, b) for a, b in zip(field.state_dict().values(), back.state_dict().values()))
 
 
 def test_mirror_pickle_loads_under_the_reference(tmp_path):

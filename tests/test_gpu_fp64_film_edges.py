@@ -8,7 +8,7 @@ row's frequencies; [dir] alone for model L, whose grid feeds layer 0) and the la
 every image and in another column of the last image only, so that image b0 > 0 of a multi-image chunk sees it.  The
 committed bounds of test_gpu_fp64_reference.py apply unchanged, to every tensor and to each planted column on its own
 (relative to its layer's maximum, so that a wrong column cannot hide behind a right maximum); model L keeps its own
-exact-mode bounds for the grid gradient and the forward (test_grid_trunk.py).
+exact-mode bounds for the grid gradient and the forward (tests/_cases.py, MODEL_DATA).
 
 Measured on an H100 80GB HBM3 (400 W): backward exact 1.7e-5, default 1.07e-2 (model H, L2; planted columns 8.0e-3),
 layout invariance within LAYOUT_BOUND; forward exact 2.2e-6, fast 7.9e-4 (model K).  Models J, L, M, N on the same
@@ -19,9 +19,10 @@ case gave NaN FiLM gradients at f = 0 in both precisions.
 import pytest
 import torch
 
+import _cases
 from _fp64 import EDGE_FREQS, _film, _siren, field_ref, film_rows, plant_frequencies
 from fenerf_b200 import backward, ops
-from test_gpu_fp64_reference import (FIELD_BOUND, FWD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward, _field_points,
+from test_gpu_fp64_reference import (FIELD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward, _field_points,
                                      _grad_errors, _per_point)
 
 DEV = "cuda:0"
@@ -80,15 +81,13 @@ def _planted_errors(d_film, grads, want_film, want, planted, layers):
 
 
 def _grad_bounds(names, precision):
-    """FIELD_BOUND, except the exact mode's grid gradient of model L (test_grid_trunk.GRID_BOUND_EXACT)."""
-    from test_grid_trunk import GRID_BOUND_EXACT
-    return {n: GRID_BOUND_EXACT if (precision == "exact" and n == "spatial_embeddings") else FIELD_BOUND[precision]
+    """FIELD_BOUND, except the exact mode's grid gradient: model L's bound (_cases.MODEL_DATA)."""
+    return {n: _cases.bound("L", "grid_exact") if (precision == "exact" and n == "spatial_embeddings") else FIELD_BOUND[precision]
             for n in names}
 
 
 def _fwd_bound(model, precision):
-    from test_grid_trunk import FWD_BOUND_L
-    return (FWD_BOUND_L if model == "L" else FWD_BOUND)[precision]
+    return _cases.bound(model, "fwd_" + precision)
 
 
 @gpu

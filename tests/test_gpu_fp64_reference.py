@@ -65,7 +65,17 @@ FWD_BOUND = {"exact": 1e-5, "fast": 5e-3}
 # --------------------------------------------------------------------------------------------
 # fields, FiLM tables, points
 # --------------------------------------------------------------------------------------------
-FIELD_MODELS = ("A", "B", "C", "D", "E", "F", "G", "H", "D32")   # S shares A's field; D32: the widest renderable head
+STOCK_FIELD_MODELS = ("A", "B", "C", "D", "E", "F", "G", "H", "D32")   # S shares A's field; D32: the widest renderable head
+#: and the field families: label FiLM, feature heads, grid trunk
+FIELD_MODELS = STOCK_FIELD_MODELS + ("I", "J", "K", "L")
+
+
+def _fwd_seed(model):
+    return _cases.model_data(model, "fwd_seed") or 2000 + FIELD_MODELS.index(model)
+
+
+def _bwd_seed(model, layout):
+    return (_cases.model_data(model, "bwd_seed") or 1000 + 10 * FIELD_MODELS.index(model)) + int(layout[1])
 
 
 def _render_points(batch, img, steps, seed):
@@ -378,7 +388,7 @@ _LAYOUTS = {
     "L4": (2, 393216, 24, None),        # cfg2's pass (128² rays x 24): one image per chunk, so b0 = 1
 }
 _FIELD = ([(lay, m, p, False) for lay in ("L1", "L2", "L3") for m in FIELD_MODELS for p in ("exact", "default")]
-          + [("L4", m, p, False) for m in ("A", "B") for p in ("exact", "default")]
+          + [("L4", m, p, False) for m in ("A", "B", "K") for p in ("exact", "default")]
           + [("L1", "A", p, True) for p in ("exact", "default")])
 
 
@@ -415,7 +425,7 @@ def test_field_backward_vs_fp64(monkeypatch, layout, model, precision, lock):
     if exact:
         monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)     # exact mode's torch.mm stays fp32
     siren = _siren(model, DEV)
-    seed = 1000 + 10 * FIELD_MODELS.index(model) + int(layout[1])
+    seed = _bwd_seed(model, layout)
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film = _film(siren, batch, seed, edges=True)
     out_dim = siren.field_spec().out_dim
@@ -428,7 +438,9 @@ def test_field_backward_vs_fp64(monkeypatch, layout, model, precision, lock):
     errs = _grad_errors(d_film, grads, want_film, want)
     worst = max(errs, key=errs.get)
     print("field %s %s %s: worst %s %.3g" % (layout, model, precision, worst, errs[worst]))
-    assert errs[worst] <= FIELD_BOUND[precision], {k: "%.2e" % v for k, v in errs.items() if v > FIELD_BOUND[precision]}
+    bound = {k: _cases.bound(model, "grid_exact") if (exact and k == "spatial_embeddings") else FIELD_BOUND[precision]
+             for k in errs}
+    assert all(errs[k] <= bound[k] for k in errs), {k: "%.2e" % v for k, v in errs.items() if v > bound[k]}
     if chunk:
         monkeypatch.setattr(backward, "CHUNK_POINTS", 1 << 30)
         d_film1, grads1 = _field_backward(siren, film, pts, dirs, dir_group, lock, raw, d_raw, exact)
@@ -465,20 +477,27 @@ def _forward_inputs(siren, layout, seed):
 def test_point_network_vs_fp64(model, layout):
     """Both point-network kernels against oracle.field_eval in float64, per output channel, under tile schedules derived
     from the device's SM count (one pair per CTA, a lone tile in a second pair, two pairs per CTA with the last half
-    empty, pairs across image borders); the density-only entry is bit-equal to the full fast evaluation."""
+    empty, pairs across image borders); both kernels are bit-identical between launches, and the density-only entries
+    are bit-equal to the full evaluations' sigma channel (the check that catches a density path without a grid gather)."""
     siren = _siren(model, DEV)
-    pts, dirs, film = _forward_inputs(siren, layout, 2000 + FIELD_MODELS.index(model))
+    pts, dirs, film = _forward_inputs(siren, layout, _fwd_seed(model))
     with torch.no_grad():
         exact = ops.siren_points(siren, pts, film, dirs, precision="exact")
+        exact2 = ops.siren_points(siren, pts, film, dirs, precision="exact")
         fast = ops.siren_points(siren, pts, film, dirs, precision="fast")
+        fast2 = ops.siren_points(siren, pts, film, dirs, precision="fast")
         sigma = ops.siren_sigma(siren, pts, film, precision="fast")
+        sigma_x = ops.siren_sigma(siren, pts, film, precision="exact")
     want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
     err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in (("exact", exact), ("fast", fast))}
-    print("forward %s %s: exact %.3g fast %.3g" % (model, layout, err["exact"].max(), err["fast"].max()))
+    print("forward %s %s: exact %.3g fast %.3g (sigma %.3g / %.3g)" % (model, layout, err["exact"].max(), err["fast"].max(),
+                                                                      err["exact"][-1], err["fast"][-1]))
     assert torch.isfinite(fast).all()
     for k in err:
-        assert err[k].max() <= FWD_BOUND[k], "%s: max |out - fp64| per channel %s" % (k, err[k].tolist())
+        assert err[k].max() <= _cases.bound(model, "fwd_" + k), "%s: max |out - fp64| per channel %s" % (k, err[k].tolist())
+    assert torch.equal(fast, fast2) and torch.equal(exact, exact2)
     assert torch.equal(sigma, fast[..., -1:])
+    assert torch.equal(sigma_x, exact[..., -1:])
 
 
 # --------------------------------------------------------------------------------------------

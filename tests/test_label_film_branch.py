@@ -2,20 +2,18 @@
 
     labels = Linear(256 -> 19)(FiLM_label(trunk output; FiLM row 8)),  rgb from the colour FiLM layer at row 9
 
-CPU (-m "not gpu"): the mirror's init, state_dict and pickles against the reference's, the oracle against the reference's
-forward goldens, the gradient goldens' coverage, the FiLM table order, the packed layout computed on the host, the
-flags word, the float64 restatement of the branch (gradcheck) and faults that the committed bounds must catch.
+CPU (-m "not gpu"): the mirror's module structure, the gradient goldens' coverage, the FiLM table order, the packed
+layout computed on the host, the flags word, the float64 restatement of the branch (gradcheck) and faults that the
+committed bounds must catch.
 
-GPU (-m gpu): end-to-end parity with the reference goldens, both point-network kernels against float64 under the tile
-schedules of the device, the GUARD refinement, the backward against the reference and against float64, the inversion
-path through FiLM row 8, and back-to-back ragged launches.
-
-Bounds are those of test_gpu_parity.py and test_gpu_fp64_reference.py.  Measured on an H100 80GB HBM3 (132 SMs):
+GPU (-m gpu): the installed class by name, and back-to-back ragged launches.  The end-to-end, point-network, GUARD,
+backward, inversion and repack checks of this field run with every other field's, in test_gpu_parity.py and
+test_gpu_fp64_reference.py (bounds in tests/_cases.py).  Measured on an H100 80GB HBM3 (132 SMs):
 
 | check | measured max | bound |
 |---|---|---|
 | end to end vs reference, exact | 2.4e-5 (i_cfg2) | 2e-4 |
-| end to end vs reference, default | 6.1e-4; i_cfg2 label channels 1.0e-3 | 1e-3; LABEL_TOL_CFG2 |
+| end to end vs reference, default | 6.1e-4; i_cfg2 label channels 1.0e-3 | 1e-3; render_guard_cfg2_labels 1.5e-3 |
 | point network vs float64, exact | 1.3e-6 | 1e-5 |
 | point network vs float64, fast | 4.6e-4 | 5e-3 |
 | gradients vs reference, default | 5.1e-3 (density head 2.9e-2, kink bound) | 2e-2 |
@@ -24,8 +22,6 @@ Bounds are those of test_gpu_parity.py and test_gpu_fp64_reference.py.  Measured
 """
 import copy
 import ctypes
-import gzip
-import io
 import os
 
 import numpy as np
@@ -34,62 +30,26 @@ import torch
 import torch.nn.functional as F
 
 import _cases
-import _harness
-import _label_film as LF
-from _fp64 import _film, _rel, _siren, field_ref
+from _fp64 import _film, _rel, _siren
 from fenerf_b200 import _lib, ops, packing
 from oracle import render_oracle as oracle
-from test_dropin import _LOAD_WITH_MIRROR, _reference_checkpoint, _run
-from test_gpu_fp64_reference import (FIELD_BOUND, FWD_BOUND, LAYOUT_BOUND, _LAYOUTS, _field_backward, _field_points,
-                                     _forward_inputs, _grad_errors, _per_point)
+from test_gpu_fp64_reference import FIELD_BOUND, FWD_BOUND, _field_points, _per_point
 
 DEV = "cuda:0"
 gpu = pytest.mark.gpu
-CASES = LF.CASES
 GOLDEN = _cases.GOLDEN_DIR
-TOL = 2e-5          # the oracle against the reference's goldens across hosts (test_oracle.py)
-
-
-def _gpu_parity():
-    import test_gpu_parity
-    return test_gpu_parity
 
 
 # --------------------------------------------------------------------------------------------
 # CPU: the mirror class
 # --------------------------------------------------------------------------------------------
-def test_mirror_init_and_state_dict_are_the_references():
-    """Same parameter names, order, shapes and values under manual_seed(0) (the golden's state digest covers keys and
-    bytes in order), and the same state_dict keys as the reference-made checkpoint."""
-    gold = np.load(_cases.golden_path(_cases.CASE_BY_NAME["i_small"]))
+def test_mirror_structure():
+    """The reference's child modules, in order (init, state dict and names: test_oracle.py, test_dropin.py)."""
     gen = _cases.build_mirror(_cases.CASE_BY_NAME["i_small"], "cpu")
-    assert _harness.state_digest(gen) == str(gold["state_digest"])
-    with gzip.open(os.path.join(GOLDEN, "dropin_ref_I.pth.meta.gz"), "rb") as f:
-        meta = torch.load(io.BytesIO(f.read()), map_location="cpu", weights_only=False)
-    assert list(gen.state_dict().keys()) == list(meta["state"].keys())
-    assert [n for n, _ in gen.named_parameters()] == meta["names"]
     names = [n for n, _ in gen.siren.named_children()]
     assert names == ["network", "final_layer", "label_layer_sine", "label_layer_linear", "color_layer_sine",
                      "color_layer_linear", "mapping_network", "activation", "gridwarper"]
     assert gen.siren.max_batch_size == 2500 and isinstance(gen.siren.activation, torch.nn.Softmax)
-
-
-def test_reference_pickle_loads_under_the_mirror(tmp_path):
-    out = _run(_LOAD_WITH_MIRROR, _reference_checkpoint(tmp_path, "I"), ref="")
-    assert "ok" in out
-
-
-def test_mirror_pickle_carries_no_device_buffers():
-    gen = _cases.build_mirror(_cases.CASE_BY_NAME["i_small"], "cpu")
-    gen.siren.__dict__["_packed_cache"] = ("stand-in",)
-    gen.siren.__dict__["_field_plist"] = ("stand-in",)
-    buf = io.BytesIO()
-    torch.save(gen, buf)
-    assert b"_packed_cache" not in buf.getvalue() and b"_field_plist" not in buf.getvalue()
-    back = torch.load(io.BytesIO(buf.getvalue()), weights_only=False)
-    assert type(back.siren).__name__ == "SPATIALSIRENSEMANTIC"
-    for k, v in gen.state_dict().items():
-        assert torch.equal(v, back.state_dict()[k]), k
 
 
 def test_film_table_has_ten_rows_in_the_reference_order():
@@ -144,33 +104,6 @@ def test_flags_word_rejects_unknown_bits_and_unbuildable_label_fields():
 # --------------------------------------------------------------------------------------------
 # CPU: the oracle against the reference's goldens
 # --------------------------------------------------------------------------------------------
-def _golden_pixels(pixels, gold):
-    """-> (got, want, flat index or None): every pixel, or the probe a cfg2-shaped golden stores."""
-    pixels = pixels.cpu()
-    if "pixel_probe" in gold.files:
-        assert tuple(pixels.shape) == tuple(gold["pixels_shape"])
-        idx = _cases.pixel_probe_index(pixels.numel())
-        return pixels.reshape(-1)[idx], torch.from_numpy(gold["pixel_probe"]), idx
-    assert tuple(pixels.shape) == gold["pixels"].shape
-    return pixels.reshape(-1), torch.from_numpy(gold["pixels"]).reshape(-1), None
-
-
-@pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
-def test_oracle_matches_reference_golden(case):
-    gold = np.load(_cases.golden_path(case))
-    run = _harness.oracle_run(case, keep_stages=False)
-    got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
-    diff = (got - want).abs()
-    assert diff.max() <= TOL, "max|oracle - reference| = %g" % diff.max()
-    if "pixels_abs_sum" in gold.files:
-        assert abs(run["out"]["pixels"].abs().sum().item() - float(gold["pixels_abs_sum"])) <= 1e-5 * float(gold["pixels_abs_sum"])
-    if "poses" in gold.files:
-        assert np.abs(run["out"]["poses"].numpy() - gold["poses"]).max() <= 1e-6
-    if "depth_map" in gold.files:
-        r = case.cfg["img_size"]
-        assert np.abs(run["out"]["depth"].reshape(case.batch, r, r).numpy() - gold["depth_map"]).max() <= TOL
-
-
 def test_gradient_goldens_cover_the_label_branch():
     """The gradient goldens hold the label FiLM layer, the label head and the mapping network; the frequency golden gives
     FiLM row 8 (the label layer) a non-zero gradient.  (The oracle renders under no_grad: the GPU tests below compare the
@@ -257,56 +190,6 @@ def test_faults_exceed_the_bounds(fault):
 # --------------------------------------------------------------------------------------------
 # GPU: end to end against the reference's goldens
 # --------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def runs():
-    cache = {}
-
-    def get(name):
-        if name not in cache:
-            case = _cases.CASE_BY_NAME[name]
-            cache[name] = (case, _harness.oracle_run(case))
-        return cache[name]
-    return get
-
-
-#: the default mode's label channels at cfg2 (128², 24 + 24): unlike rgb they pass through no sigmoid, so the fp16 label
-#: layer's error reaches the pixels undamped.  Measured 1.0e-3 (every other case and channel: <= 6.1e-4).
-LABEL_TOL_CFG2 = 1.5e-3
-
-
-@gpu
-@pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
-@pytest.mark.parametrize("precision,tol", [("exact", 2e-4), ("guard", 1e-3)])
-def test_end_to_end_against_reference_golden(runs, case, precision, tol):
-    """forward / staged_forward with the far-sigma exclusion rule of test_gpu_parity.py; exact <= 2e-4, default <= 1e-3
-    (cfg2's label channels in the default mode: LABEL_TOL_CFG2).  Measured: exact 2.4e-5 (i_cfg2), default 6.1e-4 on
-    the small cases."""
-    p = _gpu_parity()
-    gold = np.load(_cases.golden_path(case))
-    case, run = runs(case.name)
-    l0 = _lib.launch_count()
-    gen, pixels, poses, depth_map = p._end_to_end(case, run, precision)
-    assert _lib.launch_count() > l0
-    got, want, idx = _golden_pixels(pixels, gold)
-    err = (got - want).abs()
-    ill_rays = p._ill_conditioned_pixels(case, run)
-    assert int(ill_rays.sum()) <= max(2, 0.002 * ill_rays.numel())
-    ill = ill_rays.unsqueeze(1).expand_as(pixels).reshape(-1)
-    chan = torch.arange(pixels.numel()) // (pixels.shape[2] * pixels.shape[3]) % pixels.shape[1]
-    if idx is not None:
-        ill, chan = ill[idx], chan[idx]
-    lab, rgb = err[~ill & (chan < 19)], err[~ill & (chan >= 19)]
-    print("%s %s: max err labels %.3g rgb %.3g" % (case.name, precision, lab.max(), rgb.max()))
-    assert rgb.max() <= tol
-    assert lab.max() <= (LABEL_TOL_CFG2 if (precision == "guard" and case.name == "i_cfg2") else tol)
-    if case.name != "i_cfg2" or precision == "exact":
-        p._check_pixels(case, run, pixels, tol)
-    if poses is not None:
-        assert (poses - torch.from_numpy(gold["poses"])).abs().max() <= 1e-5
-    if depth_map is not None:
-        assert (depth_map - torch.from_numpy(gold["depth_map"])).abs()[~ill_rays].max() <= 3e-3
-
-
 @gpu
 def test_installed_generator_runs_the_class_by_name():
     import fenerf_b200
@@ -322,54 +205,6 @@ def test_installed_generator_runs_the_class_by_name():
 # --------------------------------------------------------------------------------------------
 # GPU: the point-network kernels
 # --------------------------------------------------------------------------------------------
-@gpu
-@pytest.mark.parametrize("layout", _cases.TILE_LAYOUTS)
-def test_point_network_vs_fp64(layout):
-    """Both kernels against the oracle's field evaluation (with the label branch) in float64 per channel (exact 1e-5, fast 5e-3); the fast kernel is
-    bit-identical between launches and its density-only entry equals its sigma channel."""
-    siren = _siren("I", DEV)
-    pts, dirs, film = _forward_inputs(siren, layout, 2100)
-    with torch.no_grad():
-        exact = ops.siren_points(siren, pts, film, dirs, precision="exact")
-        fast = ops.siren_points(siren, pts, film, dirs, precision="fast")
-        fast2 = ops.siren_points(siren, pts, film, dirs, precision="fast")
-        sigma = ops.siren_sigma(siren, pts, film, precision="fast")
-    want = field_ref(siren, pts, _per_point(dirs, pts.shape[1], False), film)[0]
-    err = {k: (v.double() - want).abs().amax((0, 1)) for k, v in (("exact", exact), ("fast", fast))}
-    print("forward I %s: exact %.3g (labels %.3g) fast %.3g (labels %.3g)" % (
-        layout, err["exact"].max(), err["exact"][:19].max(), err["fast"].max(), err["fast"][:19].max()))
-    assert torch.isfinite(fast).all()
-    for k in err:
-        assert err[k].max() <= FWD_BOUND[k], "%s: max |out - fp64| per channel %s" % (k, err[k].tolist())
-    assert torch.equal(fast, fast2)
-    assert torch.equal(sigma, fast[..., -1:])
-
-
-@gpu
-def test_guard_refined_rows_match_the_exact_kernel():
-    """The GUARD refinement re-evaluates the density of the far samples it lists with the exact kernel's trunk: those
-    densities equal the exact kernel's bit for bit, and every other value of the row (labels included) is the fast
-    pass's -- the refinement never touches the label branch."""
-    case = _cases.CASE_BY_NAME["i_small"]
-    siren = _siren("I", DEV)
-    film = _film(siren, 2, 77)
-    rd = ops.make_render_desc(batch=2, img_size=24, num_steps=12, hierarchical=False, clamp_mode="relu", nerf_noise=0.0,
-                              fov=12, precision="guard", guard_tau=1e9)                      # every ray refined
-    x_lin, y_lin, z_lin = ops.ray_tables(24, 12, case.cfg["ray_start"], case.cfg["ray_end"], DEV)
-    c2w = torch.eye(4, device=DEV).repeat(2, 1, 1)
-    c2w[:, 2, 3] = 1.0
-    rng = torch.rand(2, 24 * 24, 12, 1, generator=torch.Generator().manual_seed(4)).to(DEV)
-    with torch.no_grad():
-        st = ops.render_forward_stages(siren, rd, film, x_lin, y_lin, z_lin, c2w.contiguous(), rng, None, None, None)
-        pts, dirs = st["points_c"].reshape(2, -1, 3), st["dirs"]
-        fast = ops.siren_points(siren, pts, film, dirs, precision="fast").reshape(2, 24 * 24, 12, 23)
-        exact = ops.siren_points(siren, pts, film, dirs, precision="exact").reshape(2, 24 * 24, 12, 23)
-    raw = st["raw_c"]
-    assert torch.equal(raw[:, :, :-1], fast[:, :, :-1])
-    assert torch.equal(raw[:, :, -1, -1], exact[:, :, -1, -1])
-    assert torch.equal(raw[:, :, -1, :-1], fast[:, :, -1, :-1])
-
-
 @gpu
 def test_fast_kernel_stress_ragged_launches():
     """Back-to-back launches of ragged sizes on one stream, each against its own exact evaluation."""
@@ -391,94 +226,3 @@ def test_fast_kernel_stress_ragged_launches():
 # --------------------------------------------------------------------------------------------
 # GPU: the backward
 # --------------------------------------------------------------------------------------------
-@gpu
-@pytest.mark.parametrize("precision", ["exact", "guard"])
-def test_backward_matches_reference_gradients(runs, precision):
-    """Against the reference's autograd: <= 5e-4 of each tensor's max in exact mode, <= 2e-2 in the default mode (the
-    density head keeps test_gpu_parity.py's kink bound)."""
-    from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    p = _gpu_parity()
-    case, run = runs("i_small")
-    gold = np.load(os.path.join(GOLDEN, "grad_i_small.npz"))
-    gen = _cases.build_mirror(case, DEV)
-    latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
-    pixels, _ = gen(*latents, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision=precision))
-    loss = (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum()
-    loss.backward()
-    got = {"latent%d" % i: z.grad for i, z in enumerate(latents)}
-    got.update({k: q.grad for k, q in gen.named_parameters()})
-    worst = p._compare_grads(gold, got, rel=5e-4 if precision == "exact" else 2e-2,
-                             kink_rel=1e-2 if precision == "exact" else 0.3)
-    print("gradients %s: %s" % (precision, {k: "%.1e" % v for k, v in worst.items()}))
-
-
-@gpu
-@pytest.mark.parametrize("layout", ["L1", "L2", "L3"])
-@pytest.mark.parametrize("precision", ["exact", "default"])
-def test_field_backward_vs_fp64(monkeypatch, layout, precision):
-    """_FieldBackward against the float64 VJP under the chunk layouts L1-L3 (test_gpu_fp64_reference.py)."""
-    from fenerf_b200 import backward
-    batch, ppb, dir_group, chunk = _LAYOUTS[layout]
-    exact = precision == "exact"
-    if exact:
-        monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
-    siren = _siren("I", DEV)
-    seed = 3100 + int(layout[1])
-    pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
-    film = _film(siren, batch, seed, edges=True)
-    d_raw = torch.randn(batch, ppb, 23, generator=torch.Generator().manual_seed(seed)).to(DEV) * 1e-3
-    out64, want_film, want = field_ref(siren, pts, _per_point(dirs, ppb, False), film, d_raw)
-    raw = out64.float().contiguous()
-    if chunk:
-        monkeypatch.setattr(backward, "CHUNK_POINTS", chunk)
-    d_film, grads = _field_backward(siren, film, pts, dirs, dir_group, False, raw, d_raw, exact)
-    errs = _grad_errors(d_film, grads, want_film, want)
-    worst = max(errs, key=errs.get)
-    print("field I %s %s: worst %s %.3g (label layer %.3g, film8 %.3g)" % (
-        layout, precision, worst, errs[worst], errs["label_layer_sine.layer.weight"],
-        max(errs["film8.freq"], errs["film8.phase"])))
-    assert errs[worst] <= FIELD_BOUND[precision], {k: "%.2e" % v for k, v in errs.items() if v > FIELD_BOUND[precision]}
-    if chunk:
-        monkeypatch.setattr(backward, "CHUNK_POINTS", 1 << 30)
-        d_film1, grads1 = _field_backward(siren, film, pts, dirs, dir_group, False, raw, d_raw, exact)
-        inv = _grad_errors(d_film, grads, d_film1, grads1)
-        assert max(inv.values()) <= LAYOUT_BOUND
-
-
-@gpu
-def test_inversion_gradients_reach_the_label_row(runs):
-    """forward_with_frequencies (inverse_render_double_semantic.py:385-407) against the reference's frequency gradients,
-    FiLM row 8 included."""
-    from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    p = _gpu_parity()
-    case, run = runs("i_small")
-    gold = np.load(os.path.join(GOLDEN, "gradfreq_i_small.npz"))
-    gen = _cases.build_mirror(case, DEV)
-    with torch.no_grad():
-        fp = [t.clone().requires_grad_(True) for t in gen.siren.mapping_network(p._cuda(run["latents"][0]))]
-    for q in gen.parameters():
-        q.requires_grad_(False)
-    pixels, _ = gen.forward_with_frequencies(*fp, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="exact"))
-    (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-    worst = p._compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=5e-4)
-    row8 = max(_rel(t.grad[:, 8 * 256:9 * 256].cpu(), torch.from_numpy(gold["arg%d" % i])[:, 8 * 256:9 * 256])
-               for i, t in enumerate(fp))
-    print("inversion: %s, row 8 %.2e" % (worst, row8))
-    assert row8 <= 5e-4
-
-
-@gpu
-def test_label_film_weights_written_through_data_are_seen():
-    """An EMA-style write to the label FiLM layer's weights (param.data.copy_, no version bump) changes the fingerprint,
-    so staged_forward repacks."""
-    siren = _siren("I", DEV)
-    before = packing.fingerprint(siren)
-    w = siren.label_layer_sine.layer.weight
-    with torch.no_grad():
-        w.data.copy_(w.data * 1.5)
-    assert packing.fingerprint(siren) != before
-    w2 = siren.color_layer_sine.layer.weight
-    mid = packing.fingerprint(siren)
-    with torch.no_grad():
-        w2.data.copy_(w2.data * 1.5)
-    assert packing.fingerprint(siren) != mid

@@ -96,16 +96,15 @@ def test_descriptor_check_accepts_num_steps_up_to_256(num_steps):
 @pytest.mark.parametrize("case", ms.CASES, ids=lambda c: c.name)
 def test_goldens(case, precision, bound):
     """The generator API against the reference's output; rays whose far sample sits on the relu step (|sigma| below
-    test_gpu_parity.ILL_TAU, ill-conditioned for any fp32 render) are excluded, as the stock cases' tests do."""
+    _harness.ILL_TAU, ill-conditioned for any fp32 render) are excluded, as the stock cases' tests do."""
     import _harness
-    import test_gpu_parity as p
     run = _harness.oracle_run(case)
     gold = np.load(_cases.golden_path(case))
     l0 = _lib.launch_count()
-    _, pixels, poses, depth_map = p._end_to_end(case, run, precision)
+    _, pixels, poses, depth_map = _harness.end_to_end(case, run, precision)
     assert _lib.launch_count() > l0
     err = (pixels - torch.from_numpy(gold["pixels"])).abs()
-    ill = p._ill_conditioned_pixels(case, run).unsqueeze(1).expand_as(err)
+    ill = _harness.ill_conditioned_pixels(case, run).unsqueeze(1).expand_as(err)
     assert int(ill[:, 0].sum()) <= max(2, 0.002 * ill[:, 0].numel())
     print("%s %s: max|gpu - reference| = %.2e (%d rays excluded)" % (case.name, precision, err[~ill].max(),
                                                                      int(ill[:, 0].sum())))
@@ -138,7 +137,6 @@ def test_gradients_against_the_reference(precision, rel, kink):
     """forward() at 96 + 96 with autograd: the bounds of the stock gradient goldens (test_gpu_parity.py) and, in the
     default precision, the density bias measured against the density head's weight gradient (test_point_forward.py)."""
     import _harness
-    import test_gpu_parity as p
     case = ms.CASE_BY_NAME[ms.GRAD_CASE]
     run = _harness.oracle_run(case, keep_stages=False)
     gold = np.load(ms.grad_golden_path())
@@ -159,7 +157,7 @@ def test_gradients_against_the_reference(precision, rel, kink):
         keys.remove(bias)
     kept = {k: gold[k] for k in keys}
     gold = type("Gold", (), {"files": keys, "__getitem__": lambda self, k: kept[k]})()
-    worst = p._compare_grads(gold, got, rel=rel, kink_rel=kink)
+    worst = _harness.compare_grads(gold, got, rel=rel, kink_rel=kink)
     print("forward %s, 96 + 96: %s" % (precision, {k: "%.1e" % v for k, v in worst.items()}))
 
 

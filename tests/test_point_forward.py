@@ -13,6 +13,7 @@ import pytest
 import torch
 
 import _cases
+import _harness
 import _point_forward as pf
 from fenerf_b200 import _lib, backward, ops
 from fenerf_b200.generators import volumetric_rendering as vr
@@ -247,7 +248,6 @@ def test_rays_in_equals_the_camera_render(model, precision, shape):
 @gpu
 @pytest.mark.parametrize("precision,rel,kink", [("exact", 5e-4, 1e-2), ("guard", 2e-2, 0.3)])
 def test_gradients_against_the_reference(precision, rel, kink):
-    import test_gpu_parity as p
     case = pf.CASE_BY_NAME[pf.GRAD_CASE]
     run = pf.oracle_run(case)
     gold = np.load(pf.grad_golden_path())
@@ -272,7 +272,7 @@ def test_gradients_against_the_reference(precision, rel, kink):
         assert berr <= kink
         kept = {k: gold[k] for k in gold.files if k != bias}
         gold = type("Gold", (), {"files": list(kept), "__getitem__": lambda self, k: kept[k]})()
-    worst = p._compare_grads(gold, got, rel=rel, kink_rel=kink)
+    worst = _harness.compare_grads(gold, got, rel=rel, kink_rel=kink)
     assert "probe_siren.spatial_embeddings" in worst
     print("point_forward %s: %s" % (precision, {k: "%.1e" % v for k, v in worst.items()}))
 
@@ -281,7 +281,6 @@ def test_gradients_against_the_reference(precision, rel, kink):
 def test_split_gradients_against_the_reference():
     """grad_precision='split' after a split forward: within the bound tests/test_split_backward.py gives model B's render
     gradients (5e-4 of each tensor's largest entry; the density head's relu kink 1e-2)."""
-    import test_gpu_parity as p
     case = pf.CASE_BY_NAME[pf.GRAD_CASE]
     run = pf.oracle_run(case)
     gold = np.load(pf.grad_golden_path())
@@ -289,7 +288,7 @@ def test_split_gradients_against_the_reference():
     latents = [z.to(DEV).requires_grad_(True) for z in run["latents"]]
     px = _point_forward(case, run, "split", gen=gen, latents=latents, grad_precision="split")
     (px * _cases.loss_weights(px.shape).to(DEV)).sum().backward()
-    p._compare_grads(gold, pf.grad_record(latents, dict(gen.named_parameters())), rel=5e-4, kink_rel=1e-2)
+    _harness.compare_grads(gold, pf.grad_record(latents, dict(gen.named_parameters())), rel=5e-4, kink_rel=1e-2)
 
 
 @gpu

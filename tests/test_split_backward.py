@@ -15,11 +15,11 @@ import torch
 
 import _cases
 import _harness
-import _wo_dir_fields as WF
+from _harness import runs  # noqa: F401  (the module's oracle-run fixture)
 from _fp64 import _film, _siren, field_ref
 from fenerf_b200 import _lib, backward, ops
 from fenerf_b200.generators.volumetric_rendering import ReplayRng
-from test_gpu_fp64_reference import (FIELD_BOUND, FIELD_MODELS, LAYOUT_BOUND, _LAYOUTS, _field_points, _grad_errors,
+from test_gpu_fp64_reference import (FIELD_BOUND, STOCK_FIELD_MODELS, LAYOUT_BOUND, _LAYOUTS, _field_points, _grad_errors,
                                      _per_point)
 from tools import split_backward_precision as SB
 
@@ -242,7 +242,7 @@ def test_tn_split_vs_fp64(batch, ppb):
 #: exact mode).  Measured on an H100 80GB HBM3: split <= 4.1e-3, the exact mode 1.5e-3 on the same inputs -- the split
 #: operands' 22 bits against fp32's 24, as in the forward (tests/test_split_precision.py).
 P_BOUND = 6e-3
-_FIELD = ([(lay, m) for lay in ("L1", "L2", "L3") for m in FIELD_MODELS + ("P",)] + [("L4", "A"), ("L4", "B")])
+_FIELD = ([(lay, m) for lay in ("L1", "L2", "L3") for m in STOCK_FIELD_MODELS + ("P",)] + [("L4", "A"), ("L4", "B")])
 
 
 def _field_backward(siren, film, pts, dirs, dir_group, raw, d_raw, grad_split=True):
@@ -262,7 +262,7 @@ def test_field_backward_split_vs_fp64(monkeypatch, layout, model):
     FiLM tables with edge frequencies; the chunked layouts (L2, L3) agree with one chunk within LAYOUT_BOUND."""
     batch, ppb, dir_group, chunk = _LAYOUTS[layout]
     siren = _siren(model, DEV)
-    seed = 3000 + 10 * (FIELD_MODELS + ("P",)).index(model) + int(layout[1])
+    seed = 3000 + 10 * (STOCK_FIELD_MODELS + ("P",)).index(model) + int(layout[1])
     pts, dirs = (t.to(DEV) for t in _field_points(batch, ppb, dir_group, seed))
     film = _film(siren, batch, seed, edges=True)
     out_dim = siren.field_spec().out_dim
@@ -296,23 +296,10 @@ def test_field_backward_split_vs_fp64(monkeypatch, layout, model):
 # --------------------------------------------------------------------------------------------
 # GPU: gradients through renders against the reference's goldens
 # --------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def runs():
-    cache = {}
-
-    def get(name):
-        if name not in cache:
-            case = _cases.CASE_BY_NAME[name]
-            cache[name] = (case, _harness.oracle_run(case))
-        return cache[name]
-    return get
-
-
 def _latent_grads(runs, name, precision, **extra):
-    import test_gpu_parity as p
     case, run = runs(name)
     gen = _cases.build_mirror(case, DEV)
-    latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
+    latents = [_harness.cuda(z).requires_grad_(True) for z in run["latents"]]
     kw = {k: v for k, v in case.cfg.items() if k != "fill_mode"}
     pixels, _ = gen(*latents, **dict(kw, _rng=ReplayRng(run["draws"], DEV), precision=precision, **extra))
     (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
@@ -327,12 +314,11 @@ def _latent_grads(runs, name, precision, **extra):
 def test_render_gradients_against_reference(runs, name, precision):
     """forward() with grad_precision='split' after an exact or split forward: within the exact mode's 5e-4 (the density
     head's relu kink: 1e-2, as the exact test) of the reference's gradients."""
-    import test_gpu_parity as p
     gold = np.load(os.path.join(_cases.GOLDEN_DIR, "grad_%s.npz" % name))
     l0 = _lib.launch_count()
     got = _latent_grads(runs, name, precision, grad_precision="split")
     assert _lib.launch_count() - l0 > 20
-    worst = p._compare_grads(gold, got, rel=5e-4, kink_rel=1e-2)
+    worst = _harness.compare_grads(gold, got, rel=5e-4, kink_rel=1e-2)
     print("%s %s + grad split: %s" % (name, precision, {k: "%.2e" % v for k, v in worst.items()}))
 
 
@@ -340,16 +326,15 @@ def test_render_gradients_against_reference(runs, name, precision):
 @pytest.mark.parametrize("name", ["a_small", "d_small"])
 def test_inversion_gradients_against_reference(runs, name):
     """forward_with_frequencies with grad_precision='split': the FiLM-offset gradients within 5e-4."""
-    import test_gpu_parity as p
     case, run = runs(name)
     gold = np.load(os.path.join(_cases.GOLDEN_DIR, "gradfreq_%s.npz" % name))
     gen = _cases.build_mirror(case, DEV)
     with torch.no_grad():
         if case.model == "A":
-            fp = list(gen.siren.mapping_network(p._cuda(run["latents"][0])))
+            fp = list(gen.siren.mapping_network(_harness.cuda(run["latents"][0])))
         else:
-            fg, pg = gen.siren.geo_mapping_network(p._cuda(run["latents"][0]))
-            fa, pa = gen.siren.app_mapping_network(p._cuda(run["latents"][1]))
+            fg, pg = gen.siren.geo_mapping_network(_harness.cuda(run["latents"][0]))
+            fa, pa = gen.siren.app_mapping_network(_harness.cuda(run["latents"][1]))
             fp = [fg, fa, pg, pa]
     fp = [t.clone().requires_grad_(True) for t in fp]
     for q in gen.parameters():
@@ -357,7 +342,7 @@ def test_inversion_gradients_against_reference(runs, name):
     pixels, _ = gen.forward_with_frequencies(*fp, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="split",
                                                          grad_precision="split"))
     (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-    worst = p._compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=5e-4)
+    worst = _harness.compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=5e-4)
     print("%s inversion grad split: %s" % (name, {k: "%.2e" % v for k, v in worst.items()}))
 
 
@@ -366,28 +351,27 @@ def test_inversion_gradients_against_reference(runs, name):
 def test_direction_free_gradients_against_reference(runs, golden):
     """The direction-free field (P) through forward() and forward_with_frequencies with grad_precision='split': within the
     1e-2 of each tensor's largest entry that its split-render gradient test uses."""
-    import test_gpu_parity as p
-    case, run = runs(WF.GRAD_CASE)
-    gold = np.load(os.path.join(_cases.GOLDEN_DIR, "%s_%s.npz" % (golden, WF.GRAD_CASE)))
+    case, run = runs("p_small_opaque")
+    gold = np.load(os.path.join(_cases.GOLDEN_DIR, "%s_%s.npz" % (golden, "p_small_opaque")))
     gen = _cases.build_mirror(case, DEV)
     kw = dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="split", grad_precision="split")
     if golden == "grad":
-        latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
+        latents = [_harness.cuda(z).requires_grad_(True) for z in run["latents"]]
         pixels, _ = gen(*latents, **kw)
         (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
         got = {"latent%d" % i: z.grad for i, z in enumerate(latents)}
         got.update({k: q.grad for k, q in gen.named_parameters()})
-        worst = p._compare_grads(gold, got, rel=1e-2, kink_rel=1e-2)
+        worst = _harness.compare_grads(gold, got, rel=1e-2, kink_rel=1e-2)
     else:
         with torch.no_grad():
-            lat = [p._cuda(z) for z in run["latents"]]
+            lat = [_harness.cuda(z) for z in run["latents"]]
             fp = [t.clone().requires_grad_(True)
                   for t in gen.siren.geo_mapping_network(lat[0]) + gen.siren.app_mapping_network(lat[1])]
         for q in gen.parameters():
             q.requires_grad_(False)
         pixels, _ = gen.forward_with_frequencies(fp[0], fp[2], fp[1], fp[3], **kw)
         (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-        worst = p._compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=1e-2)
+        worst = _harness.compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=1e-2)
     print("%s P grad split: %s" % (golden, {k: "%.2e" % v for k, v in worst.items()}))
 
 

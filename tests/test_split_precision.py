@@ -18,7 +18,7 @@ import torch.nn.functional as F
 
 import _cases
 import _harness
-import _wo_dir_fields as WF
+from _harness import runs  # noqa: F401  (the module's oracle-run fixture)
 from _fp64 import _film, _siren, field_ref
 from fenerf_b200 import _lib, ops, packing
 from fenerf_b200.generators.volumetric_rendering import ReplayRng
@@ -182,35 +182,21 @@ _RENDER = ["a_small", "a_cfg2", "a_cfg5", "b_small", "b_cfg2", "c_small", "a_noh
            "s_small", "s_staged_weight", "p_small", "p_small_opaque", "p_cfg2", "p_staged_white"]
 
 
-@pytest.fixture(scope="module")
-def runs():
-    cache = {}
-
-    def get(name):
-        if name not in cache:
-            case = _cases.CASE_BY_NAME[name]
-            cache[name] = (case, _harness.oracle_run(case))
-        return cache[name]
-    return get
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", _RENDER)
 def test_end_to_end_against_reference(runs, name):
     """Split renders with the far-sigma exclusion rule of test_gpu_parity.py: A-H and S within the exact mode's 2e-4 of the
     oracle run (which matches the reference's goldens); P within its exact mode's 1e-3 of the reference's goldens (the
     reference's own fp32 forward is up to 5.6e-4 off float64 on this field)."""
-    import test_gpu_parity as p
     case, run = runs(name)
     if case.model != "P":
-        gen, pixels, poses, depth_map = p._end_to_end(case, run, "split")
-        p._check_pixels(case, run, pixels, 2e-4)
+        gen, pixels, poses, depth_map = _harness.end_to_end(case, run, "split")
+        _harness.check_pixels(case, run, pixels, 2e-4)
         return
-    from test_hd_fields import _golden_pixels
     gold = np.load(_cases.golden_path(case))
-    gen, pixels, poses, depth_map = p._end_to_end(case, run, "split")
-    ill_rays = p._ill_conditioned_pixels(case, run)
-    got, want, idx = _golden_pixels(pixels, gold)
+    gen, pixels, poses, depth_map = _harness.end_to_end(case, run, "split")
+    ill_rays = _harness.ill_conditioned_pixels(case, run)
+    got, want, idx = _harness.golden_pixels(pixels, gold)
     ill = ill_rays.unsqueeze(1).expand_as(pixels).reshape(-1)
     if idx is not None:
         ill = ill[idx]
@@ -224,29 +210,28 @@ def test_end_to_end_against_reference(runs, name):
 def test_direction_free_gradients_through_a_split_render(runs, golden):
     """forward() (and forward_with_frequencies) with autograd in split precision: forward on the split kernel, the exact
     mode's backward; within the exact-mode tests' 1e-2 of each tensor's largest entry of the reference's gradients."""
-    import test_gpu_parity as p
     from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    case, run = runs(WF.GRAD_CASE)
-    gold = np.load(os.path.join(GOLDEN, "%s_%s.npz" % (golden, WF.GRAD_CASE)))
+    case, run = runs("p_small_opaque")
+    gold = np.load(os.path.join(GOLDEN, "%s_%s.npz" % (golden, "p_small_opaque")))
     gen = _cases.build_mirror(case, DEV)
     kw = dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="split")
     if golden == "grad":
-        latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
+        latents = [_harness.cuda(z).requires_grad_(True) for z in run["latents"]]
         pixels, _ = gen(*latents, **kw)
         (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
         got = {"latent%d" % i: z.grad for i, z in enumerate(latents)}
         got.update({k: q.grad for k, q in gen.named_parameters()})
-        worst = p._compare_grads(gold, got, rel=1e-2, kink_rel=1e-2)
+        worst = _harness.compare_grads(gold, got, rel=1e-2, kink_rel=1e-2)
     else:
         with torch.no_grad():
-            lat = [p._cuda(z) for z in run["latents"]]
+            lat = [_harness.cuda(z) for z in run["latents"]]
             fp = [t.clone().requires_grad_(True)
                   for t in gen.siren.geo_mapping_network(lat[0]) + gen.siren.app_mapping_network(lat[1])]
         for q in gen.parameters():
             q.requires_grad_(False)
         pixels, _ = gen.forward_with_frequencies(fp[0], fp[2], fp[1], fp[3], **kw)
         (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-        worst = p._compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=1e-2)
+        worst = _harness.compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=1e-2)
     print("%s P split: %s" % (golden, worst))
 
 

@@ -1,24 +1,17 @@
 """The direction-free texture-grid field (TextureEmbeddingPiGAN256SEMANTICDISENTANGLE_WO_DIR_DIM_96, model P): the first
-colour layer reads cat[feat, x] with U(+-1/3) weights and no ray direction.  CPU: the mirror against the reference's init,
-the flag rules and the layout of the C-ABI, the oracle against the reference's goldens, the restatement's gradients and
-the faults the bounds catch.  GPU: the exact point network against a float64 restatement, the refusal of the fp16 colour
-path (and the density-only entry it leaves), the renders and gradients against the reference's goldens, the backward
-against float64 under production chunk layouts, and repacking."""
+colour layer reads cat[feat, x] with U(+-1/3) weights and no ray direction.  CPU: the field spec, the flag rules and the
+layout of the C-ABI, the restatement's gradients and the faults the bounds catch.  GPU: the exact point network against a
+float64 restatement, the refusal of the fp16 colour path (and the density-only entry it leaves), and the backward against
+float64 under production chunk layouts.  The init, oracle, end-to-end, gradient, inversion and repack checks of this field
+run with every other field's, in test_oracle.py, test_dropin.py and test_gpu_parity.py (its bounds in tests/_cases.py)."""
 import copy
 import ctypes
-import io
-import json
-import os
-
-import numpy as np
 
 import pytest
 import torch
 import torch.nn.functional as F
 
 import _cases
-import _harness
-import _wo_dir_fields as WF
 from _fp64 import _film, _siren, field_ref
 from fenerf_b200 import _lib, backward, ops, packing
 from fenerf_b200.siren import siren as S
@@ -27,7 +20,7 @@ from test_gpu_fp64_reference import (_LAYOUTS, _field_backward, _field_points, _
                                      _grad_errors, _per_point)
 
 DEV = "cuda:0"
-GOLDEN = _cases.GOLDEN_DIR
+CLASSES = _cases.INIT_GOLDENS["wo_dir_init.json"][1]
 #: exact point network, max |out - fp64| over the (labels, rgb, sigma) channels.  Measured on an H100 80GB HBM3 (700 W
 #: power limit): labels 8.1e-8, rgb 8.4e-5, sigma 7.6e-7.  The wgmma colour path is refused for this field: its rgb error
 #: was 2.1e-2 at 2 x 2048 points, the fp16 trunk's own error amplified by the first colour layer's U(+-1/3) weights at
@@ -44,38 +37,16 @@ BWD_BOUND = 3e-3
 
 def _mirror(name, seed=0):
     torch.manual_seed(seed)
-    return getattr(S, name)(**WF.KWARGS)
+    return _cases.construct_field(S, name)
 
 
 # --------------------------------------------------------------------------------------------
 # CPU: the mirror classes, the flag, the layout
 # --------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name", WF.CLASSES)
-def test_mirror_init_and_state_dict_are_the_references(name):
-    with open(os.path.join(GOLDEN, "wo_dir_init.json")) as f:
-        gold = json.load(f)[name]
-    siren = _mirror(name)
-    assert torch.rand(1).item() == gold["next_draw"]          # the init drew exactly the reference's draws
-    assert _harness.state_digest(siren) == gold["digest"]
-    assert [n for n, _ in siren.named_parameters()] == gold["names"]
-    assert {k: list(v.shape) for k, v in siren.state_dict().items()} == gold["state"]
-    assert [n for n, _ in siren.named_children()] == gold["children"]
-    spec = siren.field_spec()
+@pytest.mark.parametrize("name", CLASSES)
+def test_field_spec(name):
+    spec = _mirror(name).field_spec()
     assert spec.wo_dir and spec.color_layers == 8 and spec.label_dim == 18 and spec.grid_channels == 32
-
-
-@pytest.mark.parametrize("name", WF.CLASSES)
-def test_mirror_pickles_and_resolves_by_name(name):
-    import fenerf_b200
-    fenerf_b200.install()
-    import siren.siren as installed
-    assert getattr(installed, name) is getattr(S, name)
-    siren = _mirror(name)
-    buf = io.BytesIO()
-    torch.save(siren, buf)
-    back = torch.load(io.BytesIO(buf.getvalue()), map_location="cpu", weights_only=False)
-    assert type(back) is getattr(S, name)
-    assert all(torch.equal(a, b) for a, b in zip(siren.state_dict().values(), back.state_dict().values()))
 
 
 def _desc(flags, label_dim=18, grid=32, trunk=8, color=8):
@@ -93,13 +64,13 @@ def test_wo_dir_flag_only_in_the_reference_shape():
         assert lib.fenerf_packed_bytes(ctypes.byref(d)) == 0
         assert b"unknown field flag combination" in lib.fenerf_last_error()
         assert lib.fenerf_pack_field(ctypes.byref(d), ctypes.byref(params), None, 0, None) == -2
-    d = packing.field_desc(_mirror(WF.CLASSES[1]).field_spec())
+    d = packing.field_desc(_mirror(CLASSES[1]).field_spec())
     assert d.reserved == WD and d.grid_channels == 32 and d.color_layers == 8 and d.label_dim == 18
 
 
 def test_hidden_width_128_is_refused():
     with pytest.raises(ValueError, match="hidden_dim=256"):
-        packing.collect_params(_mirror(WF.CLASSES[0]), torch.device("cpu"))
+        packing.collect_params(_mirror(CLASSES[0]), torch.device("cpu"))
 
 
 def test_packed_layout_is_the_plain_grid_layout():
@@ -148,17 +119,6 @@ def test_faults_move_the_colours_past_the_exact_bound(fault):
     err = (good - bad)[..., 18:21].abs().max().item()
     print("fault %s: max |rgb| move %.3g" % (fault, err))
     assert err > EXACT_BOUND[1]
-
-
-@pytest.mark.parametrize("case", WF.CASES, ids=lambda c: c.name)
-def test_oracle_matches_reference_golden(case):
-    from test_hd_fields import _golden_pixels
-    if case.name in WF.BIG and not os.environ.get("FENERF_SLOW_TESTS") and not torch.cuda.is_available():
-        pytest.skip("minutes of CPU oracle (FENERF_SLOW_TESTS=1 runs it)")
-    gold = np.load(_cases.golden_path(case))
-    run = _harness.oracle_run(case, keep_stages=False)
-    got, want, _ = _golden_pixels(run["out"]["pixels"], gold)
-    assert (got - want).abs().max() <= 2e-5
 
 
 # --------------------------------------------------------------------------------------------
@@ -301,98 +261,3 @@ def test_backward_matches_float64_autograd(monkeypatch, layout, lock, edges):
 # --------------------------------------------------------------------------------------------
 # GPU: renders and gradients against the reference's goldens
 # --------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def runs():
-    cache = {}
-
-    def get(name):
-        if name not in cache:
-            case = _cases.CASE_BY_NAME[name]
-            cache[name] = (case, _harness.oracle_run(case))
-        return cache[name]
-    return get
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("case", WF.CASES, ids=lambda c: c.name)
-def test_end_to_end_against_reference_golden(runs, case):
-    """Exact renders against the reference's: measured on an H100 80GB HBM3 (700 W) <= 5.6e-4 (p_cfg2; 2.5e-4 .. 3.4e-4 on
-    the small cases) -- the reference's own fp32 forward differs from float64 by the same amplification of its rounding."""
-    import test_gpu_parity as p
-    from test_hd_fields import _golden_pixels
-    gold = np.load(_cases.golden_path(case))
-    case, run = runs(case.name)
-    gen, pixels, poses, depth_map = p._end_to_end(case, run, "exact")
-    ill_rays = p._ill_conditioned_pixels(case, run)
-    got, want, idx = _golden_pixels(pixels, gold)
-    err = (got - want).abs()
-    assert int(ill_rays.sum()) <= max(2, 0.002 * ill_rays.numel())
-    ill = ill_rays.unsqueeze(1).expand_as(pixels).reshape(-1)
-    if idx is not None:
-        ill = ill[idx]
-    print("%s exact: max err %.3g" % (case.name, err[~ill].max()))
-    assert err[~ill].max() <= 1e-3
-    if poses is not None:
-        assert (poses - torch.from_numpy(gold["poses"])).abs().max() <= 1e-5
-
-
-@pytest.mark.gpu
-def test_generator_gradients_match_reference(runs):
-    """forward() with autograd (exact mode) against the reference's autograd on the opaque case: <= 1e-2 of each tensor's
-    max (measured <= 6.6e-3)."""
-    import test_gpu_parity as p
-    from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    case, run = runs(WF.GRAD_CASE)
-    gold = np.load(os.path.join(GOLDEN, "grad_%s.npz" % WF.GRAD_CASE))
-    gen = _cases.build_mirror(case, DEV)
-    latents = [p._cuda(z).requires_grad_(True) for z in run["latents"]]
-    pixels, _ = gen(*latents, **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="exact"))
-    (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-    got = {"latent%d" % i: z.grad for i, z in enumerate(latents)}
-    got.update({k: q.grad for k, q in gen.named_parameters()})
-    worst = p._compare_grads(gold, got, rel=1e-2, kink_rel=1e-2)
-    print("gradients P exact: %s" % ({k: "%.1e" % v for k, v in worst.items()},))
-
-
-@pytest.mark.gpu
-def test_inversion_gradients_through_forward_with_frequencies(runs):
-    """d pixels / d (frequencies, phase shifts) through forward_with_frequencies, exact mode: <= 1e-2 (measured 5.9e-3)."""
-    import test_gpu_parity as p
-    from fenerf_b200.generators.volumetric_rendering import ReplayRng
-    case, run = runs(WF.GRAD_CASE)
-    gold = np.load(os.path.join(GOLDEN, "gradfreq_%s.npz" % WF.GRAD_CASE))
-    gen = _cases.build_mirror(case, DEV)
-    with torch.no_grad():
-        lat = [p._cuda(z) for z in run["latents"]]
-        fp = [t.clone().requires_grad_(True) for t in gen.siren.geo_mapping_network(lat[0]) + gen.siren.app_mapping_network(lat[1])]
-    for q in gen.parameters():
-        q.requires_grad_(False)
-    pixels, _ = gen.forward_with_frequencies(fp[0], fp[2], fp[1], fp[3],
-                                             **dict(case.cfg, _rng=ReplayRng(run["draws"], DEV), precision="exact"))
-    (pixels * _cases.loss_weights(pixels.shape).to(DEV)).sum().backward()
-    worst = p._compare_grads(gold, {"arg%d" % i: t.grad for i, t in enumerate(fp)}, rel=1e-2)
-    print("inversion P: %s" % (worst,))
-
-
-@pytest.mark.gpu
-def test_staged_forward_sees_first_colour_layer_writes():
-    """torch_ema's copy_to writes through param.data without a version bump: a write to color_layer_sine[0] alone -- its
-    feature columns alone, too -- must reach staged_forward (the fingerprint covers all 288 columns)."""
-    case = _cases.CASE_BY_NAME["p_small_opaque"]
-    gen = _cases.build_mirror(case, DEV)
-    s = gen.siren
-    g = torch.Generator().manual_seed(8)
-    z = [torch.randn(1, 256, generator=g).to(DEV) for _ in range(2)]
-    kw = dict(case.cfg, psi=0.7, max_batch_size=2400000, precision="exact")
-    w = s.color_layer_sine[0].layer.weight
-
-    def render():
-        torch.manual_seed(1)
-        return torch.cat([t.reshape(-1).cpu() for t in gen.staged_forward(*z, **kw)[:2]])
-    with torch.no_grad():
-        for cols in (slice(None), slice(0, 32)):
-            a = render()
-            w.data[:, cols].copy_(w.detach()[:, cols] * -3.0)
-            b = render()
-            s.invalidate_packed()
-            assert not torch.equal(a, b) and torch.equal(b, render())
